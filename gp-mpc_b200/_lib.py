@@ -37,6 +37,8 @@ SYMBOLS = [
     ('gpmpc_nlml', C.c_int, [_H, C.c_int, _dp, _dp, _dp]),
     ('gpmpc_predict', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp]),
     ('gpmpc_predict_grad', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
+    ('gpmpc_predict_hess', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp,
+                                     _dp, _dp, _dp]),
     ('gpmpc_get_size', C.c_int, [_H, _ip, _ip, _ip]),
     ('gpmpc_append', C.c_int, [_H, _dp, _dp]),
     ('gpmpc_posterior_cov', C.c_int, [_H, C.c_int, _dp, _dp]),
@@ -71,6 +73,15 @@ for _f in ('gp_b200', 'jac_gp_b200'):
     ]
 SYMBOLS += [('gp_b200_bind', C.c_int, [_H, C.c_int, C.c_int]), ('gp_b200_unbind', None, []),
             ('gp_b200_incref', None, []), ('gp_b200_decref', None, [])]
+# the Jacobian of jac_gp_b200 (second derivatives, include/gpmpc_casadi.h), bound by load() next to SYMBOLS
+SYMBOLS_JAC_JAC = [
+    ('jac_jac_gp_b200_n_in', _ll, []), ('jac_jac_gp_b200_n_out', _ll, []),
+    ('jac_jac_gp_b200_name_in', C.c_char_p, [_ll]), ('jac_jac_gp_b200_name_out', C.c_char_p, [_ll]),
+    ('jac_jac_gp_b200_sparsity_in', _llp, [_ll]), ('jac_jac_gp_b200_sparsity_out', _llp, [_ll]),
+    ('jac_jac_gp_b200_work', C.c_int, [_llp, _llp, _llp, _llp]),
+    ('jac_jac_gp_b200_incref', None, []), ('jac_jac_gp_b200_decref', None, []),
+    ('jac_jac_gp_b200', C.c_int, [_dpp, _dpp, _llp, _dp, C.c_int]),
+]
 
 _lib = None
 
@@ -91,7 +102,7 @@ def load():
             'libgpmpc.so not found at %s -- build it with `python -c "import __graft_entry__ as g; '
             'g.build()"` (nvcc, sm_90a).  This engine has no CPU fallback.' % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
-    for name, res, args in SYMBOLS:
+    for name, res, args in SYMBOLS + SYMBOLS_JAC_JAC:
         fn = getattr(lib, name)      # AttributeError if the symbol is missing
         fn.restype = res
         fn.argtypes = args
@@ -265,6 +276,27 @@ class Engine:
         self._check(self.lib.gpmpc_predict_grad(self.h, int(method), H, _ptr(Z), _ptr(Sigma), spp, _ptr(out['mean']),
                                                 _ptr(out['var']), _ptr(out['cov']), _ptr(out['jac']), _ptr(out['dvar_dz']),
                                                 _ptr(out['dcov_dz']), _ptr(out.get('hess'))))
+        return out
+
+    def predict_hess(self, Z, Sigma=None, method=METHOD_TA):
+        """predict_grad(..., want_hess=True) plus the second derivatives w.r.t. the test inputs (gpmpc_predict_hess):
+        d2var_dz2 (H,Ny,Nx,Nx), d3mean_dz3 (H,Ny,Nx,Nx,Nx), d2cov_dz2 (H,Ny,Ny,Nx,Nx)."""
+        Z = _f64(Z).reshape(-1, self.Nx)
+        H = Z.shape[0]
+        spp = 0
+        if Sigma is not None:
+            Sigma = _f64(Sigma)
+            spp = 1 if Sigma.ndim == 3 else 0
+            assert Sigma.shape == ((H, self.Nx, self.Nx) if spp else (self.Nx, self.Nx))
+        Ny, Nx = self.Ny, self.Nx
+        out = dict(mean=np.empty((H, Ny)), var=np.empty((H, Ny)), cov=np.empty((H, Ny, Ny)), jac=np.empty((H, Ny, Nx)),
+                   dvar_dz=np.empty((H, Ny, Nx)), dcov_dz=np.empty((H, Ny, Ny, Nx)), hess=np.empty((H, Ny, Nx, Nx)),
+                   d2var_dz2=np.empty((H, Ny, Nx, Nx)), d3mean_dz3=np.empty((H, Ny, Nx, Nx, Nx)),
+                   d2cov_dz2=np.empty((H, Ny, Ny, Nx, Nx)))
+        self._check(self.lib.gpmpc_predict_hess(
+            self.h, int(method), H, _ptr(Z), _ptr(Sigma), spp,
+            *[_ptr(out[k]) for k in ('mean', 'var', 'cov', 'jac', 'dvar_dz', 'dcov_dz', 'hess', 'd2var_dz2', 'd3mean_dz3',
+                                     'd2cov_dz2')]))
         return out
 
     def append(self, x_new, y_new):

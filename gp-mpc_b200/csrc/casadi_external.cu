@@ -1,4 +1,4 @@
-// CasADi `external`-shaped entry points around gpmpc_predict_grad (SURVEY 8f row 1).
+// CasADi `external`-shaped entry points around gpmpc_predict_grad / gpmpc_predict_hess (SURVEY 8f row 1).
 //
 // mpc_class.py:361-423 calls gp.predict(mean_t, u_t, covar_t) once per shooting node with MX
 // symbols and nlpsol (:496-513) differentiates the resulting graph.  With
@@ -17,8 +17,18 @@
 //   jac_gp_b200: inputs (i0, i1, o0, o1), outputs block-diagonal sparse
 //            jac_o0_i0 (Ny*Nt x Nx*Nt), jac_o0_i1 (empty), jac_o1_i0 (Ny*Ny*Nt x Nx*Nt),
 //            jac_o1_i1 (Ny*Ny*Nt x Nx*Nx*Nt;  d cov[a][b] / d Sigma[d][e] = J_a[d] J_b[e] for 'TA')
+//   jac_jac_gp_b200: inputs (i0, i1, o0, o1, and the four outputs of jac_gp_b200), outputs the Jacobians of
+//            jac_gp_b200's four outputs w.r.t. its four inputs (output-major), what IPOPT's exact Hessian
+//            needs.  Rows index the column-major dense vec of the differentiated Jacobian, columns the dense
+//            vec of the input (the convention of jac_gp_b200).  Nonzero blocks per node:
+//              jac_mean_z  / z      Ny*Nx*Nx         d^2 mean_a / d z_d d z_e        (hess)
+//              jac_cov_z   / z      Ny*Ny*Nx*Nx      d^2 cov[a][b] / d z_e d z_f     (d2cov_dz2)
+//              jac_cov_z   / sigma  Ny*Ny*Nx*Nx*Nx   hess_a[d][e] J_b[e'] + J_a[d] hess_b[e'][e]   ('TA')
+//              jac_cov_sigma / z    Ny*Ny*Nx*Nx*Nx   the same values, w.r.t. z_f of d cov / d Sigma[d][e]  ('TA')
+//            everything else is structurally zero.
 #include "../../include/gpmpc.h"
 
+#include <functional>
 #include <mutex>
 #include <vector>
 
@@ -29,8 +39,8 @@ namespace {
 struct Bound {
     gpmpc_handle_t h = nullptr;
     int method = GPMPC_METHOD_TA, Nt = 0, Nx = 0, Ny = 0;
-    std::vector<casadi_int> sp_in[2], sp_out[2], sp_jac[4];
-    std::vector<double> sig, mean, var, cov, jac, dvar, dcov;
+    std::vector<casadi_int> sp_in[2], sp_out[2], sp_jac[4], sp_jj[16];
+    std::vector<double> sig, mean, var, cov, jac, dvar, dcov, hess, d2cov;
     int refs = 0;
 };
 Bound g_b;
@@ -57,9 +67,32 @@ std::vector<casadi_int> empty_sp(casadi_int r, casadi_int c)
     return sp;
 }
 
-// evaluate mean/cov (+ derivatives when grad) for the bound handle; Sigma blocks are transposed to
-// the engine's row-major convention (a symmetric Sigma is unchanged)
-int eval(const casadi_real* Z, const casadi_real* Sigma, bool grad)
+// CCS pattern of Nt diagonal blocks: node t owns the C columns [t*C, (t+1)*C), each holding the rows rows(t)
+// (ascending)
+std::vector<casadi_int> nodes_sp(casadi_int nrow, casadi_int C, casadi_int Nt,
+                                 const std::function<std::vector<casadi_int>(casadi_int)>& rows)
+{
+    std::vector<casadi_int> sp = {nrow, C * Nt};
+    std::vector<casadi_int> ri;
+    casadi_int nnz = 0;
+    sp.push_back(0);
+    for (casadi_int t = 0; t < Nt; ++t) {
+        const std::vector<casadi_int> r = rows(t);
+        for (casadi_int c = 0; c < C; ++c) {
+            ri.insert(ri.end(), r.begin(), r.end());
+            nnz += (casadi_int)r.size();
+            sp.push_back(nnz);
+        }
+    }
+    sp.insert(sp.end(), ri.begin(), ri.end());
+    return sp;
+}
+
+enum { EVAL_VALUE = 0, EVAL_GRAD = 1, EVAL_HESS = 2 };
+
+// evaluate mean/cov (+ derivatives for EVAL_GRAD / EVAL_HESS) for the bound handle; Sigma blocks are
+// transposed to the engine's row-major convention (a symmetric Sigma is unchanged)
+int eval(const casadi_real* Z, const casadi_real* Sigma, int mode)
 {
     Bound& b = g_b;
     if (!b.h || !Z) return 1;
@@ -72,7 +105,11 @@ int eval(const casadi_real* Z, const casadi_real* Sigma, bool grad)
                 for (int e = 0; e < Nx; ++e)
                     b.sig[((size_t)t * Nx + d) * Nx + e] = Sigma[((size_t)t * Nx + e) * Nx + d];
     }
-    if (!grad)
+    if (mode == EVAL_HESS)
+        return gpmpc_predict_hess(b.h, b.method, Nt, Z, ta ? b.sig.data() : nullptr, 1, b.mean.data(), b.var.data(),
+                                  b.cov.data(), b.jac.data(), b.dvar.data(), b.dcov.data(), b.hess.data(), nullptr, nullptr,
+                                  b.d2cov.data()) == GPMPC_OK ? 0 : 1;
+    if (mode == EVAL_VALUE)
         return gpmpc_predict(b.h, b.method, Nt, Z, ta ? b.sig.data() : nullptr, 1, b.mean.data(), b.var.data(),
                              b.cov.data(), b.jac.data()) == GPMPC_OK ? 0 : 1;
     return gpmpc_predict_grad(b.h, b.method, Nt, Z, ta ? b.sig.data() : nullptr, 1, b.mean.data(), b.var.data(),
@@ -101,6 +138,38 @@ extern "C" int gp_b200_bind(gpmpc_handle_t h, int method, int Nt)
     b.mean.assign((size_t)Nt * Ny, 0.0); b.var.assign((size_t)Nt * Ny, 0.0);
     b.cov.assign((size_t)Nt * Ny * Ny, 0.0); b.jac.assign((size_t)Nt * Ny * Nx, 0.0);
     b.dvar.assign((size_t)Nt * Ny * Nx, 0.0); b.dcov.assign((size_t)Nt * Ny * Ny * Nx, 0.0);
+    b.hess.assign((size_t)Nt * Ny * Nx * Nx, 0.0); b.d2cov.assign((size_t)Nt * Ny * Ny * Nx * Nx, 0.0);
+    // jac_jac_gp_b200: numel of jac_gp_b200's outputs (rows) and inputs (columns)
+    const casadi_int T = Nt, X = Nx, Y = Ny;
+    const casadi_int n_out[4] = {Y * T * X * T, Y * T * X * X * T, Y * Y * T * X * T, Y * Y * T * X * X * T};
+    const casadi_int n_in[4] = {X * T, X * X * T, Y * T, Y * Y * T};
+    for (int o = 0; o < 4; ++o)
+        for (int i = 0; i < 4; ++i) b.sp_jj[o * 4 + i] = empty_sp(n_out[o], n_in[i]);
+    b.sp_jj[0] = nodes_sp(n_out[0], X, T, [&](casadi_int t) {         // jac_mean_z (a + Y t, d + X t) / z
+        std::vector<casadi_int> r;
+        for (casadi_int d = 0; d < X; ++d)
+            for (casadi_int a = 0; a < Y; ++a) r.push_back((a + Y * t) + Y * T * (d + X * t));
+        return r;
+    });
+    auto cov_z_rows = [&](casadi_int t) {                             // jac_cov_z (a + Y b + Y^2 t, e + X t)
+        std::vector<casadi_int> r;
+        for (casadi_int e = 0; e < X; ++e)
+            for (casadi_int bb = 0; bb < Y; ++bb)
+                for (casadi_int a = 0; a < Y; ++a) r.push_back((a + Y * bb + Y * Y * t) + Y * Y * T * (e + X * t));
+        return r;
+    };
+    b.sp_jj[8] = nodes_sp(n_out[2], X, T, cov_z_rows);
+    if (method == GPMPC_METHOD_TA) {
+        b.sp_jj[9] = nodes_sp(n_out[2], X * X, T, cov_z_rows);
+        b.sp_jj[12] = nodes_sp(n_out[3], X, T, [&](casadi_int t) {   // jac_cov_sigma (a + Y b + Y^2 t, d + X e + X^2 t) / z
+            std::vector<casadi_int> r;
+            for (casadi_int e = 0; e < X; ++e)
+                for (casadi_int d = 0; d < X; ++d)
+                    for (casadi_int bb = 0; bb < Y; ++bb)
+                        for (casadi_int a = 0; a < Y; ++a) r.push_back((a + Y * bb + Y * Y * t) + Y * Y * T * (d + X * e + X * X * t));
+            return r;
+        });
+    }
     return GPMPC_OK;
 }
 
@@ -133,7 +202,7 @@ extern "C" int gp_b200(const casadi_real** arg, casadi_real** res, casadi_int* i
     (void)iw; (void)w; (void)mem;
     std::lock_guard<std::mutex> lock(g_mtx);
     if (!arg || !res) return 1;
-    if (eval(arg[0], arg[1], false)) return 1;
+    if (eval(arg[0], arg[1], EVAL_VALUE)) return 1;
     const Bound& b = g_b;
     // (Nt,Ny) row-major == Ny x Nt column-major; each Ny x Ny block is written column-major
     // (element (a,b) at a + Ny*b) -- the blocks are symmetric only up to rounding
@@ -179,7 +248,7 @@ extern "C" int jac_gp_b200(const casadi_real** arg, casadi_real** res, casadi_in
     (void)iw; (void)w; (void)mem;
     std::lock_guard<std::mutex> lock(g_mtx);
     if (!arg || !res) return 1;
-    if (eval(arg[0], arg[1], true)) return 1;
+    if (eval(arg[0], arg[1], EVAL_GRAD)) return 1;
     const Bound& b = g_b;
     const int Nt = b.Nt, Nx = b.Nx, Ny = b.Ny;
     if (res[0])          // block t, column d, row a:  d mean_a / d z_d
@@ -200,5 +269,96 @@ extern "C" int jac_gp_b200(const casadi_real** arg, casadi_real** res, casadi_in
                         for (int a = 0; a < Ny; ++a)
                             res[3][((((size_t)t * Nx + e) * Nx + d) * Ny + bb) * Ny + a] =
                                 b.jac[((size_t)t * Ny + a) * Nx + d] * b.jac[((size_t)t * Ny + bb) * Nx + e];
+    return 0;
+}
+
+// ---- the Jacobian of jac_gp_b200 (second derivatives): inputs (z, sigma, mean, cov, and jac_gp_b200's four outputs),
+// outputs jac_jac_<o>_<i> in CCS nonzero order
+extern "C" casadi_int jac_jac_gp_b200_n_in(void) { return 8; }
+extern "C" casadi_int jac_jac_gp_b200_n_out(void) { return 16; }
+extern "C" const char* jac_jac_gp_b200_name_in(casadi_int i)
+{
+    static const char* n[] = {"z", "sigma", "out_mean", "out_cov", "out_jac_mean_z", "out_jac_mean_sigma", "out_jac_cov_z",
+                              "out_jac_cov_sigma"};
+    return (i >= 0 && i < 8) ? n[i] : nullptr;
+}
+extern "C" const char* jac_jac_gp_b200_name_out(casadi_int i)
+{
+    static const char* n[] = {
+        "jac_jac_mean_z_z", "jac_jac_mean_z_sigma", "jac_jac_mean_z_out_mean", "jac_jac_mean_z_out_cov",
+        "jac_jac_mean_sigma_z", "jac_jac_mean_sigma_sigma", "jac_jac_mean_sigma_out_mean", "jac_jac_mean_sigma_out_cov",
+        "jac_jac_cov_z_z", "jac_jac_cov_z_sigma", "jac_jac_cov_z_out_mean", "jac_jac_cov_z_out_cov",
+        "jac_jac_cov_sigma_z", "jac_jac_cov_sigma_sigma", "jac_jac_cov_sigma_out_mean", "jac_jac_cov_sigma_out_cov"};
+    return (i >= 0 && i < 16) ? n[i] : nullptr;
+}
+extern "C" const casadi_int* jac_jac_gp_b200_sparsity_in(casadi_int i)
+{
+    if (!g_b.h || i < 0 || i > 7) return nullptr;
+    return i < 2 ? g_b.sp_in[i].data() : i < 4 ? g_b.sp_out[i - 2].data() : g_b.sp_jac[i - 4].data();
+}
+extern "C" const casadi_int* jac_jac_gp_b200_sparsity_out(casadi_int i)
+{
+    return (i >= 0 && i < 16 && g_b.h) ? g_b.sp_jj[i].data() : nullptr;
+}
+extern "C" int jac_jac_gp_b200_work(casadi_int* sz_arg, casadi_int* sz_res, casadi_int* sz_iw, casadi_int* sz_w)
+{
+    if (sz_arg) *sz_arg = 8;
+    if (sz_res) *sz_res = 16;
+    if (sz_iw) *sz_iw = 0;
+    if (sz_w) *sz_w = 0;
+    return 0;
+}
+extern "C" void jac_jac_gp_b200_incref(void) { std::lock_guard<std::mutex> lock(g_mtx); ++g_b.refs; }
+extern "C" void jac_jac_gp_b200_decref(void) { std::lock_guard<std::mutex> lock(g_mtx); --g_b.refs; }
+
+extern "C" int jac_jac_gp_b200(const casadi_real** arg, casadi_real** res, casadi_int* iw, casadi_real* w, int mem)
+{
+    (void)iw; (void)w; (void)mem;
+    std::lock_guard<std::mutex> lock(g_mtx);
+    if (!arg || !res) return 1;
+    if (eval(arg[0], arg[1], EVAL_HESS)) return 1;
+    const Bound& b = g_b;
+    const size_t Nt = b.Nt, Nx = b.Nx, Ny = b.Ny;
+    const double* Hs = b.hess.data();
+    const double* J = b.jac.data();
+    auto H = [&](size_t t, size_t a, size_t d, size_t e) { return Hs[((t * Ny + a) * Nx + d) * Nx + e]; };
+    auto Jv = [&](size_t t, size_t a, size_t d) { return J[(t * Ny + a) * Nx + d]; };
+    // nonzeros in the order of the patterns built by gp_b200_bind: node, column, then rows ascending
+    if (res[0]) {        // column e, rows (d, a):  d^2 mean_a / d z_d d z_e
+        size_t k = 0;
+        for (size_t t = 0; t < Nt; ++t)
+            for (size_t e = 0; e < Nx; ++e)
+                for (size_t d = 0; d < Nx; ++d)
+                    for (size_t a = 0; a < Ny; ++a) res[0][k++] = H(t, a, d, e);
+    }
+    if (res[8]) {        // column f, rows (e, b, a):  d^2 cov[a][b] / d z_e d z_f
+        size_t k = 0;
+        for (size_t t = 0; t < Nt; ++t)
+            for (size_t f = 0; f < Nx; ++f)
+                for (size_t e = 0; e < Nx; ++e)
+                    for (size_t bb = 0; bb < Ny; ++bb)
+                        for (size_t a = 0; a < Ny; ++a) res[8][k++] = b.d2cov[((((t * Ny + a) * Ny + bb) * Nx + e) * Nx + f)];
+    }
+    if (b.method != GPMPC_METHOD_TA) return 0;
+    if (res[9]) {        // column d' + Nx e' (vec of Sigma), rows (e, b, a):  d^2 cov[a][b] / d z_e d Sigma[d'][e']
+        size_t k = 0;
+        for (size_t t = 0; t < Nt; ++t)
+            for (size_t ep = 0; ep < Nx; ++ep)
+                for (size_t dp = 0; dp < Nx; ++dp)
+                    for (size_t e = 0; e < Nx; ++e)
+                        for (size_t bb = 0; bb < Ny; ++bb)
+                            for (size_t a = 0; a < Ny; ++a)
+                                res[9][k++] = H(t, a, dp, e) * Jv(t, bb, ep) + Jv(t, a, dp) * H(t, bb, ep, e);
+    }
+    if (res[12]) {       // column f, rows (e, d, b, a) of d cov[a][b] / d Sigma[d][e]:  its derivative by z_f
+        size_t k = 0;
+        for (size_t t = 0; t < Nt; ++t)
+            for (size_t f = 0; f < Nx; ++f)
+                for (size_t e = 0; e < Nx; ++e)
+                    for (size_t d = 0; d < Nx; ++d)
+                        for (size_t bb = 0; bb < Ny; ++bb)
+                            for (size_t a = 0; a < Ny; ++a)
+                                res[12][k++] = H(t, a, d, f) * Jv(t, bb, e) + Jv(t, a, d) * H(t, bb, e, f);
+    }
     return 0;
 }

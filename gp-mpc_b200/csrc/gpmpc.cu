@@ -84,6 +84,8 @@ struct gpmpc_handle_s {
     double *dCovV = nullptr, *dCovOut = nullptr; long long covVcap = 0, covOutcap = 0;   // GP.covar scratch pool
     // predict_grad: U = Linv^T per output (lazy), beta rows, partial sums, per-batch derivative slabs
     double *dUall = nullptr, *dBeta = nullptr, *dPDV = nullptr, *dPH = nullptr, *dGradOut = nullptr; bool u_valid = false; int gradHcap = 0;
+    // predict_hess: derivative rows d ks / dz and their L^-1 products (lazy), block partials, per-batch second-derivative slabs
+    double *dDR = nullptr, *dVD = nullptr, *dPG = nullptr, *dPB2 = nullptr, *dPM3 = nullptr, *dHessOut = nullptr; int hessHcap = 0;
     double *dG = nullptr, *dZ = nullptr, *dSigma = nullptr, *dMean = nullptr, *dVar = nullptr, *dJ = nullptr, *dCov = nullptr;
     double* dRoll = nullptr; size_t rollCap = 0;   // gpmpc_rollout: [Z | Sigma | U | scale | means | vars | cov]
     double *dIn = nullptr, *dOut = nullptr;   // [Z | Sigma] and [mean | var | J | cov] slabs: one H2D + one D2H per host call
@@ -497,7 +499,7 @@ extern "C" int gpmpc_destroy(gpmpc_handle_t h)
     if (h->dCnt) cudaFree(h->dCnt);
     if (h->hPeerStatus) cudaFreeHost(h->hPeerStatus);
     double* bufs[] = {h->dXT, h->dMu, h->dY, h->dHyp, h->dHypTmp, h->dJit, h->dL, h->dLi, h->dW1, h->dW2, h->dAlpha, h->dTmp,
-                      h->dRes, h->dKST, h->dPart, h->dPMJ, h->dSQ, h->dV, h->dR, h->dR2, h->dCovV, h->dCovOut, h->dUall, h->dBeta, h->dPDV, h->dPH, h->dGradOut, h->dG, h->dRoll, h->dIn, h->dOut, h->dU, h->dKinv, h->dGradPart, h->dGrad,
+                      h->dRes, h->dKST, h->dPart, h->dPMJ, h->dSQ, h->dV, h->dR, h->dR2, h->dCovV, h->dCovOut, h->dUall, h->dBeta, h->dPDV, h->dPH, h->dGradOut, h->dDR, h->dVD, h->dPG, h->dPB2, h->dPM3, h->dHessOut, h->dG, h->dRoll, h->dIn, h->dOut, h->dU, h->dKinv, h->dGradPart, h->dGrad,
                       h->dEmTr, h->dEmLQ, h->dEmVec, h->dEmE2, h->dEmF2, h->dEMP, h->dEmE, h->dEmF, h->dEmW, h->dEmIJ, h->dEmMeanPart, h->dEmPart};
     for (double* b : bufs) if (b) cudaFree(b);
     if (h->dInfo) cudaFree(h->dInfo);
@@ -1441,19 +1443,64 @@ static cudaError_t launch_grad_reduce(gpmpc_handle_t h, const double* dZc, int H
     return cudaGetLastError();
 }
 
-extern "C" int gpmpc_predict_grad(gpmpc_handle_t h, int method, int H, const double* Z, const double* Sigma, int spp,
-                                  double* mean, double* var, double* cov, double* jac,
-                                  double* dvar_dz, double* dcov_dz, double* hess)
+template <int NXP>
+static cudaError_t launch_hess_reduce(gpmpc_handle_t h, const double* dZc, int Hc, int p0, int Rc, int nblk)
+{
+    dim3 g(nblk, Rc, h->nloc);
+    const int smem = (2 * h->Nx * 257 + 512) * 8;
+    static std::atomic<bool> conf[GPMPC_MAX_DEVICES];
+    if (!conf[h->device % GPMPC_MAX_DEVICES].load(std::memory_order_acquire)) {      // static + dynamic may pass 48 KB
+        cudaError_t e = cudaFuncSetAttribute(hess_reduce_kernel<NXP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (2 * NX_MAX * 257 + 512) * 8);
+        if (e != cudaSuccess) return e;
+        conf[h->device % GPMPC_MAX_DEVICES].store(true, std::memory_order_release);
+    }
+    hess_reduce_kernel<NXP><<<g, 256, smem, h->st>>>(h->dXT, h->Npad, h->N, h->Nx, h->dHyp, h->Nx + 2, h->dAlpha, h->Npad, dZc,
+                                                      h->dKST, h->dBeta, h->dVD, h->Npad, (long long)HB * h->Npad,
+                                                      h->dPG, h->dPB2, h->dPM3, nblk, Hc, p0);
+    return cudaGetLastError();
+}
+
+// Second derivatives of one chunk of Hc <= 64 points, after predict_grad's chain for it (ks, v, beta, records):
+// R = 64/Nx points per pass, each pass = derivative rows -> V_d = L^-1 d_d ks on the predict product (lower
+// mode, rows stored, no finalize) -> Gram / moment partials; one finalize per chunk.
+static int hess_chunk(gpmpc_handle_t h, const double* dZc, int Hc, int H, int h0, double* d_d2var, double* d_d3mean)
+{
+    const int np = h->Npad, Nx = h->Nx, R = HB / Nx, nblk = (np + GR_CHUNK - 1) / GR_CHUNK;
+    for (int p0 = 0; p0 < Hc; p0 += R) {
+        const int Rc = std::min(R, Hc - p0), rows = Rc * Nx;
+        hess_rows_kernel<<<dim3((np + 255) / 256, Rc, h->nloc), 256, 0, h->st>>>(h->dXT, np, h->N, Nx, h->dHyp, Nx + 2, dZc,
+                                                                                h->dKST, np, (long long)HB * np, h->dDR, p0);
+        CUDA_TRY(cudaGetLastError());
+        int rc = tri_product(h, h->dDR, h->dLi, (rows + 7) / 8 * 8, rows, h->dVD);
+        if (rc) return rc;
+        cudaError_t e = (Nx <= 8) ? launch_hess_reduce<8>(h, dZc, Hc, p0, Rc, nblk)
+                      : (Nx <= 16) ? launch_hess_reduce<16>(h, dZc, Hc, p0, Rc, nblk) : launch_hess_reduce<32>(h, dZc, Hc, p0, Rc, nblk);
+        CUDA_TRY(e);
+    }
+    hess_finalize_kernel<<<dim3(Hc, h->nloc), 128, 0, h->st>>>(h->dPG, h->dPB2, h->dPM3, nblk, Hc, h->dHyp, Nx + 2, Nx, h->Ny,
+                                                               h->dG, H, h0, d_d2var, d_d3mean);
+    CUDA_TRY(cudaGetLastError());
+    return GPMPC_OK;
+}
+
+// Second-derivative outputs of predict_derivs (null: first derivatives only, gpmpc_predict_grad)
+struct HessOutputs {
+    double *d2var_dz2, *d3mean_dz3, *d2cov_dz2;
+};
+
+static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, const double* Z, const double* Sigma, int spp,
+                          double* mean, double* var, double* cov, double* jac,
+                          double* dvar_dz, double* dcov_dz, double* hess, const HessOutputs* ho)
 {
     int rc = predict_check(h, method, H);
     if (rc) return rc;
-    if (method == GPMPC_METHOD_EM) { set_error(h, "gpmpc_predict_grad: derivatives are available for ME and TA"); return GPMPC_ERR_ARG; }
-    if (!Z || (method == GPMPC_METHOD_TA && !Sigma)) { set_error(h, "gpmpc_predict_grad: null Z / Sigma"); return GPMPC_ERR_ARG; }
-    if (h->nloc != h->Ny || h->world != 1) { set_error(h, "gpmpc_predict_grad needs all outputs on one handle (replicate the model, shard the points)"); return GPMPC_ERR_STATE; }
+    if (method == GPMPC_METHOD_EM) { set_error(h, "%s: derivatives are available for ME and TA", fn); return GPMPC_ERR_ARG; }
+    if (!Z || (method == GPMPC_METHOD_TA && !Sigma)) { set_error(h, "%s: null Z / Sigma", fn); return GPMPC_ERR_ARG; }
+    if (h->nloc != h->Ny || h->world != 1) { set_error(h, "%s needs all outputs on one handle (replicate the model, shard the points)", fn); return GPMPC_ERR_STATE; }
     CUDA_TRY(cudaSetDevice(h->device));
     rc = ensure_predict_bufs(h, H);
     if (rc) return rc;
-    NvtxRange nvtx_r("gpmpc.predict_grad");
+    NvtxRange nvtx_r(ho ? "gpmpc.predict_hess" : "gpmpc.predict_grad");
     const int np = h->Npad, Nx = h->Nx, Ny = h->Ny, npairs = Nx * (Nx + 1) / 2;
     const int nblk_g = (np + GR_CHUNK - 1) / GR_CHUNK, nblk_mj = (np + ks_chunk(h) - 1) / ks_chunk(h);
     if (!h->dUall) {
@@ -1482,6 +1529,30 @@ extern "C" int gpmpc_predict_grad(gpmpc_handle_t h, int method, int H, const dou
     double* d_dvar = h->dGradOut;
     double* d_dcov = d_dvar + (long long)H * Ny * Nx;
     double* d_hess = d_dcov + (long long)H * Ny * Ny * Nx;
+    const long long nxx = (long long)Nx * Nx, ntri = (long long)Nx * (Nx + 1) * (Nx + 2) / 6;
+    double *d_d2var = nullptr, *d_d3mean = nullptr, *d_d2cov = nullptr, *d_sh = nullptr;
+    if (ho) {
+        if (!h->dDR) {
+            ALLOC(h->dDR, (long long)h->nloc * HB * np);
+            ALLOC(h->dVD, (long long)h->nloc * HB * np);
+            CUDA_TRY(cudaMemsetAsync(h->dDR, 0, (size_t)h->nloc * HB * np * 8, h->st));   // rows past a pass's last are never written
+            ALLOC(h->dPG, (long long)h->nloc * HB * nblk_g * npairs);
+            ALLOC(h->dPB2, (long long)h->nloc * HB * nblk_g * npairs);
+            ALLOC(h->dPM3, (long long)h->nloc * HB * nblk_g * ntri);
+        }
+        const long long hper = 2 * Ny * nxx + Ny * nxx * Nx + (long long)Ny * Ny * nxx;      // d2var | SH scratch | d3mean | d2cov
+        if (H > h->hessHcap) {
+            CUDA_TRY(cudaStreamSynchronize(h->st));
+            if (h->dHessOut) cudaFree(h->dHessOut);
+            h->dHessOut = nullptr; h->hessHcap = 0;
+            ALLOC(h->dHessOut, (long long)std::max(H, HB) * hper);
+            h->hessHcap = std::max(H, HB);
+        }
+        d_d2var = h->dHessOut;
+        d_sh = d_d2var + (long long)H * Ny * nxx;
+        d_d3mean = d_sh + (long long)H * Ny * nxx;
+        d_d2cov = d_d3mean + (long long)H * Ny * nxx * Nx;
+    }
     const size_t nz = (size_t)H * Nx, ns = (method == GPMPC_METHOD_TA) ? (size_t)(spp ? H : 1) * Nx * Nx : 0;
     CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, nz * 8, cudaMemcpyHostToDevice, h->st));
     if (ns) CUDA_TRY(cudaMemcpyAsync(h->dSigma, Sigma, ns * 8, cudaMemcpyHostToDevice, h->st));
@@ -1510,6 +1581,10 @@ extern "C" int gpmpc_predict_grad(gpmpc_handle_t h, int method, int H, const dou
         grad_finalize_kernel<<<dim3(Hc, h->nloc), 128, 0, h->st>>>(h->dPDV, h->dPH, nblk_g, Hc, h->dHyp, Nx + 2, Nx, Ny,
                                                                    h->dG, H, h0, d_dvar, d_hess);
         CUDA_TRY(cudaGetLastError());
+        if (ho) {
+            rc = hess_chunk(h, dZc, Hc, H, h0, d_d2var, d_d3mean);
+            if (rc) return rc;
+        }
     }
     {
         const int smem = (2 * Ny * Nx + Ny) * 8;
@@ -1517,6 +1592,11 @@ extern "C" int gpmpc_predict_grad(gpmpc_handle_t h, int method, int H, const dou
         CUDA_TRY(cudaGetLastError());
         grad_cov_kernel<<<H, 128, 2 * Ny * Nx * 8, h->st>>>(Ny, Nx, method == GPMPC_METHOD_TA, h->dSigma, spp, h->dJ, d_dvar, d_hess, d_dcov);
         CUDA_TRY(cudaGetLastError());
+        if (ho) {
+            hess_cov_kernel<<<H, 128, 2 * Ny * Nx * 8, h->st>>>(Ny, Nx, method == GPMPC_METHOD_TA, h->dSigma, spp, h->dJ, d_hess,
+                                                                d_d2var, d_d3mean, d_sh, d_d2cov);
+            CUDA_TRY(cudaGetLastError());
+        }
     }
     if (mean) CUDA_TRY(cudaMemcpyAsync(mean, h->dMean, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
     if (var) CUDA_TRY(cudaMemcpyAsync(var, h->dVar, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
@@ -1525,8 +1605,28 @@ extern "C" int gpmpc_predict_grad(gpmpc_handle_t h, int method, int H, const dou
     if (dvar_dz) CUDA_TRY(cudaMemcpyAsync(dvar_dz, d_dvar, (size_t)H * Ny * Nx * 8, cudaMemcpyDeviceToHost, h->st));
     if (dcov_dz) CUDA_TRY(cudaMemcpyAsync(dcov_dz, d_dcov, (size_t)H * Ny * Ny * Nx * 8, cudaMemcpyDeviceToHost, h->st));
     if (hess) CUDA_TRY(cudaMemcpyAsync(hess, d_hess, (size_t)H * Ny * Nx * Nx * 8, cudaMemcpyDeviceToHost, h->st));
+    if (ho && ho->d2var_dz2) CUDA_TRY(cudaMemcpyAsync(ho->d2var_dz2, d_d2var, (size_t)H * Ny * nxx * 8, cudaMemcpyDeviceToHost, h->st));
+    if (ho && ho->d3mean_dz3) CUDA_TRY(cudaMemcpyAsync(ho->d3mean_dz3, d_d3mean, (size_t)H * Ny * nxx * Nx * 8, cudaMemcpyDeviceToHost, h->st));
+    if (ho && ho->d2cov_dz2) CUDA_TRY(cudaMemcpyAsync(ho->d2cov_dz2, d_d2cov, (size_t)H * Ny * Ny * nxx * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
     return GPMPC_OK;
+}
+
+extern "C" int gpmpc_predict_grad(gpmpc_handle_t h, int method, int H, const double* Z, const double* Sigma, int spp,
+                                  double* mean, double* var, double* cov, double* jac,
+                                  double* dvar_dz, double* dcov_dz, double* hess)
+{
+    return predict_derivs(h, "gpmpc_predict_grad", method, H, Z, Sigma, spp, mean, var, cov, jac, dvar_dz, dcov_dz, hess, nullptr);
+}
+
+// predict_grad plus the second derivatives IPOPT's exact Hessian needs (see include/gpmpc.h)
+extern "C" int gpmpc_predict_hess(gpmpc_handle_t h, int method, int H, const double* Z, const double* Sigma, int spp,
+                                  double* mean, double* var, double* cov, double* jac,
+                                  double* dvar_dz, double* dcov_dz, double* hess,
+                                  double* d2var_dz2, double* d3mean_dz3, double* d2cov_dz2)
+{
+    const HessOutputs ho = {d2var_dz2, d3mean_dz3, d2cov_dz2};
+    return predict_derivs(h, "gpmpc_predict_hess", method, H, Z, Sigma, spp, mean, var, cov, jac, dvar_dz, dcov_dz, hess, &ho);
 }
 
 extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double* y_new)

@@ -1791,3 +1791,262 @@ grad_cov_kernel(int Ny, int Nx, int method_ta, const double* __restrict__ Sigma,
         out[idx] = s;
     }
 }
+
+// ---------------------------------------------------------------------------------------
+// Second derivatives of the prediction w.r.t. the test input (gpmpc_predict_hess: what CasADi's AD
+// produces when IPOPT uses the exact Hessian of the MPC's NLP, mpc_class.py:390-412, :496-513).  Per
+// output a and test point z, s_id = (X_id - z_d)/ell_d^2, beta = K^-1 ks, J / Hm the mean Jacobian / Hessian:
+//   d3 mean / dz_d dz_e dz_f = M3_def - d_de J_f/ell_d^2 - d_df J_e/ell_d^2 - d_ef J_d/ell_e^2
+//   d2 var / dz_d dz_e       = -2 [G_de + B2_de - d_de (ks^T K^-1 ks)/ell_d^2]
+//   M3_def = sum_i alpha_i ks_i s_id s_ie s_if     B2_de = sum_i beta_i ks_i s_id s_ie
+//   G_de = (L^-1 d_d ks)^T (L^-1 d_e ks)           ks^T K^-1 ks = sf2 - var
+// The rows d_d ks of R = 64/Nx test points at a time go through the predict product (V_d = L^-1 d_d ks);
+// everything else is fixed-order block partials like grad_reduce / grad_finalize.
+// ---------------------------------------------------------------------------------------
+
+// packed index q -> (d <= e <= f): d-major, then e, then f (the pair order of grad_reduce within each d)
+__device__ __forceinline__ void triple_of(int q, int Nx, int& d, int& e, int& f)
+{
+    int base = 0;
+    d = 0;
+    while (base + (Nx - d) * (Nx - d + 1) / 2 <= q) { base += (Nx - d) * (Nx - d + 1) / 2; ++d; }
+    const int r = q - base, m = Nx - d;
+    int e0 = 0, b2 = 0;
+    while (b2 + (m - e0) <= r) { b2 += m - e0; ++e0; }
+    e = d + e0;
+    f = e + (r - b2);
+}
+
+__device__ __forceinline__ void pair_of(int q, int Nx, int& d, int& e)
+{
+    int base = 0;
+    d = 0;
+    while (base + (Nx - d) <= q) { base += Nx - d; ++d; }
+    e = d + (q - base);
+}
+
+// A operand of the derivative product: row pt*Nx + d of output a = d_d ks of test point p0 + pt of the chunk
+// (h-major like KST, zero for i >= N).  grid (ceil(Npad/256), points of the pass, outputs), 256 threads.
+__global__ void __launch_bounds__(256)
+hess_rows_kernel(const double* __restrict__ XT, int ldx, int N, int Nx, const double* __restrict__ hyp, int hyp_ld,
+                 const double* __restrict__ Z, const double* __restrict__ KST, int ldk, long long sK,
+                 double* __restrict__ D, int p0)
+{
+    const int a = blockIdx.z, pt = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= ldk) return;
+    const int h = p0 + pt;
+    const double* hp = hyp + (long long)a * hyp_ld;
+    const double k = (i < N) ? KST[(long long)a * sK + (long long)h * ldk + i] : 0.0;
+    double* out = D + (long long)a * sK + (long long)pt * Nx * ldk + i;
+    for (int d = 0; d < Nx; ++d) {
+        const double e = hp[d], ie2 = 1.0 / (e * e);
+        const double sd = (i < N) ? (XT[(long long)d * ldx + i] - Z[(long long)h * Nx + d]) * ie2 : 0.0;
+        out[(long long)d * ldk] = k * sd;
+    }
+}
+
+// Stage 1 per (output, test point of the pass, 1024-point block): partial sums
+//   PG[q(d<=e)] = sum_i V_d,i V_e,i    PB[q] = sum_i beta_i ks_i s_id s_ie    PM[t(d<=e<=f)] = sum_i alpha_i ks_i s_id s_ie s_if
+// V rows from the derivative product, ks from KST, beta from the second product of predict_grad.
+// grid (Npad/1024, points of the pass, outputs), 256 threads; NX_MAX = 32: 528 pairs, 5984 triples.
+template <int NXP>
+__global__ void __launch_bounds__(256)
+hess_reduce_kernel(const double* __restrict__ XT, int ldx, int N, int Nx,
+                   const double* __restrict__ hyp, int hyp_ld,
+                   const double* __restrict__ alpha, long long sal,
+                   const double* __restrict__ Z,
+                   const double* __restrict__ KST, const double* __restrict__ BETA, const double* __restrict__ VD,
+                   int ldk, long long sK,
+                   double* __restrict__ PG, double* __restrict__ PB, double* __restrict__ PM, int nblk, int Hc, int p0)
+{
+    constexpr int NPR = (NXP * (NXP + 1) / 2 + 255) / 256;
+    constexpr int NTR = (NXP * (NXP + 1) * (NXP + 2) / 6 + 255) / 256;
+    extern __shared__ double hsm[];                 // S[Nx][257] (s_id), W[Nx][257] (V rows), WA[256], WB[256]
+    __shared__ double zs[NXP], ie2[NXP];
+    const int a = blockIdx.z, pt = blockIdx.y, blk = blockIdx.x, tid = threadIdx.x, h = p0 + pt;
+    double* S = hsm; double* W = hsm + Nx * 257; double* WA = W + Nx * 257; double* WB = WA + 256;
+    const double* hp = hyp + (long long)a * hyp_ld;
+    if (tid < NXP) {
+        const double e = (tid < Nx) ? hp[tid] : 1.0;
+        zs[tid] = (tid < Nx) ? Z[(long long)h * Nx + tid] : 0.0;
+        ie2[tid] = 1.0 / (e * e);
+    }
+    const int npairs = Nx * (Nx + 1) / 2, ntri = Nx * (Nx + 1) * (Nx + 2) / 6;
+    int pc[NPR], tc[NTR];                           // (d, e[, f]) of this thread's pairs / triples, 5 bits each
+#pragma unroll
+    for (int r = 0; r < NPR; ++r) {
+        int d = 0, e = 0;
+        if (tid + 256 * r < npairs) pair_of(tid + 256 * r, Nx, d, e);
+        pc[r] = d | (e << 5);
+    }
+#pragma unroll
+    for (int r = 0; r < NTR; ++r) {
+        int d = 0, e = 0, f = 0;
+        if (tid + 256 * r < ntri) triple_of(tid + 256 * r, Nx, d, e, f);
+        tc[r] = d | (e << 5) | (f << 10);
+    }
+    __syncthreads();
+    const double* ks = KST + (long long)a * sK + (long long)h * ldk;
+    const double* be = BETA + (long long)a * sK + (long long)h * ldk;
+    const double* vd = VD + (long long)a * sK + (long long)pt * Nx * ldk;
+    const double* al = alpha + (long long)a * sal;
+    double gacc[NPR], bacc[NPR], macc[NTR];
+#pragma unroll
+    for (int r = 0; r < NPR; ++r) { gacc[r] = 0.0; bacc[r] = 0.0; }
+#pragma unroll
+    for (int r = 0; r < NTR; ++r) macc[r] = 0.0;
+    for (int sub = 0; sub < GR_CHUNK / 256; ++sub) {
+        const int i = blk * GR_CHUNK + sub * 256 + tid;
+        double k = 0.0, wb = 0.0, wa = 0.0;
+        if (i < N) { k = ks[i]; wb = be[i] * k; wa = al[i] * k; }
+#pragma unroll
+        for (int d = 0; d < NXP; ++d) {
+            if (d < Nx) {
+                S[d * 257 + tid] = (i < N) ? (XT[(long long)d * ldx + i] - zs[d]) * ie2[d] : 0.0;
+                W[d * 257 + tid] = (i < N) ? vd[(long long)d * ldk + i] : 0.0;
+            }
+        }
+        WA[tid] = wa; WB[tid] = wb;
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < NPR; ++r) {
+            if (tid + 256 * r < npairs) {
+                const double* sd = S + (pc[r] & 31) * 257; const double* se = S + (pc[r] >> 5) * 257;
+                const double* vd_ = W + (pc[r] & 31) * 257; const double* ve = W + (pc[r] >> 5) * 257;
+                double g = 0.0, b = 0.0;
+                for (int t = 0; t < 256; ++t) {
+                    g = fma(vd_[t], ve[t], g);
+                    b = fma(WB[t] * sd[t], se[t], b);
+                }
+                gacc[r] += g; bacc[r] += b;
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < NTR; ++r) {
+            if (tid + 256 * r < ntri) {
+                const double* sd = S + (tc[r] & 31) * 257; const double* se = S + ((tc[r] >> 5) & 31) * 257;
+                const double* sf = S + (tc[r] >> 10) * 257;
+                double m = 0.0;
+                for (int t = 0; t < 256; ++t) m = fma(WA[t] * sd[t] * se[t], sf[t], m);
+                macc[r] += m;
+            }
+        }
+        __syncthreads();
+    }
+    const long long rec = ((long long)a * Hc + h) * nblk + blk;
+#pragma unroll
+    for (int r = 0; r < NPR; ++r) {
+        const int q = tid + 256 * r;
+        if (q < npairs) { PG[rec * npairs + q] = gacc[r]; PB[rec * npairs + q] = bacc[r]; }
+    }
+#pragma unroll
+    for (int r = 0; r < NTR; ++r) {
+        const int q = tid + 256 * r;
+        if (q < ntri) PM[rec * ntri + q] = macc[r];
+    }
+}
+
+// Stage 2 per (test point h of the chunk, output a): d2var (Nx,Nx) and d3mean (Nx,Nx,Nx) from the block
+// partials, each value written to every symmetric position (exactly symmetric).  grid (Hc, outputs), 128 threads.
+__global__ void __launch_bounds__(128)
+hess_finalize_kernel(const double* __restrict__ PG, const double* __restrict__ PB, const double* __restrict__ PM,
+                     int nblk, int Hc, const double* __restrict__ hyp, int hyp_ld, int Nx, int Ny,
+                     const double* __restrict__ G, int Htot, int h0,
+                     double* __restrict__ d2var, double* __restrict__ d3mean)
+{
+    const int h = blockIdx.x, a = blockIdx.y, tid = threadIdx.x;
+    const int npairs = Nx * (Nx + 1) / 2, ntri = Nx * (Nx + 1) * (Nx + 2) / 6;
+    const long long rec = ((long long)a * Hc + h) * nblk;
+    const double* hp = hyp + (long long)a * hyp_ld;
+    const double* g = G + (((long long)a) * Htot + h0 + h) * (Nx + 2);     // [mean, var, J]
+    const double sf = hp[Nx], q_kk = sf * sf - g[1];                       // ks^T K^-1 ks
+    double* V2 = d2var + (((long long)(h0 + h)) * Ny + a) * Nx * Nx;
+    double* T3 = d3mean + (((long long)(h0 + h)) * Ny + a) * Nx * Nx * Nx;
+    for (int q = tid; q < npairs; q += 128) {
+        int d, e;
+        pair_of(q, Nx, d, e);
+        double sg = 0.0, sb = 0.0;
+        for (int b = 0; b < nblk; ++b) { sg += PG[(rec + b) * npairs + q]; sb += PB[(rec + b) * npairs + q]; }
+        double s = sg + sb;
+        if (d == e) s -= q_kk / (hp[d] * hp[d]);
+        s *= -2.0;
+        V2[d * Nx + e] = s;
+        V2[e * Nx + d] = s;
+    }
+    for (int q = tid; q < ntri; q += 128) {
+        int d, e, f;
+        triple_of(q, Nx, d, e, f);
+        double s = 0.0;
+        for (int b = 0; b < nblk; ++b) s += PM[(rec + b) * ntri + q];
+        if (d == e) s -= g[2 + f] / (hp[d] * hp[d]);
+        if (d == f) s -= g[2 + e] / (hp[d] * hp[d]);
+        if (e == f) s -= g[2 + d] / (hp[e] * hp[e]);
+        T3[(d * Nx + e) * Nx + f] = s; T3[(d * Nx + f) * Nx + e] = s;
+        T3[(e * Nx + d) * Nx + f] = s; T3[(e * Nx + f) * Nx + d] = s;
+        T3[(f * Nx + d) * Nx + e] = s; T3[(f * Nx + e) * Nx + d] = s;
+    }
+}
+
+// Stage 3: d2 cov[a][b] / dz_f dz_g for every test point (grid H, 128 threads), the second-order analogue of
+// grad_cov_kernel (diag(var) + J Sigma J^T, gp_functions.py:167-171; Sigma need not be symmetric):
+//   'ME': delta_ab d2var_a[f][g]
+//   'TA': delta_ab d2var_a[f][g] + sum_d T_a[d][f][g] (Sigma J_b)[d] + sum_d (J_a Sigma)[d] T_b[d][f][g]
+//         + P_ab[f][g] + P_ab[g][f],   P_ab = Hm_a^T Sigma Hm_b  (SH_b = Sigma Hm_b staged in SHg, (H,Ny,Nx,Nx))
+// computed for f <= g and written to both halves.
+__global__ void __launch_bounds__(128)
+hess_cov_kernel(int Ny, int Nx, int method_ta, const double* __restrict__ Sigma, int sigma_per_point,
+                const double* __restrict__ J, const double* __restrict__ hess, const double* __restrict__ d2var,
+                const double* __restrict__ d3mean, double* __restrict__ SHg, double* __restrict__ d2cov)
+{
+    extern __shared__ double sh[];                  // SJ[Ny][Nx] = Sigma J_b, JS[Ny][Nx] = J_a Sigma
+    double* SJ = sh; double* JS = sh + Ny * Nx;
+    const int h = blockIdx.x, tid = threadIdx.x, nxx = Nx * Nx;
+    const double* Jh = J + (long long)h * Ny * Nx;
+    const double* Hh = hess + (long long)h * Ny * nxx;
+    double* SH = SHg + (long long)h * Ny * nxx;
+    if (method_ta) {
+        const double* Sg = Sigma + (sigma_per_point ? (long long)h * nxx : 0);
+        for (int idx = tid; idx < Ny * Nx; idx += 128) {
+            const int a = idx / Nx, d = idx % Nx;
+            double s1 = 0.0, s2 = 0.0;
+            for (int e = 0; e < Nx; ++e) {
+                s1 = fma(Sg[d * Nx + e], Jh[a * Nx + e], s1);          // (Sigma J_a)[d]
+                s2 = fma(Jh[a * Nx + e], Sg[e * Nx + d], s2);          // (J_a Sigma)[d]
+            }
+            SJ[idx] = s1; JS[idx] = s2;
+        }
+        for (int idx = tid; idx < Ny * nxx; idx += 128) {
+            const int b = idx / nxx, d = (idx / Nx) % Nx, g = idx % Nx;
+            const double* Hb = Hh + (long long)b * nxx;
+            double s = 0.0;
+            for (int e = 0; e < Nx; ++e) s = fma(Sg[d * Nx + e], Hb[e * Nx + g], s);
+            SH[idx] = s;
+        }
+    }
+    __syncthreads();
+    const int npairs = Nx * (Nx + 1) / 2;
+    const double* V2 = d2var + (long long)h * Ny * nxx;
+    const double* T3 = d3mean + (long long)h * Ny * nxx * Nx;
+    double* out = d2cov + (long long)h * Ny * Ny * nxx;
+    for (int idx = tid; idx < Ny * Ny * npairs; idx += 128) {
+        const int q = idx % npairs, b = (idx / npairs) % Ny, a = idx / (npairs * Ny);
+        int f, g;
+        pair_of(q, Nx, f, g);
+        double s = (a == b) ? V2[(long long)a * nxx + f * Nx + g] : 0.0;
+        if (method_ta) {
+            const double* Ta = T3 + (long long)a * nxx * Nx; const double* Tb = T3 + (long long)b * nxx * Nx;
+            const double* Ha = Hh + (long long)a * nxx; const double* SHb = SH + (long long)b * nxx;
+            double t = 0.0, pfg = 0.0, pgf = 0.0;
+            for (int d = 0; d < Nx; ++d) {
+                t = fma(Ta[d * nxx + f * Nx + g], SJ[b * Nx + d], t);
+                t = fma(JS[a * Nx + d], Tb[d * nxx + f * Nx + g], t);
+                pfg = fma(Ha[d * Nx + f], SHb[d * Nx + g], pfg);
+                pgf = fma(Ha[d * Nx + g], SHb[d * Nx + f], pgf);
+            }
+            s += t + (pfg + pgf);
+        }
+        double* o = out + ((long long)a * Ny + b) * nxx;
+        o[f * Nx + g] = s;
+        o[g * Nx + f] = s;
+    }
+}

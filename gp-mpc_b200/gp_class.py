@@ -372,6 +372,44 @@ class GP:
         out.update(mean=mean, dmean_dz=jac, dcov_dz=dcov)
         return out
 
+    def predict_batch_hess(self, x, u, cov=None, method=None):
+        """predict_batch_grad plus the second derivatives IPOPT's default exact Hessian makes CasADi extract
+        from the symbolic GP (mpc_class.py:496-513).  Adds, in the CALLER's units for z = [x,u]:
+            d2mean_dz2 (H,Ny,Nx,Nx)       d^2 mean_a / dz_d dz_e = hess * stdY_a / (stdZ_d stdZ_e)
+            d2cov_dz2  (H,Ny,Ny,Nx,Nx)    d^2 cov[a][b] / dz_f dz_g  (cov is not rescaled: 1/(stdZ_f stdZ_g))
+            dcov_dSigma_hess (H,Ny,Nx,Nx) hess_a[d][f] / stdZ_f, so that for 'TA' (Sigma in the GP's input space)
+                d^2 cov[a][b] / dz_f dSigma[d][e] = dcov_dSigma_hess[a,d,f] J[b,e] + J[a,d] dcov_dSigma_hess[b,e,f]
+                with J = dcov_dSigma_factor;  d^2 cov / dSigma^2 = 0.
+        Methods 'ME' and 'TA', errors as predict_batch_grad.  The same numbers reach `casadi.external` through
+        jac_jac_gp_b200 (include/gpmpc_casadi.h)."""
+        method = method or self.__gp_method
+        if method not in ('ME', 'TA'):
+            raise NotImplementedError("derivatives are available for gp_method 'ME' and 'TA'")
+        if self.__comm.world > 1 and self.__mode == 'outputs':
+            raise NotImplementedError('predict_batch_hess needs all outputs on one GPU (build the GP with a single-process Comm)')
+        x = np.asarray(x, dtype=np.float64).reshape(-1, self.__Ny)
+        u = np.asarray(u, dtype=np.float64).reshape(x.shape[0], self.__Nu)
+        if self.__normalize:
+            x = self.standardize(x, self.__meanX, self.__stdX)
+            u = self.standardize(u, self.__meanU, self.__stdU)
+        Z = np.hstack([x, u])
+        if cov is None and method == 'TA':
+            cov = np.zeros((self.__Nx, self.__Nx))
+        g = self.__engine.predict_hess(Z, cov if method == 'TA' else None, _GPU_METHODS[method])
+        mean, jac, dcov, hess, d2cov = g['mean'], g['jac'], g['dcov_dz'], g['hess'], g['d2cov_dz2']
+        out = dict(cov=g['cov'], dcov_dSigma_factor=jac.copy())
+        dS_hess = hess.copy()
+        if self.__normalize:
+            sz = self.__stdZ
+            mean = self.inverse_mean(mean, self.__meanY, self.__stdY)
+            jac = jac * self.__stdY[None, :, None] / sz[None, None, :]
+            dcov = dcov / sz[None, None, None, :]
+            hess = hess * self.__stdY[None, :, None, None] / (sz[:, None] * sz[None, :])[None, None]
+            d2cov = d2cov / (sz[:, None] * sz[None, :])[None, None, None]
+            dS_hess = dS_hess / sz[None, None, None, :]
+        out.update(mean=mean, dmean_dz=jac, dcov_dz=dcov, d2mean_dz2=hess, d2cov_dz2=d2cov, dcov_dSigma_hess=dS_hess)
+        return out
+
     def predict(self, x, u, cov):
         """ Predict future state  (reference gp_class.py:245-263)
 

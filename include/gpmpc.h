@@ -142,6 +142,21 @@ int gpmpc_predict_grad(gpmpc_handle_t h, int method, int H, const double* Z, con
                        int sigma_per_point, double* mean, double* var, double* cov, double* jac,
                        double* dvar_dz, double* dcov_dz, double* hess);
 
+/* gpmpc_predict_grad plus the second derivatives w.r.t. the test inputs: what CasADi's AD extracts from the
+ * same graphs (gp_functions.py:111-173) when IPOPT runs with its default exact Hessian
+ * (hessian_approximation 'exact'; nlpsol, mpc_class.py:496-513, over the shooting nodes of :390-412).  The
+ * first seven outputs equal gpmpc_predict_grad's bit for bit; further outputs, each optional (NULL to skip):
+ *   d2var_dz2  (H,Ny,Nx,Nx)        d^2 var_a / d z_d d z_e
+ *   d3mean_dz3 (H,Ny,Nx,Nx,Nx)     d^3 mean_a / d z_d d z_e d z_f  (the derivative of hess)
+ *   d2cov_dz2  (H,Ny,Ny,Nx,Nx)     d^2 cov[a][b] / d z_f d z_g of diag(var) ('ME') or diag(var) + J Sigma J^T ('TA')
+ * Symmetric tensors are exactly symmetric.  The mixed and Sigma-only second derivatives of 'TA' need no new
+ * quantities and are formed by the caller:  d^2 cov[a][b] / d z_f d Sigma[d][e] = hess_a[d][f] J_b[e] + J_a[d] hess_b[e][f],
+ * d^2 cov / d Sigma^2 = 0.  Methods ME and TA (EM: GPMPC_ERR_ARG); the handle must own all outputs (GPMPC_ERR_STATE). */
+int gpmpc_predict_hess(gpmpc_handle_t h, int method, int H, const double* Z, const double* Sigma,
+                       int sigma_per_point, double* mean, double* var, double* cov, double* jac,
+                       double* dvar_dz, double* dcov_dz, double* hess,
+                       double* d2var_dz2, double* d3mean_dz3, double* d2cov_dz2);
+
 /* Open-loop multi-step prediction with the state kept on the device: the numeric loop of GP.predict_compare
  * (gp_class.py:746-804, :779-792: mean_t, covar_x = predict(mean_t, u_t, covar); covar[:Ny,:Ny] = covar_x) for a
  * model whose inputs are z = [x, u] (Nx = Ny + Nu).  All Nt steps are enqueued back to back, one synchronisation.

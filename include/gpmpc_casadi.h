@@ -15,6 +15,8 @@
  *   z (Nx x Nt), sigma (Nx x Nx*Nt)  ->  mean (Ny x Nt), cov (Ny x Ny*Nt)
  *   jac_gp_b200(z, sigma, mean, cov) -> jac_mean_z, jac_mean_sigma (empty), jac_cov_z, jac_cov_sigma
  *   (block-diagonal: node t only depends on node t's inputs).
+ *   jac_jac_gp_b200(z, sigma, mean, cov, jac_mean_z, jac_mean_sigma, jac_cov_z, jac_cov_sigma) -> 16 blocks of
+ *   second derivatives (IPOPT's default exact Hessian; see below).
  */
 #ifndef GPMPC_CASADI_H
 #define GPMPC_CASADI_H
@@ -45,6 +47,23 @@ const long long* jac_gp_b200_sparsity_in(long long i);
 const long long* jac_gp_b200_sparsity_out(long long i);
 int jac_gp_b200_work(long long* sz_arg, long long* sz_res, long long* sz_iw, long long* sz_w);
 int jac_gp_b200(const double** arg, double** res, long long* iw, double* w, int mem);
+
+/* Second derivatives for IPOPT's exact Hessian: the Jacobian function CasADi looks up by name when it
+ * differentiates jac_gp_b200.  Inputs (z, sigma, out_mean, out_cov, out_jac_mean_z, out_jac_mean_sigma,
+ * out_jac_cov_z, out_jac_cov_sigma); outputs jac_jac_<o>_<i> for o in jac_gp_b200's outputs x i in its inputs
+ * (output-major, 16).  Rows index the column-major dense vec of the differentiated Jacobian, columns the
+ * dense vec of the input.  Nonzero: jac_mean_z/z, jac_cov_z/z and, for 'TA', jac_cov_z/sigma and
+ * jac_cov_sigma/z (block-diagonal over the nodes); all other outputs are structurally empty. */
+long long jac_jac_gp_b200_n_in(void);
+long long jac_jac_gp_b200_n_out(void);
+const char* jac_jac_gp_b200_name_in(long long i);
+const char* jac_jac_gp_b200_name_out(long long i);
+const long long* jac_jac_gp_b200_sparsity_in(long long i);
+const long long* jac_jac_gp_b200_sparsity_out(long long i);
+int jac_jac_gp_b200_work(long long* sz_arg, long long* sz_res, long long* sz_iw, long long* sz_w);
+void jac_jac_gp_b200_incref(void);
+void jac_jac_gp_b200_decref(void);
+int jac_jac_gp_b200(const double** arg, double** res, long long* iw, double* w, int mem);
 
 #ifdef __cplusplus
 }
