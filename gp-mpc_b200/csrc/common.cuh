@@ -49,7 +49,7 @@ __device__ __forceinline__ double warp_sum(double v) {
     return v;
 }
 
-// ---- TMA (bulk async copy) + mbarrier primitives: cp.async.bulk -> SASS UBLKCP, expect_tx -> SYNCS
+// ---- mbarrier primitives for the TMA tensor-map feeds: expect_tx -> SASS SYNCS
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(smem_u32(bar)), "r"(count) : "memory");
 }
@@ -77,11 +77,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
             else if (now - t0 > 20000000000ull) __trap();
         }
     } while (!ok);
-}
-// global -> shared bulk copy of `bytes` (multiple of 16), completion counted on `bar`
-__device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
-                 :: "r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {

@@ -31,11 +31,6 @@ struct GemmParams {
     double alpha, beta;
     int kflags;
     int lower;                       // compute tiles it >= jt only; mask col > row on diagonal tiles
-    int ksplit;                      // split-K chunk length (multiple of 16), 0 = off (blockIdx.y = chunk)
-    long long sPart;                 // element stride between split-K partial outputs
-    int lpt;                         // longest-processing-time-first block order for k <= j products:
-                                     // grid = (batch, nt reversed, chunk): every output's longest tiles
-                                     // are dispatched first, short partial chunks fill the tail
 };
 
 constexpr int GEMM_BK = 16;
@@ -49,9 +44,7 @@ struct GemmSmem {
     static constexpr int BYTES = STAGES * (A_STAGE + B_STAGE) * 8;
 };
 
-// TMA = true: tile rows are fetched with 1-D bulk async copies (cp.async.bulk, SASS UBLKCP) that
-// complete on one mbarrier per stage instead of cp.async groups; same smem layout and compute.
-template <int BM, int BN, int WM, int WN, bool BT, int STAGES, int MINB, bool TMA = false>
+template <int BM, int BN, int WM, int WN, bool BT, int STAGES, int MINB>
 __global__ void __launch_bounds__(WM * WN * 32, MINB)
 gemm_dmma_kernel(const GemmParams p)
 {
@@ -66,8 +59,6 @@ gemm_dmma_kernel(const GemmParams p)
     extern __shared__ __align__(16) double smem[];
     double* As = smem;
     double* Bs = smem + STAGES * A_STAGE;
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * (A_STAGE + B_STAGE));   // TMA only
-    constexpr uint32_t STAGE_TX = BT ? (BM + BN) * BK * 8 : (BM * BK + BK * BN) * 8;
 
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
@@ -75,14 +66,8 @@ gemm_dmma_kernel(const GemmParams p)
     const int wm = warp / WN, wn = warp % WN;
 
     int it, jt;
-    long long bz = blockIdx.z;
-    int chunk = blockIdx.y;
-    if (p.lpt) {
-        it = 0;
-        jt = p.nt - 1 - (int)blockIdx.y;
-        bz = blockIdx.x;
-        chunk = blockIdx.z;
-    } else if (p.lower) {
+    const long long bz = blockIdx.z;
+    if (p.lower) {
         const int tt = blockIdx.x;
         constexpr int R = RL > 0 ? RL : 1;
         it = (int)((sqrt(8.0 * (double)tt / R + 1.0) - 1.0) * 0.5);
@@ -99,14 +84,6 @@ gemm_dmma_kernel(const GemmParams p)
     if (p.kflags & GEMM_KI_GE) k_lo = max(k_lo, it * BM);
     if (p.kflags & GEMM_KJ_LE) k_hi = min(k_hi, (jt + 1) * BN);
     if (p.kflags & GEMM_KJ_GE) k_lo = max(k_lo, jt * BN);
-    long long part_off = 0;
-    if (p.ksplit) {
-        const int cs = chunk * p.ksplit;
-        k_lo = max(k_lo, cs);
-        k_hi = min(k_hi, cs + p.ksplit);
-        if (k_lo >= k_hi) return;            // the reducer applies the same chunk-validity rule
-        part_off = (long long)chunk * p.sPart;
-    }
     const int nk = (k_hi - k_lo) / BK;
 
     const double* Ag = p.A + bz * p.sA + (long long)it * BM * p.lda;
@@ -116,29 +93,22 @@ gemm_dmma_kernel(const GemmParams p)
     auto load_stage = [&](int s, int k0) {
         double* as = As + s * A_STAGE;
         double* bs = Bs + s * B_STAGE;
-        if constexpr (TMA) {
-            if (tid == 0) mbar_arrive_expect_tx(full + s, STAGE_TX);
-            for (int r = tid; r < BM; r += NT) tma_bulk_g2s(as + r * LDA_S, Ag + (long long)r * p.lda + k0, BK * 8, full + s);
-            if (BT) { for (int r = tid; r < BN; r += NT) tma_bulk_g2s(bs + r * LDB_S, Bg + (long long)r * p.ldb + k0, BK * 8, full + s); }
-            else { for (int r = tid; r < BK; r += NT) tma_bulk_g2s(bs + r * LDB_S, Bg + (long long)(k0 + r) * p.ldb, BN * 8, full + s); }
+#pragma unroll
+        for (int c = tid; c < BM * 8; c += NT) {
+            const int r = c >> 3, ch = c & 7;
+            cp_async16(as + r * LDA_S + ch * 2, Ag + (long long)r * p.lda + k0 + ch * 2);
+        }
+        if (BT) {
+#pragma unroll
+            for (int c = tid; c < BN * 8; c += NT) {
+                const int r = c >> 3, ch = c & 7;
+                cp_async16(bs + r * LDB_S + ch * 2, Bg + (long long)r * p.ldb + k0 + ch * 2);
+            }
         } else {
 #pragma unroll
-            for (int c = tid; c < BM * 8; c += NT) {
-                const int r = c >> 3, ch = c & 7;
-                cp_async16(as + r * LDA_S + ch * 2, Ag + (long long)r * p.lda + k0 + ch * 2);
-            }
-            if (BT) {
-#pragma unroll
-                for (int c = tid; c < BN * 8; c += NT) {
-                    const int r = c >> 3, ch = c & 7;
-                    cp_async16(bs + r * LDB_S + ch * 2, Bg + (long long)r * p.ldb + k0 + ch * 2);
-                }
-            } else {
-#pragma unroll
-                for (int c = tid; c < BK * (BN / 2); c += NT) {
-                    const int r = c / (BN / 2), ch = c % (BN / 2);
-                    cp_async16(bs + r * LDB_S + ch * 2, Bg + (long long)(k0 + r) * p.ldb + ch * 2);
-                }
+            for (int c = tid; c < BK * (BN / 2); c += NT) {
+                const int r = c / (BN / 2), ch = c % (BN / 2);
+                cp_async16(bs + r * LDB_S + ch * 2, Bg + (long long)(k0 + r) * p.ldb + ch * 2);
             }
         }
     };
@@ -149,28 +119,19 @@ gemm_dmma_kernel(const GemmParams p)
 #pragma unroll
         for (int ni = 0; ni < NF; ++ni) { acc[mi][ni][0] = 0.0; acc[mi][ni][1] = 0.0; }
 
-    if (TMA) {
-        if (tid == 0) {
-#pragma unroll
-            for (int s = 0; s < STAGES; ++s) mbar_init(full + s, 1);
-            mbar_fence_init();
-        }
-        __syncthreads();
-    }
 #pragma unroll
     for (int s = 0; s < STAGES - 1; ++s) {
         if (s < nk) load_stage(s, k_lo + s * BK);
-        if (!TMA) cp_async_commit();
+        cp_async_commit();
     }
 
     for (int kt = 0; kt < nk; ++kt) {
-        if (TMA) mbar_wait(full + kt % STAGES, (kt / STAGES) & 1);
-        else cp_async_wait<STAGES - 2>();
+        cp_async_wait<STAGES - 2>();
         __syncthreads();
         {   // prefetch the stage that was consumed in the previous iteration
             const int kn = kt + STAGES - 1;
             if (kn < nk) load_stage(kn % STAGES, k_lo + kn * BK);
-            if (!TMA) cp_async_commit();
+            cp_async_commit();
         }
         const int s = kt % STAGES;
         const double* as = As + s * A_STAGE + (wm * WTM + g) * LDA_S + t;
@@ -191,10 +152,10 @@ gemm_dmma_kernel(const GemmParams p)
                     dmma884(acc[mi][ni][0], acc[mi][ni][1], a[mi], b[ni]);
         }
     }
-    if (!TMA) cp_async_wait<0>();
+    cp_async_wait<0>();
 
     // epilogue: each lane owns two adjacent columns of every 8x8 fragment -> 16-byte accesses
-    double* Cg = p.C + bz * p.sC + part_off;
+    double* Cg = p.C + bz * p.sC;
     const double* Cing = p.Cin ? (p.Cin + bz * p.sCin) : nullptr;
     const bool diag = p.lower && ((jt + 1) * BN > it * BM);      // tile reaches the diagonal
 #pragma unroll
@@ -219,12 +180,12 @@ gemm_dmma_kernel(const GemmParams p)
     }
 }
 
-template <int BM, int BN, int WM, int WN, bool BT, int STAGES, int MINB, bool TMA = false>
-static cudaError_t gemm_launch(const GemmParams& p, int batch, int nchunks, cudaStream_t st)
+template <int BM, int BN, int WM, int WN, bool BT, int STAGES, int MINB>
+static cudaError_t gemm_launch(const GemmParams& p, int batch, cudaStream_t st)
 {
     using SM = GemmSmem<BM, BN, BT, STAGES>;
-    auto kern = gemm_dmma_kernel<BM, BN, WM, WN, BT, STAGES, MINB, TMA>;
-    constexpr int BYTES = SM::BYTES + (TMA ? STAGES * 8 : 0);
+    auto kern = gemm_dmma_kernel<BM, BN, WM, WN, BT, STAGES, MINB>;
+    constexpr int BYTES = SM::BYTES;
     static std::atomic<bool> configured[GPMPC_MAX_DEVICES];    // the attribute is per device; set-attribute is idempotent
     int dev = 0;
     cudaGetDevice(&dev);
@@ -235,9 +196,7 @@ static cudaError_t gemm_launch(const GemmParams& p, int batch, int nchunks, cuda
     }
     constexpr int R = (BM >= BN) ? BM / BN : 1;
     const int tiles = p.lower ? R * p.mt * (p.mt + 1) / 2 : p.mt * p.nt;
-    dim3 grid(tiles, p.ksplit ? nchunks : 1, batch);
-    if (p.lpt) grid = dim3(batch, p.nt, p.ksplit ? nchunks : 1);      // requires mt == 1
-    kern<<<grid, WM * WN * 32, BYTES, st>>>(p);
+    kern<<<dim3(tiles, 1, batch), WM * WN * 32, BYTES, st>>>(p);
     return cudaGetLastError();
 }
 
@@ -248,7 +207,7 @@ static cudaError_t gemm_launch(const GemmParams& p, int batch, int nchunks, cuda
 //     step kk, lane t  ->  k = 2 kk + (t & 1) + 8 (t >> 1)
 // (the MMA sums over k, so any permutation applied to A and B alike is valid); with the
 // 128B swizzle  chunk' = chunk ^ (row & 7)  the 16 lanes of a half-warp hit 16 distinct
-// 8-byte banks.  Same tiling / k-range / split-K / epilogue logic as gemm_dmma_kernel.
+// 8-byte banks.  Same tiling / k-range / epilogue logic as gemm_dmma_kernel.
 // =======================================================================================
 #include <cuda.h>
 #include <mutex>
@@ -290,11 +249,8 @@ gemm_dmma_tmap_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tm
     const int wm = warp / WN, wn = warp % WN;
 
     int it, jt;
-    long long bz = blockIdx.z;
-    int chunk = blockIdx.y;
-    if (p.lpt) {
-        it = 0; jt = p.nt - 1 - (int)blockIdx.y; bz = blockIdx.x; chunk = blockIdx.z;
-    } else if (p.lower) {
+    const long long bz = blockIdx.z;
+    if (p.lower) {
         const int tt = blockIdx.x;
         constexpr int R = RL > 0 ? RL : 1;
         it = (int)((sqrt(8.0 * (double)tt / R + 1.0) - 1.0) * 0.5);
@@ -310,14 +266,6 @@ gemm_dmma_tmap_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tm
     if (p.kflags & GEMM_KI_GE) k_lo = max(k_lo, it * BM);
     if (p.kflags & GEMM_KJ_LE) k_hi = min(k_hi, (jt + 1) * BN);
     if (p.kflags & GEMM_KJ_GE) k_lo = max(k_lo, jt * BN);
-    long long part_off = 0;
-    if (p.ksplit) {
-        const int cs = chunk * p.ksplit;
-        k_lo = max(k_lo, cs);
-        k_hi = min(k_hi, cs + p.ksplit);
-        if (k_lo >= k_hi) return;
-        part_off = (long long)chunk * p.sPart;
-    }
     const int nk = (k_hi - k_lo) / BK;
 
     if (tid == 0) {
@@ -373,7 +321,7 @@ gemm_dmma_tmap_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tm
         }
     }
 
-    double* Cg = p.C + bz * p.sC + part_off;
+    double* Cg = p.C + bz * p.sC;
     const double* Cing = p.Cin ? (p.Cin + bz * p.sCin) : nullptr;
     const bool diag = p.lower && ((jt + 1) * BN > it * BM);
 #pragma unroll
@@ -436,7 +384,7 @@ static bool tmap_make(CUtensorMap* tm, const double* base, int K, int rows, int 
 }
 
 template <int BM, int BN, int WM, int WN, int STAGES, int MINB>
-static cudaError_t gemm_tmap_launch(const GemmParams& p, int batch, int nchunks, cudaStream_t st)
+static cudaError_t gemm_tmap_launch(const GemmParams& p, int batch, cudaStream_t st)
 {
     auto kern = gemm_dmma_tmap_kernel<BM, BN, WM, WN, STAGES, MINB>;
     constexpr int BYTES = STAGES * (BM + BN) * GEMM_BK * 8 + STAGES * 8 + 1024;
@@ -453,8 +401,6 @@ static cudaError_t gemm_tmap_launch(const GemmParams& p, int batch, int nchunks,
     if (!tmap_make(&tmB, p.B, p.K, p.nt * BN, p.ldb, p.sB, batch, BN)) return cudaErrorInvalidValue;
     constexpr int R = (BM >= BN) ? BM / BN : 1;
     const int tiles = p.lower ? R * p.mt * (p.mt + 1) / 2 : p.mt * p.nt;
-    dim3 grid(tiles, p.ksplit ? nchunks : 1, batch);
-    if (p.lpt) grid = dim3(batch, p.nt, p.ksplit ? nchunks : 1);
-    kern<<<grid, WM * WN * 32, BYTES, st>>>(p, tmA, tmB);
+    kern<<<dim3(tiles, 1, batch), WM * WN * 32, BYTES, st>>>(p, tmA, tmB);
     return cudaGetLastError();
 }

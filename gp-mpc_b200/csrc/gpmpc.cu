@@ -24,6 +24,7 @@
 #define NX_MAX 32
 #define PSK_MAX_CTAS 2048
 #define MAX_DEPTH 12           // recursion depth bound: 128 * 2^12 rows
+#define LOOKAHEAD_MIN_ROWS 1024   // potrf_inv_rec defers part of a trailing update only on blocks at least this tall
 
 // ------------------------------------------------------------------------------------
 // minimal NCCL surface, bound at run time with dlopen (no link-time dependency)
@@ -71,7 +72,7 @@ struct gpmpc_handle_s {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // factorisation overlap: step 5a of every recursion depth runs on its own side stream
     cudaStream_t sideSt[MAX_DEPTH] = {nullptr}; cudaEvent_t evA[MAX_DEPTH] = {nullptr}, evB[MAX_DEPTH] = {nullptr}, evT[MAX_DEPTH] = {nullptr}, evS[MAX_DEPTH] = {nullptr};
-    long long w2off[MAX_DEPTH + 1] = {0}; int opt_overlap = 1, opt_lookahead = 1, opt_lookahead_min = 1024;
+    long long w2off[MAX_DEPTH + 1] = {0};
     // model
     double *dXT = nullptr, *dMu = nullptr, *dY = nullptr, *dHyp = nullptr, *dJit = nullptr, *dHypTmp = nullptr;
     double *dL = nullptr, *dLi = nullptr, *dW1 = nullptr, *dW2 = nullptr;
@@ -90,7 +91,7 @@ struct gpmpc_handle_s {
     double* dRoll = nullptr; size_t rollCap = 0;   // gpmpc_rollout: [Z | Sigma | U | scale | means | vars | cov]
     double *dIn = nullptr, *dOut = nullptr;   // [Z | Sigma] and [mean | var | J | cov] slabs: one H2D + one D2H per host call
     int Hcap = 0;
-    double* hPinned = nullptr; double* dPinnedAlias = nullptr; size_t hPinnedBytes = 0; int opt_zero_copy = 1;
+    double* hPinned = nullptr; double* dPinnedAlias = nullptr; size_t hPinnedBytes = 0;
     // nlml scratch
     double *dU = nullptr, *dKinv = nullptr, *dGradPart = nullptr, *dGrad = nullptr;
     bool has_data = false, has_hyper = false, factorized = false;
@@ -102,7 +103,7 @@ struct gpmpc_handle_s {
     std::vector<double> logdet, yalpha;
     std::vector<int> jitter_used;
     int sms = 132;                    // multiprocessors of the device (queried in create)
-    int opt_refine = 0, opt_gemm_variant = 3, opt_leaf_variant = 3, opt_small_tiles = 528;   // 128x64-tile count below which 64x32 tiles are used (4 per SM)
+    int opt_refine = 0, opt_small_tiles = 528;   // 128x64-tile count below which 64x32 tiles are used (4 per SM)
     // comm
     nccl_comm_t comm = nullptr; int rank = 0, world = 1;
     // peer (CUDA IPC) exchange: [flags: 2*MAXW u64][gather buffer parity 0][parity 1]
@@ -127,53 +128,29 @@ struct NvtxRange {
 };
 
 static inline long long slab(gpmpc_handle_t h) { return (long long)h->Npad * h->Npad; }
-static inline long long wslab(gpmpc_handle_t h) { return (long long)h->Npad * h->Npad / 4 + 128; }
 static inline long long w2slab(gpmpc_handle_t h) { return h->w2off[MAX_DEPTH]; }   // all depths, one batch entry
 
 // ------------------------------------------------------------------------------------
 // GEMM helpers (all operands live in slabs with leading dimension ld)
 // ------------------------------------------------------------------------------------
-static cudaError_t gemm128_on(gpmpc_handle_t h, cudaStream_t st, bool bt, const GemmParams& p, int batch);
-
-// callers describe the problem in 128x128 tiles (mt, nt); variant 1 re-tiles N by 64
-static cudaError_t gemm128(gpmpc_handle_t h, bool bt, const GemmParams& p, int batch)
+// Callers describe the problem in 128x128 tiles (mt, nt); the launch re-tiles it.  Tile-granular TMA
+// (tensor maps, 128B swizzle) serves the NT products that fill the GPU for at least two waves; everything
+// else (NN products, small launches) takes the cp.async kernel.
+static cudaError_t gemm128(gpmpc_handle_t h, cudaStream_t st, bool bt, const GemmParams& p, int batch)
 {
-    return gemm128_on(h, h->st, bt, p, batch);
-}
-
-static cudaError_t gemm128_on(gpmpc_handle_t h, cudaStream_t st, bool bt, const GemmParams& p, int batch)
-{
-    if (h->opt_gemm_variant == 3) {
-        // tile-granular TMA (tensor maps, 128B swizzle) for the NT products that fill the GPU for at
-        // least two waves; everything else (NN products, small launches) takes the cp.async variant
-        const long long tiles = (long long)batch * (p.lower ? (long long)p.mt * (p.mt + 1) : 2LL * p.mt * p.nt);
-        GemmParams q = p;
-        if (tiles < h->opt_small_tiles) {
-            // deep recursion levels: a handful of 128x64 tiles cannot occupy 132 SMs; 64x32 tiles
-            // (8x more CTAs, 4 CTAs/SM) cut the latency of these critical-path launches
-            q.mt = p.mt * 2; q.nt = p.nt * 4;
-            return bt ? gemm_launch<64, 32, 2, 2, true, 3, 4>(q, batch, 1, st)
-                      : gemm_launch<64, 32, 2, 2, false, 3, 4>(q, batch, 1, st);
-        }
-        q.nt = p.nt * 2;
-        if (bt && tiles >= 4LL * h->sms) return gemm_tmap_launch<128, 64, 2, 2, 4, 2>(q, batch, 1, st);
-        return bt ? gemm_launch<128, 64, 2, 2, true, 3, 2>(q, batch, 1, st)
-                  : gemm_launch<128, 64, 2, 2, false, 3, 2>(q, batch, 1, st);
+    const long long tiles = (long long)batch * (p.lower ? (long long)p.mt * (p.mt + 1) : 2LL * p.mt * p.nt);
+    GemmParams q = p;
+    if (tiles < h->opt_small_tiles) {
+        // deep recursion levels: a handful of 128x64 tiles cannot occupy 132 SMs; 64x32 tiles
+        // (8x more CTAs, 4 CTAs/SM) cut the latency of these critical-path launches
+        q.mt = p.mt * 2; q.nt = p.nt * 4;
+        return bt ? gemm_launch<64, 32, 2, 2, true, 3, 4>(q, batch, st)
+                  : gemm_launch<64, 32, 2, 2, false, 3, 4>(q, batch, st);
     }
-    if (h->opt_gemm_variant == 2) {       // variant 1 with the TMA (cp.async.bulk + mbarrier) feed
-        GemmParams q = p;
-        q.nt = p.nt * 2;
-        return bt ? gemm_launch<128, 64, 2, 2, true, 3, 2, true>(q, batch, 1, st)
-                  : gemm_launch<128, 64, 2, 2, false, 3, 2, true>(q, batch, 1, st);
-    }
-    if (h->opt_gemm_variant == 1) {       // 128x64 tiles, 4 warps, 3 stages, 2 CTAs/SM
-        GemmParams q = p;
-        q.nt = p.nt * 2;
-        return bt ? gemm_launch<128, 64, 2, 2, true, 3, 2>(q, batch, 1, st)
-                  : gemm_launch<128, 64, 2, 2, false, 3, 2>(q, batch, 1, st);
-    }
-    return bt ? gemm_launch<128, 128, 2, 4, true, 4, 1>(p, batch, 1, st)
-              : gemm_launch<128, 128, 2, 4, false, 4, 1>(p, batch, 1, st);
+    q.nt = p.nt * 2;
+    if (bt && tiles >= 4LL * h->sms) return gemm_tmap_launch<128, 64, 2, 2, 4, 2>(q, batch, st);
+    return bt ? gemm_launch<128, 64, 2, 2, true, 3, 2>(q, batch, st)
+              : gemm_launch<128, 64, 2, 2, false, 3, 2>(q, batch, st);
 }
 
 // Recursive blocked Cholesky + triangular inverse on the diagonal block
@@ -192,24 +169,11 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
         if (pend) CUDA_TRY(cudaStreamWaitEvent(h->st, pend, 0));
         static std::atomic<bool> conf[GPMPC_MAX_DEVICES];
         if (!conf[h->device % GPMPC_MAX_DEVICES].load(std::memory_order_acquire)) {
-            CUDA_TRY(cudaFuncSetAttribute(leaf_potrf_trtri_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LEAF_N * LEAF_LD * 8));
-            CUDA_TRY(cudaFuncSetAttribute(leaf_potrf_trtri_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LF_SMEM_DOUBLES * 8));
-            CUDA_TRY(cudaFuncSetAttribute(leaf_potrf_trtri_v3_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, LF3_SMEM_DOUBLES * 8));
-            CUDA_TRY(cudaFuncSetAttribute(leaf_potrf_trtri_v3_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, LF3_SMEM_DOUBLES * 8));
+            CUDA_TRY(cudaFuncSetAttribute(leaf_potrf_trtri_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LEAF_SMEM_DOUBLES * 8));
             conf[h->device % GPMPC_MAX_DEVICES].store(true, std::memory_order_release);
         }
-        if (h->opt_leaf_variant == 0)
-            leaf_potrf_trtri_kernel<<<batch, 256, LEAF_N * LEAF_LD * 8, h->st>>>(A + (long long)off * ld + off, ld, sA,
-                                                                              Li + (long long)off * ld + off, ld, sLi, dInfo, off);
-        else if (h->opt_leaf_variant == 1)
-            leaf_potrf_trtri_v2_kernel<<<batch, 256, LF_SMEM_DOUBLES * 8, h->st>>>(A + (long long)off * ld + off, ld, sA,
-                                                                                Li + (long long)off * ld + off, ld, sLi, dInfo, off);
-        else if (h->opt_leaf_variant == 2)
-            leaf_potrf_trtri_v3_kernel<false><<<batch, 256, LF3_SMEM_DOUBLES * 8, h->st>>>(A + (long long)off * ld + off, ld, sA,
-                                                                                        Li + (long long)off * ld + off, ld, sLi, dInfo, off);
-        else       // 3: v3 with two pivots per step
-            leaf_potrf_trtri_v3_kernel<true><<<batch, 256, LF3_SMEM_DOUBLES * 8, h->st>>>(A + (long long)off * ld + off, ld, sA,
-                                                                                       Li + (long long)off * ld + off, ld, sLi, dInfo, off);
+        leaf_potrf_trtri_kernel<<<batch, 256, LEAF_SMEM_DOUBLES * 8, h->st>>>(A + (long long)off * ld + off, ld, sA,
+                                                                           Li + (long long)off * ld + off, ld, sLi, dInfo, off);
         CUDA_TRY(cudaGetLastError());
         return GPMPC_OK;
     }
@@ -228,7 +192,7 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
     double* W1 = h->dW1 + h->w2off[depth];                 // one region per depth (deferred work of different depths is in flight together)
     double* W2 = h->dW2 + h->w2off[depth];
     const long long sW = w2slab(h), sW2 = w2slab(h);
-    const bool ovl = h->opt_overlap && depth < MAX_DEPTH;
+    const bool ovl = depth < MAX_DEPTH;
     cudaStream_t side = ovl ? h->sideSt[depth] : h->st;
     // LOOK-AHEAD.  rec(A22) starts with the leading h2 x h2 block of A22 (its own first half) and does not touch the rest
     // before its panel step.  So only the top h2 rows of the panel and the (1,1) block of the trailing update stay on the
@@ -236,7 +200,7 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
     // low-priority side stream beside the latency-bound recursion into A22_11 (leaves, small products) and are joined by
     // the child right before its panel step (`pend`).  On-chain share of a level's flops: 0.44 instead of 0.75.
     const int h2 = ((n2 / GPMPC_TILE) / 2) * GPMPC_TILE;
-    const bool split = ovl && h->opt_lookahead && h2 >= GPMPC_TILE && n >= h->opt_lookahead_min;
+    const bool split = ovl && h2 >= GPMPC_TILE && n >= LOOKAHEAD_MIN_ROWS;
     GemmParams p;
     auto panel = [&](cudaStream_t st, int r0, int rows) -> cudaError_t {     // W1[r0:r0+rows] = A21[r0:..] Li11^T ; L21 rows <- W1 rows
         GemmParams q;
@@ -245,7 +209,7 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
         q.B = Li11; q.ldb = ld; q.sB = sLi;                                   // B[j][k] = Li11[j][k] != 0 only for k <= j
         q.C = W1 + (long long)r0 * n1; q.ldc = n1; q.sC = sW;
         q.mt = rows / 128; q.nt = n1 / 128; q.K = n1; q.alpha = 1.0; q.beta = 0.0; q.kflags = GEMM_KJ_LE;
-        cudaError_t e = gemm128_on(h, st, true, q, batch);
+        cudaError_t e = gemm128(h, st, true, q, batch);
         if (e != cudaSuccess) return e;
         dim3 g(std::max(1, std::min(64, n1 / 2 / 128)), std::min(rows, 4096), batch);
         copy2d_kernel<<<g, 128, 0, st>>>(W1 + (long long)r0 * n1, n1, sW, A21 + (long long)r0 * ld, ld, sA, rows, n1);
@@ -258,7 +222,7 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
         q.B = W1 + (long long)c0 * n1; q.ldb = n1; q.sB = sW;
         q.C = A22 + (long long)r0 * ld + c0; q.ldc = ld; q.sC = sA; q.Cin = q.C; q.ldcin = ld; q.sCin = sA;
         q.mt = rows / 128; q.nt = cols / 128; q.K = n1; q.alpha = -1.0; q.beta = 1.0; q.lower = lower;
-        return gemm128_on(h, st, true, q, batch);
+        return gemm128(h, st, true, q, batch);
     };
     if (ovl) {
         CUDA_TRY(cudaEventRecord(h->evA[depth], h->st));
@@ -289,21 +253,21 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
     p.C = W2; p.ldc = n1; p.sC = sW2;
     p.mt = n2 / 128; p.nt = n1 / 128; p.K = n1; p.alpha = 1.0; p.beta = 0.0; p.kflags = GEMM_KJ_GE;
     if (ovl) {
-        CUDA_TRY(gemm128_on(h, side, false, p, batch));
+        CUDA_TRY(gemm128(h, side, false, p, batch));
         CUDA_TRY(cudaEventRecord(h->evB[depth], side));
     }
     // 4.
     rc = potrf_inv_rec(h, A, Li, sA, sLi, dInfo, off + n1, n2, batch, depth + 1, split ? h->evS[depth] : nullptr);
     if (rc) return rc;
     if (ovl) CUDA_TRY(cudaStreamWaitEvent(h->st, h->evB[depth], 0));
-    else CUDA_TRY(gemm128(h, false, p, batch));
+    else CUDA_TRY(gemm128(h, h->st, false, p, batch));
     // 5b. Li21 = -Li22 * W2   A[i][k] = Li22[i][k] != 0 only for k <= i
     memset(&p, 0, sizeof(p));
     p.A = Li22; p.lda = ld; p.sA = sLi;
     p.B = W2; p.ldb = n1; p.sB = sW2;
     p.C = Li21; p.ldc = ld; p.sC = sLi;
     p.mt = n2 / 128; p.nt = n1 / 128; p.K = n2; p.alpha = -1.0; p.beta = 0.0; p.kflags = GEMM_KI_LE;
-    CUDA_TRY(gemm128(h, false, p, batch));
+    CUDA_TRY(gemm128(h, h->st, false, p, batch));
     return GPMPC_OK;
 }
 
@@ -689,7 +653,7 @@ static int compute_kinv(gpmpc_handle_t h, int al)
     p.A = h->dU; p.lda = np; p.B = h->dU; p.ldb = np; p.C = h->dKinv; p.ldc = np;
     p.mt = np / 128; p.nt = np / 128; p.K = np; p.alpha = 1.0; p.beta = 0.0;
     p.kflags = GEMM_KI_GE | GEMM_KJ_GE; p.lower = 1;
-    CUDA_TRY(gemm128(h, true, p, 1));
+    CUDA_TRY(gemm128(h, h->st, true, p, 1));
     return GPMPC_OK;
 }
 
@@ -778,15 +742,9 @@ extern "C" int gpmpc_set_option(gpmpc_handle_t h, const char* name, double value
         if (v < 0 || v > PSK_MAX_CTAS) { set_error(h, "predict_ctas must be in [0, %d]", PSK_MAX_CTAS); return GPMPC_ERR_ARG; }
         h->opt_predict_ctas = v; return GPMPC_OK;
     }
-    if (!strcmp(name, "zero_copy")) { h->opt_zero_copy = value != 0.0; return GPMPC_OK; }
     if (!strcmp(name, "peer_timeout_s")) { h->opt_peer_timeout_s = value > 0.0 ? value : 60.0; return GPMPC_OK; }
-    if (!strcmp(name, "gemm_variant")) { h->opt_gemm_variant = (int)value; return GPMPC_OK; }
     if (!strcmp(name, "small_tiles")) { h->opt_small_tiles = (int)value; return GPMPC_OK; }
-    if (!strcmp(name, "overlap")) { h->opt_overlap = value != 0.0; return GPMPC_OK; }
-    if (!strcmp(name, "lookahead")) { h->opt_lookahead = value != 0.0; return GPMPC_OK; }
-    if (!strcmp(name, "lookahead_min")) { h->opt_lookahead_min = (int)value; return GPMPC_OK; }
     if (!strcmp(name, "peer")) { h->opt_peer = value != 0.0; return GPMPC_OK; }
-    if (!strcmp(name, "leaf_variant")) { h->opt_leaf_variant = (int)value; return GPMPC_OK; }
     set_error(h, "unknown option %s", name);
     return GPMPC_ERR_ARG;
 }
@@ -922,7 +880,7 @@ static inline int ks_chunk(gpmpc_handle_t h)
 template <int NXP, int CH>
 static cudaError_t launch_ks(gpmpc_handle_t h, const double* dZc, int Hc, int bm, int nblk)
 {
-    auto kern = ks_tile_kernel<NXP, CH, 2>;
+    auto kern = ks_tile_kernel<NXP, CH>;
     const int smem = (NXP + 1) * CH * 8;
     static std::atomic<bool> conf[GPMPC_MAX_DEVICES];
     if (!conf[h->device % GPMPC_MAX_DEVICES].load(std::memory_order_acquire)) {      // static + dynamic may pass 48 KB
@@ -1228,7 +1186,7 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
             gp.C = h->dU; gp.ldc = np;
             gp.mt = np / 128; gp.nt = np / 128; gp.K = np; gp.alpha = 1.0; gp.beta = 0.0;
             gp.kflags = GEMM_KI_LE; gp.lower = 1;
-            CUDA_TRY(gemm128(h, true, gp, 1));
+            CUDA_TRY(gemm128(h, h->st, true, gp, 1));
             em_trdot_kernel<<<ntr, 256, 0, h->st>>>(h->dU, h->dLi + (long long)a * slab(h), np, h->dEmTr + (long long)a * ntr);
             CUDA_TRY(cudaGetLastError());
         }
@@ -1401,8 +1359,8 @@ extern "C" int gpmpc_predict(gpmpc_handle_t h, int method, int H, const double* 
     // assembling CTA writes mean / var / J / cov straight into it (posted writes, visible after the stream sync).
     const int np_ = h->Npad;
     const long long ks_ctas = (long long)((np_ + ks_chunk(h) - 1) / ks_chunk(h)) * ((std::min(H, HB) + 7) / 8 * 8) * h->nloc;
-    const bool zc_in = h->opt_zero_copy && H <= HB && ks_ctas * Nx * 8 <= 256 * 1024 && in_span * 8 <= 64 * 1024;
-    const bool zc_out = h->opt_zero_copy && out_span * 8 <= 1024 * 1024;
+    const bool zc_in = H <= HB && ks_ctas * Nx * 8 <= 256 * 1024 && in_span * 8 <= 64 * 1024;
+    const bool zc_out = out_span * 8 <= 1024 * 1024;
     double* po = pin + in_span;
     const double* dZ_ = h->dZ; const double* dS_ = h->dSigma;
     if (zc_in) { dZ_ = h->dPinnedAlias; dS_ = h->dPinnedAlias + cap * Nx; }
@@ -1957,7 +1915,7 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
             p.A = h->dW1; p.lda = n1; p.B = h->dW1; p.ldb = n1;
             p.C = h->dLi; p.ldc = np; p.Cin = h->dLi; p.ldcin = np;
             p.mt = n2 / 128; p.nt = n2 / 128; p.K = n1; p.alpha = -1e-30; p.beta = 1.0; p.lower = 1;
-            cudaError_t e = gemm128(h, true, p, 1);
+            cudaError_t e = gemm128(h, h->st, true, p, 1);
             if (e != cudaSuccess) { set_error(h, "profile syrk: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
             return GPMPC_OK;
         }

@@ -13,7 +13,7 @@
 //   With u_i = sqrt(log2 e) (x_i - mu)/ell and q_i = -1/2 |u_i|^2 + 1/2 log2 sf2,
 //       log2 k(x_i, x_j) = q_i + q_j + u_i . u_j            (= log2 sf2 - log2(e)/2 |xs_i - xs_j|^2)
 //   so the O(N^2 Nx) part is a rank-Nx product done with DMMA m8n8k4 (tensor pipe), leaving the
-//   fp64 pipe only ~12 instructions per pair (two adds, clamp, a 256-entry-table exp2 with a
+//   fp64 pipe only ~12 instructions per pair (two adds, clamp, a two-level-table exp2 with a
 //   degree-4 polynomial).  a profile of the first (direct-difference, libm exp) kernel showed the fp64 pipe and DRAM
 //   traffic not overlapping: the two pipes now overlap and the kernel becomes write-bandwidth bound.
 //   The kernel is translation invariant, so inputs are centred on the column means mu: the
@@ -24,121 +24,18 @@
 //   mirrored tile (each exp2 serves two outputs).  q_i + q_j and the k-ordered dot product are
 //   commutative, so K is bitwise symmetric, including inside diagonal tiles.
 // ---------------------------------------------------------------------------------------
-// 2^(n/256), n = 0..255, correctly rounded (generated with 40-digit arithmetic)
-__constant__ double c_exp2_tab256[256] = {
-    1, 1.0027112750502025, 1.0054299011128027, 1.0081558981184175,
-    1.0108892860517005, 1.0136300849514894, 1.0163783149109531, 1.0191339960777379,
-    1.0218971486541166, 1.0246677928971357, 1.0274459491187637, 1.030231637686041,
-    1.0330248790212284, 1.0358256936019572, 1.0386341019613787, 1.0414501246883161,
-    1.0442737824274138, 1.0471050958792898, 1.0499440858006872, 1.0527907730046264,
-    1.0556451783605572, 1.0585073227945128, 1.0613772272892621, 1.0642549128844645,
-    1.0671404006768237, 1.0700337118202419, 1.0729348675259756, 1.075843889062791,
-    1.0787607977571199, 1.0816856149932152, 1.0846183622133092, 1.0875590609177697,
-    1.0905077326652577, 1.0934643990728858, 1.0964290818163769, 1.0994018026302219,
-    1.1023825833078409, 1.1053714457017412, 1.1083684117236787, 1.1113735033448175,
-    1.1143867425958924, 1.1174081515673693, 1.1204377524096067, 1.1234755673330199,
-    1.1265216186082418, 1.1295759285662881, 1.1326385195987192, 1.1357094141578055,
-    1.1387886347566916, 1.1418762039695616, 1.1449721444318042, 1.1480764788401789,
-    1.1511892299529827, 1.1543104205902159, 1.1574400736337511, 1.1605782120274988,
-    1.1637248587775775, 1.1668800369524817, 1.1700437696832502, 1.1732160801636373,
-    1.1763969916502812, 1.1795865274628758, 1.182784710984341, 1.1859915656609938,
-    1.189207115002721, 1.1924313825831512, 1.1956643920398273, 1.1989061670743806,
-    1.2021567314527031, 1.2054161090051239, 1.2086843236265816, 1.2119613992768012,
-    1.215247359980469, 1.2185422298274085, 1.2218460329727576, 1.2251587936371455,
-    1.22848053610687, 1.2318112847340759, 1.2351510639369334, 1.2384998981998165,
-    1.241857812073484, 1.245224830175258, 1.2486009771892048, 1.2519862778663162,
-    1.2553807570246911, 1.2587844395497165, 1.2621973503942507, 1.2656195145788063,
-    1.2690509571917332, 1.2724917033894028, 1.275941778396392, 1.2794012075056693,
-    1.2828700160787783, 1.2863482295460256, 1.2898358734066657, 1.2933329732290895,
-    1.2968395546510096, 1.3003556433796506, 1.3038812651919358, 1.3074164459346773,
-    1.3109612115247644, 1.3145155879493546, 1.318079601266064, 1.3216532776031575,
-    1.3252366431597413, 1.3288297242059544, 1.3324325470831615, 1.3360451382041458,
-    1.3396675240533029, 1.3432997311868353, 1.3469417862329458, 1.3505937158920345,
-    1.3542555469368927, 1.3579273062129011, 1.3616090206382248, 1.3653007172040119,
-    1.3690024229745905, 1.3727141650876684, 1.3764359707545302, 1.380167867260238,
-    1.383909881963832, 1.3876620422985291, 1.3914243757719262, 1.3951969099662003,
-    1.3989796725383112, 1.4027726912202048, 1.4065759938190154, 1.4103896082172707,
-    1.4142135623730951, 1.4180478843204152, 1.4218926021691656, 1.4257477441054942,
-    1.42961333839197, 1.4334894133677889, 1.4373759974489824, 1.4412731191286257,
-    1.4451808069770467, 1.449099089642035, 1.4530279958490526, 1.4569675544014438,
-    1.460917794180647, 1.4648787441464057, 1.4688504333369818, 1.4728328908693675,
-    1.4768261459394993, 1.4808302278224719, 1.4848451658727524, 1.488870989524397,
-    1.4929077282912648, 1.4969554117672355, 1.5010140696264256, 1.5050837316234065,
-    1.5091644275934228, 1.5132561874526098, 1.5173590411982147, 1.5214730189088146,
-    1.5255981507445384, 1.529734466947287, 1.5338819978409559, 1.5380407738316568,
-    1.5422108254079407, 1.5463921831410214, 1.550584877685, 1.5547889397770887,
-    1.5590044002378369, 1.5632312899713576, 1.567469639965553, 1.5717194812923414,
-    1.5759808451078865, 1.5802537626528246, 1.5845382652524937, 1.588834384317164,
-    1.593142151342267, 1.5974615979086271, 1.6017927556826934, 1.606135656416771,
-    1.6104903319492543, 1.6148568142048607, 1.6192351351948637, 1.6236253270173289,
-    1.6280274218573478, 1.632441451987275, 1.6368674497669644, 1.6413054476440063,
-    1.6457554781539649, 1.6502175739206177, 1.6546917676561943, 1.6591780921616162,
-    1.6636765803267364, 1.6681872651305825, 1.6727101796415966, 1.6772453570178785,
-    1.681792830507429, 1.6863526334483934, 1.6909247992693053, 1.6955093614893326,
-    1.7001063537185235, 1.7047158096580513, 1.7093377631004629, 1.713972247929926,
-    1.7186192981224779, 1.723278947746274, 1.7279512309618377, 1.7326361820223111,
-    1.7373338352737062, 1.7420442251551564, 1.746767386199169, 1.7515033530318782,
-    1.7562521603732995, 1.7610138430375839, 1.7657884359332727, 1.7705759740635547,
-    1.7753764925265212, 1.7801900265154245, 1.785016611318935, 1.789856282321401,
-    1.7947090750031072, 1.7995750249405351, 1.8044541678066239, 1.809346539371032,
-    1.8142521755003989, 1.8191711121586085, 1.8241033854070534, 1.8290490314048973,
-    1.8340080864093424, 1.8389805867758937, 1.843966568958626, 1.8489660695104508,
-    1.8539791250833855, 1.8590057724288205, 1.864046048397789, 1.8690999899412386,
-    1.8741676341103, 1.8792490180565602, 1.8843441790323345, 1.8894531543909392,
-    1.8945759815869656, 1.8997126981765553, 1.9048633418176741, 1.9100279502703899,
-    1.9152065613971474, 1.9203992131630474, 1.925605943636125, 1.9308267909876271,
-    1.9360617934922943, 1.9413109895286405, 1.9465744175792332, 1.9518521162309783,
-    1.9571441241754002, 1.9624504802089273, 1.9677712232331759, 1.9731063922552343,
-    1.9784560263879509, 1.9838201648502194, 1.9891988469672663, 1.9945921121709402};
-
-// 2^t for -1020 <= t <= ~1000 (the CALLER clamps: rint(256 t) must fit the low word and the exponent stay normal): 256-entry table + degree-4 polynomial on
-// |f| <= 1/512 (truncation 3.8e-17), ~1.7 ulp.  Per value: 2 (rint by magic constant) + 1 (f) +
-// 4 (Horner) + table load + multiply + exponent insert -- the r1 kernel (16-entry table, degree 7)
-// was bound by issue slots, not by HBM.
-__device__ __forceinline__ double exp2_t256(double t, const double* __restrict__ T256)
-{
-    const double SH = 6755399441055744.0;            // 1.5 * 2^52: rint(256 t) lands in the low word
-    const double s = fma(t, 256.0, SH);
-    const int n = __double2loint(s);
-    const double f = fma(s - SH, -0.00390625, t);    // |f| <= 1/512, exact
-    double p = 0.009618129107628477;                 // (ln 2)^k / k!, k = 4..1
-    p = fma(p, f, 0.05550410866482158);
-    p = fma(p, f, 0.24022650695910072);
-    p = fma(p, f, 0.6931471805599453);
-    p = fma(p, f, 1.0);
-    p *= T256[n & 255];
-    return __hiloint2double(__double2hiint(p) + ((n >> 8) << 20), __double2loint(p));
-}
-
-// same with the 16-entry table (c_exp2_tab, one entry per shared-memory bank => conflict-free) and a
-// degree-7 polynomial on |f| <= 1/32
+// 2^(k/16) and 2^(m/256), k, m = 0..15, correctly rounded (generated with 40-digit arithmetic)
 __constant__ double c_exp2_tab[16] = {
     1.0, 1.0442737824274138, 1.0905077326652577, 1.1387886347566916, 1.189207115002721,
     1.241857812073484, 1.2968395546510096, 1.3542555469368927, 1.4142135623730951,
     1.4768261459394993, 1.5422108254079407, 1.6104903319492543, 1.681792830507429,
     1.7562521603732995, 1.8340080864093424, 1.9152065613971474};
-__device__ __forceinline__ double exp2_t16(double t, const double* __restrict__ T16)
-{
-    const double SH = 6755399441055744.0;
-    const double s = fma(t, 16.0, SH);
-    const int n = __double2loint(s);
-    const double f = fma(s - SH, -0.0625, t);        // |f| <= 1/32, exact
-    double p = 1.5252733804059838e-05;               // (ln 2)^k / k!, k = 7..1
-    p = fma(p, f, 0.00015403530393381606);
-    p = fma(p, f, 0.0013333558146428441);
-    p = fma(p, f, 0.009618129107628477);
-    p = fma(p, f, 0.055504108664821576);
-    p = fma(p, f, 0.2402265069591007);
-    p = fma(p, f, 0.6931471805599453);
-    p = fma(p, f, 1.0);
-    p *= T16[n & 15];
-    return __hiloint2double(__double2hiint(p) + ((n >> 4) << 20), __double2loint(p));
-}
-
 // Two-level table: 2^t = 2^e * T1[(n >> 4) & 15] * T2[n & 15] * 2^f with n = rint(256 t), T1[k] = 2^(k/16), T2[m] = 2^(m/256),
 // |f| <= 1/512 (degree-4 polynomial, truncation 3.8e-17).  Both tables have ONE entry per shared-memory bank, so the
-// lookups are conflict-free whatever the lane pattern (the flat 256-entry table replays ~3x), and the polynomial needs four
-// coefficients instead of seven (each costs two UMOVs in the loop on this target).  ~2.2 ulp.
+// lookups are conflict-free whatever the lane pattern (a flat 256-entry table replays ~3x), and the polynomial needs four
+// coefficients where a single 16-entry table needs seven (each costs two UMOVs in the loop on this target).  ~2.2 ulp.
+// Valid for -1020 <= t <= ~1000: the CALLER clamps (rint(256 t) must fit the low word and the exponent stay normal).
+// T32 is a shared-memory copy of both tables: T32[0..15] = c_exp2_tab, T32[16..31] = c_exp2_tab2.
 __constant__ double c_exp2_tab2[16] = {
     1, 1.0027112750502025, 1.0054299011128027, 1.0081558981184175, 1.0108892860517005, 1.0136300849514894,
     1.0163783149109531, 1.0191339960777379, 1.0218971486541166, 1.0246677928971357, 1.0274459491187637,
@@ -291,296 +188,28 @@ kbuild_dmma_kernel(const double* __restrict__ XT, int ldx, int N, int Nx, const 
 //   np.linalg.cholesky at optimize.py:346/485; a non-positive pivot is reported LAPACK
 //   style (1-based global index) so the host can apply the reference's single 1e-8
 //   jitter retry (optimize.py:347-350).  One CTA per batch entry; whole block in smem.
-// ---------------------------------------------------------------------------------------
-#define LEAF_N 128
-#define LEAF_LD 129
-__global__ void __launch_bounds__(256, 1)
-leaf_potrf_trtri_kernel(double* __restrict__ A, int lda, long long sA,
-                        double* __restrict__ Li, int ldi, long long sLi,
-                        int* __restrict__ info, int info_base)
-{
-    extern __shared__ double S[];           // [128][129]
-    __shared__ double colbuf[LEAF_N];
-    const int tid = threadIdx.x;
-    double* Ab = A + (long long)blockIdx.x * sA;
-    double* Lb = Li + (long long)blockIdx.x * sLi;
-    for (int idx = tid; idx < LEAF_N * LEAF_N; idx += 256) {
-        const int r = idx >> 7, c = idx & 127;
-        S[r * LEAF_LD + c] = Ab[(long long)r * lda + c];
-    }
-    __syncthreads();
-    const int tx = tid & 15, ty = tid >> 4;
-    for (int j = 0; j < LEAF_N; ++j) {
-        const double d = S[j * LEAF_LD + j];
-        if (!(d > 0.0) && tid == 0) atomicCAS(info + blockIdx.x, 0, info_base + j + 1);
-        const double dj = sqrt(d);
-        const double inv = 1.0 / dj;
-        __syncthreads();                    // everyone has read the pivot
-        if (tid < LEAF_N) {
-            if (tid == j) S[j * LEAF_LD + j] = dj;
-            else if (tid > j) S[tid * LEAF_LD + j] *= inv;
-        }
-        __syncthreads();
-        for (int i = j + 1 + ty; i < LEAF_N; i += 16) {
-            const double lij = S[i * LEAF_LD + j];
-            for (int k = j + 1 + tx; k <= i; k += 16)
-                S[i * LEAF_LD + k] = fma(-lij, S[k * LEAF_LD + j], S[i * LEAF_LD + k]);
-        }
-        __syncthreads();
-    }
-    for (int idx = tid; idx < LEAF_N * LEAF_N; idx += 256) {
-        const int r = idx >> 7, c = idx & 127;
-        Ab[(long long)r * lda + c] = (c <= r) ? S[r * LEAF_LD + c] : 0.0;
-    }
-    // in-place lower-triangular inverse, last column first:
-    //   Linv[j][j] = 1/L[j][j];  Linv[i][j] = -Linv[j][j] * sum_{k=j+1..i} Linv[i][k] * L[k][j]
-    for (int j = LEAF_N - 1; j >= 0; --j) {
-        if (tid < LEAF_N && tid > j) colbuf[tid] = S[tid * LEAF_LD + j];
-        const double djj = 1.0 / S[j * LEAF_LD + j];
-        __syncthreads();
-        const int i = j + 1 + (tid >> 1);
-        double s0 = 0.0, s1 = 0.0;
-        if (i < LEAF_N) {
-            int k = j + 1 + (tid & 1);
-            for (; k + 2 <= i; k += 4) {
-                s0 = fma(S[i * LEAF_LD + k], colbuf[k], s0);
-                s1 = fma(S[i * LEAF_LD + k + 2], colbuf[k + 2], s1);
-            }
-            if (k <= i) s0 = fma(S[i * LEAF_LD + k], colbuf[k], s0);
-        }
-        double s = s0 + s1;
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        __syncthreads();
-        if (i < LEAF_N && (tid & 1) == 0) S[i * LEAF_LD + j] = -djj * s;
-        if (tid == 0) S[j * LEAF_LD + j] = djj;
-        __syncthreads();
-    }
-    for (int idx = tid; idx < LEAF_N * LEAF_N; idx += 256) {
-        const int r = idx >> 7, c = idx & 127;
-        Lb[(long long)r * ldi + c] = (c <= r) ? S[r * LEAF_LD + c] : 0.0;
-    }
-}
-
-// ---------------------------------------------------------------------------------------
-// a3 leaf v2: blocked (nb = 16) Cholesky + triangular inverse of a 128x128 diagonal block,
-// entirely in shared memory.  Per block step: one warp factorises and inverts the 16x16
-// diagonal block (smem, __syncwarp only); all threads form the panel L21 = A21 D^-T with the
-// small inverse; the trailing update and the inverse assembly run on DMMA fragments read
-// straight from shared memory (row stride 132 doubles: (g*32 + t*8) mod 128 conflict-free).
-// Same outputs / info convention as the v1 kernel (which it replaced).
-// ---------------------------------------------------------------------------------------
-#define LF_LD 132
-// optional phase clock stamps of CTA 0 (diagnostics: gpmpc_profile_leaf)
-__device__ long long* d_leaf_prof = nullptr;
-#define LEAF_STAMP(k) do { if (d_leaf_prof && blockIdx.x == 0 && threadIdx.x == 0) d_leaf_prof[k] = clock64(); } while (0)
-#define LF_NB 16
-#define LF_XLD 20
-#define LF_SMEM_DOUBLES (LEAF_N * LF_LD + 8 * 16 * 17 + 2 * LEAF_N * LF_XLD)
-
-__device__ __forceinline__ void warp_potrf16_trtri16(double* D, double* Dinv, int* info, int info_val0, int lane)
-{
-    // D: 16x16 block (lower part valid) with row stride LF_LD; Dinv: [16][17].
-    // Register-resident: lane r (and its mirror r+16) holds row r; pivots / multipliers travel
-    // by shuffle, so the 16 column steps need no shared-memory round trips.
-    const unsigned full = 0xffffffffu;
-    const int r = lane & 15;
-    double a[16], ipd[16];
-#pragma unroll
-    for (int k = 0; k < 16; ++k) a[k] = D[r * LF_LD + k];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-        const double d = __shfl_sync(full, a[j], j);
-        if (!(d > 0.0) && lane == 0) atomicCAS(info, 0, info_val0 + j + 1);
-        // sqrt and reciprocal from one rsqrt + Newton corrections (shorter dependent chain than
-        // DSQRT followed by a division; both results are correctly rounded to ~0.5 ulp)
-        double y = rsqrt(d);
-        double pv = d * y;
-        pv = fma(fma(-pv, pv, d), 0.5 * y, pv);
-        y = fma(fma(-pv, y, 1.0), y, y);
-        if (!(d > 0.0)) { pv = sqrt(d); y = 1.0 / pv; }     // keep NaN/inf propagation of the plain formula
-        ipd[j] = y;
-        a[j] = (r == j) ? pv : a[j] * ipd[j];              // l_rj for r > j (LAPACK dpotf2 scales by 1/ajj too)
-#pragma unroll
-        for (int k = j + 1; k < 16; ++k) {
-            const double lkj = __shfl_sync(full, a[j], k);
-            a[k] = fma(-a[j], lkj, a[k]);                  // meaningful for r >= k; upper part is never read
-        }
-    }
-    __syncwarp();
-    if (lane < 16) {
-#pragma unroll
-        for (int k = 0; k < 16; ++k) if (k <= r) D[r * LF_LD + k] = a[k];
-    }
-    // column r of the inverse by forward substitution; L[i][k] is broadcast from lane i
-    double x[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-        double sacc = 0.0;
-#pragma unroll
-        for (int k = 0; k < i; ++k) sacc = fma(__shfl_sync(full, a[k], i), x[k], sacc);
-        x[i] = (i < r) ? 0.0 : ((i == r) ? ipd[i] : -sacc * ipd[i]);
-        if (lane < 16) Dinv[i * 17 + r] = x[i];
-    }
-    __syncwarp();
-}
-
-__global__ void __launch_bounds__(256, 1)
-leaf_potrf_trtri_v2_kernel(double* __restrict__ A, int lda, long long sA,
-                           double* __restrict__ Li, int ldi, long long sLi,
-                           int* __restrict__ info, int info_base)
-{
-    extern __shared__ __align__(16) double S[];                // [128][132]
-    double* DinvAll = S + LEAF_N * LF_LD;                      // [8][16][17]
-    double* Xs = DinvAll + 8 * 16 * 17;                        // scratch for the inverse assembly (2 x 128 x 20 doubles)
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
-    double* Ab = A + (long long)blockIdx.x * sA;
-    double* Lb = Li + (long long)blockIdx.x * sLi;
-    LEAF_STAMP(0);
-    for (int idx = tid; idx < LEAF_N * LEAF_N; idx += 256) {
-        const int r = idx >> 7, c = idx & 127;
-        S[r * LF_LD + c] = Ab[(long long)r * lda + c];
-    }
-    __syncthreads();
-    LEAF_STAMP(1);
-
-    // ---------------- Cholesky, right-looking, nb = 16, with look-ahead ----------------
-    // After the panel of step kb only the next block column is updated by everyone (C1); then warp 0
-    // factorises + inverts the next diagonal block WHILE warps 1..7 finish the trailing update (C2).
-    auto panel = [&](int c0, const double* Dinv) {
-        // P[r][j] = sum_{k<=j} A[r][c0+k] * Dinv[j][k]; two threads per row (8 columns each)
-        const int nbel = LEAF_N - c0 - LF_NB;
-        const int rr = tid >> 1, half = tid & 1;
-        double a[16];
-        if (rr < nbel) {
-            const double* src = S + (c0 + LF_NB + rr) * LF_LD + c0;
-#pragma unroll
-            for (int k = 0; k < 16; ++k) a[k] = src[k];
-        }
-        __syncwarp();
-        if (rr < nbel) {
-            double* dst = S + (c0 + LF_NB + rr) * LF_LD + c0;
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-                const int j = half * 8 + jj;
-                double sacc = 0.0;
-#pragma unroll
-                for (int k = 0; k < 16; ++k) if (k <= j) sacc = fma(a[k], Dinv[j * 17 + k], sacc);
-                dst[j] = sacc;
-            }
-        }
-    };
-    auto update_tile = [&](int c0, int ti, int tj) {      // C(8x8 at tile ti,tj of the trailing block) -= P_R P_C^T
-        const int R0 = c0 + LF_NB + 8 * ti, C0 = c0 + LF_NB + 8 * tj;
-        double* cp = S + (R0 + g) * LF_LD + C0 + 2 * t;
-        double acc0 = cp[0], acc1 = cp[1];
-        const double* pa = S + (R0 + g) * LF_LD + c0 + t;
-        const double* pb = S + (C0 + g) * LF_LD + c0 + t;
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) dmma884(acc0, acc1, -pa[kk * 4], pb[kk * 4]);
-        cp[0] = acc0; cp[1] = acc1;
-    };
-    if (warp == 0) warp_potrf16_trtri16(S, DinvAll, info + blockIdx.x, info_base, lane);
-    __syncthreads();
-    panel(0, DinvAll);
-    __syncthreads();
-    LEAF_STAMP(2);
-    for (int kb = 0; kb < 7; ++kb) {
-        const int c0 = kb * LF_NB, b0 = c0 + LF_NB;
-        const int nt8 = (LEAF_N - b0) >> 3;
-        // C1: the two 8-wide tile columns of the next block column
-        for (int tl = warp; tl < 2 * nt8; tl += 8) {
-            const int ti = tl >> 1, tj = tl & 1;
-            if (tj <= ti) update_tile(c0, ti, tj);
-        }
-        __syncthreads();
-        if (warp == 0) {
-            warp_potrf16_trtri16(S + b0 * LF_LD + b0, DinvAll + (kb + 1) * 16 * 17, info + blockIdx.x, info_base + b0, lane);
-        } else {
-            // C2: tiles 2 <= tj <= ti < nt8 on warps 1..7
-            const int m = nt8 - 2;
-            const int ntile = m > 0 ? m * (m + 1) / 2 : 0;
-            for (int tl = warp - 1; tl < ntile; tl += 7) {
-                int ti = (int)((sqrtf(8.0f * (float)tl + 1.0f) - 1.0f) * 0.5f);
-                while (ti * (ti + 1) / 2 > tl) --ti;
-                while ((ti + 1) * (ti + 2) / 2 <= tl) ++ti;
-                const int tj = tl - ti * (ti + 1) / 2;
-                update_tile(c0, ti + 2, tj + 2);
-            }
-        }
-        __syncthreads();
-        panel(b0, DinvAll + (kb + 1) * 16 * 17);
-        __syncthreads();
-        LEAF_STAMP(3 + kb);
-    }
-    for (int idx = tid; idx < LEAF_N * LEAF_N; idx += 256) {
-        const int r = idx >> 7, c = idx & 127;
-        Ab[(long long)r * lda + c] = (c <= r) ? S[r * LF_LD + c] : 0.0;
-    }
-    __syncthreads();
-    LEAF_STAMP(10);
-
-    // ---------------- triangular inverse by recursive doubling ----------------
-    // the 16x16 diagonal inverses are known; for s = 16, 32, 64 every aligned pair of inverted
-    // blocks [A^-1 (p..p+s), C^-1 (p+s..p+2s)] is completed with  X = -C^-1 (B A^-1)  written over
-    // B = L[p+s.., p..] in place: 3 levels x 2 DMMA products instead of 8 sequential block columns
-    {
-        const int r = tid >> 4, c = tid & 15;               // 16 x 16 threads
-        for (int kb = 0; kb < 8; ++kb)                      // exact zeros above the diagonal: DMMA k-ranges read them
-            S[(kb * 16 + r) * LF_LD + kb * 16 + c] = (c <= r) ? DinvAll[kb * 16 * 17 + r * 17 + c] : 0.0;
-    }
-    __syncthreads();
-    double* T1 = Xs;                                        // [pairs][s][s+4], at most 4096+ doubles (Xs and Ys are adjacent)
-    for (int sz = 16; sz < LEAF_N; sz <<= 1) {
-        const int npair = LEAF_N / (2 * sz), t8 = sz >> 3, ldt = sz + 4;
-        const int ntile = npair * t8 * t8;
-        // T1 = B * Ainv   (Ainv lower: k >= j)
-        for (int tl = warp; tl < ntile; tl += 8) {
-            const int pr = tl / (t8 * t8), ti = (tl / t8) % t8, tj = tl % t8;
-            const int p0 = pr * 2 * sz;
-            const double* pa = S + (p0 + sz + 8 * ti + g) * LF_LD + p0 + t;            // B rows
-            const double* pb = S + (p0 + t) * LF_LD + p0 + 8 * tj + g;                 // Ainv[k][n]
-            double a0 = 0.0, a1 = 0.0;
-            for (int k0 = 8 * tj; k0 < sz; k0 += 4) dmma884(a0, a1, pa[k0], pb[k0 * LF_LD]);
-            double* tp = T1 + pr * sz * ldt + (8 * ti + g) * ldt + 8 * tj + 2 * t;
-            tp[0] = a0; tp[1] = a1;
-        }
-        __syncthreads();
-        // X = -Cinv * T1  (Cinv lower: k <= i), written over B
-        for (int tl = warp; tl < ntile; tl += 8) {
-            const int pr = tl / (t8 * t8), ti = (tl / t8) % t8, tj = tl % t8;
-            const int p0 = pr * 2 * sz;
-            const double* pa = S + (p0 + sz + 8 * ti + g) * LF_LD + p0 + sz + t;       // Cinv rows
-            const double* pb = T1 + pr * sz * ldt + t * ldt + 8 * tj + g;              // T1[k][n]
-            double a0 = 0.0, a1 = 0.0;
-            for (int k0 = 0; k0 < 8 * ti + 8; k0 += 4) dmma884(a0, a1, -pa[k0], pb[k0 * ldt]);
-            double* xp = S + (p0 + sz + 8 * ti + g) * LF_LD + p0 + 8 * tj + 2 * t;
-            xp[0] = a0; xp[1] = a1;
-        }
-        __syncthreads();
-        LEAF_STAMP(sz == 16 ? 11 : (sz == 32 ? 12 : 13));
-    }
-    for (int idx = tid; idx < LEAF_N * LEAF_N; idx += 256) {
-        const int r = idx >> 7, c = idx & 127;
-        Lb[(long long)r * ldi + c] = (c <= r) ? S[r * LF_LD + c] : 0.0;
-    }
-    LEAF_STAMP(14);
-}
-
-// ---------------------------------------------------------------------------------------
-// a3 leaf v3.  Same contract as v2; the 128-pivot dependency chain is the only thing left on
-// the critical path (a profile of v2 split its time between the warp-level 16x16 potrf+trtri,
-// the Dinv panel products, the block load and the serial inverse assembly):
-//   * per 16-column block step the chain is  potrf16 (warp 0, registers + shuffles, fp32-seeded
-//     rsqrt)  ->  panel by FORWARD SUBSTITUTION with the 16x16 factor (one
+//   Blocked (nb = 16) right-looking Cholesky + triangular inverse; the trailing updates and the
+//   inverse assembly run on DMMA fragments read straight from shared memory (row stride
+//   LF_LD = 132 doubles: (g*32 + t*8) mod 128 is conflict-free).  The 128-pivot dependency chain
+//   is the only thing on the critical path:
+//   * per 16-column block step the chain is  potrf16 (warp 0, registers + shuffles, two pivots
+//     per step)  ->  panel by FORWARD SUBSTITUTION with the 16x16 factor (one
 //     thread per row, the factor is broadcast from shared memory; no 16x16 inverse needed)  ->
 //     DMMA update of the next block column;
 //   * everything else runs beside it: warps 2..7 finish the trailing update of the previous step
 //     and warp 1 inverts the previous 16x16 diagonal block (needed only by the inverse assembly)
 //     while warp 0 factorises the next one;
 //   * the triangular inverse is assembled by recursive doubling with four independent DMMA
-//     accumulator chains per warp (v2 ran one dependent chain per 8x8 tile);
+//     accumulator chains per warp;
 //   * 16-byte global loads / stores.
 // ---------------------------------------------------------------------------------------
+#define LEAF_N 128
+#define LF_LD 132
+#define LF_NB 16
+// optional phase clock stamps of CTA 0 (diagnostics: gpmpc_profile_leaf)
+__device__ long long* d_leaf_prof = nullptr;
+#define LEAF_STAMP(k) do { if (d_leaf_prof && blockIdx.x == 0 && threadIdx.x == 0) d_leaf_prof[k] = clock64(); } while (0)
+
 __device__ __forceinline__ double rsqrt_seeded(double d)
 {
     // rsqrt.approx.f64 (SASS MUFU.RSQ64H on the high word, ~2^-22, no fp32 round trip) + two Newton steps in
@@ -596,40 +225,8 @@ __device__ __forceinline__ double rsqrt_seeded(double d)
 }
 
 // 16x16 Cholesky in registers (lane r and r+16 hold row r); writes the factor back (lower part) and
-// the reciprocal pivots to ipd[16]
-__device__ __forceinline__ void warp_potrf16(double* D, double* ipd, int* info, int info_val0, int lane)
-{
-    const unsigned full = 0xffffffffu;
-    const int r = lane & 15;
-    double a[16];
-#pragma unroll
-    for (int k = 0; k < 16; ++k) a[k] = D[r * LF_LD + k];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-        const double d = __shfl_sync(full, a[j], j);
-        if (!(d > 0.0) && lane == 0) atomicCAS(info, 0, info_val0 + j + 1);
-        double y = rsqrt_seeded(d);
-        double pv = d * y;
-        pv = fma(fma(-pv, pv, d), 0.5 * y, pv);             // sqrt(d) to ~0.5 ulp
-        if (!(d > 0.0)) { pv = sqrt(d); y = 1.0 / pv; }     // keep NaN/inf propagation of the plain formula
-        a[j] = (r == j) ? pv : a[j] * y;
-        if (lane == 0) ipd[j] = y;
-#pragma unroll
-        for (int k = j + 1; k < 16; ++k) {
-            const double lkj = __shfl_sync(full, a[j], k);
-            a[k] = fma(-a[j], lkj, a[k]);                  // meaningful for r >= k; upper part is never read
-        }
-    }
-    __syncwarp();                                           // lanes 16..31 read the same rows above (ordered by the shuffles; explicit for racecheck)
-    if (lane < 16) {
-#pragma unroll
-        for (int k = 0; k < 16; ++k) if (k <= r) D[r * LF_LD + k] = a[k];
-    }
-    __syncwarp();
-}
-
-// Same contract, TWO columns per step: the pivots' reciprocal square roots are the longest dependent chain
-// of the whole factorisation (about nine dependent fp64 operations per pivot).  For columns
+// the reciprocal pivots to ipd[16].  TWO columns per step: the pivots' reciprocal square roots are the
+// longest dependent chain of the whole factorisation (about nine dependent fp64 operations per pivot).  For columns
 // j, j+1 with Schur-complement entries p = S_jj, q = S_j+1,j, r = S_j+1,j+1 the second pivot is
 // s = r - q^2/p = det/p with det = p r - q^2, so  1/sqrt(s) = rsqrt(det) * sqrt(p):  rsqrt(p) and rsqrt(det)
 // are independent and run concurrently -- 11 dependent operations per two pivots instead of 18.  Arithmetic is
@@ -701,12 +298,11 @@ __device__ __forceinline__ void warp_trtri16(const double* D, const double* ipd,
     }
 }
 
-#define LF3_SMEM_DOUBLES (LEAF_N * LF_LD + 8 * 16 * 17 + 8 * 16 + 64 * 68 + 64)
-template <bool TWOCOL>
+#define LEAF_SMEM_DOUBLES (LEAF_N * LF_LD + 8 * 16 * 17 + 8 * 16 + 64 * 68 + 64)
 __global__ void __launch_bounds__(256, 1)
-leaf_potrf_trtri_v3_kernel(double* __restrict__ A, int lda, long long sA,
-                           double* __restrict__ Li, int ldi, long long sLi,
-                           int* __restrict__ info, int info_base)
+leaf_potrf_trtri_kernel(double* __restrict__ A, int lda, long long sA,
+                        double* __restrict__ Li, int ldi, long long sLi,
+                        int* __restrict__ info, int info_base)
 {
     extern __shared__ __align__(16) double S[];                // [128][132]
     double* DinvAll = S + LEAF_N * LF_LD;                      // [8][16][17]
@@ -764,10 +360,7 @@ leaf_potrf_trtri_v3_kernel(double* __restrict__ A, int lda, long long sA,
         for (int kk = 0; kk < 4; ++kk) dmma884(acc0, acc1, -pa[kk * 4], pb[kk * 4]);
         cp[0] = acc0; cp[1] = acc1;
     };
-    if (warp == 0) {
-        if (TWOCOL) warp_potrf16x2(S, ipdAll, info + blockIdx.x, info_base, lane);
-        else warp_potrf16(S, ipdAll, info + blockIdx.x, info_base, lane);
-    }
+    if (warp == 0) warp_potrf16x2(S, ipdAll, info + blockIdx.x, info_base, lane);
     __syncthreads();
     panel(0, ipdAll);
     __syncthreads();
@@ -782,8 +375,7 @@ leaf_potrf_trtri_v3_kernel(double* __restrict__ A, int lda, long long sA,
         }
         __syncthreads();
         if (warp == 0) {
-            if (TWOCOL) warp_potrf16x2(S + b0 * LF_LD + b0, ipdAll + (kb + 1) * 16, info + blockIdx.x, info_base + b0, lane);
-            else warp_potrf16(S + b0 * LF_LD + b0, ipdAll + (kb + 1) * 16, info + blockIdx.x, info_base + b0, lane);
+            warp_potrf16x2(S + b0 * LF_LD + b0, ipdAll + (kb + 1) * 16, info + blockIdx.x, info_base + b0, lane);
         } else if (warp == 1) {
             warp_trtri16(S + c0 * LF_LD + c0, ipdAll + kb * 16, DinvAll + kb * 16 * 17, lane);
         } else {
@@ -1056,7 +648,7 @@ logdet_dot_kernel(const double* __restrict__ L, int ld, long long sL,
 // reads 4 consecutive training points, a warp stores 8 rows x 32 B of KS^T per step.
 // grid (Npad/CH, BM/8, outputs); PMJ[a][h][blk][1 + Nx].
 // ---------------------------------------------------------------------------------------
-template <int NXP, int CH, int UNR>
+template <int NXP, int CH>
 __global__ void __launch_bounds__(256, (NXP <= 12 ? 2 : 1))
 ks_tile_kernel(const double* __restrict__ XT, int ldx, int N, int Nx,
                const double* __restrict__ hyp, int hyp_ld,
@@ -1120,7 +712,7 @@ ks_tile_kernel(const double* __restrict__ XT, int ldx, int N, int Nx,
     __syncthreads();
     double* krow = KST + (long long)a * sK + (long long)h * ldk + i0;
     if (active) {
-#pragma unroll UNR
+#pragma unroll 2
         for (int il = s; il < CH; il += 32) {
             double df[NXP], d0 = 0.0, d1 = 0.0;
 #pragma unroll
@@ -1474,7 +1066,6 @@ em_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
             const int j = j0 + tx + 16 * c;
-            const double lq = (i < N && j < N) ? E[(long long)p * ldn + i] + F[(long long)p * ldn + j] + 2.0 * acc[r][c] : 0.0;
             // mode 1 stores only the part of Q beyond its rank-one backbone: Q_ij = e^{E_i} e^{F_j} (1 + expm1(2 acc_ij));
             // the backbone's trace term |L^-1 e^E|^2 is formed like the ME variance (em_qvec_kernel + trmv), which keeps
             // EM -> ME exact to ~1e-11 as Sigma -> 0 instead of amplifying the full Q through L^-1 twice
@@ -1559,15 +1150,12 @@ __global__ void em_finalize_kernel(int Nx, int Ny, int npairs, const double* __r
                                    const double* __restrict__ trPart, int ntr, const double* __restrict__ trVec,
                                    double* __restrict__ mean, double* __restrict__ var, double* __restrict__ cov)
 {
-    __shared__ double mu[64];
     const int tid = threadIdx.x, nn = Nx * Nx;
-    if (tid < Ny) {
+    if (tid < Ny && mean) {
         double s = 0.0;
         for (int b = 0; b < nblk; ++b) s += meanPart[(long long)tid * nblk + b];
-        mu[tid] = s;
-        if (mean) mean[tid] = s;
+        mean[tid] = s;
     }
-    __syncthreads();
     if (tid < npairs) {
         const double* P = EMP + (long long)Ny * (2 * nn + 2) + (long long)tid * (nn + 4);
         const int a = (int)P[nn + 1], b = (int)P[nn + 2];

@@ -186,7 +186,8 @@ int gpmpc_get(gpmpc_handle_t h, int what, int a, double* dst);
 /* Engine options: "refine" (0/1: one step of iterative refinement of v = L\ks through
  * the stored factor), "predict_ctas" (persistent grid of the stream-K predict product,
  * 0 = two CTAs per SM), "peer" (0/1), "peer_timeout_s" (consumer wait for a peer's flag),
- * "overlap", "gemm_variant", "leaf_variant", "small_tiles" (factorisation A/B switches). */
+ * "small_tiles" (batched 128x64 tile count of a factorisation GEMM below which it runs on
+ * 64x32 tiles; default 4 per SM).  Any other name returns GPMPC_ERR_ARG. */
 int gpmpc_set_option(gpmpc_handle_t h, const char* name, double value);
 
 /* Multi-GPU: one process per GPU.  Rank 0 calls gpmpc_comm_unique_id and ships the

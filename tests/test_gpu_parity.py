@@ -754,8 +754,9 @@ def test_argument_errors_fail_loudly():
     eng.factorize()
     with pytest.raises(L.GpmpcError):
         eng.get(L.GET_CHOL, 3)                                   # output not owned
-    with pytest.raises(L.GpmpcError):
-        eng.set_option('no_such_option', 1)
+    for name in ('no_such_option', 'gemm_variant', 'leaf_variant', 'overlap', 'lookahead', 'lookahead_min', 'zero_copy'):
+        with pytest.raises(L.GpmpcError):
+            eng.set_option(name, 1)
     with pytest.raises(L.GpmpcError):
         eng.predict(np.zeros((2, 2)), None, L.METHOD_EM, want_jac=False)     # EM needs Sigma
     eng.close()
