@@ -4,8 +4,26 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <atomic>
+
 #define GPMPC_TILE 128          // all internal matrices are padded to a multiple of this
 #define GPMPC_MAX_DEVICES 64
+
+// Lets kernel Kern use `bytes` of dynamic shared memory (a launch above 48 KB needs it).  The attribute is per device, so
+// it is set once per device; setting it twice is harmless.  Devices past GPMPC_MAX_DEVICES set it at every call.
+template <auto Kern>
+static cudaError_t smem_opt_in(int bytes)
+{
+    static std::atomic<bool> done[GPMPC_MAX_DEVICES];
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    const bool cached = dev >= 0 && dev < GPMPC_MAX_DEVICES;
+    if (cached && done[dev].load(std::memory_order_acquire)) return cudaSuccess;
+    e = cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess && cached) done[dev].store(true, std::memory_order_release);
+    return e;
+}
 
 #define CUDA_TRY(expr)                                                        \
     do {                                                                      \

@@ -12,7 +12,6 @@
 // All dimensions are multiples of the tile sizes (every matrix in the engine is padded
 // to GPMPC_TILE with an identity tail), so there is no bounds handling anywhere.
 #pragma once
-#include <atomic>
 #include "common.cuh"
 
 enum : int {
@@ -186,14 +185,8 @@ static cudaError_t gemm_launch(const GemmParams& p, int batch, cudaStream_t st)
     using SM = GemmSmem<BM, BN, BT, STAGES>;
     auto kern = gemm_dmma_kernel<BM, BN, WM, WN, BT, STAGES, MINB>;
     constexpr int BYTES = SM::BYTES;
-    static std::atomic<bool> configured[GPMPC_MAX_DEVICES];    // the attribute is per device; set-attribute is idempotent
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < GPMPC_MAX_DEVICES && !configured[dev].load(std::memory_order_acquire)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BYTES);
-        if (e != cudaSuccess) return e;
-        configured[dev].store(true, std::memory_order_release);
-    }
+    const cudaError_t e = smem_opt_in<gemm_dmma_kernel<BM, BN, WM, WN, BT, STAGES, MINB>>(BYTES);
+    if (e != cudaSuccess) return e;
     constexpr int R = (BM >= BN) ? BM / BN : 1;
     const int tiles = p.lower ? R * p.mt * (p.mt + 1) / 2 : p.mt * p.nt;
     kern<<<dim3(tiles, 1, batch), WM * WN * 32, BYTES, st>>>(p);
@@ -388,14 +381,8 @@ static cudaError_t gemm_tmap_launch(const GemmParams& p, int batch, cudaStream_t
 {
     auto kern = gemm_dmma_tmap_kernel<BM, BN, WM, WN, STAGES, MINB>;
     constexpr int BYTES = STAGES * (BM + BN) * GEMM_BK * 8 + STAGES * 8 + 1024;
-    static std::atomic<bool> configured[GPMPC_MAX_DEVICES];    // the attribute is per device; set-attribute is idempotent
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < GPMPC_MAX_DEVICES && !configured[dev].load(std::memory_order_acquire)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BYTES);
-        if (e != cudaSuccess) return e;
-        configured[dev].store(true, std::memory_order_release);
-    }
+    const cudaError_t e = smem_opt_in<gemm_dmma_tmap_kernel<BM, BN, WM, WN, STAGES, MINB>>(BYTES);
+    if (e != cudaSuccess) return e;
     CUtensorMap tmA, tmB;
     if (!tmap_make(&tmA, p.A, p.K, p.mt * BM, p.lda, p.sA, batch, BM)) return cudaErrorInvalidValue;
     if (!tmap_make(&tmB, p.B, p.K, p.nt * BN, p.ldb, p.sB, batch, BN)) return cudaErrorInvalidValue;

@@ -9,7 +9,7 @@
 #include <string.h>
 
 #include <algorithm>
-#include <atomic>
+#include <type_traits>
 #include <vector>
 
 #include <nvtx3/nvToolsExt.h>
@@ -65,6 +65,20 @@ static bool nccl_load(char* err, size_t errn)
 }
 
 // ------------------------------------------------------------------------------------
+// One device allocation of `cap` elements, freed with its owner.  It converts to its pointer, so kernels and copies take
+// it as they take a raw pointer.
+template <typename T>
+struct DevBuf {
+    T* p = nullptr;
+    size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { cudaFree(p); }
+    operator T*() const { return p; }
+    int ensure(gpmpc_handle_t h, long long count, const char* name);
+};
+
 struct gpmpc_handle_s {
     int N = 0, Nx = 0, Ny = 0, a0 = 0, nloc = 0, Npad = 0, device = 0;
     int nloc_max = 0;                 // ceil(Ny / world): slots per rank in the gather buffer
@@ -74,31 +88,31 @@ struct gpmpc_handle_s {
     cudaStream_t sideSt[MAX_DEPTH] = {nullptr}; cudaEvent_t evA[MAX_DEPTH] = {nullptr}, evB[MAX_DEPTH] = {nullptr}, evT[MAX_DEPTH] = {nullptr}, evS[MAX_DEPTH] = {nullptr};
     long long w2off[MAX_DEPTH + 1] = {0};
     // model
-    double *dXT = nullptr, *dMu = nullptr, *dY = nullptr, *dHyp = nullptr, *dJit = nullptr, *dHypTmp = nullptr;
-    double *dL = nullptr, *dLi = nullptr, *dW1 = nullptr, *dW2 = nullptr;
-    double *dAlpha = nullptr, *dTmp = nullptr, *dRes = nullptr;
-    int* dInfo = nullptr;
+    DevBuf<double> dXT, dMu, dY, dHyp, dJit, dHypTmp;
+    DevBuf<double> dL, dLi, dW1, dW2;
+    DevBuf<double> dAlpha, dTmp, dRes;
+    DevBuf<int> dInfo;
     // predict
-    double *dKST = nullptr, *dPart = nullptr, *dPMJ = nullptr, *dSQ = nullptr, *dV = nullptr, *dR = nullptr, *dR2 = nullptr;
-    unsigned int* dCnt = nullptr;     // stream-K counters: [nloc*nt tile | nloc output | 1 done], self-cleaning
-    int psk_ctas = 0, opt_predict_ctas = 0, partCtas = 0;   // persistent grid of the predict product (2 CTAs per SM)
-    double *dCovV = nullptr, *dCovOut = nullptr; long long covVcap = 0, covOutcap = 0;   // GP.covar scratch pool
+    DevBuf<double> dKST, dPart, dPMJ, dSQ, dV, dR, dR2;
+    DevBuf<unsigned int> dCnt;        // stream-K counters: [nloc*nt tile | nloc output | 1 done], self-cleaning
+    int psk_ctas = 0, opt_predict_ctas = 0;   // persistent grid of the predict product (2 CTAs per SM)
+    DevBuf<double> dCovV, dCovOut;    // GP.covar scratch pool
     // predict_grad: U = Linv^T per output (lazy), beta rows, partial sums, per-batch derivative slabs
-    double *dUall = nullptr, *dBeta = nullptr, *dPDV = nullptr, *dPH = nullptr, *dGradOut = nullptr; bool u_valid = false; int gradHcap = 0;
+    DevBuf<double> dUall, dBeta, dPDV, dPH, dGradOut; bool u_valid = false;
     // predict_hess: derivative rows d ks / dz and their L^-1 products (lazy), block partials, per-batch second-derivative slabs
-    double *dDR = nullptr, *dVD = nullptr, *dPG = nullptr, *dPB2 = nullptr, *dPM3 = nullptr, *dHessOut = nullptr; int hessHcap = 0;
-    double *dG = nullptr, *dZ = nullptr, *dSigma = nullptr, *dMean = nullptr, *dVar = nullptr, *dJ = nullptr, *dCov = nullptr;
-    double* dRoll = nullptr; size_t rollCap = 0;   // gpmpc_rollout: [Z | Sigma | U | scale | means | vars | cov]
-    double *dIn = nullptr, *dOut = nullptr;   // [Z | Sigma] and [mean | var | J | cov] slabs: one H2D + one D2H per host call
-    int Hcap = 0;
+    DevBuf<double> dDR, dVD, dPG, dPB2, dPM3, dHessOut;
+    DevBuf<double> dG;
+    double *dZ = nullptr, *dSigma = nullptr, *dMean = nullptr, *dVar = nullptr, *dJ = nullptr, *dCov = nullptr;   // in dIn / dOut
+    DevBuf<double> dRoll;             // gpmpc_rollout: [Z | Sigma | U | scale | means | vars | cov]
+    DevBuf<double> dIn, dOut;         // [Z | Sigma] and [mean | var | J | cov] slabs: one H2D + one D2H per host call
+    int Hcap = 0;                     // test points the slab layout behind dZ .. dCov holds (0: not laid out)
     double* hPinned = nullptr; double* dPinnedAlias = nullptr; size_t hPinnedBytes = 0;
     // nlml scratch
-    double *dU = nullptr, *dKinv = nullptr, *dGradPart = nullptr, *dGrad = nullptr;
+    DevBuf<double> dU, dKinv, dGradPart, dGrad;
     bool has_data = false, has_hyper = false, factorized = false;
     // EM scratch
-    double *dEmTr = nullptr, *dEMP = nullptr, *dEmE = nullptr, *dEmF = nullptr, *dEmW = nullptr, *dEmIJ = nullptr;
-    double *dEmMeanPart = nullptr, *dEmPart = nullptr, *dEmLQ = nullptr, *dEmVec = nullptr, *dEmE2 = nullptr, *dEmF2 = nullptr;
-    int emHcap = 0;
+    DevBuf<double> dEmTr, dEMP, dEmE, dEmF, dEmW, dEmIJ;
+    DevBuf<double> dEmMeanPart, dEmPart, dEmLQ, dEmVec, dEmE2, dEmF2;
     std::vector<double> hyper;        // (nloc, Nx+2)
     std::vector<double> logdet, yalpha;
     std::vector<int> jitter_used;
@@ -107,7 +121,7 @@ struct gpmpc_handle_s {
     // comm
     nccl_comm_t comm = nullptr; int rank = 0, world = 1;
     // peer (CUDA IPC) exchange: [flags: 2*MAXW u64][gather buffer parity 0][parity 1]
-    double* dPeerBlock = nullptr; long long peerGsz = 0; int peerHcap = 0; bool peer_ready = false;
+    DevBuf<double> dPeerBlock; long long peerGsz = 0; int peerHcap = 0; bool peer_ready = false;
     double* peerBase[GPMPC_MAXW] = {nullptr}; bool peerOpened[GPMPC_MAXW] = {false};
     int* dPeerStatus = nullptr; int* hPeerStatus = nullptr;
     unsigned long long peer_step = 0; int opt_peer = 1; double opt_peer_timeout_s = 60.0; int clock_khz = 1980000;
@@ -121,6 +135,39 @@ static void set_error(gpmpc_handle_t h, const char* fmt, ...)
     va_end(ap);
 }
 
+// Grow to at least `count` elements, zero-filled on the handle's stream (the stream-K counters, the zero upper tiles of
+// Li and the zero rows of dDR rely on it).  The old buffer is freed only once the stream has drained.  On failure the
+// buffer is left empty and the error names it.
+template <typename T>
+int DevBuf<T>::ensure(gpmpc_handle_t h, long long count, const char* name)
+{
+    if ((size_t)count <= cap) return GPMPC_OK;
+    if (p) {
+        CUDA_TRY(cudaStreamSynchronize(h->st));
+        cudaFree(p);
+        p = nullptr; cap = 0;
+    }
+    const size_t bytes = (size_t)count * sizeof(T);
+    cudaError_t e = cudaMalloc((void**)&p, bytes);
+    if (e != cudaSuccess) {
+        p = nullptr;
+        set_error(h, "cudaMalloc(%s, %zu bytes) failed: %s", name, bytes, cudaGetErrorString(e));
+        return GPMPC_ERR_CUDA;
+    }
+    e = cudaMemsetAsync(p, 0, bytes, h->st);
+    if (e != cudaSuccess) { cudaFree(p); p = nullptr; }
+    CUDA_TRY(e);
+    cap = (size_t)count;
+    return GPMPC_OK;
+}
+
+// buf.ensure(count), returning its error code; the message names the buffer as written at the call
+#define ENSURE(buf, count)                                          \
+    do {                                                            \
+        const int _rc = (buf).ensure(h, (long long)(count), #buf);  \
+        if (_rc) return _rc;                                        \
+    } while (0)
+
 // NVTX range per phase (header-only nvtx3: a no-op unless a profiler injects the library)
 struct NvtxRange {
     explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
@@ -129,6 +176,16 @@ struct NvtxRange {
 
 static inline long long slab(gpmpc_handle_t h) { return (long long)h->Npad * h->Npad; }
 static inline long long w2slab(gpmpc_handle_t h) { return h->w2off[MAX_DEPTH]; }   // all depths, one batch entry
+
+// f(std::integral_constant<int, NXP>) with NXP = 8, 16 or 32 >= Nx: the register-array extent of the kernels that keep
+// one Nx-vector per thread (nlml gradient, EM, predict derivatives)
+template <typename F>
+static cudaError_t nxp_dispatch(int Nx, F&& f)
+{
+    if (Nx <= 8) return f(std::integral_constant<int, 8>());
+    if (Nx <= 16) return f(std::integral_constant<int, 16>());
+    return f(std::integral_constant<int, 32>());
+}
 
 // ------------------------------------------------------------------------------------
 // GEMM helpers (all operands live in slabs with leading dimension ld)
@@ -167,11 +224,7 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
     const int ld = h->Npad;
     if (n <= LEAF_N) {
         if (pend) CUDA_TRY(cudaStreamWaitEvent(h->st, pend, 0));
-        static std::atomic<bool> conf[GPMPC_MAX_DEVICES];
-        if (!conf[h->device % GPMPC_MAX_DEVICES].load(std::memory_order_acquire)) {
-            CUDA_TRY(cudaFuncSetAttribute(leaf_potrf_trtri_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LEAF_SMEM_DOUBLES * 8));
-            conf[h->device % GPMPC_MAX_DEVICES].store(true, std::memory_order_release);
-        }
+        CUDA_TRY(smem_opt_in<leaf_potrf_trtri_kernel>(LEAF_SMEM_DOUBLES * 8));
         leaf_potrf_trtri_kernel<<<batch, 256, LEAF_SMEM_DOUBLES * 8, h->st>>>(A + (long long)off * ld + off, ld, sA,
                                                                            Li + (long long)off * ld + off, ld, sLi, dInfo, off);
         CUDA_TRY(cudaGetLastError());
@@ -275,16 +328,11 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
 // output slabs at K (stride slab).  full = 1 writes the whole square, 0 the lower triangle.
 static int launch_kbuild(gpmpc_handle_t h, const double* dHyp, const double* dJit, double* K, int batch, int full)
 {
-    static std::atomic<bool> conf[GPMPC_MAX_DEVICES];
     const int KD = (h->Nx + 3) & ~3, S = ((KD >> 2) & 1) ? KD : KD + 4;
     const int smem = (2 * KB2_TILE * S + 2 * KB2_TILE + 256) * 8;
-    if (!conf[h->device % GPMPC_MAX_DEVICES].load(std::memory_order_acquire)) {
-        CUDA_TRY(cudaFuncSetAttribute(kbuild_dmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (2 * KB2_TILE * 36 + 2 * KB2_TILE + 256) * 8));
-        CUDA_TRY(cudaFuncSetAttribute(kbuild_dmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (2 * KB2_TILE * 36 + 2 * KB2_TILE + 256) * 8));
-        conf[h->device % GPMPC_MAX_DEVICES].store(true, std::memory_order_release);
-    }
+    const int smem_max = (2 * KB2_TILE * 36 + 2 * KB2_TILE + 256) * 8;   // S at NX_MAX
+    CUDA_TRY(smem_opt_in<kbuild_dmma_kernel<true>>(smem_max));
+    CUDA_TRY(smem_opt_in<kbuild_dmma_kernel<false>>(smem_max));
     const int T = h->Npad / KB2_TILE;
     dim3 grid(T * (T + 1) / 2, 1, batch);
     if (full)
@@ -348,17 +396,6 @@ extern "C" int gpmpc_version(void) { return GPMPC_VERSION; }
 
 extern "C" const char* gpmpc_last_error(gpmpc_handle_t h) { return h ? h->err : g_create_err; }
 
-#define ALLOC(ptr, count)                                                               \
-    do {                                                                                \
-        cudaError_t _e = cudaMalloc((void**)&(ptr), (size_t)(count) * sizeof(*(ptr)));  \
-        if (_e != cudaSuccess) {                                                        \
-            set_error(h, "cudaMalloc(%s, %zu bytes) failed: %s", #ptr,                  \
-                      (size_t)(count) * sizeof(*(ptr)), cudaGetErrorString(_e));        \
-            return GPMPC_ERR_CUDA;                                                      \
-        }                                                                               \
-        cudaMemsetAsync((ptr), 0, (size_t)(count) * sizeof(*(ptr)), h->st);             \
-    } while (0)
-
 extern "C" int gpmpc_destroy(gpmpc_handle_t h);
 
 static int create_fill(gpmpc_handle_t h, int N, int Nx, int Ny, int out_begin, int out_count, int device)
@@ -369,6 +406,8 @@ static int create_fill(gpmpc_handle_t h, int N, int Nx, int Ny, int out_begin, i
     CUDA_TRY(cudaSetDevice(device));
     CUDA_TRY(cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, device));
     h->opt_small_tiles = 4 * h->sms;      // two waves of 2 CTAs per SM
+    h->psk_ctas = 2 * h->sms;
+    cudaDeviceGetAttribute(&h->clock_khz, cudaDevAttrClockRate, device);
     {
         int lo = 0, hi = 0;
         cudaDeviceGetStreamPriorityRange(&lo, &hi);
@@ -377,14 +416,14 @@ static int create_fill(gpmpc_handle_t h, int N, int Nx, int Ny, int out_begin, i
     CUDA_TRY(cudaEventCreate(&h->ev0));
     CUDA_TRY(cudaEventCreate(&h->ev1));
     const long long np = h->Npad;
-    ALLOC(h->dXT, (long long)Nx * np);
-    ALLOC(h->dMu, NX_MAX);
-    ALLOC(h->dY, (long long)out_count * np);
-    ALLOC(h->dHyp, (long long)out_count * (Nx + 2));
-    ALLOC(h->dHypTmp, Nx + 2);
-    ALLOC(h->dJit, out_count);
-    ALLOC(h->dL, out_count * slab(h));
-    ALLOC(h->dLi, out_count * slab(h));
+    ENSURE(h->dXT, (long long)Nx * np);
+    ENSURE(h->dMu, NX_MAX);
+    ENSURE(h->dY, (long long)out_count * np);
+    ENSURE(h->dHyp, (long long)out_count * (Nx + 2));
+    ENSURE(h->dHypTmp, Nx + 2);
+    ENSURE(h->dJit, out_count);
+    ENSURE(h->dL, out_count * slab(h));
+    ENSURE(h->dLi, out_count * slab(h));
     {   // W2 workspace: one region per recursion depth (n_d = ceil(nb / 2^d) * 128 rows at depth d)
         const int nb = h->Npad / 128;
         long long off = 0;
@@ -404,13 +443,13 @@ static int create_fill(gpmpc_handle_t h, int N, int Nx, int Ny, int out_begin, i
             CUDA_TRY(cudaEventCreateWithFlags(&h->evS[d], cudaEventDisableTiming));
         }
     }
-    ALLOC(h->dW1, out_count * w2slab(h));      // same per-depth layout as W2
-    ALLOC(h->dW2, out_count * w2slab(h));
-    ALLOC(h->dAlpha, (long long)out_count * np);
-    ALLOC(h->dTmp, (long long)out_count * np);
-    ALLOC(h->dRes, 2 * out_count);
-    ALLOC(h->dInfo, out_count);
-    ALLOC(h->dGrad, Nx + 2);
+    ENSURE(h->dW1, out_count * w2slab(h));      // same per-depth layout as W2
+    ENSURE(h->dW2, out_count * w2slab(h));
+    ENSURE(h->dAlpha, (long long)out_count * np);
+    ENSURE(h->dTmp, (long long)out_count * np);
+    ENSURE(h->dRes, 2 * out_count);
+    ENSURE(h->dInfo, out_count);
+    ENSURE(h->dGrad, Nx + 2);
     h->hyper.assign((size_t)out_count * (Nx + 2), 0.0);
     h->logdet.assign(out_count, 0.0); h->yalpha.assign(out_count, 0.0); h->jitter_used.assign(out_count, 0);
     CUDA_TRY(cudaStreamSynchronize(h->st));
@@ -459,14 +498,7 @@ extern "C" int gpmpc_destroy(gpmpc_handle_t h)
     if (h->st) cudaStreamSynchronize(h->st);
     if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
     for (int r = 0; r < GPMPC_MAXW; ++r) if (h->peerOpened[r]) cudaIpcCloseMemHandle(h->peerBase[r]);
-    if (h->dPeerBlock) cudaFree(h->dPeerBlock);
-    if (h->dCnt) cudaFree(h->dCnt);
     if (h->hPeerStatus) cudaFreeHost(h->hPeerStatus);
-    double* bufs[] = {h->dXT, h->dMu, h->dY, h->dHyp, h->dHypTmp, h->dJit, h->dL, h->dLi, h->dW1, h->dW2, h->dAlpha, h->dTmp,
-                      h->dRes, h->dKST, h->dPart, h->dPMJ, h->dSQ, h->dV, h->dR, h->dR2, h->dCovV, h->dCovOut, h->dUall, h->dBeta, h->dPDV, h->dPH, h->dGradOut, h->dDR, h->dVD, h->dPG, h->dPB2, h->dPM3, h->dHessOut, h->dG, h->dRoll, h->dIn, h->dOut, h->dU, h->dKinv, h->dGradPart, h->dGrad,
-                      h->dEmTr, h->dEmLQ, h->dEmVec, h->dEmE2, h->dEmF2, h->dEMP, h->dEmE, h->dEmF, h->dEmW, h->dEmIJ, h->dEmMeanPart, h->dEmPart};
-    for (double* b : bufs) if (b) cudaFree(b);
-    if (h->dInfo) cudaFree(h->dInfo);
     if (h->hPinned) cudaFreeHost(h->hPinned);
     for (int d = 0; d < MAX_DEPTH; ++d) {
         if (h->sideSt[d]) { cudaStreamSynchronize(h->sideSt[d]); cudaStreamDestroy(h->sideSt[d]); }
@@ -478,7 +510,7 @@ extern "C" int gpmpc_destroy(gpmpc_handle_t h)
     if (h->ev0) cudaEventDestroy(h->ev0);
     if (h->ev1) cudaEventDestroy(h->ev1);
     if (h->st) cudaStreamDestroy(h->st);
-    delete h;
+    delete h;                        // frees the device buffers
     return GPMPC_OK;
 }
 
@@ -560,19 +592,17 @@ static int local_index(gpmpc_handle_t h, int a)
 
 static int ensure_nlml_scratch(gpmpc_handle_t h)
 {
-    if (!h->dU) { ALLOC(h->dU, slab(h)); }
-    if (!h->dKinv) { ALLOC(h->dKinv, slab(h)); }
-    if (!h->dGradPart) {
-        const int T = h->Npad / KB_TILE;
-        ALLOC(h->dGradPart, (long long)T * (T + 1) / 2 * (h->Nx + 2));
-    }
+    const int T = h->Npad / KB_TILE;
+    ENSURE(h->dU, slab(h));
+    ENSURE(h->dKinv, slab(h));
+    ENSURE(h->dGradPart, (long long)T * (T + 1) / 2 * (h->Nx + 2));
     return GPMPC_OK;
 }
 
 static int extract_to_host(gpmpc_handle_t h, const double* src, double* dst, int mode)
 {
     const int N = h->N;
-    if (!h->dKinv) { int rc = ensure_nlml_scratch(h); if (rc) return rc; }
+    { int rc = ensure_nlml_scratch(h); if (rc) return rc; }
     // stage through dU (N*N fits: Npad >= N)
     dim3 g((N + 127) / 128, N);
     extract_kernel<<<g, 128, 0, h->st>>>(src, h->Npad, h->dU, N, mode);
@@ -689,9 +719,7 @@ extern "C" int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* 
     if (grad) {
         rc = compute_kinv(h, al);
         if (rc) return rc;
-        cudaError_t e = (h->Nx <= 8) ? launch_grad<8>(h, al, h->dHypTmp)
-                      : (h->Nx <= 16) ? launch_grad<16>(h, al, h->dHypTmp) : launch_grad<32>(h, al, h->dHypTmp);
-        CUDA_TRY(e);
+        CUDA_TRY(nxp_dispatch(h->Nx, [&](auto nxp) { return launch_grad<decltype(nxp)::value>(h, al, h->dHypTmp); }));
         const int T = h->Npad / KB_TILE;
         nlml_grad_final_kernel<<<m, 256, 0, h->st>>>(h->dGradPart, T * (T + 1) / 2, h->Nx, h->dHypTmp, h->dGrad);
         CUDA_TRY(cudaGetLastError());
@@ -752,47 +780,51 @@ extern "C" int gpmpc_set_option(gpmpc_handle_t h, const char* name, double value
 // ------------------------------------------------------------------------------------
 // predict
 // ------------------------------------------------------------------------------------
-static inline int ks_chunk(gpmpc_handle_t h);
+// training points per CTA of the ks kernel (ks_tile_kernel): 128-point chunks below N = 8192 so small problems still fill
+// the machine; 512 at large N (few partial blocks for the record sums); 1024 when a rank also holds several outputs --
+// the per-CTA prologue / epilogue (a large share of a CTA's time at 512) is then amortised over twice the evaluations, and the
+// 16 chunks x 7 row groups x outputs still cover the SMs.  (Nx <= 12: the chunk of X^T must leave room for 2 CTAs per SM.)
+static inline int ks_chunk(gpmpc_handle_t h)
+{
+    if (h->Npad < 8192) return 128;
+    return (h->nloc >= 2 && h->Nx <= 12) ? 1024 : 512;
+}
+
+// blocks of the ks kernel along the training points (one partial record each)
+static inline int ks_blocks(gpmpc_handle_t h) { return (h->Npad + ks_chunk(h) - 1) / ks_chunk(h); }
+
+// the solved rows v (and r, for refinement and append) of one 64-point chunk, every output
+static int ensure_rows(gpmpc_handle_t h)
+{
+    ENSURE(h->dV, (long long)h->nloc * HB * h->Npad);
+    ENSURE(h->dR, (long long)h->nloc * HB * h->Npad);
+    return GPMPC_OK;
+}
 
 static int ensure_predict_bufs(gpmpc_handle_t h, int H)
 {
-    const long long np = h->Npad;
-    if (!h->dKST) {
-        cudaDeviceGetAttribute(&h->clock_khz, cudaDevAttrClockRate, h->device);
-        h->psk_ctas = 2 * h->sms;
-        const long long nt = np / 128;
-        ALLOC(h->dKST, (long long)h->nloc * HB * np);
-        ALLOC(h->dPMJ, (long long)h->nloc * HB * ((np + ks_chunk(h) - 1) / ks_chunk(h)) * (h->Nx + 1));
-        ALLOC(h->dSQ, (long long)h->nloc * HB * nt);
-        ALLOC(h->dCnt, (long long)h->nloc * nt + h->nloc + 1);
-    }
-    {   // parked stream-K partials: two BM x 128 slots per persistent CTA
-        const int want = std::max(h->psk_ctas, h->opt_predict_ctas);
-        if (want > h->partCtas) {
-            CUDA_TRY(cudaStreamSynchronize(h->st));
-            if (h->dPart) cudaFree(h->dPart);
-            h->dPart = nullptr; h->partCtas = 0;
-            ALLOC(h->dPart, (long long)want * 2 * HB * PSK_BN);
-            h->partCtas = want;
-        }
-    }
-    if (h->opt_refine && !h->dR2) {
-        if (!h->dV) { ALLOC(h->dV, (long long)h->nloc * HB * np); ALLOC(h->dR, (long long)h->nloc * HB * np); }
-        ALLOC(h->dR2, (long long)h->nloc * HB * np);
+    const long long np = h->Npad, nt = np / 128;
+    ENSURE(h->dKST, (long long)h->nloc * HB * np);
+    ENSURE(h->dPMJ, (long long)h->nloc * HB * ks_blocks(h) * (h->Nx + 1));
+    ENSURE(h->dSQ, (long long)h->nloc * HB * nt);
+    ENSURE(h->dCnt, (long long)h->nloc * nt + h->nloc + 1);
+    // parked stream-K partials: two BM x 128 slots per persistent CTA
+    ENSURE(h->dPart, (long long)std::max(h->psk_ctas, h->opt_predict_ctas) * 2 * HB * PSK_BN);
+    if (h->opt_refine) {
+        int rc = ensure_rows(h);
+        if (rc) return rc;
+        ENSURE(h->dR2, (long long)h->nloc * HB * np);
     }
     if (H > h->Hcap) {
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-        double* bufs[] = {h->dG, h->dIn, h->dOut};
-        for (double* b : bufs) if (b) cudaFree(b);
-        h->dG = h->dIn = h->dOut = nullptr;
+        // dZ .. dCov point into dIn / dOut: they are laid out again once both hold the new capacity
+        h->Hcap = 0;
+        h->dZ = h->dSigma = h->dMean = h->dVar = h->dJ = h->dCov = nullptr;
         const long long cap = std::max(H, HB);
         const int nyp = h->nloc_max * h->world;
         const long long Nx = h->Nx, Ny = h->Ny;
-        ALLOC(h->dG, (long long)nyp * cap * (Nx + 2));
-        ALLOC(h->dIn, cap * Nx + cap * Nx * Nx);
-        ALLOC(h->dOut, cap * (2 * Ny + Ny * Nx + Ny * Ny));
-        // defined contents for the profiling selectors when every call so far went through the zero-copy path
-        CUDA_TRY(cudaMemsetAsync(h->dIn, 0, (size_t)(cap * Nx + cap * Nx * Nx) * 8, h->st));
+        ENSURE(h->dG, (long long)nyp * cap * (Nx + 2));
+        ENSURE(h->dIn, cap * Nx + cap * Nx * Nx);
+        ENSURE(h->dOut, cap * (2 * Ny + Ny * Nx + Ny * Ny));
         h->dZ = h->dIn; h->dSigma = h->dIn + cap * Nx;
         h->dMean = h->dOut; h->dVar = h->dOut + cap * Ny; h->dJ = h->dOut + 2 * cap * Ny;
         h->dCov = h->dOut + 2 * cap * Ny + cap * Ny * Nx;
@@ -806,16 +838,9 @@ template <int BM>
 static cudaError_t psk_launch_bm(const PredictParams& p, const double* A, long long sA, const double* B, long long sB,
                                  int np, int grid, cudaStream_t st)
 {
-    auto kern = predict_streamk_kernel<BM>;
     constexpr int BYTES = PSK_STAGES * (BM + PSK_BN) * GEMM_BK * 8 + 2 * PSK_STAGES * 8 + 1024;
-    static std::atomic<bool> configured[GPMPC_MAX_DEVICES];
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < GPMPC_MAX_DEVICES && !configured[dev].load(std::memory_order_acquire)) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, BYTES);
-        if (e != cudaSuccess) return e;
-        configured[dev].store(true, std::memory_order_release);
-    }
+    const cudaError_t e = smem_opt_in<predict_streamk_kernel<BM>>(BYTES);
+    if (e != cudaSuccess) return e;
     CUtensorMap tmA, tmB;
     if (!tmap_make(&tmA, A, np, BM, np, sA, p.nloc, BM)) return cudaErrorInvalidValue;
     if (!tmap_make(&tmB, B, np, np, np, sB, p.nloc, PSK_BN)) return cudaErrorInvalidValue;
@@ -827,7 +852,7 @@ static cudaError_t psk_launch_bm(const PredictParams& p, const double* A, long l
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kern, p, tmA, tmB);
+    return cudaLaunchKernelEx(&cfg, predict_streamk_kernel<BM>, p, tmA, tmB);
 }
 
 static cudaError_t psk_launch(int bm, const PredictParams& p, const double* A, long long sA, const double* B, long long sB,
@@ -867,30 +892,38 @@ static void psk_base(gpmpc_handle_t h, PredictParams& p, int Hc)
     p.hyp = h->dHyp; p.hyp_ld = h->Nx + 2; p.Nx = h->Nx;
 }
 
-// training points per CTA of the ks kernel (ks_tile_kernel): 128-point chunks below N = 8192 so small problems still fill
-// the machine; 512 at large N (few partial blocks for the record sums); 1024 when a rank also holds several outputs --
-// the per-CTA prologue / epilogue (a large share of a CTA's time at 512) is then amortised over twice the evaluations, and the
-// 16 chunks x 7 row groups x outputs still cover the SMs.  (Nx <= 12: the chunk of X^T must leave room for 2 CTAs per SM.)
-static inline int ks_chunk(gpmpc_handle_t h)
+// after psk_base: the product also finalises chunk [h0, h0 + Hc) of an H-point step (records from the ks partials into dG)
+static void psk_finalize(gpmpc_handle_t h, PredictParams& p, int H, int h0)
 {
-    if (h->Npad < 8192) return 128;
-    return (h->nloc >= 2 && h->Nx <= 12) ? 1024 : 512;
+    p.finalize = 1; p.PMJ = h->dPMJ; p.nblk_mj = ks_blocks(h);
+    p.Gloc = h->dG; p.slot0 = h->a0; p.Htot = H; p.h0 = h0;
+}
+
+// assembly of a single-rank step of H points (predict_core adds the multi-rank fields).  stage_g: the gather records fit
+// next to J Sigma in the product kernel's stage buffers (PSK_STAGES (bm + 128) 16 doubles), read by the fused assembly only
+static AssembleArgs assemble_args(gpmpc_handle_t h, int H, int method, const double* Sigma, int spp,
+                                  double* mean, double* var, double* J, double* cov)
+{
+    AssembleArgs as;
+    memset(&as, 0, sizeof(as));
+    as.G = h->dG; as.Ny = h->Ny; as.Nx = h->Nx; as.H = H; as.method_ta = (method == GPMPC_METHOD_TA);
+    as.Sigma = Sigma; as.sigma_per_point = spp;
+    as.mean = mean; as.var = var; as.J = J; as.cov = cov;
+    as.world = 1;
+    const long long bm1 = (std::min(H, HB) + 7) / 8 * 8;
+    as.stage_g = (assemble_rows_doubles(H, h->Ny, h->Nx) <= (long long)PSK_STAGES * (bm1 + PSK_BN) * GEMM_BK) ? 1 : 0;
+    return as;
 }
 
 template <int NXP, int CH>
 static cudaError_t launch_ks(gpmpc_handle_t h, const double* dZc, int Hc, int bm, int nblk)
 {
-    auto kern = ks_tile_kernel<NXP, CH>;
     const int smem = (NXP + 1) * CH * 8;
-    static std::atomic<bool> conf[GPMPC_MAX_DEVICES];
-    if (!conf[h->device % GPMPC_MAX_DEVICES].load(std::memory_order_acquire)) {      // static + dynamic may pass 48 KB
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return e;
-        conf[h->device % GPMPC_MAX_DEVICES].store(true, std::memory_order_release);
-    }
+    const cudaError_t e = smem_opt_in<ks_tile_kernel<NXP, CH>>(smem);      // static + dynamic may pass 48 KB
+    if (e != cudaSuccess) return e;
     dim3 g(nblk, bm / 8, h->nloc);
-    kern<<<g, 256, smem, h->st>>>(h->dXT, h->Npad, h->N, h->Nx, h->dHyp, h->Nx + 2, h->dAlpha, h->Npad,
-                                  dZc, Hc, h->dKST, h->Npad, (long long)HB * h->Npad, h->dPMJ, nblk);
+    ks_tile_kernel<NXP, CH><<<g, 256, smem, h->st>>>(h->dXT, h->Npad, h->N, h->Nx, h->dHyp, h->Nx + 2, h->dAlpha, h->Npad,
+                                                     dZc, Hc, h->dKST, h->Npad, (long long)HB * h->Npad, h->dPMJ, nblk);
     return cudaGetLastError();
 }
 
@@ -948,7 +981,6 @@ static int predict_core(gpmpc_handle_t h, int method, int H, const double* dZ, c
                         double* d_mean, double* d_var, double* d_cov, double* d_jac)
 {
     const int np = h->Npad, Nx = h->Nx;
-    const int nblk_mj = (np + ks_chunk(h) - 1) / ks_chunk(h);
     NvtxRange nvtx_r("gpmpc.predict");
     // fused epilogue + all-gather over peer memory when the exchange block is attached
     const int use_peers = (h->world > 1 && h->peer_ready && h->opt_peer && H <= h->peerHcap) ? 1 : 0;
@@ -965,32 +997,22 @@ static int predict_core(gpmpc_handle_t h, int method, int H, const double* dZ, c
         pa.step = h->peer_step;
         pa.timeout_clocks = timeout_clocks;
     }
-    AssembleArgs as;
-    memset(&as, 0, sizeof(as));
-    as.G = use_peers ? h->dPeerBlock + pa.goff : h->dG;
-    as.Ny = h->Ny; as.Nx = Nx; as.H = H; as.method_ta = (method == GPMPC_METHOD_TA);
-    as.Sigma = dSigma; as.sigma_per_point = spp;
-    as.mean = d_mean; as.var = d_var; as.J = d_jac; as.cov = d_cov;
-    as.flags = use_peers ? reinterpret_cast<const unsigned long long*>(h->dPeerBlock) + (h->peer_step & 1) * GPMPC_MAXW : nullptr;
+    AssembleArgs as = assemble_args(h, H, method, dSigma, spp, d_mean, d_var, d_jac, d_cov);
+    if (use_peers) as.G = h->dPeerBlock + pa.goff;
+    as.flags = use_peers ? reinterpret_cast<const unsigned long long*>(h->dPeerBlock.p) + (h->peer_step & 1) * GPMPC_MAXW : nullptr;
     as.world = h->world; as.step = h->peer_step; as.status = h->dPeerStatus; as.timeout_clocks = timeout_clocks;
     // one chunk and no NCCL call in between: the product kernel's last CTA assembles too (2 launches per step)
     // (it keeps J Sigma for all H points in the pipeline's shared memory: H Ny Nx doubles, >= 68 KB available)
     const bool fused_assemble = (H <= HB) && !nccl_gather && ((long long)H * h->Ny * Nx * 8 <= 64 * 1024);
-    {   // gather records next to J Sigma in the product kernel's stage buffers (PSK_STAGES (bm + 128) 16 doubles)
-        const long long bm1 = (std::min(H, HB) + 7) / 8 * 8;
-        as.stage_g = (assemble_rows_doubles(H, h->Ny, Nx) <= (long long)PSK_STAGES * (bm1 + PSK_BN) * GEMM_BK) ? 1 : 0;
-    }
     for (int h0 = 0; h0 < H; h0 += HB) {
         const int Hc = std::min(HB, H - h0);
         const int bm = (Hc + 7) / 8 * 8;
         const bool last_chunk = (h0 + HB >= H);
         const double* dZc = dZ + (long long)h0 * Nx;
-        CUDA_TRY(launch_ks_any(h, dZc, Hc, bm, nblk_mj));
+        CUDA_TRY(launch_ks_any(h, dZc, Hc, bm, ks_blocks(h)));
         PredictParams p;
         psk_base(h, p, Hc);
-        p.finalize = 1;
-        p.PMJ = h->dPMJ; p.nblk_mj = nblk_mj;
-        p.Gloc = h->dG; p.slot0 = h->a0; p.Htot = H; p.h0 = h0;
+        psk_finalize(h, p, H, h0);
         p.pa = pa; p.use_peers = use_peers; p.publish = last_chunk ? 1 : 0;
         p.as = as; p.do_assemble = (fused_assemble && !h->opt_refine) ? 1 : 0;
         if (!h->opt_refine) {
@@ -1133,23 +1155,15 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
     if (npairs > 1024) { set_error(h, "EM supports Ny <= 44"); return GPMPC_ERR_ARG; }
     const size_t per = (size_t)Ny * (2 * nn + 2) + (size_t)npairs * (nn + 4);
     const int nblk = (np + 255) / 256, T = (h->N + 63) / 64, Tq = np / 64, ntr = Tq * (Tq + 1) / 2;
-    if (!h->dEmTr) {
-        ALLOC(h->dEmTr, (long long)Ny * ntr);
-        ALLOC(h->dEmLQ, (long long)Ny * np);
-        ALLOC(h->dEmVec, 2LL * np + Ny);
-        ALLOC(h->dEmE, (long long)npairs * np); ALLOC(h->dEmF, (long long)npairs * np);
-        ALLOC(h->dEmE2, (long long)npairs * np); ALLOC(h->dEmF2, (long long)npairs * np);
-        ALLOC(h->dEmW, (long long)npairs * Nx * np); ALLOC(h->dEmIJ, (long long)npairs * Nx * np);
-        ALLOC(h->dEmMeanPart, (long long)Ny * nblk); ALLOC(h->dEmPart, (long long)npairs * T * T);
-    }
+    ENSURE(h->dEmTr, (long long)Ny * ntr);
+    ENSURE(h->dEmLQ, (long long)Ny * np);
+    ENSURE(h->dEmVec, 2LL * np + Ny);
+    ENSURE(h->dEmE, (long long)npairs * np); ENSURE(h->dEmF, (long long)npairs * np);
+    ENSURE(h->dEmE2, (long long)npairs * np); ENSURE(h->dEmF2, (long long)npairs * np);
+    ENSURE(h->dEmW, (long long)npairs * Nx * np); ENSURE(h->dEmIJ, (long long)npairs * Nx * np);
+    ENSURE(h->dEmMeanPart, (long long)Ny * nblk); ENSURE(h->dEmPart, (long long)npairs * T * T);
     { int rcs = ensure_nlml_scratch(h); if (rcs) return rcs; }      // dKinv <- Q_aa, dU <- L^-1 Q_aa (one slab each)
-    if (H > h->emHcap) {
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-        if (h->dEMP) cudaFree(h->dEMP);
-        h->dEMP = nullptr;
-        ALLOC(h->dEMP, (long long)H * per);
-        h->emHcap = H;
-    }
+    ENSURE(h->dEMP, (long long)H * per);
     std::vector<double> emp((size_t)H * per);
     for (int p = 0; p < H; ++p) {
         int rc = em_prepare_point(h, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per);
@@ -1160,9 +1174,7 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
     for (int p = 0; p < H; ++p) {
         const double* dz = h->dZ + (size_t)p * Nx;
         const double* dP = h->dEMP + (size_t)p * per;
-        cudaError_t e = (Nx <= 8) ? launch_em_prep<8>(h, npairs, dz, dP, nblk)
-                      : (Nx <= 16) ? launch_em_prep<16>(h, npairs, dz, dP, nblk) : launch_em_prep<32>(h, npairs, dz, dP, nblk);
-        CUDA_TRY(e);
+        CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_prep<decltype(nxp)::value>(h, npairs, dz, dP, nblk); }));
         em_pair_kernel<<<dim3(T, T, npairs), 256, 2 * Nx * 64 * 8, h->st>>>(h->N, Nx, Ny, dP, h->dAlpha, np,
                                                                           h->dEmE, h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2, h->dEmPart, 0, 0, nullptr, 0);
         CUDA_TRY(cudaGetLastError());
@@ -1287,13 +1299,7 @@ extern "C" int gpmpc_rollout(gpmpc_handle_t h, int method, int Nt, const double*
     // device slab: [Z | Sigma | U | scale | means | vars | cov], host mirror in the pinned buffer
     const size_t o_sig = Nx, o_u = o_sig + (size_t)Nx * Nx, o_sc = o_u + (size_t)Nt * Nu, o_m = o_sc + 4 * (size_t)Ny;
     const size_t o_v = o_m + (size_t)Nt * Ny, o_c = o_v + (size_t)Nt * Ny, tot = o_c + (size_t)Nt * Ny * Ny;   // one cov per step
-    if (tot > h->rollCap) {
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-        if (h->dRoll) cudaFree(h->dRoll);
-        h->dRoll = nullptr; h->rollCap = 0;
-        ALLOC(h->dRoll, tot);
-        h->rollCap = tot;
-    }
+    ENSURE(h->dRoll, tot);
     rc = ensure_pinned(h, tot * 8);
     if (rc) return rc;
     double* pin = h->hPinned;
@@ -1357,8 +1363,7 @@ extern "C" int gpmpc_predict(gpmpc_handle_t h, int method, int H, const double* 
     // Small batches skip both copy operations: the ks kernel reads Z / Sigma from the mapped pinned buffer
     // (each of its CTAs reads HG x Nx doubles once: only worthwhile while that re-read volume is small) and the
     // assembling CTA writes mean / var / J / cov straight into it (posted writes, visible after the stream sync).
-    const int np_ = h->Npad;
-    const long long ks_ctas = (long long)((np_ + ks_chunk(h) - 1) / ks_chunk(h)) * ((std::min(H, HB) + 7) / 8 * 8) * h->nloc;
+    const long long ks_ctas = (long long)ks_blocks(h) * ((std::min(H, HB) + 7) / 8 * 8) * h->nloc;
     const bool zc_in = H <= HB && ks_ctas * Nx * 8 <= 256 * 1024 && in_span * 8 <= 64 * 1024;
     const bool zc_out = out_span * 8 <= 1024 * 1024;
     double* po = pin + in_span;
@@ -1390,12 +1395,8 @@ static cudaError_t launch_grad_reduce(gpmpc_handle_t h, const double* dZc, int H
 {
     dim3 g(nblk, Hc, h->nloc);
     const int smem = (h->Nx * 257 + 256) * 8;
-    static std::atomic<bool> conf[GPMPC_MAX_DEVICES];
-    if (!conf[h->device % GPMPC_MAX_DEVICES].load(std::memory_order_acquire)) {      // static + dynamic may pass 48 KB
-        cudaError_t e = cudaFuncSetAttribute(grad_reduce_kernel<NXP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (NX_MAX * 257 + 256) * 8);
-        if (e != cudaSuccess) return e;
-        conf[h->device % GPMPC_MAX_DEVICES].store(true, std::memory_order_release);
-    }
+    const cudaError_t e = smem_opt_in<grad_reduce_kernel<NXP>>((NX_MAX * 257 + 256) * 8);   // static + dynamic may pass 48 KB
+    if (e != cudaSuccess) return e;
     grad_reduce_kernel<NXP><<<g, 256, smem, h->st>>>(h->dXT, h->Npad, h->N, h->Nx, h->dHyp, h->Nx + 2, h->dAlpha, h->Npad, dZc,
                                                       h->dKST, h->dBeta, h->Npad, (long long)HB * h->Npad, h->dPDV, h->dPH, nblk, Hc);
     return cudaGetLastError();
@@ -1406,12 +1407,8 @@ static cudaError_t launch_hess_reduce(gpmpc_handle_t h, const double* dZc, int H
 {
     dim3 g(nblk, Rc, h->nloc);
     const int smem = (2 * h->Nx * 257 + 512) * 8;
-    static std::atomic<bool> conf[GPMPC_MAX_DEVICES];
-    if (!conf[h->device % GPMPC_MAX_DEVICES].load(std::memory_order_acquire)) {      // static + dynamic may pass 48 KB
-        cudaError_t e = cudaFuncSetAttribute(hess_reduce_kernel<NXP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (2 * NX_MAX * 257 + 512) * 8);
-        if (e != cudaSuccess) return e;
-        conf[h->device % GPMPC_MAX_DEVICES].store(true, std::memory_order_release);
-    }
+    const cudaError_t e = smem_opt_in<hess_reduce_kernel<NXP>>((2 * NX_MAX * 257 + 512) * 8);   // static + dynamic may pass 48 KB
+    if (e != cudaSuccess) return e;
     hess_reduce_kernel<NXP><<<g, 256, smem, h->st>>>(h->dXT, h->Npad, h->N, h->Nx, h->dHyp, h->Nx + 2, h->dAlpha, h->Npad, dZc,
                                                       h->dKST, h->dBeta, h->dVD, h->Npad, (long long)HB * h->Npad,
                                                       h->dPG, h->dPB2, h->dPM3, nblk, Hc, p0);
@@ -1431,9 +1428,7 @@ static int hess_chunk(gpmpc_handle_t h, const double* dZc, int Hc, int H, int h0
         CUDA_TRY(cudaGetLastError());
         int rc = tri_product(h, h->dDR, h->dLi, (rows + 7) / 8 * 8, rows, h->dVD);
         if (rc) return rc;
-        cudaError_t e = (Nx <= 8) ? launch_hess_reduce<8>(h, dZc, Hc, p0, Rc, nblk)
-                      : (Nx <= 16) ? launch_hess_reduce<16>(h, dZc, Hc, p0, Rc, nblk) : launch_hess_reduce<32>(h, dZc, Hc, p0, Rc, nblk);
-        CUDA_TRY(e);
+        CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_hess_reduce<decltype(nxp)::value>(h, dZc, Hc, p0, Rc, nblk); }));
     }
     hess_finalize_kernel<<<dim3(Hc, h->nloc), 128, 0, h->st>>>(h->dPG, h->dPB2, h->dPM3, nblk, Hc, h->dHyp, Nx + 2, Nx, h->Ny,
                                                                h->dG, H, h0, d_d2var, d_d3mean);
@@ -1460,14 +1455,13 @@ static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, c
     if (rc) return rc;
     NvtxRange nvtx_r(ho ? "gpmpc.predict_hess" : "gpmpc.predict_grad");
     const int np = h->Npad, Nx = h->Nx, Ny = h->Ny, npairs = Nx * (Nx + 1) / 2;
-    const int nblk_g = (np + GR_CHUNK - 1) / GR_CHUNK, nblk_mj = (np + ks_chunk(h) - 1) / ks_chunk(h);
-    if (!h->dUall) {
-        ALLOC(h->dUall, (long long)h->nloc * slab(h));
-        ALLOC(h->dBeta, (long long)h->nloc * HB * np);
-        ALLOC(h->dPDV, (long long)h->nloc * HB * nblk_g * Nx);
-        ALLOC(h->dPH, (long long)h->nloc * HB * nblk_g * npairs);
-        if (!h->dV) { ALLOC(h->dV, (long long)h->nloc * HB * np); ALLOC(h->dR, (long long)h->nloc * HB * np); }
-    }
+    const int nblk_g = (np + GR_CHUNK - 1) / GR_CHUNK;
+    ENSURE(h->dUall, (long long)h->nloc * slab(h));
+    ENSURE(h->dBeta, (long long)h->nloc * HB * np);
+    ENSURE(h->dPDV, (long long)h->nloc * HB * nblk_g * Nx);
+    ENSURE(h->dPH, (long long)h->nloc * HB * nblk_g * npairs);
+    rc = ensure_rows(h);
+    if (rc) return rc;
     if (!h->u_valid) {                 // U = Linv^T (upper): the K-contiguous operand of beta = Linv^T v
         dim3 g(np / 32, np / 32), b(32, 8);
         for (int a = 0; a < h->nloc; ++a) {
@@ -1477,35 +1471,20 @@ static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, c
         h->u_valid = true;
     }
     const long long per = (long long)Ny * Nx + (long long)Ny * Ny * Nx + (long long)Ny * Nx * Nx;   // dvar | dcov | hess per point
-    if (H > h->gradHcap) {
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-        if (h->dGradOut) cudaFree(h->dGradOut);
-        h->dGradOut = nullptr; h->gradHcap = 0;
-        ALLOC(h->dGradOut, (long long)std::max(H, HB) * per);
-        h->gradHcap = std::max(H, HB);
-    }
+    ENSURE(h->dGradOut, (long long)std::max(H, HB) * per);
     double* d_dvar = h->dGradOut;
     double* d_dcov = d_dvar + (long long)H * Ny * Nx;
     double* d_hess = d_dcov + (long long)H * Ny * Ny * Nx;
     const long long nxx = (long long)Nx * Nx, ntri = (long long)Nx * (Nx + 1) * (Nx + 2) / 6;
     double *d_d2var = nullptr, *d_d3mean = nullptr, *d_d2cov = nullptr, *d_sh = nullptr;
     if (ho) {
-        if (!h->dDR) {
-            ALLOC(h->dDR, (long long)h->nloc * HB * np);
-            ALLOC(h->dVD, (long long)h->nloc * HB * np);
-            CUDA_TRY(cudaMemsetAsync(h->dDR, 0, (size_t)h->nloc * HB * np * 8, h->st));   // rows past a pass's last are never written
-            ALLOC(h->dPG, (long long)h->nloc * HB * nblk_g * npairs);
-            ALLOC(h->dPB2, (long long)h->nloc * HB * nblk_g * npairs);
-            ALLOC(h->dPM3, (long long)h->nloc * HB * nblk_g * ntri);
-        }
+        ENSURE(h->dDR, (long long)h->nloc * HB * np);      // zero-filled: rows past a pass's last are never written
+        ENSURE(h->dVD, (long long)h->nloc * HB * np);
+        ENSURE(h->dPG, (long long)h->nloc * HB * nblk_g * npairs);
+        ENSURE(h->dPB2, (long long)h->nloc * HB * nblk_g * npairs);
+        ENSURE(h->dPM3, (long long)h->nloc * HB * nblk_g * ntri);
         const long long hper = 2 * Ny * nxx + Ny * nxx * Nx + (long long)Ny * Ny * nxx;      // d2var | SH scratch | d3mean | d2cov
-        if (H > h->hessHcap) {
-            CUDA_TRY(cudaStreamSynchronize(h->st));
-            if (h->dHessOut) cudaFree(h->dHessOut);
-            h->dHessOut = nullptr; h->hessHcap = 0;
-            ALLOC(h->dHessOut, (long long)std::max(H, HB) * hper);
-            h->hessHcap = std::max(H, HB);
-        }
+        ENSURE(h->dHessOut, (long long)std::max(H, HB) * hper);
         d_d2var = h->dHessOut;
         d_sh = d_d2var + (long long)H * Ny * nxx;
         d_d3mean = d_sh + (long long)H * Ny * nxx;
@@ -1514,28 +1493,20 @@ static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, c
     const size_t nz = (size_t)H * Nx, ns = (method == GPMPC_METHOD_TA) ? (size_t)(spp ? H : 1) * Nx * Nx : 0;
     CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, nz * 8, cudaMemcpyHostToDevice, h->st));
     if (ns) CUDA_TRY(cudaMemcpyAsync(h->dSigma, Sigma, ns * 8, cudaMemcpyHostToDevice, h->st));
-    AssembleArgs as;
-    memset(&as, 0, sizeof(as));
-    as.G = h->dG; as.Ny = Ny; as.Nx = Nx; as.H = H; as.method_ta = (method == GPMPC_METHOD_TA);
-    as.Sigma = h->dSigma; as.sigma_per_point = spp;
-    as.mean = h->dMean; as.var = h->dVar; as.J = h->dJ; as.cov = h->dCov;
-    as.world = 1;
+    const AssembleArgs as = assemble_args(h, H, method, h->dSigma, spp, h->dMean, h->dVar, h->dJ, h->dCov);
     for (int h0 = 0; h0 < H; h0 += HB) {
         const int Hc = std::min(HB, H - h0), bm = (Hc + 7) / 8 * 8;
         const double* dZc = h->dZ + (long long)h0 * Nx;
-        CUDA_TRY(launch_ks_any(h, dZc, Hc, bm, nblk_mj));
+        CUDA_TRY(launch_ks_any(h, dZc, Hc, bm, ks_blocks(h)));
         PredictParams p;
         psk_base(h, p, Hc);                                   // v = Linv ks: records + the rows themselves
-        p.finalize = 1; p.PMJ = h->dPMJ; p.nblk_mj = nblk_mj;
-        p.Gloc = h->dG; p.slot0 = h->a0; p.Htot = H; p.h0 = h0;
+        psk_finalize(h, p, H, h0);
         p.Vout = h->dV; p.sV = (long long)HB * np; p.ldv = np;
         CUDA_TRY(psk_launch(bm, p, h->dKST, (long long)HB * np, h->dLi, slab(h), np, psk_grid(h, p.G), h->st));
         psk_base(h, p, Hc);                                   // beta = Linv^T v = K^-1 ks  (rows of V times U^T)
         p.upper = 1; p.Vout = h->dBeta; p.sV = (long long)HB * np; p.ldv = np;
         CUDA_TRY(psk_launch(bm, p, h->dV, (long long)HB * np, h->dUall, slab(h), np, psk_grid(h, p.G), h->st));
-        cudaError_t e = (Nx <= 8) ? launch_grad_reduce<8>(h, dZc, Hc, nblk_g)
-                      : (Nx <= 16) ? launch_grad_reduce<16>(h, dZc, Hc, nblk_g) : launch_grad_reduce<32>(h, dZc, Hc, nblk_g);
-        CUDA_TRY(e);
+        CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_grad_reduce<decltype(nxp)::value>(h, dZc, Hc, nblk_g); }));
         grad_finalize_kernel<<<dim3(Hc, h->nloc), 128, 0, h->st>>>(h->dPDV, h->dPH, nblk_g, Hc, h->dHyp, Nx + 2, Nx, Ny,
                                                                    h->dG, H, h0, d_dvar, d_hess);
         CUDA_TRY(cudaGetLastError());
@@ -1598,9 +1569,10 @@ extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double*
     const int N = h->N, Nx = h->Nx, np = h->Npad, nl = h->nloc;
     // k(X, x_new) for every owned output through the predict ks kernel (H = 1): row 0 of KS^T
     CUDA_TRY(cudaMemcpyAsync(h->dZ, x_new, Nx * 8, cudaMemcpyHostToDevice, h->st));
-    CUDA_TRY(launch_ks_any(h, h->dZ, 1, 8, (np + ks_chunk(h) - 1) / ks_chunk(h)));
+    CUDA_TRY(launch_ks_any(h, h->dZ, 1, 8, ks_blocks(h)));
     // l = Li k (rows < N), r = Li^T l
-    if (!h->dV) { ALLOC(h->dV, (long long)nl * HB * np); ALLOC(h->dR, (long long)nl * HB * np); }
+    rc = ensure_rows(h);
+    if (rc) return rc;
     dim3 g1((np + 7) / 8, 1, nl);
     trmv_lower_kernel<<<g1, 256, 0, h->st>>>(h->dLi, np, slab(h), h->dKST, (long long)HB * np, h->dV, (long long)HB * np, N);
     CUDA_TRY(cudaGetLastError());
@@ -1647,44 +1619,26 @@ extern "C" int gpmpc_posterior_cov(gpmpc_handle_t h, int H, const double* Z, dou
     const int np = h->Npad, Nx = h->Nx, nl = h->nloc;
     const long long sVall = (long long)H * np;            // all H solved rows of one output
     // scratch is pooled on the handle (grown on demand), not allocated per call
-    if ((long long)nl * sVall > h->covVcap) {
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-        if (h->dCovV) cudaFree(h->dCovV);
-        h->dCovV = nullptr; h->covVcap = 0;
-        ALLOC(h->dCovV, (long long)nl * sVall);
-        h->covVcap = (long long)nl * sVall;
-    }
-    if ((long long)nl * H * H > h->covOutcap) {
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-        if (h->dCovOut) cudaFree(h->dCovOut);
-        h->dCovOut = nullptr; h->covOutcap = 0;
-        ALLOC(h->dCovOut, (long long)nl * H * H);
-        h->covOutcap = (long long)nl * H * H;
-    }
-    double *dVall = h->dCovV, *dOut = h->dCovOut;
-    if (!h->dV) { ALLOC(h->dV, (long long)nl * HB * np); ALLOC(h->dR, (long long)nl * HB * np); }
+    ENSURE(h->dCovV, (long long)nl * sVall);
+    ENSURE(h->dCovOut, (long long)nl * H * H);
+    rc = ensure_rows(h);
+    if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, (size_t)H * Nx * 8, cudaMemcpyHostToDevice, h->st));
-    const int nblk_mj = (np + ks_chunk(h) - 1) / ks_chunk(h);
-    for (int h0 = 0; h0 < H && rc == GPMPC_OK; h0 += HB) {
+    for (int h0 = 0; h0 < H; h0 += HB) {
         const int Hc = std::min(HB, H - h0), bm = (Hc + 7) / 8 * 8;
         const double* dZc = h->dZ + (long long)h0 * Nx;
-        cudaError_t e = launch_ks_any(h, dZc, Hc, bm, nblk_mj);
-        if (e != cudaSuccess) { set_error(h, "posterior_cov ks: %s", cudaGetErrorString(e)); rc = GPMPC_ERR_CUDA; break; }
+        CUDA_TRY(launch_ks_any(h, dZc, Hc, bm, ks_blocks(h)));
         rc = tri_product(h, h->dKST, h->dLi, bm, Hc, h->dV);
-        if (rc) break;
-        dim3 g(1, Hc, nl);
+        if (rc) return rc;
         copy2d_kernel<<<dim3(16, std::min(Hc, 64), nl), 128, 0, h->st>>>(h->dV, np, (long long)HB * np,
-                                                                     dVall + (long long)h0 * np, np, sVall, Hc, np);
-        if (cudaGetLastError() != cudaSuccess) { rc = GPMPC_ERR_CUDA; break; }
+                                                                     h->dCovV + (long long)h0 * np, np, sVall, Hc, np);
+        CUDA_TRY(cudaGetLastError());
     }
-    if (rc == GPMPC_OK) {
-        gram_cov_kernel<<<dim3(H, H, nl), 256, 0, h->st>>>(dVall, np, sVall, np, h->dHyp, Nx + 2, Nx, H, dOut);
-        if (cudaGetLastError() != cudaSuccess) rc = GPMPC_ERR_CUDA;
-    }
-    if (rc == GPMPC_OK && cudaMemcpyAsync(out, dOut, (size_t)nl * H * H * 8, cudaMemcpyDeviceToHost, h->st) != cudaSuccess) rc = GPMPC_ERR_CUDA;
-    cudaStreamSynchronize(h->st);
-    if (rc == GPMPC_ERR_CUDA) set_error(h, "gpmpc_posterior_cov: CUDA failure %s", cudaGetErrorString(cudaGetLastError()));
-    return rc;
+    gram_cov_kernel<<<dim3(H, H, nl), 256, 0, h->st>>>(h->dCovV, np, sVall, np, h->dHyp, Nx + 2, Nx, H, h->dCovOut);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(out, h->dCovOut, (size_t)nl * H * H * 8, cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    return GPMPC_OK;
 }
 
 // ------------------------------------------------------------------------------------
@@ -1732,7 +1686,7 @@ extern "C" int gpmpc_peer_export(gpmpc_handle_t h, int Hcap, void* handle64)
     const int nyp = h->nloc_max * h->world;
     h->peerGsz = (long long)nyp * Hcap * (h->Nx + 2);
     h->peerHcap = Hcap;
-    ALLOC(h->dPeerBlock, 2 * GPMPC_MAXW + 2 * h->peerGsz);
+    ENSURE(h->dPeerBlock, 2 * GPMPC_MAXW + 2 * h->peerGsz);
     if (!h->dPeerStatus) {     // status word in mapped pinned host memory: the host reads it without a copy
         CUDA_TRY(cudaHostAlloc((void**)&h->hPeerStatus, sizeof(int), cudaHostAllocMapped));
         *h->hPeerStatus = 0;
@@ -1794,18 +1748,17 @@ extern "C" int gpmpc_profile_balance(gpmpc_handle_t h, int H, double* out4)
     PredictParams p;
     psk_base(h, p, H);
     const int grid = psk_grid(h, p.G);
-    unsigned long long* dbg = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&dbg, (size_t)grid * 16));
+    DevBuf<unsigned long long> dbg;
+    ENSURE(dbg, (long long)grid * 2);
     p.dbg = dbg;
     const int np = h->Npad, bm = (H + 7) / 8 * 8;
     for (int rep = 0; rep < 2; ++rep) {
         cudaError_t e = psk_launch(bm, p, h->dKST, (long long)HB * np, h->dLi, slab(h), np, grid, h->st);
-        if (e != cudaSuccess) { cudaFree(dbg); set_error(h, "profile_balance: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
+        if (e != cudaSuccess) { set_error(h, "profile_balance: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
     }
     std::vector<unsigned long long> t((size_t)grid * 2);
     cudaMemcpyAsync(t.data(), dbg, t.size() * 8, cudaMemcpyDeviceToHost, h->st);
     cudaStreamSynchronize(h->st);
-    cudaFree(dbg);
     unsigned long long lo = ~0ull, hi = 0; double mn = 1e300, mx = 0.0, sum = 0.0;
     for (int c = 0; c < grid; ++c) {
         const double d = (double)(t[2 * c + 1] - t[2 * c]) * 1e-3;
@@ -1831,27 +1784,20 @@ extern "C" int gpmpc_profile_tail(gpmpc_handle_t h, int H, double* out8)
     PredictParams p;
     psk_base(h, p, H);
     const int grid = psk_grid(h, p.G);
-    unsigned long long* dbg = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&dbg, (size_t)(grid * 2 + 8) * 8));
-    CUDA_TRY(cudaMemset(dbg, 0, (size_t)(grid * 2 + 8) * 8));
+    DevBuf<unsigned long long> dbg;
+    ENSURE(dbg, (long long)grid * 2 + 8);
     p.dbg = dbg;
-    p.finalize = 1; p.PMJ = h->dPMJ; p.nblk_mj = (np + ks_chunk(h) - 1) / ks_chunk(h);
-    p.Gloc = h->dG; p.slot0 = h->a0; p.Htot = H; p.h0 = 0;
-    AssembleArgs as;
-    memset(&as, 0, sizeof(as));
-    as.G = h->dG; as.Ny = h->Ny; as.Nx = h->Nx; as.H = H; as.method_ta = 1; as.Sigma = h->dSigma;
-    as.mean = h->dMean; as.var = h->dVar; as.J = h->dJ; as.cov = h->dCov; as.world = 1;
-    as.stage_g = (assemble_rows_doubles(H, h->Ny, h->Nx) <= (long long)PSK_STAGES * (bm + PSK_BN) * GEMM_BK) ? 1 : 0;
-    as.dbg = dbg + 2 * grid;
-    p.as = as; p.do_assemble = 1;
+    psk_finalize(h, p, H, 0);
+    p.as = assemble_args(h, H, GPMPC_METHOD_TA, h->dSigma, 0, h->dMean, h->dVar, h->dJ, h->dCov);
+    p.as.dbg = dbg + 2 * grid;
+    p.do_assemble = 1;
     for (int rep = 0; rep < 2; ++rep) {
         cudaError_t e = psk_launch(bm, p, h->dKST, (long long)HB * np, h->dLi, slab(h), np, grid, h->st);
-        if (e != cudaSuccess) { cudaFree(dbg); set_error(h, "profile_tail: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
+        if (e != cudaSuccess) { set_error(h, "profile_tail: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
     }
     std::vector<unsigned long long> t((size_t)grid * 2 + 8);
     cudaMemcpyAsync(t.data(), dbg, t.size() * 8, cudaMemcpyDeviceToHost, h->st);
     cudaStreamSynchronize(h->st);
-    cudaFree(dbg);
     unsigned long long lo = ~0ull, hi = 0, hi2 = 0; int cmax = 0;
     for (int c = 0; c < grid; ++c) {
         lo = std::min(lo, t[2 * c]);
@@ -1870,10 +1816,9 @@ extern "C" int gpmpc_profile_leaf(gpmpc_handle_t h, double* out15)
     if (!h || !out15) return GPMPC_ERR_ARG;
     if (!h->has_data || !h->has_hyper) { set_error(h, "gpmpc_profile_leaf: set_data and set_hyper first"); return GPMPC_ERR_STATE; }
     CUDA_TRY(cudaSetDevice(h->device));
-    long long* d = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&d, 16 * sizeof(long long)));
-    CUDA_TRY(cudaMemset(d, 0, 16 * sizeof(long long)));
-    CUDA_TRY(cudaMemcpyToSymbol(d_leaf_prof, &d, sizeof(d)));
+    DevBuf<long long> d;
+    ENSURE(d, 16);
+    CUDA_TRY(cudaMemcpyToSymbol(d_leaf_prof, &d.p, sizeof(d.p)));
     int rc = GPMPC_OK;
     for (int rep = 0; rep < 2 && rc == GPMPC_OK; ++rep) {           // second run: warm instruction cache
         rc = launch_kbuild(h, h->dHyp, h->dJit, h->dL, 1, 0);
@@ -1884,7 +1829,6 @@ extern "C" int gpmpc_profile_leaf(gpmpc_handle_t h, double* out15)
     cudaMemcpy(hst, d, sizeof(hst), cudaMemcpyDeviceToHost);
     long long* nul = nullptr;
     cudaMemcpyToSymbol(d_leaf_prof, &nul, sizeof(nul));
-    cudaFree(d);
     for (int k = 0; k < 15; ++k) out15[k] = (double)(hst[k] - hst[0]);
     h->factorized = false;
     return rc;
@@ -1901,7 +1845,7 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
     const int np = h->Npad;
     float ms = 0.f;
     int rc = GPMPC_OK;
-    auto run = [&](int rep) -> int {
+    auto run = [&]() -> int {
         switch (what) {
         case GPMPC_PROF_KBUILD_FULL: return launch_kbuild(h, h->dHyp, h->dJit, h->dL, 1, 1);
         case GPMPC_PROF_KBUILD_LOWER: return launch_kbuild(h, h->dHyp, h->dJit, h->dL, 1, 0);
@@ -1930,7 +1874,7 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
         }
         case GPMPC_PROF_KS: {             // the ks / mean / Jacobian partial kernel alone (Z = the last batch's inputs)
             const int Hc = (n > 0 && n <= HB) ? n : 56;
-            cudaError_t e = launch_ks_any(h, h->dZ, Hc, (Hc + 7) / 8 * 8, (np + ks_chunk(h) - 1) / ks_chunk(h));
+            cudaError_t e = launch_ks_any(h, h->dZ, Hc, (Hc + 7) / 8 * 8, ks_blocks(h));
             if (e != cudaSuccess) { set_error(h, "profile ks: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
             return GPMPC_OK;
         }
@@ -1938,14 +1882,9 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
             const int Hc = (n > 0 && n <= HB) ? n : 56;
             PredictParams p;
             psk_base(h, p, Hc);
-            p.finalize = 1; p.PMJ = h->dPMJ; p.nblk_mj = (np + ks_chunk(h) - 1) / ks_chunk(h);
-            p.Gloc = h->dG; p.slot0 = h->a0; p.Htot = Hc; p.h0 = 0;
-            AssembleArgs as;
-            memset(&as, 0, sizeof(as));
-            as.G = h->dG; as.Ny = h->Ny; as.Nx = h->Nx; as.H = Hc; as.method_ta = 1; as.Sigma = h->dSigma;
-            as.mean = h->dMean; as.var = h->dVar; as.J = h->dJ; as.cov = h->dCov; as.world = 1;
-            as.stage_g = (assemble_rows_doubles(Hc, h->Ny, h->Nx) <= (long long)PSK_STAGES * ((Hc + 7) / 8 * 8 + PSK_BN) * GEMM_BK) ? 1 : 0;
-            p.as = as; p.do_assemble = (h->world == 1 && h->nloc == h->Ny) ? 1 : 0;
+            psk_finalize(h, p, Hc, 0);
+            p.as = assemble_args(h, Hc, GPMPC_METHOD_TA, h->dSigma, 0, h->dMean, h->dVar, h->dJ, h->dCov);
+            p.do_assemble = (h->world == 1 && h->nloc == h->Ny) ? 1 : 0;
             cudaError_t e = psk_launch((Hc + 7) / 8 * 8, p, h->dKST, (long long)HB * np, h->dLi, slab(h), np, psk_grid(h, p.G), h->st);
             if (e != cudaSuccess) { set_error(h, "profile predict tail: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
             return GPMPC_OK;
@@ -1955,11 +1894,11 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
     };
     if (what == GPMPC_PROF_TRIGEMM || what == GPMPC_PROF_KS || what == GPMPC_PROF_PREDICT_TAIL) { rc = ensure_predict_bufs(h, HB); if (rc) return rc; }
     CUDA_TRY(cudaMemsetAsync(h->dJit, 0, h->nloc * sizeof(double), h->st));
-    rc = run(-1);
+    rc = run();
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(h->st));
     CUDA_TRY(cudaEventRecord(h->ev0, h->st));
-    for (int r = 0; r < reps; ++r) { rc = run(r); if (rc) return rc; }
+    for (int r = 0; r < reps; ++r) { rc = run(); if (rc) return rc; }
     CUDA_TRY(cudaEventRecord(h->ev1, h->st));
     CUDA_TRY(cudaEventSynchronize(h->ev1));
     CUDA_TRY(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
