@@ -39,6 +39,7 @@ SYMBOLS = [
     ('gpmpc_predict_grad', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     ('gpmpc_predict_hess', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp,
                                      _dp, _dp, _dp]),
+    ('gpmpc_predict_em_grad', C.c_int, [_H, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     ('gpmpc_get_size', C.c_int, [_H, _ip, _ip, _ip]),
     ('gpmpc_append', C.c_int, [_H, _dp, _dp]),
     ('gpmpc_posterior_cov', C.c_int, [_H, C.c_int, _dp, _dp]),
@@ -297,6 +298,24 @@ class Engine:
             self.h, int(method), H, _ptr(Z), _ptr(Sigma), spp,
             *[_ptr(out[k]) for k in ('mean', 'var', 'cov', 'jac', 'dvar_dz', 'dcov_dz', 'hess', 'd2var_dz2', 'd3mean_dz3',
                                      'd2cov_dz2')]))
+        return out
+
+    def predict_em_grad(self, Z, Sigma):
+        """'EM' prediction + first derivatives w.r.t. the test input mean and the input covariance
+        (gpmpc_predict_em_grad).  Sigma: (Nx,Nx) shared or (H,Nx,Nx).  Returns dict(mean (H,Ny), var, cov (H,Ny,Ny),
+        dmean_dz (H,Ny,Nx), dmean_dSigma (H,Ny,Nx,Nx), dcov_dz (H,Ny,Ny,Nx), dcov_dSigma (H,Ny,Ny,Nx,Nx))."""
+        Z = _f64(Z).reshape(-1, self.Nx)
+        H = Z.shape[0]
+        Sigma = _f64(Sigma)
+        spp = 1 if Sigma.ndim == 3 else 0
+        assert Sigma.shape == ((H, self.Nx, self.Nx) if spp else (self.Nx, self.Nx))
+        Ny, Nx = self.Ny, self.Nx
+        out = dict(mean=np.empty((H, Ny)), var=np.empty((H, Ny)), cov=np.empty((H, Ny, Ny)),
+                   dmean_dz=np.empty((H, Ny, Nx)), dmean_dSigma=np.empty((H, Ny, Nx, Nx)),
+                   dcov_dz=np.empty((H, Ny, Ny, Nx)), dcov_dSigma=np.empty((H, Ny, Ny, Nx, Nx)))
+        self._check(self.lib.gpmpc_predict_em_grad(
+            self.h, H, _ptr(Z), _ptr(Sigma), spp,
+            *[_ptr(out[k]) for k in ('mean', 'var', 'cov', 'dmean_dz', 'dmean_dSigma', 'dcov_dz', 'dcov_dSigma')]))
         return out
 
     def append(self, x_new, y_new):

@@ -1,4 +1,5 @@
-// CasADi `external`-shaped entry points around gpmpc_predict_grad / gpmpc_predict_hess (SURVEY 8f row 1).
+// CasADi `external`-shaped entry points around gpmpc_predict_grad / gpmpc_predict_hess / gpmpc_predict_em_grad
+// (SURVEY 8f row 1).
 //
 // mpc_class.py:361-423 calls gp.predict(mean_t, u_t, covar_t) once per shooting node with MX
 // symbols and nlpsol (:496-513) differentiates the resulting graph.  With
@@ -13,10 +14,12 @@
 //   inputs : i0 = Z     (Nx  x Nt)     test inputs of all shooting nodes, standardised space
 //            i1 = Sigma (Nx  x Nx*Nt)  input covariance of every node (Nt blocks side by side)
 //   outputs: o0 = mean  (Ny  x Nt)
-//            o1 = cov   (Ny  x Ny*Nt)  'TA' / 'ME' covariance blocks
+//            o1 = cov   (Ny  x Ny*Nt)  'TA' / 'ME' / 'EM' covariance blocks
 //   jac_gp_b200: inputs (i0, i1, o0, o1), outputs block-diagonal sparse
-//            jac_o0_i0 (Ny*Nt x Nx*Nt), jac_o0_i1 (empty), jac_o1_i0 (Ny*Ny*Nt x Nx*Nt),
-//            jac_o1_i1 (Ny*Ny*Nt x Nx*Nx*Nt;  d cov[a][b] / d Sigma[d][e] = J_a[d] J_b[e] for 'TA')
+//            jac_o0_i0 (Ny*Nt x Nx*Nt), jac_o0_i1 (empty; 'EM': Ny x Nx*Nx per node, d mean_a / d Sigma[d][e]),
+//            jac_o1_i0 (Ny*Ny*Nt x Nx*Nt),
+//            jac_o1_i1 (Ny*Ny*Nt x Nx*Nx*Nt;  d cov[a][b] / d Sigma[d][e] = J_a[d] J_b[e] for 'TA', the exact
+//            gradient of gpmpc_predict_em_grad for 'EM'; column d + Nx*e <-> Sigma[d][e]; empty for 'ME')
 //   jac_jac_gp_b200: inputs (i0, i1, o0, o1, and the four outputs of jac_gp_b200), outputs the Jacobians of
 //            jac_gp_b200's four outputs w.r.t. its four inputs (output-major), what IPOPT's exact Hessian
 //            needs.  Rows index the column-major dense vec of the differentiated Jacobian, columns the dense
@@ -25,7 +28,8 @@
 //              jac_cov_z   / z      Ny*Ny*Nx*Nx      d^2 cov[a][b] / d z_e d z_f     (d2cov_dz2)
 //              jac_cov_z   / sigma  Ny*Ny*Nx*Nx*Nx   hess_a[d][e] J_b[e'] + J_a[d] hess_b[e'][e]   ('TA')
 //              jac_cov_sigma / z    Ny*Ny*Nx*Nx*Nx   the same values, w.r.t. z_f of d cov / d Sigma[d][e]  ('TA')
-//            everything else is structurally zero.
+//            everything else is structurally zero.  'EM' has no second derivatives: jac_jac_gp_b200 returns failure
+//            (run IPOPT with hessian_approximation 'limited-memory').
 #include "../../include/gpmpc.h"
 
 #include <functional>
@@ -40,7 +44,7 @@ struct Bound {
     gpmpc_handle_t h = nullptr;
     int method = GPMPC_METHOD_TA, Nt = 0, Nx = 0, Ny = 0;
     std::vector<casadi_int> sp_in[2], sp_out[2], sp_jac[4], sp_jj[16];
-    std::vector<double> sig, mean, var, cov, jac, dvar, dcov, hess, d2cov;
+    std::vector<double> sig, mean, var, cov, jac, dvar, dcov, hess, d2cov, dmS, dcS;   // dmS / dcS: 'EM' d / d Sigma
     int refs = 0;
 };
 Bound g_b;
@@ -97,13 +101,21 @@ int eval(const casadi_real* Z, const casadi_real* Sigma, int mode)
     Bound& b = g_b;
     if (!b.h || !Z) return 1;
     const int Nt = b.Nt, Nx = b.Nx;
-    const bool ta = b.method == GPMPC_METHOD_TA;
-    if (ta) {
+    const bool ta = b.method == GPMPC_METHOD_TA, em = b.method == GPMPC_METHOD_EM;
+    if (ta || em) {
         if (!Sigma) return 1;
         for (int t = 0; t < Nt; ++t)
             for (int d = 0; d < Nx; ++d)
                 for (int e = 0; e < Nx; ++e)
                     b.sig[((size_t)t * Nx + d) * Nx + e] = Sigma[((size_t)t * Nx + e) * Nx + d];
+    }
+    if (em) {
+        if (mode == EVAL_VALUE)
+            return gpmpc_predict(b.h, b.method, Nt, Z, b.sig.data(), 1, b.mean.data(), b.var.data(), b.cov.data(), nullptr) == GPMPC_OK ? 0 : 1;
+        if (mode == EVAL_GRAD)
+            return gpmpc_predict_em_grad(b.h, Nt, Z, b.sig.data(), 1, b.mean.data(), b.var.data(), b.cov.data(), b.jac.data(),
+                                         b.dmS.data(), b.dcov.data(), b.dcS.data()) == GPMPC_OK ? 0 : 1;
+        return 1;                       // no second derivatives of 'EM'
     }
     if (mode == EVAL_HESS)
         return gpmpc_predict_hess(b.h, b.method, Nt, Z, ta ? b.sig.data() : nullptr, 1, b.mean.data(), b.var.data(),
@@ -117,28 +129,31 @@ int eval(const casadi_real* Z, const casadi_real* Sigma, int mode)
 }
 }  // namespace
 
-// Bind the (process-global) external to a factorised engine handle: method GPMPC_METHOD_ME / _TA,
+// Bind the (process-global) external to a factorised engine handle: method GPMPC_METHOD_ME / _TA / _EM,
 // Nt shooting nodes per call.  Call again to re-bind (e.g. after a refit or another horizon).
 extern "C" int gp_b200_bind(gpmpc_handle_t h, int method, int Nt)
 {
     std::lock_guard<std::mutex> lock(g_mtx);
     int N = 0, Nx = 0, Ny = 0;
-    if (!h || Nt < 1 || (method != GPMPC_METHOD_ME && method != GPMPC_METHOD_TA)) return GPMPC_ERR_ARG;
+    if (!h || Nt < 1 || (method != GPMPC_METHOD_ME && method != GPMPC_METHOD_TA && method != GPMPC_METHOD_EM)) return GPMPC_ERR_ARG;
     if (gpmpc_get_size(h, &N, &Nx, &Ny) != GPMPC_OK) return GPMPC_ERR_ARG;
     Bound& b = g_b;
     b.h = h; b.method = method; b.Nt = Nt; b.Nx = Nx; b.Ny = Ny;
     b.sp_in[0] = dense_sp(Nx, Nt); b.sp_in[1] = dense_sp(Nx, (casadi_int)Nx * Nt);
     b.sp_out[0] = dense_sp(Ny, Nt); b.sp_out[1] = dense_sp(Ny, (casadi_int)Ny * Nt);
     b.sp_jac[0] = blockdiag_sp(Ny, Nx, Nt);
-    b.sp_jac[1] = empty_sp((casadi_int)Ny * Nt, (casadi_int)Nx * Nx * Nt);
+    b.sp_jac[1] = (method == GPMPC_METHOD_EM) ? blockdiag_sp(Ny, (casadi_int)Nx * Nx, Nt)
+                                              : empty_sp((casadi_int)Ny * Nt, (casadi_int)Nx * Nx * Nt);
     b.sp_jac[2] = blockdiag_sp((casadi_int)Ny * Ny, Nx, Nt);
-    b.sp_jac[3] = (method == GPMPC_METHOD_TA) ? blockdiag_sp((casadi_int)Ny * Ny, (casadi_int)Nx * Nx, Nt)
+    b.sp_jac[3] = (method != GPMPC_METHOD_ME) ? blockdiag_sp((casadi_int)Ny * Ny, (casadi_int)Nx * Nx, Nt)
                                               : empty_sp((casadi_int)Ny * Ny * Nt, (casadi_int)Nx * Nx * Nt);
     b.sig.assign((size_t)Nt * Nx * Nx, 0.0);
     b.mean.assign((size_t)Nt * Ny, 0.0); b.var.assign((size_t)Nt * Ny, 0.0);
     b.cov.assign((size_t)Nt * Ny * Ny, 0.0); b.jac.assign((size_t)Nt * Ny * Nx, 0.0);
     b.dvar.assign((size_t)Nt * Ny * Nx, 0.0); b.dcov.assign((size_t)Nt * Ny * Ny * Nx, 0.0);
     b.hess.assign((size_t)Nt * Ny * Nx * Nx, 0.0); b.d2cov.assign((size_t)Nt * Ny * Ny * Nx * Nx, 0.0);
+    if (method == GPMPC_METHOD_EM) { b.dmS.assign((size_t)Nt * Ny * Nx * Nx, 0.0); b.dcS.assign((size_t)Nt * Ny * Ny * Nx * Nx, 0.0); }
+    else { b.dmS.clear(); b.dcS.clear(); }
     // jac_jac_gp_b200: numel of jac_gp_b200's outputs (rows) and inputs (columns)
     const casadi_int T = Nt, X = Nx, Y = Ny;
     const casadi_int n_out[4] = {Y * T * X * T, Y * T * X * X * T, Y * Y * T * X * T, Y * Y * T * X * X * T};
@@ -261,6 +276,23 @@ extern "C" int jac_gp_b200(const casadi_real** arg, casadi_real** res, casadi_in
                 for (int bb = 0; bb < Ny; ++bb)
                     for (int a = 0; a < Ny; ++a)
                         res[2][(((size_t)t * Nx + e) * Ny + bb) * Ny + a] = b.dcov[(((size_t)t * Ny + a) * Ny + bb) * Nx + e];
+    if (b.method == GPMPC_METHOD_EM) {
+        if (res[1])      // block t, column d + Nx*e (vec of Sigma), row a:  d mean_a / d Sigma[d][e]
+            for (int t = 0; t < Nt; ++t)
+                for (int e = 0; e < Nx; ++e)
+                    for (int d = 0; d < Nx; ++d)
+                        for (int a = 0; a < Ny; ++a)
+                            res[1][(((size_t)t * Nx + e) * Nx + d) * Ny + a] = b.dmS[(((size_t)t * Ny + a) * Nx + d) * Nx + e];
+        if (res[3])      // column d + Nx*e, row a + Ny*b:  d cov[a][b] / d Sigma[d][e]
+            for (int t = 0; t < Nt; ++t)
+                for (int e = 0; e < Nx; ++e)
+                    for (int d = 0; d < Nx; ++d)
+                        for (int bb = 0; bb < Ny; ++bb)
+                            for (int a = 0; a < Ny; ++a)
+                                res[3][((((size_t)t * Nx + e) * Nx + d) * Ny + bb) * Ny + a] =
+                                    b.dcS[((((size_t)t * Ny + a) * Ny + bb) * Nx + d) * Nx + e];
+        return 0;
+    }
     if (res[3] && b.method == GPMPC_METHOD_TA)   // column d + Nx*e (vec of Sigma), row a + Ny*b:  J_a[d] J_b[e]
         for (int t = 0; t < Nt; ++t)
             for (int e = 0; e < Nx; ++e)

@@ -113,6 +113,9 @@ struct gpmpc_handle_s {
     // EM scratch
     DevBuf<double> dEmTr, dEMP, dEmE, dEmF, dEmW, dEmIJ;
     DevBuf<double> dEmMeanPart, dEmPart, dEmLQ, dEmVec, dEmE2, dEmF2;
+    // EM derivatives: full symmetric K^-1 per output (lazy, one per factorisation), record partials and sums,
+    // backbone rows [e | e v_d] and their L^-1 products
+    DevBuf<double> dEmKinv, dEmGPart, dEmGRec, dEmBB; bool em_kinv_valid = false;
     std::vector<double> hyper;        // (nloc, Nx+2)
     std::vector<double> logdet, yalpha;
     std::vector<int> jitter_used;
@@ -563,7 +566,7 @@ extern "C" int gpmpc_set_y(gpmpc_handle_t h, int a, const double* y)
     if (al < 0) return GPMPC_ERR_ARG;
     CUDA_TRY(cudaMemcpyAsync(h->dY + (long long)al * h->Npad, y, (size_t)h->N * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
-    h->factorized = false;
+    h->factorized = false; h->em_kinv_valid = false;
     return GPMPC_OK;
 }
 
@@ -580,7 +583,7 @@ extern "C" int gpmpc_set_hyper(gpmpc_handle_t h, const double* hyper, int ld)
         }
     CUDA_TRY(cudaMemcpyAsync(h->dHyp, h->hyper.data(), h->hyper.size() * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
-    h->has_hyper = true; h->factorized = false;
+    h->has_hyper = true; h->factorized = false; h->em_kinv_valid = false;
     return GPMPC_OK;
 }
 
@@ -665,7 +668,7 @@ extern "C" int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info)
     CUDA_TRY(cudaMemcpyAsync(res.data(), h->dRes, 2 * nl * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
     for (int a = 0; a < nl; ++a) { h->logdet[a] = res[2 * a]; h->yalpha[a] = res[2 * a + 1]; }
-    h->factorized = true; h->u_valid = false;
+    h->factorized = true; h->u_valid = false; h->em_kinv_valid = false;
     return GPMPC_OK;
 }
 
@@ -706,7 +709,7 @@ extern "C" int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* 
     if (al < 0) return GPMPC_ERR_ARG;
     const int m = h->Nx + 2;
     for (int d = 0; d < h->Nx; ++d) if (theta[d] == 0.0) { set_error(h, "gpmpc_nlml: zero length scale"); return GPMPC_ERR_ARG; }
-    h->factorized = false;
+    h->factorized = false; h->em_kinv_valid = false;
     NvtxRange nvtx_r("gpmpc.nlml");
     CUDA_TRY(cudaMemcpyAsync(h->dHypTmp, theta, m * 8, cudaMemcpyHostToDevice, h->st));
     int used = 0;
@@ -1144,8 +1147,190 @@ static cudaError_t launch_em_prep(gpmpc_handle_t h, int npairs, const double* dz
     return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------
+// 'EM' first derivatives w.r.t. z and Sigma (gpmpc_predict_em_grad).  Per point, after the forward chain, the
+// O(N) / O(N^2) sums go into records (kernels.cuh, em_moments_kernel / em_grad_pair_kernel); the host forms the
+// Nx x Nx derivatives from them (em_grad_finish).  Record order per point:
+//   [mean moments a | cross pair p, owner rows / columns | trace remainder a | backbone a | backbone Gram a]
+// ------------------------------------------------------------------------------------
+struct EmGradOutputs {
+    double *dmean_dz, *dmean_dSigma, *dcov_dz, *dcov_dSigma;
+};
+
+static inline int em_rec_len(int Nx) { return 1 + Nx + 2 * Nx * Nx; }
+
+template <int NXP>
+static cudaError_t launch_em_grad(gpmpc_handle_t h, const double* dz, const double* dP, int npairs, int nb, double* rec_out)
+{
+    const int N = h->N, Nx = h->Nx, Ny = h->Ny, np = h->Npad, RL = em_rec_len(Nx);
+    const int r_cross = Ny, r_tr = Ny + 2 * npairs, r_bb = r_tr + Ny, r_gram = r_bb + Ny, nrec = r_gram + Ny;
+    double* part = h->dEmGPart;
+    const long long srec = (long long)nb * RL;
+    const int smem = (4 * NXP * 64 + 64 * 65) * 8;
+    cudaError_t e = smem_opt_in<em_grad_pair_kernel<NXP>>(smem);
+    if (e != cudaSuccess) return e;
+    em_moments_kernel<NXP><<<dim3(nb, Ny), 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, h->dAlpha, h->dEmLQ, np, part, srec, RL);
+    em_grad_pair_kernel<NXP><<<dim3(nb, npairs, 2), 256, smem, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE, h->dEmF,
+                                                                        h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2, nullptr, 0,
+                                                                        r_cross, part, nb, RL);
+    em_grad_pair_kernel<NXP><<<dim3(nb, Ny, 1), 256, smem, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE, h->dEmF,
+                                                                    h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2, h->dEmKinv, 1,
+                                                                    r_tr, part, nb, RL);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    // rank-one backbone e e^T of Q_aa through L^-1: u = L^-1 e and Yd = L^-1 (e o v_d) in one batched trmv,
+    // K^-1 e = L^-T u; records of r_i = e_i (K^-1 e)_i and the Gram Y^T Y
+    double* rows = h->dEmBB;
+    double* prod = rows + (long long)(Nx + 1) * np;
+    double* kie = prod + (long long)(Nx + 1) * np;
+    for (int a = 0; a < Ny; ++a) {
+        const int paa = a * (a + 1) / 2 + a;
+        const double* Li = h->dLi + (long long)a * slab(h);
+        em_bb_rows_kernel<<<(np + 255) / 256, 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, h->dEmE + (long long)paa * np, np, rows);
+        trmv_lower_kernel<<<dim3((np + 7) / 8, 1, Nx + 1), 256, 0, h->st>>>(Li, np, 0, rows, np, prod, np, np);
+        trmv_lower_T_kernel<<<dim3(np / 32, 1, 1), 256, 0, h->st>>>(Li, np, 0, prod, np, kie, np, np);
+        em_moments_kernel<NXP><<<dim3(nb, 1), 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, kie, h->dEmE + (long long)paa * np, 0,
+                                                               part + (long long)(r_bb + a) * srec, 0, RL);
+        em_moments_kernel<NXP><<<dim3(nb, 1), 256, 0, h->st>>>(prod + np, np, N, Nx, nullptr, nullptr, nullptr, 0,
+                                                               part + (long long)(r_gram + a) * srec, 0, RL);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    em_sum_parts_kernel<<<nrec, 256, 0, h->st>>>(part, nb, RL, rec_out);
+    return cudaGetLastError();
+}
+
+// n x n helpers for the host side of the EM derivatives
+static void mat_mul(int n, const double* A, const double* B, double* C, bool bt = false)
+{
+    for (int i = 0; i < n; ++i)
+        for (int j = 0; j < n; ++j) {
+            double s = 0.0;
+            for (int k = 0; k < n; ++k) s += A[i * n + k] * (bt ? B[j * n + k] : B[k * n + j]);
+            C[i * n + j] = s;
+        }
+}
+
+static bool mat_inv(int n, const double* A, double* Ai)
+{
+    std::vector<double> LU(A, A + n * n);
+    std::vector<int> piv(n);
+    double det = 0.0;
+    if (!lu_factor(n, LU.data(), piv.data(), &det)) return false;
+    for (int i = 0; i < n * n; ++i) Ai[i] = 0.0;
+    for (int i = 0; i < n; ++i) Ai[i * n + i] = 1.0;
+    lu_solve(n, LU.data(), piv.data(), Ai, n);
+    return true;
+}
+
+// derivatives of one point from its records (DESIGN 4.8).  emp: the point's em_prepare_point block (iR_a, t_ab),
+// rec: its records, mean: its Ny means.  d/dSigma is symmetrised (the gradient at a symmetric Sigma is symmetric).
+static int em_grad_finish(gpmpc_handle_t h, const double* S, const double* emp, const double* rec, const double* mean,
+                          double* dmz, double* dmS, double* dcz, double* dcS)
+{
+    const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, m = Nx + 2, RL = em_rec_len(Nx), npairs = Ny * (Ny + 1) / 2;
+    const int r_cross = Ny, r_tr = Ny + 2 * npairs, r_bb = r_tr + Ny, r_gram = r_bb + Ny;
+    auto R = [&](int r) { return rec + (size_t)r * RL; };
+    auto sym_store = [&](const double* G, double* o1, double* o2) {
+        for (int d = 0; d < Nx; ++d)
+            for (int e = 0; e <= d; ++e) {
+                const double v = 0.5 * (G[d * Nx + e] + G[e * Nx + d]);
+                o1[d * Nx + e] = o1[e * Nx + d] = v;
+                if (o2) o2[d * Nx + e] = o2[e * Nx + d] = v;
+            }
+    };
+    std::vector<double> t1(nn), t2(nn), t3(nn), G(nn), C(nn), A(nn), B(nn), Fa(nn), Fb(nn), CP(nn), Z1(nn), dz(Nx);
+    std::vector<double> ila(Nx), ilb(Nx), ga(Nx), gb(Nx);
+    for (int a = 0; a < Ny; ++a) {
+        const double* iR = emp + (size_t)a * (2 * nn + 2);
+        const double* sa = R(a) + 1;
+        const double* Sa = R(a) + 1 + Nx;
+        for (int d = 0; d < Nx; ++d) {
+            double s = 0.0;
+            for (int k = 0; k < Nx; ++k) s += iR[d * Nx + k] * sa[k];
+            if (dmz) dmz[(size_t)a * Nx + d] = s;
+        }
+        mat_mul(Nx, iR, Sa, t1.data());
+        mat_mul(Nx, t1.data(), iR, G.data());
+        for (int q = 0; q < nn; ++q) G[q] = 0.5 * G[q] - 0.5 * mean[a] * iR[q];
+        if (dmS) sym_store(G.data(), dmS + (size_t)a * nn, nullptr);
+    }
+    int p = 0;
+    for (int a = 0; a < Ny; ++a)
+        for (int b = 0; b <= a; ++b, ++p) {
+            const double* la = &h->hyper[(size_t)a * m];
+            const double* lb = &h->hyper[(size_t)b * m];
+            const double* iRa = emp + (size_t)a * (2 * nn + 2);
+            const double* iRb = emp + (size_t)b * (2 * nn + 2);
+            const double t = emp[(size_t)Ny * (2 * nn + 2) + (size_t)p * (nn + 4) + nn];
+            const double Ma = mean[a], Mb = mean[b];
+            const double *sa = R(a) + 1, *Sa = R(a) + 1 + Nx, *sb = R(b) + 1, *Sb = R(b) + 1 + Nx;
+            for (int d = 0; d < Nx; ++d) { ila[d] = 1.0 / (la[d] * la[d]); ilb[d] = 1.0 / (lb[d] * lb[d]); }
+            // C = (I + P Sigma)^-1, Fa = C La^-1, Fb = C Lb^-1, CP = C P,
+            // A = -C Lb^-1 Sigma iR_a = C La^-1 - iR_a,  B = -C La^-1 Sigma iR_b  (formed without the subtraction)
+            for (int i = 0; i < Nx; ++i)
+                for (int j = 0; j < Nx; ++j) t1[i * Nx + j] = (i == j ? 1.0 : 0.0) + (ila[i] + ilb[i]) * S[i * Nx + j];
+            if (!mat_inv(Nx, t1.data(), C.data())) { set_error(h, "EM: I + P Sigma is singular"); return GPMPC_ERR_ARG; }
+            for (int i = 0; i < Nx; ++i)
+                for (int j = 0; j < Nx; ++j) {
+                    Fa[i * Nx + j] = C[i * Nx + j] * ila[j]; Fb[i * Nx + j] = C[i * Nx + j] * ilb[j];
+                    CP[i * Nx + j] = C[i * Nx + j] * (ila[j] + ilb[j]);
+                }
+            mat_mul(Nx, Fb.data(), S, t1.data()); mat_mul(Nx, t1.data(), iRa, A.data());
+            mat_mul(Nx, Fa.data(), S, t1.data()); mat_mul(Nx, t1.data(), iRb, B.data());
+            for (int q = 0; q < nn; ++q) { A[q] = -A[q]; B[q] = -B[q]; }
+            const double *r0 = R(r_cross + 2 * p), *r1 = R(r_cross + 2 * p + 1);
+            const double *u1 = r0 + 1, *Mii = r0 + 1 + Nx, *Mij = r0 + 1 + Nx + nn, *u2 = r1 + 1, *Mjj = r1 + 1 + Nx;
+            // d/dz: iR_a u1 + iR_b u2 + A (u1 + s_a Mb) + B (u2 + Ma s_b)
+            for (int d = 0; d < Nx; ++d) {
+                double s = 0.0;
+                for (int k = 0; k < Nx; ++k)
+                    s += iRa[d * Nx + k] * u1[k] + iRb[d * Nx + k] * u2[k] + A[d * Nx + k] * (u1[k] + sa[k] * Mb) + B[d * Nx + k] * (u2[k] + Ma * sb[k]);
+                dz[d] = s;
+            }
+            // d/dSigma: 1/2 C Z1 C^T - 1/2 (sum m) C P  (the expm1 part), Z1 = sum m zeta zeta^T
+            for (int d = 0; d < Nx; ++d)
+                for (int e = 0; e < Nx; ++e)
+                    Z1[d * Nx + e] = Mii[d * Nx + e] * ila[d] * ila[e] + Mij[d * Nx + e] * ila[d] * ilb[e]
+                                   + Mij[e * Nx + d] * ilb[d] * ila[e] + Mjj[d * Nx + e] * ilb[d] * ilb[e];
+            mat_mul(Nx, C.data(), Z1.data(), t1.data()); mat_mul(Nx, t1.data(), C.data(), G.data(), true);
+            for (int q = 0; q < nn; ++q) G[q] = 0.5 * G[q] - 0.5 * r0[0] * CP[q];
+            // + sum_ij w_ij d delta_ij: w is rank one, so these are products of the per-output moments
+            auto add_side = [&](const double* X, const double* S_, const double* iR, double scale) {   // scale (X S iR + iR S X^T + X S X^T) / 2
+                mat_mul(Nx, X, S_, t1.data());
+                mat_mul(Nx, t1.data(), iR, t2.data());
+                mat_mul(Nx, t1.data(), X, t3.data(), true);
+                for (int d = 0; d < Nx; ++d)
+                    for (int e = 0; e < Nx; ++e) G[d * Nx + e] += 0.5 * scale * (t2[d * Nx + e] + t2[e * Nx + d] + t3[d * Nx + e]);
+            };
+            add_side(A.data(), Sa, iRa, Mb);
+            add_side(B.data(), Sb, iRb, Ma);
+            for (int d = 0; d < Nx; ++d) {
+                ga[d] = 0.0; gb[d] = 0.0;
+                for (int k = 0; k < Nx; ++k) { ga[d] += Fa[d * Nx + k] * sa[k]; gb[d] += Fb[d * Nx + k] * sb[k]; }
+            }
+            for (int d = 0; d < Nx; ++d)
+                for (int e = 0; e < Nx; ++e)
+                    G[d * Nx + e] += 0.5 * (ga[d] * gb[e] + gb[d] * ga[e]) - 0.5 * (A[d * Nx + e] + B[d * Nx + e]) * Ma * Mb;
+            if (a == b) {       // - d T_a, T_a = t tr(K^-1 Q_aa): backbone records plus the remainder's
+                const double *rt = R(r_tr + a), *rb = R(r_bb + a), *rg = R(r_gram + a);
+                const double T = t * (rb[0] + rt[0]);
+                for (int d = 0; d < Nx; ++d) {
+                    double s = 0.0;
+                    for (int k = 0; k < Nx; ++k) s += Fa[d * Nx + k] * t * (rb[1 + k] + rt[1 + k]);
+                    dz[d] -= 2.0 * s;
+                }
+                for (int q = 0; q < nn; ++q) Z1[q] = t * (rb[1 + Nx + q] + rt[1 + Nx + q] + rg[1 + Nx + q] + rt[1 + Nx + nn + q]);
+                mat_mul(Nx, Fa.data(), Z1.data(), t1.data()); mat_mul(Nx, t1.data(), Fa.data(), t2.data(), true);
+                for (int q = 0; q < nn; ++q) G[q] -= t2[q] - 0.5 * T * CP[q];
+            }
+            if (dcz)
+                for (int d = 0; d < Nx; ++d) dcz[((size_t)a * Ny + b) * Nx + d] = dcz[((size_t)b * Ny + a) * Nx + d] = dz[d];
+            if (dcS) sym_store(G.data(), dcS + ((size_t)a * Ny + b) * nn, dcS + ((size_t)b * Ny + a) * nn);
+        }
+    return GPMPC_OK;
+}
+
 static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Sigma, int spp,
-                      double* mean, double* var, double* cov)
+                      double* mean, double* var, double* cov, const EmGradOutputs* go = nullptr)
 {
     const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, np = h->Npad;
     NvtxRange nvtx_r("gpmpc.predict_em");
@@ -1164,6 +1349,22 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
     ENSURE(h->dEmMeanPart, (long long)Ny * nblk); ENSURE(h->dEmPart, (long long)npairs * T * T);
     { int rcs = ensure_nlml_scratch(h); if (rcs) return rcs; }      // dKinv <- Q_aa, dU <- L^-1 Q_aa (one slab each)
     ENSURE(h->dEMP, (long long)H * per);
+    const int RL = em_rec_len(Nx), nrec = 4 * Ny + 2 * npairs;
+    if (go) {
+        ENSURE(h->dEmGPart, (long long)nrec * T * RL);
+        ENSURE(h->dEmGRec, (long long)H * nrec * RL);
+        ENSURE(h->dEmBB, (2LL * (Nx + 1) + 1) * np);
+        ENSURE(h->dEmKinv, (long long)Ny * slab(h));
+        if (!h->em_kinv_valid) {        // K^-1 = U U^T per output (compute_kinv, lower), stored full and symmetric
+            for (int a = 0; a < Ny; ++a) {
+                int rck = compute_kinv(h, a);
+                if (rck) return rck;
+                sym_from_lower_kernel<<<dim3(np / 32, np / 32), dim3(32, 8), 0, h->st>>>(h->dKinv, h->dEmKinv + (long long)a * slab(h), np);
+                CUDA_TRY(cudaGetLastError());
+            }
+            h->em_kinv_valid = true;
+        }
+    }
     std::vector<double> emp((size_t)H * per);
     for (int p = 0; p < H; ++p) {
         int rc = em_prepare_point(h, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per);
@@ -1206,11 +1407,31 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
                                                    h->dEmTr, ntr, h->dEmVec + 2LL * np,
                                                    h->dMean + (size_t)p * Ny, h->dVar + (size_t)p * Ny, h->dCov + (size_t)p * Ny * Ny);
         CUDA_TRY(cudaGetLastError());
+        if (go) {
+            double* rec = h->dEmGRec + (size_t)p * nrec * RL;
+            CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_grad<decltype(nxp)::value>(h, dz, dP, npairs, T, rec); }));
+        }
     }
     if (mean) CUDA_TRY(cudaMemcpyAsync(mean, h->dMean, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
     if (var) CUDA_TRY(cudaMemcpyAsync(var, h->dVar, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
     if (cov) CUDA_TRY(cudaMemcpyAsync(cov, h->dCov, (size_t)H * Ny * Ny * 8, cudaMemcpyDeviceToHost, h->st));
+    if (!go) {
+        CUDA_TRY(cudaStreamSynchronize(h->st));
+        return GPMPC_OK;
+    }
+    std::vector<double> recs((size_t)H * nrec * RL), mh((size_t)H * Ny);
+    CUDA_TRY(cudaMemcpyAsync(recs.data(), h->dEmGRec, recs.size() * 8, cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaMemcpyAsync(mh.data(), h->dMean, mh.size() * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
+    for (int p = 0; p < H; ++p) {
+        const int rc = em_grad_finish(h, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per, recs.data() + (size_t)p * nrec * RL,
+                                      mh.data() + (size_t)p * Ny,
+                                      go->dmean_dz ? go->dmean_dz + (size_t)p * Ny * Nx : nullptr,
+                                      go->dmean_dSigma ? go->dmean_dSigma + (size_t)p * Ny * nn : nullptr,
+                                      go->dcov_dz ? go->dcov_dz + (size_t)p * Ny * Ny * Nx : nullptr,
+                                      go->dcov_dSigma ? go->dcov_dSigma + (size_t)p * Ny * Ny * nn : nullptr);
+        if (rc) return rc;
+    }
     return GPMPC_OK;
 }
 
@@ -1558,6 +1779,24 @@ extern "C" int gpmpc_predict_hess(gpmpc_handle_t h, int method, int H, const dou
     return predict_derivs(h, "gpmpc_predict_hess", method, H, Z, Sigma, spp, mean, var, cov, jac, dvar_dz, dcov_dz, hess, &ho);
 }
 
+// 'EM' prediction plus its first derivatives w.r.t. z and Sigma (see include/gpmpc.h)
+extern "C" int gpmpc_predict_em_grad(gpmpc_handle_t h, int H, const double* Z, const double* Sigma, int spp,
+                                     double* mean, double* var, double* cov,
+                                     double* dmean_dz, double* dmean_dSigma, double* dcov_dz, double* dcov_dSigma)
+{
+    int rc = predict_check(h, GPMPC_METHOD_EM, H);
+    if (rc) return rc;
+    if (!Z || !Sigma) { set_error(h, "gpmpc_predict_em_grad: null Z / Sigma"); return GPMPC_ERR_ARG; }
+    if (h->nloc != h->Ny || h->world != 1) { set_error(h, "gpmpc_predict_em_grad needs all outputs on one handle (replicate the model, shard the points)"); return GPMPC_ERR_STATE; }
+    CUDA_TRY(cudaSetDevice(h->device));
+    rc = ensure_predict_bufs(h, H);
+    if (rc) return rc;
+    NvtxRange nvtx_r("gpmpc.predict_em_grad");
+    const EmGradOutputs go = {dmean_dz, dmean_dSigma, dcov_dz, dcov_dSigma};
+    const bool any = dmean_dz || dmean_dSigma || dcov_dz || dcov_dSigma;   // none: the forward call alone, no K^-1 cache
+    return predict_em(h, H, Z, Sigma, spp, mean, var, cov, any ? &go : nullptr);
+}
+
 extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double* y_new)
 {
     if (!h || !x_new || !y_new) return GPMPC_ERR_ARG;
@@ -1599,7 +1838,7 @@ extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double*
             return GPMPC_ERR_NOTPD;
         }
     h->N = N + 1;
-    h->u_valid = false;
+    h->u_valid = false; h->em_kinv_valid = false;
     rc = launch_alpha(h, 0, nl);
     if (rc) return rc;
     std::vector<double> res(2 * nl);

@@ -1175,6 +1175,214 @@ __global__ void em_finalize_kernel(int Nx, int Ny, int npairs, const double* __r
 }
 
 // ---------------------------------------------------------------------------------------
+// 'EM' first derivatives (gpmpc_predict_em_grad).  Every O(N) / O(N^2) sum ends in a record of
+// RL = 1 + Nx + 2 Nx^2 doubles over a weight m_k (k the "owner" index) and v_k = x_k - z:
+//   [ sum m_k | sum m_k v_k (Nx) | sum m_k v_k v_k^T (Nx^2) | sum_k v_k Y_k^T (Nx^2, pair sums only) ]
+// written as one partial per 64-index block and summed in block order by em_sum_parts_kernel; the host
+// forms the derivatives from the records (gpmpc.cu, em_grad_finish).
+// ---------------------------------------------------------------------------------------
+// Record of weights m_k = x1_k exp(x2_k) (a null operand counts as 1 / 0) over the d-major vectors
+// V[d][k] - z[d] (z may be null), k < n; one 64-index block per CTA (blockIdx.x), one record per blockIdx.y
+// (operands offset by sx, record by srec).  The last Nx^2 slot is written as zero.
+template <int NXP>
+__global__ void __launch_bounds__(256)
+em_moments_kernel(const double* __restrict__ V, int ldv, int n, int Nx, const double* __restrict__ z,
+                  const double* __restrict__ x1, const double* __restrict__ x2, long long sx,
+                  double* __restrict__ part, long long srec, int RL)
+{
+    __shared__ double w[64], vs[NXP * 64];
+    const int tid = threadIdx.x, k0 = blockIdx.x * 64;
+    if (x1) x1 += blockIdx.y * sx;
+    if (x2) x2 += blockIdx.y * sx;
+    if (tid < 64) {
+        const int k = k0 + tid;
+        w[tid] = (k < n) ? (x1 ? x1[k] : 1.0) * (x2 ? exp(x2[k]) : 1.0) : 0.0;
+    }
+    for (int idx = tid; idx < NXP * 64; idx += 256) {
+        const int d = idx >> 6, k = k0 + (idx & 63);
+        vs[idx] = (d < Nx && k < n) ? V[(long long)d * ldv + k] - (z ? z[d] : 0.0) : 0.0;
+    }
+    __syncthreads();
+    double* out = part + blockIdx.y * srec + (long long)blockIdx.x * RL;
+    const int nn = Nx * Nx;
+    for (int q = tid; q < RL; q += 256) {
+        double s = 0.0;
+        if (q == 0) { for (int k = 0; k < 64; ++k) s += w[k]; }
+        else if (q <= Nx) { const int d = q - 1; for (int k = 0; k < 64; ++k) s = fma(w[k], vs[d * 64 + k], s); }
+        else if (q <= Nx + nn) {
+            const int d = (q - 1 - Nx) / Nx, e = (q - 1 - Nx) % Nx;
+            for (int k = 0; k < 64; ++k) s = fma(w[k] * vs[d * 64 + k], vs[e * 64 + k], s);
+        }
+        out[q] = s;
+    }
+}
+
+// Pair sums of one 64-index owner block (blockIdx.x) against every other block, the 64x64 tiles recomputed
+// as em_pair_kernel does (no N x N array is written):
+//   mode 0, pair p = blockIdx.y, orientation o = blockIdx.z:  m_ij = w_ij expm1(delta_ij) (the cross term's
+//     small weights, w_ij = beta_ai q_ai beta_bj q_bj); owner = rows i (o = 0) or columns j (o = 1);
+//     record rec0 + 2p + o.
+//   mode 1, output a = blockIdx.y (pair (a,a)):  m_ij = K^-1_ij Qt_ij with Qt = e^{E_i+F_j} expm1(2 acc_ij) the
+//     O(Sigma) remainder of Q_aa; Kinv = full symmetric K^-1 per output (stride ldn^2); record rec0 + a.
+// The owner's sums over the other index, R_k = sum m and Y_k = sum m v_other, stay in registers across the
+// tiles (fixed order); the record then sums over the owner block in index order.
+template <int NXP>
+__global__ void __launch_bounds__(256)
+em_grad_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
+                    const double* __restrict__ alpha, long long sal,
+                    const double* __restrict__ XT, int ldx, const double* __restrict__ z,
+                    const double* __restrict__ E, const double* __restrict__ F, const double* __restrict__ W,
+                    const double* __restrict__ IJ, int ldn, const double* __restrict__ LQ,
+                    const double* __restrict__ E2, const double* __restrict__ F2,
+                    const double* __restrict__ Kinv, int mode, int rec0, double* __restrict__ part, int nb, int RL)
+{
+    constexpr int KF = NXP / 4 + 1;                  // features per thread: f = g + 4k, f = 0 (ones), 1 + d (v_d)
+    extern __shared__ double sm[];
+    double* Wo = sm;                                  // [NXP][64] W rows of the i block
+    double* Jo = Wo + NXP * 64;                       // [NXP][64] IJ rows of the j block
+    double* Vown = Jo + NXP * 64;                     // [NXP][64] v of the owner block
+    double* Voth = Vown + NXP * 64;                   // [NXP][64] v of the other block
+    double* Ms = Voth + NXP * 64;                     // [64][65] m tile, owner-major
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int nn = Nx * Nx;
+    const int o = mode ? 0 : blockIdx.z;
+    const int p = mode ? blockIdx.y * (blockIdx.y + 1) / 2 + blockIdx.y : blockIdx.y;
+    const double* P = EMP + (long long)Ny * (2 * nn + 2) + (long long)p * (nn + 4);
+    const int a = (int)P[nn + 1], b = (int)P[nn + 2];
+    const double cab = P[nn + 3];
+    const double* Ka = mode ? Kinv + (long long)a * ldn * ldn : nullptr;
+    const int own0 = blockIdx.x * 64, T = (N + 63) / 64;
+    for (int idx = tid; idx < NXP * 64; idx += 256) {
+        const int d = idx >> 6, k = own0 + (idx & 63);
+        const bool ok = d < Nx && k < N;
+        Vown[idx] = ok ? XT[(long long)d * ldx + k] - z[d] : 0.0;
+        if (o == 0) Wo[idx] = ok ? W[((long long)p * Nx + d) * ldn + k] : 0.0;
+        else Jo[idx] = ok ? IJ[((long long)p * Nx + d) * ldn + k] : 0.0;
+    }
+    const int ko = tid & 63, g = tid >> 6;
+    double acc2[KF];
+#pragma unroll
+    for (int q = 0; q < KF; ++q) acc2[q] = 0.0;
+    for (int t = 0; t < T; ++t) {
+        const int oth0 = t * 64;
+        __syncthreads();                              // previous tile's readers are done
+        for (int idx = tid; idx < NXP * 64; idx += 256) {
+            const int d = idx >> 6, k = oth0 + (idx & 63);
+            const bool ok = d < Nx && k < N;
+            Voth[idx] = ok ? XT[(long long)d * ldx + k] - z[d] : 0.0;
+            if (o == 0) Jo[idx] = ok ? IJ[((long long)p * Nx + d) * ldn + k] : 0.0;
+            else Wo[idx] = ok ? W[((long long)p * Nx + d) * ldn + k] : 0.0;
+        }
+        __syncthreads();
+        const int i0 = o ? oth0 : own0, j0 = o ? own0 : oth0;
+        double acc[4][4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) acc[r][c] = 0.0;
+        for (int d = 0; d < Nx; ++d) {
+            double wv[4], jv[4];
+#pragma unroll
+            for (int r = 0; r < 4; ++r) wv[r] = Wo[d * 64 + ty + 16 * r];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) jv[c] = Jo[d * 64 + tx + 16 * c];
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) acc[r][c] = fma(wv[r], jv[c], acc[r][c]);
+        }
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int il = ty + 16 * r, i = i0 + il;
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const int jl = tx + 16 * c, j = j0 + jl;
+                double m = 0.0;
+                if (i < N && j < N) {
+                    if (mode) {
+                        m = Ka[(long long)i * ldn + j] * (exp(E[(long long)p * ldn + i] + F[(long long)p * ldn + j]) * expm1(2.0 * acc[r][c]));
+                    } else {
+                        const double la = LQ[(long long)a * ldn + i], lb = LQ[(long long)b * ldn + j];
+                        const double wgt = (alpha[(long long)a * sal + i] * exp(la)) * (alpha[(long long)b * sal + j] * exp(lb));
+                        m = wgt * expm1(cab + E2[(long long)p * ldn + i] + F2[(long long)p * ldn + j] + 2.0 * acc[r][c]);
+                    }
+                }
+                if (o == 0) Ms[il * 65 + jl] = m; else Ms[jl * 65 + il] = m;
+            }
+        }
+        __syncthreads();
+        for (int x = 0; x < 64; ++x) {
+            const double mv = Ms[ko * 65 + x];
+#pragma unroll
+            for (int q = 0; q < KF; ++q) {
+                const int f = g + 4 * q;
+                if (f <= Nx) acc2[q] = fma(mv, f == 0 ? 1.0 : Voth[(f - 1) * 64 + x], acc2[q]);
+            }
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int q = 0; q < KF; ++q) {
+        const int f = g + 4 * q;
+        if (f <= Nx) Ms[ko * 65 + f] = acc2[q];       // Ms[k][0] = R_k, Ms[k][1+d] = Y_k,d
+    }
+    __syncthreads();
+    const int rec = rec0 + (mode ? (int)blockIdx.y : 2 * p + o);
+    double* out = part + ((long long)rec * nb + blockIdx.x) * RL;
+    for (int q = tid; q < RL; q += 256) {
+        double s = 0.0;
+        if (q == 0) { for (int k = 0; k < 64; ++k) s += Ms[k * 65]; }
+        else if (q <= Nx) { const int d = q - 1; for (int k = 0; k < 64; ++k) s = fma(Ms[k * 65], Vown[d * 64 + k], s); }
+        else if (q <= Nx + nn) {
+            const int d = (q - 1 - Nx) / Nx, e = (q - 1 - Nx) % Nx;
+            for (int k = 0; k < 64; ++k) s = fma(Ms[k * 65] * Vown[d * 64 + k], Vown[e * 64 + k], s);
+        } else {
+            const int d = (q - 1 - Nx - nn) / Nx, e = (q - 1 - Nx - nn) % Nx;
+            for (int k = 0; k < 64; ++k) s = fma(Vown[d * 64 + k], Ms[k * 65 + 1 + e], s);
+        }
+        out[q] = s;
+    }
+}
+
+// rows of the rank-one backbone of Q_aa for L^-1: R[0][i] = e_i = exp(E_i), R[1+d][i] = e_i (x_id - z_d); zero for i >= N
+__global__ void em_bb_rows_kernel(const double* __restrict__ XT, int ldx, int N, int Nx, const double* __restrict__ z,
+                                  const double* __restrict__ E, int n, double* __restrict__ R)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const double e = (i < N) ? exp(E[i]) : 0.0;
+    R[i] = e;
+    for (int d = 0; d < Nx; ++d) R[(long long)(1 + d) * n + i] = (i < N) ? e * (XT[(long long)d * ldx + i] - z[d]) : 0.0;
+}
+
+// out[rec][q] = sum over the nb block partials of rec, in block order
+__global__ void em_sum_parts_kernel(const double* __restrict__ part, int nb, int RL, double* __restrict__ out)
+{
+    const long long rec = blockIdx.x;
+    for (int q = threadIdx.x; q < RL; q += blockDim.x) {
+        double s = 0.0;
+        for (int b = 0; b < nb; ++b) s += part[(rec * nb + b) * RL + q];
+        out[rec * RL + q] = s;
+    }
+}
+
+// full symmetric copy of a lower-stored matrix (32x32 tiles, every entry taken from the lower triangle)
+__global__ void sym_from_lower_kernel(const double* __restrict__ Kl, double* __restrict__ Kf, int ld)
+{
+    __shared__ double tile[32][33];
+    const int bi = blockIdx.y, bj = blockIdx.x;
+    if (bj > bi) return;
+    const int tx = threadIdx.x, ty = threadIdx.y;   // 32 x 8
+    for (int r = ty; r < 32; r += 8) tile[r][tx] = Kl[(long long)(bi * 32 + r) * ld + bj * 32 + tx];
+    __syncthreads();
+    for (int r = ty; r < 32; r += 8) {
+        const double lo = (bi > bj || r >= tx) ? tile[r][tx] : tile[tx][r];
+        Kf[(long long)(bi * 32 + r) * ld + bj * 32 + tx] = lo;
+        if (bi > bj) Kf[(long long)(bj * 32 + r) * ld + bi * 32 + tx] = tile[tx][r];
+    }
+}
+
+// ---------------------------------------------------------------------------------------
 // Rank-1 append of one training point (SURVEY 8f row 3; the reference's update_data,
 // gp_class.py:384-471, is self-declared broken -- this is the textbook update):
 //   l = L^-1 k(X, x_new);  lambda = sqrt(k(x_new,x_new) + sn2 - l^T l)

@@ -347,11 +347,16 @@ class GP:
             dmean_dz (H,Ny,Nx)    d mean / d [x,u] in the CALLER's units (chain rule through the scalers)
             dcov_dz  (H,Ny,Ny,Nx) d cov / d [x,u]  (cov itself is not rescaled, so only 1/stdZ enters)
             dcov_dSigma_factor (H,Ny,Nx)  J with d cov[a][b] / d Sigma[d][e] = J[a][d] J[b][e] ('TA')
-        Methods 'ME' and 'TA'.  This is what a casadi.Callback's Jacobian function returns; the same
+        With method 'EM' (gpmpc_predict_em_grad) the covariance of the input enters the mean as well, and the dict
+        holds mean, cov, dmean_dz, dcov_dz and, for Sigma in the GP's (standardised) input space,
+            dmean_dSigma (H,Ny,Nx,Nx)     d mean / d Sigma[d][e], de-standardised (carries stdY)
+            dcov_dSigma  (H,Ny,Ny,Nx,Nx)  d cov / d Sigma[d][e] (cov and Sigma both standardised: unscaled)
+        each entry of Sigma varied with the others fixed (exactly symmetric in d, e).
+        This is what a casadi.Callback's Jacobian function returns; the same
         numbers are available to `casadi.external` through gp_b200 / jac_gp_b200 (include/gpmpc_casadi.h)."""
         method = method or self.__gp_method
-        if method not in ('ME', 'TA'):
-            raise NotImplementedError("derivatives are available for gp_method 'ME' and 'TA'")
+        if method not in ('ME', 'TA', 'EM'):
+            raise NotImplementedError("derivatives are available for gp_method 'ME', 'TA' and 'EM'")
         if self.__comm.world > 1 and self.__mode == 'outputs':
             raise NotImplementedError('predict_batch_grad needs all outputs on one GPU (build the GP with a single-process Comm)')
         x = np.asarray(x, dtype=np.float64).reshape(-1, self.__Ny)
@@ -360,6 +365,15 @@ class GP:
             x = self.standardize(x, self.__meanX, self.__stdX)
             u = self.standardize(u, self.__meanU, self.__stdU)
         Z = np.hstack([x, u])
+        if method == 'EM':
+            g = self.__engine.predict_em_grad(Z, np.zeros((self.__Nx, self.__Nx)) if cov is None else cov)
+            mean, dmz, dmS, dcz = g['mean'], g['dmean_dz'], g['dmean_dSigma'], g['dcov_dz']
+            if self.__normalize:
+                mean = self.inverse_mean(mean, self.__meanY, self.__stdY)
+                dmz = dmz * self.__stdY[None, :, None] / self.__stdZ[None, None, :]
+                dmS = dmS * self.__stdY[None, :, None, None]
+                dcz = dcz / self.__stdZ[None, None, None, :]
+            return dict(mean=mean, cov=g['cov'], dmean_dz=dmz, dcov_dz=dcz, dmean_dSigma=dmS, dcov_dSigma=g['dcov_dSigma'])
         if cov is None and method == 'TA':
             cov = np.zeros((self.__Nx, self.__Nx))
         g = self.__engine.predict_grad(Z, cov if method == 'TA' else None, _GPU_METHODS[method])

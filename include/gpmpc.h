@@ -157,6 +157,18 @@ int gpmpc_predict_hess(gpmpc_handle_t h, int method, int H, const double* Z, con
                        double* dvar_dz, double* dcov_dz, double* hess,
                        double* d2var_dz2, double* d3mean_dz3, double* d2cov_dz2);
 
+/* 'EM' prediction plus its first derivatives w.r.t. the test input mean z and the input covariance Sigma: what CasADi's AD
+ * extracts from gp_exact_moment (gp_functions.py:344-418) when nlpsol differentiates the MPC's NLP with gp_method 'EM'.
+ * Same inputs as gpmpc_predict (Sigma required).  Outputs, each optional (NULL to skip):
+ *   mean (H,Ny)  var (H,Ny)  cov (H,Ny,Ny)   -- bit-identical to gpmpc_predict(GPMPC_METHOD_EM)
+ *   dmean_dz (H,Ny,Nx)   dmean_dSigma (H,Ny,Nx,Nx)   dcov_dz (H,Ny,Ny,Nx)   dcov_dSigma (H,Ny,Ny,Nx,Nx)
+ * d/dSigma[d][e] holds every other entry fixed (the convention jac_gp_b200 already uses for 'TA'); at a symmetric Sigma
+ * that gradient is symmetric in (d,e), and it is returned exactly symmetric.  The handle must own all outputs
+ * (GPMPC_ERR_STATE); Ny <= 44 as for EM.  gpmpc_predict_grad keeps rejecting 'EM'. */
+int gpmpc_predict_em_grad(gpmpc_handle_t h, int H, const double* Z, const double* Sigma, int sigma_per_point,
+                          double* mean, double* var, double* cov,
+                          double* dmean_dz, double* dmean_dSigma, double* dcov_dz, double* dcov_dSigma);
+
 /* Open-loop multi-step prediction with the state kept on the device: the numeric loop of GP.predict_compare
  * (gp_class.py:746-804, :779-792: mean_t, covar_x = predict(mean_t, u_t, covar); covar[:Ny,:Ny] = covar_x) for a
  * model whose inputs are z = [x, u] (Nx = Ny + Nu).  All Nt steps are enqueued back to back, one synchronisation.

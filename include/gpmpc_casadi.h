@@ -13,8 +13,11 @@
  * ({nrow, ncol, 1} = dense).  Shapes for Nt shooting nodes (all in the GP's standardised space;
  * the scaling of gp_class.py:253-262 is two elementwise CasADi expressions around F):
  *   z (Nx x Nt), sigma (Nx x Nx*Nt)  ->  mean (Ny x Nt), cov (Ny x Ny*Nt)
- *   jac_gp_b200(z, sigma, mean, cov) -> jac_mean_z, jac_mean_sigma (empty), jac_cov_z, jac_cov_sigma
- *   (block-diagonal: node t only depends on node t's inputs).
+ *   jac_gp_b200(z, sigma, mean, cov) -> jac_mean_z, jac_mean_sigma, jac_cov_z, jac_cov_sigma
+ *   (block-diagonal: node t only depends on node t's inputs).  jac_mean_sigma is empty for 'ME' / 'TA' and
+ *   Ny x Nx^2 per node for 'EM'; jac_cov_sigma is Ny^2 x Nx^2 per node for 'TA' and 'EM' (empty for 'ME');
+ *   column d + Nx*e holds d / d Sigma[d][e] with every other entry fixed.  'EM' values come from
+ *   gpmpc_predict_em_grad.
  *   jac_jac_gp_b200(z, sigma, mean, cov, jac_mean_z, jac_mean_sigma, jac_cov_z, jac_cov_sigma) -> 16 blocks of
  *   second derivatives (IPOPT's default exact Hessian; see below).
  */
@@ -25,6 +28,7 @@
 extern "C" {
 #endif
 
+/* method GPMPC_METHOD_ME, _TA or _EM; Nt shooting nodes per call.  GPMPC_ERR_ARG otherwise. */
 int gp_b200_bind(gpmpc_handle_t h, int method, int Nt);
 void gp_b200_unbind(void);
 
@@ -53,7 +57,8 @@ int jac_gp_b200(const double** arg, double** res, long long* iw, double* w, int 
  * out_jac_cov_z, out_jac_cov_sigma); outputs jac_jac_<o>_<i> for o in jac_gp_b200's outputs x i in its inputs
  * (output-major, 16).  Rows index the column-major dense vec of the differentiated Jacobian, columns the
  * dense vec of the input.  Nonzero: jac_mean_z/z, jac_cov_z/z and, for 'TA', jac_cov_z/sigma and
- * jac_cov_sigma/z (block-diagonal over the nodes); all other outputs are structurally empty. */
+ * jac_cov_sigma/z (block-diagonal over the nodes); all other outputs are structurally empty.  With 'EM' bound there
+ * are no second derivatives and jac_jac_gp_b200 returns failure (IPOPT: hessian_approximation 'limited-memory'). */
 long long jac_jac_gp_b200_n_in(void);
 long long jac_jac_gp_b200_n_out(void);
 const char* jac_jac_gp_b200_name_in(long long i);

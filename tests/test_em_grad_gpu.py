@@ -1,0 +1,252 @@
+"""gpmpc_predict_em_grad and GP.predict_batch_grad('EM') on the GPU: 'EM' first derivatives against the closed-form
+oracle fed with the engine's own alpha and factor, against fourth-order differences of the engine's own EM
+prediction, bit-identity of the forward outputs with gpmpc_predict(EM), exact symmetry, reproducibility, the
+K^-1 cache after append and the argument checks."""
+import ctypes as C
+
+import numpy as np
+import pytest
+
+from oracle import em_grad_oracle as emo
+from oracle import gp_oracle as orc
+from tests._util import load_fixture, load_golden, relinf
+
+pytestmark = pytest.mark.gpu
+
+DERIV = ('dmean_dz', 'dmean_dSigma', 'dcov_dz', 'dcov_dSigma')
+
+
+def _L():
+    import gp_mpc_b200
+    return gp_mpc_b200._lib
+
+
+def _fit(X, Y, hyper, **kw):
+    import gp_mpc_b200
+    eng = gp_mpc_b200.Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, **kw)
+    eng.set_data(X, Y)
+    eng.set_hyper(hyper)
+    eng.factorize()
+    return eng
+
+
+def _case(case):
+    if case.startswith('tank'):
+        m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
+        rng = np.random.default_rng(5)
+        Nx = X.shape[1]
+        Z = X[rng.choice(X.shape[0], 4, replace=False)] + 0.05 * rng.standard_normal((4, Nx))
+        A = rng.standard_normal((Nx, Nx)); Sigma = 1e-3 * np.eye(Nx) + 1e-4 * A @ A.T
+        if case == 'tank_large':          # about a tenth of the smallest length scale squared
+            Sigma = 0.1 * np.min(hyper[:, :Nx] ** 2) * (np.eye(Nx) + 0.1 * (A @ A.T) / np.abs(A @ A.T).max())
+        if case == 'tank_pp':
+            Sigma = np.stack([Sigma * (1 + 0.1 * h) for h in range(Z.shape[0])])
+        return X, Y, hyper, Z, Sigma
+    N, Nx, Ny, H = {'syn1000': (1000, 8, 4, 3), 'syn300': (300, 17, 2, 2)}[case]
+    p = orc.synthetic_problem(N, Nx, Ny, config_id=N + Nx, H=H)
+    return p['X'], p['Y'], p['hyper'], p['Z'], p['Sigma']
+
+
+def _engine_factor(eng, Ny):
+    L = _L()
+    return (np.stack([eng.get(L.GET_ALPHA, a) for a in range(Ny)]),
+            np.stack([eng.get(L.GET_CHOL, a) for a in range(Ny)]))
+
+
+@pytest.mark.parametrize('case', ['tank', 'tank_pp', 'tank_large', 'syn1000', 'syn300'])
+def test_em_grad_vs_closed_oracle(case):
+    """syn1000: Nx = 8, N ~ 1000 (16 tiles); syn300: Nx = 17, the 32 bucket; tank_pp: one Sigma per point."""
+    X, Y, hyper, Z, Sigma = _case(case)
+    Ny = Y.shape[1]
+    eng = _fit(X, Y, hyper)
+    L = _L()
+    o = eng.predict_em_grad(Z, Sigma)
+    mean, var, cov, _ = eng.predict(Z, Sigma, L.METHOD_EM, want_jac=False)
+    assert np.array_equal(o['mean'], mean) and np.array_equal(o['var'], var) and np.array_equal(o['cov'], cov)
+    for k in DERIV:
+        assert np.all(np.isfinite(o[k])), k
+    alpha, chol = _engine_factor(eng, Ny)
+    ref = emo.em_grad_closed(X, hyper, alpha, chol, Z, Sigma)
+    errs = {k: relinf(o[k], ref[k]) for k in DERIV}
+    assert errs['dmean_dz'] < 1e-6 and errs['dmean_dSigma'] < 1e-6, errs
+    assert errs['dcov_dz'] < 1e-5 and errs['dcov_dSigma'] < 1e-5, errs
+    assert np.array_equal(o['dmean_dSigma'], np.swapaxes(o['dmean_dSigma'], 2, 3))
+    assert np.array_equal(o['dcov_dSigma'], np.swapaxes(o['dcov_dSigma'], 3, 4))
+    assert np.array_equal(o['dcov_dSigma'], np.swapaxes(o['dcov_dSigma'], 1, 2))
+    assert np.array_equal(o['dcov_dz'], np.swapaxes(o['dcov_dz'], 1, 2))
+    o2 = eng.predict_em_grad(Z, Sigma)
+    for k in o:
+        assert np.array_equal(o[k], o2[k]), k
+    eng.close()
+
+
+@pytest.mark.parametrize('case,tol', [('tank', 1e-5), ('car', 1e-3)])
+def test_em_grad_vs_differences_of_the_engine(case, tol):
+    """Fourth-order differences of the engine's own gpmpc_predict(EM).  The car fixture (cond K ~ 1e10) gets 1e-3:
+    its EM covariance carries the alpha floor of DESIGN 4.8, which the differences amplify."""
+    m = load_fixture(case); X, Y, hyper = m['X'], m['Y'], m['hyper']
+    Nx, Ny = X.shape[1], Y.shape[1]
+    rng = np.random.default_rng(11)
+    Z = X[:2] + 0.05 * rng.standard_normal((2, Nx))
+    A = rng.standard_normal((Nx, Nx)); S = 1e-3 * np.eye(Nx) + 1e-4 * A @ A.T
+    eng = _fit(X, Y, hyper)
+    L = _L()
+    o = eng.predict_em_grad(Z, S)
+    for k in DERIV:
+        assert np.all(np.isfinite(o[k])), k
+
+    def f(Zp, Sp):
+        mean, _, cov, _ = eng.predict(Zp, Sp, L.METHOD_EM, want_jac=False)
+        return mean, cov
+
+    def d4(fun, h):
+        r = {k: fun(k * h) for k in (-2, -1, 1, 2)}
+        return [(r[-2][i] - 8 * r[-1][i] + 8 * r[1][i] - r[2][i]) / (12 * h) for i in range(2)]
+
+    dmz = np.zeros_like(o['dmean_dz']); dcz = np.zeros_like(o['dcov_dz'])
+    for d in range(Nx):
+        e = np.zeros(Nx); e[d] = 1.0
+        dmz[:, :, d], dcz[:, :, :, d] = d4(lambda s: f(Z + s * e, S), 3e-2)
+    dmS = np.zeros_like(o['dmean_dSigma']); dcS = np.zeros_like(o['dcov_dSigma'])
+    for d in range(Nx):
+        for e in range(d + 1):
+            E = np.zeros((Nx, Nx)); E[d, e] = E[e, d] = 1.0
+            dm, dc = d4(lambda s: f(Z, S + s * E), 3e-4)
+            dmS[:, :, d, e] = dmS[:, :, e, d] = dm
+            dcS[:, :, :, d, e] = dcS[:, :, :, e, d] = dc
+    assert relinf(o['dmean_dz'], dmz) < tol and relinf(o['dcov_dz'], dcz) < tol
+    assert relinf(emo.sym_pair(o['dmean_dSigma']), dmS) < tol
+    assert relinf(emo.sym_pair(o['dcov_dSigma']), dcS) < tol
+    eng.close()
+
+
+def test_em_grad_argument_checks():
+    L = _L(); lib = L.load()
+    m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
+    Ny, Nx = Y.shape[1], X.shape[1]
+    eng = _fit(X, Y, hyper)
+    Z = np.ascontiguousarray(X[:3] + 0.01)
+    S = 1e-3 * np.eye(Nx)
+    dp = C.POINTER(C.c_double)
+    rc = lib.gpmpc_predict_em_grad(eng.h, 3, Z.ctypes.data_as(dp), None, 0, *([None] * 7))
+    assert rc == L.ERR_ARG
+    with pytest.raises(L.GpmpcError) as e:
+        eng.predict_grad(Z, S, L.METHOD_EM)
+    assert e.value.code == L.ERR_ARG
+    full = eng.predict_em_grad(Z, S)
+    names = ('mean', 'var', 'cov') + DERIV
+    for k, name in enumerate(names):            # every output is optional: one at a time
+        out = np.empty_like(full[name])
+        ptrs = [None] * 7
+        ptrs[k] = out.ctypes.data_as(dp)
+        assert lib.gpmpc_predict_em_grad(eng.h, 3, Z.ctypes.data_as(dp), S.ctypes.data_as(dp), 0, *ptrs) == L.OK
+        assert np.array_equal(out, full[name]), name
+    eng.close()
+    part = _fit(X, Y, hyper, out_begin=0, out_count=Ny - 1)
+    with pytest.raises(L.GpmpcError) as e:
+        part.predict_em_grad(Z, S)
+    assert e.value.code == L.ERR_STATE
+    part.close()
+
+
+def test_em_grad_after_append_matches_a_refit():
+    """The cached K^-1 must follow gpmpc_append."""
+    m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
+    Nx = X.shape[1]
+    rng = np.random.default_rng(3)
+    Z = X[:3] + 0.05 * rng.standard_normal((3, Nx))
+    S = 1e-3 * np.eye(Nx)
+    eng = _fit(X[:-2], Y[:-2], hyper)
+    eng.predict_em_grad(Z, S)                   # builds the cache for the smaller model
+    assert eng.append(X[-2], Y[-2]) and eng.append(X[-1], Y[-1])
+    got = eng.predict_em_grad(Z, S)
+    eng.close()
+    ref_eng = _fit(X, Y, hyper)
+    ref = ref_eng.predict_em_grad(Z, S)
+    ref_eng.close()
+    for k in DERIV:
+        assert relinf(got[k], ref[k]) < 1e-8, k
+
+
+def test_gp_predict_batch_grad_em_vs_central_differences():
+    from tests.test_gpu_parity import _gp_from_fixture
+    gp, m = _gp_from_fixture('tank')
+    assert m['normalize']
+    d = load_golden('derived', 'tank')
+    xs = np.tile(d['x0'], (3, 1)) * (1 + 0.02 * np.arange(3)[:, None]); us = np.tile(d['u0'], (3, 1))
+    Sigma = d['Sigma']
+    g = gp.predict_batch_grad(xs, us, Sigma, method='EM')
+    mb, cb = gp.predict_batch(xs, us, Sigma, method='EM')
+    assert np.array_equal(g['mean'], mb) and np.array_equal(g['cov'], cb)
+    zs = np.hstack([xs, us])
+    Nx = zs.shape[1]
+    for e in range(Nx):
+        h = 1e-2 * max(1.0, abs(zs[0, e]))
+        r = {}
+        for k in (-2, -1, 1, 2):
+            zk = zs.copy(); zk[:, e] += k * h
+            r[k] = gp.predict_batch(zk[:, :4], zk[:, 4:], Sigma, method='EM')
+        fd = [(r[-2][i] - 8 * r[-1][i] + 8 * r[1][i] - r[2][i]) / (12 * h) for i in range(2)]
+        assert relinf(g['dmean_dz'][..., e], fd[0]) < 1e-5
+        assert relinf(g['dcov_dz'][..., e], fd[1]) < 1e-4
+    E = np.zeros((Nx, Nx)); E[0, 1] = E[1, 0] = 1.0
+    hs = 3e-4
+    r = {k: gp.predict_batch(xs, us, Sigma + k * hs * E, method='EM') for k in (-2, -1, 1, 2)}
+    fd = [(r[-2][i] - 8 * r[-1][i] + 8 * r[1][i] - r[2][i]) / (12 * hs) for i in range(2)]
+    assert relinf(g['dmean_dSigma'][..., 0, 1] + g['dmean_dSigma'][..., 1, 0], fd[0]) < 1e-4
+    assert relinf(g['dcov_dSigma'][..., 0, 1] + g['dcov_dSigma'][..., 1, 0], fd[1]) < 1e-4
+    gp.close()
+
+
+def _ccs(ptr):
+    nrow, ncol = ptr[0], ptr[1]
+    colind = [ptr[2 + k] for k in range(ncol + 1)]
+    rows = [ptr[2 + ncol + 1 + k] for k in range(colind[-1])]
+    return nrow, ncol, colind, rows
+
+
+def test_casadi_external_entry_points_with_em():
+    """gp_b200_bind(EM) driven through ctypes the way CasADi drives it: gp_b200 equals gpmpc_predict(EM), the CCS
+    nonzeros of jac_gp_b200 equal gpmpc_predict_em_grad (jac_mean_sigma and jac_cov_sigma block-diagonal, column
+    d + Nx*e <-> Sigma[d][e]), and jac_jac_gp_b200 reports failure."""
+    m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
+    Ny, Nx, Nt = Y.shape[1], X.shape[1], 4
+    eng = _fit(X, Y, hyper)
+    Lb = _L(); lib = Lb.load()
+    rng = np.random.default_rng(8)
+    Z = X[:Nt] + 0.1 * rng.standard_normal((Nt, Nx))
+    Sg = np.stack([1e-3 * np.eye(Nx) + 1e-4 * (lambda A: A @ A.T)(rng.standard_normal((Nx, Nx))) for _ in range(Nt)])
+    assert lib.gp_b200_bind(eng.h, Lb.METHOD_EM, Nt) == 0
+    dp = C.POINTER(C.c_double)
+
+    def call(fn, ins, outs):
+        arg = (dp * len(ins))(*[a.ctypes.data_as(dp) for a in ins])
+        res = (dp * len(outs))(*[a.ctypes.data_as(dp) for a in outs])
+        return fn(arg, res, None, None, 0)
+
+    z_cm = np.ascontiguousarray(Z)                                        # Nx x Nt column-major
+    s_cm = np.ascontiguousarray(np.transpose(Sg, (0, 2, 1)))               # Nx x Nx*Nt column-major
+    mean_cm = np.empty((Nt, Ny)); cov_cm = np.empty((Nt, Ny, Ny))
+    assert call(lib.gp_b200, [z_cm, s_cm], [mean_cm, cov_cm]) == 0
+    o = eng.predict_em_grad(Z, Sg)
+    assert np.array_equal(mean_cm, o['mean'])
+    assert np.array_equal(cov_cm, np.transpose(o['cov'], (0, 2, 1)))
+    pats = [_ccs(lib.jac_gp_b200_sparsity_out(k)) for k in range(4)]
+    assert [(p[0], p[1], p[2][-1]) for p in pats] == [
+        (Ny * Nt, Nx * Nt, Ny * Nx * Nt), (Ny * Nt, Nx * Nx * Nt, Ny * Nx * Nx * Nt),
+        (Ny * Ny * Nt, Nx * Nt, Ny * Ny * Nx * Nt), (Ny * Ny * Nt, Nx * Nx * Nt, Ny * Ny * Nx * Nx * Nt)]
+    outs = [np.zeros(p[2][-1]) for p in pats]
+    assert call(lib.jac_gp_b200, [z_cm, s_cm, mean_cm, cov_cm], outs) == 0
+    # nonzeros in pattern order: node t, column (d + Nx*e for Sigma), rows ascending (a, or a + Ny*b)
+    exp_mz = np.transpose(o['dmean_dz'], (0, 2, 1)).reshape(-1)                        # t, d, a
+    exp_ms = np.transpose(o['dmean_dSigma'], (0, 3, 2, 1)).reshape(-1)                 # t, e, d, a
+    exp_cz = np.transpose(o['dcov_dz'], (0, 3, 2, 1)).reshape(-1)                      # t, e, b, a
+    exp_cs = np.transpose(o['dcov_dSigma'], (0, 4, 3, 2, 1)).reshape(-1)               # t, e, d, b, a
+    for got, exp in zip(outs, (exp_mz, exp_ms, exp_cz, exp_cs)):
+        assert np.array_equal(got, exp)
+    jj = [_ccs(lib.jac_jac_gp_b200_sparsity_out(k)) for k in range(16)]
+    jins = [z_cm, s_cm, mean_cm, cov_cm] + [np.zeros(max(1, p[2][-1])) for p in pats]
+    assert call(lib.jac_jac_gp_b200, jins, [np.zeros(max(1, p[2][-1])) for p in jj]) != 0
+    lib.gp_b200_unbind()
+    assert not lib.jac_gp_b200_sparsity_out(0)
+    eng.close()
