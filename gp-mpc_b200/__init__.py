@@ -9,6 +9,6 @@ Import name: ``gp_mpc_b200`` (the directory is ``gp-mpc_b200/``; the repo-root m
 from . import _lib, optimize, partition            # noqa: F401
 from ._lib import Engine, GpmpcError                # noqa: F401
 from .comm import Comm                              # noqa: F401
-from .gp_class import GP                            # noqa: F401
+from .gp_class import GP, lqr                       # noqa: F401
 
-__all__ = ['GP', 'Engine', 'Comm', 'GpmpcError', 'optimize', 'partition']
+__all__ = ['GP', 'lqr', 'Engine', 'Comm', 'GpmpcError', 'optimize', 'partition']

@@ -44,6 +44,7 @@ SYMBOLS = [
     ('gpmpc_append', C.c_int, [_H, _dp, _dp]),
     ('gpmpc_posterior_cov', C.c_int, [_H, C.c_int, _dp, _dp]),
     ('gpmpc_rollout', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
+    ('gpmpc_rollout_batch', C.c_int, [_H, C.c_int, C.c_int, C.c_int] + [_dp] * 10),
     ('gpmpc_predict_device', C.c_int, [_H, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     ('gpmpc_get', C.c_int, [_H, C.c_int, C.c_int, _dp]),
@@ -256,6 +257,27 @@ class Engine:
         means = np.empty((Nt, self.Ny)); var = np.empty((Nt, self.Ny)); cov = np.empty((self.Ny, self.Ny))
         self._check(self.lib.gpmpc_rollout(self.h, int(method), Nt, _ptr(z0), _ptr(U) if Nu > 0 else None, _ptr(Sigma0),
                                            _ptr(scale), _ptr(means), _ptr(var), _ptr(cov)))
+        return means, var, cov
+
+    def rollout_batch(self, z0, U, Sigma0, method=METHOD_TA, scale=None, K=None, x_ref=None, uscale=None):
+        """gpmpc_rollout_batch: B trajectories of Nt steps in one pass, open loop or with the feedback u = K (x - x_ref).
+        z0:(B,Nx), U:(B,Nt,Nu) (GP input units; with K only its shape is used), Sigma0:(B,Nx,Nx), scale:(4,Ny)|None,
+        K:(Nu,Ny)|None, x_ref:(Ny,)|None, uscale:(2,Nu)|None -> means (B,Nt,Ny), vars (B,Nt,Ny), cov_last (B,Ny,Ny)."""
+        Nu = self.Nx - self.Ny
+        z0 = _f64(z0).reshape(-1, self.Nx)
+        B = z0.shape[0]
+        Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
+        Nt = int(np.shape(U)[1])
+        U = _f64(U, (B, Nt, Nu)) if (Nu > 0 and K is None) else None
+        if scale is not None:
+            scale = _f64(scale, (4, self.Ny))
+        if K is not None:
+            K = _f64(K, (Nu, self.Ny))
+            x_ref = None if x_ref is None else _f64(x_ref, (self.Ny,))
+            uscale = None if uscale is None else _f64(uscale, (2, Nu))
+        means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
+        self._check(self.lib.gpmpc_rollout_batch(self.h, int(method), B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale),
+                                                 _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means), _ptr(var), _ptr(cov)))
         return means, var, cov
 
     def predict_grad(self, Z, Sigma=None, method=METHOD_TA, want_hess=False):

@@ -103,7 +103,7 @@ struct gpmpc_handle_s {
     DevBuf<double> dDR, dVD, dPG, dPB2, dPM3, dHessOut;
     DevBuf<double> dG;
     double *dZ = nullptr, *dSigma = nullptr, *dMean = nullptr, *dVar = nullptr, *dJ = nullptr, *dCov = nullptr;   // in dIn / dOut
-    DevBuf<double> dRoll;             // gpmpc_rollout: [Z | Sigma | U | scale | means | vars | cov]
+    DevBuf<double> dRoll;             // gpmpc_rollout_batch: [Z | Sigma | U | scale | K | x_ref | uscale | means | vars | cov]
     DevBuf<double> dIn, dOut;         // [Z | Sigma] and [mean | var | J | cov] slabs: one H2D + one D2H per host call
     int Hcap = 0;                     // test points the slab layout behind dZ .. dCov holds (0: not laid out)
     double* hPinned = nullptr; double* dPinnedAlias = nullptr; size_t hPinnedBytes = 0;
@@ -1474,80 +1474,145 @@ extern "C" int gpmpc_predict_device(gpmpc_handle_t h, int method, int H, const d
 }
 
 // ------------------------------------------------------------------------------------
-// Open-loop multi-step prediction with the state kept on the device (GP.rollout = the numeric loop of
+// Multi-step prediction of B trajectories with the state kept on the device (GP.rollout = the numeric loop of
 // predict_compare, gp_class.py:746-804).  The host loop pays a call (launches + sync + copies + Python) per step
-// although a step's device work at MPC sizes is tens of microseconds; here all Nt steps are enqueued back to back:
-//   z_t = [ (mean_{t-1} sY + mY - mX) / sX , u_{t-1} ],  Sigma_t = [cov_{t-1} 0; 0 Sigma_uu]  ->  (mean_t, cov_t)
-// with the reference's operation order (gp_class.py:629-638), so the trajectory is the host loop's bit for bit.
+// although a step's device work at MPC sizes is tens of microseconds; here all Nt steps are enqueued back to back, each one
+// predict pass over the B current inputs (H = B, one Sigma per point):
+//   open loop:  z_t = [ (mean_{t-1} sY + mY - mX) / sX , u_{t-1} ],  Sigma_t = [cov_{t-1} Sigma_xu; Sigma_ux Sigma_uu] (u blocks kept)
+//   feedback:   x = mean_{t-1} sY + mY,  u = K (x - x_ref) [then (u - mU) / sU],  Sigma_uu = K cov K^T,  Sigma_xu = cov K^T
+//               (gp_class.py:770-804 with the LQR gain of mpc_class.py:956-976; cov stays in the GP's units, q4)
+// with the reference's operation order (gp_class.py:629-638), so the trajectory is the host loop's bit for bit in open loop.
 // ------------------------------------------------------------------------------------
+// One CTA per trajectory b.  Dynamic shared memory with K: x (Ny) | K cov (Nu x Ny).
 __global__ void __launch_bounds__(256)
 rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restrict__ cov_t, const double* __restrict__ u_t,
-                        const double* __restrict__ scale, int Ny, int Nu, double* __restrict__ Z, double* __restrict__ Sigma)
+                        long long u_stride, const double* __restrict__ scale, const double* __restrict__ K,
+                        const double* __restrict__ x_ref, const double* __restrict__ uscale, int Ny, int Nu,
+                        double* __restrict__ Z, double* __restrict__ Sigma)
 {
-    const int Nx = Ny + Nu, tid = threadIdx.x;
+    extern __shared__ double fb_sh[];
+    const int Nx = Ny + Nu, tid = threadIdx.x, b = blockIdx.x;
+    mean_t += (size_t)b * Ny; cov_t += (size_t)b * Ny * Ny;
+    Z += (size_t)b * Nx; Sigma += (size_t)b * Nx * Nx;
     for (int j = tid; j < Nx; j += 256) {
         if (j < Ny) {
-            double z = mean_t[j];
+            double z = mean_t[j], x = z;
             if (scale) {                                     // [sY | mY | mX | sX]; no fused multiply-add: numpy does not fuse
-                const double x = __dadd_rn(__dmul_rn(z, scale[j]), scale[Ny + j]);
+                x = __dadd_rn(__dmul_rn(z, scale[j]), scale[Ny + j]);
                 z = __ddiv_rn(__dsub_rn(x, scale[2 * Ny + j]), scale[3 * Ny + j]);
             }
             Z[j] = z;
-        } else {
-            Z[j] = u_t[j - Ny];
+            if (K) fb_sh[j] = x;
+        } else if (!K) {
+            Z[j] = u_t[(size_t)b * u_stride + (j - Ny)];
         }
     }
     for (int idx = tid; idx < Ny * Ny; idx += 256) {
         const int r = idx / Ny, c = idx - r * Ny;
         Sigma[r * Nx + c] = cov_t[idx];
     }
+    if (!K) return;                                          // uniform over the CTA
+    double* KC = fb_sh + Ny;
+    __syncthreads();
+    // u = K (x - x_ref), standardised as GP.predict standardises its input
+    for (int i = tid; i < Nu; i += 256) {
+        double u = 0.0;
+        for (int k = 0; k < Ny; ++k) u = __dadd_rn(u, __dmul_rn(K[i * Ny + k], x_ref ? __dsub_rn(fb_sh[k], x_ref[k]) : fb_sh[k]));
+        if (uscale) u = __ddiv_rn(__dsub_rn(u, uscale[i]), uscale[Nu + i]);
+        Z[Ny + i] = u;
+    }
+    // K cov (kept for Sigma_uu = (K cov) K^T) and Sigma_xu = cov K^T, Sigma_ux = Sigma_xu^T
+    for (int idx = tid; idx < Nu * Ny; idx += 256) {
+        const int i = idx / Ny, c = idx - i * Ny;
+        double s = 0.0;
+        for (int k = 0; k < Ny; ++k) s = __dadd_rn(s, __dmul_rn(K[i * Ny + k], cov_t[k * Ny + c]));
+        KC[idx] = s;
+    }
+    for (int idx = tid; idx < Ny * Nu; idx += 256) {
+        const int r = idx / Nu, i = idx - r * Nu;
+        double s = 0.0;
+        for (int k = 0; k < Ny; ++k) s = __dadd_rn(s, __dmul_rn(cov_t[r * Ny + k], K[i * Ny + k]));
+        Sigma[r * Nx + Ny + i] = s;
+        Sigma[(Ny + i) * Nx + r] = s;
+    }
+    __syncthreads();
+    for (int idx = tid; idx < Nu * Nu; idx += 256) {
+        const int i = idx / Nu, j = idx - i * Nu;
+        double s = 0.0;
+        for (int k = 0; k < Ny; ++k) s = __dadd_rn(s, __dmul_rn(KC[i * Ny + k], K[j * Ny + k]));
+        Sigma[(Ny + i) * Nx + Ny + j] = s;
+    }
 }
 
-extern "C" int gpmpc_rollout(gpmpc_handle_t h, int method, int Nt, const double* z0, const double* U, const double* Sigma0,
-                             const double* scale, double* means, double* vars, double* cov_last)
+extern "C" int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, const double* z0, const double* U,
+                                   const double* Sigma0, const double* scale, const double* K, const double* x_ref,
+                                   const double* uscale, double* means, double* vars, double* cov_last)
 {
     int rc = predict_check(h, method, 1);
     if (rc) return rc;
     const int Nx = h->Nx, Ny = h->Ny, Nu = Nx - Ny;
     if (method == GPMPC_METHOD_EM) { set_error(h, "gpmpc_rollout: methods ME and TA (EM prepares every point on the host)"); return GPMPC_ERR_ARG; }
-    if (Nt < 1 || !z0 || !Sigma0 || !means || !vars || (Nu > 0 && !U)) { set_error(h, "gpmpc_rollout: null argument / Nt < 1"); return GPMPC_ERR_ARG; }
+    if (B < 1 || Nt < 1 || !z0 || !Sigma0 || !means || !vars || (Nu > 0 && !K && !U)) { set_error(h, "gpmpc_rollout: null argument / B < 1 / Nt < 1"); return GPMPC_ERR_ARG; }
     if (Nu < 0) { set_error(h, "gpmpc_rollout: needs Nx = Ny + Nu with Nu >= 0 (Nx=%d, Ny=%d)", Nx, Ny); return GPMPC_ERR_ARG; }
+    if (K && Nu == 0) { set_error(h, "gpmpc_rollout: a feedback gain needs inputs (Nu = 0)"); return GPMPC_ERR_ARG; }
     if (h->world != 1 || h->nloc != Ny) { set_error(h, "gpmpc_rollout: all outputs must live on this handle"); return GPMPC_ERR_STATE; }
     CUDA_TRY(cudaSetDevice(h->device));
-    rc = ensure_predict_bufs(h, 1);
+    rc = ensure_predict_bufs(h, B);
     if (rc) return rc;
     NvtxRange nvtx_r("gpmpc.rollout");
-    // device slab: [Z | Sigma | U | scale | means | vars | cov], host mirror in the pinned buffer
-    const size_t o_sig = Nx, o_u = o_sig + (size_t)Nx * Nx, o_sc = o_u + (size_t)Nt * Nu, o_m = o_sc + 4 * (size_t)Ny;
-    const size_t o_v = o_m + (size_t)Nt * Ny, o_c = o_v + (size_t)Nt * Ny, tot = o_c + (size_t)Nt * Ny * Ny;   // one cov per step
+    // device slab: [Z (B,Nx) | Sigma (B,Nx,Nx) | U (B,Nt,Nu) | scale (4,Ny) | K (Nu,Ny) | x_ref (Ny) | uscale (2,Nu) |
+    //               means (Nt,B,Ny) | vars (Nt,B,Ny) | cov (Nt,B,Ny,Ny)], host mirror in the pinned buffer.  Step t reads
+    //               and writes B consecutive points, so its outputs are one (B,...) block.
+    const size_t Bs = (size_t)B, nU = U && !K ? Bs * Nt * Nu : 0;
+    const size_t o_sig = Bs * Nx, o_u = o_sig + Bs * Nx * Nx, o_sc = o_u + nU, o_k = o_sc + 4 * (size_t)Ny;
+    const size_t o_xr = o_k + (size_t)Nu * Ny, o_us = o_xr + Ny, o_m = o_us + 2 * (size_t)Nu;
+    const size_t o_v = o_m + (size_t)Nt * Bs * Ny, o_c = o_v + (size_t)Nt * Bs * Ny, tot = o_c + (size_t)Nt * Bs * Ny * Ny;
     ENSURE(h->dRoll, tot);
     rc = ensure_pinned(h, tot * 8);
     if (rc) return rc;
     double* pin = h->hPinned;
-    memcpy(pin, z0, (size_t)Nx * 8);
-    memcpy(pin + o_sig, Sigma0, (size_t)Nx * Nx * 8);
-    if (Nu > 0) memcpy(pin + o_u, U, (size_t)Nt * Nu * 8);
+    memcpy(pin, z0, Bs * Nx * 8);
+    memcpy(pin + o_sig, Sigma0, Bs * Nx * Nx * 8);
+    if (nU) memcpy(pin + o_u, U, nU * 8);
     if (scale) memcpy(pin + o_sc, scale, 4 * (size_t)Ny * 8);
+    if (K) memcpy(pin + o_k, K, (size_t)Nu * Ny * 8);
+    if (K && x_ref) memcpy(pin + o_xr, x_ref, (size_t)Ny * 8);
+    if (K && uscale) memcpy(pin + o_us, uscale, 2 * (size_t)Nu * 8);
     CUDA_TRY(cudaMemcpyAsync(h->dRoll, pin, o_m * 8, cudaMemcpyHostToDevice, h->st));
     double* d = h->dRoll;
+    const int fb_smem = K ? (Ny + Nu * Ny) * 8 : 0;
     for (int t = 0; t < Nt; ++t) {
-        double* cov_t = d + o_c + (size_t)t * Ny * Ny;
-        rc = predict_core(h, method, 1, d, d + o_sig, 0, d + o_m + (size_t)t * Ny, d + o_v + (size_t)t * Ny, cov_t, nullptr);
+        double* cov_t = d + o_c + (size_t)t * Bs * Ny * Ny;
+        rc = predict_core(h, method, B, d, d + o_sig, 1, d + o_m + (size_t)t * Bs * Ny, d + o_v + (size_t)t * Bs * Ny, cov_t, nullptr);
         if (rc) return rc;
         if (t + 1 < Nt) {
-            rollout_feedback_kernel<<<1, 256, 0, h->st>>>(d + o_m + (size_t)t * Ny, cov_t, d + o_u + (size_t)(t + 1) * Nu,
-                                                          scale ? d + o_sc : nullptr, Ny, Nu, d, d + o_sig);
+            rollout_feedback_kernel<<<B, 256, fb_smem, h->st>>>(d + o_m + (size_t)t * Bs * Ny, cov_t, d + o_u + (size_t)(t + 1) * Nu,
+                                                                (long long)Nt * Nu, scale ? d + o_sc : nullptr, K ? d + o_k : nullptr,
+                                                                K && x_ref ? d + o_xr : nullptr, K && uscale ? d + o_us : nullptr,
+                                                                Ny, Nu, d, d + o_sig);
             CUDA_TRY(cudaGetLastError());
         }
     }
     CUDA_TRY(cudaMemcpyAsync(pin + o_m, d + o_m, (tot - o_m) * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
-    memcpy(means, pin + o_m, (size_t)Nt * Ny * 8);
-    // the reference records diag(covar_x) of every step (gp_class.py:793): the propagated variance, JSigmaJ^T included
-    for (int t = 0; t < Nt; ++t)
-        for (int a = 0; a < Ny; ++a) vars[(size_t)t * Ny + a] = pin[o_c + (size_t)t * Ny * Ny + (size_t)a * Ny + a];
-    if (cov_last) memcpy(cov_last, pin + o_c + (size_t)(Nt - 1) * Ny * Ny, (size_t)Ny * Ny * 8);
+    // (t, b) -> (b, t); the reference records diag(covar_x) of every step (gp_class.py:793): the propagated variance, J Sigma J^T included
+    for (size_t b = 0; b < Bs; ++b)
+        for (int t = 0; t < Nt; ++t) {
+            const size_t src = (size_t)t * Bs + b, dst = b * Nt + t;
+            memcpy(means + dst * Ny, pin + o_m + src * Ny, (size_t)Ny * 8);
+            for (int a = 0; a < Ny; ++a) vars[dst * Ny + a] = pin[o_c + src * Ny * Ny + (size_t)a * Ny + a];
+        }
+    if (cov_last)
+        for (size_t b = 0; b < Bs; ++b)
+            memcpy(cov_last + b * Ny * Ny, pin + o_c + ((size_t)(Nt - 1) * Bs + b) * Ny * Ny, (size_t)Ny * Ny * 8);
     return GPMPC_OK;
+}
+
+// the single open-loop trajectory: B = 1 of the batched loop
+extern "C" int gpmpc_rollout(gpmpc_handle_t h, int method, int Nt, const double* z0, const double* U, const double* Sigma0,
+                             const double* scale, double* means, double* vars, double* cov_last)
+{
+    return gpmpc_rollout_batch(h, method, 1, Nt, z0, U, Sigma0, scale, nullptr, nullptr, nullptr, means, vars, cov_last);
 }
 
 extern "C" int gpmpc_predict(gpmpc_handle_t h, int method, int H, const double* Z, const double* Sigma,

@@ -21,6 +21,7 @@ import json
 import os
 
 import numpy as np
+import scipy.linalg
 
 from . import _lib
 from .comm import Comm
@@ -30,6 +31,27 @@ from .partition import choose_mode, output_block, point_block
 
 _GPU_METHODS = {'ME': _lib.METHOD_ME, 'TA': _lib.METHOD_TA, 'EM': _lib.METHOD_EM}
 _KNOWN_METHODS = ('ME', 'TA', 'EM', 'old_ME', 'old_TA')      # gp_class.py:197-205
+
+
+def _matmul_seq(A, B):
+    """A @ B with every sum in index order and separate multiplies and adds, as rollout_feedback_kernel forms the
+    feedback products.  BLAS's order and use of fused multiply-adds differ between builds, and a closed loop amplifies
+    one rounding step (1e-10 on the car model), so the host loop and the device roll-out share this order."""
+    out = np.zeros((A.shape[0], B.shape[1]))
+    for k in range(A.shape[1]):
+        out = out + A[:, k:k + 1] * B[k:k + 1, :]
+    return out
+
+
+def lqr(A, B, Q, R):
+    """ Infinite-horizon discrete-time LQR for x[k+1] = A x[k] + B u[k], u[k] = K x[k] (the reference's
+    ``lqr``, mpc_class.py:956-976): P solves the discrete algebraic Riccati equation and
+    K = -(R + B^T P B)^-1 B^T P A.  Returns K (Nu, Ny), P and the eigenvalues of A + B K. """
+    A = np.asarray(A, dtype=np.float64); B = np.asarray(B, dtype=np.float64)
+    P = scipy.linalg.solve_discrete_are(A, B, np.asarray(Q, dtype=np.float64), np.asarray(R, dtype=np.float64))
+    BtP = B.T @ P
+    K = -np.linalg.solve(R + BtP @ B, BtP @ A)
+    return K, P, np.linalg.eigvals(A + B @ K)
 
 
 def _is_symbolic(v):
@@ -444,57 +466,132 @@ class GP:
                                      None if cov is None else np.asarray(cov, dtype=np.float64))
         return mean.reshape(self.__Ny, 1), c[0]
 
-    def rollout(self, x0, u, methods=None, device_rollout=True):
-        """ The numeric multi-step prediction of ``predict_compare`` (reference
-        gp_class.py:746-804, open-loop branch) without the plotting / plant simulation:
-        for every method, propagate (mean, covariance) through ``predict`` over the input
-        sequence u:(Nt,Nu), starting from x0 with covariance diag(sn2) (+1e-6 on the inputs).
-        Returns mean, var of shape (len(methods), Nt+1, Ny); var is rescaled by stdY^2 when
-        normalize (:795-796)."""
-        Nx, Ny = self.__Nx, self.__Ny
+    def rollout(self, x0, u, methods=None, device_rollout=True, feedback=False, x_ref=None, Q=None, R=None):
+        """ The numeric multi-step prediction of ``predict_compare`` (reference gp_class.py:746-804)
+        without the plotting / plant simulation: for every method, propagate (mean, covariance)
+        through ``predict`` over the input sequence u:(Nt,Nu), starting from x0 with covariance
+        diag(sn2) (+1e-6 on the inputs).  Returns mean, var of shape (len(methods), Nt+1, Ny); var
+        is rescaled by stdY^2 when normalize (:795-796).
+
+        feedback=True is the reference's closed-loop branch (:770-804): the GP is linearised at
+        (x0, u[0]) (``discrete_linearize``), ``lqr(A, B, Q, R)`` gives K, and every step applies
+        u_t = K (mean_t - x_ref) with the input covariance blocks Sigma_uu = K cov K^T and
+        Sigma_xu = cov K^T; u then only sets Nt and the linearisation point.  Defaults as in the
+        reference: Q = I_Ny, R = I_Nu, x_ref = 0.  Like the reference, K (caller units) acts on the
+        GP's standardised covariance (q4).
+
+        A batch x0:(B,Ny) with u:(B,Nt,Nu) gives mean, var of shape (len(methods), B, Nt+1, Ny);
+        trajectory b is what x0[b], u[b] give alone (its own covariance chain and, with feedback,
+        its own gain).  'ME' / 'TA' on a single handle run on the device (gpmpc_rollout_batch: one
+        predict pass over all trajectories per step, one pass per distinct gain with feedback);
+        'EM', sharded models and prior_mean_in_predict keep the host loop."""
+        Nx, Ny, Nu = self.__Nx, self.__Ny, self.__Nu
+        x0 = np.asarray(x0, dtype=np.float64)
+        single = x0.ndim < 2
+        X0 = x0.reshape(1, Ny) if single else x0.reshape(-1, Ny)
+        nb = X0.shape[0]
         u = np.asarray(u, dtype=np.float64)
-        u = u.reshape(-1, self.__Nu) if self.__Nu > 0 else np.zeros((u.shape[0] if u.ndim else 0, 0))   # Nu = 0: Nt = len(u)
-        Nt = u.shape[0]
+        if single:
+            U = (u.reshape(-1, Nu) if Nu > 0 else np.zeros((u.shape[0] if u.ndim else 0, 0)))[None]   # Nu = 0: Nt = len(u)
+        else:
+            U = u.reshape(nb, -1, Nu) if Nu > 0 else np.zeros((nb, u.shape[1] if u.ndim > 1 else 0, 0))
+        Nt = U.shape[1]
+        if feedback:
+            if Nu == 0:
+                raise ValueError('rollout(feedback=True) needs a model with inputs (Nu > 0)')
+            Q = np.eye(Ny) if Q is None else np.asarray(Q, dtype=np.float64)      # gp_class.py:760-766
+            R = np.eye(Nu) if R is None else np.asarray(R, dtype=np.float64)
+            x_ref = np.zeros(Ny) if x_ref is None else np.asarray(x_ref, dtype=np.float64).reshape(Ny)
         initVar = self.__hyper[:, Nx + 1] ** 2
         if methods is None:                             # gp_class.py:747 default; 'EM' only where it can run
             methods = ['TA', 'ME'] if self.__sharded_outputs() else ['EM', 'TA', 'ME']
         methods = list(methods)
-        mean = np.zeros((len(methods), Nt + 1, Ny))
-        var = np.zeros((len(methods), Nt + 1, Ny))
-        covar = np.eye(Nx) * 1e-6                       # shared across methods, as in the reference
+        mean = np.zeros((len(methods), nb, Nt + 1, Ny))
+        var = np.zeros((len(methods), nb, Nt + 1, Ny))
+        # one input covariance per trajectory, shared across methods as in the reference: with feedback, method i+1
+        # starts from the Sigma_uu / Sigma_xu blocks that method i left behind (gp_class.py:764, :797-801)
+        covar = np.tile(np.eye(Nx) * 1e-6, (nb, 1, 1))
         keep = self.__gp_method
-        # 'ME' / 'TA' on a single handle: all Nt steps run on the device (gpmpc_rollout), same arithmetic as the loop below
-        on_device = (device_rollout and hasattr(self.__engine, 'rollout') and self.__comm.world == 1
+        # 'ME' / 'TA' on a single handle: all Nt steps run on the device, same arithmetic as the loop below
+        on_device = (device_rollout and self.__comm.world == 1
                      and not (self.__prior_mean_in_predict and self.__has_prior_mean()))
         for i, meth in enumerate(methods):
             self.set_method(meth)
-            mean_t = np.asarray(x0, dtype=np.float64).reshape(-1)
-            covar[:Ny, :Ny] = np.diag(initVar)
-            mean[i, 0, :] = mean_t
-            if on_device and meth in ('ME', 'TA') and Nt > 0:
-                un = u
-                z_x = mean_t
-                scale = None
-                if self.__normalize:
-                    z_x = self.standardize(mean_t, self.__meanX, self.__stdX)
-                    un = self.standardize(u, self.__meanU, self.__stdU)
-                    scale = np.stack([self.__stdY, self.__meanY, self.__meanX, self.__stdX])
-                z0 = np.concatenate([np.asarray(z_x, dtype=np.float64).reshape(-1), un[0].reshape(-1)])
-                m_std, v_std, c_last = self.__engine.rollout(z0, un, covar, _GPU_METHODS[meth], scale)
-                mean[i, 1:, :] = self.inverse_mean(m_std, self.__meanY, self.__stdY) if self.__normalize else m_std
-                var[i, 1:, :] = self.inverse_variance(v_std) if self.__normalize else v_std
-                covar[:Ny, :Ny] = c_last
+            covar[:, :Ny, :Ny] = np.diag(initVar)
+            mean[i, :, 0, :] = X0
+            K = self.__lqr_gains(X0, U[:, 0], Q, R) if feedback else None      # once per method, as the reference
+            if on_device and meth in ('ME', 'TA') and Nt > 0 and self.__rollout_device(i, meth, X0, U, covar, K, x_ref,
+                                                                                      single, mean, var):
                 continue
-            for t in range(1, Nt + 1):
-                mean_t, covar_x = self.predict(mean_t, u[t - 1, :], covar)
-                mean_t = np.array(mean_t).reshape(Ny)
-                mean[i, t, :] = mean_t
-                var[i, t, :] = np.diag(covar_x)
-                if self.__normalize:
-                    var[i, t, :] = self.inverse_variance(var[i, t, :])
-                covar[:Ny, :Ny] = covar_x
+            for b in range(nb):
+                mean_t = X0[b]
+                cv = covar[b]
+                for t in range(1, Nt + 1):
+                    u_t = _matmul_seq(K[b], (mean_t - x_ref)[:, None])[:, 0] if feedback else U[b, t - 1, :]
+                    mean_t, covar_x = self.predict(mean_t, u_t, cv)
+                    mean_t = np.array(mean_t).reshape(Ny)
+                    mean[i, b, t, :] = mean_t
+                    var[i, b, t, :] = np.diag(covar_x)
+                    if self.__normalize:
+                        var[i, b, t, :] = self.inverse_variance(var[i, b, t, :])
+                    if feedback:
+                        self.__feedback_blocks(cv, K[b], covar_x)
+                    cv[:Ny, :Ny] = covar_x
         self.set_method(keep)
+        if single:
+            return mean[:, 0], var[:, 0]
         return mean, var
+
+    def __lqr_gains(self, X0, U0, Q, R):
+        """The reference's K = lqr(discrete_linearize(x0, u[0]))[0] for every trajectory: (B, Nu, Ny)."""
+        Ks = []
+        for b in range(X0.shape[0]):
+            A, Bm = self.discrete_linearize(X0[b], U0[b], None)
+            Ks.append(lqr(A, Bm, Q, R)[0])
+        return np.stack(Ks)
+
+    def __feedback_blocks(self, cv, K, covar_x):
+        """gp_class.py:797-801: the input blocks of the next step's covariance under u = K x."""
+        Ny = self.__Ny
+        cov_xu = _matmul_seq(covar_x, K.T)
+        cv[Ny:, Ny:] = _matmul_seq(_matmul_seq(K, covar_x), K.T)
+        cv[Ny:, :Ny] = cov_xu.T
+        cv[:Ny, Ny:] = cov_xu
+
+    def __rollout_device(self, i, meth, X0, U, covar, K, x_ref, single, mean, var):
+        """Method i of every trajectory on the device; False when the engine has no roll-out entry for the case."""
+        eng, nb = self.__engine, X0.shape[0]
+        use_single = single and K is None and hasattr(eng, 'rollout')       # gpmpc_rollout, the one open-loop trajectory
+        if not (use_single or hasattr(eng, 'rollout_batch')):
+            return False
+        zx, un, scale, uscale = X0, U, None, None
+        if K is not None:
+            un = np.stack([_matmul_seq(K[b], (X0[b] - x_ref)[:, None])[:, 0] for b in range(nb)])[:, None, :]   # the loop's first u_t
+        if self.__normalize:
+            zx = self.standardize(X0, self.__meanX, self.__stdX)
+            un = self.standardize(un, self.__meanU, self.__stdU)
+            scale = np.stack([self.__stdY, self.__meanY, self.__meanX, self.__stdX])
+            uscale = np.stack([self.__meanU, self.__stdU])
+        z0 = np.concatenate([zx, un[:, 0, :]], 1)
+        method = _GPU_METHODS[meth]
+        if use_single:
+            parts = [(np.arange(1),) + tuple(r[None] for r in eng.rollout(z0[0], un[0], covar[0], method, scale))]
+        elif K is None:
+            parts = [(np.arange(nb),) + tuple(eng.rollout_batch(z0, un, covar, method, scale))]
+        else:                                            # one pass per distinct gain
+            groups = {}
+            for b in range(nb):
+                groups.setdefault(K[b].tobytes(), []).append(b)
+            parts = [(g,) + tuple(eng.rollout_batch(z0[g], U[g], covar[g], method, scale, K[g[0]], x_ref, uscale))
+                     for g in map(np.array, groups.values())]
+        for g, m_std, v_std, c_last in parts:
+            mean[i, g, 1:, :] = self.inverse_mean(m_std, self.__meanY, self.__stdY) if self.__normalize else m_std
+            var[i, g, 1:, :] = self.inverse_variance(v_std) if self.__normalize else v_std
+            for k, b in enumerate(g):
+                if K is not None:
+                    self.__feedback_blocks(covar[b], K[b], c_last[k])
+                covar[b, :self.__Ny, :self.__Ny] = c_last[k]
+        return True
 
     def get_size(self):
         """ (N, Ny, Nu)  (reference gp_class.py:266-274) """

@@ -179,9 +179,30 @@ int gpmpc_predict_em_grad(gpmpc_handle_t h, int H, const double* Z, const double
  *                       inverse_mean / standardize pair of gp_class.py:629-638 in the same operation order
  *   means, vars (Nt, Ny) predicted means / diag(cov_t) (the propagated variance the reference records, gp_class.py:793)
  *                       in the GP's output units, cov_last (Ny, Ny) or NULL
- * method GPMPC_METHOD_ME or _TA; the handle must own all outputs. */
+ * method GPMPC_METHOD_ME or _TA; the handle must own all outputs.  Same as gpmpc_rollout_batch with B = 1, K = NULL. */
 int gpmpc_rollout(gpmpc_handle_t h, int method, int Nt, const double* z0, const double* U, const double* Sigma0,
                   const double* scale, double* means, double* vars, double* cov_last);
+
+/* gpmpc_rollout for B trajectories in one pass, optionally closed-loop: the feedback branch of GP.predict_compare
+ * (gp_class.py:770-804) with a gain K from the reference's lqr (mpc_class.py:956-976: DARE, K = -(R + B^T P B)^-1 B^T P A).
+ * Each step is one predict pass over the B current inputs (H = B, one Sigma per trajectory); a kernel then forms every
+ * trajectory's next input and covariance.  With K, after step t (x = mean_t * stdY + meanY, or mean_t without scale):
+ *   u = K (x - x_ref), then (u - meanU) / stdU when uscale is given  (the caller's units, as GP.predict standardises u)
+ *   Sigma_uu = K cov_t K^T,  Sigma_xu = cov_t K^T,  Sigma_ux = Sigma_xu^T,  then cov_t into the top-left block
+ * with cov_t in the GP's output units, as the reference does (q4).  Without K the inputs come from U as in gpmpc_rollout and
+ * the u blocks of Sigma are kept.
+ *   z0      (B, Nx)       first inputs [x_0, u_0] in the GP's input units (with K: u_0 = K (x_0 - x_ref), standardised)
+ *   U       (B, Nt, Nu)   open-loop inputs, GP input units; NULL when Nu = 0 or K is given
+ *   Sigma0  (B, Nx, Nx)   input covariance of each trajectory's first step
+ *   scale   (4, Ny)       [stdY | meanY | meanX | stdX] or NULL, as gpmpc_rollout
+ *   K       (Nu, Ny)      feedback gain in the caller's units, or NULL (open loop); needs Nu > 0
+ *   x_ref   (Ny)          caller units, NULL = 0 (read only with K)
+ *   uscale  (2, Nu)       [meanU | stdU] or NULL (read only with K)
+ *   means, vars (B, Nt, Ny) as gpmpc_rollout per trajectory;  cov_last (B, Ny, Ny) or NULL
+ * Methods ME and TA (EM: GPMPC_ERR_ARG); B, Nt >= 1; the handle must own all outputs (GPMPC_ERR_STATE). */
+int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, const double* z0, const double* U,
+                        const double* Sigma0, const double* scale, const double* K, const double* x_ref,
+                        const double* uscale, double* means, double* vars, double* cov_last);
 
 /* Problem sizes of a handle (GP.get_size, gp_class.py:266-274: N, and Nx, Ny). */
 int gpmpc_get_size(gpmpc_handle_t h, int* N, int* Nx, int* Ny);
