@@ -39,6 +39,15 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
+// The dynamic shared buffer rounded up to the 1024-byte period of the TMA 128B swizzle.  The rounding is taken on the
+// 32-bit shared address and applied as an element offset from smem_raw, so the pointer keeps the shared state space
+// and fragment reads compile to LDS.  (Rounding the generic pointer through uintptr_t loses it: every read becomes a
+// generic LD.E with 64-bit address arithmetic.)
+__device__ __forceinline__ double* smem_align1024(double* smem_raw) {
+    const uint32_t b = smem_u32(smem_raw);
+    return smem_raw + ((((b + 1023u) & ~1023u) - b) >> 3);
+}
+
 // 16-byte asynchronous global->shared copy (LDGSTS), L2-only caching: tiles are
 // streamed once per CTA, reuse happens in L2 across CTAs.
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
@@ -59,6 +68,20 @@ __device__ __forceinline__ void dmma884(double& d0, double& d1, double a, double
     asm volatile(
         "mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
         : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
+}
+
+// fp64 tensor-core MMA: D(16x8) = A(16x16,row) * B(16x8,col) + C.  SASS: DMMA.16x8x16 (8x the work of DMMA.8x8x4).
+// lane l = 4 g + t holds A[g + 8 (i & 1)][kappa(t, i >> 1)] in a[i], B[kappa(t, j)][g] in b[j] and
+// C/D[g + 8 (i >> 1)][2 t + (i & 1)] in d[i].  kappa(t, j) is the k index the hardware assigns to register slot j of
+// lane group t; a[2j], a[2j+1] and b[j] of a lane share it.  The MMA sums over k, so a caller may put any k into slot
+// (t, j) as long as it puts the same k into A and B.
+__device__ __forceinline__ void dmma16816(double (&d)[4], const double (&a)[8], const double (&b)[4]) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+        "{%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+        : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+        : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
+          "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
 }
 
 __device__ __forceinline__ double warp_sum(double v) {

@@ -1,8 +1,9 @@
 // fp64 tensor-core (DMMA m8n8k4) GEMM family used by every O(N^3) / O(N^2 H) step of the
 // GP hot path: Cholesky trailing updates (SYRK), explicit-inverse panel solves, the
-// triangular inverse assembly, K^-1 = Linv^T Linv, and the batched predictive
-// v = Linv * ks product.  The fp64 tensor path (Hopper wgmma has no fp64 kind)
-// is mma.sync.m8n8k4 (SASS DMMA.8x8x4) fed by a 4-stage cp.async shared-memory pipeline.
+// triangular inverse assembly and K^-1 = Linv^T Linv.  The fp64 tensor path (Hopper
+// wgmma has no fp64 kind) is mma.sync.m8n8k4 (SASS DMMA.8x8x4) fed by a 4-stage cp.async
+// shared-memory pipeline.  (The predictive v = Linv * ks product, predict_streamk.cuh,
+// issues DMMA.16x8x16.)
 //
 //   C[i][j] = alpha * sum_k A[i][k] * Bop[k][j] + beta * Cin[i][j]
 //   A   : row-major M x K (K contiguous)
@@ -231,7 +232,7 @@ gemm_dmma_tmap_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tm
     static_assert((BM * 128) % 1024 == 0 && (BN * 128) % 1024 == 0, "tiles must be whole swizzle atoms");
 
     extern __shared__ __align__(16) double smem_raw[];
-    double* smem = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    double* smem = smem_align1024(smem_raw);
     double* As = smem;
     double* Bs = smem + STAGES * A_STAGE;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * (A_STAGE + B_STAGE));

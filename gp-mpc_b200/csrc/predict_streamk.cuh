@@ -439,18 +439,34 @@ finalize_kernel(const PredictParams p)
     psk_step_tail(p, sh, threadIdx.x, PSK_THREADS, &s_flag, &s_ok);
 }
 
+// The product on DMMA.16x8x16 (dmma16816).  tmA delivers the BM x 16 box of ks^T (test points x k), tmB the 128 x 16
+// box of the L-side matrix (L^-1, U in upper mode, L in the refinement), both in rows of 128 bytes with the 128B
+// swizzle: the 16-byte chunk c of row r sits at chunk c ^ (r & 7).  Per k-step (16 k) warp w computes the 16 x BM
+// block V^T[L-rows 16w .. 16w+15][points] with the L tile as the MMA's A operand (row layout, M = 16 L-rows) and
+// ks^T as its B operand (col layout, N = 8 points per fragment, BM / 8 fragments).
+//   k-permutation: lane (g, t) puts k = 2j + (t & 1) + 8 (t >> 1) into register slot j (the one gemm_dmma_tmap_kernel
+//   uses per 4-k step), i.e. logical chunk j + 4 (t >> 1), half t & 1.  Each value is one LDS.64 straight into its
+//   MMA register, and the 16 lanes of a half-warp hit 16 distinct 8-byte banks under the swizzle.
+//   A: a[2j] = L-row 16w + g, a[2j+1] = L-row 16w + g + 8 (8 LDS.64);  B: point row 8 ni + g (4 LDS.64 per fragment).
+//   accumulators acc[ni][i]: L-row 16w + g + 8 (i >> 1), point 8 ni + 2t + (i & 1).
+//   (Contiguous k = 4t + j would allow LDS.128, but the MMA pairs rows g and g + 8 in adjacent A registers, so every
+//   A load then needs register moves; ptxas kept two copies of the A fragment and spilled 192-236 B per thread.)
+// Every BM uses this one instruction shape, k-permutation and reduction order (sum of squares over the thread's two
+// L-rows, xor shuffles over g, then warps 0..7 in order), so a point's var does not depend on BM or on its row in
+// the chunk.
 template <int BM>
 __global__ void __launch_bounds__(PSK_THREADS, 2)
 predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB)
 {
     constexpr int BK = GEMM_BK, BN = PSK_BN, STAGES = PSK_STAGES;
-    constexpr int WTN = BN / 8, MF = BM / 8, NF = WTN / 8;        // 8 warps side by side: 16 columns each
+    constexpr int NF = BM / 8;                                     // 8-point fragments; 8 warps x 16 L-rows = BN
+    static_assert(BK == 16 && BN == 8 * 16, "one m16n8k16 per fragment and k-step, 16 L-rows per warp");
     constexpr int A_STAGE = BM * BK, B_STAGE = BN * BK;           // doubles, 128-byte rows, 128B swizzle
     constexpr uint32_t STAGE_TX = (BM + BN) * BK * 8;
     static_assert(BM % 8 == 0 && BM >= 8 && BM <= 64, "BM");
 
     extern __shared__ __align__(16) double smem_raw[];
-    double* smem = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    double* smem = smem_align1024(smem_raw);
     double* As = smem;
     double* Bs = smem + STAGES * A_STAGE;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * (A_STAGE + B_STAGE));
@@ -525,35 +541,34 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
 
     PskIter cit;
     psk_iter_init(cit, g0, p.T);
-    const int kperm_hi = 4 * (t >> 1), kpar = t & 1;
+    int cj[4];                                                      // slot j: k = 2j + (t & 1) + 8 (t >> 1)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) cj[j] = (((j + 4 * (t >> 1)) ^ g) << 1) + (t & 1);
     int i = 0;
     while (i < nsteps) {
         const int a = cit.a, jt = cit.jt, s_begin = cit.s, ksteps = cit.ks;
         const int seg = min(ksteps - s_begin, nsteps - i);
-        double acc[MF][NF][2];
+        double acc[NF][4];
 #pragma unroll
-        for (int mi = 0; mi < MF; ++mi)
+        for (int ni = 0; ni < NF; ++ni)
 #pragma unroll
-            for (int ni = 0; ni < NF; ++ni) { acc[mi][ni][0] = 0.0; acc[mi][ni][1] = 0.0; }
+            for (int r = 0; r < 4; ++r) acc[ni][r] = 0.0;
 
         for (int q = 0; q < seg; ++q, ++i) {
             const int s = i % STAGES;
             if (tid == 0 && i + AHEAD < nsteps) issue();  // s_pg == i + AHEAD
             mbar_wait(full + s, (uint32_t)((i / STAGES) & 1));
-            const double* as = As + s * A_STAGE + g * 16 + kpar;
-            const double* bs = Bs + s * B_STAGE + (warp * WTN + g) * 16 + kpar;
+            const double* ls = Bs + s * B_STAGE + (warp * 16 + g) * 16;    // L-rows 16w + g (+ 8: 128 doubles on)
+            const double* ps = As + s * A_STAGE + g * 16;                  // point rows 8 ni + g
+            double av[8];
 #pragma unroll
-            for (int kk = 0; kk < BK / 4; ++kk) {
-                const int coff = (((kk + kperm_hi) ^ g) << 1);
-                double av[MF], bv[NF];
+            for (int j = 0; j < 4; ++j) { av[2 * j] = ls[cj[j]]; av[2 * j + 1] = ls[128 + cj[j]]; }
 #pragma unroll
-                for (int mi = 0; mi < MF; ++mi) av[mi] = as[mi * 8 * 16 + coff];
+            for (int ni = 0; ni < NF; ++ni) {
+                double bv[4];
 #pragma unroll
-                for (int ni = 0; ni < NF; ++ni) bv[ni] = bs[ni * 8 * 16 + coff];
-#pragma unroll
-                for (int mi = 0; mi < MF; ++mi)
-#pragma unroll
-                    for (int ni = 0; ni < NF; ++ni) dmma884(acc[mi][ni][0], acc[mi][ni][1], av[mi], bv[ni]);
+                for (int j = 0; j < 4; ++j) bv[j] = ps[ni * 8 * 16 + cj[j]];
+                dmma16816(acc[ni], av, bv);
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(empty + s);        // this warp is done reading stage s
@@ -565,14 +580,14 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
         bool have_tile = true;
         if (seg != ksteps) {
             const long long tg0 = (long long)a * p.T + 4LL * jt * (jt + 1), tg1 = tg0 + ksteps;
-            const int c_first = (int)(((tg0 + 1) * C - 1) / p.G), c_last = (int)((tg1 * C - 1) / p.G);
-            double* mine = p.part + ((long long)c * 2 + (s_begin == 0 ? 1 : 0)) * (BM * BN);
+            const long long Cf = gridDim.x;                           // re-read: keeps C and c out of the loop's registers
+            const int c_first = (int)(((tg0 + 1) * Cf - 1) / p.G), c_last = (int)((tg1 * Cf - 1) / p.G);
+            double2* mine = reinterpret_cast<double2*>(p.part + ((long long)blockIdx.x * 2 + (s_begin == 0 ? 1 : 0)) * (BM * BN)) + tid;
 #pragma unroll
-            for (int mi = 0; mi < MF; ++mi)
+            for (int ni = 0; ni < NF; ++ni)
 #pragma unroll
-                for (int ni = 0; ni < NF; ++ni)
-                    __stcg(reinterpret_cast<double2*>(mine + ((mi * NF + ni) * PSK_THREADS + tid) * 2),
-                           make_double2(acc[mi][ni][0], acc[mi][ni][1]));
+                for (int hf = 0; hf < 2; ++hf)
+                    __stcg(mine + (ni * 2 + hf) * PSK_THREADS, make_double2(acc[ni][2 * hf], acc[ni][2 * hf + 1]));
             __threadfence();
             __syncthreads();
             if (tid == 0) {
@@ -587,17 +602,17 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
             if (have_tile) {
                 __threadfence();
 #pragma unroll
-                for (int mi = 0; mi < MF; ++mi)
+                for (int ni = 0; ni < NF; ++ni)
 #pragma unroll
-                    for (int ni = 0; ni < NF; ++ni) { acc[mi][ni][0] = 0.0; acc[mi][ni][1] = 0.0; }
+                    for (int r = 0; r < 4; ++r) acc[ni][r] = 0.0;
                 for (int cc = c_first; cc <= c_last; ++cc) {          // contributor (= ascending k) order
-                    const double* src = p.part + ((long long)cc * 2 + (cc == c_first ? 1 : 0)) * (BM * BN);
+                    const double2* src = reinterpret_cast<const double2*>(p.part + ((long long)cc * 2 + (cc == c_first ? 1 : 0)) * (BM * BN)) + tid;
 #pragma unroll
-                    for (int mi = 0; mi < MF; ++mi)
+                    for (int ni = 0; ni < NF; ++ni)
 #pragma unroll
-                        for (int ni = 0; ni < NF; ++ni) {
-                            const double2 v = __ldcg(reinterpret_cast<const double2*>(src + ((mi * NF + ni) * PSK_THREADS + tid) * 2));
-                            acc[mi][ni][0] += v.x; acc[mi][ni][1] += v.y;
+                        for (int hf = 0; hf < 2; ++hf) {
+                            const double2 v = __ldcg(src + (ni * 2 + hf) * PSK_THREADS);
+                            acc[ni][2 * hf] += v.x; acc[ni][2 * hf + 1] += v.y;
                         }
                 }
             }
@@ -606,24 +621,25 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
 
         // ---- complete tile: optional store of the solved rows, squared row norms of this column tile
         if (p.Vout) {
+            const int col = (p.upper ? p.nt - 1 - jt : jt) * BN + warp * 16 + g;
+            double* vo = p.Vout + (long long)a * p.sV + col;
 #pragma unroll
-            for (int mi = 0; mi < MF; ++mi)
+            for (int ni = 0; ni < NF; ++ni)
 #pragma unroll
-                for (int ni = 0; ni < NF; ++ni) {
-                    const int row = mi * 8 + g, col = (p.upper ? p.nt - 1 - jt : jt) * BN + warp * WTN + ni * 8 + 2 * t;
-                    *reinterpret_cast<double2*>(p.Vout + (long long)a * p.sV + (long long)row * p.ldv + col) =
-                        make_double2(acc[mi][ni][0], acc[mi][ni][1]);
-                }
+                for (int r = 0; r < 4; ++r)
+                    vo[(long long)(ni * 8 + 2 * t + (r & 1)) * p.ldv + 8 * (r >> 1)] = acc[ni][r];
         }
 #pragma unroll
-        for (int mi = 0; mi < MF; ++mi) {
-            double r = 0.0;
+        for (int ni = 0; ni < NF; ++ni)
 #pragma unroll
-            for (int ni = 0; ni < NF; ++ni) { r = fma(acc[mi][ni][0], acc[mi][ni][0], r); r = fma(acc[mi][ni][1], acc[mi][ni][1], r); }
-            r += __shfl_xor_sync(0xffffffffu, r, 1);
-            r += __shfl_xor_sync(0xffffffffu, r, 2);
-            if (t == 0) red[warp][mi * 8 + g] = r;
-        }
+            for (int j = 0; j < 2; ++j) {
+                double r = acc[ni][j] * acc[ni][j];                   // L-row g, then g + 8
+                r = fma(acc[ni][j + 2], acc[ni][j + 2], r);
+                r += __shfl_xor_sync(0xffffffffu, r, 4);
+                r += __shfl_xor_sync(0xffffffffu, r, 8);
+                r += __shfl_xor_sync(0xffffffffu, r, 16);
+                if (g == 0) red[warp][ni * 8 + 2 * t + j] = r;
+            }
         __syncthreads();
         if (tid < BM) {
             double r = 0.0;
