@@ -95,7 +95,7 @@ struct gpmpc_handle_s {
     // predict
     DevBuf<double> dKST, dPart, dPMJ, dSQ, dV, dR, dR2;
     DevBuf<unsigned int> dCnt;        // stream-K counters: [nloc*nt tile | nloc output | 1 done], self-cleaning
-    int psk_ctas = 0, opt_predict_ctas = 0;   // persistent grid of the predict product (2 CTAs per SM)
+    int psk_ctas = 0, opt_predict_ctas = 0;   // persistent grid of the predict product (PSK_CTAS_PER_SM per SM)
     DevBuf<double> dCovV, dCovOut;    // GP.covar scratch pool
     // predict_grad: U = Linv^T per output (lazy), beta rows, partial sums, per-batch derivative slabs
     DevBuf<double> dUall, dBeta, dPDV, dPH, dGradOut; bool u_valid = false;
@@ -409,7 +409,7 @@ static int create_fill(gpmpc_handle_t h, int N, int Nx, int Ny, int out_begin, i
     CUDA_TRY(cudaSetDevice(device));
     CUDA_TRY(cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, device));
     h->opt_small_tiles = 4 * h->sms;      // two waves of 2 CTAs per SM
-    h->psk_ctas = 2 * h->sms;
+    h->psk_ctas = PSK_CTAS_PER_SM * h->sms;
     cudaDeviceGetAttribute(&h->clock_khz, cudaDevAttrClockRate, device);
     {
         int lo = 0, hi = 0;
@@ -768,7 +768,7 @@ extern "C" int gpmpc_set_option(gpmpc_handle_t h, const char* name, double value
 {
     if (!h || !name) return GPMPC_ERR_ARG;
     if (!strcmp(name, "refine")) { h->opt_refine = value != 0.0; return GPMPC_OK; }
-    if (!strcmp(name, "predict_ctas")) {       // persistent grid of the predict product (0 = 2 per SM)
+    if (!strcmp(name, "predict_ctas")) {       // persistent grid of the predict product (0 = PSK_CTAS_PER_SM per SM)
         const int v = (int)value;
         if (v < 0 || v > PSK_MAX_CTAS) { set_error(h, "predict_ctas must be in [0, %d]", PSK_MAX_CTAS); return GPMPC_ERR_ARG; }
         h->opt_predict_ctas = v; return GPMPC_OK;
@@ -806,12 +806,12 @@ static int ensure_rows(gpmpc_handle_t h)
 
 static int ensure_predict_bufs(gpmpc_handle_t h, int H)
 {
-    const long long np = h->Npad, nt = np / 128;
+    const long long np = h->Npad, nt = np / 128;      // nt >= the product's tiles per output (tile_cnt below)
     ENSURE(h->dKST, (long long)h->nloc * HB * np);
     ENSURE(h->dPMJ, (long long)h->nloc * HB * ks_blocks(h) * (h->Nx + 1));
     ENSURE(h->dSQ, (long long)h->nloc * HB * nt);
     ENSURE(h->dCnt, (long long)h->nloc * nt + h->nloc + 1);
-    // parked stream-K partials: two BM x 128 slots per persistent CTA
+    // parked stream-K partials: two BM x PSK_BN slots per persistent CTA
     ENSURE(h->dPart, (long long)std::max(h->psk_ctas, h->opt_predict_ctas) * 2 * HB * PSK_BN);
     if (h->opt_refine) {
         int rc = ensure_rows(h);
@@ -841,7 +841,7 @@ template <int BM>
 static cudaError_t psk_launch_bm(const PredictParams& p, const double* A, long long sA, const double* B, long long sB,
                                  int np, int grid, cudaStream_t st)
 {
-    constexpr int BYTES = PSK_STAGES * (BM + PSK_BN) * GEMM_BK * 8 + 2 * PSK_STAGES * 8 + 1024;
+    constexpr int BYTES = psk_pipe_doubles(BM) * 8 + 2 * PSK_STAGES * 8 + 1024;
     const cudaError_t e = smem_opt_in<predict_streamk_kernel<BM>>(BYTES);
     if (e != cudaSuccess) return e;
     CUtensorMap tmA, tmB;
@@ -873,7 +873,7 @@ static cudaError_t psk_launch(int bm, const PredictParams& p, const double* A, l
     }
 }
 
-// persistent grid: 2 CTAs per SM, but never fewer than 4 k-steps per CTA (at small N, more CTAs with fewer steps each beat
+// persistent grid: PSK_CTAS_PER_SM CTAs per SM, but never fewer than 4 k-steps per CTA (at small N, more CTAs with fewer steps each beat
 // fewer with more -- the fixed cost per CTA overlaps across SMs, the steps do not)
 static int psk_grid(gpmpc_handle_t h, long long G)
 {
@@ -883,12 +883,14 @@ static int psk_grid(gpmpc_handle_t h, long long G)
     return (int)std::min<long long>(ctas, h->opt_predict_ctas > 0 ? G : by_work);
 }
 
-static void psk_base(gpmpc_handle_t h, PredictParams& p, int Hc)
+// upper: the L-side operand is upper triangular (its k-step list is shorter when Npad / 128 is odd)
+static void psk_base(gpmpc_handle_t h, PredictParams& p, int Hc, int upper = 0)
 {
     memset(&p, 0, sizeof(p));
     const long long nt = h->Npad / 128;
-    p.nloc = h->nloc; p.nt = (int)nt; p.Hc = Hc;
-    p.T = 4 * nt * (nt + 1); p.G = p.T * h->nloc;
+    p.nloc = h->nloc; p.nt = (int)nt; p.Hc = Hc; p.upper = upper;
+    p.ntb = (int)((h->Npad + PSK_BN - 1) / PSK_BN); p.nk = h->Npad / GEMM_BK;
+    p.T = psk_steps_per_output(p.ntb, p.nk, upper); p.G = p.T * h->nloc;
     p.part = h->dPart;
     p.tile_cnt = h->dCnt; p.out_cnt = h->dCnt + (long long)h->nloc * nt; p.done_cnt = p.out_cnt + h->nloc;
     p.SQ = h->dSQ;
@@ -903,7 +905,7 @@ static void psk_finalize(gpmpc_handle_t h, PredictParams& p, int H, int h0)
 }
 
 // assembly of a single-rank step of H points (predict_core adds the multi-rank fields).  stage_g: the gather records fit
-// next to J Sigma in the product kernel's stage buffers (PSK_STAGES (bm + 128) 16 doubles), read by the fused assembly only
+// next to J Sigma in the product kernel's stage buffers (psk_pipe_doubles), read by the fused assembly only
 static AssembleArgs assemble_args(gpmpc_handle_t h, int H, int method, const double* Sigma, int spp,
                                   double* mean, double* var, double* J, double* cov)
 {
@@ -914,7 +916,7 @@ static AssembleArgs assemble_args(gpmpc_handle_t h, int H, int method, const dou
     as.mean = mean; as.var = var; as.J = J; as.cov = cov;
     as.world = 1;
     const long long bm1 = (std::min(H, HB) + 7) / 8 * 8;
-    as.stage_g = (assemble_rows_doubles(H, h->Ny, h->Nx) <= (long long)PSK_STAGES * (bm1 + PSK_BN) * GEMM_BK) ? 1 : 0;
+    as.stage_g = (assemble_rows_doubles(H, h->Ny, h->Nx) <= psk_pipe_doubles((int)bm1)) ? 1 : 0;
     return as;
 }
 
@@ -1789,8 +1791,8 @@ static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, c
         psk_finalize(h, p, H, h0);
         p.Vout = h->dV; p.sV = (long long)HB * np; p.ldv = np;
         CUDA_TRY(psk_launch(bm, p, h->dKST, (long long)HB * np, h->dLi, slab(h), np, psk_grid(h, p.G), h->st));
-        psk_base(h, p, Hc);                                   // beta = Linv^T v = K^-1 ks  (rows of V times U^T)
-        p.upper = 1; p.Vout = h->dBeta; p.sV = (long long)HB * np; p.ldv = np;
+        psk_base(h, p, Hc, 1);                                // beta = Linv^T v = K^-1 ks  (rows of V times U^T)
+        p.Vout = h->dBeta; p.sV = (long long)HB * np; p.ldv = np;
         CUDA_TRY(psk_launch(bm, p, h->dV, (long long)HB * np, h->dUall, slab(h), np, psk_grid(h, p.G), h->st));
         CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_grad_reduce<decltype(nxp)::value>(h, dZc, Hc, nblk_g); }));
         grad_finalize_kernel<<<dim3(Hc, h->nloc), 128, 0, h->st>>>(h->dPDV, h->dPH, nblk_g, Hc, h->dHyp, Nx + 2, Nx, Ny,

@@ -5,8 +5,8 @@
 //   cov = diag(var) (+ J Sigma J^T)                         -> mean / var / J / cov outputs
 //
 // Scheduling is stream-K: the triangular product's work is the list of BK=16 k-steps of every
-// (output a, 128-column tile jt) pair -- tile jt has (jt+1)*8 steps because L^-1 is lower
-// triangular -- and the persistent grid (2 CTAs per SM) cuts that list into equal contiguous
+// (output a, PSK_BN-row tile jt) pair -- tile jt has min((jt+1) BN, Npad) / 16 steps because L^-1 is
+// lower triangular -- and the persistent grid cuts that list into equal contiguous
 // ranges, so every CTA issues the same number of DMMAs regardless of where tile borders fall
 // (the static split-K grid it replaces lost a visible share to the tail at one output per GPU).  A tile cut
 // by a range border is completed by its LAST-ARRIVING contributor: everyone else parks its partial
@@ -21,9 +21,19 @@
 #include "gemm_dmma.cuh"
 
 #define GPMPC_MAXW 16
-#define PSK_BN 128
-#define PSK_STAGES 4
-#define PSK_THREADS 256
+// The product kernel: PSK_CW warps of 32 L-rows each (tile height PSK_BN).  Registers are handed out per SM
+// sub-partition (a quarter of the resident warps each, 512 per thread slot): at 8 warps per SM every warp can hold the
+// 2 x BM / 8 x 4 fp64 accumulators with no spill, a 9th (producer) warp would cap all of them at 168 and spill.
+// One 256-row CTA per SM (5 stages of 39-41 KB) measured faster at C5 than two 128-row CTAs per SM (4 stages each).
+#define PSK_CW 8
+#define PSK_BN (32 * PSK_CW)
+#define PSK_STAGES 5
+#define PSK_CTAS_PER_SM 1
+#define PSK_THREADS (32 * PSK_CW)
+
+// doubles of the product kernel's stage buffers at bm test points (the fused tail reuses them as scratch)
+__host__ __device__ constexpr long long psk_pipe_doubles(int bm) { return (long long)PSK_STAGES * (bm + PSK_BN) * GEMM_BK; }
+
 
 // Peer ("fused epilogue + all-gather") mode: instead of writing into the local gather buffer and
 // calling ncclAllGather, every rank stores its [mean,var,J] records directly into the gather
@@ -53,11 +63,12 @@ struct AssembleArgs {
 };
 
 struct PredictParams {
-    int nloc, nt, Hc;                 // local outputs, 128-column tiles per output, valid rows of this chunk
+    int nloc, nt, Hc;                 // local outputs, 128-column groups per output (Npad / 128), valid rows of this chunk
+    int ntb, nk;                      // PSK_BN-row tiles per output (the last one 128 rows high when nt is odd), Npad / 16
     int upper;                        // 0: B lower triangular (k <= j, v = Linv ks); 1: B upper (k >= j, beta = Linv^T v)
-    long long T, G;                   // k-steps per output = 4 nt (nt+1), total = nloc * T
-    double* part;                     // [grid][2][BM*128] parked partial accumulators (fragment-major)
-    unsigned int* tile_cnt;           // [nloc*nt]
+    long long T, G;                   // k-steps per output (psk_steps_per_output), total = nloc * T
+    double* part;                     // [grid][2][BM*PSK_BN] parked partial accumulators (fragment-major)
+    unsigned int* tile_cnt;           // [nloc*ntb]
     unsigned int* out_cnt;            // [nloc]
     unsigned int* done_cnt;           // [1]
     double* SQ;                       // [nloc][64][nt] per-tile sums of squares
@@ -299,23 +310,46 @@ assemble_kernel(const AssembleArgs A)
     for (int h = blockIdx.x; h < A.H; h += gridDim.x) assemble_point<false>(A, h, sh, threadIdx.x, blockDim.x);
 }
 
+// The k-step list of one output.  Lower: tile jt covers k < min((jt+1) BN, Npad).  Upper: list position jt stands for
+// column tile ntb-1-jt, which covers k in [(ntb-1-jt) BN, Npad).  Only a tile that reaches Npad can be short (the half
+// tile of an odd Npad / 128: the L-side map's row bound zero-fills its upper half), so with d = SB ntb - nk (0 or 8)
+// position jt has SB (jt+1) steps in lower mode, except the last one (SB ntb - d), and SB (jt+1) - d in upper mode.
+// The two modes' totals differ when d != 0.
+#define PSK_SB (PSK_BN / GEMM_BK)     // k-steps per full tile height
+__host__ __device__ inline long long psk_kstart(int ntb, int nk, int upper, int jt)   // first step of position jt
+{
+    const long long full = (long long)(PSK_SB / 2) * jt * (jt + 1), d = (long long)PSK_SB * ntb - nk;
+    return upper ? full - jt * d : (jt == ntb ? full - d : full);
+}
+__host__ __device__ inline long long psk_steps_per_output(int ntb, int nk, int upper) { return psk_kstart(ntb, nk, upper, ntb); }
+__device__ __forceinline__ long long psk_kstart(const PredictParams& p, int jt) { return psk_kstart(p.ntb, p.nk, p.upper, jt); }
+// A tile's k range reaches 128 columns past the diagonal of its first (lower) / before the diagonal of its second (upper)
+// 128-row half.  Only the leaf kernel's diagonal 128 x 128 blocks are stored with explicit zeros on their far side; the
+// off-diagonal block beyond is not kept zero (a full K build leaves K's upper triangle in the L slab), so the warps of
+// that half skip those 8 k-steps in the product kernel's main loop and never read it.
+__device__ __forceinline__ int psk_ksteps(const PredictParams& p, int jt)
+{
+    return p.upper ? p.nk - PSK_SB * (p.ntb - 1 - jt) : min(PSK_SB * (jt + 1), p.nk);
+}
+
 struct PskIter { int a, jt, s, ks; };
 
-__device__ __forceinline__ void psk_iter_init(PskIter& it, long long g, long long T)
+__device__ __forceinline__ void psk_iter_init(PskIter& it, long long g, const PredictParams& p)
 {
-    it.a = (int)(g / T);
-    const long long r = g - (long long)it.a * T;               // 4 jt (jt+1) <= r
-    int jt = (int)((sqrt((double)r + 1.0) - 1.0) * 0.5);
-    while (4LL * jt * (jt + 1) > r) --jt;
-    while (4LL * (jt + 1) * (jt + 2) <= r) ++jt;
-    it.jt = jt; it.s = (int)(r - 4LL * jt * (jt + 1)); it.ks = (jt + 1) * 8;
+    it.a = (int)(g / p.T);
+    const long long r = g - (long long)it.a * p.T;            // (SB/2) jt (jt+1) <= r, about
+    int jt = (int)((sqrt(8.0 * (double)r / PSK_SB + 1.0) - 1.0) * 0.5);
+    jt = max(0, min(jt, p.ntb - 1));
+    while (jt > 0 && psk_kstart(p, jt) > r) --jt;
+    while (jt + 1 < p.ntb && psk_kstart(p, jt + 1) <= r) ++jt;
+    it.jt = jt; it.s = (int)(r - psk_kstart(p, jt)); it.ks = psk_ksteps(p, jt);
 }
-__device__ __forceinline__ void psk_iter_next(PskIter& it, int nt)
+__device__ __forceinline__ void psk_iter_next(PskIter& it, const PredictParams& p)
 {
     if (++it.s == it.ks) {
         it.s = 0;
-        if (++it.jt == nt) { it.jt = 0; ++it.a; }
-        it.ks = (it.jt + 1) * 8;
+        if (++it.jt == p.ntb) { it.jt = 0; ++it.a; }
+        it.ks = psk_ksteps(p, it.jt);
     }
 }
 
@@ -439,28 +473,32 @@ finalize_kernel(const PredictParams p)
     psk_step_tail(p, sh, threadIdx.x, PSK_THREADS, &s_flag, &s_ok);
 }
 
-// The product on DMMA.16x8x16 (dmma16816).  tmA delivers the BM x 16 box of ks^T (test points x k), tmB the 128 x 16
+// The product on DMMA.16x8x16 (dmma16816).  tmA delivers the BM x 16 box of ks^T (test points x k), tmB the BN x 16
 // box of the L-side matrix (L^-1, U in upper mode, L in the refinement), both in rows of 128 bytes with the 128B
-// swizzle: the 16-byte chunk c of row r sits at chunk c ^ (r & 7).  Per k-step (16 k) warp w computes the 16 x BM
-// block V^T[L-rows 16w .. 16w+15][points] with the L tile as the MMA's A operand (row layout, M = 16 L-rows) and
-// ks^T as its B operand (col layout, N = 8 points per fragment, BM / 8 fragments).
+// swizzle: the 16-byte chunk c of row r sits at chunk c ^ (r & 7).
+//   Per k-step (16 k) warp w computes the 32 x BM block V^T[L-rows 32w .. 32w+31][points] as two MMA A
+//   operands (mi = 0, 1: L-rows 32w + 16 mi .. +15, row layout) against ks^T as the B operand (col layout, N = 8
+//   points per fragment, BM / 8 fragments).  Each B fragment feeds both A fragments: 16 + 4 BM / 8 LDS.64 per 2 BM / 8
+//   DMMAs, where 16 L-rows per warp needed 8 + 4 BM / 8 per BM / 8.
 //   k-permutation: lane (g, t) puts k = 2j + (t & 1) + 8 (t >> 1) into register slot j (the one gemm_dmma_tmap_kernel
 //   uses per 4-k step), i.e. logical chunk j + 4 (t >> 1), half t & 1.  Each value is one LDS.64 straight into its
-//   MMA register, and the 16 lanes of a half-warp hit 16 distinct 8-byte banks under the swizzle.
-//   A: a[2j] = L-row 16w + g, a[2j+1] = L-row 16w + g + 8 (8 LDS.64);  B: point row 8 ni + g (4 LDS.64 per fragment).
-//   accumulators acc[ni][i]: L-row 16w + g + 8 (i >> 1), point 8 ni + 2t + (i & 1).
+//   MMA register, and the 16 lanes of a half-warp hit 16 distinct 8-byte banks under the swizzle (rows g, g + 8,
+//   g + 16, g + 24 of a warp all sit at swizzle phase g).
+//   A: av[mi][2j] = L-row 32w + 16 mi + g, av[mi][2j+1] = the row 8 below;  B: point row 8 ni + g.
+//   accumulators acc[mi][ni][i]: L-row 32w + 16 mi + g + 8 (i >> 1), point 8 ni + 2t + (i & 1).
 //   (Contiguous k = 4t + j would allow LDS.128, but the MMA pairs rows g and g + 8 in adjacent A registers, so every
-//   A load then needs register moves; ptxas kept two copies of the A fragment and spilled 192-236 B per thread.)
-// Every BM uses this one instruction shape, k-permutation and reduction order (sum of squares over the thread's two
-// L-rows, xor shuffles over g, then warps 0..7 in order), so a point's var does not depend on BM or on its row in
-// the chunk.
+//   A load then needs register moves; ptxas kept two copies of the A fragment and spilled.)
+// Every BM uses this one instruction shape, k-permutation and reduction order (per 128-column group: sum of squares
+// over the thread's two L-rows, xor shuffles over g, then the group's eight 16-row blocks in order), so a point's var
+// does not depend on BM or on its row in the chunk.
 template <int BM>
-__global__ void __launch_bounds__(PSK_THREADS, 2)
+__global__ void __launch_bounds__(PSK_THREADS, PSK_CTAS_PER_SM)
 predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB)
 {
-    constexpr int BK = GEMM_BK, BN = PSK_BN, STAGES = PSK_STAGES;
-    constexpr int NF = BM / 8;                                     // 8-point fragments; 8 warps x 16 L-rows = BN
-    static_assert(BK == 16 && BN == 8 * 16, "one m16n8k16 per fragment and k-step, 16 L-rows per warp");
+    constexpr int BK = GEMM_BK, BN = PSK_BN, STAGES = PSK_STAGES, CW = PSK_CW, NT = PSK_THREADS;
+    constexpr int NF = BM / 8;                                     // 8-point fragments; CW warps x 32 L-rows = BN
+    static_assert(BK == 16 && BN == 32 * CW && BN % 128 == 0, "one m16n8k16 per fragment and k-step, 32 L-rows per warp");
+    constexpr int GR = BN / 128;                                   // 128-column groups per tile
     constexpr int A_STAGE = BM * BK, B_STAGE = BN * BK;           // doubles, 128-byte rows, 128B swizzle
     constexpr uint32_t STAGE_TX = (BM + BN) * BK * 8;
     static_assert(BM % 8 == 0 && BM >= 8 && BM <= 64, "BM");
@@ -471,7 +509,7 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
     double* Bs = smem + STAGES * A_STAGE;
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * (A_STAGE + B_STAGE));
     uint64_t* empty = full + STAGES;
-    __shared__ double red[8][64];
+    __shared__ double red[BN / 16][64];
     __shared__ unsigned int s_flag;
     __shared__ int s_ok;
 
@@ -488,40 +526,37 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
     __shared__ uint64_t s_pol[2];
     if (tid == 0) {
 #pragma unroll
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, PSK_THREADS / 32); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, CW); }
         mbar_fence_init();
     }
     __syncthreads();
 
-    // Pipeline without CTA-wide barriers: stage s is FULL when its two TMA boxes have landed and EMPTY
-    // when all 8 warps have read it.  Thread 0 refills two steps ahead: the stage it overwrites at
-    // step i was last read at step i-2, so its empty-wait is almost never a real wait and the warps
-    // may drift up to a step apart instead of meeting at a __syncthreads every 16 k.
+    // Pipeline without CTA-wide barriers: stage s is FULL when its two TMA boxes have landed and EMPTY when all CW warps
+    // have read it.  Thread 0 refills AHEAD = STAGES - 2 steps ahead: the stage it overwrites at step i was last read at
+    // step i - 2, so its empty-wait is almost never a real wait and the warps may drift up to a step apart.
     auto issue = [&]() {               // thread 0: TMA loads of step s_pg into stage s_pg % STAGES
         PskIter it = s_pit;
         const int pg = s_pg, s = pg % STAGES;
         if (pg >= STAGES) mbar_wait(empty + s, (uint32_t)(((pg / STAGES) - 1) & 1));
         mbar_arrive_expect_tx(full + s, STAGE_TX);
-        // lower: tile jt covers k in [0, (jt+1) 128); upper: the list position jt stands for column tile
-        // nt-1-jt, which covers k in [(nt-1-jt) 128, Npad) -- the same (jt+1)*8 steps
-        const int jta = p.upper ? p.nt - 1 - it.jt : it.jt;
+        const int jta = p.upper ? p.ntb - 1 - it.jt : it.jt;
         const int k0 = (p.upper ? jta * BN : 0) + it.s * BK;
         // ks^T (A) is re-read by every column tile: keep it in L2; L^-1 (B) is streamed exactly once.  Also when ks^T is
         // larger than the L2 (8 outputs at N=16384 on H100: 59 MB vs 50 MB) evict_last measured no slower than evict_normal
         tma_tile_g2s_3d_hint(As + s * A_STAGE, &tmA, k0, 0, it.a, full + s, s_pol[1]);
         tma_tile_g2s_3d_hint(Bs + s * B_STAGE, &tmB, k0, jta * BN, it.a, full + s, s_pol[0]);
-        psk_iter_next(it, p.nt);
+        psk_iter_next(it, p);
         s_pit = it;
         s_pg = pg + 1;
     };
-    constexpr int AHEAD = 2;           // prefetch distance in steps
+    constexpr int AHEAD = STAGES - 2;  // prefetch distance in steps
     // programmatic dependent launch: everything above overlapped the tail of the ks kernel; its output
     // (KS^T, the partial mean / Jacobian sums) is only touched below this point.  A no-op when the
     // kernel was launched without the attribute.
     asm volatile("griddepcontrol.wait;" ::: "memory");
     if (tid == 0) {
         PskIter it;
-        psk_iter_init(it, g0, p.T);
+        psk_iter_init(it, g0, p);
         s_pit = it; s_pg = 0;
         s_pol[0] = l2_policy_evict_first(); s_pol[1] = l2_policy_evict_last();
 #pragma unroll
@@ -529,18 +564,18 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
             if (s_pg < nsteps) issue();
     }
     if (p.finalize) {
-        // this CTA's share of the mean / Jacobian records (warps 1..7; thread 0 is the TMA producer), while the first
+        // this CTA's share of the mean / Jacobian records (warps 1..; thread 0 is the TMA producer), while the first
         // stages are in flight.  Ordered before the step's publication by the fence + counter chain every CTA's tiles
         // go through (each CTA owns at least one k-step).
         const int tot = p.nloc * p.Hc * (p.Nx + 1), per = (tot + (int)C - 1) / (int)C;
         if (tid >= 32) {
-            psk_reduce_mj(p, min(tot, (int)c * per), min(tot, ((int)c + 1) * per), tid - 32, PSK_THREADS - 32);
+            psk_reduce_mj(p, min(tot, (int)c * per), min(tot, ((int)c + 1) * per), tid - 32, NT - 32);
             if (p.use_peers) __threadfence_system();
         }
     }
 
     PskIter cit;
-    psk_iter_init(cit, g0, p.T);
+    psk_iter_init(cit, g0, p);
     int cj[4];                                                      // slot j: k = 2j + (t & 1) + 8 (t >> 1)
 #pragma unroll
     for (int j = 0; j < 4; ++j) cj[j] = (((j + 4 * (t >> 1)) ^ g) << 1) + (t & 1);
@@ -548,50 +583,65 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
     while (i < nsteps) {
         const int a = cit.a, jt = cit.jt, s_begin = cit.s, ksteps = cit.ks;
         const int seg = min(ksteps - s_begin, nsteps - i);
-        double acc[NF][4];
+        // steps [st_lo, st_hi) of the tile touch this warp's 128-row half below (lower) / above (upper) the diagonal; the
+        // others would read the 128 x 128 block on the wrong side of it, which no caller keeps zero (psk_ksteps)
+        const int hh = warp / (128 / 32);
+        const int st_lo = p.upper ? (128 / BK) * hh : 0;
+        const int st_hi = p.upper ? ksteps : PSK_SB * jt + (128 / BK) * (hh + 1);
+        double acc[2][NF][4];
 #pragma unroll
-        for (int ni = 0; ni < NF; ++ni)
+        for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-            for (int r = 0; r < 4; ++r) acc[ni][r] = 0.0;
+            for (int ni = 0; ni < NF; ++ni)
+#pragma unroll
+                for (int r = 0; r < 4; ++r) acc[mi][ni][r] = 0.0;
 
         for (int q = 0; q < seg; ++q, ++i) {
             const int s = i % STAGES;
             if (tid == 0 && i + AHEAD < nsteps) issue();  // s_pg == i + AHEAD
             mbar_wait(full + s, (uint32_t)((i / STAGES) & 1));
-            const double* ls = Bs + s * B_STAGE + (warp * 16 + g) * 16;    // L-rows 16w + g (+ 8: 128 doubles on)
-            const double* ps = As + s * A_STAGE + g * 16;                  // point rows 8 ni + g
-            double av[8];
+            const int st = s_begin + q;
+            if (st >= st_lo && st < st_hi) {
+                const double* ls = Bs + s * B_STAGE + (warp * 32 + g) * 16;    // L-rows 32w + g (+ 8, 16, 24: 128 doubles apart)
+                const double* ps = As + s * A_STAGE + g * 16;                  // point rows 8 ni + g
+                double av[2][8];
 #pragma unroll
-            for (int j = 0; j < 4; ++j) { av[2 * j] = ls[cj[j]]; av[2 * j + 1] = ls[128 + cj[j]]; }
+                for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-            for (int ni = 0; ni < NF; ++ni) {
-                double bv[4];
+                    for (int j = 0; j < 4; ++j) { av[mi][2 * j] = ls[256 * mi + cj[j]]; av[mi][2 * j + 1] = ls[256 * mi + 128 + cj[j]]; }
 #pragma unroll
-                for (int j = 0; j < 4; ++j) bv[j] = ps[ni * 8 * 16 + cj[j]];
-                dmma16816(acc[ni], av, bv);
+                for (int ni = 0; ni < NF; ++ni) {
+                    double bv[4];
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) bv[j] = ps[ni * 8 * 16 + cj[j]];
+                    dmma16816(acc[0][ni], av[0], bv);
+                    dmma16816(acc[1][ni], av[1], bv);
+                }
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(empty + s);        // this warp is done reading stage s
         }
         cit.s = s_begin + seg - 1;
-        psk_iter_next(cit, p.nt);
+        psk_iter_next(cit, p);
 
         // ---- tile fix-up: a tile cut by a range border is finished by its last-arriving contributor
         bool have_tile = true;
         if (seg != ksteps) {
-            const long long tg0 = (long long)a * p.T + 4LL * jt * (jt + 1), tg1 = tg0 + ksteps;
+            const long long tg0 = (long long)a * p.T + psk_kstart(p, jt), tg1 = tg0 + ksteps;
             const long long Cf = gridDim.x;                           // re-read: keeps C and c out of the loop's registers
             const int c_first = (int)(((tg0 + 1) * Cf - 1) / p.G), c_last = (int)((tg1 * Cf - 1) / p.G);
             double2* mine = reinterpret_cast<double2*>(p.part + ((long long)blockIdx.x * 2 + (s_begin == 0 ? 1 : 0)) * (BM * BN)) + tid;
 #pragma unroll
-            for (int ni = 0; ni < NF; ++ni)
+            for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-                for (int hf = 0; hf < 2; ++hf)
-                    __stcg(mine + (ni * 2 + hf) * PSK_THREADS, make_double2(acc[ni][2 * hf], acc[ni][2 * hf + 1]));
+                for (int ni = 0; ni < NF; ++ni)
+#pragma unroll
+                    for (int hf = 0; hf < 2; ++hf)
+                        __stcg(mine + ((mi * NF + ni) * 2 + hf) * NT, make_double2(acc[mi][ni][2 * hf], acc[mi][ni][2 * hf + 1]));
             __threadfence();
             __syncthreads();
             if (tid == 0) {
-                unsigned int* cnt = p.tile_cnt + (long long)a * p.nt + jt;
+                unsigned int* cnt = p.tile_cnt + (long long)a * p.ntb + jt;
                 const unsigned int old = atomicAdd(cnt, 1u);
                 const unsigned int last = (old == (unsigned int)(c_last - c_first)) ? 1u : 0u;
                 if (last) *cnt = 0u;                      // self-cleaning: every contributor has arrived
@@ -602,57 +652,69 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
             if (have_tile) {
                 __threadfence();
 #pragma unroll
-                for (int ni = 0; ni < NF; ++ni)
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) acc[ni][r] = 0.0;
-                for (int cc = c_first; cc <= c_last; ++cc) {          // contributor (= ascending k) order
-                    const double2* src = reinterpret_cast<const double2*>(p.part + ((long long)cc * 2 + (cc == c_first ? 1 : 0)) * (BM * BN)) + tid;
+                for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
                     for (int ni = 0; ni < NF; ++ni)
 #pragma unroll
-                        for (int hf = 0; hf < 2; ++hf) {
-                            const double2 v = __ldcg(src + (ni * 2 + hf) * PSK_THREADS);
-                            acc[ni][2 * hf] += v.x; acc[ni][2 * hf + 1] += v.y;
-                        }
+                        for (int r = 0; r < 4; ++r) acc[mi][ni][r] = 0.0;
+                for (int cc = c_first; cc <= c_last; ++cc) {          // contributor (= ascending k) order
+                    const double2* src = reinterpret_cast<const double2*>(p.part + ((long long)cc * 2 + (cc == c_first ? 1 : 0)) * (BM * BN)) + tid;
+#pragma unroll
+                    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+                        for (int ni = 0; ni < NF; ++ni)
+#pragma unroll
+                            for (int hf = 0; hf < 2; ++hf) {
+                                const double2 v = __ldcg(src + ((mi * NF + ni) * 2 + hf) * NT);
+                                acc[mi][ni][2 * hf] += v.x; acc[mi][ni][2 * hf + 1] += v.y;
+                            }
                 }
             }
         }
         if (!have_tile) continue;
 
-        // ---- complete tile: optional store of the solved rows, squared row norms of this column tile
-        if (p.Vout) {
-            const int col = (p.upper ? p.nt - 1 - jt : jt) * BN + warp * 16 + g;
-            double* vo = p.Vout + (long long)a * p.sV + col;
+        // ---- complete tile: optional store of the solved rows, squared row norms of each 128-column group
+        const int jta = p.upper ? p.ntb - 1 - jt : jt;
+        const int row0 = jta * BN + warp * 32;                       // this warp's first L-row
+        if (p.Vout && row0 < p.nk * BK) {                             // none past Npad (the half tile's zero rows)
+            double* vo = p.Vout + (long long)a * p.sV + row0 + g;
+#pragma unroll
+            for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+                for (int ni = 0; ni < NF; ++ni)
+#pragma unroll
+                    for (int r = 0; r < 4; ++r)
+                        vo[(long long)(ni * 8 + 2 * t + (r & 1)) * p.ldv + 16 * mi + 8 * (r >> 1)] = acc[mi][ni][r];
+        }
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
             for (int ni = 0; ni < NF; ++ni)
 #pragma unroll
-                for (int r = 0; r < 4; ++r)
-                    vo[(long long)(ni * 8 + 2 * t + (r & 1)) * p.ldv + 8 * (r >> 1)] = acc[ni][r];
-        }
-#pragma unroll
-        for (int ni = 0; ni < NF; ++ni)
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                double r = acc[ni][j] * acc[ni][j];                   // L-row g, then g + 8
-                r = fma(acc[ni][j + 2], acc[ni][j + 2], r);
-                r += __shfl_xor_sync(0xffffffffu, r, 4);
-                r += __shfl_xor_sync(0xffffffffu, r, 8);
-                r += __shfl_xor_sync(0xffffffffu, r, 16);
-                if (g == 0) red[warp][ni * 8 + 2 * t + j] = r;
-            }
+                for (int j = 0; j < 2; ++j) {
+                    double r = acc[mi][ni][j] * acc[mi][ni][j];       // L-row g, then g + 8
+                    r = fma(acc[mi][ni][j + 2], acc[mi][ni][j + 2], r);
+                    r += __shfl_xor_sync(0xffffffffu, r, 4);
+                    r += __shfl_xor_sync(0xffffffffu, r, 8);
+                    r += __shfl_xor_sync(0xffffffffu, r, 16);
+                    if (g == 0) red[2 * warp + mi][ni * 8 + 2 * t + j] = r;   // 16-row block 2w + mi of the tile
+                }
         __syncthreads();
-        if (tid < BM) {
-            double r = 0.0;
+        for (int idx = tid; idx < GR * BM; idx += NT) {             // (group, point): blocks 8 gr .. 8 gr + 7 in order
+            const int gr = idx / BM, pt = idx - gr * BM, col = jta * GR + gr;
+            if (col < p.nt) {
+                double r = 0.0;
 #pragma unroll
-            for (int w = 0; w < 8; ++w) r += red[w][tid];
-            __stcg(p.SQ + ((long long)a * 64 + tid) * p.nt + jt, r);
+                for (int b = 0; b < 8; ++b) r += red[8 * gr + b][pt];
+                __stcg(p.SQ + ((long long)a * 64 + pt) * p.nt + col, r);
+            }
         }
         __threadfence();
         __syncthreads();
         if (tid == 0) {
             unsigned int* cnt = p.out_cnt + a;
             const unsigned int old = atomicAdd(cnt, 1u);
-            const unsigned int last = (old == (unsigned int)(p.nt - 1)) ? 1u : 0u;
+            const unsigned int last = (old == (unsigned int)(p.ntb - 1)) ? 1u : 0u;
             if (last) *cnt = 0u;
             s_flag = last;
         }
@@ -662,9 +724,9 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
         // ---- this CTA completed output a: build its records; last output => publish / assemble
         __threadfence();
         tail_stamp(p.as.dbg, 0, tid);
-        if (p.finalize) psk_finalize_output(p, a, tid, PSK_THREADS);
+        if (p.finalize) psk_finalize_output(p, a, tid, NT);
         tail_stamp(p.as.dbg, 1, tid);
-        psk_step_tail(p, smem, tid, PSK_THREADS, &s_flag, &s_ok);
+        psk_step_tail(p, smem, tid, NT, &s_flag, &s_ok);
     }
     if (p.dbg && threadIdx.x == 0) { unsigned long long t1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1)); p.dbg[2 * blockIdx.x + 1] = t1; }
 }
