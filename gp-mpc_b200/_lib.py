@@ -210,20 +210,22 @@ class Engine:
         self._check(self.lib.gpmpc_set_option(self.h, name.encode(), float(value)))
 
     # -- predict ----------------------------------------------------------------------
-    def predict(self, Z, Sigma=None, method=METHOD_TA, want_cov=True, want_jac=True):
-        """Z:(H,Nx) -> mean:(H,Ny), var:(H,Ny), cov:(H,Ny,Ny)|None, jac:(H,Ny,Nx)|None (host arrays).
-        Building the six ctypes pointer objects was a visible share of a small call, so the call
-        goes through per-shape staging arrays whose pointers are built once; the results are returned as fresh copies."""
+    def _points(self, Z, Sigma):
+        """Z -> (H,Nx); Sigma: None, one (Nx,Nx) for every point or one per point (H,Nx,Nx) -> (Z, Sigma, H, spp)."""
         Z = _f64(Z).reshape(-1, self.Nx)
         H = Z.shape[0]
         spp = 0
         if Sigma is not None:
             Sigma = _f64(Sigma)
-            if Sigma.ndim == 3:
-                assert Sigma.shape == (H, self.Nx, self.Nx)
-                spp = 1
-            else:
-                assert Sigma.shape == (self.Nx, self.Nx)
+            spp = 1 if Sigma.ndim == 3 else 0
+            assert Sigma.shape == ((H, self.Nx, self.Nx) if spp else (self.Nx, self.Nx))
+        return Z, Sigma, H, spp
+
+    def predict(self, Z, Sigma=None, method=METHOD_TA, want_cov=True, want_jac=True):
+        """Z:(H,Nx) -> mean:(H,Ny), var:(H,Ny), cov:(H,Ny,Ny)|None, jac:(H,Ny,Nx)|None (host arrays).
+        Building the six ctypes pointer objects was a visible share of a small call, so the call
+        goes through per-shape staging arrays whose pointers are built once; the results are returned as fresh copies."""
+        Z, Sigma, H, spp = self._points(Z, Sigma)
         key = (H, spp, Sigma is None, bool(want_cov), bool(want_jac))
         with self._stage_lock:
             st = self._stage.get(key)
@@ -284,13 +286,7 @@ class Engine:
         """Predict + first derivatives w.r.t. the test inputs (gpmpc_predict_grad).
         Returns dict(mean (H,Ny), var, cov (H,Ny,Ny), jac = dmean_dz (H,Ny,Nx), dvar_dz (H,Ny,Nx),
         dcov_dz (H,Ny,Ny,Nx)[, hess (H,Ny,Nx,Nx)])."""
-        Z = _f64(Z).reshape(-1, self.Nx)
-        H = Z.shape[0]
-        spp = 0
-        if Sigma is not None:
-            Sigma = _f64(Sigma)
-            spp = 1 if Sigma.ndim == 3 else 0
-            assert Sigma.shape == ((H, self.Nx, self.Nx) if spp else (self.Nx, self.Nx))
+        Z, Sigma, H, spp = self._points(Z, Sigma)
         out = dict(mean=np.empty((H, self.Ny)), var=np.empty((H, self.Ny)), cov=np.empty((H, self.Ny, self.Ny)),
                    jac=np.empty((H, self.Ny, self.Nx)), dvar_dz=np.empty((H, self.Ny, self.Nx)),
                    dcov_dz=np.empty((H, self.Ny, self.Ny, self.Nx)))
@@ -304,13 +300,7 @@ class Engine:
     def predict_hess(self, Z, Sigma=None, method=METHOD_TA):
         """predict_grad(..., want_hess=True) plus the second derivatives w.r.t. the test inputs (gpmpc_predict_hess):
         d2var_dz2 (H,Ny,Nx,Nx), d3mean_dz3 (H,Ny,Nx,Nx,Nx), d2cov_dz2 (H,Ny,Ny,Nx,Nx)."""
-        Z = _f64(Z).reshape(-1, self.Nx)
-        H = Z.shape[0]
-        spp = 0
-        if Sigma is not None:
-            Sigma = _f64(Sigma)
-            spp = 1 if Sigma.ndim == 3 else 0
-            assert Sigma.shape == ((H, self.Nx, self.Nx) if spp else (self.Nx, self.Nx))
+        Z, Sigma, H, spp = self._points(Z, Sigma)
         Ny, Nx = self.Ny, self.Nx
         out = dict(mean=np.empty((H, Ny)), var=np.empty((H, Ny)), cov=np.empty((H, Ny, Ny)), jac=np.empty((H, Ny, Nx)),
                    dvar_dz=np.empty((H, Ny, Nx)), dcov_dz=np.empty((H, Ny, Ny, Nx)), hess=np.empty((H, Ny, Nx, Nx)),
@@ -326,11 +316,7 @@ class Engine:
         """'EM' prediction + first derivatives w.r.t. the test input mean and the input covariance
         (gpmpc_predict_em_grad).  Sigma: (Nx,Nx) shared or (H,Nx,Nx).  Returns dict(mean (H,Ny), var, cov (H,Ny,Ny),
         dmean_dz (H,Ny,Nx), dmean_dSigma (H,Ny,Nx,Nx), dcov_dz (H,Ny,Ny,Nx), dcov_dSigma (H,Ny,Ny,Nx,Nx))."""
-        Z = _f64(Z).reshape(-1, self.Nx)
-        H = Z.shape[0]
-        Sigma = _f64(Sigma)
-        spp = 1 if Sigma.ndim == 3 else 0
-        assert Sigma.shape == ((H, self.Nx, self.Nx) if spp else (self.Nx, self.Nx))
+        Z, Sigma, H, spp = self._points(Z, Sigma)
         Ny, Nx = self.Ny, self.Nx
         out = dict(mean=np.empty((H, Ny)), var=np.empty((H, Ny)), cov=np.empty((H, Ny, Ny)),
                    dmean_dz=np.empty((H, Ny, Nx)), dmean_dSigma=np.empty((H, Ny, Nx, Nx)),

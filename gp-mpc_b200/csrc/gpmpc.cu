@@ -529,6 +529,11 @@ static int ensure_pinned(gpmpc_handle_t h, size_t bytes)
     return GPMPC_OK;
 }
 
+// the caches derived from the factor (Li^T for predict_grad, K^-1 for the EM derivatives) no longer match it
+static void factor_caches_stale(gpmpc_handle_t h) { h->u_valid = false; h->em_kinv_valid = false; }
+// the factor no longer matches the data or hyper-parameters, or its slabs were used as scratch: gpmpc_factorize first
+static void factor_stale(gpmpc_handle_t h) { h->factorized = false; factor_caches_stale(h); }
+
 extern "C" int gpmpc_set_data(gpmpc_handle_t h, const double* X, const double* Y)
 {
     if (!h || !X || !Y) return GPMPC_ERR_ARG;
@@ -549,7 +554,7 @@ extern "C" int gpmpc_set_data(gpmpc_handle_t h, const double* X, const double* Y
     CUDA_TRY(cudaMemcpyAsync(h->dXT, xt.data(), xt.size() * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaMemcpyAsync(h->dY, yl.data(), yl.size() * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
-    h->has_data = true; h->factorized = false;
+    h->has_data = true; factor_stale(h);
     return GPMPC_OK;
 }
 
@@ -566,7 +571,7 @@ extern "C" int gpmpc_set_y(gpmpc_handle_t h, int a, const double* y)
     if (al < 0) return GPMPC_ERR_ARG;
     CUDA_TRY(cudaMemcpyAsync(h->dY + (long long)al * h->Npad, y, (size_t)h->N * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
-    h->factorized = false; h->em_kinv_valid = false;
+    factor_stale(h);
     return GPMPC_OK;
 }
 
@@ -583,7 +588,7 @@ extern "C" int gpmpc_set_hyper(gpmpc_handle_t h, const double* hyper, int ld)
         }
     CUDA_TRY(cudaMemcpyAsync(h->dHyp, h->hyper.data(), h->hyper.size() * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
-    h->has_hyper = true; h->factorized = false; h->em_kinv_valid = false;
+    h->has_hyper = true; factor_stale(h);
     return GPMPC_OK;
 }
 
@@ -668,7 +673,7 @@ extern "C" int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info)
     CUDA_TRY(cudaMemcpyAsync(res.data(), h->dRes, 2 * nl * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
     for (int a = 0; a < nl; ++a) { h->logdet[a] = res[2 * a]; h->yalpha[a] = res[2 * a + 1]; }
-    h->factorized = true; h->u_valid = false; h->em_kinv_valid = false;
+    factor_caches_stale(h); h->factorized = true;
     return GPMPC_OK;
 }
 
@@ -709,7 +714,7 @@ extern "C" int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* 
     if (al < 0) return GPMPC_ERR_ARG;
     const int m = h->Nx + 2;
     for (int d = 0; d < h->Nx; ++d) if (theta[d] == 0.0) { set_error(h, "gpmpc_nlml: zero length scale"); return GPMPC_ERR_ARG; }
-    h->factorized = false; h->em_kinv_valid = false;
+    factor_stale(h);
     NvtxRange nvtx_r("gpmpc.nlml");
     CUDA_TRY(cudaMemcpyAsync(h->dHypTmp, theta, m * 8, cudaMemcpyHostToDevice, h->st));
     int used = 0;
@@ -796,6 +801,9 @@ static inline int ks_chunk(gpmpc_handle_t h)
 // blocks of the ks kernel along the training points (one partial record each)
 static inline int ks_blocks(gpmpc_handle_t h) { return (h->Npad + ks_chunk(h) - 1) / ks_chunk(h); }
 
+// rows of the A-side tile (BM) of the predict product for n <= HB solved rows, and of the ks kernel's grid
+static inline int round8(int n) { return (n + 7) / 8 * 8; }
+
 // the solved rows v (and r, for refinement and append) of one 64-point chunk, every output
 static int ensure_rows(gpmpc_handle_t h)
 {
@@ -858,21 +866,6 @@ static cudaError_t psk_launch_bm(const PredictParams& p, const double* A, long l
     return cudaLaunchKernelEx(&cfg, predict_streamk_kernel<BM>, p, tmA, tmB);
 }
 
-static cudaError_t psk_launch(int bm, const PredictParams& p, const double* A, long long sA, const double* B, long long sB,
-                              int np, int grid, cudaStream_t st)
-{
-    switch (bm) {
-    case 8: return psk_launch_bm<8>(p, A, sA, B, sB, np, grid, st);
-    case 16: return psk_launch_bm<16>(p, A, sA, B, sB, np, grid, st);
-    case 24: return psk_launch_bm<24>(p, A, sA, B, sB, np, grid, st);
-    case 32: return psk_launch_bm<32>(p, A, sA, B, sB, np, grid, st);
-    case 40: return psk_launch_bm<40>(p, A, sA, B, sB, np, grid, st);
-    case 48: return psk_launch_bm<48>(p, A, sA, B, sB, np, grid, st);
-    case 56: return psk_launch_bm<56>(p, A, sA, B, sB, np, grid, st);
-    default: return psk_launch_bm<64>(p, A, sA, B, sB, np, grid, st);
-    }
-}
-
 // persistent grid: PSK_CTAS_PER_SM CTAs per SM, but never fewer than 4 k-steps per CTA (at small N, more CTAs with fewer steps each beat
 // fewer with more -- the fixed cost per CTA overlaps across SMs, the steps do not)
 static int psk_grid(gpmpc_handle_t h, long long G)
@@ -881,6 +874,23 @@ static int psk_grid(gpmpc_handle_t h, long long G)
     ctas = std::min(ctas, PSK_MAX_CTAS);
     const long long by_work = std::max(1LL, G / 4);
     return (int)std::min<long long>(ctas, h->opt_predict_ctas > 0 ? G : by_work);
+}
+
+// the predict product p (psk_base) of A (h-major rows, HB * Npad per output) and the slab B of each output: BM = round8(p.Hc)
+static cudaError_t psk_launch(gpmpc_handle_t h, const PredictParams& p, const double* A, const double* B)
+{
+    const long long sA = (long long)HB * h->Npad, sB = slab(h);
+    const int np = h->Npad, grid = psk_grid(h, p.G);
+    switch (round8(p.Hc)) {
+    case 8: return psk_launch_bm<8>(p, A, sA, B, sB, np, grid, h->st);
+    case 16: return psk_launch_bm<16>(p, A, sA, B, sB, np, grid, h->st);
+    case 24: return psk_launch_bm<24>(p, A, sA, B, sB, np, grid, h->st);
+    case 32: return psk_launch_bm<32>(p, A, sA, B, sB, np, grid, h->st);
+    case 40: return psk_launch_bm<40>(p, A, sA, B, sB, np, grid, h->st);
+    case 48: return psk_launch_bm<48>(p, A, sA, B, sB, np, grid, h->st);
+    case 56: return psk_launch_bm<56>(p, A, sA, B, sB, np, grid, h->st);
+    default: return psk_launch_bm<64>(p, A, sA, B, sB, np, grid, h->st);
+    }
 }
 
 // upper: the L-side operand is upper triangular (its k-step list is shorter when Npad / 128 is odd)
@@ -915,59 +925,57 @@ static AssembleArgs assemble_args(gpmpc_handle_t h, int H, int method, const dou
     as.Sigma = Sigma; as.sigma_per_point = spp;
     as.mean = mean; as.var = var; as.J = J; as.cov = cov;
     as.world = 1;
-    const long long bm1 = (std::min(H, HB) + 7) / 8 * 8;
-    as.stage_g = (assemble_rows_doubles(H, h->Ny, h->Nx) <= psk_pipe_doubles((int)bm1)) ? 1 : 0;
+    as.stage_g = (assemble_rows_doubles(H, h->Ny, h->Nx) <= psk_pipe_doubles(round8(std::min(H, HB)))) ? 1 : 0;
     return as;
 }
 
+// ks rows of the Hc points at dZc into dKST (round8(Hc) rows per output), their mean / Jacobian partials into dPMJ
 template <int NXP, int CH>
-static cudaError_t launch_ks(gpmpc_handle_t h, const double* dZc, int Hc, int bm, int nblk)
+static cudaError_t launch_ks(gpmpc_handle_t h, const double* dZc, int Hc)
 {
-    const int smem = (NXP + 1) * CH * 8;
+    const int smem = (NXP + 1) * CH * 8, nblk = ks_blocks(h);
     const cudaError_t e = smem_opt_in<ks_tile_kernel<NXP, CH>>(smem);      // static + dynamic may pass 48 KB
     if (e != cudaSuccess) return e;
-    dim3 g(nblk, bm / 8, h->nloc);
+    dim3 g(nblk, round8(Hc) / 8, h->nloc);
     ks_tile_kernel<NXP, CH><<<g, 256, smem, h->st>>>(h->dXT, h->Npad, h->N, h->Nx, h->dHyp, h->Nx + 2, h->dAlpha, h->Npad,
                                                      dZc, Hc, h->dKST, h->Npad, (long long)HB * h->Npad, h->dPMJ, nblk);
     return cudaGetLastError();
 }
 
 template <int CH>
-static cudaError_t launch_ks_nx(gpmpc_handle_t h, const double* dZc, int Hc, int bm, int nblk)
+static cudaError_t launch_ks_nx(gpmpc_handle_t h, const double* dZc, int Hc)
 {
     const int Nx = h->Nx;       // register-array extent NXP: the next even count up to 12, then 16 / 24 / 32
-    if (Nx <= 4) return launch_ks<4, CH>(h, dZc, Hc, bm, nblk);
-    if (Nx <= 6) return launch_ks<6, CH>(h, dZc, Hc, bm, nblk);
-    if (Nx <= 8) return launch_ks<8, CH>(h, dZc, Hc, bm, nblk);
-    if (Nx <= 10) return launch_ks<10, CH>(h, dZc, Hc, bm, nblk);
-    if (Nx <= 12) return launch_ks<12, CH>(h, dZc, Hc, bm, nblk);
+    if (Nx <= 4) return launch_ks<4, CH>(h, dZc, Hc);
+    if (Nx <= 6) return launch_ks<6, CH>(h, dZc, Hc);
+    if (Nx <= 8) return launch_ks<8, CH>(h, dZc, Hc);
+    if (Nx <= 10) return launch_ks<10, CH>(h, dZc, Hc);
+    if (Nx <= 12) return launch_ks<12, CH>(h, dZc, Hc);
     if (CH <= 512) {
-        if (Nx <= 16) return launch_ks<16, (CH <= 512 ? CH : 512)>(h, dZc, Hc, bm, nblk);
-        if (Nx <= 24) return launch_ks<24, (CH <= 512 ? CH : 512)>(h, dZc, Hc, bm, nblk);
-        return launch_ks<32, (CH <= 512 ? CH : 512)>(h, dZc, Hc, bm, nblk);
+        if (Nx <= 16) return launch_ks<16, (CH <= 512 ? CH : 512)>(h, dZc, Hc);
+        if (Nx <= 24) return launch_ks<24, (CH <= 512 ? CH : 512)>(h, dZc, Hc);
+        return launch_ks<32, (CH <= 512 ? CH : 512)>(h, dZc, Hc);
     }
     return cudaErrorInvalidValue;                              // ks_chunk never picks 1024 above Nx = 12
 }
 
-// bm = the chunk's row count rounded up to 8 (the rows of the product's A operand)
-static cudaError_t launch_ks_any(gpmpc_handle_t h, const double* dZc, int Hc, int bm, int nblk)
+static cudaError_t launch_ks(gpmpc_handle_t h, const double* dZc, int Hc)
 {
     switch (ks_chunk(h)) {
-    case 1024: return launch_ks_nx<1024>(h, dZc, Hc, bm, nblk);
-    case 512: return launch_ks_nx<512>(h, dZc, Hc, bm, nblk);
-    default: return launch_ks_nx<128>(h, dZc, Hc, bm, nblk);
+    case 1024: return launch_ks_nx<1024>(h, dZc, Hc);
+    case 512: return launch_ks_nx<512>(h, dZc, Hc);
+    default: return launch_ks_nx<128>(h, dZc, Hc);
     }
 }
 
 // rows of Amat (h-major, stride HB*np per output) times T^T with T = Li or L (lower triangular):
 // the solved rows go to Vout (may be null), their per-tile squared norms to dSQ
-static int tri_product(gpmpc_handle_t h, const double* Amat, const double* T, int bm, int Hc, double* Vout)
+static int tri_product(gpmpc_handle_t h, const double* Amat, const double* T, int Hc, double* Vout)
 {
-    const int np = h->Npad;
     PredictParams p;
     psk_base(h, p, Hc);
-    p.Vout = Vout; p.sV = (long long)HB * np; p.ldv = np;
-    CUDA_TRY(psk_launch(bm, p, Amat, (long long)HB * np, T, slab(h), np, psk_grid(h, p.G), h->st));
+    p.Vout = Vout; p.sV = (long long)HB * h->Npad; p.ldv = h->Npad;
+    CUDA_TRY(psk_launch(h, p, Amat, T));
     return GPMPC_OK;
 }
 
@@ -1011,27 +1019,27 @@ static int predict_core(gpmpc_handle_t h, int method, int H, const double* dZ, c
     const bool fused_assemble = (H <= HB) && !nccl_gather && ((long long)H * h->Ny * Nx * 8 <= 64 * 1024);
     for (int h0 = 0; h0 < H; h0 += HB) {
         const int Hc = std::min(HB, H - h0);
-        const int bm = (Hc + 7) / 8 * 8;
         const bool last_chunk = (h0 + HB >= H);
         const double* dZc = dZ + (long long)h0 * Nx;
-        CUDA_TRY(launch_ks_any(h, dZc, Hc, bm, ks_blocks(h)));
+        CUDA_TRY(launch_ks(h, dZc, Hc));
         PredictParams p;
         psk_base(h, p, Hc);
         psk_finalize(h, p, H, h0);
         p.pa = pa; p.use_peers = use_peers; p.publish = last_chunk ? 1 : 0;
         p.as = as; p.do_assemble = (fused_assemble && !h->opt_refine) ? 1 : 0;
         if (!h->opt_refine) {
-            CUDA_TRY(psk_launch(bm, p, h->dKST, (long long)HB * np, h->dLi, slab(h), np, psk_grid(h, p.G), h->st));
+            CUDA_TRY(psk_launch(h, p, h->dKST, h->dLi));
         } else {
             // v1 = Li ks ; r = ks - L v1 ; v = v1 + Li r   (one step of iterative refinement)
-            int rc = tri_product(h, h->dKST, h->dLi, bm, Hc, h->dV);
+            int rc = tri_product(h, h->dKST, h->dLi, Hc, h->dV);
             if (rc) return rc;
-            rc = tri_product(h, h->dV, h->dL, bm, Hc, h->dR);                  // dR = L v1
+            rc = tri_product(h, h->dV, h->dL, Hc, h->dR);                      // dR = L v1
             if (rc) return rc;
+            const int bm = round8(Hc);
             dim3 g((np + 255) / 256, bm, h->nloc);
             axpby_rows_kernel<<<g, 256, 0, h->st>>>(h->dKST, h->dR, 1.0, -1.0, h->dR, np, (long long)HB * np, bm);
             CUDA_TRY(cudaGetLastError());
-            rc = tri_product(h, h->dR, h->dLi, bm, Hc, h->dR2);                // dR2 = Li r
+            rc = tri_product(h, h->dR, h->dLi, Hc, h->dR2);                    // dR2 = Li r
             if (rc) return rc;
             axpby_rows_kernel<<<g, 256, 0, h->st>>>(h->dV, h->dR2, 1.0, 1.0, h->dV, np, (long long)HB * np, bm);
             CUDA_TRY(cudaGetLastError());
@@ -1336,7 +1344,6 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
 {
     const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, np = h->Npad;
     NvtxRange nvtx_r("gpmpc.predict_em");
-    if (h->nloc != Ny) { set_error(h, "EM needs all outputs on one handle (replicate the model, shard the points)"); return GPMPC_ERR_STATE; }
     if (!Sigma) { set_error(h, "EM needs an input covariance"); return GPMPC_ERR_ARG; }
     const int npairs = Ny * (Ny + 1) / 2;
     if (npairs > 1024) { set_error(h, "EM supports Ny <= 44"); return GPMPC_ERR_ARG; }
@@ -1450,24 +1457,32 @@ static int peer_status_check(gpmpc_handle_t h)
     return GPMPC_OK;
 }
 
-static int predict_check(gpmpc_handle_t h, int method, int H)
+// First check of every predict-family entry `fn` (the name its errors carry): a factorised model, H >= 1 and a known method.
+static int predict_guard(gpmpc_handle_t h, const char* fn, int method, int H)
 {
     if (!h) return GPMPC_ERR_ARG;
-    if (!h->factorized) { set_error(h, "gpmpc_predict: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
-    if (H < 1) { set_error(h, "gpmpc_predict: H < 1"); return GPMPC_ERR_ARG; }
-    if (method != GPMPC_METHOD_ME && method != GPMPC_METHOD_TA && method != GPMPC_METHOD_EM) { set_error(h, "gpmpc_predict: unknown method %d", method); return GPMPC_ERR_ARG; }
+    if (!h->factorized) { set_error(h, "%s: call gpmpc_factorize first", fn); return GPMPC_ERR_STATE; }
+    if (H < 1) { set_error(h, "%s: H < 1", fn); return GPMPC_ERR_ARG; }
+    if (method != GPMPC_METHOD_ME && method != GPMPC_METHOD_TA && method != GPMPC_METHOD_EM) { set_error(h, "%s: unknown method %d", fn, method); return GPMPC_ERR_ARG; }
     return GPMPC_OK;
+}
+
+// after an entry's own argument checks: every output on this handle and one rank if all_outputs, then device and buffers
+static int predict_prepare(gpmpc_handle_t h, const char* fn, int H, bool all_outputs)
+{
+    if (all_outputs && (h->nloc != h->Ny || h->world != 1)) { set_error(h, "%s needs all outputs on one handle (replicate the model, shard the points)", fn); return GPMPC_ERR_STATE; }
+    CUDA_TRY(cudaSetDevice(h->device));
+    return ensure_predict_bufs(h, H);
 }
 
 extern "C" int gpmpc_predict_device(gpmpc_handle_t h, int method, int H, const double* dZ, const double* dSigma,
                                     int spp, double* d_mean, double* d_var, double* d_cov, double* d_jac, int sync)
 {
-    int rc = predict_check(h, method, H);
+    int rc = predict_guard(h, __func__, method, H);
     if (rc) return rc;
     if (method == GPMPC_METHOD_EM) { set_error(h, "gpmpc_predict_device: EM needs host inputs (use gpmpc_predict)"); return GPMPC_ERR_ARG; }
     if (!dZ || (method == GPMPC_METHOD_TA && d_cov && !dSigma)) { set_error(h, "gpmpc_predict_device: null Z / Sigma"); return GPMPC_ERR_ARG; }
-    CUDA_TRY(cudaSetDevice(h->device));
-    rc = ensure_predict_bufs(h, H);
+    rc = predict_prepare(h, __func__, H, false);
     if (rc) return rc;
     rc = predict_core(h, method, H, dZ, dSigma, spp, d_mean, d_var, d_cov, d_jac);
     if (rc) return rc;
@@ -1546,20 +1561,19 @@ rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restr
     }
 }
 
-extern "C" int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, const double* z0, const double* U,
-                                   const double* Sigma0, const double* scale, const double* K, const double* x_ref,
-                                   const double* uscale, double* means, double* vars, double* cov_last)
+// gpmpc_rollout_batch and gpmpc_rollout; fn names the entry in errors
+static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, int Nt, const double* z0, const double* U,
+                         const double* Sigma0, const double* scale, const double* K, const double* x_ref,
+                         const double* uscale, double* means, double* vars, double* cov_last)
 {
-    int rc = predict_check(h, method, 1);
+    int rc = predict_guard(h, fn, method, 1);
     if (rc) return rc;
     const int Nx = h->Nx, Ny = h->Ny, Nu = Nx - Ny;
-    if (method == GPMPC_METHOD_EM) { set_error(h, "gpmpc_rollout: methods ME and TA (EM prepares every point on the host)"); return GPMPC_ERR_ARG; }
-    if (B < 1 || Nt < 1 || !z0 || !Sigma0 || !means || !vars || (Nu > 0 && !K && !U)) { set_error(h, "gpmpc_rollout: null argument / B < 1 / Nt < 1"); return GPMPC_ERR_ARG; }
-    if (Nu < 0) { set_error(h, "gpmpc_rollout: needs Nx = Ny + Nu with Nu >= 0 (Nx=%d, Ny=%d)", Nx, Ny); return GPMPC_ERR_ARG; }
-    if (K && Nu == 0) { set_error(h, "gpmpc_rollout: a feedback gain needs inputs (Nu = 0)"); return GPMPC_ERR_ARG; }
-    if (h->world != 1 || h->nloc != Ny) { set_error(h, "gpmpc_rollout: all outputs must live on this handle"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
-    rc = ensure_predict_bufs(h, B);
+    if (method == GPMPC_METHOD_EM) { set_error(h, "%s: methods ME and TA (EM prepares every point on the host)", fn); return GPMPC_ERR_ARG; }
+    if (B < 1 || Nt < 1 || !z0 || !Sigma0 || !means || !vars || (Nu > 0 && !K && !U)) { set_error(h, "%s: null argument / B < 1 / Nt < 1", fn); return GPMPC_ERR_ARG; }
+    if (Nu < 0) { set_error(h, "%s: needs Nx = Ny + Nu with Nu >= 0 (Nx=%d, Ny=%d)", fn, Nx, Ny); return GPMPC_ERR_ARG; }
+    if (K && Nu == 0) { set_error(h, "%s: a feedback gain needs inputs (Nu = 0)", fn); return GPMPC_ERR_ARG; }
+    rc = predict_prepare(h, fn, B, true);
     if (rc) return rc;
     NvtxRange nvtx_r("gpmpc.rollout");
     // device slab: [Z (B,Nx) | Sigma (B,Nx,Nx) | U (B,Nt,Nu) | scale (4,Ny) | K (Nu,Ny) | x_ref (Ny) | uscale (2,Nu) |
@@ -1610,26 +1624,30 @@ extern "C" int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, 
     return GPMPC_OK;
 }
 
+extern "C" int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, const double* z0, const double* U,
+                                   const double* Sigma0, const double* scale, const double* K, const double* x_ref,
+                                   const double* uscale, double* means, double* vars, double* cov_last)
+{
+    return rollout_batch(h, __func__, method, B, Nt, z0, U, Sigma0, scale, K, x_ref, uscale, means, vars, cov_last);
+}
+
 // the single open-loop trajectory: B = 1 of the batched loop
 extern "C" int gpmpc_rollout(gpmpc_handle_t h, int method, int Nt, const double* z0, const double* U, const double* Sigma0,
                              const double* scale, double* means, double* vars, double* cov_last)
 {
-    return gpmpc_rollout_batch(h, method, 1, Nt, z0, U, Sigma0, scale, nullptr, nullptr, nullptr, means, vars, cov_last);
+    return rollout_batch(h, __func__, method, 1, Nt, z0, U, Sigma0, scale, nullptr, nullptr, nullptr, means, vars, cov_last);
 }
 
 extern "C" int gpmpc_predict(gpmpc_handle_t h, int method, int H, const double* Z, const double* Sigma,
                              int spp, double* mean, double* var, double* cov, double* jac)
 {
-    int rc = predict_check(h, method, H);
+    int rc = predict_guard(h, __func__, method, H);
     if (rc) return rc;
     if (!Z || (method == GPMPC_METHOD_TA && cov && !Sigma)) { set_error(h, "gpmpc_predict: null Z / Sigma"); return GPMPC_ERR_ARG; }
-    CUDA_TRY(cudaSetDevice(h->device));
-    rc = ensure_predict_bufs(h, H);
+    if (method == GPMPC_METHOD_EM && jac) { set_error(h, "gpmpc_predict: EM does not return a Jacobian"); return GPMPC_ERR_ARG; }
+    rc = predict_prepare(h, __func__, H, method == GPMPC_METHOD_EM);
     if (rc) return rc;
-    if (method == GPMPC_METHOD_EM) {
-        if (jac) { set_error(h, "gpmpc_predict: EM does not return a Jacobian"); return GPMPC_ERR_ARG; }
-        return predict_em(h, H, Z, Sigma, spp, mean, var, cov);
-    }
+    if (method == GPMPC_METHOD_EM) return predict_em(h, H, Z, Sigma, spp, mean, var, cov);
     const int Nx = h->Nx, Ny = h->Ny;
     const size_t nz = (size_t)H * Nx, ns = (method == GPMPC_METHOD_TA && Sigma) ? (size_t)(spp ? H : 1) * Nx * Nx : 0;
     const size_t nm = (size_t)H * Ny, nj = (size_t)H * Ny * Nx, nc = (size_t)H * Ny * Ny;
@@ -1651,7 +1669,7 @@ extern "C" int gpmpc_predict(gpmpc_handle_t h, int method, int H, const double* 
     // Small batches skip both copy operations: the ks kernel reads Z / Sigma from the mapped pinned buffer
     // (each of its CTAs reads HG x Nx doubles once: only worthwhile while that re-read volume is small) and the
     // assembling CTA writes mean / var / J / cov straight into it (posted writes, visible after the stream sync).
-    const long long ks_ctas = (long long)ks_blocks(h) * ((std::min(H, HB) + 7) / 8 * 8) * h->nloc;
+    const long long ks_ctas = (long long)ks_blocks(h) * round8(std::min(H, HB)) * h->nloc;
     const bool zc_in = H <= HB && ks_ctas * Nx * 8 <= 256 * 1024 && in_span * 8 <= 64 * 1024;
     const bool zc_out = out_span * 8 <= 1024 * 1024;
     double* po = pin + in_span;
@@ -1714,7 +1732,7 @@ static int hess_chunk(gpmpc_handle_t h, const double* dZc, int Hc, int H, int h0
         hess_rows_kernel<<<dim3((np + 255) / 256, Rc, h->nloc), 256, 0, h->st>>>(h->dXT, np, h->N, Nx, h->dHyp, Nx + 2, dZc,
                                                                                 h->dKST, np, (long long)HB * np, h->dDR, p0);
         CUDA_TRY(cudaGetLastError());
-        int rc = tri_product(h, h->dDR, h->dLi, (rows + 7) / 8 * 8, rows, h->dVD);
+        int rc = tri_product(h, h->dDR, h->dLi, rows, h->dVD);
         if (rc) return rc;
         CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_hess_reduce<decltype(nxp)::value>(h, dZc, Hc, p0, Rc, nblk); }));
     }
@@ -1733,13 +1751,11 @@ static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, c
                           double* mean, double* var, double* cov, double* jac,
                           double* dvar_dz, double* dcov_dz, double* hess, const HessOutputs* ho)
 {
-    int rc = predict_check(h, method, H);
+    int rc = predict_guard(h, fn, method, H);
     if (rc) return rc;
     if (method == GPMPC_METHOD_EM) { set_error(h, "%s: derivatives are available for ME and TA", fn); return GPMPC_ERR_ARG; }
     if (!Z || (method == GPMPC_METHOD_TA && !Sigma)) { set_error(h, "%s: null Z / Sigma", fn); return GPMPC_ERR_ARG; }
-    if (h->nloc != h->Ny || h->world != 1) { set_error(h, "%s needs all outputs on one handle (replicate the model, shard the points)", fn); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
-    rc = ensure_predict_bufs(h, H);
+    rc = predict_prepare(h, fn, H, true);
     if (rc) return rc;
     NvtxRange nvtx_r(ho ? "gpmpc.predict_hess" : "gpmpc.predict_grad");
     const int np = h->Npad, Nx = h->Nx, Ny = h->Ny, npairs = Nx * (Nx + 1) / 2;
@@ -1783,17 +1799,17 @@ static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, c
     if (ns) CUDA_TRY(cudaMemcpyAsync(h->dSigma, Sigma, ns * 8, cudaMemcpyHostToDevice, h->st));
     const AssembleArgs as = assemble_args(h, H, method, h->dSigma, spp, h->dMean, h->dVar, h->dJ, h->dCov);
     for (int h0 = 0; h0 < H; h0 += HB) {
-        const int Hc = std::min(HB, H - h0), bm = (Hc + 7) / 8 * 8;
+        const int Hc = std::min(HB, H - h0);
         const double* dZc = h->dZ + (long long)h0 * Nx;
-        CUDA_TRY(launch_ks_any(h, dZc, Hc, bm, ks_blocks(h)));
+        CUDA_TRY(launch_ks(h, dZc, Hc));
         PredictParams p;
         psk_base(h, p, Hc);                                   // v = Linv ks: records + the rows themselves
         psk_finalize(h, p, H, h0);
         p.Vout = h->dV; p.sV = (long long)HB * np; p.ldv = np;
-        CUDA_TRY(psk_launch(bm, p, h->dKST, (long long)HB * np, h->dLi, slab(h), np, psk_grid(h, p.G), h->st));
+        CUDA_TRY(psk_launch(h, p, h->dKST, h->dLi));
         psk_base(h, p, Hc, 1);                                // beta = Linv^T v = K^-1 ks  (rows of V times U^T)
         p.Vout = h->dBeta; p.sV = (long long)HB * np; p.ldv = np;
-        CUDA_TRY(psk_launch(bm, p, h->dV, (long long)HB * np, h->dUall, slab(h), np, psk_grid(h, p.G), h->st));
+        CUDA_TRY(psk_launch(h, p, h->dV, h->dUall));
         CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_grad_reduce<decltype(nxp)::value>(h, dZc, Hc, nblk_g); }));
         grad_finalize_kernel<<<dim3(Hc, h->nloc), 128, 0, h->st>>>(h->dPDV, h->dPH, nblk_g, Hc, h->dHyp, Nx + 2, Nx, Ny,
                                                                    h->dG, H, h0, d_dvar, d_hess);
@@ -1851,12 +1867,10 @@ extern "C" int gpmpc_predict_em_grad(gpmpc_handle_t h, int H, const double* Z, c
                                      double* mean, double* var, double* cov,
                                      double* dmean_dz, double* dmean_dSigma, double* dcov_dz, double* dcov_dSigma)
 {
-    int rc = predict_check(h, GPMPC_METHOD_EM, H);
+    int rc = predict_guard(h, __func__, GPMPC_METHOD_EM, H);
     if (rc) return rc;
     if (!Z || !Sigma) { set_error(h, "gpmpc_predict_em_grad: null Z / Sigma"); return GPMPC_ERR_ARG; }
-    if (h->nloc != h->Ny || h->world != 1) { set_error(h, "gpmpc_predict_em_grad needs all outputs on one handle (replicate the model, shard the points)"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
-    rc = ensure_predict_bufs(h, H);
+    rc = predict_prepare(h, __func__, H, true);
     if (rc) return rc;
     NvtxRange nvtx_r("gpmpc.predict_em_grad");
     const EmGradOutputs go = {dmean_dz, dmean_dSigma, dcov_dz, dcov_dSigma};
@@ -1869,13 +1883,12 @@ extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double*
     if (!h || !x_new || !y_new) return GPMPC_ERR_ARG;
     if (!h->factorized) { set_error(h, "gpmpc_append: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
     if (h->N >= h->Npad) { set_error(h, "gpmpc_append: capacity %d reached, refit on a new handle", h->Npad); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
-    int rc = ensure_predict_bufs(h, 1);
+    int rc = predict_prepare(h, __func__, 1, false);
     if (rc) return rc;
     const int N = h->N, Nx = h->Nx, np = h->Npad, nl = h->nloc;
     // k(X, x_new) for every owned output through the predict ks kernel (H = 1): row 0 of KS^T
     CUDA_TRY(cudaMemcpyAsync(h->dZ, x_new, Nx * 8, cudaMemcpyHostToDevice, h->st));
-    CUDA_TRY(launch_ks_any(h, h->dZ, 1, 8, ks_blocks(h)));
+    CUDA_TRY(launch_ks(h, h->dZ, 1));
     // l = Li k (rows < N), r = Li^T l
     rc = ensure_rows(h);
     if (rc) return rc;
@@ -1899,13 +1912,13 @@ extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double*
     CUDA_TRY(cudaStreamSynchronize(h->st));
     for (int a = 0; a < nl; ++a)
         if (inf[a]) {
-            h->factorized = false;       // row N of that output is unusable: the caller must refactorise
+            factor_stale(h);             // row N of that output is unusable: the caller must refactorise
             set_error(h, "gpmpc_append: output %d lost positive definiteness (refactorise, jitter applies there)", h->a0 + a);
             h->N = N + 1;
             return GPMPC_ERR_NOTPD;
         }
     h->N = N + 1;
-    h->u_valid = false; h->em_kinv_valid = false;
+    factor_caches_stale(h);
     rc = launch_alpha(h, 0, nl);
     if (rc) return rc;
     std::vector<double> res(2 * nl);
@@ -1919,8 +1932,7 @@ extern "C" int gpmpc_posterior_cov(gpmpc_handle_t h, int H, const double* Z, dou
 {
     if (!h || !Z || !out || H < 1) return GPMPC_ERR_ARG;
     if (!h->factorized) { set_error(h, "gpmpc_posterior_cov: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
-    int rc = ensure_predict_bufs(h, H);
+    int rc = predict_prepare(h, __func__, H, false);
     if (rc) return rc;
     const int np = h->Npad, Nx = h->Nx, nl = h->nloc;
     const long long sVall = (long long)H * np;            // all H solved rows of one output
@@ -1931,10 +1943,10 @@ extern "C" int gpmpc_posterior_cov(gpmpc_handle_t h, int H, const double* Z, dou
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, (size_t)H * Nx * 8, cudaMemcpyHostToDevice, h->st));
     for (int h0 = 0; h0 < H; h0 += HB) {
-        const int Hc = std::min(HB, H - h0), bm = (Hc + 7) / 8 * 8;
+        const int Hc = std::min(HB, H - h0);
         const double* dZc = h->dZ + (long long)h0 * Nx;
-        CUDA_TRY(launch_ks_any(h, dZc, Hc, bm, ks_blocks(h)));
-        rc = tri_product(h, h->dKST, h->dLi, bm, Hc, h->dV);
+        CUDA_TRY(launch_ks(h, dZc, Hc));
+        rc = tri_product(h, h->dKST, h->dLi, Hc, h->dV);
         if (rc) return rc;
         copy2d_kernel<<<dim3(16, std::min(Hc, 64), nl), 128, 0, h->st>>>(h->dV, np, (long long)HB * np,
                                                                      h->dCovV + (long long)h0 * np, np, sVall, Hc, np);
@@ -2042,29 +2054,41 @@ extern "C" int gpmpc_synchronize(gpmpc_handle_t h)
     return peer_status_check(h);
 }
 
+// gpmpc_profile_balance / _tail (fn): two stamped runs of the predict product over the last predict call's operands, the
+// second one warm.  setup(p, tail) adds what the entry profiles; t = {start, end} of the grid CTAs, then n_tail stamps.
+template <typename Setup>
+static int profile_product(gpmpc_handle_t h, const char* fn, int H, const double* out, bool all_outputs, int n_tail,
+                           Setup&& setup, std::vector<unsigned long long>& t, int* grid)
+{
+    if (!h || !out || H < 1 || H > HB) return GPMPC_ERR_ARG;
+    int rc = predict_guard(h, fn, GPMPC_METHOD_TA, H);
+    if (rc) return rc;
+    rc = predict_prepare(h, fn, HB, all_outputs);
+    if (rc) return rc;
+    PredictParams p;
+    psk_base(h, p, H);
+    *grid = psk_grid(h, p.G);
+    DevBuf<unsigned long long> dbg;
+    ENSURE(dbg, (long long)*grid * 2 + n_tail);
+    p.dbg = dbg;
+    setup(p, dbg + 2 * *grid);
+    for (int rep = 0; rep < 2; ++rep) {
+        const cudaError_t e = psk_launch(h, p, h->dKST, h->dLi);
+        if (e != cudaSuccess) { set_error(h, "%s: %s", fn, cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
+    }
+    t.resize((size_t)*grid * 2 + n_tail);
+    cudaMemcpyAsync(t.data(), dbg, t.size() * 8, cudaMemcpyDeviceToHost, h->st);
+    cudaStreamSynchronize(h->st);
+    return GPMPC_OK;
+}
+
 // load balance of the persistent predict product: per-CTA busy time (globaltimer at CTA start / end)
 //   out = {shortest CTA, longest CTA, mean CTA, first start -> last end} in microseconds
 extern "C" int gpmpc_profile_balance(gpmpc_handle_t h, int H, double* out4)
 {
-    if (!h || !out4 || H < 1 || H > HB) return GPMPC_ERR_ARG;
-    if (!h->factorized) { set_error(h, "gpmpc_profile_balance: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
-    int rc = ensure_predict_bufs(h, HB);
+    std::vector<unsigned long long> t; int grid = 0;
+    const int rc = profile_product(h, __func__, H, out4, false, 0, [](PredictParams&, unsigned long long*) {}, t, &grid);
     if (rc) return rc;
-    PredictParams p;
-    psk_base(h, p, H);
-    const int grid = psk_grid(h, p.G);
-    DevBuf<unsigned long long> dbg;
-    ENSURE(dbg, (long long)grid * 2);
-    p.dbg = dbg;
-    const int np = h->Npad, bm = (H + 7) / 8 * 8;
-    for (int rep = 0; rep < 2; ++rep) {
-        cudaError_t e = psk_launch(bm, p, h->dKST, (long long)HB * np, h->dLi, slab(h), np, grid, h->st);
-        if (e != cudaSuccess) { set_error(h, "profile_balance: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
-    }
-    std::vector<unsigned long long> t((size_t)grid * 2);
-    cudaMemcpyAsync(t.data(), dbg, t.size() * 8, cudaMemcpyDeviceToHost, h->st);
-    cudaStreamSynchronize(h->st);
     unsigned long long lo = ~0ull, hi = 0; double mn = 1e300, mx = 0.0, sum = 0.0;
     for (int c = 0; c < grid; ++c) {
         const double d = (double)(t[2 * c + 1] - t[2 * c]) * 1e-3;
@@ -2080,30 +2104,15 @@ extern "C" int gpmpc_profile_balance(gpmpc_handle_t h, int H, double* out4)
 // J Sigma done, outputs written}, then the kernel's span and the tail CTA's own span.  Needs a predict call before it.
 extern "C" int gpmpc_profile_tail(gpmpc_handle_t h, int H, double* out8)
 {
-    if (!h || !out8 || H < 1 || H > HB) return GPMPC_ERR_ARG;
-    if (!h->factorized) { set_error(h, "gpmpc_profile_tail: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
-    if (h->world != 1 || h->nloc != h->Ny) { set_error(h, "gpmpc_profile_tail: single-rank handles only"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
-    int rc = ensure_predict_bufs(h, HB);
+    std::vector<unsigned long long> t; int grid = 0;
+    auto setup = [&](PredictParams& p, unsigned long long* tail) {
+        psk_finalize(h, p, H, 0);
+        p.as = assemble_args(h, H, GPMPC_METHOD_TA, h->dSigma, 0, h->dMean, h->dVar, h->dJ, h->dCov);
+        p.as.dbg = tail;
+        p.do_assemble = 1;
+    };
+    const int rc = profile_product(h, __func__, H, out8, true, 8, setup, t, &grid);
     if (rc) return rc;
-    const int np = h->Npad, bm = (H + 7) / 8 * 8;
-    PredictParams p;
-    psk_base(h, p, H);
-    const int grid = psk_grid(h, p.G);
-    DevBuf<unsigned long long> dbg;
-    ENSURE(dbg, (long long)grid * 2 + 8);
-    p.dbg = dbg;
-    psk_finalize(h, p, H, 0);
-    p.as = assemble_args(h, H, GPMPC_METHOD_TA, h->dSigma, 0, h->dMean, h->dVar, h->dJ, h->dCov);
-    p.as.dbg = dbg + 2 * grid;
-    p.do_assemble = 1;
-    for (int rep = 0; rep < 2; ++rep) {
-        cudaError_t e = psk_launch(bm, p, h->dKST, (long long)HB * np, h->dLi, slab(h), np, grid, h->st);
-        if (e != cudaSuccess) { set_error(h, "profile_tail: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
-    }
-    std::vector<unsigned long long> t((size_t)grid * 2 + 8);
-    cudaMemcpyAsync(t.data(), dbg, t.size() * 8, cudaMemcpyDeviceToHost, h->st);
-    cudaStreamSynchronize(h->st);
     unsigned long long lo = ~0ull, hi = 0, hi2 = 0; int cmax = 0;
     for (int c = 0; c < grid; ++c) {
         lo = std::min(lo, t[2 * c]);
@@ -2136,7 +2145,7 @@ extern "C" int gpmpc_profile_leaf(gpmpc_handle_t h, double* out15)
     long long* nul = nullptr;
     cudaMemcpyToSymbol(d_leaf_prof, &nul, sizeof(nul));
     for (int k = 0; k < 15; ++k) out15[k] = (double)(hst[k] - hst[0]);
-    h->factorized = false;
+    factor_stale(h);
     return rc;
 }
 
@@ -2148,7 +2157,7 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
     if (!h || !ms_out || reps < 1) return GPMPC_ERR_ARG;
     if (!h->has_data || !h->has_hyper) { set_error(h, "gpmpc_profile: set_data and set_hyper first"); return GPMPC_ERR_STATE; }
     CUDA_TRY(cudaSetDevice(h->device));
-    const int np = h->Npad;
+    const int np = h->Npad, Hc = (n > 0 && n <= HB) ? n : 56;       // Hc: test points of the product selectors
     float ms = 0.f;
     int rc = GPMPC_OK;
     auto run = [&]() -> int {
@@ -2174,31 +2183,28 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
             if (r) return r;
             return potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, np, 1);
         }
-        case GPMPC_PROF_TRIGEMM: {
-            const int Hc = (n > 0 && n <= HB) ? n : 56;
-            return tri_product(h, h->dKST, h->dLi, (Hc + 7) / 8 * 8, Hc, nullptr);
-        }
+        case GPMPC_PROF_TRIGEMM: return tri_product(h, h->dKST, h->dLi, Hc, nullptr);
         case GPMPC_PROF_KS: {             // the ks / mean / Jacobian partial kernel alone (Z = the last batch's inputs)
-            const int Hc = (n > 0 && n <= HB) ? n : 56;
-            cudaError_t e = launch_ks_any(h, h->dZ, Hc, (Hc + 7) / 8 * 8, ks_blocks(h));
+            cudaError_t e = launch_ks(h, h->dZ, Hc);
             if (e != cudaSuccess) { set_error(h, "profile ks: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
             return GPMPC_OK;
         }
         case GPMPC_PROF_PREDICT_TAIL: {   // the fused kernel WITH finalize + assembly, without the ks kernel in front
-            const int Hc = (n > 0 && n <= HB) ? n : 56;
             PredictParams p;
             psk_base(h, p, Hc);
             psk_finalize(h, p, Hc, 0);
             p.as = assemble_args(h, Hc, GPMPC_METHOD_TA, h->dSigma, 0, h->dMean, h->dVar, h->dJ, h->dCov);
             p.do_assemble = (h->world == 1 && h->nloc == h->Ny) ? 1 : 0;
-            cudaError_t e = psk_launch((Hc + 7) / 8 * 8, p, h->dKST, (long long)HB * np, h->dLi, slab(h), np, psk_grid(h, p.G), h->st);
+            cudaError_t e = psk_launch(h, p, h->dKST, h->dLi);
             if (e != cudaSuccess) { set_error(h, "profile predict tail: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
             return GPMPC_OK;
         }
         default: set_error(h, "gpmpc_profile: unknown selector %d", what); return GPMPC_ERR_ARG;
         }
     };
-    if (what == GPMPC_PROF_TRIGEMM || what == GPMPC_PROF_KS || what == GPMPC_PROF_PREDICT_TAIL) { rc = ensure_predict_bufs(h, HB); if (rc) return rc; }
+    // the product selectors run on the predict buffers; the others use the factor's slabs as scratch
+    const bool product = what == GPMPC_PROF_TRIGEMM || what == GPMPC_PROF_KS || what == GPMPC_PROF_PREDICT_TAIL;
+    if (product) { rc = ensure_predict_bufs(h, HB); if (rc) return rc; }
     CUDA_TRY(cudaMemsetAsync(h->dJit, 0, h->nloc * sizeof(double), h->st));
     rc = run();
     if (rc) return rc;
@@ -2209,6 +2215,6 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
     CUDA_TRY(cudaEventSynchronize(h->ev1));
     CUDA_TRY(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
     ms_out[0] = (double)ms / reps;
-    if (what != GPMPC_PROF_TRIGEMM && what != GPMPC_PROF_KS && what != GPMPC_PROF_PREDICT_TAIL) h->factorized = false;   // slabs were used as scratch
+    if (!product) factor_stale(h);
     return GPMPC_OK;
 }
