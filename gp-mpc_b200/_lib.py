@@ -27,6 +27,7 @@ _H = C.c_void_p
 SYMBOLS = [
     ('gpmpc_version', C.c_int, []),
     ('gpmpc_create', C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_H)]),
+    ('gpmpc_create_reserve', C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_H)]),
     ('gpmpc_destroy', C.c_int, [_H]),
     ('gpmpc_last_error', C.c_char_p, [_H]),
     ('gpmpc_set_data', C.c_int, [_H, _dp, _dp]),
@@ -42,6 +43,7 @@ SYMBOLS = [
     ('gpmpc_predict_em_grad', C.c_int, [_H, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     ('gpmpc_get_size', C.c_int, [_H, _ip, _ip, _ip]),
     ('gpmpc_append', C.c_int, [_H, _dp, _dp]),
+    ('gpmpc_append_greedy', C.c_int, [_H, C.c_int, _dp, _dp, C.c_int, _ip, _dp, _ip]),
     ('gpmpc_posterior_cov', C.c_int, [_H, C.c_int, _dp, _dp]),
     ('gpmpc_rollout', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     ('gpmpc_rollout_batch', C.c_int, [_H, C.c_int, C.c_int, C.c_int] + [_dp] * 10),
@@ -126,16 +128,23 @@ def _f64(a, shape=None):
 class Engine:
     """One handle = one GPU.  Thin, typed veneer over the C ABI; all heavy work is CUDA."""
 
-    def __init__(self, N, Nx, Ny, out_begin=0, out_count=None, device=0):
+    def __init__(self, N, Nx, Ny, out_begin=0, out_count=None, device=0, capacity=None):
+        """capacity: training points to reserve room for (gpmpc_create_reserve), so appends up to it need no refit."""
         self.lib = load()
         self.N, self.Nx, self.Ny = int(N), int(Nx), int(Ny)
         self._stage, self._stage_lock = {}, threading.Lock()     # predict(): per-shape host staging arrays + their pointers
         self.out_begin = int(out_begin)
         self.out_count = int(Ny - out_begin if out_count is None else out_count)
         self.device = int(device)
+        # the padded size the library allocates: appends succeed while N stays within it
+        self.capacity = -(-max(self.N, int(capacity or 0)) // 128) * 128
         self.h = _H()
-        rc = self.lib.gpmpc_create(self.N, self.Nx, self.Ny, self.out_begin, self.out_count, self.device,
-                                   C.byref(self.h))
+        if capacity is None:
+            rc = self.lib.gpmpc_create(self.N, self.Nx, self.Ny, self.out_begin, self.out_count, self.device,
+                                       C.byref(self.h))
+        else:
+            rc = self.lib.gpmpc_create_reserve(self.N, int(capacity), self.Nx, self.Ny, self.out_begin, self.out_count,
+                                               self.device, C.byref(self.h))
         if rc != OK:
             msg = self.lib.gpmpc_last_error(None).decode()
             self.h = None
@@ -336,6 +345,26 @@ class Engine:
         self._check(rc)
         self.N += 1
         return True
+
+    def append_greedy(self, Xc, Yc, n_new):
+        """gpmpc_append_greedy: append n_new points of the pool Xc:(n,Nx), Yc:(n,Ny) (GP units), each the one of largest
+        combined posterior variance after the previous appends.  Returns (picked (k,) pool indices in order, score (k,)
+        combined variance at pick time, ok); ok False means positive definiteness was lost at the last pick, as for
+        append (the k points are in, the handle needs a refactorisation)."""
+        Xc = _f64(Xc).reshape(-1, self.Nx)
+        n = Xc.shape[0]
+        Yc = _f64(Yc, (n, self.Ny))
+        n_new = int(n_new)
+        picked = np.zeros(max(n_new, 1), dtype=np.int32)
+        score = np.zeros(max(n_new, 1))
+        added = C.c_int(0)
+        rc = self.lib.gpmpc_append_greedy(self.h, n, _ptr(Xc), _ptr(Yc), n_new, picked.ctypes.data_as(_ip), _ptr(score),
+                                          C.byref(added))
+        if rc not in (OK, ERR_NOTPD):
+            self._check(rc)
+        k = added.value
+        self.N += k
+        return picked[:k].astype(np.int64), score[:k].copy(), rc == OK
 
     def posterior_cov(self, Z):
         """(out_count, H, H): sf2 - V^T V per owned output (GP.covar)."""

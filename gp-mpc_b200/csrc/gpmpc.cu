@@ -96,7 +96,9 @@ struct gpmpc_handle_s {
     DevBuf<double> dKST, dPart, dPMJ, dSQ, dV, dR, dR2;
     DevBuf<unsigned int> dCnt;        // stream-K counters: [nloc*nt tile | nloc output | 1 done], self-cleaning
     int psk_ctas = 0, opt_predict_ctas = 0;   // persistent grid of the predict product (PSK_CTAS_PER_SM per SM)
-    DevBuf<double> dCovV, dCovOut;    // GP.covar scratch pool
+    DevBuf<double> dCovV, dCovOut;    // GP.covar scratch pool; dCovV also holds the greedy selection's pool V
+    DevBuf<double> dGrD;              // gpmpc_append_greedy: [var (nloc, n) | Xc (n, Nx) | Yc (n, Ny) | score (n_new)]
+    DevBuf<int> dGrI;                 //                      [active (n) | picked (n_new) | stop]
     // predict_grad: U = Linv^T per output (lazy), beta rows, partial sums, per-batch derivative slabs
     DevBuf<double> dUall, dBeta, dPDV, dPH, dGradOut; bool u_valid = false;
     // predict_hess: derivative rows d ks / dz and their L^-1 products (lazy), block partials, per-batch second-derivative slabs
@@ -401,11 +403,12 @@ extern "C" const char* gpmpc_last_error(gpmpc_handle_t h) { return h ? h->err : 
 
 extern "C" int gpmpc_destroy(gpmpc_handle_t h);
 
-static int create_fill(gpmpc_handle_t h, int N, int Nx, int Ny, int out_begin, int out_count, int device)
+// N_cap: training points the padded slabs must hold (appends up to it need no refit); the tail past N is identity in K
+static int create_fill(gpmpc_handle_t h, int N, int N_cap, int Nx, int Ny, int out_begin, int out_count, int device)
 {
     h->N = N; h->Nx = Nx; h->Ny = Ny; h->a0 = out_begin; h->nloc = out_count; h->device = device;
     h->nloc_max = out_count; h->world = 1; h->rank = 0;
-    h->Npad = (N + GPMPC_TILE - 1) / GPMPC_TILE * GPMPC_TILE;
+    h->Npad = (std::max(N, N_cap) + GPMPC_TILE - 1) / GPMPC_TILE * GPMPC_TILE;
     CUDA_TRY(cudaSetDevice(device));
     CUDA_TRY(cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, device));
     h->opt_small_tiles = 4 * h->sms;      // two waves of 2 CTAs per SM
@@ -462,12 +465,18 @@ static int create_fill(gpmpc_handle_t h, int N, int Nx, int Ny, int out_begin, i
 
 extern "C" int gpmpc_create(int N, int Nx, int Ny, int out_begin, int out_count, int device, gpmpc_handle_t* out)
 {
+    return gpmpc_create_reserve(N, N, Nx, Ny, out_begin, out_count, device, out);
+}
+
+extern "C" int gpmpc_create_reserve(int N, int N_cap, int Nx, int Ny, int out_begin, int out_count, int device,
+                                    gpmpc_handle_t* out)
+{
     gpmpc_handle_t h = nullptr;
     if (!out) return GPMPC_ERR_ARG;
     *out = nullptr;
     if (N < 1 || Nx < 1 || Nx > NX_MAX || Ny < 1 || out_begin < 0 || out_count < 1 || out_begin + out_count > Ny) {
-        set_error(nullptr, "gpmpc_create: bad sizes N=%d Nx=%d (max %d) Ny=%d outputs [%d,%d)", N, Nx, NX_MAX, Ny,
-                  out_begin, out_begin + out_count);
+        set_error(nullptr, "gpmpc_create: bad sizes N=%d (capacity %d) Nx=%d (max %d) Ny=%d outputs [%d,%d)", N, N_cap, Nx,
+                  NX_MAX, Ny, out_begin, out_begin + out_count);
         return GPMPC_ERR_ARG;
     }
     int ndev = 0;
@@ -484,7 +493,7 @@ extern "C" int gpmpc_create(int N, int Nx, int Ny, int out_begin, int out_count,
         return GPMPC_ERR_CUDA;
     }
     h = new gpmpc_handle_s();
-    const int rc = create_fill(h, N, Nx, Ny, out_begin, out_count, device);
+    const int rc = create_fill(h, N, N_cap, Nx, Ny, out_begin, out_count, device);
     if (rc != GPMPC_OK) {            // no partially built handle survives: message to the create slot, everything freed
         snprintf(g_create_err, sizeof(g_create_err), "gpmpc_create: %s", h->err);
         gpmpc_destroy(h);
@@ -1902,7 +1911,8 @@ extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double*
     trmv_lower_T_kernel<<<g2, 256, 0, h->st>>>(h->dLi, np, slab(h), h->dV, (long long)HB * np, h->dR, (long long)HB * np, np);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemsetAsync(h->dInfo, 0, nl * sizeof(int), h->st));
-    append_row_kernel<<<nl, 256, 0, h->st>>>(h->dL, h->dLi, np, slab(h), h->dV, h->dR, (long long)HB * np, h->dHyp, Nx + 2, Nx, N, h->dInfo);
+    append_row_kernel<<<nl, 256, 0, h->st>>>(h->dL, h->dLi, np, slab(h), h->dV, h->dR, (long long)HB * np, h->dHyp, Nx + 2, Nx, N,
+                                             h->dInfo, nullptr);
     CUDA_TRY(cudaGetLastError());
     std::vector<int> inf(nl, 0);
     CUDA_TRY(cudaMemcpyAsync(inf.data(), h->dInfo, nl * sizeof(int), cudaMemcpyDeviceToHost, h->st));
@@ -1928,23 +1938,19 @@ extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double*
     return GPMPC_OK;
 }
 
-extern "C" int gpmpc_posterior_cov(gpmpc_handle_t h, int H, const double* Z, double* out)
+// The solved rows v = L^-1 k(X, z) of the H points at dZ (device, (H, Nx)) for every owned output into the pooled dCovV,
+// layout (nloc, H, Npad) with row stride Npad: HB-point chunks through the ks kernel and the predict product.
+static int solve_rows(gpmpc_handle_t h, const double* dZ, int H)
 {
-    if (!h || !Z || !out || H < 1) return GPMPC_ERR_ARG;
-    if (!h->factorized) { set_error(h, "gpmpc_posterior_cov: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
-    int rc = predict_prepare(h, __func__, H, false);
-    if (rc) return rc;
     const int np = h->Npad, Nx = h->Nx, nl = h->nloc;
     const long long sVall = (long long)H * np;            // all H solved rows of one output
     // scratch is pooled on the handle (grown on demand), not allocated per call
     ENSURE(h->dCovV, (long long)nl * sVall);
-    ENSURE(h->dCovOut, (long long)nl * H * H);
-    rc = ensure_rows(h);
+    int rc = ensure_rows(h);
     if (rc) return rc;
-    CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, (size_t)H * Nx * 8, cudaMemcpyHostToDevice, h->st));
     for (int h0 = 0; h0 < H; h0 += HB) {
         const int Hc = std::min(HB, H - h0);
-        const double* dZc = h->dZ + (long long)h0 * Nx;
+        const double* dZc = dZ + (long long)h0 * Nx;
         CUDA_TRY(launch_ks(h, dZc, Hc));
         rc = tri_product(h, h->dKST, h->dLi, Hc, h->dV);
         if (rc) return rc;
@@ -1952,10 +1958,119 @@ extern "C" int gpmpc_posterior_cov(gpmpc_handle_t h, int H, const double* Z, dou
                                                                      h->dCovV + (long long)h0 * np, np, sVall, Hc, np);
         CUDA_TRY(cudaGetLastError());
     }
+    return GPMPC_OK;
+}
+
+extern "C" int gpmpc_posterior_cov(gpmpc_handle_t h, int H, const double* Z, double* out)
+{
+    if (!h || !Z || !out || H < 1) return GPMPC_ERR_ARG;
+    if (!h->factorized) { set_error(h, "gpmpc_posterior_cov: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
+    int rc = predict_prepare(h, __func__, H, false);
+    if (rc) return rc;
+    const int np = h->Npad, Nx = h->Nx, nl = h->nloc;
+    const long long sVall = (long long)H * np;
+    ENSURE(h->dCovOut, (long long)nl * H * H);
+    CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, (size_t)H * Nx * 8, cudaMemcpyHostToDevice, h->st));
+    rc = solve_rows(h, h->dZ, H);
+    if (rc) return rc;
     gram_cov_kernel<<<dim3(H, H, nl), 256, 0, h->st>>>(h->dCovV, np, sVall, np, h->dHyp, Nx + 2, Nx, H, h->dCovOut);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(out, h->dCovOut, (size_t)nl * H * H * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
+    return GPMPC_OK;
+}
+
+// Greedy max-variance selection (kernels.cuh, greedy_*): the pool's V and variances are formed once, then each step
+// appends the candidate with the largest combined variance by the rank-1 update of gpmpc_append and downdates the rest.
+// Every step is enqueued back to back (Nk = N + k is known here); one synchronisation at the end.
+extern "C" int gpmpc_append_greedy(gpmpc_handle_t h, int n, const double* Xc, const double* Yc, int n_new,
+                                   int* picked, double* score, int* n_added)
+{
+    if (!h) return GPMPC_ERR_ARG;
+    if (!Xc || !Yc || !picked || !n_added) { set_error(h, "gpmpc_append_greedy: null Xc / Yc / picked / n_added"); return GPMPC_ERR_ARG; }
+    *n_added = 0;
+    if (n < 1 || n_new < 0 || n_new > n) { set_error(h, "gpmpc_append_greedy: need n >= 1 and 0 <= n_new <= n (n = %d, n_new = %d)", n, n_new); return GPMPC_ERR_ARG; }
+    if (!h->factorized) { set_error(h, "gpmpc_append_greedy: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
+    int rc = predict_prepare(h, __func__, 1, true);
+    if (rc) return rc;
+    if (h->N + n_new > h->Npad) {
+        set_error(h, "gpmpc_append_greedy: N + n_new = %d exceeds the capacity %d (reserve it with gpmpc_create_reserve)", h->N + n_new, h->Npad);
+        return GPMPC_ERR_STATE;
+    }
+    if (n_new == 0) return GPMPC_OK;
+    NvtxRange nvtx_r("gpmpc.append_greedy");
+    const int N = h->N, Nx = h->Nx, np = h->Npad, nl = h->nloc;
+    const long long sV = (long long)n * np, sl = (long long)HB * np;
+    ENSURE(h->dGrD, (long long)nl * n + (long long)n * (Nx + nl) + n_new);
+    ENSURE(h->dGrI, (long long)n + n_new + 1);
+    double* dVar = h->dGrD;
+    double* dXc = dVar + (long long)nl * n;
+    double* dYc = dXc + (long long)n * Nx;
+    double* dScore = dYc + (long long)n * nl;
+    int* dAct = h->dGrI;
+    int* dPick = dAct + n;
+    int* dStop = dPick + n_new;
+    {
+        const std::vector<int> ones(n, 1);
+        CUDA_TRY(cudaMemcpyAsync(dAct, ones.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, h->st));
+    }
+    CUDA_TRY(cudaMemcpyAsync(dXc, Xc, (size_t)n * Nx * 8, cudaMemcpyHostToDevice, h->st));
+    CUDA_TRY(cudaMemcpyAsync(dYc, Yc, (size_t)n * nl * 8, cudaMemcpyHostToDevice, h->st));
+    CUDA_TRY(cudaMemsetAsync(dStop, 0, sizeof(int), h->st));
+    CUDA_TRY(cudaMemsetAsync(h->dInfo, 0, nl * sizeof(int), h->st));
+    rc = solve_rows(h, dXc, n);
+    if (rc) return rc;
+    const dim3 gw((n + 7) / 8, nl);
+    greedy_var_kernel<<<gw, 256, 0, h->st>>>(h->dCovV, np, sV, N, n, h->dHyp, Nx + 2, Nx, dVar);
+    CUDA_TRY(cudaGetLastError());
+    for (int k = 0; k < n_new; ++k) {
+        const int Nk = N + k;
+        greedy_pick_kernel<<<1, 1024, 0, h->st>>>(dVar, n, nl, dAct, dXc, dYc, Nx, h->dXT, h->dY, np, Nk, h->dInfo, dStop,
+                                                 dPick, dScore, k);
+        CUDA_TRY(cudaGetLastError());
+        greedy_gather_kernel<<<dim3((np + 255) / 256, nl), 256, 0, h->st>>>(h->dCovV, np, sV, dPick, k, Nk, h->dV, sl, np, dStop);
+        CUDA_TRY(cudaGetLastError());
+        // r = Li^T l over the Nk rows l occupies (scratch: after a failed pivot it is computed and never read)
+        trmv_lower_T_kernel<<<dim3((Nk + 31) / 32, 1, nl), 256, 0, h->st>>>(h->dLi, np, slab(h), h->dV, sl, h->dR, sl, Nk);
+        CUDA_TRY(cudaGetLastError());
+        append_row_kernel<<<nl, 256, 0, h->st>>>(h->dL, h->dLi, np, slab(h), h->dV, h->dR, sl, h->dHyp, Nx + 2, Nx, Nk,
+                                                 h->dInfo, dStop);
+        CUDA_TRY(cudaGetLastError());
+        greedy_downdate_kernel<<<gw, 256, 0, h->st>>>(h->dCovV, np, sV, dVar, n, dAct, h->dV, sl, h->dL, np, slab(h), dXc, Nx,
+                                                     h->dHyp, Nx + 2, dPick, k, Nk, h->dInfo, nl);
+        CUDA_TRY(cudaGetLastError());
+    }
+    std::vector<int> inf(nl, 0), pk(n_new, 0);
+    std::vector<double> sc(n_new, 0.0);
+    CUDA_TRY(cudaMemcpyAsync(inf.data(), h->dInfo, nl * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaMemcpyAsync(pk.data(), dPick, n_new * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaMemcpyAsync(sc.data(), dScore, n_new * 8, cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    // append_row_kernel records a failed pivot of step k as Nk + 1 = N + k + 1; later steps did nothing.  The first
+    // failing step (the smallest k over the outputs) and the points appended up to and including it:
+    int fail = n_new, bad = -1;
+    for (int a = 0; a < nl; ++a)
+        if (inf[a] && inf[a] - N - 1 < fail) { fail = inf[a] - N - 1; bad = a; }
+    const int added = (bad >= 0) ? fail + 1 : n_new;
+    for (int k = 0; k < added; ++k) {
+        picked[k] = pk[k];
+        if (score) score[k] = sc[k];
+    }
+    *n_added = added;
+    h->N = N + added;
+    if (bad >= 0) {
+        factor_stale(h);                 // row N + added - 1 of that output is unusable: the caller must refactorise
+        set_error(h, "gpmpc_append_greedy: output %d lost positive definiteness at pick %d (refactorise, jitter applies there)",
+                  h->a0 + bad, added - 1);
+        return GPMPC_ERR_NOTPD;
+    }
+    factor_caches_stale(h);
+    rc = launch_alpha(h, 0, nl);
+    if (rc) return rc;
+    std::vector<double> res(2 * nl);
+    CUDA_TRY(cudaMemcpyAsync(res.data(), h->dRes, 2 * nl * 8, cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    for (int a = 0; a < nl; ++a) { h->logdet[a] = res[2 * a]; h->yalpha[a] = res[2 * a + 1]; }
     return GPMPC_OK;
 }
 

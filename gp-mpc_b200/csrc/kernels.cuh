@@ -1388,15 +1388,18 @@ __global__ void sym_from_lower_kernel(const double* __restrict__ Kl, double* __r
 //   l = L^-1 k(X, x_new);  lambda = sqrt(k(x_new,x_new) + sn2 - l^T l)
 //   L    <- [[L, 0], [l^T, lambda]]          L^-1 <- [[L^-1, 0], [-(l^T L^-1)/lambda, 1/lambda]]
 // lvec = L^-1 k, rvec = (L^-1)^T lvec are produced by the trmv kernels; this kernel writes
-// row N of both factors (the identity tail row it replaces).  One CTA per output.
+// row N of both factors (the identity tail row it replaces).  One CTA per output.  stop (may be null): a greedy
+// selection step after a failed pivot, nothing is written.
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 append_row_kernel(double* __restrict__ L, double* __restrict__ Li, int ld, long long sL,
                   const double* __restrict__ lvec, const double* __restrict__ rvec, long long sv,
-                  const double* __restrict__ hyp, int hyp_ld, int Nx, int N, int* __restrict__ info)
+                  const double* __restrict__ hyp, int hyp_ld, int Nx, int N, int* __restrict__ info,
+                  const int* __restrict__ stop)
 {
     __shared__ double red[8];
     __shared__ double lam_s;
+    if (stop && *stop) return;
     const int a = blockIdx.x, tid = threadIdx.x;
     const double* lv = lvec + (long long)a * sv;
     const double* rv = rvec + (long long)a * sv;
@@ -1419,6 +1422,147 @@ append_row_kernel(double* __restrict__ L, double* __restrict__ Li, int ld, long 
     double* Lir = Li + (long long)a * sL + (long long)N * ld;
     for (int j = tid; j < N; j += 256) { Lr[j] = lv[j]; Lir[j] = -rv[j] * il; }
     if (tid == 0) { Lr[N] = lam; Lir[N] = il; }
+}
+
+// ---------------------------------------------------------------------------------------
+// Greedy max-variance selection from a pool of n candidates (gpmpc_append_greedy).  V[a][c][0..Npad) = L_a^-1 k_a(X, c)
+// (row stride ldv, output stride sV), var[a][c] = sf2_a - |V[a][c]|^2 (noise free, q3).  Step k (Nk = N + k points):
+//   pick c* -> gather l_a = V[a][c*] -> trmv_lower_T + append_row (row Nk of L, L^-1) -> downdate the active candidates:
+//   w = (k_a(x*, c) - l_a . v_ac) / L_a[Nk][Nk],  v_ac[Nk] = w,  var[a][c] -= w^2
+// Every dot product runs in a fixed order (two calls give the same bits).  Once a pivot failed (info != 0 on any
+// output) the kernels of the later steps return at once: nothing is written past the failing row.
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ bool greedy_failed(const int* __restrict__ info, int nloc)
+{
+    for (int a = 0; a < nloc; ++a)
+        if (info[a]) return true;
+    return false;
+}
+
+// sum of a row of n doubles times another, lane-strided with four accumulators (fixed order); every lane gets it
+__device__ __forceinline__ double warp_dot(const double* __restrict__ x, const double* __restrict__ y, int n)
+{
+    const int lane = threadIdx.x & 31;
+    double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+    int i = lane;
+    for (; i + 96 < n; i += 128) {
+        s0 = fma(x[i], y[i], s0);
+        s1 = fma(x[i + 32], y[i + 32], s1);
+        s2 = fma(x[i + 64], y[i + 64], s2);
+        s3 = fma(x[i + 96], y[i + 96], s3);
+    }
+    for (; i < n; i += 32) s0 = fma(x[i], y[i], s0);
+    return warp_sum((s0 + s1) + (s2 + s3));
+}
+
+// var[a][c] = sf2_a - |V[a][c][0..N)|^2; one warp per (candidate, output), grid (ceil(n/8), nloc)
+__global__ void __launch_bounds__(256)
+greedy_var_kernel(const double* __restrict__ V, int ldv, long long sV, int N, int n,
+                  const double* __restrict__ hyp, int hyp_ld, int Nx, double* __restrict__ var)
+{
+    const int c = blockIdx.x * 8 + (threadIdx.x >> 5), a = blockIdx.y;
+    if (c >= n) return;
+    const double* v = V + (long long)a * sV + (long long)c * ldv;
+    const double s = warp_dot(v, v, N);
+    if ((threadIdx.x & 31) == 0) {
+        const double sf = hyp[(long long)a * hyp_ld + Nx];
+        var[(long long)a * n + c] = sf * sf - s;
+    }
+}
+
+// true if (s1, i1) beats (s2, i2): larger score, ties to the lower index; index n is "none"
+__device__ __forceinline__ bool greedy_better(double s1, int i1, double s2, int i2, int n)
+{
+    return i1 != n && (i2 == n || s1 > s2 || (s1 == s2 && i1 < i2));
+}
+
+// One CTA: score[c] = sum_a var[a][c] (outputs in order) over the active candidates, argmax with ties to the lowest
+// index.  Records c* and its score, deactivates it, writes x* into column Nk of X^T and y* into row Nk of Y.  After a
+// failed pivot it only raises `stop` for the rest of the step.
+__global__ void __launch_bounds__(1024)
+greedy_pick_kernel(const double* __restrict__ var, int n, int nloc, int* __restrict__ active,
+                   const double* __restrict__ Xc, const double* __restrict__ Yc, int Nx,
+                   double* __restrict__ XT, double* __restrict__ Y, int ld, int Nk,
+                   const int* __restrict__ info, int* __restrict__ stop,
+                   int* __restrict__ picked, double* __restrict__ score, int k)
+{
+    __shared__ double bs[32];
+    __shared__ int bi[32];
+    const int tid = threadIdx.x, lane = tid & 31, wp = tid >> 5;
+    if (greedy_failed(info, nloc)) {
+        if (tid == 0) *stop = 1;
+        return;
+    }
+    double best = 0.0;
+    int bidx = n;
+    for (int c = tid; c < n; c += 1024) {        // ascending c: the first of equal scores stays
+        if (!active[c]) continue;
+        double s = 0.0;
+        for (int a = 0; a < nloc; ++a) s += var[(long long)a * n + c];
+        if (bidx == n || s > best) { best = s; bidx = c; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const double s2 = __shfl_xor_sync(0xffffffffu, best, o);
+        const int i2 = __shfl_xor_sync(0xffffffffu, bidx, o);
+        if (greedy_better(s2, i2, best, bidx, n)) { best = s2; bidx = i2; }
+    }
+    if (lane == 0) { bs[wp] = best; bi[wp] = bidx; }
+    __syncthreads();
+    if (wp == 0) {
+        best = bs[lane]; bidx = bi[lane];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const double s2 = __shfl_xor_sync(0xffffffffu, best, o);
+            const int i2 = __shfl_xor_sync(0xffffffffu, bidx, o);
+            if (greedy_better(s2, i2, best, bidx, n)) { best = s2; bidx = i2; }
+        }
+        if (bidx < n) {                           // always: the host asks for at most n picks
+            if (lane == 0) { picked[k] = bidx; score[k] = best; active[bidx] = 0; }
+            if (lane < Nx) XT[(long long)lane * ld + Nk] = Xc[(long long)bidx * Nx + lane];
+            for (int a = lane; a < nloc; a += 32) Y[(long long)a * ld + Nk] = Yc[(long long)bidx * nloc + a];
+        }
+    }
+}
+
+// l_a[i] = V[a][c*][i] for i < Nk, 0 up to ld (as gpmpc_append leaves its l); grid (ceil(ld/256), nloc)
+__global__ void __launch_bounds__(256)
+greedy_gather_kernel(const double* __restrict__ V, int ldv, long long sV, const int* __restrict__ picked, int k, int Nk,
+                     double* __restrict__ l, long long sl, int ld, const int* __restrict__ stop)
+{
+    if (*stop) return;
+    const int a = blockIdx.y, i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= ld) return;
+    l[(long long)a * sl + i] = (i < Nk) ? V[(long long)a * sV + (long long)picked[k] * ldv + i] : 0.0;
+}
+
+// w = (k_a(x*, c) - l_a . v_ac) / lambda_a for every active candidate c, one warp per (candidate, output),
+// grid (ceil(n/8), nloc); lambda_a = L_a[Nk][Nk] as append_row_kernel wrote it
+__global__ void __launch_bounds__(256)
+greedy_downdate_kernel(double* __restrict__ V, int ldv, long long sV, double* __restrict__ var, int n,
+                       const int* __restrict__ active, const double* __restrict__ l, long long sl,
+                       const double* __restrict__ L, int ld, long long sL, const double* __restrict__ Xc, int Nx,
+                       const double* __restrict__ hyp, int hyp_ld, const int* __restrict__ picked, int k, int Nk,
+                       const int* __restrict__ info, int nloc)
+{
+    const int lane = threadIdx.x & 31, c = blockIdx.x * 8 + (threadIdx.x >> 5), a = blockIdx.y;
+    if (c >= n || !active[c] || greedy_failed(info, nloc)) return;
+    const double* hp = hyp + (long long)a * hyp_ld;
+    double* v = V + (long long)a * sV + (long long)c * ldv;
+    const double s = warp_dot(l + (long long)a * sl, v, Nk);
+    const int cs = picked[k];
+    double q = 0.0;
+    if (lane < Nx) {                              // Nx <= 32
+        const double df = (Xc[(long long)cs * Nx + lane] - Xc[(long long)c * Nx + lane]) / hp[lane];
+        q = df * df;
+    }
+    q = warp_sum(q);
+    if (lane == 0) {
+        const double sf = hp[Nx];
+        const double w = (sf * sf * exp(-0.5 * q) - s) / L[(long long)a * sL + (long long)Nk * ld + Nk];
+        v[Nk] = w;
+        var[(long long)a * n + c] -= w * w;
+    }
 }
 
 // ---------------------------------------------------------------------------------------

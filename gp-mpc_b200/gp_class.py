@@ -136,7 +136,8 @@ class GP:
         self.__hyper_noise_variance = self.__hyper[:, Nx + 1] ** 2
         self.__hyper_mean = self.__hyper[:, (Nx + 1):]
 
-    def __build_engine(self):
+    def __build_engine(self, capacity=None):
+        """capacity: training points to reserve room for (append_greedy); passed to the factory only when given."""
         if self.__engine is not None:
             self.__engine.close()
         c = self.__comm
@@ -145,7 +146,8 @@ class GP:
             b, n = output_block(self.__Ny, c.rank, c.world)
         else:
             b, n = 0, self.__Ny
-        self.__engine = self.__engine_factory(self.__N, self.__Nx, self.__Ny, b, n, self.__device)
+        kw = {} if capacity is None else dict(capacity=int(capacity))
+        self.__engine = self.__engine_factory(self.__N, self.__Nx, self.__Ny, b, n, self.__device, **kw)
         self.__engine.set_data(self.__X, self.__Y)
         if c.world > 1 and self.__mode == 'outputs':
             uid = self.__engine_factory.comm_unique_id() if c.rank == 0 else None
@@ -733,8 +735,90 @@ class GP:
     def update_data(self, X_new, Y_new, N_new=None):
         """reference gp_class.py:384-471 is self-declared broken ("NOT working as intended",
         :397; SURVEY q14).  Not replicated."""
-        raise NotImplementedError('GP.update_data is broken in the reference (gp_class.py:397); '
-                                  'use update_data_all / replace_data_all')
+        raise NotImplementedError('GP.update_data is broken in the reference (gp_class.py:397); use append_greedy '
+                                  '(max-variance selection), update_data_all or replace_data_all')
+
+    def append_greedy(self, X_new, Y_new, N_new=None, device_select=True):
+        """ Grow the model by the N_new points of the pool (X_new, Y_new) with the highest combined posterior variance
+        (sum over outputs, noise free), chosen one at a time after the previous choice has been absorbed: what the
+        reference's ``update_data`` (gp_class.py:384-471) set out to do, with its argmin / sqrt(k - |l|) fixed (SURVEY
+        q14).  Hyper-parameters are kept.  Returns the picked row indices into X_new, in selection order (ties go to
+        the lowest index).
+
+        device_select: the whole selection runs in one device call (gpmpc_append_greedy) when this rank's engine owns
+        every output; the engine is rebuilt once with enough reserved capacity first if needed.  Otherwise (outputs
+        sharded over ranks, or False) each step predicts the pool's variances and appends the best point with
+        ``append_data``; every rank makes the same choice. """
+        X_new = np.array(X_new, dtype=np.float64).reshape(-1, self.__Nx)
+        Y_new = np.array(Y_new, dtype=np.float64).reshape(-1, self.__Ny)
+        n = X_new.shape[0]
+        if Y_new.shape[0] != n:
+            raise ValueError('X_new and Y_new must have the same number of rows')
+        N_new = n if N_new is None else int(N_new)
+        if not 0 <= N_new <= n:
+            raise ValueError('N_new must be in [0, %d], got %d' % (n, N_new))
+        if N_new == 0:
+            return np.zeros(0, dtype=np.int64)
+        Xs, Ys = X_new, Y_new
+        if self.__normalize:                         # gp_class.py:406-408
+            Ys = self.standardize(Y_new, self.__meanY, self.__stdY)
+            Xs = self.standardize(X_new, self.__meanZ, self.__stdZ)
+        eng = self.__engine
+        on_device = (device_select and hasattr(eng, 'append_greedy') and not self.__sharded_outputs()
+                     and eng.out_count == self.__Ny)
+        picked = self.__greedy_device(Xs, Ys, N_new) if on_device else self.__greedy_host(X_new, Y_new, Xs, N_new)
+        self.__invK = None
+        return np.asarray(picked, dtype=np.int64)
+
+    def __greedy_device(self, Xs, Ys, N_new):
+        Yr = Ys
+        if self.__has_prior_mean():                  # the engine factorises on y - m(x), as __factorize does
+            Yr = Ys - np.column_stack([mean_function(self.__hyper[a], Xs, self.__mean_func) for a in range(self.__Ny)])
+        remaining = np.arange(Xs.shape[0])
+        picked = []
+        while len(picked) < N_new:
+            need = N_new - len(picked)
+            if self.__engine.capacity - self.__engine.N < need:
+                self.__build_engine(capacity=self.__N + need)
+                self.__factorize()
+            idx, _, ok = self.__engine.append_greedy(Xs[remaining], Yr[remaining], need)
+            if self.__comm.world > 1:
+                # replicated engines ('points' mode): the kept picks and the refit decision are collective, so a rank
+                # that alone lost positive definiteness cannot leave the others in __factorize's barrier
+                res = self.__comm.allgather_object((idx.tolist(), bool(ok)))
+                k = min(len(r[0]) for r in res)
+                if any(r[0][:k] != res[0][0][:k] for r in res):
+                    raise RuntimeError('append_greedy: ranks selected different points')
+                if not all(r[1] and len(r[0]) == k for r in res):
+                    idx, ok = idx[:k], False          # every rank keeps the common picks and refits on them
+            sel = remaining[idx]
+            self.__X = np.vstack([self.__X, Xs[sel]])
+            self.__Y = np.vstack([self.__Y, Ys[sel]])
+            self.__N = self.__X.shape[0]
+            picked.extend(sel.tolist())
+            remaining = np.delete(remaining, idx)
+            if not ok:
+                # positive definiteness lost at the last pick (it is in X): refactorise, the jitter policy applies there
+                need = N_new - len(picked)
+                self.__build_engine(capacity=self.__N + need if need else None)
+                self.__factorize()
+        return picked
+
+    def __greedy_host(self, X_new, Y_new, Xs, N_new):
+        remaining = np.arange(Xs.shape[0])
+        picked = []
+        for _ in range(N_new):
+            # gathered over ranks: every rank holds every output's variance and makes the same choice
+            var = self.__predict_std(Xs[remaining], None, 'ME', want_cov=False, want_jac=False)[1]
+            score = var[:, 0].copy()
+            for a in range(1, self.__Ny):            # outputs in order, as the device pick sums them
+                score += var[:, a]
+            j = int(np.argmax(score))                # first maximum: ties to the lowest index
+            c = int(remaining[j])
+            self.append_data(X_new[c:c + 1], Y_new[c:c + 1])      # its refit decision is collective
+            picked.append(c)
+            remaining = np.delete(remaining, j)
+        return picked
 
     def standardize(self, Y, mean, std):
         return (Y - mean) / std                      # gp_class.py:629-630

@@ -71,6 +71,11 @@ int gpmpc_version(void);
  * independent per-output GPs, optimize.py:433 / gp_functions.py:128).  device = CUDA
  * ordinal.  Replaces the array allocations of train_gp_numpy, optimize.py:424-427. */
 int gpmpc_create(int N, int Nx, int Ny, int out_begin, int out_count, int device, gpmpc_handle_t* out);
+/* gpmpc_create with room reserved for appends: the padded size is ceil(max(N, N_cap)/128)*128 instead of
+ * ceil(N/128)*128, so gpmpc_append and gpmpc_append_greedy can grow the model up to it without a refit.  The padded
+ * tail is an identity block of K; every entry point gives the results of an unreserved handle.  N_cap <= N is
+ * gpmpc_create. */
+int gpmpc_create_reserve(int N, int N_cap, int Nx, int Ny, int out_begin, int out_count, int device, gpmpc_handle_t* out);
 int gpmpc_destroy(gpmpc_handle_t h);
 const char* gpmpc_last_error(gpmpc_handle_t h);   /* h may be NULL: last create error */
 
@@ -118,10 +123,24 @@ int gpmpc_predict(gpmpc_handle_t h, int method, int H, const double* Z, const do
 
 /* Append ONE training point (x_new:(Nx,), y_new:(Ny,) host, GP input space) to a factorised
  * model in O(N^2): new rows of L and L^-1, alpha refreshed.  Capacity is the padded size
- * ceil(N/128)*128 (GPMPC_ERR_STATE beyond it: refit on a new handle).  GPMPC_ERR_NOTPD if the
- * Schur complement is not positive: refactorise (the jitter policy applies there).  The correct
- * counterpart of the reference's broken GP.update_data (gp_class.py:384-471). */
+ * ceil(N/128)*128, or the one reserved by gpmpc_create_reserve (GPMPC_ERR_STATE beyond it: refit on
+ * a new handle).  GPMPC_ERR_NOTPD if the Schur complement is not positive: refactorise (the jitter
+ * policy applies there).  Appends every point given, in order; gpmpc_append_greedy chooses. */
 int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double* y_new);
+
+/* Greedy selection from a pool: n_new times, append the pool point with the largest sum over outputs of the
+ * posterior variance sf2_a - |L_a^-1 k_a(X, c)|^2 (noise-free, q3), ties to the lowest index.  Each choice is made
+ * after the previous point has been absorbed by the rank-1 update of gpmpc_append.  This is what GP.update_data
+ * (gp_class.py:384-471) set out to do, with SURVEY q14 fixed (it takes argmin and sqrt(k - |l|)).
+ *   Xc (n, Nx), Yc (n, Ny) host, GP input / output space (Yc = the residual y - m(x) under a prior mean)
+ *   picked (n_new) pool indices in selection order; score (n_new) or NULL: combined variance at pick time
+ *   n_added: points appended (== n_new on success)
+ * Hyper-parameters kept; alpha and logdet refreshed once at the end.  Handle must own all outputs on one rank
+ * (GPMPC_ERR_STATE); N + n_new > capacity -> GPMPC_ERR_STATE before any work (model untouched); n >= 1 and
+ * 0 <= n_new <= n, non-null Xc, Yc, picked, n_added (GPMPC_ERR_ARG).  Pool memory: 8 Ny n Npad bytes on the device.
+ * GPMPC_ERR_NOTPD as gpmpc_append: *n_added includes the failing point, the handle needs gpmpc_factorize. */
+int gpmpc_append_greedy(gpmpc_handle_t h, int n, const double* Xc, const double* Yc, int n_new,
+                        int* picked, double* score, int* n_added);
 
 /* Full posterior covariance between H test points for every OWNED output:
  * out:(out_count,H,H) host, out[a] = sf2_a - V_a^T V_a with V_a = L_a \ k(X, Z)  (the scalar
