@@ -44,6 +44,7 @@ SYMBOLS = [
     ('gpmpc_get_size', C.c_int, [_H, _ip, _ip, _ip]),
     ('gpmpc_append', C.c_int, [_H, _dp, _dp]),
     ('gpmpc_append_greedy', C.c_int, [_H, C.c_int, _dp, _dp, C.c_int, _ip, _dp, _ip]),
+    ('gpmpc_remove', C.c_int, [_H, C.c_int, _ip]),
     ('gpmpc_posterior_cov', C.c_int, [_H, C.c_int, _dp, _dp]),
     ('gpmpc_rollout', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     ('gpmpc_rollout_batch', C.c_int, [_H, C.c_int, C.c_int, C.c_int] + [_dp] * 10),
@@ -365,6 +366,13 @@ class Engine:
         k = added.value
         self.N += k
         return picked[:k].astype(np.int64), score[:k].copy(), rc == OK
+
+    def remove(self, idx):
+        """gpmpc_remove: drop the training points idx (distinct indices into the current model, any order) by rank-1
+        updates of L and L^-1; raises GpmpcError on a bad index or an unfactorised model (which is then untouched)."""
+        idx = np.ascontiguousarray(np.asarray(idx, dtype=np.int64).reshape(-1), dtype=np.int32)
+        self._check(self.lib.gpmpc_remove(self.h, idx.size, idx.ctypes.data_as(_ip) if idx.size else None))
+        self.N -= idx.size
 
     def posterior_cov(self, Z):
         """(out_count, H, H): sf2 - V^T V per owned output (GP.covar)."""

@@ -99,6 +99,7 @@ struct gpmpc_handle_s {
     DevBuf<double> dCovV, dCovOut;    // GP.covar scratch pool; dCovV also holds the greedy selection's pool V
     DevBuf<double> dGrD;              // gpmpc_append_greedy: [var (nloc, n) | Xc (n, Nx) | Yc (n, Ny) | score (n_new)]
     DevBuf<int> dGrI;                 //                      [active (n) | picked (n_new) | stop]
+    DevBuf<double> dRm;               // gpmpc_remove: [p | d | g] (Npad each) per owned output
     // predict_grad: U = Linv^T per output (lazy), beta rows, partial sums, per-batch derivative slabs
     DevBuf<double> dUall, dBeta, dPDV, dPH, dGradOut; bool u_valid = false;
     // predict_hess: derivative rows d ks / dz and their L^-1 products (lazy), block partials, per-batch second-derivative slabs
@@ -2064,6 +2065,67 @@ extern "C" int gpmpc_append_greedy(gpmpc_handle_t h, int n, const double* Xc, co
                   h->a0 + bad, added - 1);
         return GPMPC_ERR_NOTPD;
     }
+    factor_caches_stale(h);
+    rc = launch_alpha(h, 0, nl);
+    if (rc) return rc;
+    std::vector<double> res(2 * nl);
+    CUDA_TRY(cudaMemcpyAsync(res.data(), h->dRes, 2 * nl * 8, cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    for (int a = 0; a < nl; ++a) { h->logdet[a] = res[2 * a]; h->yalpha[a] = res[2 * a + 1]; }
+    return GPMPC_OK;
+}
+
+// Removal of training points by rank-1 updates of the trailing blocks of L and L^-1 (kernels.cuh, remove_*), one point
+// at a time in descending index order.  Per point: p, d, g for every output, then per output the L rows into dU, the
+// L^-1 rows into dKinv (partials over row blocks in the W1 workspace), the copy back with the identity tail row; then
+// the point leaves X^T and Y.  alpha and logdet are refreshed once, at the end.
+extern "C" int gpmpc_remove(gpmpc_handle_t h, int n, const int* idx)
+{
+    if (!h) return GPMPC_ERR_ARG;
+    if (!h->factorized) { set_error(h, "gpmpc_remove: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
+    if (n < 0 || (n > 0 && !idx)) { set_error(h, "gpmpc_remove: need n >= 0 and idx non-null for n > 0 (n = %d)", n); return GPMPC_ERR_ARG; }
+    if (n == 0) return GPMPC_OK;
+    const int N = h->N, Nx = h->Nx, np = h->Npad, nl = h->nloc;
+    if (n >= N) { set_error(h, "gpmpc_remove: removing %d of %d points leaves none", n, N); return GPMPC_ERR_ARG; }
+    std::vector<int> order(idx, idx + n);
+    std::sort(order.begin(), order.end(), [](int u, int v) { return u > v; });
+    if (order[0] >= N || order[n - 1] < 0) { set_error(h, "gpmpc_remove: index out of range [0, %d)", N); return GPMPC_ERR_ARG; }
+    for (int k = 1; k < n; ++k)
+        if (order[k] == order[k - 1]) { set_error(h, "gpmpc_remove: index %d given twice", order[k]); return GPMPC_ERR_ARG; }
+    CUDA_TRY(cudaSetDevice(h->device));
+    int rc = ensure_nlml_scratch(h);           // dU / dKinv: the work slabs of the new rows
+    if (rc) return rc;
+    ENSURE(h->dRm, (long long)nl * 3 * np);
+    NvtxRange nvtx_r("gpmpc.remove");
+    const dim3 gcol((np + 255) / 256);
+    for (int k = 0; k < n; ++k) {
+        const int i = order[k], Nk = N - k, m = Nk - i - 1;     // m trailing points
+        if (m > 0) {
+            remove_coef_kernel<<<nl, 1024, 0, h->st>>>(h->dL, h->dLi, np, slab(h), i, m, h->dRm);
+            CUDA_TRY(cudaGetLastError());
+        }
+        for (int a = 0; a < nl; ++a) {
+            double* L = h->dL + (long long)a * slab(h);
+            double* Li = h->dLi + (long long)a * slab(h);
+            const double* coef = h->dRm + (long long)a * 3 * np;
+            if (m > 0) {
+                const int nb = (m + RM_RB - 1) / RM_RB;
+                remove_l_rows_kernel<<<m, 256, 0, h->st>>>(L, h->dU, np, coef, i, m);
+                CUDA_TRY(cudaGetLastError());
+                remove_li_part_kernel<<<dim3(gcol.x, nb), 256, 0, h->st>>>(Li, np, coef, i, m, h->dW1);
+                CUDA_TRY(cudaGetLastError());
+                remove_li_scan_kernel<<<gcol, 256, 0, h->st>>>(h->dW1, np, nb);
+                CUDA_TRY(cudaGetLastError());
+                remove_li_apply_kernel<<<dim3(gcol.x, nb), 256, 0, h->st>>>(Li, h->dKinv, np, coef, i, m, h->dW1);
+                CUDA_TRY(cudaGetLastError());
+            }
+            remove_commit_kernel<<<m + 1, 256, 0, h->st>>>(L, Li, h->dU, h->dKinv, np, i, Nk);
+            CUDA_TRY(cudaGetLastError());
+        }
+        remove_shift_kernel<<<Nx + nl, 256, 0, h->st>>>(h->dXT, Nx, h->dY, np, i, Nk);
+        CUDA_TRY(cudaGetLastError());
+    }
+    h->N = N - n;
     factor_caches_stale(h);
     rc = launch_alpha(h, 0, nl);
     if (rc) return rc;

@@ -1566,6 +1566,210 @@ greedy_downdate_kernel(double* __restrict__ V, int ldv, long long sV, double* __
 }
 
 // ---------------------------------------------------------------------------------------
+// Removal of training point i from an N-point factorisation (gpmpc_remove), O(N^2) per output.  With lambda = L[i][i],
+// n = N - i - 1 trailing points (r, s, j, k index them: old row / column i + 1 + r):
+//   p_r = -lambda Li[i+1+r][i] (= L33^-1 l32),  t_-1 = 1,  t_r = t_{r-1} + p_r^2,
+//   d_r = sqrt(t_r / t_{r-1}),  g_r = p_r / sqrt(t_r t_{r-1})
+// chol(I + p p^T) = diag(d) + strict_lower(p g^T), its inverse diag(1/d) - strict_lower(g p^T).  New rows i + r:
+//   L'[i+r][c]   = L[i+1+r][c] (c < i),   L'[i+r][i+j] = d_j L[i+1+r][i+1+j] + g_j sum_{j<k<=r} p_k L[i+1+r][i+1+k]
+//   R_r = Li[i+1+r][.] + p_r Li[i][.]  (its column i vanishes and is dropped),
+//   Li'[i+r][.]  = R_r / d_r - g_r sum_{s<r} p_s R_s
+// A rank-1 update of the trailing block (every t_r >= 1): it cannot lose positive definiteness.  The L rows are
+// suffix scans along each row, the L^-1 rows prefix scans down each column (row blocks of RM_RB: partials, their scan
+// over blocks, the apply pass).  Both write rows i .. N-2 into a work slab (a row moves up over the row another CTA
+// still reads), which remove_commit_kernel copies back.  Rows are written up to the end of their 128-wide diagonal
+// block, zeros right of the diagonal; the strictly-upper 128-tiles are never written.  Every sum runs in a fixed order.
+// ---------------------------------------------------------------------------------------
+#define RM_RB 64
+
+// Exclusive prefix sum of v over the CTA's threads in thread order, and the CTA total (*total), in a fixed order: warp
+// shuffles, then the warp totals scanned in warp order.  sh: 33 doubles of shared memory; every thread must call it.
+__device__ __forceinline__ double block_exclusive_scan(double v, double* sh, double* total)
+{
+    const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    double x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const double y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    double ex = __shfl_up_sync(0xffffffffu, x, 1);
+    if (lane == 0) ex = 0.0;
+    if (lane == 31) sh[wp] = x;
+    __syncthreads();
+    if (wp == 0) {
+        double w = lane < nw ? sh[lane] : 0.0;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const double y = __shfl_up_sync(0xffffffffu, w, o);
+            if (lane >= o) w += y;
+        }
+        double wex = __shfl_up_sync(0xffffffffu, w, 1);
+        if (lane == 0) wex = 0.0;
+        __syncwarp();
+        sh[lane] = wex;
+        if (lane == 31) sh[32] = w;
+    }
+    __syncthreads();
+    const double r = ex + sh[wp];
+    *total = sh[32];
+    __syncthreads();                              // sh is free for the next call
+    return r;
+}
+
+// p, d, g of the removal of point i for every output (one CTA each): coef[a] = [p (ld) | d (ld) | g (ld)]
+__global__ void __launch_bounds__(1024)
+remove_coef_kernel(const double* __restrict__ L, const double* __restrict__ Li, int ld, long long sL, int i, int n,
+                   double* __restrict__ coef)
+{
+    __shared__ double sh[33];
+    const double* Lib = Li + (long long)blockIdx.x * sL;
+    double* p = coef + (long long)blockIdx.x * 3 * ld;
+    double* d = p + ld;
+    double* g = d + ld;
+    const double lam = L[(long long)blockIdx.x * sL + (long long)i * ld + i];
+    const int C = (n + 1023) / 1024, r0 = threadIdx.x * C, r1 = min(n, r0 + C);   // contiguous chunk per thread
+    double s = 0.0;
+    for (int r = r0; r < r1; ++r) {
+        const double pr = -lam * Lib[(long long)(i + 1 + r) * ld + i];
+        p[r] = pr;
+        s = fma(pr, pr, s);
+    }
+    double tot;
+    double tp = 1.0 + block_exclusive_scan(s, sh, &tot);
+    for (int r = r0; r < r1; ++r) {
+        const double pr = p[r], t = fma(pr, pr, tp);
+        d[r] = sqrt(t / tp);
+        g[r] = pr / sqrt(t * tp);
+        tp = t;
+    }
+}
+
+// New rows i .. i+n-1 of L into W (one CTA per row, the longest first): the moved columns < i, the suffix scan of
+// p_k L[i+1+r][i+1+k] from the diagonal leftwards in 256-element segments, zeros up to the diagonal block's end
+__global__ void __launch_bounds__(256)
+remove_l_rows_kernel(const double* __restrict__ L, double* __restrict__ W, int ld, const double* __restrict__ coef,
+                     int i, int n)
+{
+    __shared__ double sh[33];
+    const int tid = threadIdx.x, r = n - 1 - blockIdx.x, R = i + r;
+    const double* src = L + (long long)(R + 1) * ld;
+    double* dst = W + (long long)R * ld;
+    const double* p = coef;
+    const double* d = coef + ld;
+    const double* g = coef + 2 * ld;
+    for (int c = tid; c < i; c += 256) dst[c] = src[c];
+    const int be = (R / 128 + 1) * 128;
+    for (int c = R + 1 + tid; c < be; c += 256) dst[c] = 0.0;
+    double carry = 0.0;                            // sum of p_k a_k over the segments already done (larger k)
+    for (int hi = r + 1; hi > 0; hi -= 256) {
+        const int j = hi - 1 - tid;               // thread order = descending j: a prefix over threads is a suffix in j
+        const double a = j >= 0 ? src[i + 1 + j] : 0.0;
+        const double pa = j >= 0 ? p[j] * a : 0.0;
+        double tot;
+        const double s = block_exclusive_scan(pa, sh, &tot);
+        if (j >= 0) dst[i + j] = fma(g[j], carry + s, d[j] * a);
+        carry += tot;
+    }
+}
+
+// Q[b][c] = sum_{r in row block b} p_r R_r[c'] for new column c (old column c' = c + (c >= i)); grid (ceil(ld/256), nb)
+__global__ void __launch_bounds__(256)
+remove_li_part_kernel(const double* __restrict__ Li, int ld, const double* __restrict__ coef, int i, int n,
+                      double* __restrict__ Q)
+{
+    const int c = blockIdx.x * 256 + threadIdx.x, b = blockIdx.y;
+    const int r0 = b * RM_RB, r1 = min(n, r0 + RM_RB);
+    if (c >= ld) return;
+    const double* p = coef;
+    const int oc = c + (c >= i);
+    const double li = c < i ? Li[(long long)i * ld + c] : 0.0;
+    double q = 0.0;
+    for (int r = max(r0, c - i); r < r1; ++r) {  // new row i + r holds column c from r >= c - i on
+        const double x = fma(p[r], li, Li[(long long)(i + 1 + r) * ld + oc]);
+        q = fma(p[r], x, q);
+    }
+    Q[(long long)b * ld + c] = q;
+}
+
+// exclusive scan of Q over the nb row blocks, per column (in place)
+__global__ void __launch_bounds__(256)
+remove_li_scan_kernel(double* __restrict__ Q, int ld, int nb)
+{
+    const int c = blockIdx.x * 256 + threadIdx.x;
+    if (c >= ld) return;
+    double e = 0.0;
+    for (int b = 0; b < nb; ++b) {
+        const double q = Q[(long long)b * ld + c];
+        Q[(long long)b * ld + c] = e;
+        e += q;
+    }
+}
+
+// New rows i + r of L^-1 into W for the rows of block b, from the scanned partials Q; grid as remove_li_part_kernel
+__global__ void __launch_bounds__(256)
+remove_li_apply_kernel(const double* __restrict__ Li, double* __restrict__ W, int ld, const double* __restrict__ coef,
+                       int i, int n, const double* __restrict__ Q)
+{
+    const int c = blockIdx.x * 256 + threadIdx.x, b = blockIdx.y;
+    const int r0 = b * RM_RB, r1 = min(n, r0 + RM_RB);
+    if (c >= ld || c >= ((i + r1 - 1) / 128 + 1) * 128) return;   // right of the last row's diagonal block
+    const double* p = coef;
+    const double* d = coef + ld;
+    const double* g = coef + 2 * ld;
+    const int oc = c + (c >= i);
+    const double li = c < i ? Li[(long long)i * ld + c] : 0.0;
+    double P = Q[(long long)b * ld + c];
+    for (int r = r0; r < r1; ++r) {
+        const int R = i + r;
+        if (c >= (R / 128 + 1) * 128) continue;
+        double o = 0.0;
+        if (c <= R) {
+            const double x = fma(p[r], li, Li[(long long)(i + 1 + r) * ld + oc]);
+            o = fma(-g[r], P, x / d[r]);
+            P = fma(p[r], x, P);
+        }
+        W[(long long)R * ld + c] = o;
+    }
+}
+
+// Rows i .. N-2 of L and L^-1 from the work slabs (columns up to the diagonal block's end), row N-1 the identity tail
+// row; one CTA per row
+__global__ void __launch_bounds__(256)
+remove_commit_kernel(double* __restrict__ L, double* __restrict__ Li, const double* __restrict__ WL,
+                     const double* __restrict__ WLi, int ld, int i, int N)
+{
+    const int R = i + blockIdx.x, be2 = (R / 128 + 1) * 64;
+    double2* l = reinterpret_cast<double2*>(L + (long long)R * ld);
+    double2* li = reinterpret_cast<double2*>(Li + (long long)R * ld);
+    if (R == N - 1) {
+        for (int c = threadIdx.x; c < be2; c += 256) {
+            const double2 v = make_double2(2 * c == R ? 1.0 : 0.0, 2 * c + 1 == R ? 1.0 : 0.0);
+            l[c] = v; li[c] = v;
+        }
+        return;
+    }
+    const double2* wl = reinterpret_cast<const double2*>(WL + (long long)R * ld);
+    const double2* wli = reinterpret_cast<const double2*>(WLi + (long long)R * ld);
+    for (int c = threadIdx.x; c < be2; c += 256) { l[c] = wl[c]; li[c] = wli[c]; }
+}
+
+// Entry i leaves each of the `rows` rows of stride ld (X^T, then Y): later entries move down one, entry N-1 becomes 0.
+// One CTA per row; each segment is read before any of it is written, so the in-place move is race-free.
+__global__ void __launch_bounds__(256)
+remove_shift_kernel(double* __restrict__ XT, int nx, double* __restrict__ Y, int ld, int i, int N)
+{
+    double* x = blockIdx.x < nx ? XT + (long long)blockIdx.x * ld : Y + (long long)(blockIdx.x - nx) * ld;
+    for (int c0 = i; c0 < N - 1; c0 += 256) {
+        const int c = c0 + threadIdx.x;
+        const double v = c < N - 1 ? x[c + 1] : 0.0;
+        __syncthreads();
+        if (c < N - 1) x[c] = v;
+    }
+    if (threadIdx.x == 0) x[N - 1] = 0.0;
+}
+
+// ---------------------------------------------------------------------------------------
 // First derivatives of the prediction w.r.t. the test input z (SURVEY 8f row 1: what CasADi's
 // AD produces for the MPC's NLP from the symbolic build_gp / build_TA_cov graphs,
 // gp_functions.py:111-173; mpc_class.py:390-412 differentiates them inside nlpsol):

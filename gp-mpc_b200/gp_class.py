@@ -686,18 +686,52 @@ class GP:
         self.__factorize()
         self.set_method(self.__gp_method)
 
-    def append_data(self, X_new, Y_new):
+    def remove_data(self, indices):
+        """ Drop the training points ``indices`` (distinct row indices into the current training set, any order) with
+        the O(N^2) rank-1 update of L, L^-1 and alpha: no refit, hyper-parameters kept, the freed rows are append
+        capacity again.  Raises ValueError on a bad index (non-integer, repeated, out of range, or no point left)
+        before the model is touched.  In 'outputs' mode every rank passes the same indices. """
+        idx = np.asarray(indices).reshape(-1)
+        if idx.size and not np.issubdtype(idx.dtype, np.integer):
+            raise ValueError('indices must be integers, got dtype %s' % idx.dtype)
+        idx = idx.astype(np.int64)
+        if np.unique(idx).size != idx.size:
+            raise ValueError('indices must be unique')
+        if idx.size and (idx.min() < 0 or idx.max() >= self.__N):
+            raise ValueError('indices must be in [0, %d)' % self.__N)
+        if idx.size >= self.__N:
+            raise ValueError('removing %d of %d points leaves none' % (idx.size, self.__N))
+        if idx.size == 0:
+            return
+        self.__engine.remove(idx)
+        self.__X = np.delete(self.__X, idx, axis=0)
+        self.__Y = np.delete(self.__Y, idx, axis=0)
+        self.__N = self.__X.shape[0]
+        self.__invK = None
+
+    def append_data(self, X_new, Y_new, max_points=None):
         """ Add observations one at a time with the O(N^2) rank-1 update of L, L^-1 and alpha
         (what the reference's ``update_data``, gp_class.py:384-471, set out to do); hyper-
         parameters are kept.  Falls back to a full refactorisation (``update_data_all``) when the
-        padded capacity is exhausted or an update loses positive definiteness. """
+        padded capacity is exhausted or an update loses positive definiteness.
+
+        max_points: a sliding window.  Before each point the oldest points (row 0, 1, ...) are removed with
+        ``remove_data`` so that at most max_points remain after the append: N stays constant once the window is
+        full, so a model at its full padded size keeps updating without a refit.  The refit fallback also keeps only
+        the newest max_points points.  None (default): the model only grows. """
         X_new = np.array(X_new, dtype=np.float64).reshape(-1, self.__Nx)
         Y_new = np.array(Y_new, dtype=np.float64).reshape(-1, self.__Ny)
+        if max_points is not None:
+            max_points = int(max_points)
+            if max_points < 2:                       # one old point at least stays beside each new one
+                raise ValueError('max_points must be >= 2, got %d' % max_points)
         Xs, Ys = X_new, Y_new
         if self.__normalize:
             Ys = self.standardize(Y_new, self.__meanY, self.__stdY)
             Xs = self.standardize(X_new, self.__meanZ, self.__stdZ)
         for k in range(Xs.shape[0]):
+            if max_points is not None and self.__N + 1 > max_points:
+                self.remove_data(np.arange(self.__N + 1 - max_points))
             ok = self.__engine.append(Xs[k], Ys[k])
             if self.__comm.world > 1:
                 # the fallback below runs collectives (engine rebuild): the decision must be collective
@@ -706,6 +740,8 @@ class GP:
             if not ok:
                 self.__X = np.vstack([self.__X, Xs[k:]])
                 self.__Y = np.vstack([self.__Y, Ys[k:]])
+                if max_points is not None:           # the window: the newest max_points
+                    self.__X, self.__Y = self.__X[-max_points:], self.__Y[-max_points:]
                 self.__N = self.__X.shape[0]
                 self.__build_engine()
                 self.__factorize()

@@ -142,6 +142,19 @@ int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double* y_new);
 int gpmpc_append_greedy(gpmpc_handle_t h, int n, const double* Xc, const double* Yc, int n_new,
                         int* picked, double* score, int* n_added);
 
+/* Remove the n distinct training points idx (indices into the model before the call, any order) from a factorised
+ * model in O(N^2) per point: rank-1 updates of the trailing blocks of L and L^-1 (never a refit, and they cannot lose
+ * positive definiteness), rows and columns past each point moved up, the freed row the identity tail again (the
+ * capacity is unchanged, so a later gpmpc_append reuses it).  Points go in descending index order; the point leaves
+ * X and every owned output's y.  Hyper-parameters kept; alpha and logdet refreshed once at the end.  Any handle,
+ * sharded or not: it updates the outputs it owns.  With gpmpc_append this keeps a sliding window of the newest
+ * measurements at a constant N, where the reference refits (replace_data_all, gp_class.py:553-626) or appends with
+ * its broken update_data (gp_class.py:384-471).
+ *   n = 0: no-op.  GPMPC_ERR_STATE: not factorised.  GPMPC_ERR_ARG: n < 0, idx NULL with n > 0, an index outside
+ *   [0, N), a duplicate, or n >= N (one point must remain).  Every check runs before any work: an error leaves the
+ *   model bit-identical.  Scratch: the two Npad^2 slabs of gpmpc_nlml's gradient (allocated once, if not yet). */
+int gpmpc_remove(gpmpc_handle_t h, int n, const int* idx);
+
 /* Full posterior covariance between H test points for every OWNED output:
  * out:(out_count,H,H) host, out[a] = sf2_a - V_a^T V_a with V_a = L_a \ k(X, Z)  (the scalar
  * kss = sf2 is broadcast over the whole matrix exactly as the reference does).  Replaces
