@@ -48,6 +48,7 @@ SYMBOLS = [
     ('gpmpc_posterior_cov', C.c_int, [_H, C.c_int, _dp, _dp]),
     ('gpmpc_rollout', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     ('gpmpc_rollout_batch', C.c_int, [_H, C.c_int, C.c_int, C.c_int] + [_dp] * 10),
+    ('gpmpc_rollout_sample', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 10 + [_ip]),
     ('gpmpc_predict_device', C.c_int, [_H, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     ('gpmpc_get', C.c_int, [_H, C.c_int, C.c_int, _dp]),
@@ -291,6 +292,33 @@ class Engine:
         self._check(self.lib.gpmpc_rollout_batch(self.h, int(method), B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale),
                                                  _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means), _ptr(var), _ptr(cov)))
         return means, var, cov
+
+    def rollout_sample(self, z0, U, eps, xi=None, scale=None, K=None, x_ref=None, uscale=None):
+        """gpmpc_rollout_sample: B trajectories of Nt steps, each one consistent draw of the GP posterior along the inputs
+        it visits.  z0:(B,Nx) (drawn first inputs, GP input units), U:(B,Nt,Nu) (with K only its shape is used),
+        eps:(B,Nt,Ny) standard normals of the draws, xi:(B,Nt,Ny)|None process-noise normals, scale / K / x_ref / uscale
+        as rollout_batch -> samples (B,Nt,Ny) GP output units, z_out (B,Nt,Nx) inputs used, kept (B,Nt,Ny) int32 (1 where
+        the point entered the conditioning set)."""
+        Nu = self.Nx - self.Ny
+        z0 = _f64(z0).reshape(-1, self.Nx)
+        B = z0.shape[0]
+        eps = _f64(eps)
+        Nt = int(eps.shape[1])
+        eps = eps.reshape(B, Nt, self.Ny)
+        xi = None if xi is None else _f64(xi, (B, Nt, self.Ny))
+        U = _f64(U, (B, Nt, Nu)) if (Nu > 0 and K is None) else None
+        if scale is not None:
+            scale = _f64(scale, (4, self.Ny))
+        if K is not None:
+            K = _f64(K, (Nu, self.Ny))
+            x_ref = None if x_ref is None else _f64(x_ref, (self.Ny,))
+            uscale = None if uscale is None else _f64(uscale, (2, Nu))
+        samples = np.empty((B, Nt, self.Ny)); z_out = np.empty((B, Nt, self.Nx))
+        kept = np.empty((B, Nt, self.Ny), dtype=np.int32)
+        self._check(self.lib.gpmpc_rollout_sample(self.h, B, Nt, _ptr(z0), _ptr(U), _ptr(eps), _ptr(xi), _ptr(scale),
+                                                  _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(samples), _ptr(z_out),
+                                                  kept.ctypes.data_as(_ip)))
+        return samples, z_out, kept
 
     def predict_grad(self, Z, Sigma=None, method=METHOD_TA, want_hess=False):
         """Predict + first derivatives w.r.t. the test inputs (gpmpc_predict_grad).

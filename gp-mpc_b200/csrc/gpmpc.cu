@@ -107,6 +107,8 @@ struct gpmpc_handle_s {
     DevBuf<double> dG;
     double *dZ = nullptr, *dSigma = nullptr, *dMean = nullptr, *dVar = nullptr, *dJ = nullptr, *dCov = nullptr;   // in dIn / dOut
     DevBuf<double> dRoll;             // gpmpc_rollout_batch: [Z | Sigma | U | scale | K | x_ref | uscale | means | vars | cov]
+    DevBuf<double> dSmV;              // gpmpc_rollout_sample: V rows of every step (nloc, Nt, B, Npad)
+    DevBuf<double> dSmp;              //   [eps | xi | U | scale | K | x_ref | uscale | Z (Nt,B,Nx) | samples | kept | m | R]
     DevBuf<double> dIn, dOut;         // [Z | Sigma] and [mean | var | J | cov] slabs: one H2D + one D2H per host call
     int Hcap = 0;                     // test points the slab layout behind dZ .. dCov holds (0: not laid out)
     double* hPinned = nullptr; double* dPinnedAlias = nullptr; size_t hPinnedBytes = 0;
@@ -1510,7 +1512,8 @@ extern "C" int gpmpc_predict_device(gpmpc_handle_t h, int method, int H, const d
 //               (gp_class.py:770-804 with the LQR gain of mpc_class.py:956-976; cov stays in the GP's units, q4)
 // with the reference's operation order (gp_class.py:629-638), so the trajectory is the host loop's bit for bit in open loop.
 // ------------------------------------------------------------------------------------
-// One CTA per trajectory b.  Dynamic shared memory with K: x (Ny) | K cov (Nu x Ny).
+// One CTA per trajectory b.  Dynamic shared memory with K: x (Ny) | K cov (Nu x Ny).  Null cov_t and Sigma: only the next
+// input is formed (gpmpc_rollout_sample).
 __global__ void __launch_bounds__(256)
 rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restrict__ cov_t, const double* __restrict__ u_t,
                         long long u_stride, const double* __restrict__ scale, const double* __restrict__ K,
@@ -1519,6 +1522,7 @@ rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restr
 {
     extern __shared__ double fb_sh[];
     const int Nx = Ny + Nu, tid = threadIdx.x, b = blockIdx.x;
+    const bool with_cov = Sigma != nullptr;                  // before the offsets below
     mean_t += (size_t)b * Ny; cov_t += (size_t)b * Ny * Ny;
     Z += (size_t)b * Nx; Sigma += (size_t)b * Nx * Nx;
     for (int j = tid; j < Nx; j += 256) {
@@ -1534,10 +1538,11 @@ rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restr
             Z[j] = u_t[(size_t)b * u_stride + (j - Ny)];
         }
     }
-    for (int idx = tid; idx < Ny * Ny; idx += 256) {
-        const int r = idx / Ny, c = idx - r * Ny;
-        Sigma[r * Nx + c] = cov_t[idx];
-    }
+    if (with_cov)
+        for (int idx = tid; idx < Ny * Ny; idx += 256) {
+            const int r = idx / Ny, c = idx - r * Ny;
+            Sigma[r * Nx + c] = cov_t[idx];
+        }
     if (!K) return;                                          // uniform over the CTA
     double* KC = fb_sh + Ny;
     __syncthreads();
@@ -1548,6 +1553,7 @@ rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restr
         if (uscale) u = __ddiv_rn(__dsub_rn(u, uscale[i]), uscale[Nu + i]);
         Z[Ny + i] = u;
     }
+    if (!with_cov) return;                                   // a sampled roll-out carries no input covariance
     // K cov (kept for Sigma_uu = (K cov) K^T) and Sigma_xu = cov K^T, Sigma_ux = Sigma_xu^T
     for (int idx = tid; idx < Nu * Ny; idx += 256) {
         const int i = idx / Ny, c = idx - i * Ny;
@@ -1939,14 +1945,13 @@ extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double*
     return GPMPC_OK;
 }
 
-// The solved rows v = L^-1 k(X, z) of the H points at dZ (device, (H, Nx)) for every owned output into the pooled dCovV,
-// layout (nloc, H, Npad) with row stride Npad: HB-point chunks through the ks kernel and the predict product.
-static int solve_rows(gpmpc_handle_t h, const double* dZ, int H)
+// The solved rows v = L^-1 k(X, z) of the H points at dZ (device, (H, Nx)) for every owned output into dst: row h of
+// output a at dst + a * sdst + h * Npad.  HB-point chunks through the ks kernel and the predict product.  mean (may be
+// null): ks^T alpha of every point, (nloc, H), summed from each chunk's ks partials before the next chunk's ks launch
+// overwrites them, in the predict product's order (gpmpc_predict's mean bit for bit).
+static int solve_rows(gpmpc_handle_t h, const double* dZ, int H, double* dst, long long sdst, double* mean = nullptr)
 {
     const int np = h->Npad, Nx = h->Nx, nl = h->nloc;
-    const long long sVall = (long long)H * np;            // all H solved rows of one output
-    // scratch is pooled on the handle (grown on demand), not allocated per call
-    ENSURE(h->dCovV, (long long)nl * sVall);
     int rc = ensure_rows(h);
     if (rc) return rc;
     for (int h0 = 0; h0 < H; h0 += HB) {
@@ -1956,8 +1961,12 @@ static int solve_rows(gpmpc_handle_t h, const double* dZ, int H)
         rc = tri_product(h, h->dKST, h->dLi, Hc, h->dV);
         if (rc) return rc;
         copy2d_kernel<<<dim3(16, std::min(Hc, 64), nl), 128, 0, h->st>>>(h->dV, np, (long long)HB * np,
-                                                                     h->dCovV + (long long)h0 * np, np, sVall, Hc, np);
+                                                                     dst + (long long)h0 * np, np, sdst, Hc, np);
         CUDA_TRY(cudaGetLastError());
+        if (mean) {
+            ks_mean_kernel<<<(nl * Hc + 255) / 256, 256, 0, h->st>>>(h->dPMJ, ks_blocks(h), Nx, Hc, nl, mean + h0, H);
+            CUDA_TRY(cudaGetLastError());
+        }
     }
     return GPMPC_OK;
 }
@@ -1971,13 +1980,88 @@ extern "C" int gpmpc_posterior_cov(gpmpc_handle_t h, int H, const double* Z, dou
     const int np = h->Npad, Nx = h->Nx, nl = h->nloc;
     const long long sVall = (long long)H * np;
     ENSURE(h->dCovOut, (long long)nl * H * H);
+    ENSURE(h->dCovV, (long long)nl * sVall);              // pooled on the handle (grown on demand), not per call
     CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, (size_t)H * Nx * 8, cudaMemcpyHostToDevice, h->st));
-    rc = solve_rows(h, h->dZ, H);
+    rc = solve_rows(h, h->dZ, H, h->dCovV, sVall);
     if (rc) return rc;
     gram_cov_kernel<<<dim3(H, H, nl), 256, 0, h->st>>>(h->dCovV, np, sVall, np, h->dHyp, Nx + 2, Nx, H, h->dCovOut);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(out, h->dCovOut, (size_t)nl * H * H * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
+    return GPMPC_OK;
+}
+
+// A conditional variance at or below SAMPLE_DELTA sf2 is rounding: the point is a function of the earlier ones (DESIGN 4.12)
+#define SAMPLE_DELTA 1e-12
+
+// Sampled roll-outs (kernels.cuh, sample_cond_kernel): per step the V rows of the B current inputs go to slot t of the
+// store (solve_rows, with their means), one CTA per (trajectory, output) draws f_t conditioned on the trajectory's
+// earlier kept points, and rollout_feedback_kernel forms the next input from f_t.  All steps are enqueued back to back;
+// one D2H copy and one synchronisation at the end.
+extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const double* z0, const double* U, const double* eps,
+                                    const double* xi, const double* scale, const double* K, const double* x_ref,
+                                    const double* uscale, double* samples, double* z_out, int* kept)
+{
+    const char* fn = __func__;
+    int rc = predict_guard(h, fn, GPMPC_METHOD_ME, 1);
+    if (rc) return rc;
+    const int Nx = h->Nx, Ny = h->Ny, Nu = Nx - Ny, np = h->Npad, nl = h->nloc;
+    if (B < 1 || Nt < 1 || !z0 || !eps || !samples || (Nu > 0 && !K && !U)) { set_error(h, "%s: null argument / B < 1 / Nt < 1", fn); return GPMPC_ERR_ARG; }
+    if (Nu < 0) { set_error(h, "%s: needs Nx = Ny + Nu with Nu >= 0 (Nx=%d, Ny=%d)", fn, Nx, Ny); return GPMPC_ERR_ARG; }
+    if (K && Nu == 0) { set_error(h, "%s: a feedback gain needs inputs (Nu = 0)", fn); return GPMPC_ERR_ARG; }
+    const int cond_smem = (Nt + 1) * 8 + Nt * 4;           // sample_cond_kernel: c | conditioning steps
+    if (cond_smem > 48 * 1024) { set_error(h, "%s: Nt = %d steps exceed the conditioning kernel's shared memory", fn, Nt); return GPMPC_ERR_ARG; }
+    rc = predict_prepare(h, fn, B, true);
+    if (rc) return rc;
+    NvtxRange nvtx_r("gpmpc.rollout_sample");
+    const size_t Bs = (size_t)B, nE = Bs * Nt * Ny, nX = xi ? nE : 0, nU = U && !K ? Bs * Nt * Nu : 0;
+    const size_t o_xi = nE, o_u = o_xi + nX, o_sc = o_u + nU, o_k = o_sc + 4 * (size_t)Ny, o_xr = o_k + (size_t)Nu * Ny;
+    const size_t o_us = o_xr + Ny, o_z = o_us + 2 * (size_t)Nu, o_s = o_z + (size_t)Nt * Bs * Nx, o_kp = o_s + nE;
+    const size_t o_m = o_kp + nE, o_r = o_m + (size_t)nl * Bs, tot = o_r + (size_t)nl * Bs * Nt * Nt;
+    const long long sVa = (long long)Nt * B * np;          // V rows of one output: (Nt, B, Npad)
+    ENSURE(h->dSmV, nl * sVa);
+    ENSURE(h->dSmp, tot);
+    rc = ensure_pinned(h, o_m * 8);
+    if (rc) return rc;
+    double* pin = h->hPinned;
+    memcpy(pin, eps, nE * 8);
+    if (nX) memcpy(pin + o_xi, xi, nX * 8);
+    if (nU) memcpy(pin + o_u, U, nU * 8);
+    if (scale) memcpy(pin + o_sc, scale, 4 * (size_t)Ny * 8);
+    if (K) memcpy(pin + o_k, K, (size_t)Nu * Ny * 8);
+    if (K && x_ref) memcpy(pin + o_xr, x_ref, (size_t)Ny * 8);
+    if (K && uscale) memcpy(pin + o_us, uscale, 2 * (size_t)Nu * 8);
+    memcpy(pin + o_z, z0, Bs * Nx * 8);                     // slot 0 of the input history
+    double* d = h->dSmp;
+    CUDA_TRY(cudaMemcpyAsync(d, pin, (o_z + Bs * Nx) * 8, cudaMemcpyHostToDevice, h->st));
+    const int fb_smem = K ? Ny * 8 : 0;
+    for (int t = 0; t < Nt; ++t) {
+        double* Zt = d + o_z + (size_t)t * Bs * Nx;
+        rc = solve_rows(h, Zt, B, h->dSmV + (long long)t * B * np, sVa, d + o_m);
+        if (rc) return rc;
+        sample_cond_kernel<<<dim3(B, nl), 256, cond_smem, h->st>>>(h->dSmV, sVa, np, h->N, d + o_m, d + o_z, h->dHyp, Nx + 2,
+                                                                 Nx, Ny, d, xi ? d + o_xi : nullptr, d + o_r, d + o_kp,
+                                                                 d + o_s, Nt, t, SAMPLE_DELTA);
+        CUDA_TRY(cudaGetLastError());
+        if (t + 1 < Nt) {
+            rollout_feedback_kernel<<<B, 256, fb_smem, h->st>>>(d + o_s + (size_t)t * Bs * Ny, nullptr, d + o_u + (size_t)(t + 1) * Nu,
+                                                                (long long)Nt * Nu, scale ? d + o_sc : nullptr, K ? d + o_k : nullptr,
+                                                                K && x_ref ? d + o_xr : nullptr, K && uscale ? d + o_us : nullptr,
+                                                                Ny, Nu, Zt + Bs * Nx, nullptr);
+            CUDA_TRY(cudaGetLastError());
+        }
+    }
+    CUDA_TRY(cudaMemcpyAsync(pin + o_z, d + o_z, (o_m - o_z) * 8, cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    // (t, b) -> (b, t)
+    for (size_t b = 0; b < Bs; ++b)
+        for (int t = 0; t < Nt; ++t) {
+            const size_t src = (size_t)t * Bs + b, dst = b * Nt + t;
+            memcpy(samples + dst * Ny, pin + o_s + src * Ny, (size_t)Ny * 8);
+            if (z_out) memcpy(z_out + dst * Nx, pin + o_z + src * Nx, (size_t)Nx * 8);
+            if (kept)
+                for (int a = 0; a < Ny; ++a) kept[dst * Ny + a] = pin[o_kp + src * Ny + a] != 0.0 ? 1 : 0;
+        }
     return GPMPC_OK;
 }
 
@@ -2019,7 +2103,8 @@ extern "C" int gpmpc_append_greedy(gpmpc_handle_t h, int n, const double* Xc, co
     CUDA_TRY(cudaMemcpyAsync(dYc, Yc, (size_t)n * nl * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaMemsetAsync(dStop, 0, sizeof(int), h->st));
     CUDA_TRY(cudaMemsetAsync(h->dInfo, 0, nl * sizeof(int), h->st));
-    rc = solve_rows(h, dXc, n);
+    ENSURE(h->dCovV, (long long)nl * sV);
+    rc = solve_rows(h, dXc, n, h->dCovV, sV);
     if (rc) return rc;
     const dim3 gw((n + 7) / 8, nl);
     greedy_var_kernel<<<gw, 256, 0, h->st>>>(h->dCovV, np, sV, N, n, h->dHyp, Nx + 2, Nx, dVar);

@@ -1566,6 +1566,97 @@ greedy_downdate_kernel(double* __restrict__ V, int ldv, long long sV, double* __
 }
 
 // ---------------------------------------------------------------------------------------
+// Sampled roll-outs (gpmpc_rollout_sample): trajectory b, output a, step t is one draw of the GP posterior conditioned on
+// the values the same draw took at the earlier kept points z_s of b (DESIGN 4.12).  With v_t = L_a^-1 k_a(X, z_t):
+//   m_t = k_a(X, z_t)^T alpha_a,   c_s = k_a(z_t, z_s) - v_t . v_s (kept s < t),   c_tt = sf2_a - |v_t|^2
+//   w = R^-1 c,  d = c_tt - |w|^2,  f_t = m_t + sum_j w_j eps_j + sqrt(d) eps_t
+// R (lower, at most Nt x Nt per (b, a)) is the Cholesky factor of the joint covariance of the kept points, row by row
+// [w, sqrt(d)], so that f - m = R eps over the kept points.  d <= delta sf2: f_t = m_t + sum_j w_j eps_j, not kept.
+// ---------------------------------------------------------------------------------------
+// m[a][r] = ks_r^T alpha_a for the H points of one ks launch: the sum of the ks kernel's block partials PMJ[a][r][blk][0]
+// with the association of the predict product's psk_reduce_mj (even / odd blocks in ascending order, then their sum), so
+// m is gpmpc_predict's mean bit for bit.  One thread per (output, row), grid (ceil(nloc H / 256)).
+__global__ void __launch_bounds__(256)
+ks_mean_kernel(const double* __restrict__ PMJ, int nblk, int Nx, int H, int nloc, double* __restrict__ m, long long sm)
+{
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= nloc * H) return;
+    const int a = i / H, r = i - a * H;
+    const double* pm = PMJ + (long long)i * nblk * (Nx + 1);
+    double s0 = 0.0, s1 = 0.0;
+    int b = 0;
+    for (; b + 2 <= nblk; b += 2) { s0 += pm[(long long)b * (Nx + 1)]; s1 += pm[(long long)(b + 1) * (Nx + 1)]; }
+    if (b < nblk) s0 += pm[(long long)b * (Nx + 1)];
+    m[(long long)a * sm + r] = s0 + s1;
+}
+
+// One CTA per (trajectory b, output a) at step t, grid (B, nloc).  V rows of (a, s, b) at V + a sVa + (s B + b) ldv;
+// Zh (Nt, B, Nx); m (nloc, B) of this step; eps, xi (B, Nt, Ny) (xi may be null); Rf (nloc, B, Nt, Nt);
+// kept, samp (Nt, B, Ny).  Dynamic shared memory: c (Nt + 1 doubles) | conditioning steps (Nt ints).
+__global__ void __launch_bounds__(256)
+sample_cond_kernel(const double* __restrict__ V, long long sVa, int ldv, int N, const double* __restrict__ m,
+                   const double* __restrict__ Zh, const double* __restrict__ hyp, int hyp_ld, int Nx, int Ny,
+                   const double* __restrict__ eps, const double* __restrict__ xi, double* __restrict__ Rf,
+                   double* __restrict__ kept, double* __restrict__ samp, int Nt, int t, double delta)
+{
+    extern __shared__ double sc_sh[];
+    __shared__ int nk_s;
+    const int b = blockIdx.x, a = blockIdx.y, B = gridDim.x;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    double* c = sc_sh;
+    int* idx = reinterpret_cast<int*>(sc_sh + Nt + 1);
+    const double* hp = hyp + (long long)a * hyp_ld;
+    const double* Va = V + (long long)a * sVa;
+    const double* vt = Va + ((long long)t * B + b) * ldv;
+    const double* zt = Zh + ((long long)t * B + b) * Nx;
+    if (tid == 0) {
+        int k = 0;
+        for (int s = 0; s < t; ++s)
+            if (kept[((long long)s * B + b) * Ny + a] != 0.0) idx[k++] = s;
+        nk_s = k;
+    }
+    __syncthreads();
+    const int k = nk_s;
+    const double sf2 = hp[Nx] * hp[Nx];
+    for (int j = warp; j <= k; j += 8) {                  // j = k: the point itself
+        const int s = (j < k) ? idx[j] : t;
+        const double dot = warp_dot(vt, Va + ((long long)s * B + b) * ldv, N);
+        double q = 0.0;
+        if (j < k && lane < Nx) {                         // Nx <= 32; direct differences
+            const double df = (zt[lane] - Zh[((long long)s * B + b) * Nx + lane]) / hp[lane];
+            q = df * df;
+        }
+        q = warp_sum(q);
+        if (lane == 0) c[j] = ((j < k) ? sf2 * exp(-0.5 * q) : sf2) - dot;
+    }
+    __syncthreads();
+    if (tid != 0) return;
+    double* R = Rf + ((long long)a * B + b) * Nt * Nt;
+    const double* e = eps + (long long)b * Nt * Ny + a;  // eps of (b, s, a) at e[s Ny]
+    double ww = 0.0, we = 0.0;
+    for (int j = 0; j < k; ++j) {                         // forward substitution in place: c[j] <- w_j
+        double w = c[j];
+        for (int i = 0; i < j; ++i) w -= R[j * Nt + i] * c[i];
+        w /= R[j * Nt + j];
+        c[j] = w;
+        ww += w * w;
+        we += w * e[(long long)idx[j] * Ny];
+    }
+    const double d = c[k] - ww;
+    const bool keep = d > delta * sf2;
+    double f = m[(long long)a * B + b] + we;
+    if (keep) {
+        const double sd = sqrt(d);
+        f += sd * e[(long long)t * Ny];
+        for (int j = 0; j < k; ++j) R[k * Nt + j] = c[j];
+        R[k * Nt + k] = sd;
+    }
+    const long long o = ((long long)t * B + b) * Ny + a;
+    kept[o] = keep ? 1.0 : 0.0;
+    samp[o] = xi ? f + hp[Nx + 1] * xi[((long long)b * Nt + t) * Ny + a] : f;
+}
+
+// ---------------------------------------------------------------------------------------
 // Removal of training point i from an N-point factorisation (gpmpc_remove), O(N^2) per output.  With lambda = L[i][i],
 // n = N - i - 1 trailing points (r, s, j, k index them: old row / column i + 1 + r):
 //   p_r = -lambda Li[i+1+r][i] (= L33^-1 l32),  t_-1 = 1,  t_r = t_{r-1} + p_r^2,

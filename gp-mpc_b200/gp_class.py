@@ -54,6 +54,15 @@ def lqr(A, B, Q, R):
     return K, P, np.linalg.eigvals(A + B @ K)
 
 
+def _sqrt_psd(S):
+    """F with F F^T = S: the Cholesky factor, or for a singular S the eigenvalue square root (zero on its null space)."""
+    try:
+        return np.linalg.cholesky(S)
+    except np.linalg.LinAlgError:
+        w, V = np.linalg.eigh(S)
+        return V * np.sqrt(np.clip(w, 0.0, None))[None, :]
+
+
 def _is_symbolic(v):
     """CasADi SX/MX arguments (mpc_class.py:390-412 calls predict with MX symbols)."""
     return type(v).__module__.split('.')[0] == 'casadi' and type(v).__name__ in ('MX', 'SX')
@@ -594,6 +603,107 @@ class GP:
                     self.__feedback_blocks(covar[b], K[b], c_last[k])
                 covar[b, :self.__Ny, :self.__Ny] = c_last[k]
         return True
+
+    def sample_rollout(self, x0, u, n_samples, seed=None, Sigma0=None, feedback=False, x_ref=None, Q=None, R=None,
+                       process_noise=False):
+        """ Monte Carlo trajectories of the learned dynamics (gpmpc_rollout_sample): each sample is one draw f of the
+        GP posterior evaluated along the states that draw visits, x_{t+1} = f(x_t, u_t), with f(z_t) conditioned on the
+        values the same draw took at z_0 .. z_{t-1}.  This is the ground truth the propagated moments of ``rollout``
+        ('TA', 'ME', 'EM') approximate for the model.
+
+        Shapes follow ``rollout``: x0:(Ny,) with u:(Nt,Nu) returns (n_samples, Nt+1, Ny); x0:(B,Ny) with u:(B,Nt,Nu)
+        returns (B, n_samples, Nt+1, Ny).  Caller units; row 0 holds the drawn initial states.
+
+        The first GP input z_0 = [x0, u_0] (standardised when normalize) is drawn from N(z_0, Sigma0).  Sigma0 is
+        (Nx,Nx) or (B,Nx,Nx) in the GP's input units; by default it is ``rollout``'s initial covariance, diag(sn2) on x
+        and 1e-6 on u, so that step 1 of the samples is distributed exactly as the 'EM' prediction of step 1 says.
+        feedback=True applies u_t = K (x_t - x_ref) with ``rollout``'s LQR gain per trajectory (defaults Q = I, R = I,
+        x_ref = 0) to every sampled state; u then only sets Nt and the linearisation point.  process_noise=True adds
+        sn_a xi to every sampled state (the draw itself stays conditioned on the latent f).
+
+        ``numpy.random.default_rng(seed)`` draws, in this order: the initial perturbations n (B, n_samples, Nx), with
+        z_0 = mean + n F^T and F = cholesky(Sigma0) (for a singular Sigma0 the eigenvalue square root); then the function
+        draws eps (B, n_samples, Nt, Ny); then, with process_noise, xi (B, n_samples, Nt, Ny).
+
+        With normalize=True every sampled state is re-standardised with the X scalers before the next step, as
+        ``rollout`` does with the mean.  ``rollout`` feeds the Y-standardised covariance as the input covariance of the
+        next step (q4), so differences between the spread of the samples and its propagated variances at t >= 2 can
+        come from that quirk as well as from the approximations. """
+        if self.__sharded_outputs():
+            raise NotImplementedError('sample_rollout needs all outputs on one GPU (build the GP with a single-process Comm)')
+        if self.__prior_mean_in_predict and self.__has_prior_mean():
+            raise NotImplementedError('sample_rollout draws from the zero-mean posterior the engine holds; '
+                                      'prior_mean_in_predict with a prior mean function is not supported')
+        Nx, Ny, Nu = self.__Nx, self.__Ny, self.__Nu
+        x0 = np.asarray(x0, dtype=np.float64)
+        single = x0.ndim < 2
+        X0 = x0.reshape(1, Ny) if single else x0.reshape(-1, Ny)
+        nb = X0.shape[0]
+        u = np.asarray(u, dtype=np.float64)
+        if single:
+            U = (u.reshape(-1, Nu) if Nu > 0 else np.zeros((u.shape[0] if u.ndim else 0, 0)))[None]
+        else:
+            U = u.reshape(nb, -1, Nu) if Nu > 0 else np.zeros((nb, u.shape[1] if u.ndim > 1 else 0, 0))
+        Nt, ns = U.shape[1], int(n_samples)
+        if ns < 1 or Nt < 1:
+            raise ValueError('sample_rollout needs n_samples >= 1 and at least one step (got %d, %d)' % (ns, Nt))
+        if feedback and Nu == 0:
+            raise ValueError('sample_rollout(feedback=True) needs a model with inputs (Nu > 0)')
+        if Sigma0 is None:
+            S0 = np.eye(Nx) * 1e-6
+            S0[:Ny, :Ny] = np.diag(self.__hyper[:, Nx + 1] ** 2)
+            S0 = np.tile(S0, (nb, 1, 1))
+        else:
+            S0 = np.asarray(Sigma0, dtype=np.float64)
+            if S0.shape not in ((Nx, Nx), (nb, Nx, Nx)):
+                raise ValueError('Sigma0 must be (%d, %d) or (%d, %d, %d)' % (Nx, Nx, nb, Nx, Nx))
+            S0 = np.broadcast_to(S0, (nb, Nx, Nx))
+        K = None
+        if feedback:
+            Q = np.eye(Ny) if Q is None else np.asarray(Q, dtype=np.float64)
+            R = np.eye(Nu) if R is None else np.asarray(R, dtype=np.float64)
+            x_ref = np.zeros(Ny) if x_ref is None else np.asarray(x_ref, dtype=np.float64).reshape(Ny)
+            K = self.__lqr_gains(X0, U[:, 0], Q, R)
+            un = np.stack([_matmul_seq(K[b], (X0[b] - x_ref)[:, None])[:, 0] for b in range(nb)])
+        else:
+            un = U[:, 0]
+        zx, Ug, scale, uscale = X0, U, None, None
+        if self.__normalize:
+            zx = self.standardize(X0, self.__meanX, self.__stdX)
+            un = self.standardize(un, self.__meanU, self.__stdU)
+            Ug = self.standardize(U, self.__meanU, self.__stdU)
+            scale = np.stack([self.__stdY, self.__meanY, self.__meanX, self.__stdX])
+            uscale = np.stack([self.__meanU, self.__stdU])
+        zbar = np.concatenate([zx, un], 1)
+        rng = np.random.default_rng(seed)
+        n0 = rng.standard_normal((nb, ns, Nx))
+        eps = rng.standard_normal((nb, ns, Nt, Ny))
+        xi = rng.standard_normal((nb, ns, Nt, Ny)) if process_noise else None
+        z0 = np.stack([zbar[b] + n0[b] @ _sqrt_psd(S0[b]).T for b in range(nb)])        # (nb, ns, Nx)
+        Ur = np.repeat(Ug, ns, 0)
+        rows = lambda g: (np.asarray(g)[:, None] * ns + np.arange(ns)[None, :]).reshape(-1)
+        z0f, epsf = z0.reshape(nb * ns, Nx), eps.reshape(nb * ns, Nt, Ny)
+        xif = None if xi is None else xi.reshape(nb * ns, Nt, Ny)
+        samp = np.empty((nb * ns, Nt, Ny))
+        eng = self.__engine
+        if K is None:
+            samp[:] = eng.rollout_sample(z0f, Ur, epsf, xif, scale)[0]
+        else:                                            # one pass per distinct gain, as rollout
+            groups = {}
+            for b in range(nb):
+                groups.setdefault(K[b].tobytes(), []).append(b)
+            for g in groups.values():
+                r = rows(g)
+                samp[r] = eng.rollout_sample(z0f[r], Ur[r], epsf[r], None if xif is None else xif[r], scale, K[g[0]],
+                                             x_ref, uscale)[0]
+        out = np.empty((nb * ns, Nt + 1, Ny))
+        out[:, 0] = z0f[:, :Ny]
+        out[:, 1:] = samp
+        if self.__normalize:
+            out[:, 0] = self.inverse_mean(out[:, 0], self.__meanX, self.__stdX)
+            out[:, 1:] = self.inverse_mean(out[:, 1:], self.__meanY, self.__stdY)
+        out = out.reshape(nb, ns, Nt + 1, Ny)
+        return out[0] if single else out
 
     def get_size(self):
         """ (N, Ny, Nu)  (reference gp_class.py:266-274) """

@@ -236,6 +236,30 @@ int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, const doubl
                         const double* Sigma0, const double* scale, const double* K, const double* x_ref,
                         const double* uscale, double* means, double* vars, double* cov_last);
 
+/* Sample trajectories of the learned dynamics: each of the B trajectories is one draw f of the GP posterior, evaluated along
+ * the inputs that draw visits.  Per output a and step t, f_t(z_t) is drawn conditioned on the values the same draw took
+ * at the earlier points z_0 .. z_{t-1} of the trajectory, so the whole trajectory satisfies f - m = R eps with R the
+ * Cholesky factor of the joint posterior covariance of its points (a consistent function sample, not fresh noise per
+ * step).  A point whose conditional variance is at the rounding level (<= 1e-12 sf2: the trajectory returns to a point
+ * it visited) is determined by the earlier ones: f_t is the conditional mean and its eps is unused.  The next input is
+ * formed from the sampled state exactly as gpmpc_rollout_batch forms it from the mean (scale, K, x_ref, uscale).
+ *   z0      (B, Nx)       first inputs, already drawn, GP input units
+ *   U       (B, Nt, Nu)   open-loop inputs; NULL when Nu = 0 or K is given (as gpmpc_rollout_batch)
+ *   eps     (B, Nt, Ny)   standard normals of the function draws
+ *   xi      (B, Nt, Ny)   process-noise standard normals, or NULL: the state is f_t + sn_a xi (the noise does not enter
+ *                         the conditioning, which is on the latent f)
+ *   scale, K, x_ref, uscale  as gpmpc_rollout_batch
+ *   samples (B, Nt, Ny)   the next states, GP output units (like gpmpc_rollout_batch's means)
+ *   z_out   (B, Nt, Nx)   or NULL: the input used at each step
+ *   kept    (B, Nt, Ny)   or NULL: 1 where the point entered the conditioning set
+ * GPMPC_ERR_ARG: B < 1, Nt < 1, z0 / eps / samples NULL, Nu > 0 with neither U nor K, K with Nu = 0, Nt too large for
+ * the per-trajectory factor's shared memory (Nt <= 4095).  GPMPC_ERR_STATE: not factorised, or the handle does not own
+ * every output.  Every check runs before any work.  Device memory: 8 Ny Nt B Npad bytes of solved rows (8 GB at
+ * Ny = 8, Npad = 16384, B = 256, Nt = 30) plus 8 (Ny B Nt^2 + B Nt (Nx + 4 Ny)) bytes. */
+int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const double* z0, const double* U, const double* eps,
+                         const double* xi, const double* scale, const double* K, const double* x_ref,
+                         const double* uscale, double* samples, double* z_out, int* kept);
+
 /* Problem sizes of a handle (GP.get_size, gp_class.py:266-274: N, and Nx, Ny). */
 int gpmpc_get_size(gpmpc_handle_t h, int* N, int* Nx, int* Ny);
 
