@@ -751,8 +751,9 @@ ks_tile_kernel(const double* __restrict__ XT, int ldx, int N, int Nx,
         for (int d = 0; d < NXP; ++d) red[warp][r][d + 1] = aj[d];
     }
     __syncthreads();
-    if (tid < 8 * (Nx + 1)) {
-        const int rr = tid / (Nx + 1), f = tid - rr * (Nx + 1), hh = rg * 8 + rr;
+    // 8 (Nx + 1) values: more than the 256 threads at Nx = 32
+    for (int idx = tid; idx < 8 * (Nx + 1); idx += 256) {
+        const int rr = idx / (Nx + 1), f = idx - rr * (Nx + 1), hh = rg * 8 + rr;
         double sacc = ((red[0][rr][f] + red[1][rr][f]) + (red[2][rr][f] + red[3][rr][f])) +
                       ((red[4][rr][f] + red[5][rr][f]) + (red[6][rr][f] + red[7][rr][f]));
         if (f > 0) sacc *= ie[f - 1];                        // df was scaled by 1/ell: one more 1/ell makes (x - z)/ell^2

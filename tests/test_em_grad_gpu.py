@@ -42,9 +42,12 @@ def _case(case):
         if case == 'tank_pp':
             Sigma = np.stack([Sigma * (1 + 0.1 * h) for h in range(Z.shape[0])])
         return X, Y, hyper, Z, Sigma
-    N, Nx, Ny, H = {'syn1000': (1000, 8, 4, 3), 'syn300': (300, 17, 2, 2)}[case]
+    N, Nx, Ny, H = {'syn1000': (1000, 8, 4, 3), 'syn300': (300, 17, 2, 2), 'syn12': (600, 12, 3, 3)}[case]
     p = orc.synthetic_problem(N, Nx, Ny, config_id=N + Nx, H=H)
-    return p['X'], p['Y'], p['hyper'], p['Z'], p['Sigma']
+    hyper = p['hyper']
+    if case == 'syn12':                   # well-conditioned (sn = 0.3): alpha and K^-1 carry no conditioning error
+        hyper = hyper.copy(); hyper[:, Nx + 1] = 0.3
+    return p['X'], p['Y'], hyper, p['Z'], p['Sigma']
 
 
 def _engine_factor(eng, Ny):
@@ -53,9 +56,15 @@ def _engine_factor(eng, Ny):
             np.stack([eng.get(L.GET_CHOL, a) for a in range(Ny)]))
 
 
-@pytest.mark.parametrize('case', ['tank', 'tank_pp', 'tank_large', 'syn1000', 'syn300'])
+# (dmean, dcov) bars against the closed form; syn12 is well-conditioned, measured dmean 5.7e-15, dcov 2.8e-13 on an
+# H100 SXM at 700 W
+GRAD_TOL = {'syn12': (1e-13, 3e-12)}
+
+
+@pytest.mark.parametrize('case', ['tank', 'tank_pp', 'tank_large', 'syn1000', 'syn300', 'syn12'])
 def test_em_grad_vs_closed_oracle(case):
-    """syn1000: Nx = 8, N ~ 1000 (16 tiles); syn300: Nx = 17, the 32 bucket; tank_pp: one Sigma per point."""
+    """syn1000: Nx = 8, N ~ 1000 (16 tiles); syn300: Nx = 17, the 32 bucket; syn12: Nx = 12, the 16 bucket of em_prep,
+    em_moments and em_grad_pair; tank_pp: one Sigma per point."""
     X, Y, hyper, Z, Sigma = _case(case)
     Ny = Y.shape[1]
     eng = _fit(X, Y, hyper)
@@ -68,8 +77,9 @@ def test_em_grad_vs_closed_oracle(case):
     alpha, chol = _engine_factor(eng, Ny)
     ref = emo.em_grad_closed(X, hyper, alpha, chol, Z, Sigma)
     errs = {k: relinf(o[k], ref[k]) for k in DERIV}
-    assert errs['dmean_dz'] < 1e-6 and errs['dmean_dSigma'] < 1e-6, errs
-    assert errs['dcov_dz'] < 1e-5 and errs['dcov_dSigma'] < 1e-5, errs
+    tm, tc = GRAD_TOL.get(case, (1e-6, 1e-5))
+    assert errs['dmean_dz'] < tm and errs['dmean_dSigma'] < tm, errs
+    assert errs['dcov_dz'] < tc and errs['dcov_dSigma'] < tc, errs
     assert np.array_equal(o['dmean_dSigma'], np.swapaxes(o['dmean_dSigma'], 2, 3))
     assert np.array_equal(o['dcov_dSigma'], np.swapaxes(o['dcov_dSigma'], 3, 4))
     assert np.array_equal(o['dcov_dSigma'], np.swapaxes(o['dcov_dSigma'], 1, 2))
@@ -78,6 +88,20 @@ def test_em_grad_vs_closed_oracle(case):
     for k in o:
         assert np.array_equal(o[k], o2[k]), k
     eng.close()
+
+
+def test_em_forward_nxp16_vs_exact_moment():
+    """The forward 'EM' moments at Nx = 12 (em_prep / em_moments<16>) on the well-conditioned syn12 model against the
+    fp64 restatement gp_exact_moment with postfit's K^-1.  Measured on an H100 SXM at 700 W: mean 1.2e-13, cov
+    3.9e-11 (the restatement's own cancellation between beta beta^T and K^-1)."""
+    X, Y, hyper, Z, Sigma = _case('syn12')
+    eng = _fit(X, Y, hyper)
+    mean, _, cov, _ = eng.predict(Z, Sigma, _L().METHOD_EM, want_jac=False)
+    eng.close()
+    post = orc.postfit(X, Y, hyper, lapack_general_solve=False)
+    for h in range(Z.shape[0]):
+        mo, co = orc.gp_exact_moment(post['invK'], X, Y, hyper, Z[h], Sigma)
+        assert relinf(mean[h], mo) < 1e-12 and relinf(cov[h], co) < 1e-9, h
 
 
 @pytest.mark.parametrize('case,tol', [('tank', 1e-5), ('car', 1e-3)])

@@ -1,6 +1,6 @@
 """Small end-to-end pass over every kernel of the engine for compute-sanitizer
-(memcheck / racecheck / synccheck / initcheck):  K build, leaf + DMMA GEMMs (cp.async and TMA
-tensor-map feeds), alpha, NLML + gradient, the persistent stream-K predict kernel with tile
+(memcheck / racecheck / synccheck / initcheck):  K build, leaf + DMMA GEMMs (cp.async feeds; the TMA
+tensor-map feed on a second, 24-output handle), alpha, NLML + gradient, the persistent stream-K predict kernel with tile
 fix-ups (several grid sizes, lower and upper mode), predict_grad, EM and its derivatives, rank-1 append, GP.covar, sampled roll-outs.
     compute-sanitizer --tool racecheck python tools/sanitize_run.py"""
 import os, sys
@@ -15,7 +15,7 @@ N, Nx, Ny, H = int(os.environ.get('SAN_N', 700)), 5, 2, 21
 p = orc.synthetic_problem(N, Nx, Ny, config_id=3, H=H)
 eng = gp_mpc_b200.Engine(N, Nx, Ny, device=0)
 eng.set_data(p['X'], p['Y']); eng.set_hyper(p['hyper'])
-eng.set_option('small_tiles', 4)          # push the top-level products onto the TMA tensor-map GEMM as well
+eng.set_option('small_tiles', 4)          # 128x64 cp.async GEMM for all but the smallest products (TMA: eng_t below)
 eng.factorize()
 post = orc.postfit(p['X'], p['Y'], p['hyper'], lapack_general_solve=False)
 print('chol', relinf(eng.get(L.GET_CHOL, 0), post['chol'][0]), flush=True)
@@ -45,4 +45,12 @@ eng.factorize()
 ok = eng.append(p['X'][0] + 0.3, p['Y'][0])
 print('append', ok, flush=True)
 eng.close()
+# the TMA tensor-map GEMM serves products of at least 4 * SMs 128x64 tiles: Npad 1152 with 24 outputs puts the bottom
+# panel of the top-level split there (576 tiles)
+pt = orc.synthetic_problem(1130, Nx, 24, config_id=4)
+eng_t = gp_mpc_b200.Engine(1130, Nx, 24, device=0)
+eng_t.set_data(pt['X'], pt['Y']); eng_t.set_hyper(pt['hyper'])
+eng_t.factorize()
+print('chol (TMA)', relinf(eng_t.get(L.GET_CHOL, 23), orc.factor_large(pt['X'], pt['Y'][:, 23], pt['hyper'][23])['chol']), flush=True)
+eng_t.close()
 print('done', flush=True)
