@@ -1,7 +1,7 @@
 """Small end-to-end pass over every kernel of the engine for compute-sanitizer
 (memcheck / racecheck / synccheck / initcheck):  K build, leaf + DMMA GEMMs (cp.async feeds; the TMA
 tensor-map feed on a second, 24-output handle), alpha, NLML + gradient, the persistent stream-K predict kernel with tile
-fix-ups (several grid sizes, lower and upper mode), predict_grad, EM and its derivatives, rank-1 append, GP.covar, sampled roll-outs.
+fix-ups (several grid sizes, lower and upper mode), gpmpc_predict_device, gpmpc_predict's copy transports, predict_grad, EM and its derivatives, rank-1 append, GP.covar, sampled roll-outs.
     compute-sanitizer --tool racecheck python tools/sanitize_run.py"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -24,6 +24,15 @@ for ctas in (0, 1, 3, 37):
     eng.set_option('predict_ctas', ctas)
     mean, var, cov, jac = eng.predict(p['Z'], p['Sigma'], L.METHOD_TA)
     print('predict ctas=%d' % ctas, relinf(mean, mo), relinf(var, vo), flush=True)
+eng.set_option('predict_ctas', 0)
+ref = eng.predict(p['Z'], p['Sigma'], L.METHOD_TA)
+# gpmpc_predict_device (the entry bench.py times): device inputs and outputs, no host copies, same bits as gpmpc_predict
+import torch
+dZ, dS = torch.from_numpy(p['Z']).cuda(), torch.from_numpy(p['Sigma']).cuda()
+dout = [torch.empty(s, dtype=torch.float64, device='cuda') for s in ((H, Ny), (H, Ny), (H, Ny, Ny), (H, Ny, Nx))]
+torch.cuda.synchronize()
+eng.predict_device(L.METHOD_TA, H, dZ.data_ptr(), dS.data_ptr(), 0, *[t.data_ptr() for t in dout], sync=True)
+print('predict_device', all(np.array_equal(t.cpu().numpy(), r) for t, r in zip(dout, ref)), flush=True)
 eng.set_option('predict_ctas', 5)
 g = eng.predict_grad(p['Z'], p['Sigma'], L.METHOD_TA, want_hess=True)
 fd = orc.predict_grad_fd(p['X'], p['hyper'], post['alpha'], post['chol'], p['Z'], p['Sigma'], 'TA')
@@ -53,4 +62,15 @@ eng_t.set_data(pt['X'], pt['Y']); eng_t.set_hyper(pt['hyper'])
 eng_t.factorize()
 print('chol (TMA)', relinf(eng_t.get(L.GET_CHOL, 23), orc.factor_large(pt['X'], pt['Y'][:, 23], pt['hyper'][23])['chol']), flush=True)
 eng_t.close()
+# gpmpc_predict's copy transports: H = 300 points of 16 outputs (Nx = 10) are 1.07 MB of outputs, above the 1 MiB that
+# the assembling CTA writes straight into mapped host memory, so the inputs go H2D into dIn and the outputs D2H from dOut
+pc_ = orc.synthetic_problem(200, 10, 16, config_id=5)
+eng_c = gp_mpc_b200.Engine(200, 10, 16, device=0)
+eng_c.set_data(pc_['X'], pc_['Y']); eng_c.set_hyper(pc_['hyper'])
+eng_c.factorize()
+Zc = 0.5 * np.random.default_rng(5).standard_normal((300, 10))
+mc, vc, cc, jc = eng_c.predict(Zc, 1e-4 * np.eye(10), L.METHOD_TA)
+_, vj, _, _ = eng_c.predict(Zc, None, L.METHOD_ME, want_cov=False)
+print('predict (copy out)', bool(np.isfinite(cc).all()), np.array_equal(vc, vj), flush=True)
+eng_c.close()
 print('done', flush=True)
