@@ -36,6 +36,8 @@ SYMBOLS = [
     ('gpmpc_build_K', C.c_int, [_H, C.c_int, _dp]),
     ('gpmpc_factorize', C.c_int, [_H, C.c_double, _ip]),
     ('gpmpc_nlml', C.c_int, [_H, C.c_int, _dp, _dp, _dp]),
+    ('gpmpc_loo', C.c_int, [_H, _dp, _dp, _dp]),
+    ('gpmpc_loo_nlpp', C.c_int, [_H, C.c_int, _dp, _dp, _dp]),
     ('gpmpc_predict', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp]),
     ('gpmpc_predict_grad', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     ('gpmpc_predict_hess', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp,
@@ -208,6 +210,25 @@ class Engine:
             raise np.linalg.LinAlgError(self.lib.gpmpc_last_error(self.h).decode())
         self._check(rc)
         return (nll.value, g) if grad else nll.value
+
+    def loo(self):
+        """gpmpc_loo: leave-one-out predictions of the training points on the current factorisation of every owned
+        output -> mean (out_count, N), var (out_count, N) (of the noisy targets), nlpp (out_count,)."""
+        mean = np.empty((self.out_count, self.N)); var = np.empty((self.out_count, self.N))
+        nlpp = np.empty(self.out_count)
+        self._check(self.lib.gpmpc_loo(self.h, _ptr(mean), _ptr(var), _ptr(nlpp)))
+        return mean, var, nlpp
+
+    def loo_nlpp(self, a, theta, grad=True):
+        """gpmpc_loo_nlpp: the negative LOO log predictive probability of output a at theta (and its gradient)."""
+        theta = _f64(theta, (self.Nx + 2,))
+        val = C.c_double(0.0)
+        g = np.empty(self.Nx + 2) if grad else None
+        rc = self.lib.gpmpc_loo_nlpp(self.h, int(a), _ptr(theta), C.byref(val), _ptr(g))
+        if rc == ERR_NOTPD:
+            raise np.linalg.LinAlgError(self.lib.gpmpc_last_error(self.h).decode())
+        self._check(rc)
+        return (val.value, g) if grad else val.value
 
     def get(self, what, a):
         N = self.N

@@ -114,6 +114,7 @@ struct gpmpc_handle_s {
     double* hPinned = nullptr; double* dPinnedAlias = nullptr; size_t hPinnedBytes = 0;
     // nlml scratch
     DevBuf<double> dU, dKinv, dGradPart, dGrad;
+    DevBuf<double> dLoo;              // gpmpc_loo / gpmpc_loo_nlpp: [mean | var | nlpp | c partials | sw | u | b | tmp | 0]
     bool has_data = false, has_hyper = false, factorized = false;
     // EM scratch
     DevBuf<double> dEmTr, dEMP, dEmE, dEmF, dEmW, dEmIJ;
@@ -707,14 +708,19 @@ static int compute_kinv(gpmpc_handle_t h, int al)
     return GPMPC_OK;
 }
 
-template <int NXP>
-static cudaError_t launch_grad(gpmpc_handle_t h, int al, const double* dHyp)
+// 1/2 tr((W - alpha alpha^T) dK/dtheta) for every hyper-parameter into dGrad, W = the lower triangle in dKinv
+static int launch_grad(gpmpc_handle_t h, const double* dHyp, const double* alpha)
 {
     const int T = h->Npad / KB_TILE;
     const int smem = 2 * h->Nx * KB_TILE * 8;
-    nlml_grad_kernel<NXP><<<T * (T + 1) / 2, 256, smem, h->st>>>(h->dXT, h->Npad, h->N, h->Nx, dHyp, h->dKinv, h->Npad,
-                                                                 h->dAlpha + (long long)al * h->Npad, h->dGradPart);
-    return cudaGetLastError();
+    CUDA_TRY(nxp_dispatch(h->Nx, [&](auto nxp) {
+        nlml_grad_kernel<decltype(nxp)::value><<<T * (T + 1) / 2, 256, smem, h->st>>>(h->dXT, h->Npad, h->N, h->Nx, dHyp,
+                                                                                      h->dKinv, h->Npad, alpha, h->dGradPart);
+        return cudaGetLastError();
+    }));
+    nlml_grad_final_kernel<<<h->Nx + 2, 256, 0, h->st>>>(h->dGradPart, T * (T + 1) / 2, h->Nx, dHyp, h->dGrad);
+    CUDA_TRY(cudaGetLastError());
+    return GPMPC_OK;
 }
 
 extern "C" int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* nll, double* grad)
@@ -739,14 +745,127 @@ extern "C" int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* 
     if (grad) {
         rc = compute_kinv(h, al);
         if (rc) return rc;
-        CUDA_TRY(nxp_dispatch(h->Nx, [&](auto nxp) { return launch_grad<decltype(nxp)::value>(h, al, h->dHypTmp); }));
-        const int T = h->Npad / KB_TILE;
-        nlml_grad_final_kernel<<<m, 256, 0, h->st>>>(h->dGradPart, T * (T + 1) / 2, h->Nx, h->dHypTmp, h->dGrad);
-        CUDA_TRY(cudaGetLastError());
+        rc = launch_grad(h, h->dHypTmp, h->dAlpha + (long long)al * h->Npad);
+        if (rc) return rc;
         CUDA_TRY(cudaMemcpyAsync(grad, h->dGrad, m * 8, cudaMemcpyDeviceToHost, h->st));
     }
     CUDA_TRY(cudaStreamSynchronize(h->st));
     *nll = 0.5 * res[1] + 0.5 * res[0];                      // optimize.py:355
+    return GPMPC_OK;
+}
+
+// ------------------------------------------------------------------------------------
+// leave-one-out cross-validation (kernels.cuh, loo_*)
+// ------------------------------------------------------------------------------------
+// dLoo for `batch` outputs at the current N: [mean (batch*N) | var (batch*N) | nlpp (batch) | c partials
+// (batch*nch*N) | sw | u | b | tmp | zero (Npad each)]
+struct LooLayout {
+    int nch; double *mean, *var, *nlpp, *P, *sw, *u, *b, *tmp, *zero;
+};
+
+static int loo_layout(gpmpc_handle_t h, int batch, LooLayout* o)
+{
+    const long long N = h->N, np = h->Npad;
+    o->nch = (int)((N + TRT_ROWS - 1) / TRT_ROWS);
+    ENSURE(h->dLoo, 2 * batch * N + batch + (long long)batch * o->nch * N + 5 * np);
+    o->mean = h->dLoo; o->var = o->mean + batch * N; o->nlpp = o->var + batch * N; o->P = o->nlpp + batch;
+    o->sw = o->P + (long long)batch * o->nch * N; o->u = o->sw + np; o->b = o->u + np; o->tmp = o->b + np;
+    o->zero = o->tmp + np;
+    return GPMPC_OK;
+}
+
+// LOO mean, variance and NLPP of `batch` consecutive local outputs from al on the current factors (O(N^2) each);
+// with_w: also sqrt(w) and u of the (single) output
+static int loo_launch(gpmpc_handle_t h, int al, int batch, const LooLayout& o, bool with_w)
+{
+    const int N = h->N, np = h->Npad;
+    const long long nN = (long long)o.nch * N;
+    loo_colnorm_part_kernel<<<dim3((N + 31) / 32, o.nch, batch), 256, 0, h->st>>>(h->dLi + (long long)al * slab(h), np,
+                                                                                 slab(h), o.P, nN, N);
+    CUDA_TRY(cudaGetLastError());
+    loo_point_kernel<<<batch, 1024, 0, h->st>>>(o.P, nN, o.nch, h->dAlpha + (long long)al * np, h->dY + (long long)al * np,
+                                                np, N, o.mean, o.var, o.nlpp, with_w ? o.sw : nullptr,
+                                                with_w ? o.u : nullptr, np);
+    CUDA_TRY(cudaGetLastError());
+    return GPMPC_OK;
+}
+
+extern "C" int gpmpc_loo(gpmpc_handle_t h, double* mean, double* var, double* nlpp)
+{
+    if (!h) return GPMPC_ERR_ARG;
+    if (!h->factorized) { set_error(h, "gpmpc_loo: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
+    if (h->N < 2) { set_error(h, "gpmpc_loo: needs N >= 2 training points (N = %d)", h->N); return GPMPC_ERR_ARG; }
+    CUDA_TRY(cudaSetDevice(h->device));
+    NvtxRange nvtx_r("gpmpc.loo");
+    const int nl = h->nloc;
+    LooLayout o;
+    int rc = loo_layout(h, nl, &o);
+    if (rc) return rc;
+    rc = loo_launch(h, 0, nl, o, false);
+    if (rc) return rc;
+    const size_t bytes = (size_t)nl * h->N * 8;
+    if (mean) CUDA_TRY(cudaMemcpyAsync(mean, o.mean, bytes, cudaMemcpyDeviceToHost, h->st));
+    if (var) CUDA_TRY(cudaMemcpyAsync(var, o.var, bytes, cudaMemcpyDeviceToHost, h->st));
+    if (nlpp) CUDA_TRY(cudaMemcpyAsync(nlpp, o.nlpp, nl * 8, cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    return GPMPC_OK;
+}
+
+extern "C" int gpmpc_loo_nlpp(gpmpc_handle_t h, int a, const double* theta, double* nlpp, double* grad)
+{
+    if (!h || !theta || !nlpp) return GPMPC_ERR_ARG;
+    if (!h->has_data) { set_error(h, "gpmpc_loo_nlpp: set_data first"); return GPMPC_ERR_STATE; }
+    CUDA_TRY(cudaSetDevice(h->device));
+    const int al = local_index(h, a);
+    if (al < 0) return GPMPC_ERR_ARG;
+    const int m = h->Nx + 2, N = h->N, np = h->Npad;
+    for (int d = 0; d < h->Nx; ++d) if (theta[d] == 0.0) { set_error(h, "gpmpc_loo_nlpp: zero length scale"); return GPMPC_ERR_ARG; }
+    if (N < 2) { set_error(h, "gpmpc_loo_nlpp: needs N >= 2 training points (N = %d)", N); return GPMPC_ERR_ARG; }
+    factor_stale(h);
+    NvtxRange nvtx_r("gpmpc.loo_nlpp");
+    CUDA_TRY(cudaMemcpyAsync(h->dHypTmp, theta, m * 8, cudaMemcpyHostToDevice, h->st));
+    int used = 0;
+    int rc = factor_one(h, al, h->dHypTmp, 1e-8, &used);      // the jitter retry of gpmpc_nlml
+    if (rc) { if (rc == GPMPC_ERR_NOTPD) set_error(h, "gpmpc_loo_nlpp: K not positive definite even with jitter"); return rc; }
+    rc = launch_alpha(h, al, 1);
+    if (rc) return rc;
+    LooLayout o;
+    rc = loo_layout(h, 1, &o);
+    if (rc) return rc;
+    rc = loo_launch(h, al, 1, o, grad != nullptr);        // c always from the column norms: the same NLPP bits either way
+    if (rc) return rc;
+    double val = 0.0;
+    CUDA_TRY(cudaMemcpyAsync(&val, o.nlpp, 8, cudaMemcpyDeviceToHost, h->st));
+    if (grad) {
+        const double* Li = h->dLi + (long long)al * slab(h);
+        const double* alpha = h->dAlpha + (long long)al * np;
+        rc = compute_kinv(h, al);                          // C (lower) in dKinv
+        if (rc) return rc;
+        // b = C u = Li^T (Li u)
+        trmv_lower_kernel<<<(N + 7) / 8, 256, 0, h->st>>>(Li, np, 0, o.u, 0, o.tmp, 0, N);
+        CUDA_TRY(cudaGetLastError());
+        trmv_lower_T_kernel<<<(N + 31) / 32, 256, 0, h->st>>>(Li, np, 0, o.tmp, 0, o.b, 0, N);
+        CUDA_TRY(cudaGetLastError());
+        // G = (C diag(sqrt w)) (C diag(sqrt w))^T = C diag(w) C: lower tiles into dKinv, over C diag(sqrt w) in dU
+        loo_mirror_scale_kernel<<<dim3(np / 32, np / 32), dim3(32, 8), 0, h->st>>>(h->dKinv, np, o.sw, h->dU, N);
+        CUDA_TRY(cudaGetLastError());
+        GemmParams p;
+        memset(&p, 0, sizeof(p));
+        p.A = h->dU; p.lda = np; p.B = h->dU; p.ldb = np; p.C = h->dKinv; p.ldc = np;
+        p.mt = np / 128; p.nt = np / 128; p.K = np; p.alpha = 1.0; p.beta = 0.0; p.lower = 1;
+        CUDA_TRY(gemm128(h, h->st, true, p, 1));
+        loo_w_kernel<<<dim3((N + 255) / 256, N), 256, 0, h->st>>>(h->dKinv, np, o.b, alpha, N);
+        CUDA_TRY(cudaGetLastError());
+        // the trace pass with W in place of K^-1 and alpha = 0: 1/2 tr(W dK/dtheta), doubled on the host (exact)
+        CUDA_TRY(cudaMemsetAsync(o.zero, 0, (size_t)np * 8, h->st));
+        rc = launch_grad(h, h->dHypTmp, o.zero);
+        if (rc) return rc;
+        CUDA_TRY(cudaMemcpyAsync(grad, h->dGrad, m * 8, cudaMemcpyDeviceToHost, h->st));
+    }
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    if (grad)
+        for (int q = 0; q < m; ++q) grad[q] *= 2.0;
+    *nlpp = val;
     return GPMPC_OK;
 }
 

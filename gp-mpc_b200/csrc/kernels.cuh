@@ -2286,3 +2286,114 @@ hess_cov_kernel(int Ny, int Nx, int method_ta, const double* __restrict__ Sigma,
         o[g * Nx + f] = s;
     }
 }
+
+// ---------------------------------------------------------------------------------------
+// Leave-one-out cross-validation (gpmpc_loo, gpmpc_loo_nlpp; R&W section 5.4.2, eqs. 5.10-5.14).  With C = K^-1 =
+// Li^T Li, alpha = C y and c_i = C_ii = sum_{k >= i} Li[k][i]^2 (the column norms of Li):
+//   LOO mean  y_i - alpha_i / c_i,   LOO variance 1 / c_i,
+//   NLPP = sum_i [ 1/2 log 2pi - 1/2 log c_i + alpha_i^2 / (2 c_i) ]
+//   dNLPP/dtheta_j = tr(W dK/dtheta_j),  W = C diag(w) C - sym(b alpha^T),
+//   w_i = (1 + alpha_i^2 / c_i) / (2 c_i),  u = alpha / c,  b = C u,  sym(M) = (M + M^T) / 2.
+// The trace runs through nlml_grad_kernel with W in place of K^-1 and a zero vector in place of alpha.
+// ---------------------------------------------------------------------------------------
+
+// Column-norm partials of Li, only its lower triangle up to n read: grid (ceil(n/32), ceil(n/TRT_ROWS), batch).  Block
+// (k-block, chunk c) sums Li[i][k]^2 over rows [c*TRT_ROWS, (c+1)*TRT_ROWS), i >= k, of its 32 columns into P[batch][c][k]
+// (the layout of trmv_lower_T_part_kernel): each warp reads 32 consecutive entries of a row.  Chunks entirely above the
+// diagonal are skipped; loo_point_kernel sums chunks c >= k/TRT_ROWS in ascending order.
+__global__ void __launch_bounds__(256)
+loo_colnorm_part_kernel(const double* __restrict__ Li, int ld, long long sL, double* __restrict__ P, long long sP, int n)
+{
+    __shared__ double red[8][33];
+    const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+    const int k0 = blockIdx.x * 32, c = blockIdx.y;
+    const int r1 = min(n, (c + 1) * TRT_ROWS);
+    if (r1 <= k0) return;
+    const int r0 = max(c * TRT_ROWS, k0);
+    const int k = k0 + lane;
+    const double* Lb = Li + (long long)blockIdx.z * sL;
+    double s = 0.0;
+    for (int i = r0 + wp; i < r1; i += 8)
+        if (i >= k) {
+            const double v = Lb[(long long)i * ld + k];
+            s = fma(v, v, s);
+        }
+    red[wp][lane] = s;
+    __syncthreads();
+    if (wp == 0 && k < n) {
+        double r = 0.0;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) r += red[q][lane];
+        P[(long long)blockIdx.z * sP + (long long)c * n + k] = r;
+    }
+}
+
+// Per output (one CTA of 1024 threads each): c_i from the partials, the LOO mean and variance of the N points, and
+// nlpp[b] = the sum of the per-point terms in a fixed order.  sw / u (single output, may be null): sqrt(w_i) and
+// alpha_i / c_i for i < N, zero up to ldv.
+__global__ void __launch_bounds__(1024)
+loo_point_kernel(const double* __restrict__ P, long long sP, int nch,
+                 const double* __restrict__ alpha, const double* __restrict__ y, long long sv, int N,
+                 double* __restrict__ mean, double* __restrict__ var, double* __restrict__ nlpp,
+                 double* __restrict__ sw, double* __restrict__ u, int ldv)
+{
+    __shared__ double red[32];
+    const double* Pb = P + (long long)blockIdx.x * sP;
+    const double* al = alpha + (long long)blockIdx.x * sv;
+    const double* yy = y + (long long)blockIdx.x * sv;
+    double s = 0.0;
+    for (int i = threadIdx.x; i < N; i += 1024) {
+        double c = 0.0;
+        for (int q = i / TRT_ROWS; q < nch; ++q) c += Pb[(long long)q * N + i];
+        const double a = al[i], r = a / c;
+        mean[(long long)blockIdx.x * N + i] = yy[i] - r;
+        var[(long long)blockIdx.x * N + i] = 1.0 / c;
+        s += 0.91893853320467274178 - 0.5 * log(c) + 0.5 * a * r;       // 1/2 log 2pi - 1/2 log c + alpha^2 / (2c)
+        if (sw) {
+            sw[i] = sqrt(fma(a, r, 1.0) / (2.0 * c));
+            u[i] = r;
+        }
+    }
+    if (sw)
+        for (int i = N + threadIdx.x; i < ldv; i += 1024) { sw[i] = 0.0; u[i] = 0.0; }
+    s = warp_sum(s);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int q = 0; q < 32; ++q) t += red[q];
+        nlpp[blockIdx.x] = t;
+    }
+}
+
+// S = C diag(sw), full and square, from the lower-stored symmetric C (32x32 tiles through shared memory, grid
+// (ld/32, ld/32), block (32, 8)); rows and columns >= N are zero.
+__global__ void loo_mirror_scale_kernel(const double* __restrict__ C, int ld, const double* __restrict__ sw,
+                                        double* __restrict__ S, int N)
+{
+    __shared__ double tile[32][33];
+    const int bi = blockIdx.y, bj = blockIdx.x;
+    if (bj > bi) return;
+    const int tx = threadIdx.x, ty = threadIdx.y;
+    for (int r = ty; r < 32; r += 8)          // only the lower triangle of a diagonal tile holds C
+        if (bi != bj || tx <= r) tile[r][tx] = C[(long long)(bi * 32 + r) * ld + bj * 32 + tx];
+    __syncthreads();
+    for (int r = ty; r < 32; r += 8) {
+        const int row = bi * 32 + r, col = bj * 32 + tx;
+        const double v = (bi == bj && tx > r) ? tile[tx][r] : tile[r][tx];
+        S[(long long)row * ld + col] = (row < N && col < N) ? v * sw[col] : 0.0;
+        if (bi != bj) {        // the mirrored tile: S[bj*32 + r][bi*32 + tx] = C[bi*32 + tx][bj*32 + r] sw[bi*32 + tx]
+            const int row2 = bj * 32 + r, col2 = bi * 32 + tx;
+            S[(long long)row2 * ld + col2] = (row2 < N && col2 < N) ? tile[tx][r] * sw[col2] : 0.0;
+        }
+    }
+}
+
+// W = G - sym(b alpha^T) in place on the lower triangle of the first N rows (grid (ceil(N/256), N))
+__global__ void __launch_bounds__(256)
+loo_w_kernel(double* __restrict__ W, int ld, const double* __restrict__ b, const double* __restrict__ alpha, int N)
+{
+    const int r = blockIdx.y, c = blockIdx.x * 256 + threadIdx.x;
+    if (c > r) return;
+    W[(long long)r * ld + c] -= 0.5 * fma(b[r], alpha[c], alpha[r] * b[c]);
+}

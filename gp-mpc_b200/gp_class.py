@@ -26,7 +26,7 @@ import scipy.linalg
 from . import _lib
 from .comm import Comm
 from .mean_functions import mean_function, mean_jacobian
-from .optimize import train_gp_b200
+from .optimize import fit_objective, train_gp_b200
 from .partition import choose_mode, output_block, point_block
 
 _GPU_METHODS = {'ME': _lib.METHOD_ME, 'TA': _lib.METHOD_TA, 'EM': _lib.METHOD_EM}
@@ -213,7 +213,9 @@ class GP:
                  xlb=None, xub=None, ulb=None, uub=None,
                  multistart=1, normalize=True, warm_start=False,
                  optimize_nummeric=True):
-        """reference gp_class.py:78-142"""
+        """reference gp_class.py:78-142.  opts={'objective': 'loo'} fits the leave-one-out predictive probability
+        instead of the marginal likelihood (optimize.fit_objective)."""
+        fit_objective(opts)
         self.__mean_func = mean_func
         self.__normalize = normalize
 
@@ -264,19 +266,31 @@ class GP:
             Y_test = self.standardize(Y_test, self.__meanY, self.__stdY)
             X_test = self.standardize(X_test, self.__meanZ, self.__stdZ)
 
-        N, Ny = Y_test.shape
         mean, var = self.__predict_std(X_test, None, 'ME', want_cov=False, want_jac=False)[:2]
         var = var + self.noise_variance()[None, :]                      # :161
+        return self.__report_validation(Y_test, mean, var, '# Validation of GP model ', 'Num test samples')
+
+    def validate_loo(self):
+        """ Validate the GP model without a test set: validate's SMSE and MNLP, in the GP's standardised space, with
+        every training point predicted from the other N-1 (leave-one-out cross-validation, Rasmussen & Williams
+        section 5.4.2) in place of test predictions.  MNLP is the LOO NLPP over N.  Returns (SMSE, MNLP) per output. """
+        mean, var = self.__loo_std()
+        return self.__report_validation(self.__Y, mean, var, '# Leave-one-out validation of GP model ',
+                                        'Num left-out samples')
+
+    def __report_validation(self, Y_test, mean, var, title, count_label):
+        """The error measures of the reference's validate (gp_class.py:145-190) and its banner; var includes sn2."""
+        N, Ny = Y_test.shape
         loss = np.sum((Y_test - mean) ** 2, 0) / N
         NLP = np.sum(0.5 * np.log(2 * np.pi * var) + ((Y_test - mean) ** 2) / (2 * var), 0)
         SMSE = loss / np.std(Y_test, 0)                                 # :166 (q15)
         MNLP = NLP / N
 
         print('\n________________________________________')
-        print('# Validation of GP model ')
+        print(title)
         print('----------------------------------------')
         print('* Num training samples: ' + str(self.__N))
-        print('* Num test samples: ' + str(N))
+        print('* %s: %d' % (count_label, N))
         print('----------------------------------------')
         print('* Mean squared error: ')
         for i in range(Ny):
@@ -777,6 +791,33 @@ class GP:
             for k in range(blk.shape[0]):
                 covar[b + k] = blk[k].reshape(n) if one_d else blk[k]
         return covar
+
+    def loo_predict(self):
+        """ Leave-one-out predictions of the training points: point i predicted by the GP on the other N-1, from the
+        current factorisation in O(N^2) per output (gpmpc_loo).  Returns mean (N, Ny), in caller units
+        (de-standardised like predict_batch), and var (N, Ny), the variance of the noisy target in the GP's output
+        units (standardised, q4).  With a prior mean the mean is y_i - alpha_i / c_i, the prior mean included.
+        Combine with remove_data to drop points the rest of the data does not explain. """
+        mean, var = self.__loo_std()
+        if self.__normalize:
+            mean = self.inverse_mean(mean, self.__meanY, self.__stdY)
+        return mean, var
+
+    def __loo_std(self):
+        """LOO mean and variance (N, Ny) in the standardised space, gathered over ranks in 'outputs' mode."""
+        eng = self.__engine
+        m, v, _ = eng.loo()
+        mine = [(eng.out_begin, m, v)]
+        if self.__comm.world > 1 and self.__mode == 'outputs':
+            mine = self.__comm.allgather_object(mine[0])
+        mean, var = np.zeros((self.__N, self.__Ny)), np.zeros((self.__N, self.__Ny))
+        for b, mb, vb in mine:
+            mean[:, b:b + mb.shape[0]] = mb.T
+            var[:, b:b + vb.shape[0]] = vb.T
+        if self.__has_prior_mean():                  # the engine factorised the residual y - m(X)
+            mean += np.column_stack([mean_function(self.__hyper[a], self.__X, self.__mean_func)
+                                     for a in range(self.__Ny)])
+        return mean, var
 
     def update_data_all(self, X_new, Y_new):
         """ Update training data with all new observations  (reference gp_class.py:474-550):

@@ -40,6 +40,20 @@ def bounds_and_init(X, y, fixed_bounds=False):
     return np.hstack((lb.reshape(num_hyp, 1), ub.reshape(num_hyp, 1))), init
 
 
+def fit_objective(optimizer_opts):
+    """The objective optimizer_opts['objective'] selects, checked before any engine call:
+    'nlml' (default), the negative log marginal likelihood (gpmpc_nlml, R&W eq. 5.9), or
+    'loo', the negative leave-one-out log predictive probability (gpmpc_loo_nlpp, R&W eqs. 5.10-5.13), which is more
+    robust than the marginal likelihood when the SE kernel is misspecified.  'loo' does not fit mean parameters."""
+    opts = optimizer_opts or {}
+    objective = opts.get('objective', 'nlml')
+    if objective not in ('nlml', 'loo'):
+        raise ValueError("optimizer_opts['objective'] must be 'nlml' or 'loo', got %r" % (objective,))
+    if objective == 'loo' and opts.get('fit_mean', False):
+        raise ValueError("optimizer_opts: objective 'loo' cannot fit mean parameters (fit_mean=True)")
+    return objective
+
+
 def train_gp_b200(engine, X, Y, meanFunc='zero', hyper_init=None, multistart=1,
                   optimizer_opts=None, verbose=True):
     """Fit the outputs owned by `engine`; returns hyper rows for those outputs
@@ -63,12 +77,14 @@ def train_gp_b200(engine, X, Y, meanFunc='zero', hyper_init=None, multistart=1,
     fixed_bounds = False
     fit_mean = False
     parallel_fits = True
+    objective = fit_objective(optimizer_opts)
     if optimizer_opts is not None:
         optimizer_opts = dict(optimizer_opts)
         jac_mode = optimizer_opts.pop('jac', jac_mode)
         fixed_bounds = bool(optimizer_opts.pop('fixed_bounds', False))
         fit_mean = bool(optimizer_opts.pop('fit_mean', False)) and h_m > 0
         parallel_fits = bool(optimizer_opts.pop('parallel_fits', True))
+        optimizer_opts.pop('objective', None)
         options.update(optimizer_opts)
     if jac_mode not in ('analytic', 'fd'):
         raise ValueError("optimizer_opts['jac'] must be 'analytic' or 'fd'")
@@ -106,6 +122,22 @@ def train_gp_b200(engine, X, Y, meanFunc='zero', hyper_init=None, multistart=1,
         # multistart re-runs from the SAME init (optimize.py:462-469, q8): identical results,
         # so one run decides
         t0 = time.time()
+        if objective == 'loo':
+            # SLSQP runs on theta / scale with sn measured in units of its upper bound: dNLPP/dsn is ~1e5 times the other
+            # components where sn ~ 1e-3, and unscaled the quasi-Newton steps stall far from a stationary point
+            # (DESIGN section 4.13).  Same bounds and initial point in theta.
+            scale = np.ones(Nx + 2)
+            scale[Nx + 1] = bounds[Nx + 1, 1]
+
+            def fun_loo(x):
+                if jac_mode != 'analytic':
+                    return eng.loo_nlpp(a, x * scale, grad=False)
+                f, g = eng.loo_nlpp(a, x * scale, grad=True)
+                return f, g * scale
+
+            res = minimize(fun_loo, init / scale, method='SLSQP', jac=(jac_mode == 'analytic'), options=options,
+                           bounds=bounds / scale[:, None], tol=1e-12)
+            return np.clip(res.x * scale, bounds[:, 0], bounds[:, 1]), time.time() - t0
         res = minimize(fun, init, method='SLSQP', jac=(jac_mode == 'analytic'), options=options,
                        bounds=bounds, tol=1e-12)
         if fit_mean:

@@ -111,6 +111,25 @@ int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info);
  * (optimize.py:466-467).  Invalidates the factorisation of output a. */
 int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* nll, double* grad);
 
+/* Leave-one-out cross-validation on the current factorisation of every OWNED output (Rasmussen & Williams
+ * eqs. 5.10-5.12): each training point predicted from the other N-1.  With C = K^-1, alpha = C y (y the target the
+ * handle factorised, the residual y - m(X) under a prior mean) and c_i = C_ii, the column norms of L^-1:
+ *   mean[a][i] = y_i - alpha_i / c_i,  var[a][i] = 1 / c_i (the variance of the noisy y_i),
+ *   nlpp[a] = sum_i [ 1/2 log 2pi - 1/2 log c_i + alpha_i^2 / (2 c_i) ]  (the negative LOO log predictive probability).
+ * mean, var:(out_count,N), nlpp:(out_count) host buffers, each may be NULL.  O(N^2) per output, no solve; works after
+ * gpmpc_append, gpmpc_append_greedy and gpmpc_remove and on any handle, sharded or reserved.  Every sum runs in a
+ * fixed order: repeated calls give identical bits.
+ *   GPMPC_ERR_STATE: not factorised.  GPMPC_ERR_ARG: N < 2.  Every check runs before any work. */
+int gpmpc_loo(gpmpc_handle_t h, double* mean, double* var, double* nlpp);
+
+/* The LOO counterpart of gpmpc_nlml, as a hyper-parameter fit objective: factorises global output a at theta:(Nx+2,)
+ * with the same single 1e-8 jitter retry, returns the NLPP of gpmpc_loo and (grad != NULL) its analytic gradient
+ * (R&W eq. 5.13 as a trace: dNLPP/dtheta_j = tr(W dK/dtheta_j), W = C diag(w) C - sym(b alpha^T),
+ * w_i = (1 + alpha_i^2/c_i) / (2 c_i), b = C (alpha / c)).  The NLPP has the same bits with and without grad.
+ * Same argument checks as gpmpc_nlml, and GPMPC_ERR_ARG for N < 2.  Scratch: gpmpc_nlml's two Npad^2 slabs.
+ * Invalidates the factorisation of output a. */
+int gpmpc_loo_nlpp(gpmpc_handle_t h, int a, const double* theta, double* nlpp, double* grad);
+
 /* Batched prediction at H test points (host buffers; copies are part of the call).
  * Z:(H,Nx) in the GP's input space; Sigma:(Nx,Nx) or (H,Nx,Nx) when sigma_per_point
  * (ignored for ME, may be NULL); outputs (any may be NULL): mean:(H,Ny) var:(H,Ny)

@@ -1,7 +1,7 @@
 """Small end-to-end pass over every kernel of the engine for compute-sanitizer
 (memcheck / racecheck / synccheck / initcheck):  K build, leaf + DMMA GEMMs (cp.async feeds; the TMA
 tensor-map feed on a second, 24-output handle), alpha, NLML + gradient, the persistent stream-K predict kernel with tile
-fix-ups (several grid sizes, lower and upper mode), gpmpc_predict_device, gpmpc_predict's copy transports, predict_grad, EM and its derivatives, rank-1 append, GP.covar, sampled roll-outs.
+fix-ups (several grid sizes, lower and upper mode), gpmpc_predict_device, gpmpc_predict's copy transports, predict_grad, EM and its derivatives, rank-1 append, GP.covar, sampled roll-outs, leave-one-out cross-validation and its gradient.
     compute-sanitizer --tool racecheck python tools/sanitize_run.py"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -48,6 +48,9 @@ print('em_grad finite', all(bool(np.isfinite(eg[k]).all()) for k in eg), np.arra
 pc = eng.posterior_cov(p['Z'][:5])
 sm, _, kept = eng.rollout_sample(p['Z'][:3], np.repeat(p['Z'][:3, None, Ny:], 4, 1), np.ones((3, 4, Ny)))
 print('rollout_sample finite', bool(np.isfinite(sm).all()), int(kept.sum()), flush=True)
+_, _, ln = eng.loo()
+fl, gl = eng.loo_nlpp(0, p['hyper'][0] * 0.9, grad=True)
+print('loo', ln, fl, bool(np.isfinite(gl).all()), flush=True)
 nll, gr = eng.nlml(0, p['hyper'][0] * 0.9, grad=True)
 print('nlml', nll, orc.calc_NLL(p['hyper'][0] * 0.9, p['X'], p['Y'][:, 0], False), flush=True)
 eng.factorize()
