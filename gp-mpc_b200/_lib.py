@@ -135,19 +135,19 @@ class Engine:
     def __init__(self, N, Nx, Ny, out_begin=0, out_count=None, device=0, capacity=None):
         """capacity: training points to reserve room for (gpmpc_create_reserve), so appends up to it need no refit."""
         self.lib = load()
-        self.N, self.Nx, self.Ny = int(N), int(Nx), int(Ny)
+        N, self.Nx, self.Ny = int(N), int(Nx), int(Ny)
         self._stage, self._stage_lock = {}, threading.Lock()     # predict(): per-shape host staging arrays + their pointers
         self.out_begin = int(out_begin)
         self.out_count = int(Ny - out_begin if out_count is None else out_count)
         self.device = int(device)
         # the padded size the library allocates: appends succeed while N stays within it
-        self.capacity = -(-max(self.N, int(capacity or 0)) // 128) * 128
+        self.capacity = -(-max(N, int(capacity or 0)) // 128) * 128
         self.h = _H()
         if capacity is None:
-            rc = self.lib.gpmpc_create(self.N, self.Nx, self.Ny, self.out_begin, self.out_count, self.device,
+            rc = self.lib.gpmpc_create(N, self.Nx, self.Ny, self.out_begin, self.out_count, self.device,
                                        C.byref(self.h))
         else:
-            rc = self.lib.gpmpc_create_reserve(self.N, int(capacity), self.Nx, self.Ny, self.out_begin, self.out_count,
+            rc = self.lib.gpmpc_create_reserve(N, int(capacity), self.Nx, self.Ny, self.out_begin, self.out_count,
                                                self.device, C.byref(self.h))
         if rc != OK:
             msg = self.lib.gpmpc_last_error(None).decode()
@@ -156,6 +156,8 @@ class Engine:
 
     # -- plumbing ---------------------------------------------------------------------
     def _check(self, rc):
+        if rc == ERR_NOTPD:          # factorize / nlml / loo_nlpp: K not positive definite even with jitter
+            raise np.linalg.LinAlgError(self.lib.gpmpc_last_error(self.h).decode())
         if rc != OK:
             raise GpmpcError(rc, self.lib.gpmpc_last_error(self.h).decode())
 
@@ -173,6 +175,12 @@ class Engine:
     @property
     def local_outputs(self):
         return range(self.out_begin, self.out_begin + self.out_count)
+
+    @property
+    def N(self):                     # the handle's count: appends and removals change it
+        n = C.c_int(0)
+        self._check(self.lib.gpmpc_get_size(self.h, C.byref(n), None, None))
+        return n.value
 
     # -- model ------------------------------------------------------------------------
     def set_data(self, X, Y):
@@ -195,20 +203,14 @@ class Engine:
 
     def factorize(self, jitter=1e-8):
         info = np.zeros(self.out_count, dtype=np.int32)
-        rc = self.lib.gpmpc_factorize(self.h, float(jitter), info.ctypes.data_as(_ip))
-        if rc == ERR_NOTPD:
-            raise np.linalg.LinAlgError(self.lib.gpmpc_last_error(self.h).decode())
-        self._check(rc)
+        self._check(self.lib.gpmpc_factorize(self.h, float(jitter), info.ctypes.data_as(_ip)))
         return info
 
     def nlml(self, a, theta, grad=True):
         theta = _f64(theta, (self.Nx + 2,))
         nll = C.c_double(0.0)
         g = np.empty(self.Nx + 2) if grad else None
-        rc = self.lib.gpmpc_nlml(self.h, int(a), _ptr(theta), C.byref(nll), _ptr(g))
-        if rc == ERR_NOTPD:
-            raise np.linalg.LinAlgError(self.lib.gpmpc_last_error(self.h).decode())
-        self._check(rc)
+        self._check(self.lib.gpmpc_nlml(self.h, int(a), _ptr(theta), C.byref(nll), _ptr(g)))
         return (nll.value, g) if grad else nll.value
 
     def loo(self):
@@ -224,10 +226,7 @@ class Engine:
         theta = _f64(theta, (self.Nx + 2,))
         val = C.c_double(0.0)
         g = np.empty(self.Nx + 2) if grad else None
-        rc = self.lib.gpmpc_loo_nlpp(self.h, int(a), _ptr(theta), C.byref(val), _ptr(g))
-        if rc == ERR_NOTPD:
-            raise np.linalg.LinAlgError(self.lib.gpmpc_last_error(self.h).decode())
-        self._check(rc)
+        self._check(self.lib.gpmpc_loo_nlpp(self.h, int(a), _ptr(theta), C.byref(val), _ptr(g)))
         return (val.value, g) if grad else val.value
 
     def get(self, what, a):
@@ -387,13 +386,13 @@ class Engine:
 
     def append(self, x_new, y_new):
         """Rank-1 append of one training point; returns False when the padded capacity is full
-        or positive definiteness is lost (caller refits), True on success."""
+        or positive definiteness is lost (caller refits), True on success.  After a lost positive
+        definiteness the point is in the model (N counts it) and the handle needs factorize()."""
         x = _f64(x_new, (self.Nx,)); y = _f64(y_new, (self.Ny,))
         rc = self.lib.gpmpc_append(self.h, _ptr(x), _ptr(y))
         if rc in (ERR_STATE, ERR_NOTPD):
             return False
         self._check(rc)
-        self.N += 1
         return True
 
     def append_greedy(self, Xc, Yc, n_new):
@@ -413,7 +412,6 @@ class Engine:
         if rc not in (OK, ERR_NOTPD):
             self._check(rc)
         k = added.value
-        self.N += k
         return picked[:k].astype(np.int64), score[:k].copy(), rc == OK
 
     def remove(self, idx):
@@ -421,7 +419,6 @@ class Engine:
         updates of L and L^-1; raises GpmpcError on a bad index or an unfactorised model (which is then untouched)."""
         idx = np.ascontiguousarray(np.asarray(idx, dtype=np.int64).reshape(-1), dtype=np.int32)
         self._check(self.lib.gpmpc_remove(self.h, idx.size, idx.ctypes.data_as(_ip) if idx.size else None))
-        self.N -= idx.size
 
     def posterior_cov(self, Z):
         """(out_count, H, H): sf2 - V^T V per owned output (GP.covar)."""

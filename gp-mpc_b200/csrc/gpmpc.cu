@@ -547,6 +547,33 @@ static void factor_caches_stale(gpmpc_handle_t h) { h->u_valid = false; h->em_ki
 // the factor no longer matches the data or hyper-parameters, or its slabs were used as scratch: gpmpc_factorize first
 static void factor_stale(gpmpc_handle_t h) { h->factorized = false; factor_caches_stale(h); }
 
+enum ModelNeed { NEED_DATA, NEED_HYPER, NEED_FACTOR };     // data; data and hyper-parameters; a factorised model
+
+// State check of the model entry `fn` (the name its errors carry), then the handle's device is selected
+static int model_guard(gpmpc_handle_t h, const char* fn, ModelNeed need)
+{
+    if (!h) return GPMPC_ERR_ARG;
+    if (need == NEED_DATA && !h->has_data) { set_error(h, "%s: set_data first", fn); return GPMPC_ERR_STATE; }
+    if (need == NEED_HYPER && (!h->has_data || !h->has_hyper)) { set_error(h, "%s: set_data and set_hyper first", fn); return GPMPC_ERR_STATE; }
+    if (need == NEED_FACTOR && !h->factorized) { set_error(h, "%s: call gpmpc_factorize first", fn); return GPMPC_ERR_STATE; }
+    CUDA_TRY(cudaSetDevice(h->device));
+    return GPMPC_OK;
+}
+
+// alpha, log det K and y^T alpha of every owned output from the factor, after the factor changed
+static int refresh_alpha(gpmpc_handle_t h)
+{
+    const int nl = h->nloc;
+    factor_caches_stale(h);
+    int rc = launch_alpha(h, 0, nl);
+    if (rc) return rc;
+    std::vector<double> res(2 * nl);
+    CUDA_TRY(cudaMemcpyAsync(res.data(), h->dRes, 2 * nl * 8, cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    for (int a = 0; a < nl; ++a) { h->logdet[a] = res[2 * a]; h->yalpha[a] = res[2 * a + 1]; }
+    return GPMPC_OK;
+}
+
 extern "C" int gpmpc_set_data(gpmpc_handle_t h, const double* X, const double* Y)
 {
     if (!h || !X || !Y) return GPMPC_ERR_ARG;
@@ -578,8 +605,7 @@ static int local_index(gpmpc_handle_t h, int a);
 extern "C" int gpmpc_set_y(gpmpc_handle_t h, int a, const double* y)
 {
     if (!h || !y) return GPMPC_ERR_ARG;
-    if (!h->has_data) { set_error(h, "gpmpc_set_y: set_data first"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
+    { int rc = model_guard(h, __func__, NEED_DATA); if (rc) return rc; }
     const int al = local_index(h, a);
     if (al < 0) return GPMPC_ERR_ARG;
     CUDA_TRY(cudaMemcpyAsync(h->dY + (long long)al * h->Npad, y, (size_t)h->N * 8, cudaMemcpyHostToDevice, h->st));
@@ -635,12 +661,11 @@ static int extract_to_host(gpmpc_handle_t h, const double* src, double* dst, int
 
 extern "C" int gpmpc_build_K(gpmpc_handle_t h, int a, double* K_out)
 {
-    if (!h) return GPMPC_ERR_ARG;
-    if (!h->has_data || !h->has_hyper) { set_error(h, "gpmpc_build_K: set_data and set_hyper first"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
+    int rc = model_guard(h, __func__, NEED_HYPER);
+    if (rc) return rc;
     const int al = local_index(h, a);
     if (al < 0) return GPMPC_ERR_ARG;
-    int rc = ensure_nlml_scratch(h);
+    rc = ensure_nlml_scratch(h);
     if (rc) return rc;
     const double zero = 0.0;
     CUDA_TRY(cudaMemcpyAsync(h->dJit + al, &zero, 8, cudaMemcpyHostToDevice, h->st));
@@ -653,14 +678,13 @@ extern "C" int gpmpc_build_K(gpmpc_handle_t h, int a, double* K_out)
 
 extern "C" int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info)
 {
-    if (!h) return GPMPC_ERR_ARG;
-    if (!h->has_data || !h->has_hyper) { set_error(h, "gpmpc_factorize: set_data and set_hyper first"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
+    int rc = model_guard(h, __func__, NEED_HYPER);
+    if (rc) return rc;
     NvtxRange nvtx_r("gpmpc.factorize");
     const int nl = h->nloc;
     CUDA_TRY(cudaMemsetAsync(h->dJit, 0, nl * sizeof(double), h->st));
     CUDA_TRY(cudaMemsetAsync(h->dInfo, 0, nl * sizeof(int), h->st));
-    int rc = launch_kbuild(h, h->dHyp, h->dJit, h->dL, nl, 0);
+    rc = launch_kbuild(h, h->dHyp, h->dJit, h->dL, nl, 0);
     if (rc) return rc;
     rc = potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, h->Npad, nl);
     if (rc) return rc;
@@ -680,13 +704,9 @@ extern "C" int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info)
         if (info) info[a] = h->jitter_used[a];
     }
     if (worst) return worst;
-    rc = launch_alpha(h, 0, nl);
+    rc = refresh_alpha(h);
     if (rc) return rc;
-    std::vector<double> res(2 * nl);
-    CUDA_TRY(cudaMemcpyAsync(res.data(), h->dRes, 2 * nl * 8, cudaMemcpyDeviceToHost, h->st));
-    CUDA_TRY(cudaStreamSynchronize(h->st));
-    for (int a = 0; a < nl; ++a) { h->logdet[a] = res[2 * a]; h->yalpha[a] = res[2 * a + 1]; }
-    factor_caches_stale(h); h->factorized = true;
+    h->factorized = true;
     return GPMPC_OK;
 }
 
@@ -723,22 +743,29 @@ static int launch_grad(gpmpc_handle_t h, const double* dHyp, const double* alpha
     return GPMPC_OK;
 }
 
+// K(theta) -> L, Li, alpha of local output al for an objective at theta (hyper row in dHypTmp) with the jitter retry of
+// optimize.py:345-350.  The output's factor slabs are the scratch: the model needs gpmpc_factorize afterwards.
+static int factor_at_theta(gpmpc_handle_t h, const char* fn, int al, const double* theta)
+{
+    factor_stale(h);
+    CUDA_TRY(cudaMemcpyAsync(h->dHypTmp, theta, (h->Nx + 2) * 8, cudaMemcpyHostToDevice, h->st));
+    int used = 0;
+    const int rc = factor_one(h, al, h->dHypTmp, 1e-8, &used);
+    if (rc) { if (rc == GPMPC_ERR_NOTPD) set_error(h, "%s: K not positive definite even with jitter", fn); return rc; }
+    return launch_alpha(h, al, 1);
+}
+
 extern "C" int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* nll, double* grad)
 {
     if (!h || !theta || !nll) return GPMPC_ERR_ARG;
-    if (!h->has_data) { set_error(h, "gpmpc_nlml: set_data first"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
+    int rc = model_guard(h, __func__, NEED_DATA);
+    if (rc) return rc;
     const int al = local_index(h, a);
     if (al < 0) return GPMPC_ERR_ARG;
     const int m = h->Nx + 2;
     for (int d = 0; d < h->Nx; ++d) if (theta[d] == 0.0) { set_error(h, "gpmpc_nlml: zero length scale"); return GPMPC_ERR_ARG; }
-    factor_stale(h);
     NvtxRange nvtx_r("gpmpc.nlml");
-    CUDA_TRY(cudaMemcpyAsync(h->dHypTmp, theta, m * 8, cudaMemcpyHostToDevice, h->st));
-    int used = 0;
-    int rc = factor_one(h, al, h->dHypTmp, 1e-8, &used);     // optimize.py:345-350
-    if (rc) { if (rc == GPMPC_ERR_NOTPD) set_error(h, "gpmpc_nlml: K not positive definite even with jitter"); return rc; }
-    rc = launch_alpha(h, al, 1);
+    rc = factor_at_theta(h, __func__, al, theta);
     if (rc) return rc;
     double res[2];
     CUDA_TRY(cudaMemcpyAsync(res, h->dRes + 2 * al, 16, cudaMemcpyDeviceToHost, h->st));
@@ -792,14 +819,13 @@ static int loo_launch(gpmpc_handle_t h, int al, int batch, const LooLayout& o, b
 
 extern "C" int gpmpc_loo(gpmpc_handle_t h, double* mean, double* var, double* nlpp)
 {
-    if (!h) return GPMPC_ERR_ARG;
-    if (!h->factorized) { set_error(h, "gpmpc_loo: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
+    int rc = model_guard(h, __func__, NEED_FACTOR);
+    if (rc) return rc;
     if (h->N < 2) { set_error(h, "gpmpc_loo: needs N >= 2 training points (N = %d)", h->N); return GPMPC_ERR_ARG; }
-    CUDA_TRY(cudaSetDevice(h->device));
     NvtxRange nvtx_r("gpmpc.loo");
     const int nl = h->nloc;
     LooLayout o;
-    int rc = loo_layout(h, nl, &o);
+    rc = loo_layout(h, nl, &o);
     if (rc) return rc;
     rc = loo_launch(h, 0, nl, o, false);
     if (rc) return rc;
@@ -814,20 +840,15 @@ extern "C" int gpmpc_loo(gpmpc_handle_t h, double* mean, double* var, double* nl
 extern "C" int gpmpc_loo_nlpp(gpmpc_handle_t h, int a, const double* theta, double* nlpp, double* grad)
 {
     if (!h || !theta || !nlpp) return GPMPC_ERR_ARG;
-    if (!h->has_data) { set_error(h, "gpmpc_loo_nlpp: set_data first"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
+    int rc = model_guard(h, __func__, NEED_DATA);
+    if (rc) return rc;
     const int al = local_index(h, a);
     if (al < 0) return GPMPC_ERR_ARG;
     const int m = h->Nx + 2, N = h->N, np = h->Npad;
     for (int d = 0; d < h->Nx; ++d) if (theta[d] == 0.0) { set_error(h, "gpmpc_loo_nlpp: zero length scale"); return GPMPC_ERR_ARG; }
     if (N < 2) { set_error(h, "gpmpc_loo_nlpp: needs N >= 2 training points (N = %d)", N); return GPMPC_ERR_ARG; }
-    factor_stale(h);
     NvtxRange nvtx_r("gpmpc.loo_nlpp");
-    CUDA_TRY(cudaMemcpyAsync(h->dHypTmp, theta, m * 8, cudaMemcpyHostToDevice, h->st));
-    int used = 0;
-    int rc = factor_one(h, al, h->dHypTmp, 1e-8, &used);      // the jitter retry of gpmpc_nlml
-    if (rc) { if (rc == GPMPC_ERR_NOTPD) set_error(h, "gpmpc_loo_nlpp: K not positive definite even with jitter"); return rc; }
-    rc = launch_alpha(h, al, 1);
+    rc = factor_at_theta(h, __func__, al, theta);
     if (rc) return rc;
     LooLayout o;
     rc = loo_layout(h, 1, &o);
@@ -876,16 +897,15 @@ extern "C" int gpmpc_get(gpmpc_handle_t h, int what, int a, double* dst)
     const int al = local_index(h, a);
     if (al < 0) return GPMPC_ERR_ARG;
     if (what == GPMPC_GET_K) return gpmpc_build_K(h, a, dst);
-    if (what == GPMPC_GET_ALPHA_NLML) {       // alpha of the last gpmpc_nlml(a, theta) evaluation
-        CUDA_TRY(cudaMemcpyAsync(dst, h->dAlpha + (long long)al * h->Npad, h->N * 8, cudaMemcpyDeviceToHost, h->st));
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-        return GPMPC_OK;
+    if (what != GPMPC_GET_ALPHA_NLML) {       // that one: alpha of the last gpmpc_nlml(a, theta) evaluation
+        const int rc = model_guard(h, __func__, NEED_FACTOR);
+        if (rc) return rc;
     }
-    if (!h->factorized) { set_error(h, "gpmpc_get: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
     switch (what) {
     case GPMPC_GET_CHOL: return extract_to_host(h, h->dL + (long long)al * slab(h), dst, 1);
     case GPMPC_GET_LINV: return extract_to_host(h, h->dLi + (long long)al * slab(h), dst, 1);
     case GPMPC_GET_ALPHA:
+    case GPMPC_GET_ALPHA_NLML:
         CUDA_TRY(cudaMemcpyAsync(dst, h->dAlpha + (long long)al * h->Npad, h->N * 8, cudaMemcpyDeviceToHost, h->st));
         CUDA_TRY(cudaStreamSynchronize(h->st));
         return GPMPC_OK;
@@ -1591,18 +1611,17 @@ static int peer_status_check(gpmpc_handle_t h)
 // First check of every predict-family entry `fn` (the name its errors carry): a factorised model, H >= 1 and a known method.
 static int predict_guard(gpmpc_handle_t h, const char* fn, int method, int H)
 {
-    if (!h) return GPMPC_ERR_ARG;
-    if (!h->factorized) { set_error(h, "%s: call gpmpc_factorize first", fn); return GPMPC_ERR_STATE; }
+    const int rc = model_guard(h, fn, NEED_FACTOR);
+    if (rc) return rc;
     if (H < 1) { set_error(h, "%s: H < 1", fn); return GPMPC_ERR_ARG; }
     if (method != GPMPC_METHOD_ME && method != GPMPC_METHOD_TA && method != GPMPC_METHOD_EM) { set_error(h, "%s: unknown method %d", fn, method); return GPMPC_ERR_ARG; }
     return GPMPC_OK;
 }
 
-// after an entry's own argument checks: every output on this handle and one rank if all_outputs, then device and buffers
+// after the guard (device selected) and the entry's own checks: all outputs on one handle and rank if all_outputs; buffers
 static int predict_prepare(gpmpc_handle_t h, const char* fn, int H, bool all_outputs)
 {
     if (all_outputs && (h->nloc != h->Ny || h->world != 1)) { set_error(h, "%s needs all outputs on one handle (replicate the model, shard the points)", fn); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
     return ensure_predict_bufs(h, H);
 }
 
@@ -2013,55 +2032,68 @@ extern "C" int gpmpc_predict_em_grad(gpmpc_handle_t h, int H, const double* Z, c
     return predict_em(h, H, Z, Sigma, spp, mean, var, cov, any ? &go : nullptr);
 }
 
+// Row Nk of L and L^-1 of every owned output from l = L^-1 k (rows < Nk of dV): r = Li^T l over the Nk rows l occupies,
+// then append_row_kernel.  stop (may be null): a greedy step after a failed pivot writes nothing.
+static int append_rows(gpmpc_handle_t h, int Nk, const int* stop)
+{
+    const int np = h->Npad, Nx = h->Nx, nl = h->nloc;
+    const long long sl = (long long)HB * np;
+    trmv_lower_T_kernel<<<dim3((Nk + 31) / 32, 1, nl), 256, 0, h->st>>>(h->dLi, np, slab(h), h->dV, sl, h->dR, sl, Nk);
+    CUDA_TRY(cudaGetLastError());
+    append_row_kernel<<<nl, 256, 0, h->st>>>(h->dL, h->dLi, np, slab(h), h->dV, h->dR, sl, h->dHyp, Nx + 2, Nx, Nk, h->dInfo,
+                                             stop);
+    CUDA_TRY(cudaGetLastError());
+    return GPMPC_OK;
+}
+
+// End of n_new appends to N0 points (syncs): a failed pivot of step k reads N0 + k + 1 in dInfo.  N counts the points up to
+// and including the first failing step (*added); after a failure the caller must refactorise, else alpha is refreshed.
+static int finish_appends(gpmpc_handle_t h, const char* fn, int N0, int n_new, int* added)
+{
+    const int nl = h->nloc;
+    std::vector<int> inf(nl, 0);
+    CUDA_TRY(cudaMemcpyAsync(inf.data(), h->dInfo, nl * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    int fail = n_new, bad = -1;
+    for (int a = 0; a < nl; ++a)
+        if (inf[a] && inf[a] - N0 - 1 < fail) { fail = inf[a] - N0 - 1; bad = a; }
+    *added = (bad >= 0) ? fail + 1 : n_new;
+    h->N = N0 + *added;
+    if (bad >= 0) {
+        factor_stale(h);
+        set_error(h, "%s: output %d lost positive definiteness at pick %d (refactorise, jitter applies there)", fn,
+                  h->a0 + bad, *added - 1);
+        return GPMPC_ERR_NOTPD;
+    }
+    return refresh_alpha(h);
+}
+
 extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double* y_new)
 {
     if (!h || !x_new || !y_new) return GPMPC_ERR_ARG;
-    if (!h->factorized) { set_error(h, "gpmpc_append: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
+    int rc = model_guard(h, __func__, NEED_FACTOR);
+    if (rc) return rc;
     if (h->N >= h->Npad) { set_error(h, "gpmpc_append: capacity %d reached, refit on a new handle", h->Npad); return GPMPC_ERR_STATE; }
-    int rc = predict_prepare(h, __func__, 1, false);
+    rc = predict_prepare(h, __func__, 1, false);
     if (rc) return rc;
     const int N = h->N, Nx = h->Nx, np = h->Npad, nl = h->nloc;
     // k(X, x_new) for every owned output through the predict ks kernel (H = 1): row 0 of KS^T
     CUDA_TRY(cudaMemcpyAsync(h->dZ, x_new, Nx * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(launch_ks(h, h->dZ, 1));
-    // l = Li k (rows < N), r = Li^T l
+    // l = Li k (rows < N)
     rc = ensure_rows(h);
     if (rc) return rc;
     dim3 g1((np + 7) / 8, 1, nl);
     trmv_lower_kernel<<<g1, 256, 0, h->st>>>(h->dLi, np, slab(h), h->dKST, (long long)HB * np, h->dV, (long long)HB * np, N);
     CUDA_TRY(cudaGetLastError());
-    // rows >= N of l must be zero for the transposed product over the padded matrix
-    for (int a = 0; a < nl; ++a)
-        CUDA_TRY(cudaMemsetAsync(h->dV + (long long)a * HB * np + N, 0, (size_t)(np - N) * 8, h->st));
-    dim3 g2(np / 32, 1, nl);
-    trmv_lower_T_kernel<<<g2, 256, 0, h->st>>>(h->dLi, np, slab(h), h->dV, (long long)HB * np, h->dR, (long long)HB * np, np);
-    CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemsetAsync(h->dInfo, 0, nl * sizeof(int), h->st));
-    append_row_kernel<<<nl, 256, 0, h->st>>>(h->dL, h->dLi, np, slab(h), h->dV, h->dR, (long long)HB * np, h->dHyp, Nx + 2, Nx, N,
-                                             h->dInfo, nullptr);
-    CUDA_TRY(cudaGetLastError());
-    std::vector<int> inf(nl, 0);
-    CUDA_TRY(cudaMemcpyAsync(inf.data(), h->dInfo, nl * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    rc = append_rows(h, N, nullptr);
+    if (rc) return rc;
     // the new point joins X^T (column N) and Y
     for (int d = 0; d < Nx; ++d) CUDA_TRY(cudaMemcpyAsync(h->dXT + (long long)d * np + N, x_new + d, 8, cudaMemcpyHostToDevice, h->st));
     for (int a = 0; a < nl; ++a) CUDA_TRY(cudaMemcpyAsync(h->dY + (long long)a * np + N, y_new + h->a0 + a, 8, cudaMemcpyHostToDevice, h->st));
-    CUDA_TRY(cudaStreamSynchronize(h->st));
-    for (int a = 0; a < nl; ++a)
-        if (inf[a]) {
-            factor_stale(h);             // row N of that output is unusable: the caller must refactorise
-            set_error(h, "gpmpc_append: output %d lost positive definiteness (refactorise, jitter applies there)", h->a0 + a);
-            h->N = N + 1;
-            return GPMPC_ERR_NOTPD;
-        }
-    h->N = N + 1;
-    factor_caches_stale(h);
-    rc = launch_alpha(h, 0, nl);
-    if (rc) return rc;
-    std::vector<double> res(2 * nl);
-    CUDA_TRY(cudaMemcpyAsync(res.data(), h->dRes, 2 * nl * 8, cudaMemcpyDeviceToHost, h->st));
-    CUDA_TRY(cudaStreamSynchronize(h->st));
-    for (int a = 0; a < nl; ++a) { h->logdet[a] = res[2 * a]; h->yalpha[a] = res[2 * a + 1]; }
-    return GPMPC_OK;
+    int added = 0;
+    return finish_appends(h, __func__, N, 1, &added);
 }
 
 // The solved rows v = L^-1 k(X, z) of the H points at dZ (device, (H, Nx)) for every owned output into dst: row h of
@@ -2093,8 +2125,9 @@ static int solve_rows(gpmpc_handle_t h, const double* dZ, int H, double* dst, lo
 extern "C" int gpmpc_posterior_cov(gpmpc_handle_t h, int H, const double* Z, double* out)
 {
     if (!h || !Z || !out || H < 1) return GPMPC_ERR_ARG;
-    if (!h->factorized) { set_error(h, "gpmpc_posterior_cov: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
-    int rc = predict_prepare(h, __func__, H, false);
+    int rc = model_guard(h, __func__, NEED_FACTOR);
+    if (rc) return rc;
+    rc = predict_prepare(h, __func__, H, false);
     if (rc) return rc;
     const int np = h->Npad, Nx = h->Nx, nl = h->nloc;
     const long long sVall = (long long)H * np;
@@ -2194,8 +2227,9 @@ extern "C" int gpmpc_append_greedy(gpmpc_handle_t h, int n, const double* Xc, co
     if (!Xc || !Yc || !picked || !n_added) { set_error(h, "gpmpc_append_greedy: null Xc / Yc / picked / n_added"); return GPMPC_ERR_ARG; }
     *n_added = 0;
     if (n < 1 || n_new < 0 || n_new > n) { set_error(h, "gpmpc_append_greedy: need n >= 1 and 0 <= n_new <= n (n = %d, n_new = %d)", n, n_new); return GPMPC_ERR_ARG; }
-    if (!h->factorized) { set_error(h, "gpmpc_append_greedy: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
-    int rc = predict_prepare(h, __func__, 1, true);
+    int rc = model_guard(h, __func__, NEED_FACTOR);
+    if (rc) return rc;
+    rc = predict_prepare(h, __func__, 1, true);
     if (rc) return rc;
     if (h->N + n_new > h->Npad) {
         set_error(h, "gpmpc_append_greedy: N + n_new = %d exceeds the capacity %d (reserve it with gpmpc_create_reserve)", h->N + n_new, h->Npad);
@@ -2235,48 +2269,22 @@ extern "C" int gpmpc_append_greedy(gpmpc_handle_t h, int n, const double* Xc, co
         CUDA_TRY(cudaGetLastError());
         greedy_gather_kernel<<<dim3((np + 255) / 256, nl), 256, 0, h->st>>>(h->dCovV, np, sV, dPick, k, Nk, h->dV, sl, np, dStop);
         CUDA_TRY(cudaGetLastError());
-        // r = Li^T l over the Nk rows l occupies (scratch: after a failed pivot it is computed and never read)
-        trmv_lower_T_kernel<<<dim3((Nk + 31) / 32, 1, nl), 256, 0, h->st>>>(h->dLi, np, slab(h), h->dV, sl, h->dR, sl, Nk);
-        CUDA_TRY(cudaGetLastError());
-        append_row_kernel<<<nl, 256, 0, h->st>>>(h->dL, h->dLi, np, slab(h), h->dV, h->dR, sl, h->dHyp, Nx + 2, Nx, Nk,
-                                                 h->dInfo, dStop);
-        CUDA_TRY(cudaGetLastError());
+        rc = append_rows(h, Nk, dStop);     // after a failed pivot r is computed and never read
+        if (rc) return rc;
         greedy_downdate_kernel<<<gw, 256, 0, h->st>>>(h->dCovV, np, sV, dVar, n, dAct, h->dV, sl, h->dL, np, slab(h), dXc, Nx,
                                                      h->dHyp, Nx + 2, dPick, k, Nk, h->dInfo, nl);
         CUDA_TRY(cudaGetLastError());
     }
-    std::vector<int> inf(nl, 0), pk(n_new, 0);
+    std::vector<int> pk(n_new, 0);
     std::vector<double> sc(n_new, 0.0);
-    CUDA_TRY(cudaMemcpyAsync(inf.data(), h->dInfo, nl * sizeof(int), cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaMemcpyAsync(pk.data(), dPick, n_new * sizeof(int), cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaMemcpyAsync(sc.data(), dScore, n_new * 8, cudaMemcpyDeviceToHost, h->st));
-    CUDA_TRY(cudaStreamSynchronize(h->st));
-    // append_row_kernel records a failed pivot of step k as Nk + 1 = N + k + 1; later steps did nothing.  The first
-    // failing step (the smallest k over the outputs) and the points appended up to and including it:
-    int fail = n_new, bad = -1;
-    for (int a = 0; a < nl; ++a)
-        if (inf[a] && inf[a] - N - 1 < fail) { fail = inf[a] - N - 1; bad = a; }
-    const int added = (bad >= 0) ? fail + 1 : n_new;
-    for (int k = 0; k < added; ++k) {
+    rc = finish_appends(h, __func__, N, n_new, n_added);
+    for (int k = 0; k < *n_added; ++k) {
         picked[k] = pk[k];
         if (score) score[k] = sc[k];
     }
-    *n_added = added;
-    h->N = N + added;
-    if (bad >= 0) {
-        factor_stale(h);                 // row N + added - 1 of that output is unusable: the caller must refactorise
-        set_error(h, "gpmpc_append_greedy: output %d lost positive definiteness at pick %d (refactorise, jitter applies there)",
-                  h->a0 + bad, added - 1);
-        return GPMPC_ERR_NOTPD;
-    }
-    factor_caches_stale(h);
-    rc = launch_alpha(h, 0, nl);
-    if (rc) return rc;
-    std::vector<double> res(2 * nl);
-    CUDA_TRY(cudaMemcpyAsync(res.data(), h->dRes, 2 * nl * 8, cudaMemcpyDeviceToHost, h->st));
-    CUDA_TRY(cudaStreamSynchronize(h->st));
-    for (int a = 0; a < nl; ++a) { h->logdet[a] = res[2 * a]; h->yalpha[a] = res[2 * a + 1]; }
-    return GPMPC_OK;
+    return rc;
 }
 
 // Removal of training points by rank-1 updates of the trailing blocks of L and L^-1 (kernels.cuh, remove_*), one point
@@ -2285,8 +2293,8 @@ extern "C" int gpmpc_append_greedy(gpmpc_handle_t h, int n, const double* Xc, co
 // the point leaves X^T and Y.  alpha and logdet are refreshed once, at the end.
 extern "C" int gpmpc_remove(gpmpc_handle_t h, int n, const int* idx)
 {
-    if (!h) return GPMPC_ERR_ARG;
-    if (!h->factorized) { set_error(h, "gpmpc_remove: call gpmpc_factorize first"); return GPMPC_ERR_STATE; }
+    int rc = model_guard(h, __func__, NEED_FACTOR);
+    if (rc) return rc;
     if (n < 0 || (n > 0 && !idx)) { set_error(h, "gpmpc_remove: need n >= 0 and idx non-null for n > 0 (n = %d)", n); return GPMPC_ERR_ARG; }
     if (n == 0) return GPMPC_OK;
     const int N = h->N, Nx = h->Nx, np = h->Npad, nl = h->nloc;
@@ -2296,8 +2304,7 @@ extern "C" int gpmpc_remove(gpmpc_handle_t h, int n, const int* idx)
     if (order[0] >= N || order[n - 1] < 0) { set_error(h, "gpmpc_remove: index out of range [0, %d)", N); return GPMPC_ERR_ARG; }
     for (int k = 1; k < n; ++k)
         if (order[k] == order[k - 1]) { set_error(h, "gpmpc_remove: index %d given twice", order[k]); return GPMPC_ERR_ARG; }
-    CUDA_TRY(cudaSetDevice(h->device));
-    int rc = ensure_nlml_scratch(h);           // dU / dKinv: the work slabs of the new rows
+    rc = ensure_nlml_scratch(h);          // dU / dKinv: the work slabs of the new rows
     if (rc) return rc;
     ENSURE(h->dRm, (long long)nl * 3 * np);
     NvtxRange nvtx_r("gpmpc.remove");
@@ -2330,14 +2337,7 @@ extern "C" int gpmpc_remove(gpmpc_handle_t h, int n, const int* idx)
         CUDA_TRY(cudaGetLastError());
     }
     h->N = N - n;
-    factor_caches_stale(h);
-    rc = launch_alpha(h, 0, nl);
-    if (rc) return rc;
-    std::vector<double> res(2 * nl);
-    CUDA_TRY(cudaMemcpyAsync(res.data(), h->dRes, 2 * nl * 8, cudaMemcpyDeviceToHost, h->st));
-    CUDA_TRY(cudaStreamSynchronize(h->st));
-    for (int a = 0; a < nl; ++a) { h->logdet[a] = res[2 * a]; h->yalpha[a] = res[2 * a + 1]; }
-    return GPMPC_OK;
+    return refresh_alpha(h);
 }
 
 // ------------------------------------------------------------------------------------
@@ -2510,12 +2510,11 @@ extern "C" int gpmpc_profile_tail(gpmpc_handle_t h, int H, double* out8)
 extern "C" int gpmpc_profile_leaf(gpmpc_handle_t h, double* out15)
 {
     if (!h || !out15) return GPMPC_ERR_ARG;
-    if (!h->has_data || !h->has_hyper) { set_error(h, "gpmpc_profile_leaf: set_data and set_hyper first"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
+    int rc = model_guard(h, __func__, NEED_HYPER);
+    if (rc) return rc;
     DevBuf<long long> d;
     ENSURE(d, 16);
     CUDA_TRY(cudaMemcpyToSymbol(d_leaf_prof, &d.p, sizeof(d.p)));
-    int rc = GPMPC_OK;
     for (int rep = 0; rep < 2 && rc == GPMPC_OK; ++rep) {           // second run: warm instruction cache
         rc = launch_kbuild(h, h->dHyp, h->dJit, h->dL, 1, 0);
         if (rc == GPMPC_OK) rc = potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, 128, 1);
@@ -2536,11 +2535,10 @@ extern "C" int gpmpc_profile_leaf(gpmpc_handle_t h, double* out15)
 extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double* ms_out)
 {
     if (!h || !ms_out || reps < 1) return GPMPC_ERR_ARG;
-    if (!h->has_data || !h->has_hyper) { set_error(h, "gpmpc_profile: set_data and set_hyper first"); return GPMPC_ERR_STATE; }
-    CUDA_TRY(cudaSetDevice(h->device));
+    int rc = model_guard(h, __func__, NEED_HYPER);
+    if (rc) return rc;
     const int np = h->Npad, Hc = (n > 0 && n <= HB) ? n : 56;       // Hc: test points of the product selectors
     float ms = 0.f;
-    int rc = GPMPC_OK;
     auto run = [&]() -> int {
         switch (what) {
         case GPMPC_PROF_KBUILD_FULL: return launch_kbuild(h, h->dHyp, h->dJit, h->dL, 1, 1);

@@ -132,8 +132,7 @@ class GP:
             # is not part of the saved model.
             self.__hyper = np.array(hyper['hyper'], dtype=np.float64)
             self.__set_hyper_views()
-            self.__build_engine()
-            self.__factorize()
+            self.__refit()
 
         self.set_method(gp_method)
 
@@ -188,11 +187,18 @@ class GP:
     def __has_prior_mean(self):
         return self.__mean_func != 'zero' and self.__hyper.shape[1] > self.__Nx + 2
 
+    def __engine_targets(self, X, Y):
+        """The targets the engine factorises: the residual Y - m(X) under a prior mean (alpha = K^-1 (y - m(X)),
+        optimize.py:492-494), else Y."""
+        if not self.__has_prior_mean():
+            return Y
+        return Y - np.column_stack([mean_function(self.__hyper[a], X, self.__mean_func) for a in range(self.__Ny)])
+
     def __factorize(self):
         if self.__has_prior_mean():
-            # alpha = K^-1 (y - m(X))  (optimize.py:492-494): the engine factorises on the residual
+            T = self.__engine_targets(self.__X, self.__Y)
             for a in self.__engine.local_outputs:
-                self.__engine.set_y(a, self.__Y[:, a] - mean_function(self.__hyper[a], self.__X, self.__mean_func))
+                self.__engine.set_y(a, T[:, a])
         self.__engine.set_hyper(self.__hyper)
         info = self.__engine.factorize(1e-8)
         for k, a in enumerate(self.__engine.local_outputs):
@@ -203,6 +209,15 @@ class GP:
         # line them up again before the first predict step's peer exchange starts its timeout clock
         if self.__comm.world > 1:
             self.__comm.barrier()
+
+    def __refit(self, capacity=None):
+        """A new engine on the current X, Y, factorised at the current hyper-parameters."""
+        self.__build_engine(capacity)
+        self.__factorize()
+
+    def __set_data(self, X, Y):
+        self.__X, self.__Y, self.__N = X, Y, X.shape[0]
+        self.__invK = None
 
     @property
     def engine(self):
@@ -830,11 +845,8 @@ class GP:
         print('\n________________________________________')
         print('# Updating training data with ' + str(X_new.shape[0]) + ' new samples')
         print('----------------------------------------')
-        self.__X = np.vstack([self.__X, X_new])
-        self.__Y = np.vstack([self.__Y, Y_new])
-        self.__N = self.__X.shape[0]
-        self.__build_engine()
-        self.__factorize()
+        self.__set_data(np.vstack([self.__X, X_new]), np.vstack([self.__Y, Y_new]))
+        self.__refit()
         self.set_method(self.__gp_method)
 
     def remove_data(self, indices):
@@ -855,10 +867,7 @@ class GP:
         if idx.size == 0:
             return
         self.__engine.remove(idx)
-        self.__X = np.delete(self.__X, idx, axis=0)
-        self.__Y = np.delete(self.__Y, idx, axis=0)
-        self.__N = self.__X.shape[0]
-        self.__invK = None
+        self.__set_data(np.delete(self.__X, idx, axis=0), np.delete(self.__Y, idx, axis=0))
 
     def append_data(self, X_new, Y_new, max_points=None):
         """ Add observations one at a time with the O(N^2) rank-1 update of L, L^-1 and alpha
@@ -880,27 +889,23 @@ class GP:
         if self.__normalize:
             Ys = self.standardize(Y_new, self.__meanY, self.__stdY)
             Xs = self.standardize(X_new, self.__meanZ, self.__stdZ)
+        Ts = self.__engine_targets(Xs, Ys)
         for k in range(Xs.shape[0]):
             if max_points is not None and self.__N + 1 > max_points:
                 self.remove_data(np.arange(self.__N + 1 - max_points))
-            ok = self.__engine.append(Xs[k], Ys[k])
+            ok = self.__engine.append(Xs[k], Ts[k])
             if self.__comm.world > 1:
                 # the fallback below runs collectives (engine rebuild): the decision must be collective
                 # too -- a rank that alone lost positive definiteness would otherwise hang the others
                 ok = all(self.__comm.allgather_object(bool(ok)))
             if not ok:
-                self.__X = np.vstack([self.__X, Xs[k:]])
-                self.__Y = np.vstack([self.__Y, Ys[k:]])
+                X, Y = np.vstack([self.__X, Xs[k:]]), np.vstack([self.__Y, Ys[k:]])
                 if max_points is not None:           # the window: the newest max_points
-                    self.__X, self.__Y = self.__X[-max_points:], self.__Y[-max_points:]
-                self.__N = self.__X.shape[0]
-                self.__build_engine()
-                self.__factorize()
+                    X, Y = X[-max_points:], Y[-max_points:]
+                self.__set_data(X, Y)
+                self.__refit()
                 return
-            self.__X = np.vstack([self.__X, Xs[k:k + 1]])
-            self.__Y = np.vstack([self.__Y, Ys[k:k + 1]])
-            self.__N = self.__X.shape[0]
-        self.__invK = None
+            self.__set_data(np.vstack([self.__X, Xs[k:k + 1]]), np.vstack([self.__Y, Ys[k:k + 1]]))
 
     def replace_data_all(self, X_new, Y_new):
         """ Replace training data with new observations  (reference gp_class.py:553-626) """
@@ -912,11 +917,8 @@ class GP:
         print('\n________________________________________')
         print('# Replacing training data with ' + str(X_new.shape[0]) + ' new samples')
         print('----------------------------------------')
-        self.__X = X_new
-        self.__Y = Y_new
-        self.__N = self.__X.shape[0]
-        self.__build_engine()
-        self.__factorize()
+        self.__set_data(X_new, Y_new)
+        self.__refit()
         self.set_method(self.__gp_method)
 
     def update_data(self, X_new, Y_new, N_new=None):
@@ -954,20 +956,16 @@ class GP:
         on_device = (device_select and hasattr(eng, 'append_greedy') and not self.__sharded_outputs()
                      and eng.out_count == self.__Ny)
         picked = self.__greedy_device(Xs, Ys, N_new) if on_device else self.__greedy_host(X_new, Y_new, Xs, N_new)
-        self.__invK = None
         return np.asarray(picked, dtype=np.int64)
 
     def __greedy_device(self, Xs, Ys, N_new):
-        Yr = Ys
-        if self.__has_prior_mean():                  # the engine factorises on y - m(x), as __factorize does
-            Yr = Ys - np.column_stack([mean_function(self.__hyper[a], Xs, self.__mean_func) for a in range(self.__Ny)])
+        Yr = self.__engine_targets(Xs, Ys)
         remaining = np.arange(Xs.shape[0])
         picked = []
         while len(picked) < N_new:
             need = N_new - len(picked)
             if self.__engine.capacity - self.__engine.N < need:
-                self.__build_engine(capacity=self.__N + need)
-                self.__factorize()
+                self.__refit(capacity=self.__N + need)
             idx, _, ok = self.__engine.append_greedy(Xs[remaining], Yr[remaining], need)
             if self.__comm.world > 1:
                 # replicated engines ('points' mode): the kept picks and the refit decision are collective, so a rank
@@ -979,16 +977,13 @@ class GP:
                 if not all(r[1] and len(r[0]) == k for r in res):
                     idx, ok = idx[:k], False          # every rank keeps the common picks and refits on them
             sel = remaining[idx]
-            self.__X = np.vstack([self.__X, Xs[sel]])
-            self.__Y = np.vstack([self.__Y, Ys[sel]])
-            self.__N = self.__X.shape[0]
+            self.__set_data(np.vstack([self.__X, Xs[sel]]), np.vstack([self.__Y, Ys[sel]]))
             picked.extend(sel.tolist())
             remaining = np.delete(remaining, idx)
             if not ok:
                 # positive definiteness lost at the last pick (it is in X): refactorise, the jitter policy applies there
                 need = N_new - len(picked)
-                self.__build_engine(capacity=self.__N + need if need else None)
-                self.__factorize()
+                self.__refit(capacity=self.__N + need if need else None)
         return picked
 
     def __greedy_host(self, X_new, Y_new, Xs, N_new):

@@ -143,8 +143,9 @@ int gpmpc_predict(gpmpc_handle_t h, int method, int H, const double* Z, const do
 /* Append ONE training point (x_new:(Nx,), y_new:(Ny,) host, GP input space) to a factorised
  * model in O(N^2): new rows of L and L^-1, alpha refreshed.  Capacity is the padded size
  * ceil(N/128)*128, or the one reserved by gpmpc_create_reserve (GPMPC_ERR_STATE beyond it: refit on
- * a new handle).  GPMPC_ERR_NOTPD if the Schur complement is not positive: refactorise (the jitter
- * policy applies there).  Appends every point given, in order; gpmpc_append_greedy chooses. */
+ * a new handle).  GPMPC_ERR_NOTPD if the Schur complement is not positive: the point is in the model
+ * (N counts it) and the handle needs gpmpc_factorize (the jitter policy applies there).  Appends every
+ * point given, in order; gpmpc_append_greedy chooses. */
 int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double* y_new);
 
 /* Greedy selection from a pool: n_new times, append the pool point with the largest sum over outputs of the

@@ -1,7 +1,7 @@
 """Small end-to-end pass over every kernel of the engine for compute-sanitizer
 (memcheck / racecheck / synccheck / initcheck):  K build, leaf + DMMA GEMMs (cp.async feeds; the TMA
 tensor-map feed on a second, 24-output handle), alpha, NLML + gradient, the persistent stream-K predict kernel with tile
-fix-ups (several grid sizes, lower and upper mode), gpmpc_predict_device, gpmpc_predict's copy transports, predict_grad, EM and its derivatives, rank-1 append, GP.covar, sampled roll-outs, leave-one-out cross-validation and its gradient.
+fix-ups (several grid sizes, lower and upper mode), gpmpc_predict_device, gpmpc_predict's copy transports, predict_grad, EM and its derivatives, rank-1 append, greedy append, removal, GP.covar, sampled roll-outs, leave-one-out cross-validation and its gradient.
     compute-sanitizer --tool racecheck python tools/sanitize_run.py"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -56,6 +56,9 @@ print('nlml', nll, orc.calc_NLL(p['hyper'][0] * 0.9, p['X'], p['Y'][:, 0], False
 eng.factorize()
 ok = eng.append(p['X'][0] + 0.3, p['Y'][0])
 print('append', ok, flush=True)
+picked, _, ok = eng.append_greedy(p['Z'][:8], np.zeros((8, Ny)), 3)
+eng.remove([0, 5])
+print('append_greedy', ok, picked.tolist(), 'remove', eng.N, flush=True)
 eng.close()
 # the TMA tensor-map GEMM serves products of at least 4 * SMs 128x64 tiles: Npad 1152 with 24 outputs puts the bottom
 # panel of the top-level split there (576 tiles)
