@@ -50,6 +50,7 @@ SYMBOLS = [
     ('gpmpc_posterior_cov', C.c_int, [_H, C.c_int, _dp, _dp]),
     ('gpmpc_rollout', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     ('gpmpc_rollout_batch', C.c_int, [_H, C.c_int, C.c_int, C.c_int] + [_dp] * 10),
+    ('gpmpc_rollout_batch_grad', C.c_int, [_H, C.c_int, C.c_int, C.c_int] + [_dp] * 12),
     ('gpmpc_rollout_sample', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 10 + [_ip]),
     ('gpmpc_predict_device', C.c_int, [_H, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
@@ -312,6 +313,30 @@ class Engine:
         self._check(self.lib.gpmpc_rollout_batch(self.h, int(method), B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale),
                                                  _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means), _ptr(var), _ptr(cov)))
         return means, var, cov
+
+    def rollout_batch_grad(self, z0, U, Sigma0, method=METHOD_TA, scale=None, K=None, x_ref=None, uscale=None):
+        """gpmpc_rollout_batch_grad: rollout_batch's arguments and outputs (bit for bit) plus dmeans, dvars (B,Nt,Ny,P), the
+        derivatives of every step's mean and variance (GP output units) w.r.t. P = Nx + (Nt-1) Nu parameters [z0[b] |
+        U[b,1:] row-major] open loop, or P = Nx + Nu Ny parameters [z0[b] | K row-major] with K."""
+        Nu = self.Nx - self.Ny
+        z0 = _f64(z0).reshape(-1, self.Nx)
+        B = z0.shape[0]
+        Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
+        Nt = int(np.shape(U)[1])
+        U = _f64(U, (B, Nt, Nu)) if (Nu > 0 and K is None) else None
+        if scale is not None:
+            scale = _f64(scale, (4, self.Ny))
+        if K is not None:
+            K = _f64(K, (Nu, self.Ny))
+            x_ref = None if x_ref is None else _f64(x_ref, (self.Ny,))
+            uscale = None if uscale is None else _f64(uscale, (2, Nu))
+        P = self.Nx + (Nu * self.Ny if K is not None else (Nt - 1) * Nu)
+        means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
+        dmeans = np.empty((B, Nt, self.Ny, P)); dvars = np.empty((B, Nt, self.Ny, P))
+        self._check(self.lib.gpmpc_rollout_batch_grad(self.h, int(method), B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0),
+                                                      _ptr(scale), _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means),
+                                                      _ptr(var), _ptr(cov), _ptr(dmeans), _ptr(dvars)))
+        return means, var, cov, dmeans, dvars
 
     def rollout_sample(self, z0, U, eps, xi=None, scale=None, K=None, x_ref=None, uscale=None):
         """gpmpc_rollout_sample: B trajectories of Nt steps, each one consistent draw of the GP posterior along the inputs

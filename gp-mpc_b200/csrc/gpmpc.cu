@@ -107,6 +107,7 @@ struct gpmpc_handle_s {
     DevBuf<double> dG;
     double *dZ = nullptr, *dSigma = nullptr, *dMean = nullptr, *dVar = nullptr, *dJ = nullptr, *dCov = nullptr;   // in dIn / dOut
     DevBuf<double> dRoll;             // gpmpc_rollout_batch: [Z | Sigma | U | scale | K | x_ref | uscale | means | vars | cov]
+    DevBuf<double> dRollTg;           // gpmpc_rollout_batch_grad: [dZ | dSigma ('TA') | dmeans | dvars]
     DevBuf<double> dSmV;              // gpmpc_rollout_sample: V rows of every step (nloc, Nt, B, Npad)
     DevBuf<double> dSmp;              //   [eps | xi | U | scale | K | x_ref | uscale | Z (Nt,B,Nx) | samples | kept | m | R]
     DevBuf<double> dIn, dOut;         // [Z | Sigma] and [mean | var | J | cov] slabs: one H2D + one D2H per host call
@@ -1715,10 +1716,172 @@ rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restr
     }
 }
 
-// gpmpc_rollout_batch and gpmpc_rollout; fn names the entry in errors
+// Forward-mode tangents of one roll-out step, one CTA per trajectory b (gpmpc_rollout_batch_grad).  The P parameters of a
+// trajectory are [z0 (Nx) | U rows 1 .. Nt-1 (Nu each)] open loop or [z0 | K row-major (Nu x Ny)] with feedback; the
+// tangents are dZ (B, P, Nx) and, for 'TA', dS (B, P, Nx, Nx), each parameter's column contiguous.  Step t reads J_t, dcov_t
+// ('TA') or dvar_t ('ME') of the derivative chain and writes, per parameter p,
+//   dm = J dz,   dC = sum_e dcov[.,.,e] dz_e + J dS J^T ('TA')  or  diag(dvar dz) ('ME'),   dmeans_t = dm, dvars_t = diag(dC)
+// and unless last the next tangents, the derivatives of what rollout_feedback_kernel forms:
+//   dz[:Ny] = dm * stdY / stdX (dm without scale);  open loop: dz[Ny+i] = [p is U[t+1][i]], dS x block = dC, u blocks kept;
+//   feedback, x~ = x - x_ref, dx = dm * stdY:  du = (K dx + dK x~) / stdU,  dS_xu = dC K^T + C dK^T,
+//   dS_uu = dK C K^T + K dC K^T + K C dK^T  (dK = the unit matrix of p when p is an entry of K, else 0).
+// At t = 0 the tangents are the unit columns of z0 and zero covariance (nothing is read).  Each warp owns one column at a
+// time and rewrites it in place; every sum runs in index order in one thread, so a trajectory's bits do not depend on B.
+// Dynamic shared memory: J (Ny Nx) | x~ (Ny) | C K^T (Ny Nu) | K C (Nu Ny) | per warp [dz (Nx) | dm (Ny) | dC (Ny Ny) | T (Ny Nx)].
+__global__ void __launch_bounds__(256, 2)
+rollout_tangent_kernel(int Ny, int Nu, int P, int t, int first, int last, int method_ta,
+                       const double* __restrict__ J, const double* __restrict__ dvar, const double* __restrict__ dcov,
+                       const double* __restrict__ mean_t, const double* __restrict__ cov_t, const double* __restrict__ scale,
+                       const double* __restrict__ K, const double* __restrict__ x_ref, const double* __restrict__ uscale,
+                       double* __restrict__ dZ, double* __restrict__ dS, double* __restrict__ dmeans_t, double* __restrict__ dvars_t)
+{
+    extern __shared__ double tg_sh[];
+    const int Nx = Ny + Nu, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5, b = blockIdx.x;
+    const bool fb = K != nullptr;
+    double* sJ = tg_sh;
+    double* xt = sJ + Ny * Nx;
+    double* CKt = xt + Ny;
+    double* KC = CKt + Ny * Nu;
+    const int per_warp = Nx + Ny + Ny * Ny + Ny * Nx;
+    double* wz = KC + Nu * Ny + warp * per_warp;
+    double* wm = wz + Nx;
+    double* wC = wm + Ny;
+    double* wT = wC + Ny * Ny;
+    J += (size_t)b * Ny * Nx;
+    cov_t += (size_t)b * Ny * Ny;
+    for (int i = tid; i < Ny * Nx; i += blockDim.x) sJ[i] = J[i];
+    if (fb && !last) {
+        for (int k = tid; k < Ny; k += blockDim.x) {
+            const double m = mean_t[(size_t)b * Ny + k];
+            const double x = scale ? m * scale[k] + scale[Ny + k] : m;
+            xt[k] = x_ref ? x - x_ref[k] : x;
+        }
+        if (method_ta)
+            for (int idx = tid; idx < Ny * Nu; idx += blockDim.x) {
+                const int r = idx / Nu, i = idx - r * Nu;
+                double s1 = 0.0, s2 = 0.0;
+                for (int k = 0; k < Ny; ++k) {
+                    s1 = fma(cov_t[r * Ny + k], K[i * Ny + k], s1);      // (C K^T)[r][i]
+                    s2 = fma(K[i * Ny + k], cov_t[k * Ny + r], s2);      // (K C)[i][r]
+                }
+                CKt[idx] = s1; KC[i * Ny + r] = s2;
+            }
+    }
+    __syncthreads();
+    const double* dcv = dcov + (size_t)b * Ny * Ny * Nx;
+    const double* dvr = dvar + (size_t)b * Ny * Nx;
+    for (int p = warp; p < P; p += nwarps) {
+        double* z = dZ + ((size_t)b * P + p) * Nx;
+        double* S = method_ta ? dS + ((size_t)b * P + p) * Nx * Nx : nullptr;
+        for (int e = lane; e < Nx; e += 32) wz[e] = first ? (e == p ? 1.0 : 0.0) : z[e];
+        __syncwarp();
+        for (int a = lane; a < Ny; a += 32) {
+            double s = 0.0;
+            for (int e = 0; e < Nx; ++e) s = fma(sJ[a * Nx + e], wz[e], s);
+            wm[a] = s;
+        }
+        if (method_ta)
+            for (int idx = lane; idx < Ny * Nx; idx += 32) {         // T = J dS
+                const int a = idx / Nx, f = idx - a * Nx;
+                double s = 0.0;
+                if (!first)
+                    for (int e = 0; e < Nx; ++e) s = fma(sJ[a * Nx + e], S[e * Nx + f], s);
+                wT[idx] = s;
+            }
+        __syncwarp();
+        for (int idx = lane; idx < Ny * Ny; idx += 32) {
+            const int a = idx / Ny, c = idx - a * Ny;
+            double s = 0.0;
+            if (method_ta) {
+                const double* dc = dcv + (size_t)idx * Nx;
+                for (int e = 0; e < Nx; ++e) s = fma(dc[e], wz[e], s);
+                double q = 0.0;
+                for (int f = 0; f < Nx; ++f) q = fma(wT[a * Nx + f], sJ[c * Nx + f], q);
+                s += q;
+            } else if (a == c) {
+                for (int e = 0; e < Nx; ++e) s = fma(dvr[a * Nx + e], wz[e], s);
+            }
+            wC[idx] = s;
+        }
+        __syncwarp();
+        for (int a = lane; a < Ny; a += 32) {
+            dmeans_t[((size_t)b * Ny + a) * P + p] = wm[a];
+            dvars_t[((size_t)b * Ny + a) * P + p] = wC[a * Ny + a];
+        }
+        if (!last) {
+            // the entry of K this column stands for (ki, kk), or -1
+            const int q = p - Nx, ki = (fb && q >= 0) ? q / Ny : -1, kk = (fb && q >= 0) ? q - ki * Ny : -1;
+            for (int j = lane; j < Nx; j += 32) {
+                double d;
+                if (j < Ny) {
+                    d = wm[j];
+                    if (scale) d = d * scale[j] / scale[3 * Ny + j];
+                } else if (!fb) {
+                    d = (p == Nx + t * Nu + (j - Ny)) ? 1.0 : 0.0;
+                } else {
+                    const int i = j - Ny;
+                    d = 0.0;
+                    for (int k = 0; k < Ny; ++k) d = fma(K[i * Ny + k], scale ? wm[k] * scale[k] : wm[k], d);
+                    if (i == ki) d += xt[kk];
+                    if (uscale) d = d / uscale[Nu + i];
+                }
+                z[j] = d;
+            }
+            if (method_ta) {
+                if (fb)
+                    for (int idx = lane; idx < Nu * Ny; idx += 32) {     // K dC, into T (read only above this point)
+                        const int i = idx / Ny, c = idx - i * Ny;
+                        double s = 0.0;
+                        for (int k = 0; k < Ny; ++k) s = fma(K[i * Ny + k], wC[k * Ny + c], s);
+                        wT[idx] = s;
+                    }
+                __syncwarp();
+                for (int idx = lane; idx < Nx * Nx; idx += 32) {
+                    const int r = idx / Nx, c = idx - r * Nx;
+                    if (r < Ny && c < Ny) { S[idx] = wC[r * Ny + c]; continue; }
+                    if (!fb) {                                           // u blocks kept (zero at the start)
+                        if (first) S[idx] = 0.0;
+                        continue;
+                    }
+                    double s = 0.0;
+                    if (r < Ny || c < Ny) {                              // dS_xu[x][i] = (dC K^T + C dK^T)[x][i], dS_ux its transpose
+                        const int x = r < Ny ? r : c, i = (r < Ny ? c : r) - Ny;
+                        for (int k = 0; k < Ny; ++k) s = fma(wC[x * Ny + k], K[i * Ny + k], s);
+                        if (i == ki) s += cov_t[x * Ny + kk];
+                    } else {                                             // dS_uu[i][j]
+                        const int i = r - Ny, j = c - Ny;
+                        for (int k = 0; k < Ny; ++k) s = fma(wT[i * Ny + k], K[j * Ny + k], s);
+                        if (i == ki) s += CKt[kk * Nu + j];
+                        if (j == ki) s += KC[i * Ny + kk];
+                    }
+                    S[idx] = s;
+                }
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// Host outputs of the tangent stage of rollout_batch (gpmpc_rollout_batch_grad): (B, Nt, Ny, P) each
+struct RolloutTangents {
+    double *dmeans, *dvars;
+};
+
+// Device slabs of the derivative chain for H points: dvar (H,Ny,Nx) | dcov (H,Ny,Ny,Nx) | hess (H,Ny,Nx,Nx) in dGradOut,
+// and with second derivatives d2var | SH scratch | d3mean | d2cov in dHessOut (null otherwise)
+struct DerivSlabs {
+    double *dvar, *dcov, *hess;
+    double *d2var, *sh, *d3mean, *d2cov;
+};
+
+static int derivs_prepare(gpmpc_handle_t h, int H, bool second, DerivSlabs* s);
+static int derivs_enqueue(gpmpc_handle_t h, int method, int H, const double* dZ, const double* dSigma, int spp,
+                          const DerivSlabs& s);
+
+// gpmpc_rollout_batch, gpmpc_rollout and with tg gpmpc_rollout_batch_grad; fn names the entry in errors
 static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, int Nt, const double* z0, const double* U,
                          const double* Sigma0, const double* scale, const double* K, const double* x_ref,
-                         const double* uscale, double* means, double* vars, double* cov_last)
+                         const double* uscale, double* means, double* vars, double* cov_last, const RolloutTangents* tg = nullptr)
 {
     int rc = predict_guard(h, fn, method, 1);
     if (rc) return rc;
@@ -1727,9 +1890,10 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
     if (B < 1 || Nt < 1 || !z0 || !Sigma0 || !means || !vars || (Nu > 0 && !K && !U)) { set_error(h, "%s: null argument / B < 1 / Nt < 1", fn); return GPMPC_ERR_ARG; }
     if (Nu < 0) { set_error(h, "%s: needs Nx = Ny + Nu with Nu >= 0 (Nx=%d, Ny=%d)", fn, Nx, Ny); return GPMPC_ERR_ARG; }
     if (K && Nu == 0) { set_error(h, "%s: a feedback gain needs inputs (Nu = 0)", fn); return GPMPC_ERR_ARG; }
+    if (tg && (!tg->dmeans || !tg->dvars)) { set_error(h, "%s: null dmeans / dvars", fn); return GPMPC_ERR_ARG; }
     rc = predict_prepare(h, fn, B, true);
     if (rc) return rc;
-    NvtxRange nvtx_r("gpmpc.rollout");
+    NvtxRange nvtx_r(tg ? "gpmpc.rollout_grad" : "gpmpc.rollout");
     // device slab: [Z (B,Nx) | Sigma (B,Nx,Nx) | U (B,Nt,Nu) | scale (4,Ny) | K (Nu,Ny) | x_ref (Ny) | uscale (2,Nu) |
     //               means (Nt,B,Ny) | vars (Nt,B,Ny) | cov (Nt,B,Ny,Ny)], host mirror in the pinned buffer.  Step t reads
     //               and writes B consecutive points, so its outputs are one (B,...) block.
@@ -1738,7 +1902,18 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
     const size_t o_xr = o_k + (size_t)Nu * Ny, o_us = o_xr + Ny, o_m = o_us + 2 * (size_t)Nu;
     const size_t o_v = o_m + (size_t)Nt * Bs * Ny, o_c = o_v + (size_t)Nt * Bs * Ny, tot = o_c + (size_t)Nt * Bs * Ny * Ny;
     ENSURE(h->dRoll, tot);
-    rc = ensure_pinned(h, tot * 8);
+    // tangent slab: [dZ (B,P,Nx) | dS (B,P,Nx,Nx), 'TA' only | dmeans (Nt,B,Ny,P) | dvars (Nt,B,Ny,P)], the last two mirrored
+    // in the pinned buffer after the roll-out's outputs
+    const size_t P = !tg ? 0 : Nx + (K ? (size_t)Nu * Ny : (size_t)(Nt - 1) * Nu);
+    const size_t o_ds = Bs * P * Nx, o_dm = o_ds + (method == GPMPC_METHOD_TA ? Bs * P * Nx * Nx : 0);
+    const size_t o_dv = o_dm + (size_t)Nt * Bs * Ny * P, tg_tot = o_dv + (size_t)Nt * Bs * Ny * P;
+    DerivSlabs ds;
+    if (tg) {
+        rc = derivs_prepare(h, B, false, &ds);
+        if (rc) return rc;
+        ENSURE(h->dRollTg, tg_tot);
+    }
+    rc = ensure_pinned(h, (tot + (tg ? tg_tot - o_dm : 0)) * 8);
     if (rc) return rc;
     double* pin = h->hPinned;
     memcpy(pin, z0, Bs * Nx * 8);
@@ -1755,6 +1930,22 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
         double* cov_t = d + o_c + (size_t)t * Bs * Ny * Ny;
         rc = predict_core(h, method, B, d, d + o_sig, 1, d + o_m + (size_t)t * Bs * Ny, d + o_v + (size_t)t * Bs * Ny, cov_t, nullptr);
         if (rc) return rc;
+        if (tg) {                                 // J_t, dvar_t, dcov_t at the same points, then the step's tangents
+            rc = derivs_enqueue(h, method, B, d, d + o_sig, 1, ds);
+            if (rc) return rc;
+            const int nw = 8, per_warp = Nx + Ny + Ny * Ny + Ny * Nx;
+            const int tg_smem = (Ny * Nx + Ny + 2 * Ny * Nu + nw * per_warp) * 8;
+            // largest layout: Ny = Nx = NX_MAX for J and the warps, Ny = Nu = NX_MAX / 2 for C K^T and K C
+            CUDA_TRY(smem_opt_in<rollout_tangent_kernel>((NX_MAX * NX_MAX + NX_MAX + NX_MAX * NX_MAX / 2 + nw * (2 * NX_MAX + 2 * NX_MAX * NX_MAX)) * 8));
+            double* g = h->dRollTg;
+            rollout_tangent_kernel<<<B, nw * 32, tg_smem, h->st>>>(Ny, Nu, (int)P, t, t == 0, t + 1 == Nt, method == GPMPC_METHOD_TA,
+                                                                  h->dJ, ds.dvar, ds.dcov, d + o_m + (size_t)t * Bs * Ny, cov_t,
+                                                                  scale ? d + o_sc : nullptr, K ? d + o_k : nullptr,
+                                                                  K && x_ref ? d + o_xr : nullptr, K && uscale ? d + o_us : nullptr,
+                                                                  g, g + o_ds, g + o_dm + (size_t)t * Bs * Ny * P,
+                                                                  g + o_dv + (size_t)t * Bs * Ny * P);
+            CUDA_TRY(cudaGetLastError());
+        }
         if (t + 1 < Nt) {
             rollout_feedback_kernel<<<B, 256, fb_smem, h->st>>>(d + o_m + (size_t)t * Bs * Ny, cov_t, d + o_u + (size_t)(t + 1) * Nu,
                                                                 (long long)Nt * Nu, scale ? d + o_sc : nullptr, K ? d + o_k : nullptr,
@@ -1764,13 +1955,19 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
         }
     }
     CUDA_TRY(cudaMemcpyAsync(pin + o_m, d + o_m, (tot - o_m) * 8, cudaMemcpyDeviceToHost, h->st));
+    if (tg) CUDA_TRY(cudaMemcpyAsync(pin + tot, h->dRollTg + o_dm, (tg_tot - o_dm) * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
     // (t, b) -> (b, t); the reference records diag(covar_x) of every step (gp_class.py:793): the propagated variance, J Sigma J^T included
+    const size_t nyp = (size_t)Ny * P;
     for (size_t b = 0; b < Bs; ++b)
         for (int t = 0; t < Nt; ++t) {
             const size_t src = (size_t)t * Bs + b, dst = b * Nt + t;
             memcpy(means + dst * Ny, pin + o_m + src * Ny, (size_t)Ny * 8);
             for (int a = 0; a < Ny; ++a) vars[dst * Ny + a] = pin[o_c + src * Ny * Ny + (size_t)a * Ny + a];
+            if (tg) {
+                memcpy(tg->dmeans + dst * nyp, pin + tot + src * nyp, nyp * 8);
+                memcpy(tg->dvars + dst * nyp, pin + tot + (o_dv - o_dm) + src * nyp, nyp * 8);
+            }
         }
     if (cov_last)
         for (size_t b = 0; b < Bs; ++b)
@@ -1783,6 +1980,16 @@ extern "C" int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, 
                                    const double* uscale, double* means, double* vars, double* cov_last)
 {
     return rollout_batch(h, __func__, method, B, Nt, z0, U, Sigma0, scale, K, x_ref, uscale, means, vars, cov_last);
+}
+
+// gpmpc_rollout_batch plus the forward-mode derivatives of every step's mean and variance (see include/gpmpc.h)
+extern "C" int gpmpc_rollout_batch_grad(gpmpc_handle_t h, int method, int B, int Nt, const double* z0, const double* U,
+                                        const double* Sigma0, const double* scale, const double* K, const double* x_ref,
+                                        const double* uscale, double* means, double* vars, double* cov_last,
+                                        double* dmeans, double* dvars)
+{
+    const RolloutTangents tg = {dmeans, dvars};
+    return rollout_batch(h, __func__, method, B, Nt, z0, U, Sigma0, scale, K, x_ref, uscale, means, vars, cov_last, &tg);
 }
 
 // the single open-loop trajectory: B = 1 of the batched loop
@@ -1901,24 +2108,16 @@ struct HessOutputs {
     double *d2var_dz2, *d3mean_dz3, *d2cov_dz2;
 };
 
-static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, const double* Z, const double* Sigma, int spp,
-                          double* mean, double* var, double* cov, double* jac,
-                          double* dvar_dz, double* dcov_dz, double* hess, const HessOutputs* ho)
+// Buffers of the derivative chain for H points (predict_prepare first) and U = Linv^T, built once per factorisation
+static int derivs_prepare(gpmpc_handle_t h, int H, bool second, DerivSlabs* s)
 {
-    int rc = predict_guard(h, fn, method, H);
-    if (rc) return rc;
-    if (method == GPMPC_METHOD_EM) { set_error(h, "%s: derivatives are available for ME and TA", fn); return GPMPC_ERR_ARG; }
-    if (!Z || (method == GPMPC_METHOD_TA && !Sigma)) { set_error(h, "%s: null Z / Sigma", fn); return GPMPC_ERR_ARG; }
-    rc = predict_prepare(h, fn, H, true);
-    if (rc) return rc;
-    NvtxRange nvtx_r(ho ? "gpmpc.predict_hess" : "gpmpc.predict_grad");
     const int np = h->Npad, Nx = h->Nx, Ny = h->Ny, npairs = Nx * (Nx + 1) / 2;
     const int nblk_g = (np + GR_CHUNK - 1) / GR_CHUNK;
     ENSURE(h->dUall, (long long)h->nloc * slab(h));
     ENSURE(h->dBeta, (long long)h->nloc * HB * np);
     ENSURE(h->dPDV, (long long)h->nloc * HB * nblk_g * Nx);
     ENSURE(h->dPH, (long long)h->nloc * HB * nblk_g * npairs);
-    rc = ensure_rows(h);
+    const int rc = ensure_rows(h);
     if (rc) return rc;
     if (!h->u_valid) {                 // U = Linv^T (upper): the K-contiguous operand of beta = Linv^T v
         dim3 g(np / 32, np / 32), b(32, 8);
@@ -1930,12 +2129,12 @@ static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, c
     }
     const long long per = (long long)Ny * Nx + (long long)Ny * Ny * Nx + (long long)Ny * Nx * Nx;   // dvar | dcov | hess per point
     ENSURE(h->dGradOut, (long long)std::max(H, HB) * per);
-    double* d_dvar = h->dGradOut;
-    double* d_dcov = d_dvar + (long long)H * Ny * Nx;
-    double* d_hess = d_dcov + (long long)H * Ny * Ny * Nx;
+    s->dvar = h->dGradOut;
+    s->dcov = s->dvar + (long long)H * Ny * Nx;
+    s->hess = s->dcov + (long long)H * Ny * Ny * Nx;
     const long long nxx = (long long)Nx * Nx, ntri = (long long)Nx * (Nx + 1) * (Nx + 2) / 6;
-    double *d_d2var = nullptr, *d_d3mean = nullptr, *d_d2cov = nullptr, *d_sh = nullptr;
-    if (ho) {
+    s->d2var = s->d3mean = s->d2cov = s->sh = nullptr;
+    if (second) {
         ENSURE(h->dDR, (long long)h->nloc * HB * np);      // zero-filled: rows past a pass's last are never written
         ENSURE(h->dVD, (long long)h->nloc * HB * np);
         ENSURE(h->dPG, (long long)h->nloc * HB * nblk_g * npairs);
@@ -1943,18 +2142,27 @@ static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, c
         ENSURE(h->dPM3, (long long)h->nloc * HB * nblk_g * ntri);
         const long long hper = 2 * Ny * nxx + Ny * nxx * Nx + (long long)Ny * Ny * nxx;      // d2var | SH scratch | d3mean | d2cov
         ENSURE(h->dHessOut, (long long)std::max(H, HB) * hper);
-        d_d2var = h->dHessOut;
-        d_sh = d_d2var + (long long)H * Ny * nxx;
-        d_d3mean = d_sh + (long long)H * Ny * nxx;
-        d_d2cov = d_d3mean + (long long)H * Ny * nxx * Nx;
+        s->d2var = h->dHessOut;
+        s->sh = s->d2var + (long long)H * Ny * nxx;
+        s->d3mean = s->sh + (long long)H * Ny * nxx;
+        s->d2cov = s->d3mean + (long long)H * Ny * nxx * Nx;
     }
-    const size_t nz = (size_t)H * Nx, ns = (method == GPMPC_METHOD_TA) ? (size_t)(spp ? H : 1) * Nx * Nx : 0;
-    CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, nz * 8, cudaMemcpyHostToDevice, h->st));
-    if (ns) CUDA_TRY(cudaMemcpyAsync(h->dSigma, Sigma, ns * 8, cudaMemcpyHostToDevice, h->st));
-    const AssembleArgs as = assemble_args(h, H, method, h->dSigma, spp, h->dMean, h->dVar, h->dJ, h->dCov);
+    return GPMPC_OK;
+}
+
+// The derivative chain of H device-resident points dZ (H,Nx), Sigma dSigma (per point if spp), after derivs_prepare:
+// per 64-point chunk ks, v = Linv ks with the gather records, beta = Linv^T v, the block partials of dvar / mean Hessian
+// and their finalisation (with s.d2var, the second-derivative passes); then the assembly of mean, var, J, cov into dOut
+// and d cov / dz.  gpmpc_predict_grad / _hess run it on their uploaded points, gpmpc_rollout_batch_grad on every step's.
+static int derivs_enqueue(gpmpc_handle_t h, int method, int H, const double* dZ, const double* dSigma, int spp,
+                          const DerivSlabs& s)
+{
+    const int np = h->Npad, Nx = h->Nx, Ny = h->Ny;
+    const int nblk_g = (np + GR_CHUNK - 1) / GR_CHUNK;
+    const AssembleArgs as = assemble_args(h, H, method, dSigma, spp, h->dMean, h->dVar, h->dJ, h->dCov);
     for (int h0 = 0; h0 < H; h0 += HB) {
         const int Hc = std::min(HB, H - h0);
-        const double* dZc = h->dZ + (long long)h0 * Nx;
+        const double* dZc = dZ + (long long)h0 * Nx;
         CUDA_TRY(launch_ks(h, dZc, Hc));
         PredictParams p;
         psk_base(h, p, Hc);                                   // v = Linv ks: records + the rows themselves
@@ -1966,25 +2174,48 @@ static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, c
         CUDA_TRY(psk_launch(h, p, h->dV, h->dUall));
         CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_grad_reduce<decltype(nxp)::value>(h, dZc, Hc, nblk_g); }));
         grad_finalize_kernel<<<dim3(Hc, h->nloc), 128, 0, h->st>>>(h->dPDV, h->dPH, nblk_g, Hc, h->dHyp, Nx + 2, Nx, Ny,
-                                                                   h->dG, H, h0, d_dvar, d_hess);
+                                                                   h->dG, H, h0, s.dvar, s.hess);
         CUDA_TRY(cudaGetLastError());
-        if (ho) {
-            rc = hess_chunk(h, dZc, Hc, H, h0, d_d2var, d_d3mean);
+        if (s.d2var) {
+            const int rc = hess_chunk(h, dZc, Hc, H, h0, s.d2var, s.d3mean);
             if (rc) return rc;
         }
     }
-    {
-        const int smem = (2 * Ny * Nx + Ny) * 8;
-        assemble_kernel<<<std::min(H, 2048), 128, smem, h->st>>>(as);
+    const int smem = (2 * Ny * Nx + Ny) * 8;
+    assemble_kernel<<<std::min(H, 2048), 128, smem, h->st>>>(as);
+    CUDA_TRY(cudaGetLastError());
+    grad_cov_kernel<<<H, 128, 2 * Ny * Nx * 8, h->st>>>(Ny, Nx, method == GPMPC_METHOD_TA, dSigma, spp, h->dJ, s.dvar, s.hess, s.dcov);
+    CUDA_TRY(cudaGetLastError());
+    if (s.d2var) {
+        hess_cov_kernel<<<H, 128, 2 * Ny * Nx * 8, h->st>>>(Ny, Nx, method == GPMPC_METHOD_TA, dSigma, spp, h->dJ, s.hess,
+                                                            s.d2var, s.d3mean, s.sh, s.d2cov);
         CUDA_TRY(cudaGetLastError());
-        grad_cov_kernel<<<H, 128, 2 * Ny * Nx * 8, h->st>>>(Ny, Nx, method == GPMPC_METHOD_TA, h->dSigma, spp, h->dJ, d_dvar, d_hess, d_dcov);
-        CUDA_TRY(cudaGetLastError());
-        if (ho) {
-            hess_cov_kernel<<<H, 128, 2 * Ny * Nx * 8, h->st>>>(Ny, Nx, method == GPMPC_METHOD_TA, h->dSigma, spp, h->dJ, d_hess,
-                                                                d_d2var, d_d3mean, d_sh, d_d2cov);
-            CUDA_TRY(cudaGetLastError());
-        }
     }
+    return GPMPC_OK;
+}
+
+static int predict_derivs(gpmpc_handle_t h, const char* fn, int method, int H, const double* Z, const double* Sigma, int spp,
+                          double* mean, double* var, double* cov, double* jac,
+                          double* dvar_dz, double* dcov_dz, double* hess, const HessOutputs* ho)
+{
+    int rc = predict_guard(h, fn, method, H);
+    if (rc) return rc;
+    if (method == GPMPC_METHOD_EM) { set_error(h, "%s: derivatives are available for ME and TA", fn); return GPMPC_ERR_ARG; }
+    if (!Z || (method == GPMPC_METHOD_TA && !Sigma)) { set_error(h, "%s: null Z / Sigma", fn); return GPMPC_ERR_ARG; }
+    rc = predict_prepare(h, fn, H, true);
+    if (rc) return rc;
+    NvtxRange nvtx_r(ho ? "gpmpc.predict_hess" : "gpmpc.predict_grad");
+    const int Nx = h->Nx, Ny = h->Ny;
+    const long long nxx = (long long)Nx * Nx;
+    DerivSlabs s;
+    rc = derivs_prepare(h, H, ho != nullptr, &s);
+    if (rc) return rc;
+    const size_t nz = (size_t)H * Nx, ns = (method == GPMPC_METHOD_TA) ? (size_t)(spp ? H : 1) * Nx * Nx : 0;
+    CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, nz * 8, cudaMemcpyHostToDevice, h->st));
+    if (ns) CUDA_TRY(cudaMemcpyAsync(h->dSigma, Sigma, ns * 8, cudaMemcpyHostToDevice, h->st));
+    rc = derivs_enqueue(h, method, H, h->dZ, h->dSigma, spp, s);
+    if (rc) return rc;
+    const double *d_dvar = s.dvar, *d_dcov = s.dcov, *d_hess = s.hess, *d_d2var = s.d2var, *d_d3mean = s.d3mean, *d_d2cov = s.d2cov;
     if (mean) CUDA_TRY(cudaMemcpyAsync(mean, h->dMean, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
     if (var) CUDA_TRY(cudaMemcpyAsync(var, h->dVar, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
     if (cov) CUDA_TRY(cudaMemcpyAsync(cov, h->dCov, (size_t)H * Ny * Ny * 8, cudaMemcpyDeviceToHost, h->st));

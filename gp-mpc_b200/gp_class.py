@@ -633,6 +633,110 @@ class GP:
                 covar[b, :self.__Ny, :self.__Ny] = c_last[k]
         return True
 
+    def rollout_grad(self, x0, u, method=None, feedback=False, x_ref=None, Q=None, R=None):
+        """ ``rollout`` for one method with the exact derivatives of every step's mean and variance w.r.t. what produced
+        the trajectory: the start x0 and, open loop, the inputs u, or with feedback=True the gain K.  Forward-mode
+        tangents run on the device beside the roll-out (gpmpc_rollout_batch_grad), so one call replaces the P + 1
+        roll-outs of a difference quotient and carries no truncation error.
+
+        Shapes follow ``rollout``: x0:(Ny,) with u:(Nt,Nu), or a batch x0:(B,Ny) with u:(B,Nt,Nu), which adds a leading B
+        axis to every array below.  Returns a dict in caller units:
+          mean, var (Nt+1, Ny)             ``rollout(x0, u, methods=[method], ...)``'s arrays for this method
+          dmean_dx0, dvar_dx0 (Nt+1, Ny, Ny)   row 0 is the identity and zero
+          open loop:  dmean_du, dvar_du (Nt+1, Ny, Nt, Nu)      d mean[t] / d u[s, i]
+          feedback:   dmean_dK, dvar_dK (Nt+1, Ny, Nu, Ny)      d mean[t] / d K[i, k]
+        The initial covariance, the gain per trajectory (the LQR gain of the linearisation at (x0, u[0]); defaults Q = I,
+        R = I, x_ref = 0) and the grouping of trajectories by distinct gain are ``rollout``'s.  With feedback the gain is
+        held fixed: its own dependence on x0 through ``discrete_linearize`` and the Riccati equation is not
+        differentiated, so dmean_dx0 is the derivative of the closed loop under that fixed K, including u_0 = K (x0 - x_ref).
+        method defaults to the GP's gp_method. """
+        meth = self.__gp_method if method is None else method
+        if meth not in ('ME', 'TA'):
+            raise NotImplementedError("rollout_grad differentiates gp_method 'ME' and 'TA' (got %r)" % (meth,))
+        if self.__comm.world > 1:
+            raise NotImplementedError('rollout_grad needs all outputs on one GPU (build the GP with a single-process Comm)')
+        if self.__prior_mean_in_predict and self.__has_prior_mean():
+            raise NotImplementedError('rollout_grad differentiates the zero-mean posterior the engine holds; '
+                                      'prior_mean_in_predict with a prior mean function is not supported')
+        Nx, Ny, Nu = self.__Nx, self.__Ny, self.__Nu
+        x0 = np.asarray(x0, dtype=np.float64)
+        single = x0.ndim < 2
+        X0 = x0.reshape(1, Ny) if single else x0.reshape(-1, Ny)
+        nb = X0.shape[0]
+        u = np.asarray(u, dtype=np.float64)
+        if single:
+            U = (u.reshape(-1, Nu) if Nu > 0 else np.zeros((u.shape[0] if u.ndim else 0, 0)))[None]
+        else:
+            U = u.reshape(nb, -1, Nu) if Nu > 0 else np.zeros((nb, u.shape[1] if u.ndim > 1 else 0, 0))
+        Nt = U.shape[1]
+        if Nt < 1:
+            raise ValueError('rollout_grad needs at least one step')
+        K = None
+        if feedback:
+            if Nu == 0:
+                raise ValueError('rollout_grad(feedback=True) needs a model with inputs (Nu > 0)')
+            Q = np.eye(Ny) if Q is None else np.asarray(Q, dtype=np.float64)
+            R = np.eye(Nu) if R is None else np.asarray(R, dtype=np.float64)
+            x_ref = np.zeros(Ny) if x_ref is None else np.asarray(x_ref, dtype=np.float64).reshape(Ny)
+            K = self.__lqr_gains(X0, U[:, 0], Q, R)
+        covar = np.tile(np.eye(Nx) * 1e-6, (nb, 1, 1))                 # rollout's initial covariance
+        covar[:, :Ny, :Ny] = np.diag(self.__hyper[:, Nx + 1] ** 2)
+        # z0 and the scalers exactly as __rollout_device forms them, so mean / var are rollout's bits
+        un, scale, uscale = U, None, None
+        if K is not None:
+            un = np.stack([_matmul_seq(K[b], (X0[b] - x_ref)[:, None])[:, 0] for b in range(nb)])[:, None, :]
+        zx = X0
+        sX, sU, sY = np.ones(Ny), np.ones(Nu), np.ones(Ny)
+        if self.__normalize:
+            zx = self.standardize(X0, self.__meanX, self.__stdX)
+            un = self.standardize(un, self.__meanU, self.__stdU)
+            scale = np.stack([self.__stdY, self.__meanY, self.__meanX, self.__stdX])
+            uscale = np.stack([self.__meanU, self.__stdU])
+            sX, sU, sY = self.__stdX, self.__stdU, self.__stdY
+        z0 = np.concatenate([zx, un[:, 0, :]], 1)
+        method_id, eng = _GPU_METHODS[meth], self.__engine
+        P = Nx + (Nu * Ny if K is not None else (Nt - 1) * Nu)
+        m_std = np.empty((nb, Nt, Ny)); v_std = np.empty((nb, Nt, Ny))
+        Dm = np.empty((nb, Nt, Ny, P)); Dv = np.empty((nb, Nt, Ny, P))
+        if K is None:
+            parts = [(np.arange(nb), eng.rollout_batch_grad(z0, un, covar, method_id, scale))]
+        else:                                            # one pass per distinct gain, as rollout
+            groups = {}
+            for b in range(nb):
+                groups.setdefault(K[b].tobytes(), []).append(b)
+            parts = [(g, eng.rollout_batch_grad(z0[g], U[g], covar[g], method_id, scale, K[g[0]], x_ref, uscale))
+                     for g in map(np.array, groups.values())]
+        for g, (mg, vg, _, dmg, dvg) in parts:
+            m_std[g], v_std[g], Dm[g], Dv[g] = mg, vg, dmg, dvg
+        # caller units: mean = m stdY + meanY, var = v stdY^2; z0 = [(x0 - meanX) / stdX, (u_0 - meanU) / stdU]
+        Dm = Dm * sY[None, None, :, None]
+        Dv = Dv * (sY ** 2)[None, None, :, None]
+        out = dict(mean=np.zeros((nb, Nt + 1, Ny)), var=np.zeros((nb, Nt + 1, Ny)))
+        out['mean'][:, 0] = X0
+        out['mean'][:, 1:] = self.inverse_mean(m_std, self.__meanY, self.__stdY) if self.__normalize else m_std
+        out['var'][:, 1:] = self.inverse_variance(v_std) if self.__normalize else v_std
+        for key, D in (('mean', Dm), ('var', Dv)):
+            d_x0 = np.zeros((nb, Nt + 1, Ny, Ny))
+            if key == 'mean':
+                d_x0[:, 0] = np.eye(Ny)
+            d_x0[:, 1:] = D[..., :Ny] / sX
+            d_u0 = D[..., Ny:Nx] / sU                    # w.r.t. u_0 in caller units (nb, Nt, Ny, Nu)
+            if K is None:
+                d_u = np.zeros((nb, Nt + 1, Ny, Nt, Nu))
+                d_u[:, 1:, :, 0, :] = d_u0
+                d_u[:, 1:, :, 1:, :] = (D[..., Nx:] / np.tile(sU, Nt - 1)).reshape(nb, Nt, Ny, Nt - 1, Nu)
+                out['d%s_du' % key] = d_u
+            else:                                        # u_0 = K (x0 - x_ref): both x0 and K enter z0's tail
+                d_x0[:, 1:] += np.einsum('btai,bik->btak', d_u0, K)
+                d_K = np.zeros((nb, Nt + 1, Ny, Nu, Ny))
+                d_K[:, 1:] = D[..., Nx:].reshape(nb, Nt, Ny, Nu, Ny)
+                d_K[:, 1:] += d_u0[..., :, None] * (X0 - x_ref)[:, None, None, None, :]
+                out['d%s_dK' % key] = d_K
+            out['d%s_dx0' % key] = d_x0
+        if single:
+            return {k: v[0] for k, v in out.items()}
+        return out
+
     def sample_rollout(self, x0, u, n_samples, seed=None, Sigma0=None, feedback=False, x_ref=None, Q=None, R=None,
                        process_noise=False):
         """ Monte Carlo trajectories of the learned dynamics (gpmpc_rollout_sample): each sample is one draw f of the

@@ -256,6 +256,28 @@ int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, const doubl
                         const double* Sigma0, const double* scale, const double* K, const double* x_ref,
                         const double* uscale, double* means, double* vars, double* cov_last);
 
+/* gpmpc_rollout_batch plus the exact derivatives of every step's mean and variance w.r.t. what produced the trajectory,
+ * by forward-mode tangents carried on the device beside the roll-out (one derivative chain of gpmpc_predict_grad per step
+ * on the same points, then one tangent kernel).  Same arguments; means, vars, cov_last are bit-identical to
+ * gpmpc_rollout_batch's.  Further outputs, both required:
+ *   dmeans, dvars (B, Nt, Ny, P)  d means[b,t,a] / d theta_p and d vars[b,t,a] / d theta_p, GP output units
+ * with the P parameters of trajectory b, in this column order:
+ *   z0[b] (Nx), then open loop the rows U[b,1..Nt-1] ((Nt-1) Nu; row 0 is unused, z0 carries u_0), or with K the
+ *   entries of K row-major (Nu Ny):  P = Nx + (Nt-1) Nu open loop, Nx + Nu Ny with feedback, Nx when Nu = 0.
+ * Sigma0, scale, x_ref and uscale are held fixed.  Per parameter, step t (J_t, dcov_dz_t, dvar_dz_t of gpmpc_predict_grad):
+ *   dm = J dz,  dC = sum_e dcov_dz[.,.,e] dz_e + J dSigma J^T ('TA')  or  diag(dvar_dz dz) ('ME'),  dvars = diag(dC)
+ *   next dz[:Ny] = dm stdY / stdX (dm without scale);  open loop: dz[Ny:] the unit tangent of U[t+1], dSigma x block = dC,
+ *   u blocks kept;  with K, x = mean stdY + meanY:  du = (K dx + dK (x - x_ref)) / stdU,  dSigma_xu = dC K^T + C dK^T,
+ *   dSigma_uu = dK C K^T + K dC K^T + K C dK^T  (the derivatives of the feedback update of gpmpc_rollout_batch).
+ * Every sum runs in a fixed order: trajectory b's results do not depend on B or its row.  Methods ME and TA (EM:
+ * GPMPC_ERR_ARG); GPMPC_ERR_STATE: not factorised, or the handle does not own every output; GPMPC_ERR_ARG: every argument
+ * error of gpmpc_rollout_batch, or dmeans / dvars NULL.  Every check runs before any work.  Device memory: 8 B P (Nx + Nx^2)
+ * bytes of tangents ('TA'; 8 B P Nx for 'ME') plus 16 Nt B Ny P bytes of outputs. */
+int gpmpc_rollout_batch_grad(gpmpc_handle_t h, int method, int B, int Nt, const double* z0, const double* U,
+                             const double* Sigma0, const double* scale, const double* K, const double* x_ref,
+                             const double* uscale, double* means, double* vars, double* cov_last,
+                             double* dmeans, double* dvars);
+
 /* Sample trajectories of the learned dynamics: each of the B trajectories is one draw f of the GP posterior, evaluated along
  * the inputs that draw visits.  Per output a and step t, f_t(z_t) is drawn conditioned on the values the same draw took
  * at the earlier points z_0 .. z_{t-1} of the trajectory, so the whole trajectory satisfies f - m = R eps with R the
