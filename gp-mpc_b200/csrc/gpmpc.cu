@@ -124,6 +124,9 @@ struct gpmpc_handle_s {
     // backbone rows [e | e v_d] and their L^-1 products
     DevBuf<double> dEmKinv, dEmGPart, dEmGRec, dEmBB; bool em_kinv_valid = false;
     std::vector<double> hyper;        // (nloc, Nx+2)
+    // host copy of X (N, Nx) row-major, kept by set_data, append, append_greedy and remove: the K build's centre dMu is
+    // recomputed from it (mu_stale) before the next K build, so appends and removals never leave K centred on an old mean
+    std::vector<double> hX; bool mu_stale = false;
     std::vector<double> logdet, yalpha;
     std::vector<int> jitter_used;
     int sms = 132;                    // multiprocessors of the device (queried in create)
@@ -338,6 +341,20 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
 // output slabs at K (stride slab).  full = 1 writes the whole square, 0 the lower triangle.
 static int launch_kbuild(gpmpc_handle_t h, const double* dHyp, const double* dJit, double* K, int batch, int full)
 {
+    if (h->mu_stale) {
+        // column means of the current X: the K build centres its inputs (translation invariant), and its cancellation
+        // error grows with |u|^2 measured from that centre.  Same order as every earlier value, so a handle given its
+        // X by set_data and one that reached the same X by appends and removals build the same K bit for bit.
+        const int N = h->N, Nx = h->Nx;
+        double mu[NX_MAX] = {0.0};
+        for (int d = 0; d < Nx; ++d) {
+            double sacc = 0.0;
+            for (int i = 0; i < N; ++i) sacc += h->hX[(size_t)i * Nx + d];
+            mu[d] = sacc / N;
+        }
+        CUDA_TRY(cudaMemcpyAsync(h->dMu, mu, NX_MAX * 8, cudaMemcpyHostToDevice, h->st));
+        h->mu_stale = false;
+    }
     const int KD = (h->Nx + 3) & ~3, S = ((KD >> 2) & 1) ? KD : KD + 4;
     const int smem = (2 * KB2_TILE * S + 2 * KB2_TILE + 256) * 8;
     const int smem_max = (2 * KB2_TILE * 36 + 2 * KB2_TILE + 256) * 8;   // S at NX_MAX
@@ -585,13 +602,8 @@ extern "C" int gpmpc_set_data(gpmpc_handle_t h, const double* X, const double* Y
         for (int d = 0; d < Nx; ++d) xt[(size_t)d * np + i] = X[(size_t)i * Nx + d];
     for (int a = 0; a < h->nloc; ++a)
         for (int i = 0; i < N; ++i) yl[(size_t)a * np + i] = Y[(size_t)i * h->Ny + h->a0 + a];
-    double mu[NX_MAX] = {0.0};              // column means: the K build centres its inputs (translation invariant)
-    for (int d = 0; d < Nx; ++d) {
-        double sacc = 0.0;
-        for (int i = 0; i < N; ++i) sacc += X[(size_t)i * Nx + d];
-        mu[d] = sacc / N;
-    }
-    CUDA_TRY(cudaMemcpyAsync(h->dMu, mu, NX_MAX * 8, cudaMemcpyHostToDevice, h->st));
+    h->hX.assign(X, X + (size_t)N * Nx);
+    h->mu_stale = true;                     // launch_kbuild centres on the column means of hX
     CUDA_TRY(cudaMemcpyAsync(h->dXT, xt.data(), xt.size() * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaMemcpyAsync(h->dY, yl.data(), yl.size() * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
@@ -2324,7 +2336,12 @@ extern "C" int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double*
     for (int d = 0; d < Nx; ++d) CUDA_TRY(cudaMemcpyAsync(h->dXT + (long long)d * np + N, x_new + d, 8, cudaMemcpyHostToDevice, h->st));
     for (int a = 0; a < nl; ++a) CUDA_TRY(cudaMemcpyAsync(h->dY + (long long)a * np + N, y_new + h->a0 + a, 8, cudaMemcpyHostToDevice, h->st));
     int added = 0;
-    return finish_appends(h, __func__, N, 1, &added);
+    rc = finish_appends(h, __func__, N, 1, &added);
+    if (h->N > N) {                                   // counted even when the pivot failed
+        h->hX.insert(h->hX.end(), x_new, x_new + Nx);
+        h->mu_stale = true;
+    }
+    return rc;
 }
 
 // The solved rows v = L^-1 k(X, z) of the H points at dZ (device, (H, Nx)) for every owned output into dst: row h of
@@ -2514,7 +2531,9 @@ extern "C" int gpmpc_append_greedy(gpmpc_handle_t h, int n, const double* Xc, co
     for (int k = 0; k < *n_added; ++k) {
         picked[k] = pk[k];
         if (score) score[k] = sc[k];
+        h->hX.insert(h->hX.end(), Xc + (size_t)pk[k] * Nx, Xc + (size_t)(pk[k] + 1) * Nx);
     }
+    if (*n_added > 0) h->mu_stale = true;
     return rc;
 }
 
@@ -2567,6 +2586,10 @@ extern "C" int gpmpc_remove(gpmpc_handle_t h, int n, const int* idx)
         remove_shift_kernel<<<Nx + nl, 256, 0, h->st>>>(h->dXT, Nx, h->dY, np, i, Nk);
         CUDA_TRY(cudaGetLastError());
     }
+    // the host copy follows X^T only once every removal is enqueued, so an early error return leaves hX and N consistent
+    for (int k = 0; k < n; ++k)           // descending indices: row order kept, as in X^T
+        h->hX.erase(h->hX.begin() + (size_t)order[k] * Nx, h->hX.begin() + (size_t)(order[k] + 1) * Nx);
+    h->mu_stale = true;
     h->N = N - n;
     return refresh_alpha(h);
 }

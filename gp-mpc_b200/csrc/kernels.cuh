@@ -16,8 +16,9 @@
 //   fp64 pipe only ~12 instructions per pair (two adds, clamp, a two-level-table exp2 with a
 //   degree-4 polynomial).  a profile of the first (direct-difference, libm exp) kernel showed the fp64 pipe and DRAM
 //   traffic not overlapping: the two pipes now overlap and the kernel becomes write-bandwidth bound.
-//   The kernel is translation invariant, so inputs are centred on the column means mu: the
-//   expansion's cancellation error is eps*|u|^2 with |u| measured from the data centre
+//   The kernel is translation invariant, so inputs are centred on the column means mu of the current X (set_data,
+//   and recomputed after appends and removals): the expansion's cancellation error is eps*|u|^2 with |u| measured from
+//   the data centre
 //   (<= 6e-16 relative on both reference fixtures, same as direct differences; the reference's
 //   own numpy path uses the un-centred expansion, optimize.py:315-319).
 //   One CTA = one 128x128 tile of the lower triangle; off-diagonal tiles also store the
@@ -33,7 +34,8 @@ __constant__ double c_exp2_tab[16] = {
 // Two-level table: 2^t = 2^e * T1[(n >> 4) & 15] * T2[n & 15] * 2^f with n = rint(256 t), T1[k] = 2^(k/16), T2[m] = 2^(m/256),
 // |f| <= 1/512 (degree-4 polynomial, truncation 3.8e-17).  Both tables have ONE entry per shared-memory bank, so the
 // lookups are conflict-free whatever the lane pattern (a flat 256-entry table replays ~3x), and the polynomial needs four
-// coefficients where a single 16-entry table needs seven (each costs two UMOVs in the loop on this target).  ~2.2 ulp.
+// coefficients where a single 16-entry table needs seven (each costs two UMOVs in the loop on this target).  At most
+// 2.75 ulp (measured against mpmath on an exact restatement, tests/test_kernel_range_cpu.py).
 // Valid for -1020 <= t <= ~1000: the CALLER clamps (rint(256 t) must fit the low word and the exponent stay normal).
 // T32 is a shared-memory copy of both tables: T32[0..15] = c_exp2_tab, T32[16..31] = c_exp2_tab2.
 __constant__ double c_exp2_tab2[16] = {
@@ -722,7 +724,7 @@ ks_tile_kernel(const double* __restrict__ XT, int ldx, int N, int Nx,
                 d0 = fma(df[d], df[d], d0);
                 d1 = fma(df[d + 1], df[d + 1], d1);
             }
-            // sf2 exp(-dist/2) = 2^(log2 sf2 - log2(e)/2 dist) with the two-level table exp2 of the K build (~2 ulp)
+            // sf2 exp(-dist/2) = 2^(log2 sf2 - log2(e)/2 dist) with the two-level table exp2 of the K build (<= 2.75 ulp)
             double te = fma(-0.72134752044448170, d0 + d1, l2sf2);
             te = (te < -1020.0) ? -1020.0 : te;
             double ks = exp2_t2lvl(te, T32s);
