@@ -36,6 +36,7 @@ SYMBOLS = [
     ('gpmpc_build_K', C.c_int, [_H, C.c_int, _dp]),
     ('gpmpc_factorize', C.c_int, [_H, C.c_double, _ip]),
     ('gpmpc_nlml', C.c_int, [_H, C.c_int, _dp, _dp, _dp]),
+    ('gpmpc_nlml_batch', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, _dp, _ip]),
     ('gpmpc_loo', C.c_int, [_H, _dp, _dp, _dp]),
     ('gpmpc_loo_nlpp', C.c_int, [_H, C.c_int, _dp, _dp, _dp]),
     ('gpmpc_predict', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp]),
@@ -213,6 +214,19 @@ class Engine:
         g = np.empty(self.Nx + 2) if grad else None
         self._check(self.lib.gpmpc_nlml(self.h, int(a), _ptr(theta), C.byref(nll), _ptr(g)))
         return (nll.value, g) if grad else nll.value
+
+    def nlml_batch(self, a, thetas, grad=True):
+        """gpmpc_nlml_batch: nlml at the S rows of thetas:(S,Nx+2) in one pass -> nll (S,), grad (S,Nx+2) or None,
+        status (S,) int32 (0 ok, 1 ok after the jitter retry, ERR_NOTPD: that row's nll and grad are NaN).  Row s has the
+        bits of nlml(a, thetas[s]); the factorisation stays valid."""
+        thetas = _f64(thetas).reshape(-1, self.Nx + 2)
+        S = thetas.shape[0]
+        nll = np.empty(S)
+        g = np.empty((S, self.Nx + 2)) if grad else None
+        status = np.empty(S, dtype=np.int32)
+        self._check(self.lib.gpmpc_nlml_batch(self.h, int(a), S, _ptr(thetas), _ptr(nll), _ptr(g),
+                                              status.ctypes.data_as(_ip)))
+        return nll, g, status
 
     def loo(self):
         """gpmpc_loo: leave-one-out predictions of the training points on the current factorisation of every owned

@@ -77,6 +77,7 @@ struct DevBuf {
     ~DevBuf() { cudaFree(p); }
     operator T*() const { return p; }
     int ensure(gpmpc_handle_t h, long long count, const char* name);
+    void release() { cudaFree(p); p = nullptr; cap = 0; }     // the caller has drained the streams that use it
 };
 
 struct gpmpc_handle_s {
@@ -116,6 +117,9 @@ struct gpmpc_handle_s {
     // nlml scratch
     DevBuf<double> dU, dKinv, dGradPart, dGrad;
     DevBuf<double> dLoo;              // gpmpc_loo / gpmpc_loo_nlpp: [mean | var | nlpp | c partials | sw | u | b | tmp | 0]
+    // gpmpc_nlml_batch: per entry of a pass its own L, Li slabs and recursion workspaces (nlml_batch_scratch)
+    DevBuf<double> dNbL, dNbLi, dNbW1, dNbW2, dNbV; DevBuf<int> dNbInfo;
+    int opt_nlml_batch_max = 0;       // entries per gpmpc_nlml_batch pass (0: all)
     bool has_data = false, has_hyper = false, factorized = false;
     // EM scratch
     DevBuf<double> dEmTr, dEMP, dEmE, dEmF, dEmW, dEmIJ;
@@ -205,10 +209,12 @@ static cudaError_t nxp_dispatch(int Nx, F&& f)
 // ------------------------------------------------------------------------------------
 // Callers describe the problem in 128x128 tiles (mt, nt); the launch re-tiles it.  Tile-granular TMA
 // (tensor maps, 128B swizzle) serves the NT products that fill the GPU for at least two waves; everything
-// else (NN products, small launches) takes the cp.async kernel.
-static cudaError_t gemm128(gpmpc_handle_t h, cudaStream_t st, bool bt, const GemmParams& p, int batch)
+// else (NN products, small launches) takes the cp.async kernel.  The feed is chosen from the tiles of `sel_batch` slabs
+// while the launch covers `batch`: the feeds round differently, so a caller whose slabs must get the bits of a lone slab
+// passes sel_batch = 1.
+static cudaError_t gemm128(gpmpc_handle_t h, cudaStream_t st, bool bt, const GemmParams& p, int batch, int sel_batch)
 {
-    const long long tiles = (long long)batch * (p.lower ? (long long)p.mt * (p.mt + 1) : 2LL * p.mt * p.nt);
+    const long long tiles = (long long)sel_batch * (p.lower ? (long long)p.mt * (p.mt + 1) : 2LL * p.mt * p.nt);
     GemmParams q = p;
     if (tiles < h->opt_small_tiles) {
         // deep recursion levels: a handful of 128x64 tiles cannot occupy 132 SMs; 64x32 tiles
@@ -230,9 +236,11 @@ static cudaError_t gemm128(gpmpc_handle_t h, cudaStream_t st, bool bt, const Gem
 //   3. A22 -= L21 L21^T                 (trailing SYRK update, DMMA GEMM NT, lower tiles)
 //   4. (L22, Li22) = rec(A22)
 //   5. Li21 = -Li22 (L21 Li11)          (two DMMA GEMMs NN)
-// All flops except the 128x128 leaves run on the fp64 tensor pipe.
+// All flops except the 128x128 leaves run on the fp64 tensor pipe.  Workspace: W1b, W2b (w2slab per batch entry); every
+// GEMM picks its feed as for sel_batch slabs (gemm128).
 static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, long long sLi,
-                         int* dInfo, int off, int n, int batch, int depth = 0, cudaEvent_t pend = nullptr)
+                         int* dInfo, int off, int n, int batch, int sel_batch, double* W1b, double* W2b, int depth = 0,
+                         cudaEvent_t pend = nullptr)
 {
     const int ld = h->Npad;
     if (n <= LEAF_N) {
@@ -245,7 +253,7 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
     }
     const int nb = n / GPMPC_TILE;
     const int n1 = (nb / 2) * GPMPC_TILE, n2 = n - n1;
-    int rc = potrf_inv_rec(h, A, Li, sA, sLi, dInfo, off, n1, batch, depth + 1, nullptr);
+    int rc = potrf_inv_rec(h, A, Li, sA, sLi, dInfo, off, n1, batch, sel_batch, W1b, W2b, depth + 1, nullptr);
     if (rc) return rc;
     // the caller deferred part of its trailing update to its side stream (look-ahead, see below): everything outside this
     // sub-problem's leading n1 x n1 block is only valid once that work has finished
@@ -255,8 +263,8 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
     double* Li11 = Li + (long long)off * ld + off;
     double* Li21 = Li + (long long)(off + n1) * ld + off;
     double* Li22 = Li + (long long)(off + n1) * ld + off + n1;
-    double* W1 = h->dW1 + h->w2off[depth];                 // one region per depth (deferred work of different depths is in flight together)
-    double* W2 = h->dW2 + h->w2off[depth];
+    double* W1 = W1b + h->w2off[depth];                    // one region per depth (deferred work of different depths is in flight together)
+    double* W2 = W2b + h->w2off[depth];
     const long long sW = w2slab(h), sW2 = w2slab(h);
     const bool ovl = depth < MAX_DEPTH;
     cudaStream_t side = ovl ? h->sideSt[depth] : h->st;
@@ -275,7 +283,7 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
         q.B = Li11; q.ldb = ld; q.sB = sLi;                                   // B[j][k] = Li11[j][k] != 0 only for k <= j
         q.C = W1 + (long long)r0 * n1; q.ldc = n1; q.sC = sW;
         q.mt = rows / 128; q.nt = n1 / 128; q.K = n1; q.alpha = 1.0; q.beta = 0.0; q.kflags = GEMM_KJ_LE;
-        cudaError_t e = gemm128(h, st, true, q, batch);
+        cudaError_t e = gemm128(h, st, true, q, batch, sel_batch);
         if (e != cudaSuccess) return e;
         dim3 g(std::max(1, std::min(64, n1 / 2 / 128)), std::min(rows, 4096), batch);
         copy2d_kernel<<<g, 128, 0, st>>>(W1 + (long long)r0 * n1, n1, sW, A21 + (long long)r0 * ld, ld, sA, rows, n1);
@@ -288,7 +296,7 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
         q.B = W1 + (long long)c0 * n1; q.ldb = n1; q.sB = sW;
         q.C = A22 + (long long)r0 * ld + c0; q.ldc = ld; q.sC = sA; q.Cin = q.C; q.ldcin = ld; q.sCin = sA;
         q.mt = rows / 128; q.nt = cols / 128; q.K = n1; q.alpha = -1.0; q.beta = 1.0; q.lower = lower;
-        return gemm128(h, st, true, q, batch);
+        return gemm128(h, st, true, q, batch, sel_batch);
     };
     if (ovl) {
         CUDA_TRY(cudaEventRecord(h->evA[depth], h->st));
@@ -319,21 +327,22 @@ static int potrf_inv_rec(gpmpc_handle_t h, double* A, double* Li, long long sA, 
     p.C = W2; p.ldc = n1; p.sC = sW2;
     p.mt = n2 / 128; p.nt = n1 / 128; p.K = n1; p.alpha = 1.0; p.beta = 0.0; p.kflags = GEMM_KJ_GE;
     if (ovl) {
-        CUDA_TRY(gemm128(h, side, false, p, batch));
+        CUDA_TRY(gemm128(h, side, false, p, batch, sel_batch));
         CUDA_TRY(cudaEventRecord(h->evB[depth], side));
     }
     // 4.
-    rc = potrf_inv_rec(h, A, Li, sA, sLi, dInfo, off + n1, n2, batch, depth + 1, split ? h->evS[depth] : nullptr);
+    rc = potrf_inv_rec(h, A, Li, sA, sLi, dInfo, off + n1, n2, batch, sel_batch, W1b, W2b, depth + 1,
+                       split ? h->evS[depth] : nullptr);
     if (rc) return rc;
     if (ovl) CUDA_TRY(cudaStreamWaitEvent(h->st, h->evB[depth], 0));
-    else CUDA_TRY(gemm128(h, h->st, false, p, batch));
+    else CUDA_TRY(gemm128(h, h->st, false, p, batch, sel_batch));
     // 5b. Li21 = -Li22 * W2   A[i][k] = Li22[i][k] != 0 only for k <= i
     memset(&p, 0, sizeof(p));
     p.A = Li22; p.lda = ld; p.sA = sLi;
     p.B = W2; p.ldb = n1; p.sB = sW2;
     p.C = Li21; p.ldc = ld; p.sC = sLi;
     p.mt = n2 / 128; p.nt = n1 / 128; p.K = n2; p.alpha = -1.0; p.beta = 0.0; p.kflags = GEMM_KI_LE;
-    CUDA_TRY(gemm128(h, h->st, false, p, batch));
+    CUDA_TRY(gemm128(h, h->st, false, p, batch, sel_batch));
     return GPMPC_OK;
 }
 
@@ -370,26 +379,32 @@ static int launch_kbuild(gpmpc_handle_t h, const double* dHyp, const double* dJi
     return GPMPC_OK;
 }
 
-// alpha = Li^T (Li y) for `batch` consecutive local outputs starting at local index a
-static int launch_alpha(gpmpc_handle_t h, int a, int batch)
+// alpha = Li^T (Li y), log det K and y . alpha for `batch` factor slabs: L, Li at stride slab, targets y at stride sy,
+// tmp and alpha at stride Npad, row-chunk partials P at stride w2slab, res (2 per entry)
+static int launch_alpha_at(gpmpc_handle_t h, const double* L, const double* Li, const double* y, long long sy, double* tmp,
+                           double* P, double* alpha, double* res, int batch)
 {
     const int n = h->Npad;
-    const double* Li = h->dLi + (long long)a * slab(h);
     dim3 g1((n + 7) / 8, 1, batch);
-    trmv_lower_kernel<<<g1, 256, 0, h->st>>>(Li, n, slab(h), h->dY + (long long)a * n, n,
-                                              h->dTmp + (long long)a * n, n, n);
+    trmv_lower_kernel<<<g1, 256, 0, h->st>>>(Li, n, slab(h), y, sy, tmp, n, n);
     CUDA_TRY(cudaGetLastError());
-    // alpha = Li^T tmp in row chunks (partials in the W1 workspace, free outside the recursion), then
+    // alpha = Li^T tmp in row chunks (partials in a W1 workspace, free outside the recursion), then
     // one pass that sums the partials, takes log det and y . alpha
     const int nch = (n + TRT_ROWS - 1) / TRT_ROWS;
-    double* P = h->dW1 + (long long)a * w2slab(h);
     dim3 g2(n / 32, nch, batch);
-    trmv_lower_T_part_kernel<<<g2, 256, 0, h->st>>>(Li, n, slab(h), h->dTmp + (long long)a * n, n, P, w2slab(h), n);
+    trmv_lower_T_part_kernel<<<g2, 256, 0, h->st>>>(Li, n, slab(h), tmp, n, P, w2slab(h), n);
     CUDA_TRY(cudaGetLastError());
-    alpha_logdet_kernel<<<batch, 1024, 0, h->st>>>(P, w2slab(h), nch, h->dL + (long long)a * slab(h), n, slab(h),
-                                                   h->dY + (long long)a * n, n, h->dAlpha + (long long)a * n, n, n, h->dRes + 2 * a);
+    alpha_logdet_kernel<<<batch, 1024, 0, h->st>>>(P, w2slab(h), nch, L, n, slab(h), y, sy, alpha, n, n, res);
     CUDA_TRY(cudaGetLastError());
     return GPMPC_OK;
+}
+
+// alpha, log det and y . alpha of `batch` consecutive local outputs starting at local index a, from their factor slabs
+static int launch_alpha(gpmpc_handle_t h, int a, int batch)
+{
+    const long long n = h->Npad;
+    return launch_alpha_at(h, h->dL + a * slab(h), h->dLi + a * slab(h), h->dY + a * n, n, h->dTmp + a * n,
+                           h->dW1 + a * w2slab(h), h->dAlpha + a * n, h->dRes + 2 * a, batch);
 }
 
 // K(theta) -> L, Li for local output a with the reference's single jitter retry.
@@ -407,7 +422,7 @@ static int factor_one(gpmpc_handle_t h, int a, const double* dHyp, double jitter
             int rck = launch_kbuild(h, dHyp, h->dJit + a, L, 1, 0);
             if (rck) return rck;
         }
-        int rc = potrf_inv_rec(h, L, Li, slab(h), slab(h), h->dInfo + a, 0, h->Npad, 1);
+        int rc = potrf_inv_rec(h, L, Li, slab(h), slab(h), h->dInfo + a, 0, h->Npad, 1, 1, h->dW1, h->dW2);
         if (rc) return rc;
         int info = 0;
         CUDA_TRY(cudaMemcpyAsync(&info, h->dInfo + a, sizeof(int), cudaMemcpyDeviceToHost, h->st));
@@ -699,7 +714,7 @@ extern "C" int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info)
     CUDA_TRY(cudaMemsetAsync(h->dInfo, 0, nl * sizeof(int), h->st));
     rc = launch_kbuild(h, h->dHyp, h->dJit, h->dL, nl, 0);
     if (rc) return rc;
-    rc = potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, h->Npad, nl);
+    rc = potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, h->Npad, nl, nl, h->dW1, h->dW2);
     if (rc) return rc;
     std::vector<int> inf(nl, 0);
     CUDA_TRY(cudaMemcpyAsync(inf.data(), h->dInfo, nl * sizeof(int), cudaMemcpyDeviceToHost, h->st));
@@ -723,37 +738,56 @@ extern "C" int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info)
     return GPMPC_OK;
 }
 
-// K^-1 (lower) of local output al into dKinv:  U = Li^T,  K^-1 = U U^T
+// K^-1 (lower) of `batch` factors, slabs at stride slab:  U = Li^T,  K^-1 = U U^T.  The product's feed is the one of a
+// single slab, so every entry gets the bits compute_kinv gives it alone.
+static int kinv_at(gpmpc_handle_t h, const double* Li, double* U, double* Kinv, int batch)
+{
+    const int np = h->Npad;
+    dim3 g(np / 32, np / 32, batch), b(32, 8);
+    transpose_lower_kernel<<<g, b, 0, h->st>>>(Li, slab(h), U, slab(h), np, np / 32);
+    CUDA_TRY(cudaGetLastError());
+    GemmParams p;
+    memset(&p, 0, sizeof(p));
+    p.A = U; p.lda = np; p.sA = slab(h); p.B = U; p.ldb = np; p.sB = slab(h); p.C = Kinv; p.ldc = np; p.sC = slab(h);
+    p.mt = np / 128; p.nt = np / 128; p.K = np; p.alpha = 1.0; p.beta = 0.0;
+    p.kflags = GEMM_KI_GE | GEMM_KJ_GE; p.lower = 1;
+    CUDA_TRY(gemm128(h, h->st, true, p, batch, 1));
+    return GPMPC_OK;
+}
+
+// K^-1 (lower) of local output al into dKinv
 static int compute_kinv(gpmpc_handle_t h, int al)
 {
     int rc = ensure_nlml_scratch(h);
     if (rc) return rc;
-    const int np = h->Npad;
-    dim3 g(np / 32, np / 32), b(32, 8);
-    transpose_lower_kernel<<<g, b, 0, h->st>>>(h->dLi + (long long)al * slab(h), h->dU, np, np / 32);
+    return kinv_at(h, h->dLi + (long long)al * slab(h), h->dU, h->dKinv, 1);
+}
+
+// T(T+1)/2 tiles of the gradient's trace pass
+static inline int grad_tiles(gpmpc_handle_t h) { const int T = h->Npad / KB_TILE; return T * (T + 1) / 2; }
+
+// 1/2 tr((W - alpha alpha^T) dK/dtheta) for every hyper-parameter of `batch` entries: hyper rows at dHyp (stride Nx+2),
+// W = the lower triangle of the Kinv slabs (stride slab), alpha at stride Npad, tile partials in part (grad_tiles rows of
+// Nx+2 per entry), gradients into grad (stride Nx+2)
+static int launch_grad_at(gpmpc_handle_t h, const double* dHyp, const double* Kinv, const double* alpha, double* part,
+                          double* grad, int batch)
+{
+    const int nt = grad_tiles(h), m = h->Nx + 2;
+    const int smem = 2 * h->Nx * KB_TILE * 8;
+    CUDA_TRY(nxp_dispatch(h->Nx, [&](auto nxp) {
+        nlml_grad_kernel<decltype(nxp)::value><<<dim3(nt, batch), 256, smem, h->st>>>(
+            h->dXT, h->Npad, h->N, h->Nx, dHyp, m, Kinv, h->Npad, slab(h), alpha, h->Npad, part, (long long)nt * m);
+        return cudaGetLastError();
+    }));
+    nlml_grad_final_kernel<<<dim3(m, batch), 256, 0, h->st>>>(part, (long long)nt * m, nt, h->Nx, dHyp, m, grad);
     CUDA_TRY(cudaGetLastError());
-    GemmParams p;
-    memset(&p, 0, sizeof(p));
-    p.A = h->dU; p.lda = np; p.B = h->dU; p.ldb = np; p.C = h->dKinv; p.ldc = np;
-    p.mt = np / 128; p.nt = np / 128; p.K = np; p.alpha = 1.0; p.beta = 0.0;
-    p.kflags = GEMM_KI_GE | GEMM_KJ_GE; p.lower = 1;
-    CUDA_TRY(gemm128(h, h->st, true, p, 1));
     return GPMPC_OK;
 }
 
 // 1/2 tr((W - alpha alpha^T) dK/dtheta) for every hyper-parameter into dGrad, W = the lower triangle in dKinv
 static int launch_grad(gpmpc_handle_t h, const double* dHyp, const double* alpha)
 {
-    const int T = h->Npad / KB_TILE;
-    const int smem = 2 * h->Nx * KB_TILE * 8;
-    CUDA_TRY(nxp_dispatch(h->Nx, [&](auto nxp) {
-        nlml_grad_kernel<decltype(nxp)::value><<<T * (T + 1) / 2, 256, smem, h->st>>>(h->dXT, h->Npad, h->N, h->Nx, dHyp,
-                                                                                      h->dKinv, h->Npad, alpha, h->dGradPart);
-        return cudaGetLastError();
-    }));
-    nlml_grad_final_kernel<<<h->Nx + 2, 256, 0, h->st>>>(h->dGradPart, T * (T + 1) / 2, h->Nx, dHyp, h->dGrad);
-    CUDA_TRY(cudaGetLastError());
-    return GPMPC_OK;
+    return launch_grad_at(h, dHyp, h->dKinv, alpha, h->dGradPart, h->dGrad, 1);
 }
 
 // K(theta) -> L, Li, alpha of local output al for an objective at theta (hyper row in dHypTmp) with the jitter retry of
@@ -791,6 +825,133 @@ extern "C" int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* 
     }
     CUDA_TRY(cudaStreamSynchronize(h->st));
     *nll = 0.5 * res[1] + 0.5 * res[0];                      // optimize.py:355
+    return GPMPC_OK;
+}
+
+// gpmpc_nlml_batch scratch for a pass of c entries: the factor slabs dNbL, dNbLi, the recursion workspaces dNbW1, dNbW2
+// (W1 also holds the alpha partials), dNbV = [hyper rows (c, Nx+2) | jitter (c) | tmp (c, Npad) | alpha (c, Npad) |
+// res (c, 2) | gradient partials (c, grad_tiles, Nx+2) | gradients (c, Nx+2)], dNbInfo (c)
+static int nlml_batch_scratch(gpmpc_handle_t h, int c)
+{
+    const long long m = h->Nx + 2;
+    ENSURE(h->dNbL, c * slab(h));
+    ENSURE(h->dNbLi, c * slab(h));
+    ENSURE(h->dNbW1, c * w2slab(h));
+    ENSURE(h->dNbW2, c * w2slab(h));
+    ENSURE(h->dNbV, c * (m + 1 + 2LL * h->Npad + 2 + grad_tiles(h) * m + m));
+    ENSURE(h->dNbInfo, c);
+    return GPMPC_OK;
+}
+
+// NLML (and gradient) of local output al at the c hyper rows theta, each on its own slabs with gpmpc_nlml's arithmetic:
+// one K build, one recursion, one alpha pass and one gradient pass for the chunk, and factor_one's jitter retry for an
+// entry whose first factorisation fails.  Every GEMM takes the feed of a single slab, so no entry depends on c.
+static int nlml_batch_pass(gpmpc_handle_t h, int al, int c, const double* theta, double* nll, double* grad, int* status)
+{
+    const int m = h->Nx + 2, np = h->Npad, nt = grad_tiles(h);
+    double* hyp = h->dNbV;
+    double* jit = hyp + (long long)c * m;
+    double* tmp = jit + c;
+    double* alpha = tmp + (long long)c * np;
+    double* res = alpha + (long long)c * np;
+    double* part = res + 2 * c;
+    double* g = part + (long long)c * nt * m;
+    CUDA_TRY(cudaMemcpyAsync(hyp, theta, (size_t)c * m * 8, cudaMemcpyHostToDevice, h->st));
+    CUDA_TRY(cudaMemsetAsync(jit, 0, (size_t)c * 8, h->st));
+    CUDA_TRY(cudaMemsetAsync(h->dNbInfo, 0, (size_t)c * sizeof(int), h->st));
+    int rc = launch_kbuild(h, hyp, jit, h->dNbL, c, 0);
+    if (rc) return rc;
+    rc = potrf_inv_rec(h, h->dNbL, h->dNbLi, slab(h), slab(h), h->dNbInfo, 0, np, c, 1, h->dNbW1, h->dNbW2);
+    if (rc) return rc;
+    std::vector<int> info(c);
+    CUDA_TRY(cudaMemcpyAsync(info.data(), h->dNbInfo, (size_t)c * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    bool retried = false;
+    for (int s = 0; s < c; ++s) {
+        status[s] = GPMPC_OK;
+        if (!info[s]) continue;
+        // factor_one's second attempt, on this entry's slabs
+        const double jitter = 1e-8;
+        double* L = h->dNbL + s * slab(h);
+        CUDA_TRY(cudaMemcpyAsync(jit + s, &jitter, 8, cudaMemcpyHostToDevice, h->st));
+        CUDA_TRY(cudaMemsetAsync(h->dNbInfo + s, 0, sizeof(int), h->st));
+        rc = launch_kbuild(h, hyp + (long long)s * m, jit + s, L, 1, 0);
+        if (rc) return rc;
+        rc = potrf_inv_rec(h, L, h->dNbLi + s * slab(h), slab(h), slab(h), h->dNbInfo + s, 0, np, 1, 1,
+                           h->dNbW1 + s * w2slab(h), h->dNbW2 + s * w2slab(h));
+        if (rc) return rc;
+        status[s] = 1;
+        retried = true;
+    }
+    if (retried) {
+        CUDA_TRY(cudaMemcpyAsync(info.data(), h->dNbInfo, (size_t)c * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+        CUDA_TRY(cudaStreamSynchronize(h->st));
+        for (int s = 0; s < c; ++s) if (status[s] == 1 && info[s]) status[s] = GPMPC_ERR_NOTPD;
+    }
+    // a failed entry runs on with its slabs as they are: the passes below are per entry, so it touches no other
+    rc = launch_alpha_at(h, h->dNbL, h->dNbLi, h->dY + (long long)al * np, 0, tmp, h->dNbW1, alpha, res, c);
+    if (rc) return rc;
+    std::vector<double> hres(2 * c);
+    CUDA_TRY(cudaMemcpyAsync(hres.data(), res, (size_t)c * 16, cudaMemcpyDeviceToHost, h->st));
+    if (grad) {
+        // U = Li^T into the L slab (log det has been read from it), K^-1 = U U^T into the Li slab (alpha is done)
+        rc = kinv_at(h, h->dNbLi, h->dNbL, h->dNbLi, c);
+        if (rc) return rc;
+        rc = launch_grad_at(h, hyp, h->dNbLi, alpha, part, g, c);
+        if (rc) return rc;
+        CUDA_TRY(cudaMemcpyAsync(grad, g, (size_t)c * m * 8, cudaMemcpyDeviceToHost, h->st));
+    }
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    for (int s = 0; s < c; ++s) {
+        if (status[s] == GPMPC_ERR_NOTPD) {
+            nll[s] = NAN;
+            if (grad) for (int q = 0; q < m; ++q) grad[(size_t)s * m + q] = NAN;
+        } else {
+            nll[s] = 0.5 * hres[2 * s + 1] + 0.5 * hres[2 * s];   // gpmpc_nlml's sum
+        }
+    }
+    return GPMPC_OK;
+}
+
+static void nlml_batch_release(gpmpc_handle_t h)
+{
+    cudaStreamSynchronize(h->st);
+    h->dNbL.release(); h->dNbLi.release(); h->dNbW1.release(); h->dNbW2.release(); h->dNbV.release(); h->dNbInfo.release();
+}
+
+extern "C" int gpmpc_nlml_batch(gpmpc_handle_t h, int a, int S, const double* theta, double* nll, double* grad,
+                                int* status)
+{
+    if (!h) return GPMPC_ERR_ARG;
+    if (!theta || !nll || !status || S < 1) { set_error(h, "gpmpc_nlml_batch: NULL pointer or S < 1"); return GPMPC_ERR_ARG; }
+    int rc = model_guard(h, __func__, NEED_DATA);
+    if (rc) return rc;
+    const int al = local_index(h, a);
+    if (al < 0) return GPMPC_ERR_ARG;
+    const int m = h->Nx + 2;
+    for (int s = 0; s < S; ++s)
+        for (int d = 0; d < h->Nx; ++d)
+            if (theta[(size_t)s * m + d] == 0.0) {
+                set_error(h, "gpmpc_nlml_batch: zero length scale in row %d", s);
+                return GPMPC_ERR_ARG;
+            }
+    NvtxRange nvtx_r("gpmpc.nlml_batch");
+    // results do not depend on the pass size, so a pass that does not fit is halved
+    int pass = h->opt_nlml_batch_max > 0 ? std::min(S, h->opt_nlml_batch_max) : S;
+    for (int s0 = 0; s0 < S;) {
+        const int c = std::min(pass, S - s0);
+        rc = nlml_batch_scratch(h, c);
+        if (rc) {
+            const bool oom = cudaGetLastError() == cudaErrorMemoryAllocation;
+            nlml_batch_release(h);
+            if (!oom || c == 1) return rc;
+            pass = c / 2;
+            continue;
+        }
+        rc = nlml_batch_pass(h, al, c, theta + (size_t)s0 * m, nll + s0, grad ? grad + (size_t)s0 * m : nullptr, status + s0);
+        if (rc) return rc;
+        s0 += c;
+    }
     return GPMPC_OK;
 }
 
@@ -887,7 +1048,7 @@ extern "C" int gpmpc_loo_nlpp(gpmpc_handle_t h, int a, const double* theta, doub
         memset(&p, 0, sizeof(p));
         p.A = h->dU; p.lda = np; p.B = h->dU; p.ldb = np; p.C = h->dKinv; p.ldc = np;
         p.mt = np / 128; p.nt = np / 128; p.K = np; p.alpha = 1.0; p.beta = 0.0; p.lower = 1;
-        CUDA_TRY(gemm128(h, h->st, true, p, 1));
+        CUDA_TRY(gemm128(h, h->st, true, p, 1, 1));
         loo_w_kernel<<<dim3((N + 255) / 256, N), 256, 0, h->st>>>(h->dKinv, np, o.b, alpha, N);
         CUDA_TRY(cudaGetLastError());
         // the trace pass with W in place of K^-1 and alpha = 0: 1/2 tr(W dK/dtheta), doubled on the host (exact)
@@ -945,6 +1106,10 @@ extern "C" int gpmpc_set_option(gpmpc_handle_t h, const char* name, double value
     if (!strcmp(name, "peer_timeout_s")) { h->opt_peer_timeout_s = value > 0.0 ? value : 60.0; return GPMPC_OK; }
     if (!strcmp(name, "small_tiles")) { h->opt_small_tiles = (int)value; return GPMPC_OK; }
     if (!strcmp(name, "peer")) { h->opt_peer = value != 0.0; return GPMPC_OK; }
+    if (!strcmp(name, "nlml_batch_max")) {     // entries per gpmpc_nlml_batch pass (0 = all): a cap on its scratch
+        if (!(value >= 0.0 && value <= 1e9)) { set_error(h, "nlml_batch_max must be >= 0"); return GPMPC_ERR_ARG; }
+        h->opt_nlml_batch_max = (int)value; return GPMPC_OK;
+    }
     set_error(h, "unknown option %s", name);
     return GPMPC_ERR_ARG;
 }
@@ -1572,7 +1737,7 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
             gp.C = h->dU; gp.ldc = np;
             gp.mt = np / 128; gp.nt = np / 128; gp.K = np; gp.alpha = 1.0; gp.beta = 0.0;
             gp.kflags = GEMM_KI_LE; gp.lower = 1;
-            CUDA_TRY(gemm128(h, h->st, true, gp, 1));
+            CUDA_TRY(gemm128(h, h->st, true, gp, 1, 1));
             em_trdot_kernel<<<ntr, 256, 0, h->st>>>(h->dU, h->dLi + (long long)a * slab(h), np, h->dEmTr + (long long)a * ntr);
             CUDA_TRY(cudaGetLastError());
         }
@@ -2134,7 +2299,8 @@ static int derivs_prepare(gpmpc_handle_t h, int H, bool second, DerivSlabs* s)
     if (!h->u_valid) {                 // U = Linv^T (upper): the K-contiguous operand of beta = Linv^T v
         dim3 g(np / 32, np / 32), b(32, 8);
         for (int a = 0; a < h->nloc; ++a) {
-            transpose_lower_kernel<<<g, b, 0, h->st>>>(h->dLi + (long long)a * slab(h), h->dUall + (long long)a * slab(h), np, np / 32);
+            transpose_lower_kernel<<<g, b, 0, h->st>>>(h->dLi + (long long)a * slab(h), 0, h->dUall + (long long)a * slab(h), 0, np,
+                                                       np / 32);
             CUDA_TRY(cudaGetLastError());
         }
         h->u_valid = true;
@@ -2771,7 +2937,7 @@ extern "C" int gpmpc_profile_leaf(gpmpc_handle_t h, double* out15)
     CUDA_TRY(cudaMemcpyToSymbol(d_leaf_prof, &d.p, sizeof(d.p)));
     for (int rep = 0; rep < 2 && rc == GPMPC_OK; ++rep) {           // second run: warm instruction cache
         rc = launch_kbuild(h, h->dHyp, h->dJit, h->dL, 1, 0);
-        if (rc == GPMPC_OK) rc = potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, 128, 1);
+        if (rc == GPMPC_OK) rc = potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, 128, 1, 1, h->dW1, h->dW2);
     }
     cudaStreamSynchronize(h->st);
     long long hst[16];
@@ -2807,14 +2973,14 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
             p.A = h->dW1; p.lda = n1; p.B = h->dW1; p.ldb = n1;
             p.C = h->dLi; p.ldc = np; p.Cin = h->dLi; p.ldcin = np;
             p.mt = n2 / 128; p.nt = n2 / 128; p.K = n1; p.alpha = -1e-30; p.beta = 1.0; p.lower = 1;
-            cudaError_t e = gemm128(h, h->st, true, p, 1);
+            cudaError_t e = gemm128(h, h->st, true, p, 1, 1);
             if (e != cudaSuccess) { set_error(h, "profile syrk: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
             return GPMPC_OK;
         }
         case GPMPC_PROF_FACTORIZE: {
             int r = launch_kbuild(h, h->dHyp, h->dJit, h->dL, 1, 0);
             if (r) return r;
-            return potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, np, 1);
+            return potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, np, 1, 1, h->dW1, h->dW2);
         }
         case GPMPC_PROF_TRIGEMM: return tri_product(h, h->dKST, h->dLi, Hc, nullptr);
         case GPMPC_PROF_KS: {             // the ks / mean / Jacobian partial kernel alone (Z = the last batch's inputs)

@@ -494,13 +494,16 @@ __global__ void copy2d_kernel(const double* __restrict__ src, int lds, long long
                 reinterpret_cast<const double2*>(s + (long long)r * lds)[c];
 }
 
-// U = Linv^T for the lower tiles of Linv (32x32 smem transpose); U's strictly lower
-// tiles are never written and stay zero from allocation.
-__global__ void transpose_lower_kernel(const double* __restrict__ Li, double* __restrict__ U, int ld, int nt32)
+// U = Linv^T for the lower tiles of Linv (32x32 smem transpose), one slab per blockIdx.z (strides sLi, sU); U's strictly
+// lower tiles are written as zeros, so U is exactly upper-triangular whatever the slab held before.
+__global__ void transpose_lower_kernel(const double* __restrict__ Li, long long sLi, double* __restrict__ U, long long sU,
+                                       int ld, int nt32)
 {
     __shared__ double tile[32][33];
     const int bi = blockIdx.y, bj = blockIdx.x;
     if (bj > bi) return;
+    Li += (long long)blockIdx.z * sLi;
+    U += (long long)blockIdx.z * sU;
     const int tx = threadIdx.x, ty = threadIdx.y;   // 32 x 8
     for (int r = ty; r < 32; r += 8) tile[r][tx] = Li[(long long)(bi * 32 + r) * ld + bj * 32 + tx];
     __syncthreads();
@@ -768,14 +771,19 @@ ks_tile_kernel(const double* __restrict__ XT, int ldx, int N, int Nx,
 //   dNLL/dtheta = 1/2 tr((K^-1 - alpha alpha^T) dK/dtheta)   (R&W eq. 5.9; objective of
 //   optimize.py:322-356).  theta = [ell.., sf, sn] are standard deviations (q1):
 //   dK/dell_d = Kf (x_id-x_jd)^2/ell_d^3,  dK/dsf = 2 Kf/sf,  dK/dsn = 2 sn I.
-//   One CTA per 64x64 lower tile of K^-1; partial sums [tile][Nx+2].
+//   One CTA per 64x64 lower tile of K^-1; partial sums [tile][Nx+2].  blockIdx.y selects one
+//   batch entry: its hyper row, K^-1 slab, alpha and partials at the strides shp, sK, sal, sp.
 // ---------------------------------------------------------------------------------------
 template <int NXP>
 __global__ void __launch_bounds__(256)
 nlml_grad_kernel(const double* __restrict__ XT, int ldx, int N, int Nx,
-                 const double* __restrict__ hp, const double* __restrict__ Kinv, int ld,
-                 const double* __restrict__ alpha, double* __restrict__ partial)
+                 const double* __restrict__ hp, long long shp, const double* __restrict__ Kinv, int ld, long long sK,
+                 const double* __restrict__ alpha, long long sal, double* __restrict__ partial, long long sp)
 {
+    hp += blockIdx.y * shp;
+    Kinv += blockIdx.y * sK;
+    alpha += blockIdx.y * sal;
+    partial += blockIdx.y * sp;
     extern __shared__ double sm[];
     double* Xi = sm; double* Xj = sm + Nx * KB_TILE;
     __shared__ double red[8][NXP + 2];
@@ -841,12 +849,16 @@ nlml_grad_kernel(const double* __restrict__ XT, int ldx, int N, int Nx,
     }
 }
 
-// deterministic column sums of partial[ntile][m] -> grad[m], with the theta scalings
+// deterministic column sums of partial[ntile][m] -> grad[m], with the theta scalings; blockIdx.y selects one batch
+// entry (partials at stride sp, hyper row at stride shp, gradient at stride Nx+2)
 __global__ void __launch_bounds__(256)
-nlml_grad_final_kernel(const double* __restrict__ partial, int ntile, int Nx,
-                       const double* __restrict__ hp, double* __restrict__ grad)
+nlml_grad_final_kernel(const double* __restrict__ partial, long long sp, int ntile, int Nx,
+                       const double* __restrict__ hp, long long shp, double* __restrict__ grad)
 {
     __shared__ double red[8];
+    partial += blockIdx.y * sp;
+    hp += blockIdx.y * shp;
+    grad += blockIdx.y * (Nx + 2);
     const int q = blockIdx.x;
     double s = 0.0;
     for (int t = threadIdx.x; t < ntile; t += 256) s += partial[(long long)t * (Nx + 2) + q];

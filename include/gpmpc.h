@@ -111,6 +111,21 @@ int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info);
  * (optimize.py:466-467).  Invalidates the factorisation of output a. */
 int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* nll, double* grad);
 
+/* gpmpc_nlml at S hyper-parameter points of global output a in one pass.
+ *   theta  (S, Nx+2)  host, rows as gpmpc_nlml's theta
+ *   nll    (S)        host
+ *   grad   (S, Nx+2)  host or NULL
+ *   status (S)        host: 0 ok, 1 ok after the 1e-8 jitter retry, GPMPC_ERR_NOTPD (nll and grad rows NaN)
+ * Entry s is bit-identical to gpmpc_nlml(h, a, theta_s, ...) on the same handle, whatever S, the order of the rows and
+ * the pass size.  Entries are independent: a NOTPD entry does not change the others, and the call returns GPMPC_OK.
+ * Unlike gpmpc_nlml it leaves the factorisation valid: its slabs are its own scratch.  A pass covers
+ * min(S, option "nlml_batch_max") entries (0: all S) and holds, per entry, two Npad^2 slabs, the recursion's two
+ * workspaces (about Npad^2 / 3 each) and O(Npad) vectors, kept with the handle; a pass that cannot be allocated is
+ * halved, down to one entry.
+ *   GPMPC_ERR_ARG: S < 1, a NULL theta, nll or status, a zero length scale in any row, an output the handle does not
+ *   own.  GPMPC_ERR_STATE: no data.  Every check runs before any work. */
+int gpmpc_nlml_batch(gpmpc_handle_t h, int a, int S, const double* theta, double* nll, double* grad, int* status);
+
 /* Leave-one-out cross-validation on the current factorisation of every OWNED output (Rasmussen & Williams
  * eqs. 5.10-5.12): each training point predicted from the other N-1.  With C = K^-1, alpha = C y (y the target the
  * handle factorised, the residual y - m(X) under a prior mean) and c_i = C_ii, the column norms of L^-1:
@@ -318,7 +333,8 @@ int gpmpc_get(gpmpc_handle_t h, int what, int a, double* dst);
  * the stored factor), "predict_ctas" (persistent grid of the stream-K predict product,
  * 0 = two CTAs per SM), "peer" (0/1), "peer_timeout_s" (consumer wait for a peer's flag),
  * "small_tiles" (batched 128x64 tile count of a factorisation GEMM below which it runs on
- * 64x32 tiles; default 4 per SM).  Any other name returns GPMPC_ERR_ARG. */
+ * 64x32 tiles; default 4 per SM), "nlml_batch_max" (entries per gpmpc_nlml_batch pass, a cap
+ * on its scratch; 0 = all, the default).  Any other name returns GPMPC_ERR_ARG. */
 int gpmpc_set_option(gpmpc_handle_t h, const char* name, double value);
 
 /* Multi-GPU: one process per GPU.  Rank 0 calls gpmpc_comm_unique_id and ships the
