@@ -375,11 +375,13 @@ def _maha(a1, b1, Q1):
             - 2 * aQ @ b1.T)
 
 
-def gp_exact_moment(invK, X, Y, hyper, inputmean, inputcov, extended=False):
+def gp_exact_moment(invK, X, Y, hyper, inputmean, inputcov, extended=False, beta=None):
     """``gp_exact_moment`` ``gp_functions.py:344-418``, one test point.
 
     ``extended=True`` evaluates the N x N sums (which cancel ~6-7 digits: beta beta^T vs
     invK) in numpy longdouble -- a higher-precision yardstick for judging fp64 noise.
+    ``beta`` (Ny, N), e.g. an engine's own alpha, replaces the reference's ``invK @ Y`` (the
+    default), so a comparison can separate the evaluation's error from alpha's conditioning.
 
     Quirks kept: hyper=log(hyper) then exponentiated (:367); det through the
     product of the QR diagonal (:378-380) -- restated with slogdet's value
@@ -392,6 +394,7 @@ def gp_exact_moment(invK, X, Y, hyper, inputmean, inputcov, extended=False):
     hyper = np.atleast_2d(np.asarray(hyper, dtype=np.float64))
     inputmean = np.asarray(inputmean, dtype=np.float64).reshape(1, -1)
     inputcov = np.asarray(inputcov, dtype=np.float64)
+    beta_in = None if beta is None else np.asarray(beta, dtype=np.float64)
     lh = np.log(hyper)
     Ny = len(invK)
     N, Nx = X.shape
@@ -401,7 +404,7 @@ def gp_exact_moment(invK, X, Y, hyper, inputmean, inputcov, extended=False):
     det = np.linalg.det
     eye = np.eye(Nx)
     for a in range(Ny):
-        beta[:, a] = invK[a] @ Y[:, a]
+        beta[:, a] = invK[a] @ Y[:, a] if beta_in is None else beta_in[a]
         iLambda = np.diag(np.exp(-2 * lh[a, :Nx]))
         R = inputcov + np.diag(np.exp(2 * lh[a, :Nx]))
         iR = iLambda @ (eye - np.linalg.solve(eye + inputcov @ iLambda, inputcov @ iLambda))

@@ -1,5 +1,6 @@
 """First derivatives of 'EM' exact moment matching without a GPU: the closed-form oracle against fourth-order
-differences of the extended-precision EM formula, and its limits as Sigma -> 0."""
+differences of the extended-precision EM formula, its limits as Sigma -> 0, and its mean and cov against the
+extended-precision formula at large input covariances."""
 import numpy as np
 import pytest
 from scipy.linalg import cho_solve
@@ -8,6 +9,7 @@ from oracle import em_grad_oracle as emo
 from oracle import gp_oracle as orc
 from oracle import hess_oracle as hor
 from tests._util import load_fixture, relinf
+from tests.test_em_shapes_gpu import sigmas
 
 
 def _problem(case):
@@ -37,6 +39,28 @@ def test_em_grad_closed_forms_vs_fourth_order_differences(case):
     assert relinf(emo.sym_pair(cl['dcov_dSigma']), fd['dcov_dSigma']) < 1e-5
     mean, cov = orc.gp_exact_moment(invK, X, Y, hyper, Z[0], Sigma, extended=True)
     assert relinf(cl['mean'][0], mean) < 1e-10 and relinf(cl['cov'][0], cov) < 1e-4
+
+
+@pytest.mark.parametrize('scale', ['0.1', '1'])
+@pytest.mark.parametrize('Nx', [6, 32])
+def test_plain_and_regrouped_em_moments_agree(Nx, scale):
+    """The two EM yardsticks of the GPU tests, written independently: the reference's plain formula with its N x N sums in
+    long double (gp_exact_moment, extended) and the regrouped closed form (em_grad_closed: backbone through the factor,
+    the cross term as written), on one alpha and factor at sn = 0.3, N = 300, Sigma = 0.1 Lambda (correlated) and Lambda.
+    They agree to relinf <= 3e-14 on the mean and the covariance."""
+    N, Ny = 300, 2
+    p = orc.synthetic_problem(N, Nx, Ny, config_id=700 + Nx, H=2)
+    X, Y, hyper = p['X'], p['Y'], p['hyper'].copy()
+    hyper[:, Nx + 1] = 0.3
+    post = orc.postfit(X, Y, hyper, lapack_general_solve=False)
+    chol = post['chol']
+    invK = np.stack([cho_solve((chol[a], True), np.eye(N)) for a in range(Ny)])
+    alpha = np.stack([cho_solve((chol[a], True), Y[:, a]) for a in range(Ny)])
+    S = sigmas(hyper, Nx)[scale]
+    cl = emo.em_grad_closed(X, hyper, alpha, chol, p['Z'], S)
+    for h in range(p['Z'].shape[0]):
+        mean, cov = orc.gp_exact_moment(invK, X, Y, hyper, p['Z'][h], S, extended=True, beta=alpha)
+        assert relinf(cl['mean'][h], mean) < 3e-14 and relinf(cl['cov'][h], cov) < 3e-14, h
 
 
 def test_em_grad_limits_as_sigma_vanishes():

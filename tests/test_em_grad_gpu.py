@@ -1,15 +1,18 @@
-"""gpmpc_predict_em_grad and GP.predict_batch_grad('EM') on the GPU: 'EM' first derivatives against the closed-form
-oracle fed with the engine's own alpha and factor, against fourth-order differences of the engine's own EM
-prediction, bit-identity of the forward outputs with gpmpc_predict(EM), exact symmetry, reproducibility, the
-K^-1 cache after append and the argument checks."""
+"""gpmpc_predict_em_grad and GP.predict_batch_grad('EM') on the GPU: 'EM' first derivatives and the forward mean and cov
+against the closed-form oracle fed with the engine's own alpha and factor, against fourth-order differences of the engine's
+own EM prediction, bit-identity of the forward outputs with gpmpc_predict(EM), exact symmetry, reproducibility, the K^-1
+cache after append and the argument checks."""
 import ctypes as C
 
 import numpy as np
 import pytest
+from scipy.linalg import cho_solve
 
 from oracle import em_grad_oracle as emo
 from oracle import gp_oracle as orc
 from tests._util import load_fixture, load_golden, relinf
+from tests.test_dispatch_gpu import _require
+from tests.test_em_shapes_gpu import CASES, check_case, em_errors, em_problem, em_terms, sigmas, tma_on_device
 
 pytestmark = pytest.mark.gpu
 
@@ -31,6 +34,12 @@ def _fit(X, Y, hyper, **kw):
 
 
 def _case(case):
+    """X, Y, hyper, Z, Sigma and the handle's capacity of a case; '<shape>_s<scale>' is a case of test_em_shapes_gpu at
+    the input covariance of that scale (0.1 Lambda correlated, or Lambda)."""
+    if '_s' in case:
+        name, scale = case.split('_s')
+        X, Y, hyper, Z = em_problem(name)
+        return X, Y, hyper, Z[:1] if name == 'tma' else Z[:2], sigmas(hyper, X.shape[1])[scale], CASES[name][3]
     if case.startswith('tank'):
         m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
         rng = np.random.default_rng(5)
@@ -41,13 +50,13 @@ def _case(case):
             Sigma = 0.1 * np.min(hyper[:, :Nx] ** 2) * (np.eye(Nx) + 0.1 * (A @ A.T) / np.abs(A @ A.T).max())
         if case == 'tank_pp':
             Sigma = np.stack([Sigma * (1 + 0.1 * h) for h in range(Z.shape[0])])
-        return X, Y, hyper, Z, Sigma
+        return X, Y, hyper, Z, Sigma, None
     N, Nx, Ny, H = {'syn1000': (1000, 8, 4, 3), 'syn300': (300, 17, 2, 2), 'syn12': (600, 12, 3, 3)}[case]
     p = orc.synthetic_problem(N, Nx, Ny, config_id=N + Nx, H=H)
     hyper = p['hyper']
     if case == 'syn12':                   # well-conditioned (sn = 0.3): alpha and K^-1 carry no conditioning error
         hyper = hyper.copy(); hyper[:, Nx + 1] = 0.3
-    return p['X'], p['Y'], hyper, p['Z'], p['Sigma']
+    return p['X'], p['Y'], hyper, p['Z'], p['Sigma'], None
 
 
 def _engine_factor(eng, Ny):
@@ -56,30 +65,42 @@ def _engine_factor(eng, Ny):
             np.stack([eng.get(L.GET_CHOL, a) for a in range(Ny)]))
 
 
-# (dmean, dcov) bars against the closed form; syn12 is well-conditioned, measured dmean 5.7e-15, dcov 2.8e-13 on an
-# H100 SXM at 700 W
-GRAD_TOL = {'syn12': (1e-13, 3e-12)}
+def forward_errors(o, ref, X, hyper, alpha, chol, Z, Sigma):
+    """Largest errors of the engine's EM mean and cov against the closed form's over the points, normalised by the sums of
+    |terms| (test_em_shapes_gpu.em_terms) with K^-1 from the engine's factor."""
+    N = X.shape[0]
+    kinv = np.stack([cho_solve((c, True), np.eye(N), check_finite=False) for c in chol])
+    kinv = 0.5 * (kinv + np.swapaxes(kinv, 1, 2))
+    Sg = emo._sigmas(Sigma, Z.shape[0], X.shape[1])
+    e = dict(mean=0.0, cov=0.0)
+    for h in range(Z.shape[0]):
+        eh = em_errors(o['mean'][h], o['cov'][h], (ref['mean'][h], ref['cov'][h]), em_terms(X, hyper, alpha, kinv, Z[h], Sg[h]))
+        e = {k: max(e[k], eh[k]) for k in e}
+    return e
 
 
-@pytest.mark.parametrize('case', ['tank', 'tank_pp', 'tank_large', 'syn1000', 'syn300', 'syn12'])
-def test_em_grad_vs_closed_oracle(case):
-    """syn1000: Nx = 8, N ~ 1000 (16 tiles); syn300: Nx = 17, the 32 bucket; syn12: Nx = 12, the 16 bucket of em_prep,
-    em_moments and em_grad_pair; tank_pp: one Sigma per point."""
-    X, Y, hyper, Z, Sigma = _case(case)
+NEW_SHAPES = [n + s for n in ('nx1', 'nx32', 'tma', 'ny9', 'reserved') for s in ('_s0.1', '_s1')]
+# (dmean, dcov) bars against the closed form: the fixtures and the sn = 1e-2 synthetic cases carry cond(K) eps; the
+# well-conditioned cases (sn = 0.3) were measured on an H100 SXM at 700 W: syn12 dmean 5.7e-15, dcov 2.8e-13; the
+# shapes of test_em_shapes_gpu dmean <= 1.5e-14 (nx32), dcov <= 1.6e-13 (ny9 at Sigma = Lambda)
+GRAD_TOL = dict({'syn12': (1e-13, 3e-12)}, **{c: (1e-13, 3e-12) for c in NEW_SHAPES})
+# (mean, cov) bar against the closed form's, normalised by the sums of |terms|; measured on an H100 SXM at 700 W over every
+# case: mean <= 1.7e-16 (nx32), cov <= 4.5e-18
+FWD_TOL = (1e-15, 1e-15)
+
+
+def em_grad_errors(case):
+    """The engine's predict_em_grad on a case against em_grad_closed on the engine's own alpha and factor: relative errors
+    of the four derivatives and normalised errors of mean and cov, after the bit-level checks."""
+    X, Y, hyper, Z, Sigma, cap = _case(case)
     Ny = Y.shape[1]
-    eng = _fit(X, Y, hyper)
+    eng = _fit(X, Y, hyper, capacity=cap)
     L = _L()
     o = eng.predict_em_grad(Z, Sigma)
     mean, var, cov, _ = eng.predict(Z, Sigma, L.METHOD_EM, want_jac=False)
     assert np.array_equal(o['mean'], mean) and np.array_equal(o['var'], var) and np.array_equal(o['cov'], cov)
     for k in DERIV:
         assert np.all(np.isfinite(o[k])), k
-    alpha, chol = _engine_factor(eng, Ny)
-    ref = emo.em_grad_closed(X, hyper, alpha, chol, Z, Sigma)
-    errs = {k: relinf(o[k], ref[k]) for k in DERIV}
-    tm, tc = GRAD_TOL.get(case, (1e-6, 1e-5))
-    assert errs['dmean_dz'] < tm and errs['dmean_dSigma'] < tm, errs
-    assert errs['dcov_dz'] < tc and errs['dcov_dSigma'] < tc, errs
     assert np.array_equal(o['dmean_dSigma'], np.swapaxes(o['dmean_dSigma'], 2, 3))
     assert np.array_equal(o['dcov_dSigma'], np.swapaxes(o['dcov_dSigma'], 3, 4))
     assert np.array_equal(o['dcov_dSigma'], np.swapaxes(o['dcov_dSigma'], 1, 2))
@@ -87,14 +108,37 @@ def test_em_grad_vs_closed_oracle(case):
     o2 = eng.predict_em_grad(Z, Sigma)
     for k in o:
         assert np.array_equal(o[k], o2[k]), k
+    alpha, chol = _engine_factor(eng, Ny)
     eng.close()
+    ref = emo.em_grad_closed(X, hyper, alpha, chol, Z, Sigma)
+    errs = {k: relinf(o[k], ref[k]) for k in DERIV}
+    errs.update(forward_errors(o, ref, X, hyper, alpha, chol, Z, Sigma))
+    return errs
+
+
+@pytest.mark.parametrize('case', ['tank', 'tank_pp', 'tank_large', 'syn1000', 'syn300', 'syn12'] + NEW_SHAPES)
+def test_em_grad_vs_closed_oracle(case):
+    """syn1000: Nx = 8, N ~ 1000 (16 tiles); syn300: Nx = 17, the 32 bucket; syn12: Nx = 12, the 16 bucket of em_prep,
+    em_moments and em_grad_pair; tank_pp: one Sigma per point.  The shapes of test_em_shapes_gpu at Sigma = 0.1 Lambda and
+    Lambda: nx1, nx32 (em_grad_pair_kernel<32>'s opt-in shared memory at its largest), tma (em_moments, em_bb_rows and
+    trmv_lower_T on the 3072 pad), ny9 (nine outputs' records) and reserved (an identity tail of L^-1)."""
+    if case.startswith('tma'):
+        _require(tma_on_device(), 'the TMA feed')
+    errs = em_grad_errors(case)
+    tm, tc = GRAD_TOL.get(case, (1e-6, 1e-5))
+    assert errs['dmean_dz'] < tm and errs['dmean_dSigma'] < tm, errs
+    assert errs['dcov_dz'] < tc and errs['dcov_dSigma'] < tc, errs
+    fm, fc = FWD_TOL
+    assert errs['mean'] < fm and errs['cov'] < fc, errs
 
 
 def test_em_forward_nxp16_vs_exact_moment():
     """The forward 'EM' moments at Nx = 12 (em_prep / em_moments<16>) on the well-conditioned syn12 model against the
     fp64 restatement gp_exact_moment with postfit's K^-1.  Measured on an H100 SXM at 700 W: mean 1.2e-13, cov
-    3.9e-11 (the restatement's own cancellation between beta beta^T and K^-1)."""
-    X, Y, hyper, Z, Sigma = _case('syn12')
+    3.9e-11 (the restatement's own cancellation between beta beta^T and K^-1).  Then the nx12 case of test_em_shapes_gpu
+    (N = 600, Ny = 3) against the long-double formula on the engine's alpha and factor at Sigma = 1e-5 Lambda, 0.1 Lambda
+    and Lambda, under that file's bars (measured: mean 2.7e-17, cov 1.2e-18 of the sums of |terms|)."""
+    X, Y, hyper, Z, Sigma, _ = _case('syn12')
     eng = _fit(X, Y, hyper)
     mean, _, cov, _ = eng.predict(Z, Sigma, _L().METHOD_EM, want_jac=False)
     eng.close()
@@ -102,6 +146,7 @@ def test_em_forward_nxp16_vs_exact_moment():
     for h in range(Z.shape[0]):
         mo, co = orc.gp_exact_moment(post['invK'], X, Y, hyper, Z[h], Sigma)
         assert relinf(mean[h], mo) < 1e-12 and relinf(cov[h], co) < 1e-9, h
+    check_case('nx12')
 
 
 @pytest.mark.parametrize('case,tol', [('tank', 1e-5), ('car', 1e-3)])
