@@ -113,6 +113,102 @@ def predict_hess(X, hyper, alpha, chol, Z, Sigma, method='TA'):
     return out
 
 
+def derivs_core_ld(X, hyper, alpha, linv, Z, absolute=False):
+    """The Sigma-free part of ``predict_derivs_ld``: dict(mean, var (H,Ny), J (H,Ny,Nx), dvar_dz (H,Ny,Nx),
+    hess (H,Ny,Nx,Nx), d2var_dz2 (H,Ny,Nx,Nx), d3mean_dz3 (H,Ny,Nx,Nx,Nx)) in np.longdouble, on the path of the
+    kernels: ks by direct differences, v = L^-1 ks, beta = L^-T v and V_d = L^-1 d_d ks as products with ``linv``
+    (Ny,N,N, lower, as GET_LINV returns it), k^T K^-1 k = |v|^2.  ``absolute``: the sums of |terms| of every output
+    (see ``predict_derivs_ld``)."""
+    ld = np.longdouble
+    X = np.asarray(X, dtype=ld)
+    Z = np.atleast_2d(np.asarray(Z, dtype=ld))
+    hyper = np.atleast_2d(np.asarray(hyper, dtype=ld))
+    H, Nx = Z.shape
+    Ny = hyper.shape[0]
+    sg = 1 if absolute else -1                                    # the sign of every subtraction
+    out = {k: np.zeros(s, dtype=ld) for k, s in (('mean', (H, Ny)), ('var', (H, Ny)), ('J', (H, Ny, Nx)),
+                                                 ('dvar_dz', (H, Ny, Nx)), ('hess', (H, Ny, Nx, Nx)),
+                                                 ('d2var_dz2', (H, Ny, Nx, Nx)), ('d3mean_dz3', (H, Ny, Nx, Nx, Nx)))}
+    eye = np.eye(Nx, dtype=ld)
+    for a in range(Ny):
+        ell = hyper[a, :Nx]
+        sf2 = hyper[a, Nx] ** 2
+        il2 = 1 / ell ** 2
+        Li = np.asarray(linv[a], dtype=ld)
+        al = np.asarray(alpha[a], dtype=ld)
+        if absolute:
+            Li, al = np.abs(Li), np.abs(al)
+        diff = (X[None, :, :] - Z[:, None, :]) / ell                 # (H,N,Nx)
+        ks = sf2 * np.exp(-np.sum(diff * diff, axis=2) / 2)          # (H,N)
+        s = (X[None, :, :] - Z[:, None, :]) * il2                    # (H,N,Nx)
+        if absolute:
+            s = np.abs(s)
+        v = Li @ ks.T                                                # (N,H)
+        beta = Li.T @ v
+        q = np.sum(v * v, axis=0)                                    # k^T K^-1 k
+        wa = al[None, :] * ks                                        # (H,N)
+        wb = beta.T * ks
+        mean = wa.sum(1)
+        J = np.einsum('hi,hid->hd', wa, s)
+        out['mean'][:, a] = mean
+        out['var'][:, a] = sf2 + sg * q
+        out['J'][:, a] = J
+        out['dvar_dz'][:, a] = 2 * sg * np.einsum('hi,hid->hd', wb, s)
+        out['hess'][:, a] = np.einsum('hi,hid,hie->hde', wa, s, s) + sg * mean[:, None, None] * np.diag(il2)
+        dk = ks[:, :, None] * s                                      # (H,N,Nx): d_d ks
+        Vd = (Li @ np.transpose(dk, (1, 0, 2)).reshape(-1, H * Nx)).reshape(-1, H, Nx)
+        G = np.einsum('ihd,ihe->hde', Vd, Vd)
+        B2 = np.einsum('hi,hid,hie->hde', wb, s, s)
+        # the kernels take k^T K^-1 k as sf2 - var, whose sum of |terms| is sf2 + |var|
+        qn = sf2 + out['var'][:, a] if absolute else q
+        out['d2var_dz2'][:, a] = 2 * sg * (G + B2 + sg * qn[:, None, None] * np.diag(il2))
+        M3 = np.einsum('hi,hid,hie,hif->hdef', wa, s, s, s, optimize=True)
+        Lj = eye * il2[:, None]
+        out['d3mean_dz3'][:, a] = M3 + sg * (np.einsum('de,hf->hdef', Lj, J) + np.einsum('df,he->hdef', Lj, J)
+                                             + np.einsum('ef,hd->hdef', Lj, J))
+    return out
+
+
+def cov_derivs(core, Sigma, method):
+    """cov (H,Ny,Ny), dcov_dz (H,Ny,Ny,Nx) and d2cov_dz2 (H,Ny,Ny,Nx,Nx) from ``derivs_core_ld``'s outputs and Sigma
+    ((Nx,Nx) shared or (H,Nx,Nx), not symmetrised): diag(var) + J Sigma J^T and its derivatives for 'TA', diag(var) and
+    its derivatives for 'ME'.  Fed a core with absolute=True and |Sigma|, the sums of |terms|."""
+    var, J, Hm, V2, T3 = (core[k] for k in ('var', 'J', 'hess', 'd2var_dz2', 'd3mean_dz3'))
+    H, Ny, Nx = J.shape
+    cov = np.zeros((H, Ny, Ny), dtype=var.dtype)
+    dcov = np.zeros((H, Ny, Ny, Nx), dtype=var.dtype)
+    d2cov = np.zeros((H, Ny, Ny, Nx, Nx), dtype=var.dtype)
+    if method == 'TA':
+        S = np.asarray(Sigma, dtype=var.dtype)
+        S = np.broadcast_to(S, (H, Nx, Nx)) if S.ndim == 2 else S
+        cov += np.einsum('had,hde,hbe->hab', J, S, J)
+        dcov += np.einsum('hadf,hde,hbe->habf', Hm, S, J) + np.einsum('had,hde,hbef->habf', J, S, Hm)
+        d2cov += (np.einsum('hadfg,hde,hbe->habfg', T3, S, J, optimize=True)
+                  + np.einsum('hadf,hde,hbeg->habfg', Hm, S, Hm, optimize=True)
+                  + np.einsum('hadg,hde,hbef->habfg', Hm, S, Hm, optimize=True)
+                  + np.einsum('had,hde,hbefg->habfg', J, S, T3, optimize=True))
+    for a in range(Ny):
+        cov[:, a, a] += var[:, a]
+        dcov[:, a, a] += core['dvar_dz'][:, a]
+        d2cov[:, a, a] += V2[:, a]
+    return dict(cov=cov, dcov_dz=dcov, d2cov_dz2=d2cov)
+
+
+def predict_derivs_ld(X, hyper, alpha, linv, Z, Sigma, method, absolute=False):
+    """Every output of gpmpc_predict_hess in np.longdouble, on the engine's own alpha (Ny,N) and L^-1 (Ny,N,N) (GET_ALPHA,
+    GET_LINV) so that cond(K) enters neither side of a comparison: dict(mean, var, J, dvar_dz, hess, d2var_dz2,
+    d3mean_dz3, cov, dcov_dz, d2cov_dz2) shaped as gpmpc_predict_hess's outputs, with the module docstring's formulas.
+
+    ``absolute=True`` evaluates the same expressions on |L^-1|, |alpha|, |s|, |Sigma| with every subtraction turned into
+    an addition (var -> sf2 + |v|^2, the -delta/ell^2 terms added): the sum of |terms| of each output, including the
+    cancellation inside L^-1 ks itself.  It is the scale against which a kernel's rounding is measured."""
+    core = derivs_core_ld(X, hyper, alpha, linv, Z, absolute)
+    if absolute and Sigma is not None:
+        Sigma = np.abs(np.asarray(Sigma, dtype=np.float64))
+    core.update(cov_derivs(core, Sigma, method))
+    return core
+
+
 def predict_hess_fd(X, hyper, alpha, chol, Z, Sigma, method='TA', rel=1e-4):
     """Central differences of ``predict_grad_closed`` w.r.t. every test-input coordinate: the
     checker of ``predict_hess``.  Returns dict(d2var, d3mean, d2cov) shaped as there."""
