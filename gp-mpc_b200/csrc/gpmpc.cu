@@ -89,7 +89,8 @@ struct gpmpc_handle_s {
     cudaStream_t sideSt[MAX_DEPTH] = {nullptr}; cudaEvent_t evA[MAX_DEPTH] = {nullptr}, evB[MAX_DEPTH] = {nullptr}, evT[MAX_DEPTH] = {nullptr}, evS[MAX_DEPTH] = {nullptr};
     long long w2off[MAX_DEPTH + 1] = {0};
     // model
-    DevBuf<double> dXT, dMu, dY, dHyp, dJit, dHypTmp;
+    DevBuf<double> dXT, dMu, dY, dHyp, dJit, dHypTmp;   // dJit: the jitter of each K build (scratch)
+    DevBuf<double> dFacJit;           // the jitter on the diagonal of the K each output's current factor factorises
     DevBuf<double> dL, dLi, dW1, dW2;
     DevBuf<double> dAlpha, dTmp, dRes;
     DevBuf<int> dInfo;
@@ -465,6 +466,7 @@ static int create_fill(gpmpc_handle_t h, int N, int N_cap, int Nx, int Ny, int o
     ENSURE(h->dHyp, (long long)out_count * (Nx + 2));
     ENSURE(h->dHypTmp, Nx + 2);
     ENSURE(h->dJit, out_count);
+    ENSURE(h->dFacJit, out_count);
     ENSURE(h->dL, out_count * slab(h));
     ENSURE(h->dLi, out_count * slab(h));
     {   // W2 workspace: one region per recursion depth (n_d = ceil(nb / 2^d) * 128 rows at depth d)
@@ -732,6 +734,9 @@ extern "C" int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info)
         if (info) info[a] = h->jitter_used[a];
     }
     if (worst) return worst;
+    // dJit now holds each output's jitter (0 or the retry's); the appends extend K + that jitter, and dJit itself is
+    // scratch for later K builds (gpmpc_build_K, gpmpc_profile)
+    CUDA_TRY(cudaMemcpyAsync(h->dFacJit, h->dJit, nl * sizeof(double), cudaMemcpyDeviceToDevice, h->st));
     rc = refresh_alpha(h);
     if (rc) return rc;
     h->factorized = true;
@@ -2449,8 +2454,8 @@ static int append_rows(gpmpc_handle_t h, int Nk, const int* stop)
     const long long sl = (long long)HB * np;
     trmv_lower_T_kernel<<<dim3((Nk + 31) / 32, 1, nl), 256, 0, h->st>>>(h->dLi, np, slab(h), h->dV, sl, h->dR, sl, Nk);
     CUDA_TRY(cudaGetLastError());
-    append_row_kernel<<<nl, 256, 0, h->st>>>(h->dL, h->dLi, np, slab(h), h->dV, h->dR, sl, h->dHyp, Nx + 2, Nx, Nk, h->dInfo,
-                                             stop);
+    append_row_kernel<<<nl, 256, 0, h->st>>>(h->dL, h->dLi, np, slab(h), h->dV, h->dR, sl, h->dHyp, Nx + 2, Nx, h->dFacJit,
+                                             Nk, h->dInfo, stop);
     CUDA_TRY(cudaGetLastError());
     return GPMPC_OK;
 }

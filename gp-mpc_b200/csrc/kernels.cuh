@@ -1400,17 +1400,18 @@ __global__ void sym_from_lower_kernel(const double* __restrict__ Kl, double* __r
 // ---------------------------------------------------------------------------------------
 // Rank-1 append of one training point (SURVEY 8f row 3; the reference's update_data,
 // gp_class.py:384-471, is self-declared broken -- this is the textbook update):
-//   l = L^-1 k(X, x_new);  lambda = sqrt(k(x_new,x_new) + sn2 - l^T l)
+//   l = L^-1 k(X, x_new);  lambda = sqrt(k(x_new,x_new) + sn2 + jitter - l^T l)
 //   L    <- [[L, 0], [l^T, lambda]]          L^-1 <- [[L^-1, 0], [-(l^T L^-1)/lambda, 1/lambda]]
 // lvec = L^-1 k, rvec = (L^-1)^T lvec are produced by the trmv kernels; this kernel writes
-// row N of both factors (the identity tail row it replaces).  One CTA per output.  stop (may be null): a greedy
-// selection step after a failed pivot, nothing is written.
+// row N of both factors (the identity tail row it replaces).  jit[a]: the jitter output a's factorisation put on every
+// diagonal entry of K, which the new one gets as well.  One CTA per output.  stop (may be null): a greedy selection
+// step after a failed pivot, nothing is written.
 // ---------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 append_row_kernel(double* __restrict__ L, double* __restrict__ Li, int ld, long long sL,
                   const double* __restrict__ lvec, const double* __restrict__ rvec, long long sv,
-                  const double* __restrict__ hyp, int hyp_ld, int Nx, int N, int* __restrict__ info,
-                  const int* __restrict__ stop)
+                  const double* __restrict__ hyp, int hyp_ld, int Nx, const double* __restrict__ jit, int N,
+                  int* __restrict__ info, const int* __restrict__ stop)
 {
     __shared__ double red[8];
     __shared__ double lam_s;
@@ -1427,7 +1428,7 @@ append_row_kernel(double* __restrict__ L, double* __restrict__ Li, int ld, long 
         double r = 0.0;
         for (int w = 0; w < 8; ++w) r += red[w];
         const double sf = hyp[(long long)a * hyp_ld + Nx], sn = hyp[(long long)a * hyp_ld + Nx + 1];
-        const double d = sf * sf + sn * sn - r;
+        const double d = sf * sf + sn * sn + jit[a] - r;
         if (!(d > 0.0)) atomicCAS(info + a, 0, N + 1);
         lam_s = sqrt(d);
     }

@@ -160,7 +160,11 @@ int gpmpc_predict(gpmpc_handle_t h, int method, int H, const double* Z, const do
  * ceil(N/128)*128, or the one reserved by gpmpc_create_reserve (GPMPC_ERR_STATE beyond it: refit on
  * a new handle).  GPMPC_ERR_NOTPD if the Schur complement is not positive: the point is in the model
  * (N counts it) and the handle needs gpmpc_factorize (the jitter policy applies there).  Appends every
- * point given, in order; gpmpc_append_greedy chooses. */
+ * point given, in order; gpmpc_append_greedy chooses.  Jitter: when gpmpc_factorize needed its jitter retry
+ * for an output, the factor is that of K + jitter I, and every later append (and greedy pick) puts the same
+ * jitter on its new diagonal entry, so the model stays the factor of K_aug + jitter I, as a refit of the
+ * grown data that needed the retry would be.  The jitter is the one recorded by the last gpmpc_factorize;
+ * gpmpc_nlml and gpmpc_loo_nlpp invalidate the factor, so no append can follow them without one. */
 int gpmpc_append(gpmpc_handle_t h, const double* x_new, const double* y_new);
 
 /* Greedy selection from a pool: n_new times, append the pool point with the largest sum over outputs of the
