@@ -18,7 +18,7 @@ LIB_PATH = os.environ.get('GPMPC_LIB', os.path.join(_HERE, 'lib', 'libgpmpc.so')
 OK, ERR_ARG, ERR_CUDA, ERR_STATE, ERR_NCCL, ERR_NOTPD = 0, -1, -2, -3, -4, -5
 METHOD_ME, METHOD_TA, METHOD_EM = 0, 1, 2
 GET_CHOL, GET_ALPHA, GET_INVK, GET_K, GET_LOGDET, GET_LINV, GET_ALPHA_NLML = range(7)
-PROF_KBUILD_FULL, PROF_KBUILD_LOWER, PROF_SYRK, PROF_FACTORIZE, PROF_TRIGEMM, PROF_KS, PROF_PREDICT_TAIL = range(7)
+PROF_KBUILD_FULL, PROF_KBUILD_LOWER, PROF_SYRK, PROF_FACTORIZE, PROF_TRIGEMM, PROF_KS, PROF_PREDICT_TAIL, PROF_PANEL = range(8)
 
 # every symbol include/gpmpc.h declares: (name, restype, argtypes)
 _dp = C.POINTER(C.c_double)

@@ -220,6 +220,14 @@ __device__ __forceinline__ void tma_tile_g2s_3d_hint(void* smem_dst, const CUten
                  : "memory");
 }
 
+// non-tensor bulk copy (SASS UBLKCP) of `bytes` contiguous bytes (multiple of 16, both ends 16-byte aligned), same barrier
+__device__ __forceinline__ void bulk_g2s_hint(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint64_t policy)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;\n"
+                 :: "r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+                 : "memory");
+}
+
 template <int BM, int BN, int WM, int WN, int STAGES, int MINB>
 __global__ void __launch_bounds__(WM * WN * 32, MINB)
 gemm_dmma_tmap_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB)

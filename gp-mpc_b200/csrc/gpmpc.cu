@@ -96,6 +96,9 @@ struct gpmpc_handle_s {
     DevBuf<int> dInfo;
     // predict
     DevBuf<double> dKST, dPart, dPMJ, dSQ, dV, dR, dR2;
+    // L^-1 of every output in the product's k-step order (panel_pack_kernel, lazy) and, per output, the first L^-1 row
+    // whose panel copy may be stale (Npad: current).  Every writer of dLi lowers it; panel_refresh repacks from there.
+    DevBuf<double> dLiP; std::vector<int> panel_row;
     DevBuf<unsigned int> dCnt;        // stream-K counters: [nloc*nt tile | nloc output | 1 done], self-cleaning
     int psk_ctas = 0, opt_predict_ctas = 0;   // persistent grid of the predict product (PSK_CTAS_PER_SM per SM)
     DevBuf<double> dCovV, dCovOut;    // GP.covar scratch pool; dCovV also holds the greedy selection's pool V
@@ -194,6 +197,13 @@ struct NvtxRange {
 
 static inline long long slab(gpmpc_handle_t h) { return (long long)h->Npad * h->Npad; }
 static inline long long w2slab(gpmpc_handle_t h) { return h->w2off[MAX_DEPTH]; }   // all depths, one batch entry
+
+// L^-1 rows from `row` on of local output al (every output: al < 0) were written: their panel copy is stale
+static void panel_stale(gpmpc_handle_t h, int al, int row)
+{
+    for (int a = 0; a < h->nloc; ++a)
+        if (al < 0 || a == al) h->panel_row[a] = std::min(h->panel_row[a], std::max(row, 0));
+}
 
 // f(std::integral_constant<int, NXP>) with NXP = 8, 16 or 32 >= Nx: the register-array extent of the kernels that keep
 // one Nx-vector per thread (nlml gradient, EM, predict derivatives)
@@ -415,6 +425,7 @@ static int factor_one(gpmpc_handle_t h, int a, const double* dHyp, double jitter
     double* L = h->dL + (long long)a * slab(h);
     double* Li = h->dLi + (long long)a * slab(h);
     *used = 0;
+    panel_stale(h, a, 0);
     for (int attempt = 0; attempt < 2; ++attempt) {
         const double jit = attempt ? jitter : 0.0;
         CUDA_TRY(cudaMemcpyAsync(h->dJit + a, &jit, sizeof(double), cudaMemcpyHostToDevice, h->st));
@@ -447,6 +458,7 @@ static int create_fill(gpmpc_handle_t h, int N, int N_cap, int Nx, int Ny, int o
     h->N = N; h->Nx = Nx; h->Ny = Ny; h->a0 = out_begin; h->nloc = out_count; h->device = device;
     h->nloc_max = out_count; h->world = 1; h->rank = 0;
     h->Npad = (std::max(N, N_cap) + GPMPC_TILE - 1) / GPMPC_TILE * GPMPC_TILE;
+    h->panel_row.assign(out_count, 0);
     CUDA_TRY(cudaSetDevice(device));
     CUDA_TRY(cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, device));
     h->opt_small_tiles = 4 * h->sms;      // two waves of 2 CTAs per SM
@@ -580,7 +592,7 @@ static int ensure_pinned(gpmpc_handle_t h, size_t bytes)
 // the caches derived from the factor (Li^T for predict_grad, K^-1 for the EM derivatives) no longer match it
 static void factor_caches_stale(gpmpc_handle_t h) { h->u_valid = false; h->em_kinv_valid = false; }
 // the factor no longer matches the data or hyper-parameters, or its slabs were used as scratch: gpmpc_factorize first
-static void factor_stale(gpmpc_handle_t h) { h->factorized = false; factor_caches_stale(h); }
+static void factor_stale(gpmpc_handle_t h) { h->factorized = false; factor_caches_stale(h); panel_stale(h, -1, 0); }
 
 enum ModelNeed { NEED_DATA, NEED_HYPER, NEED_FACTOR };     // data; data and hyper-parameters; a factorised model
 
@@ -716,6 +728,7 @@ extern "C" int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info)
     CUDA_TRY(cudaMemsetAsync(h->dInfo, 0, nl * sizeof(int), h->st));
     rc = launch_kbuild(h, h->dHyp, h->dJit, h->dL, nl, 0);
     if (rc) return rc;
+    panel_stale(h, -1, 0);
     rc = potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, h->Npad, nl, nl, h->dW1, h->dW2);
     if (rc) return rc;
     std::vector<int> inf(nl, 0);
@@ -1210,11 +1223,18 @@ static int psk_grid(gpmpc_handle_t h, long long G)
     return (int)std::min<long long>(ctas, h->opt_predict_ctas > 0 ? G : by_work);
 }
 
-// the predict product p (psk_base) of A (h-major rows, HB * Npad per output) and the slab B of each output: BM = round8(p.Hc)
-static cudaError_t psk_launch(gpmpc_handle_t h, const PredictParams& p, const double* A, const double* B)
+// the predict product p (psk_base) of A (h-major rows, HB * Npad per output) and the slab B of each output: BM = round8(p.Hc).
+// A lower-mode product of L^-1 streams it from the panel, which panel_refresh must have brought up to date.
+static cudaError_t psk_launch(gpmpc_handle_t h, const PredictParams& p0, const double* A, const double* B)
 {
     const long long sA = (long long)HB * h->Npad, sB = slab(h);
-    const int np = h->Npad, grid = psk_grid(h, p.G);
+    const int np = h->Npad, grid = psk_grid(h, p0.G);
+    PredictParams p = p0;
+    if (B == h->dLi.p && !p.upper) {
+        for (int a = 0; a < h->nloc; ++a)
+            if (h->panel_row[a] < np) return cudaErrorIllegalState;
+        p.Lp = h->dLiP;
+    }
     switch (round8(p.Hc)) {
     case 8: return psk_launch_bm<8>(p, A, sA, B, sB, np, grid, h->st);
     case 16: return psk_launch_bm<16>(p, A, sA, B, sB, np, grid, h->st);
@@ -1239,6 +1259,27 @@ static void psk_base(gpmpc_handle_t h, PredictParams& p, int Hc, int upper = 0)
     p.tile_cnt = h->dCnt; p.out_cnt = h->dCnt + (long long)h->nloc * nt; p.done_cnt = p.out_cnt + h->nloc;
     p.SQ = h->dSQ;
     p.hyp = h->dHyp; p.hyp_ld = h->Nx + 2; p.Nx = h->Nx;
+}
+
+// Brings the L^-1 panel up to date: output a is repacked from the tile of its first stale row, so an append costs one tile
+// band and a factorisation everything.  Runs before any product of L^-1 (predict_prepare, gpmpc_profile).
+static int panel_refresh(gpmpc_handle_t h)
+{
+    PredictParams p;
+    psk_base(h, p, HB);
+    const long long blk = PSK_BN * GEMM_BK;
+    const double* old = h->dLiP;
+    ENSURE(h->dLiP, p.G * blk);
+    if (h->dLiP.p != old) panel_stale(h, -1, 0);
+    for (int a = 0; a < h->nloc; ++a) {
+        if (h->panel_row[a] >= h->Npad) continue;
+        const int jt0 = h->panel_row[a] / PSK_BN;
+        panel_pack_kernel<<<dim3(p.nk, p.ntb - jt0), 256, 0, h->st>>>(h->dLi + a * slab(h), h->Npad, h->dLiP + a * p.T * blk,
+                                                                      p.ntb, jt0);
+        CUDA_TRY(cudaGetLastError());
+        h->panel_row[a] = h->Npad;
+    }
+    return GPMPC_OK;
 }
 
 // after psk_base: the product also finalises chunk [h0, h0 + Hc) of an H-point step (records from the ks partials into dG)
@@ -1805,7 +1846,8 @@ static int predict_guard(gpmpc_handle_t h, const char* fn, int method, int H)
 static int predict_prepare(gpmpc_handle_t h, const char* fn, int H, bool all_outputs)
 {
     if (all_outputs && (h->nloc != h->Ny || h->world != 1)) { set_error(h, "%s needs all outputs on one handle (replicate the model, shard the points)", fn); return GPMPC_ERR_STATE; }
-    return ensure_predict_bufs(h, H);
+    const int rc = ensure_predict_bufs(h, H);
+    return rc ? rc : panel_refresh(h);
 }
 
 extern "C" int gpmpc_predict_device(gpmpc_handle_t h, int method, int H, const double* dZ, const double* dSigma,
@@ -2452,6 +2494,7 @@ static int append_rows(gpmpc_handle_t h, int Nk, const int* stop)
 {
     const int np = h->Npad, Nx = h->Nx, nl = h->nloc;
     const long long sl = (long long)HB * np;
+    panel_stale(h, -1, Nk);
     trmv_lower_T_kernel<<<dim3((Nk + 31) / 32, 1, nl), 256, 0, h->st>>>(h->dLi, np, slab(h), h->dV, sl, h->dR, sl, Nk);
     CUDA_TRY(cudaGetLastError());
     append_row_kernel<<<nl, 256, 0, h->st>>>(h->dL, h->dLi, np, slab(h), h->dV, h->dR, sl, h->dHyp, Nx + 2, Nx, h->dFacJit,
@@ -2729,6 +2772,7 @@ extern "C" int gpmpc_remove(gpmpc_handle_t h, int n, const int* idx)
     if (rc) return rc;
     ENSURE(h->dRm, (long long)nl * 3 * np);
     NvtxRange nvtx_r("gpmpc.remove");
+    panel_stale(h, -1, order[n - 1]);     // rows from the smallest removed index on move up
     const dim3 gcol((np + 255) / 256);
     for (int k = 0; k < n; ++k) {
         const int i = order[k], Nk = N - k, m = Nk - i - 1;     // m trailing points
@@ -2988,6 +3032,7 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
             return potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, np, 1, 1, h->dW1, h->dW2);
         }
         case GPMPC_PROF_TRIGEMM: return tri_product(h, h->dKST, h->dLi, Hc, nullptr);
+        case GPMPC_PROF_PANEL: panel_stale(h, -1, 0); return panel_refresh(h);
         case GPMPC_PROF_KS: {             // the ks / mean / Jacobian partial kernel alone (Z = the last batch's inputs)
             cudaError_t e = launch_ks(h, h->dZ, Hc);
             if (e != cudaSuccess) { set_error(h, "profile ks: %s", cudaGetErrorString(e)); return GPMPC_ERR_CUDA; }
@@ -3007,8 +3052,15 @@ extern "C" int gpmpc_profile(gpmpc_handle_t h, int what, int n, int reps, double
         }
     };
     // the product selectors run on the predict buffers; the others use the factor's slabs as scratch
-    const bool product = what == GPMPC_PROF_TRIGEMM || what == GPMPC_PROF_KS || what == GPMPC_PROF_PREDICT_TAIL;
-    if (product) { rc = ensure_predict_bufs(h, HB); if (rc) return rc; }
+    const bool product = what == GPMPC_PROF_TRIGEMM || what == GPMPC_PROF_KS || what == GPMPC_PROF_PREDICT_TAIL ||
+                         what == GPMPC_PROF_PANEL;
+    if (product) {
+        rc = ensure_predict_bufs(h, HB);
+        if (rc == GPMPC_OK) rc = panel_refresh(h);
+        if (rc) return rc;
+    } else {
+        panel_stale(h, -1, 0);
+    }
     CUDA_TRY(cudaMemsetAsync(h->dJit, 0, h->nloc * sizeof(double), h->st));
     rc = run();
     if (rc) return rc;

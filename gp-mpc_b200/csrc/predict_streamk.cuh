@@ -66,6 +66,7 @@ struct PredictParams {
     int nloc, nt, Hc;                 // local outputs, 128-column groups per output (Npad / 128), valid rows of this chunk
     int ntb, nk;                      // PSK_BN-row tiles per output (the last one 128 rows high when nt is odd), Npad / 16
     int upper;                        // 0: B lower triangular (k <= j, v = Linv ks); 1: B upper (k >= j, beta = Linv^T v)
+    const double* Lp;                 // lower mode, B = L^-1: its panel copy (panel_pack_kernel), one bulk copy per stage; else null
     long long T, G;                   // k-steps per output (psk_steps_per_output), total = nloc * T
     double* part;                     // [grid][2][BM*PSK_BN] parked partial accumulators (fragment-major)
     unsigned int* tile_cnt;           // [nloc*ntb]
@@ -327,10 +328,11 @@ __device__ __forceinline__ long long psk_kstart(const PredictParams& p, int jt) 
 // 128-row half.  Only the leaf kernel's diagonal 128 x 128 blocks are stored with explicit zeros on their far side; the
 // off-diagonal block beyond is not kept zero (a full K build leaves K's upper triangle in the L slab), so the warps of
 // that half skip those 8 k-steps in the product kernel's main loop and never read it.
-__device__ __forceinline__ int psk_ksteps(const PredictParams& p, int jt)
+__host__ __device__ inline int psk_ksteps(int ntb, int nk, int upper, int jt)
 {
-    return p.upper ? p.nk - PSK_SB * (p.ntb - 1 - jt) : min(PSK_SB * (jt + 1), p.nk);
+    return upper ? nk - PSK_SB * (ntb - 1 - jt) : (PSK_SB * (jt + 1) < nk ? PSK_SB * (jt + 1) : nk);
 }
+__device__ __forceinline__ int psk_ksteps(const PredictParams& p, int jt) { return psk_ksteps(p.ntb, p.nk, p.upper, jt); }
 
 struct PskIter { int a, jt, s, ks; };
 
@@ -350,6 +352,31 @@ __device__ __forceinline__ void psk_iter_next(PskIter& it, const PredictParams& 
         it.s = 0;
         if (++it.jt == p.ntb) { it.jt = 0; ++it.a; }
         it.ks = psk_ksteps(p, it.jt);
+    }
+}
+
+// The L^-1 panel (dLiP): each output's lower-mode k-step list, block after block in the order the product consumes it.
+// Block g = a T + psk_kstart(jt) + s (PSK_BN x 16 doubles) holds rows jt BN .. jt BN + BN-1 and columns 16 s .. 16 s + 15
+// of output a's L^-1 exactly as the tensor map lands them in a stage: 128-byte rows, the 16-byte chunk c of row r at
+// chunk c ^ (r & 7), rows past Npad (the half tile) zero.  A CTA's range [g0, g0 + nsteps) of the list is then one
+// contiguous stretch of memory.  The far-side 128 x 128 block the upper-half warps skip is copied as L^-1 holds it.
+// psk_panel_chunk: offset (doubles) in one output's panel of chunk c (columns 16 s + 2c, +1) of row r of tile jt, step s.
+__host__ __device__ inline long long psk_panel_chunk(int ntb, int nk, int jt, int s, int r, int c)
+{
+    return (psk_kstart(ntb, nk, 0, jt) + s) * (PSK_BN * GEMM_BK) + r * GEMM_BK + 2 * (c ^ (r & 7));
+}
+
+// grid (nk, ntb - jt0): block (s, jt - jt0) of output Li, 8 threads per row with one 16-byte load and store each
+__global__ void __launch_bounds__(256)
+panel_pack_kernel(const double* __restrict__ Li, int np, double* __restrict__ P, int ntb, int jt0)
+{
+    const int s = blockIdx.x, jt = jt0 + blockIdx.y, nk = np / GEMM_BK, c = threadIdx.x & 7;
+    if (s >= psk_ksteps(ntb, nk, 0, jt)) return;
+#pragma unroll 4
+    for (int r = threadIdx.x >> 3; r < PSK_BN; r += 32) {
+        const long long row = (long long)jt * PSK_BN + r;
+        const double2 v = row < np ? __ldcs(reinterpret_cast<const double2*>(Li + row * np + s * GEMM_BK) + c) : make_double2(0.0, 0.0);
+        *reinterpret_cast<double2*>(P + psk_panel_chunk(ntb, nk, jt, s, r, c)) = v;
     }
 }
 
@@ -475,7 +502,8 @@ finalize_kernel(const PredictParams p)
 
 // The product on DMMA.16x8x16 (dmma16816).  tmA delivers the BM x 16 box of ks^T (test points x k), tmB the BN x 16
 // box of the L-side matrix (L^-1, U in upper mode, L in the refinement), both in rows of 128 bytes with the 128B
-// swizzle: the 16-byte chunk c of row r sits at chunk c ^ (r & 7).
+// swizzle: the 16-byte chunk c of row r sits at chunk c ^ (r & 7).  A lower-mode product of L^-1 (p.Lp) copies the same
+// bytes from the panel instead (panel_pack_kernel).
 //   Per k-step (16 k) warp w computes the 32 x BM block V^T[L-rows 32w .. 32w+31][points] as two MMA A
 //   operands (mi = 0, 1: L-rows 32w + 16 mi .. +15, row layout) against ks^T as the B operand (col layout, N = 8
 //   points per fragment, BM / 8 fragments).  Each B fragment feeds both A fragments: 16 + 4 BM / 8 LDS.64 per 2 BM / 8
@@ -524,6 +552,7 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
     __shared__ PskIter s_pit;
     __shared__ int s_pg;
     __shared__ uint64_t s_pol[2];
+    __shared__ const double* s_lp;     // this CTA's stretch of the L^-1 panel (null: B through tmB)
     if (tid == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, CW); }
@@ -544,7 +573,9 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
         // ks^T (A) is re-read by every column tile: keep it in L2; L^-1 (B) is streamed exactly once.  Also when ks^T is
         // larger than the L2 (8 outputs at N=16384 on H100: 59 MB vs 50 MB) evict_last measured no slower than evict_normal
         tma_tile_g2s_3d_hint(As + s * A_STAGE, &tmA, k0, 0, it.a, full + s, s_pol[1]);
-        tma_tile_g2s_3d_hint(Bs + s * B_STAGE, &tmB, k0, jta * BN, it.a, full + s, s_pol[0]);
+        // the panel holds step g0 + pg as the tensor map would land it: one contiguous 32 KB copy instead of 256 rows
+        if (s_lp) bulk_g2s_hint(Bs + s * B_STAGE, s_lp + (long long)pg * B_STAGE, B_STAGE * 8, full + s, s_pol[0]);
+        else tma_tile_g2s_3d_hint(Bs + s * B_STAGE, &tmB, k0, jta * BN, it.a, full + s, s_pol[0]);
         psk_iter_next(it, p);
         s_pit = it;
         s_pg = pg + 1;
@@ -558,6 +589,7 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
         PskIter it;
         psk_iter_init(it, g0, p);
         s_pit = it; s_pg = 0;
+        s_lp = p.Lp ? p.Lp + g0 * B_STAGE : nullptr;
         s_pol[0] = l2_policy_evict_first(); s_pol[1] = l2_policy_evict_last();
 #pragma unroll
         for (int s = 0; s < AHEAD; ++s)

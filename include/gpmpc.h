@@ -61,7 +61,8 @@ enum {
     GPMPC_PROF_FACTORIZE = 3,     /* potrf + trtri of one output (K prebuilt each rep) */
     GPMPC_PROF_TRIGEMM = 4,       /* predict v = Linv ks product, all local outputs    */
     GPMPC_PROF_KS = 5,            /* ks / partial mean / partial Jacobian kernel alone (after a predict call) */
-    GPMPC_PROF_PREDICT_TAIL = 6   /* product + finalize + assembly in one launch, no ks kernel in front (after a predict call) */
+    GPMPC_PROF_PREDICT_TAIL = 6,  /* product + finalize + assembly in one launch, no ks kernel in front (after a predict call) */
+    GPMPC_PROF_PANEL = 7          /* full repack of every local output's L^-1 panel (the predict product's B operand) */
 };
 
 int gpmpc_version(void);
