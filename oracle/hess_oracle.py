@@ -113,12 +113,13 @@ def predict_hess(X, hyper, alpha, chol, Z, Sigma, method='TA'):
     return out
 
 
-def derivs_core_ld(X, hyper, alpha, linv, Z, absolute=False):
+def derivs_core_ld(X, hyper, alpha, linv, Z, absolute=False, second=True):
     """The Sigma-free part of ``predict_derivs_ld``: dict(mean, var (H,Ny), J (H,Ny,Nx), dvar_dz (H,Ny,Nx),
     hess (H,Ny,Nx,Nx), d2var_dz2 (H,Ny,Nx,Nx), d3mean_dz3 (H,Ny,Nx,Nx,Nx)) in np.longdouble, on the path of the
     kernels: ks by direct differences, v = L^-1 ks, beta = L^-T v and V_d = L^-1 d_d ks as products with ``linv``
     (Ny,N,N, lower, as GET_LINV returns it), k^T K^-1 k = |v|^2.  ``absolute``: the sums of |terms| of every output
-    (see ``predict_derivs_ld``)."""
+    (see ``predict_derivs_ld``).  ``second=False`` leaves out d2var_dz2 and d3mean_dz3 (what gpmpc_predict_grad and
+    the roll-outs need; V_d and the third moments dominate the cost at large Nx)."""
     ld = np.longdouble
     X = np.asarray(X, dtype=ld)
     Z = np.atleast_2d(np.asarray(Z, dtype=ld))
@@ -126,9 +127,10 @@ def derivs_core_ld(X, hyper, alpha, linv, Z, absolute=False):
     H, Nx = Z.shape
     Ny = hyper.shape[0]
     sg = 1 if absolute else -1                                    # the sign of every subtraction
-    out = {k: np.zeros(s, dtype=ld) for k, s in (('mean', (H, Ny)), ('var', (H, Ny)), ('J', (H, Ny, Nx)),
-                                                 ('dvar_dz', (H, Ny, Nx)), ('hess', (H, Ny, Nx, Nx)),
-                                                 ('d2var_dz2', (H, Ny, Nx, Nx)), ('d3mean_dz3', (H, Ny, Nx, Nx, Nx)))}
+    shapes = (('mean', (H, Ny)), ('var', (H, Ny)), ('J', (H, Ny, Nx)), ('dvar_dz', (H, Ny, Nx)), ('hess', (H, Ny, Nx, Nx)))
+    if second:
+        shapes += (('d2var_dz2', (H, Ny, Nx, Nx)), ('d3mean_dz3', (H, Ny, Nx, Nx, Nx)))
+    out = {k: np.zeros(s, dtype=ld) for k, s in shapes}
     eye = np.eye(Nx, dtype=ld)
     for a in range(Ny):
         ell = hyper[a, :Nx]
@@ -155,6 +157,8 @@ def derivs_core_ld(X, hyper, alpha, linv, Z, absolute=False):
         out['J'][:, a] = J
         out['dvar_dz'][:, a] = 2 * sg * np.einsum('hi,hid->hd', wb, s)
         out['hess'][:, a] = np.einsum('hi,hid,hie->hde', wa, s, s) + sg * mean[:, None, None] * np.diag(il2)
+        if not second:
+            continue
         dk = ks[:, :, None] * s                                      # (H,N,Nx): d_d ks
         Vd = (Li @ np.transpose(dk, (1, 0, 2)).reshape(-1, H * Nx)).reshape(-1, H, Nx)
         G = np.einsum('ihd,ihe->hde', Vd, Vd)
@@ -172,17 +176,21 @@ def derivs_core_ld(X, hyper, alpha, linv, Z, absolute=False):
 def cov_derivs(core, Sigma, method):
     """cov (H,Ny,Ny), dcov_dz (H,Ny,Ny,Nx) and d2cov_dz2 (H,Ny,Ny,Nx,Nx) from ``derivs_core_ld``'s outputs and Sigma
     ((Nx,Nx) shared or (H,Nx,Nx), not symmetrised): diag(var) + J Sigma J^T and its derivatives for 'TA', diag(var) and
-    its derivatives for 'ME'.  Fed a core with absolute=True and |Sigma|, the sums of |terms|."""
-    var, J, Hm, V2, T3 = (core[k] for k in ('var', 'J', 'hess', 'd2var_dz2', 'd3mean_dz3'))
+    its derivatives for 'ME'.  Fed a core with absolute=True and |Sigma|, the sums of |terms|.  A core made with
+    second=False gives no d2cov_dz2."""
+    second = 'd3mean_dz3' in core
+    var, J, Hm = (core[k] for k in ('var', 'J', 'hess'))
     H, Ny, Nx = J.shape
     cov = np.zeros((H, Ny, Ny), dtype=var.dtype)
     dcov = np.zeros((H, Ny, Ny, Nx), dtype=var.dtype)
-    d2cov = np.zeros((H, Ny, Ny, Nx, Nx), dtype=var.dtype)
+    d2cov = np.zeros((H, Ny, Ny, Nx, Nx) if second else (0,), dtype=var.dtype)
     if method == 'TA':
         S = np.asarray(Sigma, dtype=var.dtype)
         S = np.broadcast_to(S, (H, Nx, Nx)) if S.ndim == 2 else S
         cov += np.einsum('had,hde,hbe->hab', J, S, J)
         dcov += np.einsum('hadf,hde,hbe->habf', Hm, S, J) + np.einsum('had,hde,hbef->habf', J, S, Hm)
+    if method == 'TA' and second:
+        T3 = core['d3mean_dz3']
         d2cov += (np.einsum('hadfg,hde,hbe->habfg', T3, S, J, optimize=True)
                   + np.einsum('hadf,hde,hbeg->habfg', Hm, S, Hm, optimize=True)
                   + np.einsum('hadg,hde,hbef->habfg', Hm, S, Hm, optimize=True)
@@ -190,8 +198,12 @@ def cov_derivs(core, Sigma, method):
     for a in range(Ny):
         cov[:, a, a] += var[:, a]
         dcov[:, a, a] += core['dvar_dz'][:, a]
-        d2cov[:, a, a] += V2[:, a]
-    return dict(cov=cov, dcov_dz=dcov, d2cov_dz2=d2cov)
+        if second:
+            d2cov[:, a, a] += core['d2var_dz2'][:, a]
+    out = dict(cov=cov, dcov_dz=dcov)
+    if second:
+        out['d2cov_dz2'] = d2cov
+    return out
 
 
 def predict_derivs_ld(X, hyper, alpha, linv, Z, Sigma, method, absolute=False):
