@@ -44,6 +44,7 @@ SYMBOLS = [
     ('gpmpc_predict_hess', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp,
                                      _dp, _dp, _dp]),
     ('gpmpc_predict_em_grad', C.c_int, [_H, C.c_int, _dp, _dp, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
+    ('gpmpc_predict_em_hess', C.c_int, [_H, C.c_int, _dp, _dp, C.c_int] + [_dp] * 13),
     ('gpmpc_get_size', C.c_int, [_H, _ip, _ip, _ip]),
     ('gpmpc_append', C.c_int, [_H, _dp, _dp]),
     ('gpmpc_append_greedy', C.c_int, [_H, C.c_int, _dp, _dp, C.c_int, _ip, _dp, _ip]),
@@ -81,7 +82,8 @@ for _f in ('gp_b200', 'jac_gp_b200'):
         (_f + '_work', C.c_int, [_llp, _llp, _llp, _llp]),
         (_f, C.c_int, [_dpp, _dpp, _llp, _dp, C.c_int]),
     ]
-SYMBOLS += [('gp_b200_bind', C.c_int, [_H, C.c_int, C.c_int]), ('gp_b200_unbind', None, []),
+SYMBOLS += [('gp_b200_bind', C.c_int, [_H, C.c_int, C.c_int]), ('gp_b200_bind_em_hess', C.c_int, [_H, C.c_int]),
+            ('gp_b200_unbind', None, []),
             ('gp_b200_incref', None, []), ('gp_b200_decref', None, [])]
 # the Jacobian of jac_gp_b200 (second derivatives, include/gpmpc_casadi.h), bound by load() next to SYMBOLS
 SYMBOLS_JAC_JAC = [
@@ -421,6 +423,27 @@ class Engine:
         self._check(self.lib.gpmpc_predict_em_grad(
             self.h, H, _ptr(Z), _ptr(Sigma), spp,
             *[_ptr(out[k]) for k in ('mean', 'var', 'cov', 'dmean_dz', 'dmean_dSigma', 'dcov_dz', 'dcov_dSigma')]))
+        return out
+
+    EM_HESS_KEYS = ('d2mean_dz2', 'd2mean_dSigma_dz', 'd2mean_dSigma2', 'd2cov_dz2', 'd2cov_dSigma_dz', 'd2cov_dSigma2')
+
+    def predict_em_hess(self, Z, Sigma):
+        """'EM' prediction + first and second derivatives w.r.t. the test input mean and the input covariance
+        (gpmpc_predict_em_hess).  Returns predict_em_grad's dict (same bits) plus d2mean_dz2 (H,Ny,Nx,Nx),
+        d2mean_dSigma_dz (H,Ny,Nx,Nx,Nx), d2mean_dSigma2 (H,Ny,Nx,Nx,Nx,Nx), d2cov_dz2 (H,Ny,Ny,Nx,Nx),
+        d2cov_dSigma_dz (H,Ny,Ny,Nx,Nx,Nx), d2cov_dSigma2 (H,Ny,Ny,Nx,Nx,Nx,Nx); the differentiated index is the last."""
+        Z, Sigma, H, spp = self._points(Z, Sigma)
+        Ny, Nx = self.Ny, self.Nx
+        out = dict(mean=np.empty((H, Ny)), var=np.empty((H, Ny)), cov=np.empty((H, Ny, Ny)),
+                   dmean_dz=np.empty((H, Ny, Nx)), dmean_dSigma=np.empty((H, Ny, Nx, Nx)),
+                   dcov_dz=np.empty((H, Ny, Ny, Nx)), dcov_dSigma=np.empty((H, Ny, Ny, Nx, Nx)),
+                   d2mean_dz2=np.empty((H, Ny, Nx, Nx)), d2mean_dSigma_dz=np.empty((H, Ny, Nx, Nx, Nx)),
+                   d2mean_dSigma2=np.empty((H, Ny, Nx, Nx, Nx, Nx)), d2cov_dz2=np.empty((H, Ny, Ny, Nx, Nx)),
+                   d2cov_dSigma_dz=np.empty((H, Ny, Ny, Nx, Nx, Nx)), d2cov_dSigma2=np.empty((H, Ny, Ny, Nx, Nx, Nx, Nx)))
+        self._check(self.lib.gpmpc_predict_em_hess(
+            self.h, H, _ptr(Z), _ptr(Sigma), spp,
+            *[_ptr(out[k]) for k in ('mean', 'var', 'cov', 'dmean_dz', 'dmean_dSigma', 'dcov_dz', 'dcov_dSigma')
+              + self.EM_HESS_KEYS]))
         return out
 
     def append(self, x_new, y_new):

@@ -28,8 +28,9 @@
 //              jac_cov_z   / z      Ny*Ny*Nx*Nx      d^2 cov[a][b] / d z_e d z_f     (d2cov_dz2)
 //              jac_cov_z   / sigma  Ny*Ny*Nx*Nx*Nx   hess_a[d][e] J_b[e'] + J_a[d] hess_b[e'][e]   ('TA')
 //              jac_cov_sigma / z    Ny*Ny*Nx*Nx*Nx   the same values, w.r.t. z_f of d cov / d Sigma[d][e]  ('TA')
-//            everything else is structurally zero.  'EM' has no second derivatives: jac_jac_gp_b200 returns failure
-//            (run IPOPT with hessian_approximation 'limited-memory').
+//            everything else is structurally zero.  'EM' bound by gp_b200_bind: jac_jac_gp_b200 returns failure.
+//            'EM' bound by gp_b200_bind_em_hess: gpmpc_predict_em_hess serves the blocks of the four Jacobians w.r.t.
+//            z and sigma (0, 1, 4, 5, 8, 9, 12, 13), block-diagonal over the nodes; those w.r.t. mean and cov stay empty.
 #include "../../include/gpmpc.h"
 
 #include <functional>
@@ -45,6 +46,8 @@ struct Bound {
     int method = GPMPC_METHOD_TA, Nt = 0, Nx = 0, Ny = 0;
     std::vector<casadi_int> sp_in[2], sp_out[2], sp_jac[4], sp_jj[16];
     std::vector<double> sig, mean, var, cov, jac, dvar, dcov, hess, d2cov, dmS, dcS;   // dmS / dcS: 'EM' d / d Sigma
+    bool em_hess = false;                               // 'EM' bound by gp_b200_bind_em_hess: second derivatives served
+    std::vector<double> mSz, mSS, cSz, cSS;             // 'EM' d2mean_dSigma_dz, d2mean_dSigma2, d2cov_dSigma_dz, d2cov_dSigma2
     int refs = 0;
 };
 Bound g_b;
@@ -115,7 +118,10 @@ int eval(const casadi_real* Z, const casadi_real* Sigma, int mode)
         if (mode == EVAL_GRAD)
             return gpmpc_predict_em_grad(b.h, Nt, Z, b.sig.data(), 1, b.mean.data(), b.var.data(), b.cov.data(), b.jac.data(),
                                          b.dmS.data(), b.dcov.data(), b.dcS.data()) == GPMPC_OK ? 0 : 1;
-        return 1;                       // no second derivatives of 'EM'
+        if (!b.em_hess) return 1;       // bound by gp_b200_bind: no second derivatives of 'EM'
+        return gpmpc_predict_em_hess(b.h, Nt, Z, b.sig.data(), 1, b.mean.data(), b.var.data(), b.cov.data(), b.jac.data(),
+                                     b.dmS.data(), b.dcov.data(), b.dcS.data(), b.hess.data(), b.mSz.data(), b.mSS.data(),
+                                     b.d2cov.data(), b.cSz.data(), b.cSS.data()) == GPMPC_OK ? 0 : 1;
     }
     if (mode == EVAL_HESS)
         return gpmpc_predict_hess(b.h, b.method, Nt, Z, ta ? b.sig.data() : nullptr, 1, b.mean.data(), b.var.data(),
@@ -129,16 +135,16 @@ int eval(const casadi_real* Z, const casadi_real* Sigma, int mode)
 }
 }  // namespace
 
-// Bind the (process-global) external to a factorised engine handle: method GPMPC_METHOD_ME / _TA / _EM,
-// Nt shooting nodes per call.  Call again to re-bind (e.g. after a refit or another horizon).
-extern "C" int gp_b200_bind(gpmpc_handle_t h, int method, int Nt)
+namespace {
+int bind(gpmpc_handle_t h, int method, int Nt, bool em_hess)
 {
     std::lock_guard<std::mutex> lock(g_mtx);
     int N = 0, Nx = 0, Ny = 0;
     if (!h || Nt < 1 || (method != GPMPC_METHOD_ME && method != GPMPC_METHOD_TA && method != GPMPC_METHOD_EM)) return GPMPC_ERR_ARG;
     if (gpmpc_get_size(h, &N, &Nx, &Ny) != GPMPC_OK) return GPMPC_ERR_ARG;
+    if (em_hess && Nx > 16) return GPMPC_ERR_ARG;
     Bound& b = g_b;
-    b.h = h; b.method = method; b.Nt = Nt; b.Nx = Nx; b.Ny = Ny;
+    b.h = h; b.method = method; b.Nt = Nt; b.Nx = Nx; b.Ny = Ny; b.em_hess = em_hess;
     b.sp_in[0] = dense_sp(Nx, Nt); b.sp_in[1] = dense_sp(Nx, (casadi_int)Nx * Nt);
     b.sp_out[0] = dense_sp(Ny, Nt); b.sp_out[1] = dense_sp(Ny, (casadi_int)Ny * Nt);
     b.sp_jac[0] = blockdiag_sp(Ny, Nx, Nt);
@@ -160,12 +166,21 @@ extern "C" int gp_b200_bind(gpmpc_handle_t h, int method, int Nt)
     const casadi_int n_in[4] = {X * T, X * X * T, Y * T, Y * Y * T};
     for (int o = 0; o < 4; ++o)
         for (int i = 0; i < 4; ++i) b.sp_jj[o * 4 + i] = empty_sp(n_out[o], n_in[i]);
-    b.sp_jj[0] = nodes_sp(n_out[0], X, T, [&](casadi_int t) {         // jac_mean_z (a + Y t, d + X t) / z
+    auto mean_z_rows = [&](casadi_int t) {                            // jac_mean_z (a + Y t, d + X t)
         std::vector<casadi_int> r;
         for (casadi_int d = 0; d < X; ++d)
             for (casadi_int a = 0; a < Y; ++a) r.push_back((a + Y * t) + Y * T * (d + X * t));
         return r;
-    });
+    };
+    auto cov_s_rows = [&](casadi_int t) {                             // jac_cov_sigma (a + Y b + Y^2 t, d + X e + X^2 t)
+        std::vector<casadi_int> r;
+        for (casadi_int e = 0; e < X; ++e)
+            for (casadi_int d = 0; d < X; ++d)
+                for (casadi_int bb = 0; bb < Y; ++bb)
+                    for (casadi_int a = 0; a < Y; ++a) r.push_back((a + Y * bb + Y * Y * t) + Y * Y * T * (d + X * e + X * X * t));
+        return r;
+    };
+    b.sp_jj[0] = nodes_sp(n_out[0], X, T, mean_z_rows);
     auto cov_z_rows = [&](casadi_int t) {                             // jac_cov_z (a + Y b + Y^2 t, e + X t)
         std::vector<casadi_int> r;
         for (casadi_int e = 0; e < X; ++e)
@@ -176,17 +191,37 @@ extern "C" int gp_b200_bind(gpmpc_handle_t h, int method, int Nt)
     b.sp_jj[8] = nodes_sp(n_out[2], X, T, cov_z_rows);
     if (method == GPMPC_METHOD_TA) {
         b.sp_jj[9] = nodes_sp(n_out[2], X * X, T, cov_z_rows);
-        b.sp_jj[12] = nodes_sp(n_out[3], X, T, [&](casadi_int t) {   // jac_cov_sigma (a + Y b + Y^2 t, d + X e + X^2 t) / z
+        b.sp_jj[12] = nodes_sp(n_out[3], X, T, cov_s_rows);
+    }
+    b.mSz.clear(); b.mSS.clear(); b.cSz.clear(); b.cSS.clear();
+    if (em_hess) {
+        const size_t t = Nt, x = Nx, y = Ny;
+        b.mSz.assign(t * y * x * x * x, 0.0); b.mSS.assign(t * y * x * x * x * x, 0.0);
+        b.cSz.assign(t * y * y * x * x * x, 0.0); b.cSS.assign(t * y * y * x * x * x * x, 0.0);
+        auto mean_s_rows = [&](casadi_int t) {                        // jac_mean_sigma (a + Y t, d + X e + X^2 t)
             std::vector<casadi_int> r;
             for (casadi_int e = 0; e < X; ++e)
                 for (casadi_int d = 0; d < X; ++d)
-                    for (casadi_int bb = 0; bb < Y; ++bb)
-                        for (casadi_int a = 0; a < Y; ++a) r.push_back((a + Y * bb + Y * Y * t) + Y * Y * T * (d + X * e + X * X * t));
+                    for (casadi_int a = 0; a < Y; ++a) r.push_back((a + Y * t) + Y * T * (d + X * e + X * X * t));
             return r;
-        });
+        };
+        b.sp_jj[1] = nodes_sp(n_out[0], X * X, T, mean_z_rows);
+        b.sp_jj[4] = nodes_sp(n_out[1], X, T, mean_s_rows);
+        b.sp_jj[5] = nodes_sp(n_out[1], X * X, T, mean_s_rows);
+        b.sp_jj[9] = nodes_sp(n_out[2], X * X, T, cov_z_rows);
+        b.sp_jj[12] = nodes_sp(n_out[3], X, T, cov_s_rows);
+        b.sp_jj[13] = nodes_sp(n_out[3], X * X, T, cov_s_rows);
     }
     return GPMPC_OK;
 }
+}  // namespace
+
+// Bind the (process-global) external to a factorised engine handle: method GPMPC_METHOD_ME / _TA / _EM,
+// Nt shooting nodes per call.  Call again to re-bind (e.g. after a refit or another horizon).
+extern "C" int gp_b200_bind(gpmpc_handle_t h, int method, int Nt) { return bind(h, method, Nt, false); }
+
+// As gp_b200_bind(h, GPMPC_METHOD_EM, Nt), with jac_jac_gp_b200 served from gpmpc_predict_em_hess (Nx <= 16)
+extern "C" int gp_b200_bind_em_hess(gpmpc_handle_t h, int Nt) { return bind(h, GPMPC_METHOD_EM, Nt, true); }
 
 extern "C" void gp_b200_unbind(void)
 {
@@ -370,6 +405,68 @@ extern "C" int jac_jac_gp_b200(const casadi_real** arg, casadi_real** res, casad
                 for (size_t e = 0; e < Nx; ++e)
                     for (size_t bb = 0; bb < Ny; ++bb)
                         for (size_t a = 0; a < Ny; ++a) res[8][k++] = b.d2cov[((((t * Ny + a) * Ny + bb) * Nx + e) * Nx + f)];
+    }
+    if (b.method == GPMPC_METHOD_EM) {
+        // column f (z_f) or f + Nx g (Sigma[f][g]); rows as the vec of the differentiated jac_gp_b200 output
+        const size_t X = Nx, Y = Ny;
+        auto mz = [&](size_t t, size_t a, size_t d, size_t e, size_t f) { return b.mSz[(((t * Y + a) * X + d) * X + e) * X + f]; };
+        auto cz = [&](size_t t, size_t a, size_t bb, size_t d, size_t e, size_t f) { return b.cSz[((((t * Y + a) * Y + bb) * X + d) * X + e) * X + f]; };
+        size_t k;
+        if (res[1]) {    // d dmean_dz[a][d] / d Sigma[f][g] = d2mean_dSigma_dz[a][f][g][d]; rows (d, a)
+            k = 0;
+            for (size_t t = 0; t < Nt; ++t)
+                for (size_t g = 0; g < X; ++g)
+                    for (size_t f = 0; f < X; ++f)
+                        for (size_t d = 0; d < X; ++d)
+                            for (size_t a = 0; a < Y; ++a) res[1][k++] = mz(t, a, f, g, d);
+        }
+        if (res[4]) {    // d dmean_dSigma[a][d][e] / d z_f; rows (e, d, a)
+            k = 0;
+            for (size_t t = 0; t < Nt; ++t)
+                for (size_t f = 0; f < X; ++f)
+                    for (size_t e = 0; e < X; ++e)
+                        for (size_t d = 0; d < X; ++d)
+                            for (size_t a = 0; a < Y; ++a) res[4][k++] = mz(t, a, d, e, f);
+        }
+        if (res[5]) {    // d dmean_dSigma[a][d][e] / d Sigma[f][g]; rows (e, d, a)
+            k = 0;
+            for (size_t t = 0; t < Nt; ++t)
+                for (size_t g = 0; g < X; ++g)
+                    for (size_t f = 0; f < X; ++f)
+                        for (size_t e = 0; e < X; ++e)
+                            for (size_t d = 0; d < X; ++d)
+                                for (size_t a = 0; a < Y; ++a) res[5][k++] = b.mSS[((((t * Y + a) * X + d) * X + e) * X + f) * X + g];
+        }
+        if (res[9]) {    // d dcov_dz[a][b][e] / d Sigma[f][g] = d2cov_dSigma_dz[a][b][f][g][e]; rows (e, b, a)
+            k = 0;
+            for (size_t t = 0; t < Nt; ++t)
+                for (size_t g = 0; g < X; ++g)
+                    for (size_t f = 0; f < X; ++f)
+                        for (size_t e = 0; e < X; ++e)
+                            for (size_t bb = 0; bb < Y; ++bb)
+                                for (size_t a = 0; a < Y; ++a) res[9][k++] = cz(t, a, bb, f, g, e);
+        }
+        if (res[12]) {   // d dcov_dSigma[a][b][d][e] / d z_f; rows (e, d, b, a)
+            k = 0;
+            for (size_t t = 0; t < Nt; ++t)
+                for (size_t f = 0; f < X; ++f)
+                    for (size_t e = 0; e < X; ++e)
+                        for (size_t d = 0; d < X; ++d)
+                            for (size_t bb = 0; bb < Y; ++bb)
+                                for (size_t a = 0; a < Y; ++a) res[12][k++] = cz(t, a, bb, d, e, f);
+        }
+        if (res[13]) {   // d dcov_dSigma[a][b][d][e] / d Sigma[f][g]; rows (e, d, b, a)
+            k = 0;
+            for (size_t t = 0; t < Nt; ++t)
+                for (size_t g = 0; g < X; ++g)
+                    for (size_t f = 0; f < X; ++f)
+                        for (size_t e = 0; e < X; ++e)
+                            for (size_t d = 0; d < X; ++d)
+                                for (size_t bb = 0; bb < Y; ++bb)
+                                    for (size_t a = 0; a < Y; ++a)
+                                        res[13][k++] = b.cSS[(((((t * Y + a) * Y + bb) * X + d) * X + e) * X + f) * X + g];
+        }
+        return 0;
     }
     if (b.method != GPMPC_METHOD_TA) return 0;
     if (res[9]) {        // column d' + Nx e' (vec of Sigma), rows (e, b, a):  d^2 cov[a][b] / d z_e d Sigma[d'][e']

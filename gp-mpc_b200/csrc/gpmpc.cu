@@ -9,6 +9,10 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
+#include <functional>
+#include <map>
+#include <memory>
 #include <type_traits>
 #include <vector>
 
@@ -80,6 +84,56 @@ struct DevBuf {
     void release() { cudaFree(p); p = nullptr; cap = 0; }     // the caller has drained the streams that use it
 };
 
+// 'EM' second derivatives (gpmpc_predict_em_hess): unique monomials of degree <= 4 in Nx variables (by degree, then lexicographic over sorted index tuples), the index
+// of every (unsorted) k-tuple, and the record entries (owner monomial, feature of degree <= 2) with total degree <= 4
+struct EmHessTables {
+    int Nx = 0, nf = 0, nent = 0;
+    std::vector<int> mono, ent, entpos, deg;
+    std::vector<int> mid[5];
+    std::vector<int> dev;                  // the device copy's layout: [mono | ent | mid (orders 0..4 back to back) | entpos]
+    const int* uploaded_to = nullptr;      // the device buffer dev was copied to
+    explicit EmHessTables(int nx) : Nx(nx)
+    {
+        std::map<std::array<int, 4>, int> idx;
+        for (int k = 0; k <= 4; ++k) {
+            std::array<int, 4> t = {-1, -1, -1, -1};
+            std::function<void(int, int)> rec = [&](int s, int lo) {
+                if (s == k) {
+                    idx[t] = (int)deg.size();
+                    for (int q = 0; q < 4; ++q) mono.push_back(t[q]);
+                    deg.push_back(k);
+                    return;
+                }
+                for (int d = lo; d < Nx; ++d) { t[s] = d; rec(s + 1, d); }
+                t[s] = -1;
+            };
+            rec(0, 0);
+            if (k == 2) nf = (int)deg.size();
+            long long nk = 1;
+            for (int q = 0; q < k; ++q) nk *= Nx;
+            mid[k].resize(nk);
+            for (long long f = 0; f < nk; ++f) {
+                std::array<int, 4> u = {-1, -1, -1, -1};
+                long long r = f;
+                for (int q = k - 1; q >= 0; --q) { u[q] = (int)(r % Nx); r /= Nx; }
+                std::sort(u.begin(), u.begin() + k);
+                mid[k][f] = idx[u];
+            }
+        }
+        const int nm = (int)deg.size();
+        entpos.assign((size_t)nm * nf, -1);
+        for (int m = 0; m < nm; ++m)
+            for (int f = 0; f < nf; ++f)
+                if (deg[m] + deg[f] <= 4) { entpos[(size_t)m * nf + f] = nent++; ent.push_back(m); ent.push_back(f); }
+        dev = mono;
+        dev.insert(dev.end(), ent.begin(), ent.end());
+        for (int k = 0; k <= 4; ++k) dev.insert(dev.end(), mid[k].begin(), mid[k].end());
+        dev.insert(dev.end(), entpos.begin(), entpos.end());
+    }
+    const int* d_mid(const int* base) const { return base + mono.size() + ent.size(); }
+    const int* d_entpos(const int* base) const { return d_mid(base) + mid[0].size() + mid[1].size() + mid[2].size() + mid[3].size() + mid[4].size(); }
+};
+
 struct gpmpc_handle_s {
     int N = 0, Nx = 0, Ny = 0, a0 = 0, nloc = 0, Npad = 0, device = 0;
     int nloc_max = 0;                 // ceil(Ny / world): slots per rank in the gather buffer
@@ -131,6 +185,9 @@ struct gpmpc_handle_s {
     // EM derivatives: full symmetric K^-1 per output (lazy, one per factorisation), record partials and sums,
     // backbone rows [e | e v_d] and their L^-1 products
     DevBuf<double> dEmKinv, dEmGPart, dEmGRec, dEmBB; bool em_kinv_valid = false;
+    // EM second derivatives: degree-4 record partials and sums, backbone feature rows, monomial / entry tables
+    DevBuf<double> dEmHPart, dEmHRec, dEmHBB, dEmHEHP, dEmHMU, dEmHD, dEmHScr, dEmHOut; DevBuf<int> dEmHIdx;
+    std::unique_ptr<EmHessTables> em_tb;    // built once (they depend on Nx only), uploaded to dEmHIdx once
     std::vector<double> hyper;        // (nloc, Nx+2)
     // host copy of X (N, Nx) row-major, kept by set_data, append, append_greedy and remove: the K build's centre dMu is
     // recomputed from it (mu_stale) before the next K build, so appends and removals never leave K centred on an old mean
@@ -1714,8 +1771,105 @@ static int em_grad_finish(gpmpc_handle_t h, const double* S, const double* emp, 
     return GPMPC_OK;
 }
 
+// ------------------------------------------------------------------------------------
+// 'EM' second derivatives (gpmpc_predict_em_hess, DESIGN 4.8).  Every term of mean and cov is a Gaussian expectation,
+// Gaussian in z, so its z-derivatives are Hermite polynomials of (y, S): He_1 = y, He_2 = y y - S,
+// He_3 = y y y - 3 sym(S y), He_4 = y^4 - 6 sym(S y y) + 3 sym(S S); and d/dSigma = 1/2 d^2/dz^2 (heat equation).  The
+// device writes degree-4 records (kernels.cuh, em_hess_*); the host forms d^k mean_a / dz^k (k <= 4) and d^k cov_ab / dz^k
+// (k = 2..4) from them and assembles the Sigma blocks.  Record order per point:
+//   [mean a (weights beta_a q_a) | cross pair p, owner rows / columns | trace remainder a | trace backbone a]
+// ------------------------------------------------------------------------------------
+struct EmHessOutputs {
+    double *d2mean_dz2, *d2mean_dSigma_dz, *d2mean_dSigma2, *d2cov_dz2, *d2cov_dSigma_dz, *d2cov_dSigma2;
+};
+
+template <int NXP>
+static cudaError_t launch_em_hess(gpmpc_handle_t h, const EmHessTables& tb, const double* dz, const double* dP, int npairs,
+                                  int nb, double* rec_out)
+{
+    const int N = h->N, Nx = h->Nx, Ny = h->Ny, np = h->Npad, nf = tb.nf, RL = tb.nent;
+    constexpr int NFP = 1 + NXP + NXP * (NXP + 1) / 2;
+    const int r_cross = Ny, r_tr = Ny + 2 * npairs, r_bb = r_tr + Ny, nrec = r_bb + Ny;
+    const int* MONO = h->dEmHIdx;
+    const int* ENT = MONO + tb.mono.size();
+    double* part = h->dEmHPart;
+    const long long srec = (long long)nb * RL;
+    const int smem_pair = (4 * NXP * 64 + 64 * 65 + NFP * 64) * 8, smem_own = (NXP * 64 + 64 * NFP) * 8;
+    cudaError_t e = smem_opt_in<em_hess_pair_kernel<NXP>>(smem_pair);
+    if (e == cudaSuccess) e = smem_opt_in<em_hess_owner_kernel<NXP>>(smem_own);
+    if (e != cudaSuccess) return e;
+    em_hess_owner_kernel<NXP><<<dim3(nb, Ny), 256, smem_own, h->st>>>(h->dXT, np, N, Nx, dz, h->dAlpha, h->dEmLQ, np, nullptr, 0, 0, 1,
+                                                                      MONO, ENT, RL, part, srec);
+    em_hess_pair_kernel<NXP><<<dim3(nb, npairs, 2), 256, smem_pair, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE,
+                                                                            h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2,
+                                                                            nullptr, 0, r_cross, MONO, ENT, RL, part, nb);
+    em_hess_pair_kernel<NXP><<<dim3(nb, Ny, 1), 256, smem_pair, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE,
+                                                                        h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2,
+                                                                        h->dEmKinv, 1, r_tr, MONO, ENT, RL, part, nb);
+    if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    // rank-one backbone e e^T of Q_aa: Z_f = K^-1 (e o mono_f) = L^-T L^-1 (e o mono_f) for the nf features, then owner
+    // records with features e_i Z_f,i
+    double* rows = h->dEmHBB;
+    double* prod = rows + (long long)nf * np;
+    double* kz = prod + (long long)nf * np;
+    for (int a = 0; a < Ny; ++a) {
+        const int paa = a * (a + 1) / 2 + a;
+        const double* Li = h->dLi + (long long)a * slab(h);
+        em_hess_bb_rows_kernel<<<(np + 255) / 256, 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, h->dEmE + (long long)paa * np, np, MONO, nf, rows);
+        trmv_lower_kernel<<<dim3((np + 7) / 8, 1, nf), 256, 0, h->st>>>(Li, np, 0, rows, np, prod, np, np);
+        trmv_lower_T_kernel<<<dim3(np / 32, 1, nf), 256, 0, h->st>>>(Li, np, 0, prod, np, kz, np, np);
+        em_hess_owner_kernel<NXP><<<dim3(nb, 1), 256, smem_own, h->st>>>(h->dXT, np, N, Nx, dz, nullptr, h->dEmE + (long long)paa * np, 0,
+                                                                         kz, 0, np, nf, MONO, ENT, RL, part + (long long)(r_bb + a) * srec, 0);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    em_sum_parts_kernel<<<nrec, 256, 0, h->st>>>(part, nb, RL, rec_out);
+    return cudaGetLastError();
+}
+
+// per (point, pair) inputs of em_hess_pair_finish_kernel, formed as em_grad_finish forms them (O(Nx^3)):
+// [Fa Fb CP At Bt sAt sBt sFa sFb] (Nx^2 each), t;  C = (I + P Sigma)^-1, Fa = C La^-1, Fb = C Lb^-1, CP = C P (symmetric
+// part), At = Fa - iR_a = -C Lb^-1 Sigma iR_a and Bt = Fb - iR_b (as products, not differences), sX = symmetric part of X
+static int em_hess_pair_params(gpmpc_handle_t h, const double* S, const double* emp, double* out)
+{
+    const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, m = Nx + 2;
+    std::vector<double> t1(nn), C(nn), ila(Nx), ilb(Nx);
+    int p = 0;
+    for (int a = 0; a < Ny; ++a)
+        for (int b = 0; b <= a; ++b, ++p) {
+            const double* la = &h->hyper[(size_t)a * m];
+            const double* lb = &h->hyper[(size_t)b * m];
+            const double* iRa = emp + (size_t)a * (2 * nn + 2);
+            const double* iRb = emp + (size_t)b * (2 * nn + 2);
+            double* o = out + (size_t)p * (9 * nn + 1);
+            double *Fa = o, *Fb = o + nn, *CP = o + 2 * nn, *At = o + 3 * nn, *Bt = o + 4 * nn, *sAt = o + 5 * nn;
+            double *sBt = o + 6 * nn, *sFa = o + 7 * nn, *sFb = o + 8 * nn;
+            for (int d = 0; d < Nx; ++d) { ila[d] = 1.0 / (la[d] * la[d]); ilb[d] = 1.0 / (lb[d] * lb[d]); }
+            for (int i = 0; i < Nx; ++i)
+                for (int j = 0; j < Nx; ++j) t1[i * Nx + j] = (i == j ? 1.0 : 0.0) + (ila[i] + ilb[i]) * S[i * Nx + j];
+            if (!mat_inv(Nx, t1.data(), C.data())) { set_error(h, "EM: I + P Sigma is singular"); return GPMPC_ERR_ARG; }
+            for (int i = 0; i < Nx; ++i)
+                for (int j = 0; j < Nx; ++j) {
+                    Fa[i * Nx + j] = C[i * Nx + j] * ila[j]; Fb[i * Nx + j] = C[i * Nx + j] * ilb[j];
+                    CP[i * Nx + j] = C[i * Nx + j] * (ila[j] + ilb[j]);
+                }
+            for (int i = 0; i < Nx; ++i)        // CP = (P^-1 + Sigma)^-1 is symmetric: use the symmetric part
+                for (int j = 0; j < i; ++j) CP[i * Nx + j] = CP[j * Nx + i] = 0.5 * (CP[i * Nx + j] + CP[j * Nx + i]);
+            mat_mul(Nx, Fb, S, t1.data()); mat_mul(Nx, t1.data(), iRa, At);
+            mat_mul(Nx, Fa, S, t1.data()); mat_mul(Nx, t1.data(), iRb, Bt);
+            for (int q = 0; q < nn; ++q) { At[q] = -At[q]; Bt[q] = -Bt[q]; }
+            for (int i = 0; i < Nx; ++i)
+                for (int j = 0; j < Nx; ++j) {
+                    sAt[i * Nx + j] = 0.5 * (At[i * Nx + j] + At[j * Nx + i]); sBt[i * Nx + j] = 0.5 * (Bt[i * Nx + j] + Bt[j * Nx + i]);
+                    sFa[i * Nx + j] = iRa[i * Nx + j] + sAt[i * Nx + j]; sFb[i * Nx + j] = iRb[i * Nx + j] + sBt[i * Nx + j];
+                }
+            o[9 * nn] = emp[(size_t)Ny * (2 * nn + 2) + (size_t)p * (nn + 4) + nn];
+        }
+    return GPMPC_OK;
+}
+
 static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Sigma, int spp,
-                      double* mean, double* var, double* cov, const EmGradOutputs* go = nullptr)
+                      double* mean, double* var, double* cov, const EmGradOutputs* go = nullptr,
+                      const EmHessOutputs* ho = nullptr)
 {
     const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, np = h->Npad;
     NvtxRange nvtx_r("gpmpc.predict_em");
@@ -1738,6 +1892,30 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
         ENSURE(h->dEmGPart, (long long)nrec * T * RL);
         ENSURE(h->dEmGRec, (long long)H * nrec * RL);
         ENSURE(h->dEmBB, (2LL * (Nx + 1) + 1) * np);
+    }
+    EmHessTables* tb = nullptr;
+    const int nrech = 3 * Ny + 2 * npairs;
+    const long long TS = 1 + Nx + nn + (long long)nn * Nx + (long long)nn * nn, Q = (long long)nn * nn;
+    const long long per_pair = 6 * TS + 8 * Q, nout = (long long)nn + nn * Nx + nn * nn;    // finish scratch per CTA; one output slab
+    const int Hc = (int)std::max(1LL, std::min((long long)H, (64LL << 20) / ((long long)npairs * per_pair)));   // points per finish launch
+    if (ho) {
+        if (!h->em_tb) h->em_tb.reset(new EmHessTables(Nx));
+        tb = h->em_tb.get();
+        ENSURE(h->dEmHPart, (long long)nrech * T * tb->nent);
+        ENSURE(h->dEmHRec, (long long)H * nrech * tb->nent);
+        ENSURE(h->dEmHBB, 3LL * tb->nf * np);
+        ENSURE(h->dEmHEHP, (long long)H * npairs * (9 * nn + 1));
+        ENSURE(h->dEmHMU, (long long)H * Ny * TS);
+        ENSURE(h->dEmHD, (long long)H * Ny * TS);
+        ENSURE(h->dEmHScr, std::max((long long)H * Ny * Q, (long long)Hc * npairs * per_pair));
+        ENSURE(h->dEmHOut, (long long)H * (Ny + Ny * Ny) * nout);
+        ENSURE(h->dEmHIdx, (long long)tb->dev.size());
+        if (tb->uploaded_to != h->dEmHIdx.p) {
+            CUDA_TRY(cudaMemcpyAsync(h->dEmHIdx, tb->dev.data(), tb->dev.size() * 4, cudaMemcpyHostToDevice, h->st));
+            tb->uploaded_to = h->dEmHIdx.p;
+        }
+    }
+    if (go || ho) {
         ENSURE(h->dEmKinv, (long long)Ny * slab(h));
         if (!h->em_kinv_valid) {        // K^-1 = U U^T per output (compute_kinv, lower), stored full and symmetric
             for (int a = 0; a < Ny; ++a) {
@@ -1795,26 +1973,60 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
             double* rec = h->dEmGRec + (size_t)p * nrec * RL;
             CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_grad<decltype(nxp)::value>(h, dz, dP, npairs, T, rec); }));
         }
+        if (ho) {
+            double* rec = h->dEmHRec + (size_t)p * nrech * tb->nent;
+            CUDA_TRY(Nx <= 8 ? launch_em_hess<8>(h, *tb, dz, dP, npairs, T, rec) : launch_em_hess<16>(h, *tb, dz, dP, npairs, T, rec));   // Nx <= 16
+        }
     }
     if (mean) CUDA_TRY(cudaMemcpyAsync(mean, h->dMean, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
     if (var) CUDA_TRY(cudaMemcpyAsync(var, h->dVar, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
     if (cov) CUDA_TRY(cudaMemcpyAsync(cov, h->dCov, (size_t)H * Ny * Ny * 8, cudaMemcpyDeviceToHost, h->st));
+    if (ho) {           // the derivatives from the records, on the device: mean part, then the pairs in chunks of points
+        std::vector<double> ehp((size_t)H * npairs * (9 * nn + 1));
+        for (int p = 0; p < H; ++p) {
+            const int rc = em_hess_pair_params(h, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per,
+                                               ehp.data() + (size_t)p * npairs * (9 * nn + 1));
+            if (rc) return rc;
+        }
+        CUDA_TRY(cudaMemcpyAsync(h->dEmHEHP, ehp.data(), ehp.size() * 8, cudaMemcpyHostToDevice, h->st));
+        const int* MID = tb->d_mid(h->dEmHIdx);
+        const int* ENTPOS = tb->d_entpos(h->dEmHIdx);
+        double* om = h->dEmHOut;
+        double* oc = om + (long long)H * Ny * nout;
+        double *m2 = om, *m3 = m2 + (long long)H * Ny * nn, *m4 = m3 + (long long)H * Ny * nn * Nx;
+        double *c2 = oc, *c3 = c2 + (long long)H * Ny * Ny * nn, *c4 = c3 + (long long)H * Ny * Ny * nn * Nx;
+        em_hess_mean_finish_kernel<<<dim3(Ny, H), 256, 0, h->st>>>(Nx, Ny, h->dEMP, (long long)per, h->dEmHRec, nrech, tb->nent,
+                                                                   MID, ENTPOS, tb->nf, h->dEmHMU, h->dEmHD, h->dEmHScr, m2, m3, m4);
+        CUDA_TRY(cudaGetLastError());
+        for (int h0 = 0; h0 < H; h0 += Hc) {
+            em_hess_pair_finish_kernel<<<dim3(npairs, std::min(Hc, H - h0)), 256, 0, h->st>>>(
+                Nx, Ny, h0, h->dEMP, (long long)per, h->dEmHEHP, h->dEmHRec, nrech, tb->nent, MID, ENTPOS, tb->nf,
+                h->dEmHMU, h->dEmHD, h->dEmHScr, c2, c3, c4);
+            CUDA_TRY(cudaGetLastError());
+        }
+        const double* src[6] = {m2, m3, m4, c2, c3, c4};
+        double* dst[6] = {ho->d2mean_dz2, ho->d2mean_dSigma_dz, ho->d2mean_dSigma2, ho->d2cov_dz2, ho->d2cov_dSigma_dz, ho->d2cov_dSigma2};
+        const long long cnt[6] = {(long long)H * Ny * nn, (long long)H * Ny * nn * Nx, (long long)H * Ny * nn * nn,
+                                  (long long)H * Ny * Ny * nn, (long long)H * Ny * Ny * nn * Nx, (long long)H * Ny * Ny * nn * nn};
+        for (int q = 0; q < 6; ++q)
+            if (dst[q]) CUDA_TRY(cudaMemcpyAsync(dst[q], src[q], cnt[q] * 8, cudaMemcpyDeviceToHost, h->st));
+    }
     if (!go) {
         CUDA_TRY(cudaStreamSynchronize(h->st));
-        return GPMPC_OK;
-    }
-    std::vector<double> recs((size_t)H * nrec * RL), mh((size_t)H * Ny);
-    CUDA_TRY(cudaMemcpyAsync(recs.data(), h->dEmGRec, recs.size() * 8, cudaMemcpyDeviceToHost, h->st));
-    CUDA_TRY(cudaMemcpyAsync(mh.data(), h->dMean, mh.size() * 8, cudaMemcpyDeviceToHost, h->st));
-    CUDA_TRY(cudaStreamSynchronize(h->st));
-    for (int p = 0; p < H; ++p) {
-        const int rc = em_grad_finish(h, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per, recs.data() + (size_t)p * nrec * RL,
-                                      mh.data() + (size_t)p * Ny,
-                                      go->dmean_dz ? go->dmean_dz + (size_t)p * Ny * Nx : nullptr,
-                                      go->dmean_dSigma ? go->dmean_dSigma + (size_t)p * Ny * nn : nullptr,
-                                      go->dcov_dz ? go->dcov_dz + (size_t)p * Ny * Ny * Nx : nullptr,
-                                      go->dcov_dSigma ? go->dcov_dSigma + (size_t)p * Ny * Ny * nn : nullptr);
-        if (rc) return rc;
+    } else {
+        std::vector<double> recs((size_t)H * nrec * RL), mh((size_t)H * Ny);
+        CUDA_TRY(cudaMemcpyAsync(recs.data(), h->dEmGRec, recs.size() * 8, cudaMemcpyDeviceToHost, h->st));
+        CUDA_TRY(cudaMemcpyAsync(mh.data(), h->dMean, mh.size() * 8, cudaMemcpyDeviceToHost, h->st));
+        CUDA_TRY(cudaStreamSynchronize(h->st));
+        for (int p = 0; p < H; ++p) {
+            const int rc = em_grad_finish(h, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per, recs.data() + (size_t)p * nrec * RL,
+                                          mh.data() + (size_t)p * Ny,
+                                          go->dmean_dz ? go->dmean_dz + (size_t)p * Ny * Nx : nullptr,
+                                          go->dmean_dSigma ? go->dmean_dSigma + (size_t)p * Ny * nn : nullptr,
+                                          go->dcov_dz ? go->dcov_dz + (size_t)p * Ny * Ny * Nx : nullptr,
+                                          go->dcov_dSigma ? go->dcov_dSigma + (size_t)p * Ny * Ny * nn : nullptr);
+            if (rc) return rc;
+        }
     }
     return GPMPC_OK;
 }
@@ -2486,6 +2698,28 @@ extern "C" int gpmpc_predict_em_grad(gpmpc_handle_t h, int H, const double* Z, c
     const EmGradOutputs go = {dmean_dz, dmean_dSigma, dcov_dz, dcov_dSigma};
     const bool any = dmean_dz || dmean_dSigma || dcov_dz || dcov_dSigma;   // none: the forward call alone, no K^-1 cache
     return predict_em(h, H, Z, Sigma, spp, mean, var, cov, any ? &go : nullptr);
+}
+
+// 'EM' prediction plus its first and second derivatives w.r.t. z and Sigma (see include/gpmpc.h)
+extern "C" int gpmpc_predict_em_hess(gpmpc_handle_t h, int H, const double* Z, const double* Sigma, int spp,
+                                     double* mean, double* var, double* cov,
+                                     double* dmean_dz, double* dmean_dSigma, double* dcov_dz, double* dcov_dSigma,
+                                     double* d2mean_dz2, double* d2mean_dSigma_dz, double* d2mean_dSigma2,
+                                     double* d2cov_dz2, double* d2cov_dSigma_dz, double* d2cov_dSigma2)
+{
+    int rc = predict_guard(h, __func__, GPMPC_METHOD_EM, H);
+    if (rc) return rc;
+    if (!Z || !Sigma) { set_error(h, "gpmpc_predict_em_hess: null Z / Sigma"); return GPMPC_ERR_ARG; }
+    if (h->Nx > 16) { set_error(h, "gpmpc_predict_em_hess supports Nx <= 16"); return GPMPC_ERR_ARG; }
+    if (h->Ny > 44) { set_error(h, "EM supports Ny <= 44"); return GPMPC_ERR_ARG; }
+    rc = predict_prepare(h, __func__, H, true);
+    if (rc) return rc;
+    NvtxRange nvtx_r("gpmpc.predict_em_hess");
+    const EmGradOutputs go = {dmean_dz, dmean_dSigma, dcov_dz, dcov_dSigma};
+    const EmHessOutputs ho = {d2mean_dz2, d2mean_dSigma_dz, d2mean_dSigma2, d2cov_dz2, d2cov_dSigma_dz, d2cov_dSigma2};
+    const bool any_g = dmean_dz || dmean_dSigma || dcov_dz || dcov_dSigma;
+    const bool any_h = d2mean_dz2 || d2mean_dSigma_dz || d2mean_dSigma2 || d2cov_dz2 || d2cov_dSigma_dz || d2cov_dSigma2;
+    return predict_em(h, H, Z, Sigma, spp, mean, var, cov, any_g ? &go : nullptr, any_h ? &ho : nullptr);
 }
 
 // Row Nk of L and L^-1 of every owned output from l = L^-1 k (rows < Nk of dV): r = Li^T l over the Nk rows l occupies,

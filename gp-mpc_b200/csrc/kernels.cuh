@@ -1381,6 +1381,517 @@ __global__ void em_sum_parts_kernel(const double* __restrict__ part, int nb, int
     }
 }
 
+// ---------------------------------------------------------------------------------------
+// 'EM' second derivatives (gpmpc_predict_em_hess).  The records of em_grad extended to degree 4: per owner index k,
+// features F_k,f over the other index (f runs over the unique monomials of degree <= 2 of the other index's v: 1, v_d,
+// v_d v_e with d <= e), and the record entries
+//   sum_k mono_mo(v_k) F_k,f   for every unique owner monomial mo of degree <= 4 with deg mo + deg f <= 4.
+// Monomials are numbered by degree, then lexicographically over sorted index tuples; MONO[4 m + s] holds monomial m's
+// indices (-1 past its degree), ENT[2 q], ENT[2 q + 1] record entry q's (mo, f).  Both tables come from the host
+// (gpmpc.cu, em_hess_tables).  One partial per 64-index owner block, summed by em_sum_parts_kernel.
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ double em_mono(const int* __restrict__ MONO, int m, const double* __restrict__ V, int k)
+{
+    double r = 1.0;
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+        const int d = MONO[4 * m + s];
+        if (d >= 0) r *= V[d * 64 + k];
+    }
+    return r;
+}
+
+// record entries of one owner block: Vown [Nx][64], Fown [64][ldf] (features f < nf; entries with f >= nf are zero)
+__device__ __forceinline__ void em_hess_record(const double* __restrict__ Vown, const double* __restrict__ Fown, int ldf, int nf,
+                                               const int* __restrict__ MONO, const int* __restrict__ ENT, int nent,
+                                               double* __restrict__ out)
+{
+    for (int q = threadIdx.x; q < nent; q += blockDim.x) {
+        const int mo = ENT[2 * q], f = ENT[2 * q + 1];
+        const int d0 = MONO[4 * mo], d1 = MONO[4 * mo + 1], d2 = MONO[4 * mo + 2], d3 = MONO[4 * mo + 3];
+        double s = 0.0;
+        if (f < nf)
+            for (int k = 0; k < 64; ++k) {
+                double r = Fown[k * ldf + f];
+                if (d0 >= 0) r *= Vown[d0 * 64 + k];
+                if (d1 >= 0) r *= Vown[d1 * 64 + k];
+                if (d2 >= 0) r *= Vown[d2 * 64 + k];
+                if (d3 >= 0) r *= Vown[d3 * 64 + k];
+                s += r;
+            }
+        out[q] = s;
+    }
+}
+
+// Owner records with per-owner features: F_k,f = x1_k exp(x2_k) Fc[f][k] (null x1 / Fc count as 1, nf = 1 without Fc),
+// v_k = V[d][k] - z[d], k < n.  One 64-index block per CTA (blockIdx.x), one record per blockIdx.y (x1, x2 offset by sx,
+// Fc by sfc, record by srec).  Serves the mean records (x1 = alpha_a, x2 = log q_a) and the trace backbone (x2 = E,
+// Fc = K^-1 (e o features)).
+template <int NXP>
+__global__ void __launch_bounds__(256)
+em_hess_owner_kernel(const double* __restrict__ V, int ldv, int n, int Nx, const double* __restrict__ z,
+                     const double* __restrict__ x1, const double* __restrict__ x2, long long sx,
+                     const double* __restrict__ Fc, long long sfc, int ldfc, int nf,
+                     const int* __restrict__ MONO, const int* __restrict__ ENT, int nent,
+                     double* __restrict__ part, long long srec)
+{
+    constexpr int NFP = 1 + NXP + NXP * (NXP + 1) / 2;
+    extern __shared__ double sm[];
+    double* Vown = sm;                     // [NXP][64]
+    double* Fown = Vown + NXP * 64;        // [64][NFP]
+    const int tid = threadIdx.x, k0 = blockIdx.x * 64;
+    if (x1) x1 += blockIdx.y * sx;
+    if (x2) x2 += blockIdx.y * sx;
+    if (Fc) Fc += blockIdx.y * sfc;
+    for (int idx = tid; idx < NXP * 64; idx += 256) {
+        const int d = idx >> 6, k = k0 + (idx & 63);
+        Vown[idx] = (d < Nx && k < n) ? V[(long long)d * ldv + k] - z[d] : 0.0;
+    }
+    for (int idx = tid; idx < 64 * nf; idx += 256) {
+        const int kl = idx / nf, f = idx % nf, k = k0 + kl;
+        double w = 0.0;
+        if (k < n) w = (x1 ? x1[k] : 1.0) * (x2 ? exp(x2[k]) : 1.0) * (Fc ? Fc[(long long)f * ldfc + k] : 1.0);
+        Fown[kl * NFP + f] = w;
+    }
+    __syncthreads();
+    em_hess_record(Vown, Fown, NFP, nf, MONO, ENT, nent, part + blockIdx.y * srec + (long long)blockIdx.x * nent);
+}
+
+// Pair records: em_grad_pair_kernel's tiles and weights (mode 0: the cross term's m_ij = w_ij expm1(delta_ij), pair
+// p = blockIdx.y, owner rows (o = 0) or columns (o = 1) by blockIdx.z; mode 1: K^-1_ij times the O(Sigma) remainder of
+// Q_aa, output a = blockIdx.y, owner rows), with the owner's features over every monomial of degree <= 2 of the other
+// index instead of 1 and v (degree <= 1 for o = 1; its other entries are written as zero).  Record rec0 + 2p + o (mode 0) or rec0 + a (mode 1), nent entries each.
+template <int NXP>
+__global__ void __launch_bounds__(256)
+em_hess_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
+                    const double* __restrict__ alpha, long long sal,
+                    const double* __restrict__ XT, int ldx, const double* __restrict__ z,
+                    const double* __restrict__ E, const double* __restrict__ F, const double* __restrict__ W,
+                    const double* __restrict__ IJ, int ldn, const double* __restrict__ LQ,
+                    const double* __restrict__ E2, const double* __restrict__ F2,
+                    const double* __restrict__ Kinv, int mode, int rec0,
+                    const int* __restrict__ MONO, const int* __restrict__ ENT, int nent, double* __restrict__ part, int nb)
+{
+    constexpr int NFP = 1 + NXP + NXP * (NXP + 1) / 2;
+    constexpr int KF = (NFP + 3) / 4;                 // features per thread: f = g + 4q
+    extern __shared__ double sm[];
+    double* Wo = sm;                                  // [NXP][64] W rows of the i block
+    double* Jo = Wo + NXP * 64;                       // [NXP][64] IJ rows of the j block
+    double* Vown = Jo + NXP * 64;                     // [NXP][64] v of the owner block
+    double* Voth = Vown + NXP * 64;                   // [NXP][64] v of the other block
+    double* Ms = Voth + NXP * 64;                     // [64][65] m tile, owner-major
+    double* Foth = Ms + 64 * 65;                      // [NFP][64] features of the other block; then [64][NFP] of the owner
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int o = mode ? 0 : blockIdx.z;
+    // column owners (o = 1) serve only the entries of owner degree >= 3, whose features have degree <= 1
+    const int nn = Nx * Nx, nf = o ? 1 + Nx : 1 + Nx + Nx * (Nx + 1) / 2;
+    const int p = mode ? blockIdx.y * (blockIdx.y + 1) / 2 + blockIdx.y : blockIdx.y;
+    const double* P = EMP + (long long)Ny * (2 * nn + 2) + (long long)p * (nn + 4);
+    const int a = (int)P[nn + 1], b = (int)P[nn + 2];
+    const double cab = P[nn + 3];
+    const double* Ka = mode ? Kinv + (long long)a * ldn * ldn : nullptr;
+    const int own0 = blockIdx.x * 64, T = (N + 63) / 64;
+    for (int idx = tid; idx < NXP * 64; idx += 256) {
+        const int d = idx >> 6, k = own0 + (idx & 63);
+        const bool ok = d < Nx && k < N;
+        Vown[idx] = ok ? XT[(long long)d * ldx + k] - z[d] : 0.0;
+        if (o == 0) Wo[idx] = ok ? W[((long long)p * Nx + d) * ldn + k] : 0.0;
+        else Jo[idx] = ok ? IJ[((long long)p * Nx + d) * ldn + k] : 0.0;
+    }
+    const int ko = tid & 63, g = tid >> 6;
+    double acc2[KF];
+#pragma unroll
+    for (int q = 0; q < KF; ++q) acc2[q] = 0.0;
+    for (int t = 0; t < T; ++t) {
+        const int oth0 = t * 64;
+        __syncthreads();                              // previous tile's readers are done
+        for (int idx = tid; idx < NXP * 64; idx += 256) {
+            const int d = idx >> 6, k = oth0 + (idx & 63);
+            const bool ok = d < Nx && k < N;
+            Voth[idx] = ok ? XT[(long long)d * ldx + k] - z[d] : 0.0;
+            if (o == 0) Jo[idx] = ok ? IJ[((long long)p * Nx + d) * ldn + k] : 0.0;
+            else Wo[idx] = ok ? W[((long long)p * Nx + d) * ldn + k] : 0.0;
+        }
+        __syncthreads();
+        for (int idx = tid; idx < nf * 64; idx += 256) Foth[idx] = em_mono(MONO, idx >> 6, Voth, idx & 63);
+        const int i0 = o ? oth0 : own0, j0 = o ? own0 : oth0;
+        double acc[4][4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) acc[r][c] = 0.0;
+        for (int d = 0; d < Nx; ++d) {
+            double wv[4], jv[4];
+#pragma unroll
+            for (int r = 0; r < 4; ++r) wv[r] = Wo[d * 64 + ty + 16 * r];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) jv[c] = Jo[d * 64 + tx + 16 * c];
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) acc[r][c] = fma(wv[r], jv[c], acc[r][c]);
+        }
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int il = ty + 16 * r, i = i0 + il;
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const int jl = tx + 16 * c, j = j0 + jl;
+                double m = 0.0;
+                if (i < N && j < N) {
+                    if (mode) {
+                        m = Ka[(long long)i * ldn + j] * (exp(E[(long long)p * ldn + i] + F[(long long)p * ldn + j]) * expm1(2.0 * acc[r][c]));
+                    } else {
+                        const double la = LQ[(long long)a * ldn + i], lb = LQ[(long long)b * ldn + j];
+                        const double wgt = (alpha[(long long)a * sal + i] * exp(la)) * (alpha[(long long)b * sal + j] * exp(lb));
+                        m = wgt * expm1(cab + E2[(long long)p * ldn + i] + F2[(long long)p * ldn + j] + 2.0 * acc[r][c]);
+                    }
+                }
+                if (o == 0) Ms[il * 65 + jl] = m; else Ms[jl * 65 + il] = m;
+            }
+        }
+        __syncthreads();
+        for (int x = 0; x < 64; ++x) {
+            const double mv = Ms[ko * 65 + x];
+#pragma unroll
+            for (int q = 0; q < KF; ++q) {
+                const int f = g + 4 * q;
+                if (f < nf) acc2[q] = fma(mv, Foth[f * 64 + x], acc2[q]);
+            }
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int q = 0; q < KF; ++q) {
+        const int f = g + 4 * q;
+        if (f < nf) Foth[ko * NFP + f] = acc2[q];     // owner-major: F_k,f
+    }
+    __syncthreads();
+    const int rec = rec0 + (mode ? (int)blockIdx.y : 2 * p + o);
+    em_hess_record(Vown, Foth, NFP, nf, MONO, ENT, nent, part + ((long long)rec * nb + blockIdx.x) * nent);
+}
+
+// ---------------------------------------------------------------------------------------
+// 'EM' second derivatives from the records (gpmpc_predict_em_hess, DESIGN 4.8).  Dense symmetric tensors of order k <= 4
+// over Nx (row-major), a "family" holds orders 0..4 back to back (offsets emh_off, total emh_off(5)).  The z-derivatives
+// of a Gaussian term are Hermite polynomials He_k(y; S): He_2 = y y - S, He_3 = y y y - (3 placements of S y),
+// He_4 = y^4 - (6 placements of S y y) + (3 pairings of S S); MID (family layout) maps an index tuple to its monomial,
+// ENTPOS[m * nf + f] a (monomial, feature) pair to its record entry.  Every step is block-cooperative (ends synchronised).
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ int emh_pow(int Nx, int k) { int r = 1; for (int q = 0; q < k; ++q) r *= Nx; return r; }
+__device__ __forceinline__ int emh_off(int Nx, int k) { int s = 0, r = 1; for (int q = 0; q < k; ++q) { s += r; r *= Nx; } return s; }
+__device__ __forceinline__ void emh_digits(int f, int Nx, int k, int* d) { for (int q = k - 1; q >= 0; --q) { d[q] = f % Nx; f /= Nx; } }
+__device__ __forceinline__ int emh_sorted(const int* d, int k, int Nx)
+{
+    // a sorting network on four registers, the missing indices above every real one
+    int a0 = d[0], a1 = k > 1 ? d[1] : 1 << 30, a2 = k > 2 ? d[2] : 1 << 30, a3 = k > 3 ? d[3] : 1 << 30;
+#define EMH_CS(x, y) { const int lo_ = min(x, y), hi_ = max(x, y); x = lo_; y = hi_; }
+    EMH_CS(a0, a1) EMH_CS(a2, a3) EMH_CS(a0, a2) EMH_CS(a1, a3) EMH_CS(a1, a2)
+#undef EMH_CS
+    int f = a0;
+    if (k > 1) f = f * Nx + a1;
+    if (k > 2) f = f * Nx + a2;
+    if (k > 3) f = f * Nx + a3;
+    return f;
+}
+
+// dst = (M_0 x ... x M_{k-1}) src (matrix M_s on axis s); tmp: scratch of Nx^k; src aliases neither
+__device__ void emh_modes(const double* src, double* dst, double* tmp, int Nx, int k, const double* const* M)
+{
+    const int n = emh_pow(Nx, k);
+    if (k == 0) { if (threadIdx.x == 0) dst[0] = src[0]; __syncthreads(); return; }
+    const double* in = src;
+    for (int s = 0; s < k; ++s) {
+        double* out = ((k - 1 - s) % 2 == 0) ? dst : tmp;
+        const int inner = emh_pow(Nx, k - 1 - s);
+        const double* Ms = M[s];
+        for (int f = threadIdx.x; f < n; f += blockDim.x) {
+            const int lo = f % inner, hi = f / (inner * Nx), d = (f / inner) % Nx;
+            double acc = 0.0;
+            for (int e = 0; e < Nx; ++e) acc = fma(Ms[d * Nx + e], in[(hi * Nx + e) * inner + lo], acc);
+            out[f] = acc;
+        }
+        __syncthreads();
+        in = out;
+    }
+}
+
+// X[p][q] (i-side axes first) from a record with owner i, or the transposed record with owner j; r2 (optional) is added
+__device__ void emh_expand(const double* r, const double* r2, int pi, int qj, bool owner_j, int Nx,
+                           const int* MID, const int* ENTPOS, int nf, double* X)
+{
+    const int nq = emh_pow(Nx, qj), n = emh_pow(Nx, pi) * nq;
+    const int* ti = MID + emh_off(Nx, pi);
+    const int* tj = MID + emh_off(Nx, qj);
+    for (int x = threadIdx.x; x < n; x += blockDim.x) {
+        const int mi = ti[x / nq], mj = tj[x % nq];
+        const int e = owner_j ? ENTPOS[mj * nf + mi] : ENTPOS[mi * nf + mj];
+        X[x] = r[e] + (r2 ? r2[e] : 0.0);
+    }
+    __syncthreads();
+}
+
+// sum over the placements of S on two of the k axes of index d, T (order k - 2) on the rest
+__device__ double emh_place(const double* S, const double* T, int Nx, int k, const int* d)
+{
+    double s = 0.0;
+    for (int i = 0; i < k; ++i)
+        for (int j = i + 1; j < k; ++j) {
+            int r = 0;
+            for (int q = 0; q < k; ++q) if (q != i && q != j) r = r * Nx + d[q];
+            s += S[d[i] * Nx + d[j]] * T[r];
+        }
+    return s;
+}
+
+// the three pairings S1 (x) S2 of four axes, each symmetrised over which matrix takes which pair
+__device__ double emh_pairings(const double* S1, const double* S2, int Nx, const int* d)
+{
+    const int pr[3][4] = {{0, 1, 2, 3}, {0, 2, 1, 3}, {0, 3, 1, 2}};
+    double s = 0.0;
+    for (int q = 0; q < 3; ++q) {
+        const int* p = pr[q];
+        s += 0.5 * (S1[d[p[0]] * Nx + d[p[1]]] * S2[d[p[2]] * Nx + d[p[3]]] + S2[d[p[0]] * Nx + d[p[1]]] * S1[d[p[2]] * Nx + d[p[3]]]);
+    }
+    return s;
+}
+
+// in place: G_k = sum W y^(x)k  ->  sum W He_k(y; S)  (order 4 first: it reads G_2 and G_0)
+__device__ void emh_hermite(double* G, const double* S, int Nx)
+{
+    const double g0 = G[0];
+    int d[4];
+    for (int x = threadIdx.x; x < emh_pow(Nx, 4); x += blockDim.x) {
+        emh_digits(x, Nx, 4, d);
+        G[emh_off(Nx, 4) + x] += emh_pairings(S, S, Nx, d) * g0 - emh_place(S, G + emh_off(Nx, 2), Nx, 4, d);
+    }
+    for (int x = threadIdx.x; x < emh_pow(Nx, 3); x += blockDim.x) {
+        emh_digits(x, Nx, 3, d);
+        G[emh_off(Nx, 3) + x] -= emh_place(S, G + 1, Nx, 3, d);
+    }
+    __syncthreads();
+    for (int x = threadIdx.x; x < Nx * Nx; x += blockDim.x) G[emh_off(Nx, 2) + x] -= S[x] * g0;
+    __syncthreads();
+}
+
+// G_k = sum W (Mi v_i + Mj v_j)^(x)k from the pair records: over the axis subsets, (Mi.. x Mj..) X_{p,q}.  Records with
+// owner i serve q <= 2, with owner j q >= 3.  Scratch: X (Nx^4), Y (5 Nx^4), tmp (Nx^4).
+__device__ void emh_gmoments(const double* ri, const double* ri2, const double* rj, const double* rj2, const double* Mi,
+                             const double* Mj, int Nx, const int* MID, const int* ENTPOS, int nf,
+                             double* G, double* X, double* Y, double* tmp)
+{
+    const int Q = emh_pow(Nx, 4);
+    for (int k = 0; k <= 4; ++k) {
+        for (int pi = 0; pi <= k; ++pi) {
+            const int qj = k - pi;
+            emh_expand(qj <= 2 ? ri : rj, qj <= 2 ? ri2 : rj2, pi, qj, qj > 2, Nx, MID, ENTPOS, nf, X);
+            const double* Ms[4];
+            for (int s = 0; s < k; ++s) Ms[s] = s < pi ? Mi : Mj;
+            emh_modes(X, Y + (size_t)pi * Q, tmp, Nx, k, Ms);
+        }
+        int d[4];
+        for (int x = threadIdx.x; x < emh_pow(Nx, k); x += blockDim.x) {
+            emh_digits(x, Nx, k, d);
+            double s = 0.0;
+            for (int S = 0; S < (1 << k); ++S) {
+                int fs = 0, fc = 0, ns = 0;
+                for (int q = 0; q < k; ++q) {
+                    if (S >> q & 1) { fs = fs * Nx + d[q]; ++ns; }
+                    else fc = fc * Nx + d[q];
+                }
+                s += Y[(size_t)ns * Q + fs * emh_pow(Nx, k - ns) + fc];
+            }
+            G[emh_off(Nx, k) + x] = s;
+        }
+        __syncthreads();
+    }
+}
+
+// Delta_k = sum u [He_k(F v; sF) - He_k(iR v; iR)] from the v-moments mu (family), telescoped so that every term carries
+// X = F - iR (F^(x)k - iR^(x)k = sum_j F.. X iR..):  no difference of O(1) tensors.  muF: family scratch (orders 1, 2),
+// tj, tmp: Nx^4 scratch.
+__device__ void emh_delta(const double* mu, const double* iR, const double* F, const double* Xm, const double* sX,
+                          const double* sF, int Nx, double* Dl, double* muF, double* tj, double* tmp)
+{
+    for (int k = 0; k <= 4; ++k) {
+        const int n = emh_pow(Nx, k), o = emh_off(Nx, k);
+        for (int x = threadIdx.x; x < n; x += blockDim.x) Dl[o + x] = 0.0;
+        __syncthreads();
+        const double* Ms[4];
+        if (k == 1 || k == 2) {
+            for (int s = 0; s < k; ++s) Ms[s] = F;
+            emh_modes(mu + o, muF + o, tmp, Nx, k, Ms);
+        }
+        for (int j = 0; j < k; ++j) {
+            for (int s = 0; s < k; ++s) Ms[s] = s < j ? F : (s == j ? Xm : iR);
+            emh_modes(mu + o, tj, tmp, Nx, k, Ms);
+            for (int x = threadIdx.x; x < n; x += blockDim.x) Dl[o + x] += tj[x];
+            __syncthreads();
+        }
+    }
+    const double u0 = mu[0];
+    int d[4];
+    for (int x = threadIdx.x; x < emh_pow(Nx, 4); x += blockDim.x) {      // reads Delta_2 before it is adjusted
+        emh_digits(x, Nx, 4, d);
+        Dl[emh_off(Nx, 4) + x] += (emh_pairings(sX, sF, Nx, d) + emh_pairings(iR, sX, Nx, d)) * u0
+                                  - emh_place(sX, muF + emh_off(Nx, 2), Nx, 4, d) - emh_place(iR, Dl + emh_off(Nx, 2), Nx, 4, d);
+    }
+    for (int x = threadIdx.x; x < emh_pow(Nx, 3); x += blockDim.x) {
+        emh_digits(x, Nx, 3, d);
+        Dl[emh_off(Nx, 3) + x] -= emh_place(sX, muF + 1, Nx, 3, d) + emh_place(iR, Dl + 1, Nx, 3, d);
+    }
+    __syncthreads();
+    for (int x = threadIdx.x; x < Nx * Nx; x += blockDim.x) Dl[emh_off(Nx, 2) + x] -= sX[x] * u0;
+    __syncthreads();
+}
+
+// Mean part, one CTA per (output a = blockIdx.x, point blockIdx.y): the v-moments mu (family) from the mean record,
+// D = sum u He_k(iR v; iR) (d^k mean_a / dz^k), and the three mean blocks (each entry read at its sorted index).
+// EMP: the point's em_prepare_point block (stride per), REC: its records (stride nrec * RL), scratch: Nx^4 per CTA.
+__global__ void __launch_bounds__(256)
+em_hess_mean_finish_kernel(int Nx, int Ny, const double* __restrict__ EMP, long long per, const double* __restrict__ REC,
+                           int nrec, int RL, const int* __restrict__ MID, const int* __restrict__ ENTPOS, int nf,
+                           double* __restrict__ MU, double* __restrict__ D, double* __restrict__ scratch,
+                           double* __restrict__ o2, double* __restrict__ o3, double* __restrict__ o4)
+{
+    __shared__ double iR[256];
+    const int a = blockIdx.x, h = blockIdx.y, nn = Nx * Nx, TS = emh_off(Nx, 5);
+    for (int q = threadIdx.x; q < nn; q += blockDim.x) iR[q] = EMP[h * per + (long long)a * (2 * nn + 2) + q];
+    const double* rec = REC + ((long long)h * nrec + a) * RL;
+    double* mu = MU + ((long long)h * Ny + a) * TS;
+    double* Da = D + ((long long)h * Ny + a) * TS;
+    double* tmp = scratch + ((long long)h * Ny + a) * emh_pow(Nx, 4);
+    __syncthreads();
+    const double* Ms[4] = {iR, iR, iR, iR};
+    for (int k = 0; k <= 4; ++k) {
+        emh_expand(rec, nullptr, k, 0, false, Nx, MID, ENTPOS, nf, mu + emh_off(Nx, k));
+        emh_modes(mu + emh_off(Nx, k), Da + emh_off(Nx, k), tmp, Nx, k, Ms);
+    }
+    emh_hermite(Da, iR, Nx);
+    int d[4];
+    const long long ha = (long long)h * Ny + a;
+    for (int x = threadIdx.x; x < nn; x += blockDim.x) { emh_digits(x, Nx, 2, d); o2[ha * nn + x] = Da[emh_off(Nx, 2) + emh_sorted(d, 2, Nx)]; }
+    for (int x = threadIdx.x; x < nn * Nx; x += blockDim.x) { emh_digits(x, Nx, 3, d); o3[ha * nn * Nx + x] = 0.5 * Da[emh_off(Nx, 3) + emh_sorted(d, 3, Nx)]; }
+    for (int x = threadIdx.x; x < nn * nn; x += blockDim.x) { emh_digits(x, Nx, 4, d); o4[ha * nn * nn + x] = 0.25 * Da[emh_off(Nx, 4) + emh_sorted(d, 4, Nx)]; }
+}
+
+// Covariance part, one CTA per (pair p = blockIdx.x, point h0 + blockIdx.y): d^k cov_ab / dz^k (k = 2..4) =
+//   sum m He_k(g; CP)                                      (cross records, expm1 weights)
+// + sum_S Delta_a,|S| (x) (D_b + Delta_b)_|S'| + D_a,|S| (x) Delta_b,|S'|   (w = u_a u_b^T by the Hermite addition formula)
+// - t sum K^-1 Q He_k(g; CP)                               (a = b: trace backbone + remainder records)
+// and the three cov blocks from it and D (heat equation, product rule), each entry formed once per orbit of its index
+// symmetries and written to (a,b) and (b,a).  EHP per (point, pair): [Fa Fb CP At Bt sAt sBt sFa sFb] (Nx^2 each), t.
+__global__ void __launch_bounds__(256, 1)
+em_hess_pair_finish_kernel(int Nx, int Ny, int h0, const double* __restrict__ EMP, long long per, const double* __restrict__ EHP,
+                           const double* __restrict__ REC, int nrec, int RL, const int* __restrict__ MID,
+                           const int* __restrict__ ENTPOS, int nf, const double* __restrict__ MU, const double* __restrict__ D,
+                           double* __restrict__ scratch, double* __restrict__ o2, double* __restrict__ o3, double* __restrict__ o4)
+{
+    __shared__ double Mt[11 * 256];
+    const int p = blockIdx.x, h = h0 + blockIdx.y, nn = Nx * Nx, TS = emh_off(Nx, 5), Q = emh_pow(Nx, 4);
+    const int npairs = gridDim.x;
+    int a = 0;
+    while ((a + 1) * (a + 2) / 2 <= p) ++a;
+    const int b = p - a * (a + 1) / 2;
+    const double* ehp = EHP + ((long long)h * npairs + p) * (9 * nn + 1);
+    for (int q = threadIdx.x; q < 9 * nn; q += blockDim.x) Mt[q] = ehp[q];
+    for (int q = threadIdx.x; q < nn; q += blockDim.x) {
+        Mt[9 * nn + q] = EMP[h * per + (long long)a * (2 * nn + 2) + q];
+        Mt[10 * nn + q] = EMP[h * per + (long long)b * (2 * nn + 2) + q];
+    }
+    const double t = ehp[9 * nn];
+    const double *Fa = Mt, *Fb = Mt + nn, *CP = Mt + 2 * nn, *At = Mt + 3 * nn, *Bt = Mt + 4 * nn, *sAt = Mt + 5 * nn;
+    const double *sBt = Mt + 6 * nn, *sFa = Mt + 7 * nn, *sFb = Mt + 8 * nn, *iRa = Mt + 9 * nn, *iRb = Mt + 10 * nn;
+    double* G = scratch + (long long)blockIdx.y * npairs * (6LL * TS + 8LL * Q) + (long long)p * (6LL * TS + 8LL * Q);
+    double *Tr = G + TS, *Da = Tr + TS, *Db = Da + TS, *muF = Db + TS, *X = muF + TS, *Y = X + Q, *tmp = Y + 5 * Q, *tj = tmp + Q;
+    const double* rec = REC + (long long)h * nrec * RL;
+    const int r_cross = Ny, r_tr = Ny + 2 * npairs, r_bb = r_tr + Ny;
+    __syncthreads();
+    emh_gmoments(rec + (long long)(r_cross + 2 * p) * RL, nullptr, rec + (long long)(r_cross + 2 * p + 1) * RL, nullptr,
+                 Fa, Fb, Nx, MID, ENTPOS, nf, G, X, Y, tmp);
+    emh_hermite(G, CP, Nx);
+    const double* mua = MU + ((long long)h * Ny + a) * TS;
+    const double* mub = MU + ((long long)h * Ny + b) * TS;
+    const double* DA = D + ((long long)h * Ny + a) * TS;
+    const double* DB = D + ((long long)h * Ny + b) * TS;
+    emh_delta(mua, iRa, Fa, At, sAt, sFa, Nx, Da, muF, tj, tmp);
+    emh_delta(mub, iRb, Fb, Bt, sBt, sFb, Nx, Db, muF, tj, tmp);
+    int d[4];
+    for (int k = 2; k <= 4; ++k) {
+        for (int x = threadIdx.x; x < emh_pow(Nx, k); x += blockDim.x) {
+            emh_digits(x, Nx, k, d);
+            double s = 0.0;
+            for (int S = 0; S < (1 << k); ++S) {
+                int fs = 0, fc = 0, ns = 0;
+                for (int q = 0; q < k; ++q) {
+                    if (S >> q & 1) { fs = fs * Nx + d[q]; ++ns; }
+                    else fc = fc * Nx + d[q];
+                }
+                const int os = emh_off(Nx, ns), oc = emh_off(Nx, k - ns);
+                s += Da[os + fs] * (DB[oc + fc] + Db[oc + fc]) + DA[os + fs] * Db[oc + fc];
+            }
+            G[emh_off(Nx, k) + x] += s;
+        }
+    }
+    __syncthreads();
+    if (a == b) {
+        const double* rt = rec + (long long)(r_tr + a) * RL;
+        const double* rb = rec + (long long)(r_bb + a) * RL;
+        emh_gmoments(rt, rb, rt, rb, Fa, Fa, Nx, MID, ENTPOS, nf, Tr, X, Y, tmp);
+        emh_hermite(Tr, CP, Nx);
+        for (int x = threadIdx.x; x < TS; x += blockDim.x) if (x >= emh_off(Nx, 2)) G[x] -= t * Tr[x];
+        __syncthreads();
+    }
+    const double *Ja = DA + 1, *Jb = DB + 1, *Ha = DA + emh_off(Nx, 2), *Hb = DB + emh_off(Nx, 2);
+    const double *M3a = DA + emh_off(Nx, 3), *M3b = DB + emh_off(Nx, 3);
+    const double *C2 = G + emh_off(Nx, 2), *C3 = G + emh_off(Nx, 3), *C4 = G + emh_off(Nx, 4);
+    const long long ab = ((long long)h * Ny + a) * Ny + b, ba = ((long long)h * Ny + b) * Ny + a;
+    for (int x = threadIdx.x; x < nn; x += blockDim.x) {
+        emh_digits(x, Nx, 2, d);
+        o2[ab * nn + x] = o2[ba * nn + x] = C2[emh_sorted(d, 2, Nx)];
+    }
+    for (int x = threadIdx.x; x < nn * Nx; x += blockDim.x) {
+        emh_digits(x, Nx, 3, d);
+        const int dd = min(d[0], d[1]), e = max(d[0], d[1]), f = d[2];
+        const int s3[3] = {dd, e, f};
+        const double v = 0.5 * C3[emh_sorted(s3, 3, Nx)]
+                       + 0.5 * (Ha[dd * Nx + f] * Jb[e] + Ja[dd] * Hb[e * Nx + f] + Hb[dd * Nx + f] * Ja[e] + Jb[dd] * Ha[e * Nx + f]);
+        o3[ab * nn * Nx + x] = o3[ba * nn * Nx + x] = v;
+    }
+    for (int x = threadIdx.x; x < nn * nn; x += blockDim.x) {
+        emh_digits(x, Nx, 4, d);
+        // canonical representative under d <-> e, f <-> g and (d,e) <-> (f,g)
+        int p1a = min(d[0], d[1]), p1b = max(d[0], d[1]), p2a = min(d[2], d[3]), p2b = max(d[2], d[3]);
+        if (p2a < p1a || (p2a == p1a && p2b < p1b)) { int u = p1a; p1a = p2a; p2a = u; u = p1b; p1b = p2b; p2b = u; }
+        const int dd = p1a, e = p1b, f = p2a, g = p2b;
+        const int s4[4] = {dd, e, f, g};
+        auto m3 = [&](const double* T, int i, int j, int k) { const int s[3] = {i, j, k}; return T[emh_sorted(s, 3, Nx)]; };
+        const double lab = m3(M3a, f, dd, e) * Jb[g] + Ha[f * Nx + dd] * Hb[g * Nx + e] + Ha[f * Nx + e] * Hb[g * Nx + dd] + Ja[f] * m3(M3b, g, dd, e);
+        const double lba = m3(M3b, f, dd, e) * Ja[g] + Hb[f * Nx + dd] * Ha[g * Nx + e] + Hb[f * Nx + e] * Ha[g * Nx + dd] + Jb[f] * m3(M3a, g, dd, e);
+        const double v = 0.25 * C4[emh_sorted(s4, 4, Nx)] + 0.25 * (lab + lba)
+                       + 0.25 * (m3(M3a, dd, f, g) * Jb[e] + Ja[dd] * m3(M3b, e, f, g) + m3(M3b, dd, f, g) * Ja[e] + Jb[dd] * m3(M3a, e, f, g));
+        o4[ab * nn * nn + x] = o4[ba * nn * nn + x] = v;
+    }
+}
+
+// backbone feature rows of Q_aa for L^-1: R[f][i] = e_i mono_f(v_i) (f < nf, monomials of degree <= 2); zero for i >= N
+__global__ void em_hess_bb_rows_kernel(const double* __restrict__ XT, int ldx, int N, int Nx, const double* __restrict__ z,
+                                       const double* __restrict__ E, int n, const int* __restrict__ MONO, int nf,
+                                       double* __restrict__ R)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const double e = (i < N) ? exp(E[i]) : 0.0;
+    for (int f = 0; f < nf; ++f) {
+        double r = e;
+        for (int s = 0; s < 4; ++s) {
+            const int d = MONO[4 * f + s];
+            if (d >= 0) r *= (i < N) ? XT[(long long)d * ldx + i] - z[d] : 0.0;
+        }
+        R[(long long)f * n + i] = r;
+    }
+}
+
 // full symmetric copy of a lower-stored matrix (32x32 tiles, every entry taken from the lower triangle)
 __global__ void sym_from_lower_kernel(const double* __restrict__ Kl, double* __restrict__ Kf, int ld)
 {

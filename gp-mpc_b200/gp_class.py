@@ -428,14 +428,7 @@ class GP:
             u = self.standardize(u, self.__meanU, self.__stdU)
         Z = np.hstack([x, u])
         if method == 'EM':
-            g = self.__engine.predict_em_grad(Z, np.zeros((self.__Nx, self.__Nx)) if cov is None else cov)
-            mean, dmz, dmS, dcz = g['mean'], g['dmean_dz'], g['dmean_dSigma'], g['dcov_dz']
-            if self.__normalize:
-                mean = self.inverse_mean(mean, self.__meanY, self.__stdY)
-                dmz = dmz * self.__stdY[None, :, None] / self.__stdZ[None, None, :]
-                dmS = dmS * self.__stdY[None, :, None, None]
-                dcz = dcz / self.__stdZ[None, None, None, :]
-            return dict(mean=mean, cov=g['cov'], dmean_dz=dmz, dcov_dz=dcz, dmean_dSigma=dmS, dcov_dSigma=g['dcov_dSigma'])
+            return self.__em_grad_units(self.__engine.predict_em_grad(Z, np.zeros((self.__Nx, self.__Nx)) if cov is None else cov))
         if cov is None and method == 'TA':
             cov = np.zeros((self.__Nx, self.__Nx))
         g = self.__engine.predict_grad(Z, cov if method == 'TA' else None, _GPU_METHODS[method])
@@ -446,6 +439,47 @@ class GP:
             jac = jac * self.__stdY[None, :, None] / self.__stdZ[None, None, :]
             dcov = dcov / self.__stdZ[None, None, None, :]
         out.update(mean=mean, dmean_dz=jac, dcov_dz=dcov)
+        return out
+
+    def __em_grad_units(self, g):
+        """predict_batch_grad's 'EM' dict from the engine's: mean and the z-derivatives in the caller's units."""
+        mean, dmz, dmS, dcz = g['mean'], g['dmean_dz'], g['dmean_dSigma'], g['dcov_dz']
+        if self.__normalize:
+            mean = self.inverse_mean(mean, self.__meanY, self.__stdY)
+            dmz = dmz * self.__stdY[None, :, None] / self.__stdZ[None, None, :]
+            dmS = dmS * self.__stdY[None, :, None, None]
+            dcz = dcz / self.__stdZ[None, None, None, :]
+        return dict(mean=mean, cov=g['cov'], dmean_dz=dmz, dcov_dz=dcz, dmean_dSigma=dmS, dcov_dSigma=g['dcov_dSigma'])
+
+    def predict_batch_em_hess(self, x, u, cov=None):
+        """'EM' second derivatives for IPOPT's exact Hessian (gpmpc_predict_em_hess): predict_batch_grad(..., method='EM')'s
+        dict (the same bits) plus, for z = [x,u] in the CALLER's units and Sigma in the GP's (standardised) input space,
+            d2mean_dz2       (H,Ny,Nx,Nx)          d dmean_dz[a][d] / dz_e             (stdY_a / (stdZ_d stdZ_e))
+            d2mean_dSigma_dz (H,Ny,Nx,Nx,Nx)       d dmean_dSigma[a][d][e] / dz_f      (stdY_a / stdZ_f)
+            d2mean_dSigma2   (H,Ny,Nx,Nx,Nx,Nx)    d dmean_dSigma[a][d][e] / dSigma[f][g]   (stdY_a)
+            d2cov_dz2        (H,Ny,Ny,Nx,Nx)       d dcov_dz[a][b][d] / dz_e           (1 / (stdZ_d stdZ_e))
+            d2cov_dSigma_dz  (H,Ny,Ny,Nx,Nx,Nx)    d dcov_dSigma[a][b][d][e] / dz_f    (1 / stdZ_f)
+            d2cov_dSigma2    (H,Ny,Ny,Nx,Nx,Nx,Nx) d dcov_dSigma[a][b][d][e] / dSigma[f][g]
+        (cov stays standardised, as in predict_batch_grad).  Errors as predict_batch_grad; Nx <= 16."""
+        if self.__comm.world > 1 and self.__mode == 'outputs':
+            raise NotImplementedError('predict_batch_em_hess needs all outputs on one GPU (build the GP with a single-process Comm)')
+        x = np.asarray(x, dtype=np.float64).reshape(-1, self.__Ny)
+        u = np.asarray(u, dtype=np.float64).reshape(x.shape[0], self.__Nu)
+        if self.__normalize:
+            x = self.standardize(x, self.__meanX, self.__stdX)
+            u = self.standardize(u, self.__meanU, self.__stdU)
+        Z = np.hstack([x, u])
+        g = self.__engine.predict_em_hess(Z, np.zeros((self.__Nx, self.__Nx)) if cov is None else cov)
+        out = self.__em_grad_units(g)
+        h = {k: g[k] for k in ('d2mean_dz2', 'd2mean_dSigma_dz', 'd2mean_dSigma2', 'd2cov_dz2', 'd2cov_dSigma_dz', 'd2cov_dSigma2')}
+        if self.__normalize:
+            sy, iz = self.__stdY, 1.0 / self.__stdZ
+            h['d2mean_dz2'] = h['d2mean_dz2'] * sy[None, :, None, None] * iz[None, None, :, None] * iz[None, None, None, :]
+            h['d2mean_dSigma_dz'] = h['d2mean_dSigma_dz'] * sy[None, :, None, None, None] * iz[None, None, None, None, :]
+            h['d2mean_dSigma2'] = h['d2mean_dSigma2'] * sy[None, :, None, None, None, None]
+            h['d2cov_dz2'] = h['d2cov_dz2'] * iz[None, None, None, :, None] * iz[None, None, None, None, :]
+            h['d2cov_dSigma_dz'] = h['d2cov_dSigma_dz'] * iz[None, None, None, None, None, :]
+        out.update(h)
         return out
 
     def predict_batch_hess(self, x, u, cov=None, method=None):

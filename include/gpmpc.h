@@ -241,6 +241,32 @@ int gpmpc_predict_em_grad(gpmpc_handle_t h, int H, const double* Z, const double
                           double* mean, double* var, double* cov,
                           double* dmean_dz, double* dmean_dSigma, double* dcov_dz, double* dcov_dSigma);
 
+/* 'EM' prediction plus its first and second derivatives w.r.t. z and Sigma: the exact Hessian IPOPT asks for when nlpsol
+ * runs the MPC with gp_method 'EM'.  Inputs as gpmpc_predict_em_grad; the first seven outputs are bit-identical to its.
+ * Every output is optional (NULL to skip).  The differentiated index is always the last one:
+ *   d2mean_dz2        (H,Ny,Nx,Nx)            d dmean_dz[a][d]          / d z_e
+ *   d2mean_dSigma_dz  (H,Ny,Nx,Nx,Nx)         d dmean_dSigma[a][d][e]   / d z_f
+ *   d2mean_dSigma2    (H,Ny,Nx,Nx,Nx,Nx)      d dmean_dSigma[a][d][e]   / d Sigma[f][g]
+ *   d2cov_dz2         (H,Ny,Ny,Nx,Nx)         d dcov_dz[a][b][d]        / d z_e
+ *   d2cov_dSigma_dz   (H,Ny,Ny,Nx,Nx,Nx)      d dcov_dSigma[a][b][d][e] / d z_f
+ *   d2cov_dSigma2     (H,Ny,Ny,Nx,Nx,Nx,Nx)   d dcov_dSigma[a][b][d][e] / d Sigma[f][g]
+ * The mixed block d dmean_dz[a][f] / d Sigma[d][e] is d2mean_dSigma_dz[a][d][e][f] (and likewise for cov): it is not
+ * returned twice.  Sigma entries vary one at a time as in gpmpc_predict_em_grad, whose symmetric gradient is differentiated
+ * w.r.t. the single entry Sigma[f][g]; at a symmetric Sigma the Sigma-Sigma blocks are exactly symmetric under d <-> e,
+ * f <-> g and (d,e) <-> (f,g), the mean blocks fully symmetric (d mean/dSigma = 1/2 d^2 mean/dz^2), and every block
+ * exactly symmetric in (a,b).  Every sum runs in a fixed order: a point's results do not depend on H or its row.
+ * GPMPC_ERR_ARG: Z or Sigma NULL, H < 1, Ny > 44 or Nx > 16; GPMPC_ERR_STATE: not factorised, or the handle does not own
+ * every output; all checked before any work.  Device scratch beyond gpmpc_predict_em_grad's (which includes a full
+ * symmetric K^-1 per output, 8 B Ny Npad^2, kept until the next factor change): 8 B R (3 Ny + Ny (Ny+1)) (ceil(N/64) + H)
+ * + 24 B Npad F, with F = (Nx+1)(Nx+2)/2 and R = the number of (monomial of degree <= 4, monomial of degree <= 2) pairs
+ * of total degree <= 4 (3435 at Nx = 8, 41157 at Nx = 16); for the derivative tensors 8 B H (2 Ny T + Ny(Ny+1)/2 (9 Nx^2 + 1))
+ * with T = 1 + Nx + ... + Nx^4, the outputs 8 B H (Ny + Ny^2)(Nx^2 + Nx^3 + Nx^4), and at most 512 MB of per-CTA scratch. */
+int gpmpc_predict_em_hess(gpmpc_handle_t h, int H, const double* Z, const double* Sigma, int sigma_per_point,
+                          double* mean, double* var, double* cov,
+                          double* dmean_dz, double* dmean_dSigma, double* dcov_dz, double* dcov_dSigma,
+                          double* d2mean_dz2, double* d2mean_dSigma_dz, double* d2mean_dSigma2,
+                          double* d2cov_dz2, double* d2cov_dSigma_dz, double* d2cov_dSigma2);
+
 /* Open-loop multi-step prediction with the state kept on the device: the numeric loop of GP.predict_compare
  * (gp_class.py:746-804, :779-792: mean_t, covar_x = predict(mean_t, u_t, covar); covar[:Ny,:Ny] = covar_x) for a
  * model whose inputs are z = [x, u] (Nx = Ny + Nu).  All Nt steps are enqueued back to back, one synchronisation.

@@ -30,6 +30,12 @@ extern "C" {
 
 /* method GPMPC_METHOD_ME, _TA or _EM; Nt shooting nodes per call.  GPMPC_ERR_ARG otherwise. */
 int gp_b200_bind(gpmpc_handle_t h, int method, int Nt);
+/* As gp_b200_bind(h, GPMPC_METHOD_EM, Nt) -- the same gp_b200 and jac_gp_b200 values and patterns -- with
+ * jac_jac_gp_b200 served from gpmpc_predict_em_hess: the blocks of the four Jacobians w.r.t. z and sigma (output-major
+ * numbering o*4 + i: 0, 1, 4, 5, 8, 9, 12, 13) are block-diagonal over the nodes, rows the column-major vec of the
+ * differentiated Jacobian, column d + Nx*e <-> Sigma[d][e]; the blocks w.r.t. mean and cov stay empty.
+ * GPMPC_ERR_ARG as gp_b200_bind, or Nx > 16. */
+int gp_b200_bind_em_hess(gpmpc_handle_t h, int Nt);
 void gp_b200_unbind(void);
 
 long long gp_b200_n_in(void);
