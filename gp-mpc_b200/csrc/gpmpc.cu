@@ -84,18 +84,19 @@ struct DevBuf {
     void release() { cudaFree(p); p = nullptr; cap = 0; }     // the caller has drained the streams that use it
 };
 
-// 'EM' second derivatives (gpmpc_predict_em_hess): unique monomials of degree <= 4 in Nx variables (by degree, then lexicographic over sorted index tuples), the index
-// of every (unsorted) k-tuple, and the record entries (owner monomial, feature of degree <= 2) with total degree <= 4
-struct EmHessTables {
-    int Nx = 0, nf = 0, nent = 0;
+// 'EM' derivative records of total degree D (2: gpmpc_predict_em_grad, 4: gpmpc_predict_em_hess): the unique monomials of
+// degree <= D in Nx variables (by degree, then lexicographic over sorted index tuples), the index of every (unsorted)
+// k-tuple (mid, k <= D), and the record entries (owner monomial, feature of degree <= D/2) with total degree <= D
+struct EmTables {
+    int Nx = 0, D = 0, nf = 0, nent = 0;
     std::vector<int> mono, ent, entpos, deg;
     std::vector<int> mid[5];
-    std::vector<int> dev;                  // the device copy's layout: [mono | ent | mid (orders 0..4 back to back) | entpos]
+    std::vector<int> dev;                  // the device copy's layout: [mono | ent | mid (orders 0..D back to back) | entpos]
     const int* uploaded_to = nullptr;      // the device buffer dev was copied to
-    explicit EmHessTables(int nx) : Nx(nx)
+    EmTables(int nx, int d) : Nx(nx), D(d)
     {
         std::map<std::array<int, 4>, int> idx;
-        for (int k = 0; k <= 4; ++k) {
+        for (int k = 0; k <= D; ++k) {
             std::array<int, 4> t = {-1, -1, -1, -1};
             std::function<void(int, int)> rec = [&](int s, int lo) {
                 if (s == k) {
@@ -108,7 +109,7 @@ struct EmHessTables {
                 t[s] = -1;
             };
             rec(0, 0);
-            if (k == 2) nf = (int)deg.size();
+            if (k == D / 2) nf = (int)deg.size();
             long long nk = 1;
             for (int q = 0; q < k; ++q) nk *= Nx;
             mid[k].resize(nk);
@@ -124,14 +125,24 @@ struct EmHessTables {
         entpos.assign((size_t)nm * nf, -1);
         for (int m = 0; m < nm; ++m)
             for (int f = 0; f < nf; ++f)
-                if (deg[m] + deg[f] <= 4) { entpos[(size_t)m * nf + f] = nent++; ent.push_back(m); ent.push_back(f); }
+                if (deg[m] + deg[f] <= D) { entpos[(size_t)m * nf + f] = nent++; ent.push_back(m); ent.push_back(f); }
         dev = mono;
         dev.insert(dev.end(), ent.begin(), ent.end());
-        for (int k = 0; k <= 4; ++k) dev.insert(dev.end(), mid[k].begin(), mid[k].end());
+        for (int k = 0; k <= D; ++k) dev.insert(dev.end(), mid[k].begin(), mid[k].end());
         dev.insert(dev.end(), entpos.begin(), entpos.end());
     }
     const int* d_mid(const int* base) const { return base + mono.size() + ent.size(); }
     const int* d_entpos(const int* base) const { return d_mid(base) + mid[0].size() + mid[1].size() + mid[2].size() + mid[3].size() + mid[4].size(); }
+    // records per point: [mean a | cross pair p, owner rows / columns | trace remainder a | trace backbone a | (D = 2) backbone Gram a]
+    int nrec(int Ny) const { return (D == 2 ? 4 : 3) * Ny + Ny * (Ny + 1); }
+};
+
+// One 'EM' record set per D: its tables (built once, they depend on Nx only, and uploaded to idx once), the block
+// partials, the summed records of every point and the backbone rows [e o features | their L^-1 | K^-1 products]
+struct EmRecords {
+    std::unique_ptr<EmTables> tb;
+    DevBuf<double> part, rec, bb;
+    DevBuf<int> idx;
 };
 
 struct gpmpc_handle_s {
@@ -182,12 +193,11 @@ struct gpmpc_handle_s {
     // EM scratch
     DevBuf<double> dEmTr, dEMP, dEmE, dEmF, dEmW, dEmIJ;
     DevBuf<double> dEmMeanPart, dEmPart, dEmLQ, dEmVec, dEmE2, dEmF2;
-    // EM derivatives: full symmetric K^-1 per output (lazy, one per factorisation), record partials and sums,
-    // backbone rows [e | e v_d] and their L^-1 products
-    DevBuf<double> dEmKinv, dEmGPart, dEmGRec, dEmBB; bool em_kinv_valid = false;
-    // EM second derivatives: degree-4 record partials and sums, backbone feature rows, monomial / entry tables
-    DevBuf<double> dEmHPart, dEmHRec, dEmHBB, dEmHEHP, dEmHMU, dEmHD, dEmHScr, dEmHOut; DevBuf<int> dEmHIdx;
-    std::unique_ptr<EmHessTables> em_tb;    // built once (they depend on Nx only), uploaded to dEmHIdx once
+    // EM derivatives: full symmetric K^-1 per output (lazy, one per factorisation), the records of D = 2 and D = 4
+    DevBuf<double> dEmKinv; bool em_kinv_valid = false;
+    EmRecords em_rec[2];
+    // EM second derivatives: per-pair matrices, v-moments, mean derivatives, finish scratch and output slabs
+    DevBuf<double> dEmHEHP, dEmHMU, dEmHD, dEmHScr, dEmHOut;
     std::vector<double> hyper;        // (nloc, Nx+2)
     // host copy of X (N, Nx) row-major, kept by set_data, append, append_greedy and remove: the K build's centre dMu is
     // recomputed from it (mu_stale) before the next K build, so appends and removals never leave K centred on an old mean
@@ -1590,53 +1600,69 @@ static cudaError_t launch_em_prep(gpmpc_handle_t h, int npairs, const double* dz
 }
 
 // ------------------------------------------------------------------------------------
-// 'EM' first derivatives w.r.t. z and Sigma (gpmpc_predict_em_grad).  Per point, after the forward chain, the
-// O(N) / O(N^2) sums go into records (kernels.cuh, em_moments_kernel / em_grad_pair_kernel); the host forms the
-// Nx x Nx derivatives from them (em_grad_finish).  Record order per point:
-//   [mean moments a | cross pair p, owner rows / columns | trace remainder a | backbone a | backbone Gram a]
+// 'EM' derivatives w.r.t. z and Sigma (DESIGN 4.8).  Per point, after the forward chain, the O(N) / O(N^2) sums go into
+// records of total degree D (kernels.cuh, em_owner_rec_kernel / em_pair_rec_kernel; EmTables):
+//   D = 2 (gpmpc_predict_em_grad): the host forms the Nx x Nx first derivatives from them (em_grad_finish).
+//   D = 4 (gpmpc_predict_em_hess): every term of mean and cov is a Gaussian expectation, Gaussian in z, so its
+//     z-derivatives are Hermite polynomials of (y, S): He_1 = y, He_2 = y y - S, He_3 = y y y - 3 sym(S y),
+//     He_4 = y^4 - 6 sym(S y y) + 3 sym(S S); and d/dSigma = 1/2 d^2/dz^2 (heat equation).  The device forms
+//     d^k mean_a / dz^k (k <= 4) and d^k cov_ab / dz^k (k = 2..4) from the records and assembles the Sigma blocks.
 // ------------------------------------------------------------------------------------
 struct EmGradOutputs {
     double *dmean_dz, *dmean_dSigma, *dcov_dz, *dcov_dSigma;
 };
 
-static inline int em_rec_len(int Nx) { return 1 + Nx + 2 * Nx * Nx; }
+struct EmHessOutputs {
+    double *d2mean_dz2, *d2mean_dSigma_dz, *d2mean_dSigma2, *d2cov_dz2, *d2cov_dSigma_dz, *d2cov_dSigma2;
+};
 
-template <int NXP>
-static cudaError_t launch_em_grad(gpmpc_handle_t h, const double* dz, const double* dP, int npairs, int nb, double* rec_out)
+// the records of one point (EmTables::nrec order) into rec_out, through R's partials and backbone rows
+template <int NXP, int D>
+static cudaError_t launch_em_records(gpmpc_handle_t h, const EmRecords& R, const double* dz, const double* dP, int npairs,
+                                     int nb, double* rec_out)
 {
-    const int N = h->N, Nx = h->Nx, Ny = h->Ny, np = h->Npad, RL = em_rec_len(Nx);
-    const int r_cross = Ny, r_tr = Ny + 2 * npairs, r_bb = r_tr + Ny, r_gram = r_bb + Ny, nrec = r_gram + Ny;
-    double* part = h->dEmGPart;
+    const EmTables& tb = *R.tb;
+    const int N = h->N, Nx = h->Nx, Ny = h->Ny, np = h->Npad, nf = tb.nf, RL = tb.nent;
+    constexpr int NFP = em_nmono(NXP, D / 2);
+    const int r_cross = Ny, r_tr = Ny + 2 * npairs, r_bb = r_tr + Ny, r_gram = r_bb + Ny;
+    const int* MONO = R.idx;
+    const int* ENT = MONO + tb.mono.size();
+    double* part = R.part;
     const long long srec = (long long)nb * RL;
-    const int smem = (4 * NXP * 64 + 64 * 65) * 8;
-    cudaError_t e = smem_opt_in<em_grad_pair_kernel<NXP>>(smem);
+    const int smem_pair = (3 * NXP * 64 + 64 * 65 + NFP * 64) * 8, smem_own = (NXP * 64 + 64 * NFP) * 8;
+    cudaError_t e = smem_opt_in<em_pair_rec_kernel<NXP, D>>(smem_pair);
+    if (e == cudaSuccess) e = smem_opt_in<em_owner_rec_kernel<NXP, D>>(smem_own);
     if (e != cudaSuccess) return e;
-    em_moments_kernel<NXP><<<dim3(nb, Ny), 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, h->dAlpha, h->dEmLQ, np, part, srec, RL);
-    em_grad_pair_kernel<NXP><<<dim3(nb, npairs, 2), 256, smem, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE, h->dEmF,
-                                                                        h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2, nullptr, 0,
-                                                                        r_cross, part, nb, RL);
-    em_grad_pair_kernel<NXP><<<dim3(nb, Ny, 1), 256, smem, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE, h->dEmF,
-                                                                    h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2, h->dEmKinv, 1,
-                                                                    r_tr, part, nb, RL);
+    em_owner_rec_kernel<NXP, D><<<dim3(nb, Ny), 256, smem_own, h->st>>>(h->dXT, np, N, Nx, dz, h->dAlpha, h->dEmLQ, np, nullptr, 0, 0, 1,
+                                                                         MONO, ENT, RL, part, srec);
+    em_pair_rec_kernel<NXP, D><<<dim3(nb, npairs, 2), 256, smem_pair, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE,
+                                                                               h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2,
+                                                                               nullptr, 0, r_cross, MONO, ENT, RL, part, nb);
+    em_pair_rec_kernel<NXP, D><<<dim3(nb, Ny, 1), 256, smem_pair, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE,
+                                                                           h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2,
+                                                                           h->dEmKinv, 1, r_tr, MONO, ENT, RL, part, nb);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    // rank-one backbone e e^T of Q_aa through L^-1: u = L^-1 e and Yd = L^-1 (e o v_d) in one batched trmv,
-    // K^-1 e = L^-T u; records of r_i = e_i (K^-1 e)_i and the Gram Y^T Y
-    double* rows = h->dEmBB;
-    double* prod = rows + (long long)(Nx + 1) * np;
-    double* kie = prod + (long long)(Nx + 1) * np;
+    // rank-one backbone e e^T of Q_aa: rows e o mono_f for the nf features through L^-1 in one batched trmv.
+    // D = 2: K^-1 e = L^-T (L^-1 e), owner records of e_i (K^-1 e)_i, and the Gram Y^T Y of Y_d = L^-1 (e o v_d).
+    // D = 4: Z_f = K^-1 (e o mono_f) = L^-T L^-1 (e o mono_f) for every feature, owner records with features e_i Z_f,i.
+    const int nkz = D == 2 ? 1 : nf;
+    double* rows = R.bb;
+    double* prod = rows + (long long)nf * np;
+    double* kz = prod + (long long)nf * np;
     for (int a = 0; a < Ny; ++a) {
         const int paa = a * (a + 1) / 2 + a;
         const double* Li = h->dLi + (long long)a * slab(h);
-        em_bb_rows_kernel<<<(np + 255) / 256, 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, h->dEmE + (long long)paa * np, np, rows);
-        trmv_lower_kernel<<<dim3((np + 7) / 8, 1, Nx + 1), 256, 0, h->st>>>(Li, np, 0, rows, np, prod, np, np);
-        trmv_lower_T_kernel<<<dim3(np / 32, 1, 1), 256, 0, h->st>>>(Li, np, 0, prod, np, kie, np, np);
-        em_moments_kernel<NXP><<<dim3(nb, 1), 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, kie, h->dEmE + (long long)paa * np, 0,
-                                                               part + (long long)(r_bb + a) * srec, 0, RL);
-        em_moments_kernel<NXP><<<dim3(nb, 1), 256, 0, h->st>>>(prod + np, np, N, Nx, nullptr, nullptr, nullptr, 0,
-                                                               part + (long long)(r_gram + a) * srec, 0, RL);
+        em_backbone_rows_kernel<<<(np + 255) / 256, 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, h->dEmE + (long long)paa * np, np, MONO, nf, rows);
+        trmv_lower_kernel<<<dim3((np + 7) / 8, 1, nf), 256, 0, h->st>>>(Li, np, 0, rows, np, prod, np, np);
+        trmv_lower_T_kernel<<<dim3(np / 32, 1, nkz), 256, 0, h->st>>>(Li, np, 0, prod, np, kz, np, np);
+        em_owner_rec_kernel<NXP, D><<<dim3(nb, 1), 256, smem_own, h->st>>>(h->dXT, np, N, Nx, dz, nullptr, h->dEmE + (long long)paa * np, 0,
+                                                                            kz, 0, np, nkz, MONO, ENT, RL, part + (long long)(r_bb + a) * srec, 0);
+        if (D == 2)
+            em_owner_rec_kernel<NXP, D><<<dim3(nb, 1), 256, smem_own, h->st>>>(prod + np, np, N, Nx, nullptr, nullptr, nullptr, 0, nullptr, 0, 0, 1,
+                                                                                MONO, ENT, RL, part + (long long)(r_gram + a) * srec, 0);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
     }
-    em_sum_parts_kernel<<<nrec, 256, 0, h->st>>>(part, nb, RL, rec_out);
+    em_sum_parts_kernel<<<tb.nrec(Ny), 256, 0, h->st>>>(part, nb, RL, rec_out);
     return cudaGetLastError();
 }
 
@@ -1663,14 +1689,47 @@ static bool mat_inv(int n, const double* A, double* Ai)
     return true;
 }
 
-// derivatives of one point from its records (DESIGN 4.8).  emp: the point's em_prepare_point block (iR_a, t_ab),
+// The per-pair matrices of the 'EM' derivatives (O(Nx^3), host): ila, ilb = diag of La^-1, Lb^-1 (inverse squared
+// lengthscales of outputs a and b), C = (I + P Sigma)^-1, Fa = C La^-1, Fb = C Lb^-1, CP = C P,
+// A = -C Lb^-1 Sigma iR_a = C La^-1 - iR_a and B = -C La^-1 Sigma iR_b (formed as products, without the subtraction)
+struct EmPairMats {
+    int Nx;
+    std::vector<double> ila, ilb, C, Fa, Fb, CP, A, B, t;
+    explicit EmPairMats(int nx)
+        : Nx(nx), ila(nx), ilb(nx), C(nx * nx), Fa(nx * nx), Fb(nx * nx), CP(nx * nx), A(nx * nx), B(nx * nx), t(nx * nx) {}
+    int form(gpmpc_handle_t h, const double* S, int a, int b, const double* iRa, const double* iRb)
+    {
+        const int nn = Nx * Nx, m = Nx + 2;
+        const double* la = &h->hyper[(size_t)a * m];
+        const double* lb = &h->hyper[(size_t)b * m];
+        for (int d = 0; d < Nx; ++d) { ila[d] = 1.0 / (la[d] * la[d]); ilb[d] = 1.0 / (lb[d] * lb[d]); }
+        for (int i = 0; i < Nx; ++i)
+            for (int j = 0; j < Nx; ++j) t[i * Nx + j] = (i == j ? 1.0 : 0.0) + (ila[i] + ilb[i]) * S[i * Nx + j];
+        if (!mat_inv(Nx, t.data(), C.data())) { set_error(h, "EM: I + P Sigma is singular"); return GPMPC_ERR_ARG; }
+        for (int i = 0; i < Nx; ++i)
+            for (int j = 0; j < Nx; ++j) {
+                Fa[i * Nx + j] = C[i * Nx + j] * ila[j]; Fb[i * Nx + j] = C[i * Nx + j] * ilb[j];
+                CP[i * Nx + j] = C[i * Nx + j] * (ila[j] + ilb[j]);
+            }
+        mat_mul(Nx, Fb.data(), S, t.data()); mat_mul(Nx, t.data(), iRa, A.data());
+        mat_mul(Nx, Fa.data(), S, t.data()); mat_mul(Nx, t.data(), iRb, B.data());
+        for (int q = 0; q < nn; ++q) { A[q] = -A[q]; B[q] = -B[q]; }
+        return GPMPC_OK;
+    }
+};
+
+// first derivatives of one point from its D = 2 records (DESIGN 4.8).  emp: the point's em_prepare_point block (iR_a, t_ab),
 // rec: its records, mean: its Ny means.  d/dSigma is symmetrised (the gradient at a symmetric Sigma is symmetric).
-static int em_grad_finish(gpmpc_handle_t h, const double* S, const double* emp, const double* rec, const double* mean,
-                          double* dmz, double* dmS, double* dcz, double* dcS)
+static int em_grad_finish(gpmpc_handle_t h, const EmTables& tb, const double* S, const double* emp, const double* rec,
+                          const double* mean, double* dmz, double* dmS, double* dcz, double* dcS)
 {
-    const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, m = Nx + 2, RL = em_rec_len(Nx), npairs = Ny * (Ny + 1) / 2;
+    const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, npairs = Ny * (Ny + 1) / 2;
     const int r_cross = Ny, r_tr = Ny + 2 * npairs, r_bb = r_tr + Ny, r_gram = r_bb + Ny;
-    auto R = [&](int r) { return rec + (size_t)r * RL; };
+    const int *M1 = tb.mid[1].data(), *M2 = tb.mid[2].data();
+    // entry (owner monomial mo, feature f) of record r: at(r, 0, 0) = sum m, at(r, M1[d], 0) = sum m v_d,
+    // at(r, M2[d Nx + e], 0) = sum m v_d v_e, at(r, 0, M1[e]) = sum m v'_e and at(r, M1[d], M1[e]) = sum m v_d v'_e
+    // (v' the other index's v)
+    auto at = [&](int r, int mo, int f) { return rec[(size_t)r * tb.nent + tb.entpos[(size_t)mo * tb.nf + f]]; };
     auto sym_store = [&](const double* G, double* o1, double* o2) {
         for (int d = 0; d < Nx; ++d)
             for (int e = 0; e <= d; ++e) {
@@ -1679,12 +1738,16 @@ static int em_grad_finish(gpmpc_handle_t h, const double* S, const double* emp, 
                 if (o2) o2[d * Nx + e] = o2[e * Nx + d] = v;
             }
     };
-    std::vector<double> t1(nn), t2(nn), t3(nn), G(nn), C(nn), A(nn), B(nn), Fa(nn), Fb(nn), CP(nn), Z1(nn), dz(Nx);
-    std::vector<double> ila(Nx), ilb(Nx), ga(Nx), gb(Nx);
+    std::vector<double> t1(nn), t2(nn), t3(nn), G(nn), Z1(nn), dz(Nx), ga(Nx), gb(Nx);
+    std::vector<double> s1((size_t)Ny * Nx), s2((size_t)Ny * nn), u1(Nx), u2(Nx), Mii(nn), Mij(nn), Mjj(nn);
     for (int a = 0; a < Ny; ++a) {
         const double* iR = emp + (size_t)a * (2 * nn + 2);
-        const double* sa = R(a) + 1;
-        const double* Sa = R(a) + 1 + Nx;
+        double* sa = &s1[(size_t)a * Nx];
+        double* Sa = &s2[(size_t)a * nn];
+        for (int d = 0; d < Nx; ++d) {
+            sa[d] = at(a, M1[d], 0);
+            for (int e = 0; e < Nx; ++e) Sa[d * Nx + e] = at(a, M2[d * Nx + e], 0);
+        }
         for (int d = 0; d < Nx; ++d) {
             double s = 0.0;
             for (int k = 0; k < Nx; ++k) s += iR[d * Nx + k] * sa[k];
@@ -1695,32 +1758,28 @@ static int em_grad_finish(gpmpc_handle_t h, const double* S, const double* emp, 
         for (int q = 0; q < nn; ++q) G[q] = 0.5 * G[q] - 0.5 * mean[a] * iR[q];
         if (dmS) sym_store(G.data(), dmS + (size_t)a * nn, nullptr);
     }
+    EmPairMats pm(Nx);
+    const double *ila = pm.ila.data(), *ilb = pm.ilb.data(), *C = pm.C.data(), *Fa = pm.Fa.data(), *Fb = pm.Fb.data();
+    const double *CP = pm.CP.data(), *A = pm.A.data(), *B = pm.B.data();
     int p = 0;
     for (int a = 0; a < Ny; ++a)
         for (int b = 0; b <= a; ++b, ++p) {
-            const double* la = &h->hyper[(size_t)a * m];
-            const double* lb = &h->hyper[(size_t)b * m];
             const double* iRa = emp + (size_t)a * (2 * nn + 2);
             const double* iRb = emp + (size_t)b * (2 * nn + 2);
             const double t = emp[(size_t)Ny * (2 * nn + 2) + (size_t)p * (nn + 4) + nn];
             const double Ma = mean[a], Mb = mean[b];
-            const double *sa = R(a) + 1, *Sa = R(a) + 1 + Nx, *sb = R(b) + 1, *Sb = R(b) + 1 + Nx;
-            for (int d = 0; d < Nx; ++d) { ila[d] = 1.0 / (la[d] * la[d]); ilb[d] = 1.0 / (lb[d] * lb[d]); }
-            // C = (I + P Sigma)^-1, Fa = C La^-1, Fb = C Lb^-1, CP = C P,
-            // A = -C Lb^-1 Sigma iR_a = C La^-1 - iR_a,  B = -C La^-1 Sigma iR_b  (formed without the subtraction)
-            for (int i = 0; i < Nx; ++i)
-                for (int j = 0; j < Nx; ++j) t1[i * Nx + j] = (i == j ? 1.0 : 0.0) + (ila[i] + ilb[i]) * S[i * Nx + j];
-            if (!mat_inv(Nx, t1.data(), C.data())) { set_error(h, "EM: I + P Sigma is singular"); return GPMPC_ERR_ARG; }
-            for (int i = 0; i < Nx; ++i)
-                for (int j = 0; j < Nx; ++j) {
-                    Fa[i * Nx + j] = C[i * Nx + j] * ila[j]; Fb[i * Nx + j] = C[i * Nx + j] * ilb[j];
-                    CP[i * Nx + j] = C[i * Nx + j] * (ila[j] + ilb[j]);
+            const double *sa = &s1[(size_t)a * Nx], *Sa = &s2[(size_t)a * nn], *sb = &s1[(size_t)b * Nx], *Sb = &s2[(size_t)b * nn];
+            const int rc = pm.form(h, S, a, b, iRa, iRb);
+            if (rc) return rc;
+            // cross records: owner rows r0 (u1 = sum m v_i, Mii, Mij = sum m v_i v_j^T, u2 = sum m v_j), owner columns r1 (Mjj)
+            const int r0 = r_cross + 2 * p, r1 = r0 + 1;
+            for (int d = 0; d < Nx; ++d) {
+                u1[d] = at(r0, M1[d], 0); u2[d] = at(r0, 0, M1[d]);
+                for (int e = 0; e < Nx; ++e) {
+                    Mii[d * Nx + e] = at(r0, M2[d * Nx + e], 0); Mjj[d * Nx + e] = at(r1, M2[d * Nx + e], 0);
+                    Mij[d * Nx + e] = at(r0, M1[d], M1[e]);
                 }
-            mat_mul(Nx, Fb.data(), S, t1.data()); mat_mul(Nx, t1.data(), iRa, A.data());
-            mat_mul(Nx, Fa.data(), S, t1.data()); mat_mul(Nx, t1.data(), iRb, B.data());
-            for (int q = 0; q < nn; ++q) { A[q] = -A[q]; B[q] = -B[q]; }
-            const double *r0 = R(r_cross + 2 * p), *r1 = R(r_cross + 2 * p + 1);
-            const double *u1 = r0 + 1, *Mii = r0 + 1 + Nx, *Mij = r0 + 1 + Nx + nn, *u2 = r1 + 1, *Mjj = r1 + 1 + Nx;
+            }
             // d/dz: iR_a u1 + iR_b u2 + A (u1 + s_a Mb) + B (u2 + Ma s_b)
             for (int d = 0; d < Nx; ++d) {
                 double s = 0.0;
@@ -1733,8 +1792,9 @@ static int em_grad_finish(gpmpc_handle_t h, const double* S, const double* emp, 
                 for (int e = 0; e < Nx; ++e)
                     Z1[d * Nx + e] = Mii[d * Nx + e] * ila[d] * ila[e] + Mij[d * Nx + e] * ila[d] * ilb[e]
                                    + Mij[e * Nx + d] * ilb[d] * ila[e] + Mjj[d * Nx + e] * ilb[d] * ilb[e];
-            mat_mul(Nx, C.data(), Z1.data(), t1.data()); mat_mul(Nx, t1.data(), C.data(), G.data(), true);
-            for (int q = 0; q < nn; ++q) G[q] = 0.5 * G[q] - 0.5 * r0[0] * CP[q];
+            mat_mul(Nx, C, Z1.data(), t1.data()); mat_mul(Nx, t1.data(), C, G.data(), true);
+            const double m0 = at(r0, 0, 0);
+            for (int q = 0; q < nn; ++q) G[q] = 0.5 * G[q] - 0.5 * m0 * CP[q];
             // + sum_ij w_ij d delta_ij: w is rank one, so these are products of the per-output moments
             auto add_side = [&](const double* X, const double* S_, const double* iR, double scale) {   // scale (X S iR + iR S X^T + X S X^T) / 2
                 mat_mul(Nx, X, S_, t1.data());
@@ -1743,8 +1803,8 @@ static int em_grad_finish(gpmpc_handle_t h, const double* S, const double* emp, 
                 for (int d = 0; d < Nx; ++d)
                     for (int e = 0; e < Nx; ++e) G[d * Nx + e] += 0.5 * scale * (t2[d * Nx + e] + t2[e * Nx + d] + t3[d * Nx + e]);
             };
-            add_side(A.data(), Sa, iRa, Mb);
-            add_side(B.data(), Sb, iRb, Ma);
+            add_side(A, Sa, iRa, Mb);
+            add_side(B, Sb, iRb, Ma);
             for (int d = 0; d < Nx; ++d) {
                 ga[d] = 0.0; gb[d] = 0.0;
                 for (int k = 0; k < Nx; ++k) { ga[d] += Fa[d * Nx + k] * sa[k]; gb[d] += Fb[d * Nx + k] * sb[k]; }
@@ -1753,15 +1813,19 @@ static int em_grad_finish(gpmpc_handle_t h, const double* S, const double* emp, 
                 for (int e = 0; e < Nx; ++e)
                     G[d * Nx + e] += 0.5 * (ga[d] * gb[e] + gb[d] * ga[e]) - 0.5 * (A[d * Nx + e] + B[d * Nx + e]) * Ma * Mb;
             if (a == b) {       // - d T_a, T_a = t tr(K^-1 Q_aa): backbone records plus the remainder's
-                const double *rt = R(r_tr + a), *rb = R(r_bb + a), *rg = R(r_gram + a);
-                const double T = t * (rb[0] + rt[0]);
+                const int rt = r_tr + a, rb = r_bb + a, rg = r_gram + a;
+                const double T = t * (at(rb, 0, 0) + at(rt, 0, 0));
                 for (int d = 0; d < Nx; ++d) {
                     double s = 0.0;
-                    for (int k = 0; k < Nx; ++k) s += Fa[d * Nx + k] * t * (rb[1 + k] + rt[1 + k]);
+                    for (int k = 0; k < Nx; ++k) s += Fa[d * Nx + k] * t * (at(rb, M1[k], 0) + at(rt, M1[k], 0));
                     dz[d] -= 2.0 * s;
                 }
-                for (int q = 0; q < nn; ++q) Z1[q] = t * (rb[1 + Nx + q] + rt[1 + Nx + q] + rg[1 + Nx + q] + rt[1 + Nx + nn + q]);
-                mat_mul(Nx, Fa.data(), Z1.data(), t1.data()); mat_mul(Nx, t1.data(), Fa.data(), t2.data(), true);
+                for (int d = 0; d < Nx; ++d)
+                    for (int e = 0; e < Nx; ++e) {
+                        const int m2 = M2[d * Nx + e];
+                        Z1[d * Nx + e] = t * (at(rb, m2, 0) + at(rt, m2, 0) + at(rg, m2, 0) + at(rt, M1[d], M1[e]));
+                    }
+                mat_mul(Nx, Fa, Z1.data(), t1.data()); mat_mul(Nx, t1.data(), Fa, t2.data(), true);
                 for (int q = 0; q < nn; ++q) G[q] -= t2[q] - 0.5 * T * CP[q];
             }
             if (dcz)
@@ -1771,92 +1835,27 @@ static int em_grad_finish(gpmpc_handle_t h, const double* S, const double* emp, 
     return GPMPC_OK;
 }
 
-// ------------------------------------------------------------------------------------
-// 'EM' second derivatives (gpmpc_predict_em_hess, DESIGN 4.8).  Every term of mean and cov is a Gaussian expectation,
-// Gaussian in z, so its z-derivatives are Hermite polynomials of (y, S): He_1 = y, He_2 = y y - S,
-// He_3 = y y y - 3 sym(S y), He_4 = y^4 - 6 sym(S y y) + 3 sym(S S); and d/dSigma = 1/2 d^2/dz^2 (heat equation).  The
-// device writes degree-4 records (kernels.cuh, em_hess_*); the host forms d^k mean_a / dz^k (k <= 4) and d^k cov_ab / dz^k
-// (k = 2..4) from them and assembles the Sigma blocks.  Record order per point:
-//   [mean a (weights beta_a q_a) | cross pair p, owner rows / columns | trace remainder a | trace backbone a]
-// ------------------------------------------------------------------------------------
-struct EmHessOutputs {
-    double *d2mean_dz2, *d2mean_dSigma_dz, *d2mean_dSigma2, *d2cov_dz2, *d2cov_dSigma_dz, *d2cov_dSigma2;
-};
-
-template <int NXP>
-static cudaError_t launch_em_hess(gpmpc_handle_t h, const EmHessTables& tb, const double* dz, const double* dP, int npairs,
-                                  int nb, double* rec_out)
-{
-    const int N = h->N, Nx = h->Nx, Ny = h->Ny, np = h->Npad, nf = tb.nf, RL = tb.nent;
-    constexpr int NFP = 1 + NXP + NXP * (NXP + 1) / 2;
-    const int r_cross = Ny, r_tr = Ny + 2 * npairs, r_bb = r_tr + Ny, nrec = r_bb + Ny;
-    const int* MONO = h->dEmHIdx;
-    const int* ENT = MONO + tb.mono.size();
-    double* part = h->dEmHPart;
-    const long long srec = (long long)nb * RL;
-    const int smem_pair = (4 * NXP * 64 + 64 * 65 + NFP * 64) * 8, smem_own = (NXP * 64 + 64 * NFP) * 8;
-    cudaError_t e = smem_opt_in<em_hess_pair_kernel<NXP>>(smem_pair);
-    if (e == cudaSuccess) e = smem_opt_in<em_hess_owner_kernel<NXP>>(smem_own);
-    if (e != cudaSuccess) return e;
-    em_hess_owner_kernel<NXP><<<dim3(nb, Ny), 256, smem_own, h->st>>>(h->dXT, np, N, Nx, dz, h->dAlpha, h->dEmLQ, np, nullptr, 0, 0, 1,
-                                                                      MONO, ENT, RL, part, srec);
-    em_hess_pair_kernel<NXP><<<dim3(nb, npairs, 2), 256, smem_pair, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE,
-                                                                            h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2,
-                                                                            nullptr, 0, r_cross, MONO, ENT, RL, part, nb);
-    em_hess_pair_kernel<NXP><<<dim3(nb, Ny, 1), 256, smem_pair, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE,
-                                                                        h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2,
-                                                                        h->dEmKinv, 1, r_tr, MONO, ENT, RL, part, nb);
-    if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    // rank-one backbone e e^T of Q_aa: Z_f = K^-1 (e o mono_f) = L^-T L^-1 (e o mono_f) for the nf features, then owner
-    // records with features e_i Z_f,i
-    double* rows = h->dEmHBB;
-    double* prod = rows + (long long)nf * np;
-    double* kz = prod + (long long)nf * np;
-    for (int a = 0; a < Ny; ++a) {
-        const int paa = a * (a + 1) / 2 + a;
-        const double* Li = h->dLi + (long long)a * slab(h);
-        em_hess_bb_rows_kernel<<<(np + 255) / 256, 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, h->dEmE + (long long)paa * np, np, MONO, nf, rows);
-        trmv_lower_kernel<<<dim3((np + 7) / 8, 1, nf), 256, 0, h->st>>>(Li, np, 0, rows, np, prod, np, np);
-        trmv_lower_T_kernel<<<dim3(np / 32, 1, nf), 256, 0, h->st>>>(Li, np, 0, prod, np, kz, np, np);
-        em_hess_owner_kernel<NXP><<<dim3(nb, 1), 256, smem_own, h->st>>>(h->dXT, np, N, Nx, dz, nullptr, h->dEmE + (long long)paa * np, 0,
-                                                                         kz, 0, np, nf, MONO, ENT, RL, part + (long long)(r_bb + a) * srec, 0);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    }
-    em_sum_parts_kernel<<<nrec, 256, 0, h->st>>>(part, nb, RL, rec_out);
-    return cudaGetLastError();
-}
-
-// per (point, pair) inputs of em_hess_pair_finish_kernel, formed as em_grad_finish forms them (O(Nx^3)):
-// [Fa Fb CP At Bt sAt sBt sFa sFb] (Nx^2 each), t;  C = (I + P Sigma)^-1, Fa = C La^-1, Fb = C Lb^-1, CP = C P (symmetric
-// part), At = Fa - iR_a = -C Lb^-1 Sigma iR_a and Bt = Fb - iR_b (as products, not differences), sX = symmetric part of X
+// per (point, pair) inputs of em_hess_pair_finish_kernel (EmPairMats): [Fa Fb CP At Bt sAt sBt sFa sFb] (Nx^2 each), t;
+// CP as its symmetric part, At = A = Fa - iR_a and Bt = B = Fb - iR_b, sX = symmetric part of X
 static int em_hess_pair_params(gpmpc_handle_t h, const double* S, const double* emp, double* out)
 {
-    const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, m = Nx + 2;
-    std::vector<double> t1(nn), C(nn), ila(Nx), ilb(Nx);
+    const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx;
+    EmPairMats pm(Nx);
     int p = 0;
     for (int a = 0; a < Ny; ++a)
         for (int b = 0; b <= a; ++b, ++p) {
-            const double* la = &h->hyper[(size_t)a * m];
-            const double* lb = &h->hyper[(size_t)b * m];
             const double* iRa = emp + (size_t)a * (2 * nn + 2);
             const double* iRb = emp + (size_t)b * (2 * nn + 2);
+            const int rc = pm.form(h, S, a, b, iRa, iRb);
+            if (rc) return rc;
             double* o = out + (size_t)p * (9 * nn + 1);
             double *Fa = o, *Fb = o + nn, *CP = o + 2 * nn, *At = o + 3 * nn, *Bt = o + 4 * nn, *sAt = o + 5 * nn;
             double *sBt = o + 6 * nn, *sFa = o + 7 * nn, *sFb = o + 8 * nn;
-            for (int d = 0; d < Nx; ++d) { ila[d] = 1.0 / (la[d] * la[d]); ilb[d] = 1.0 / (lb[d] * lb[d]); }
-            for (int i = 0; i < Nx; ++i)
-                for (int j = 0; j < Nx; ++j) t1[i * Nx + j] = (i == j ? 1.0 : 0.0) + (ila[i] + ilb[i]) * S[i * Nx + j];
-            if (!mat_inv(Nx, t1.data(), C.data())) { set_error(h, "EM: I + P Sigma is singular"); return GPMPC_ERR_ARG; }
-            for (int i = 0; i < Nx; ++i)
-                for (int j = 0; j < Nx; ++j) {
-                    Fa[i * Nx + j] = C[i * Nx + j] * ila[j]; Fb[i * Nx + j] = C[i * Nx + j] * ilb[j];
-                    CP[i * Nx + j] = C[i * Nx + j] * (ila[j] + ilb[j]);
-                }
+            std::copy(pm.Fa.begin(), pm.Fa.end(), Fa); std::copy(pm.Fb.begin(), pm.Fb.end(), Fb);
+            std::copy(pm.CP.begin(), pm.CP.end(), CP);
+            std::copy(pm.A.begin(), pm.A.end(), At); std::copy(pm.B.begin(), pm.B.end(), Bt);
             for (int i = 0; i < Nx; ++i)        // CP = (P^-1 + Sigma)^-1 is symmetric: use the symmetric part
                 for (int j = 0; j < i; ++j) CP[i * Nx + j] = CP[j * Nx + i] = 0.5 * (CP[i * Nx + j] + CP[j * Nx + i]);
-            mat_mul(Nx, Fb, S, t1.data()); mat_mul(Nx, t1.data(), iRa, At);
-            mat_mul(Nx, Fa, S, t1.data()); mat_mul(Nx, t1.data(), iRb, Bt);
-            for (int q = 0; q < nn; ++q) { At[q] = -At[q]; Bt[q] = -Bt[q]; }
             for (int i = 0; i < Nx; ++i)
                 for (int j = 0; j < Nx; ++j) {
                     sAt[i * Nx + j] = 0.5 * (At[i * Nx + j] + At[j * Nx + i]); sBt[i * Nx + j] = 0.5 * (Bt[i * Nx + j] + Bt[j * Nx + i]);
@@ -1887,33 +1886,35 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
     ENSURE(h->dEmMeanPart, (long long)Ny * nblk); ENSURE(h->dEmPart, (long long)npairs * T * T);
     { int rcs = ensure_nlml_scratch(h); if (rcs) return rcs; }      // dKinv <- Q_aa, dU <- L^-1 Q_aa (one slab each)
     ENSURE(h->dEMP, (long long)H * per);
-    const int RL = em_rec_len(Nx), nrec = 4 * Ny + 2 * npairs;
-    if (go) {
-        ENSURE(h->dEmGPart, (long long)nrec * T * RL);
-        ENSURE(h->dEmGRec, (long long)H * nrec * RL);
-        ENSURE(h->dEmBB, (2LL * (Nx + 1) + 1) * np);
-    }
-    EmHessTables* tb = nullptr;
-    const int nrech = 3 * Ny + 2 * npairs;
+    // the record set of degree D: tables built and uploaded once, scratch for H points
+    auto records = [&](int D) -> int {
+        EmRecords& R = h->em_rec[D / 2 - 1];
+        if (!R.tb) R.tb.reset(new EmTables(Nx, D));
+        EmTables& tb = *R.tb;
+        ENSURE(R.part, (long long)tb.nrec(Ny) * T * tb.nent);
+        ENSURE(R.rec, (long long)H * tb.nrec(Ny) * tb.nent);
+        ENSURE(R.bb, 3LL * tb.nf * np);
+        ENSURE(R.idx, (long long)tb.dev.size());
+        if (tb.uploaded_to != R.idx.p) {
+            CUDA_TRY(cudaMemcpyAsync(R.idx, tb.dev.data(), tb.dev.size() * 4, cudaMemcpyHostToDevice, h->st));
+            tb.uploaded_to = R.idx.p;
+        }
+        return GPMPC_OK;
+    };
+    EmRecords& R2 = h->em_rec[0];
+    EmRecords& R4 = h->em_rec[1];
+    if (go) { const int rc = records(2); if (rc) return rc; }
     const long long TS = 1 + Nx + nn + (long long)nn * Nx + (long long)nn * nn, Q = (long long)nn * nn;
     const long long per_pair = 6 * TS + 8 * Q, nout = (long long)nn + nn * Nx + nn * nn;    // finish scratch per CTA; one output slab
     const int Hc = (int)std::max(1LL, std::min((long long)H, (64LL << 20) / ((long long)npairs * per_pair)));   // points per finish launch
     if (ho) {
-        if (!h->em_tb) h->em_tb.reset(new EmHessTables(Nx));
-        tb = h->em_tb.get();
-        ENSURE(h->dEmHPart, (long long)nrech * T * tb->nent);
-        ENSURE(h->dEmHRec, (long long)H * nrech * tb->nent);
-        ENSURE(h->dEmHBB, 3LL * tb->nf * np);
+        const int rc = records(4);
+        if (rc) return rc;
         ENSURE(h->dEmHEHP, (long long)H * npairs * (9 * nn + 1));
         ENSURE(h->dEmHMU, (long long)H * Ny * TS);
         ENSURE(h->dEmHD, (long long)H * Ny * TS);
         ENSURE(h->dEmHScr, std::max((long long)H * Ny * Q, (long long)Hc * npairs * per_pair));
         ENSURE(h->dEmHOut, (long long)H * (Ny + Ny * Ny) * nout);
-        ENSURE(h->dEmHIdx, (long long)tb->dev.size());
-        if (tb->uploaded_to != h->dEmHIdx.p) {
-            CUDA_TRY(cudaMemcpyAsync(h->dEmHIdx, tb->dev.data(), tb->dev.size() * 4, cudaMemcpyHostToDevice, h->st));
-            tb->uploaded_to = h->dEmHIdx.p;
-        }
     }
     if (go || ho) {
         ENSURE(h->dEmKinv, (long long)Ny * slab(h));
@@ -1970,12 +1971,13 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
                                                    h->dMean + (size_t)p * Ny, h->dVar + (size_t)p * Ny, h->dCov + (size_t)p * Ny * Ny);
         CUDA_TRY(cudaGetLastError());
         if (go) {
-            double* rec = h->dEmGRec + (size_t)p * nrec * RL;
-            CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_grad<decltype(nxp)::value>(h, dz, dP, npairs, T, rec); }));
+            double* rec = R2.rec + (size_t)p * R2.tb->nrec(Ny) * R2.tb->nent;
+            CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_records<decltype(nxp)::value, 2>(h, R2, dz, dP, npairs, T, rec); }));
         }
         if (ho) {
-            double* rec = h->dEmHRec + (size_t)p * nrech * tb->nent;
-            CUDA_TRY(Nx <= 8 ? launch_em_hess<8>(h, *tb, dz, dP, npairs, T, rec) : launch_em_hess<16>(h, *tb, dz, dP, npairs, T, rec));   // Nx <= 16
+            double* rec = R4.rec + (size_t)p * R4.tb->nrec(Ny) * R4.tb->nent;
+            CUDA_TRY((Nx <= 8 ? launch_em_records<8, 4>(h, R4, dz, dP, npairs, T, rec)
+                              : launch_em_records<16, 4>(h, R4, dz, dP, npairs, T, rec)));   // Nx <= 16
         }
     }
     if (mean) CUDA_TRY(cudaMemcpyAsync(mean, h->dMean, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
@@ -1989,18 +1991,20 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
             if (rc) return rc;
         }
         CUDA_TRY(cudaMemcpyAsync(h->dEmHEHP, ehp.data(), ehp.size() * 8, cudaMemcpyHostToDevice, h->st));
-        const int* MID = tb->d_mid(h->dEmHIdx);
-        const int* ENTPOS = tb->d_entpos(h->dEmHIdx);
+        const EmTables& tb = *R4.tb;
+        const int nrech = tb.nrec(Ny);
+        const int* MID = tb.d_mid(R4.idx);
+        const int* ENTPOS = tb.d_entpos(R4.idx);
         double* om = h->dEmHOut;
         double* oc = om + (long long)H * Ny * nout;
         double *m2 = om, *m3 = m2 + (long long)H * Ny * nn, *m4 = m3 + (long long)H * Ny * nn * Nx;
         double *c2 = oc, *c3 = c2 + (long long)H * Ny * Ny * nn, *c4 = c3 + (long long)H * Ny * Ny * nn * Nx;
-        em_hess_mean_finish_kernel<<<dim3(Ny, H), 256, 0, h->st>>>(Nx, Ny, h->dEMP, (long long)per, h->dEmHRec, nrech, tb->nent,
-                                                                   MID, ENTPOS, tb->nf, h->dEmHMU, h->dEmHD, h->dEmHScr, m2, m3, m4);
+        em_hess_mean_finish_kernel<<<dim3(Ny, H), 256, 0, h->st>>>(Nx, Ny, h->dEMP, (long long)per, R4.rec, nrech, tb.nent,
+                                                                   MID, ENTPOS, tb.nf, h->dEmHMU, h->dEmHD, h->dEmHScr, m2, m3, m4);
         CUDA_TRY(cudaGetLastError());
         for (int h0 = 0; h0 < H; h0 += Hc) {
             em_hess_pair_finish_kernel<<<dim3(npairs, std::min(Hc, H - h0)), 256, 0, h->st>>>(
-                Nx, Ny, h0, h->dEMP, (long long)per, h->dEmHEHP, h->dEmHRec, nrech, tb->nent, MID, ENTPOS, tb->nf,
+                Nx, Ny, h0, h->dEMP, (long long)per, h->dEmHEHP, R4.rec, nrech, tb.nent, MID, ENTPOS, tb.nf,
                 h->dEmHMU, h->dEmHD, h->dEmHScr, c2, c3, c4);
             CUDA_TRY(cudaGetLastError());
         }
@@ -2014,12 +2018,14 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
     if (!go) {
         CUDA_TRY(cudaStreamSynchronize(h->st));
     } else {
-        std::vector<double> recs((size_t)H * nrec * RL), mh((size_t)H * Ny);
-        CUDA_TRY(cudaMemcpyAsync(recs.data(), h->dEmGRec, recs.size() * 8, cudaMemcpyDeviceToHost, h->st));
+        const EmTables& tb = *R2.tb;
+        const size_t rl = (size_t)tb.nrec(Ny) * tb.nent;
+        std::vector<double> recs((size_t)H * rl), mh((size_t)H * Ny);
+        CUDA_TRY(cudaMemcpyAsync(recs.data(), R2.rec, recs.size() * 8, cudaMemcpyDeviceToHost, h->st));
         CUDA_TRY(cudaMemcpyAsync(mh.data(), h->dMean, mh.size() * 8, cudaMemcpyDeviceToHost, h->st));
         CUDA_TRY(cudaStreamSynchronize(h->st));
         for (int p = 0; p < H; ++p) {
-            const int rc = em_grad_finish(h, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per, recs.data() + (size_t)p * nrec * RL,
+            const int rc = em_grad_finish(h, tb, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per, recs.data() + (size_t)p * rl,
                                           mh.data() + (size_t)p * Ny,
                                           go->dmean_dz ? go->dmean_dz + (size_t)p * Ny * Nx : nullptr,
                                           go->dmean_dSigma ? go->dmean_dSigma + (size_t)p * Ny * nn : nullptr,
@@ -2684,42 +2690,40 @@ extern "C" int gpmpc_predict_hess(gpmpc_handle_t h, int method, int H, const dou
     return predict_derivs(h, "gpmpc_predict_hess", method, H, Z, Sigma, spp, mean, var, cov, jac, dvar_dz, dcov_dz, hess, &ho);
 }
 
-// 'EM' prediction plus its first derivatives w.r.t. z and Sigma (see include/gpmpc.h)
+// The 'EM' derivative entry points (see include/gpmpc.h): first derivatives, and second ones when ho is given (Nx <= 16)
+static int predict_em_derivs(gpmpc_handle_t h, const char* fn, int H, const double* Z, const double* Sigma, int spp,
+                             double* mean, double* var, double* cov, const EmGradOutputs& go, const EmHessOutputs* ho)
+{
+    int rc = predict_guard(h, fn, GPMPC_METHOD_EM, H);
+    if (rc) return rc;
+    if (!Z || !Sigma) { set_error(h, "%s: null Z / Sigma", fn); return GPMPC_ERR_ARG; }
+    if (ho && h->Nx > 16) { set_error(h, "%s supports Nx <= 16", fn); return GPMPC_ERR_ARG; }
+    rc = predict_prepare(h, fn, H, true);
+    if (rc) return rc;
+    NvtxRange nvtx_r(ho ? "gpmpc.predict_em_hess" : "gpmpc.predict_em_grad");
+    const bool any_g = go.dmean_dz || go.dmean_dSigma || go.dcov_dz || go.dcov_dSigma;   // none: no K^-1 cache for them
+    const bool any_h = ho && (ho->d2mean_dz2 || ho->d2mean_dSigma_dz || ho->d2mean_dSigma2 || ho->d2cov_dz2 ||
+                              ho->d2cov_dSigma_dz || ho->d2cov_dSigma2);
+    return predict_em(h, H, Z, Sigma, spp, mean, var, cov, any_g ? &go : nullptr, any_h ? ho : nullptr);
+}
+
 extern "C" int gpmpc_predict_em_grad(gpmpc_handle_t h, int H, const double* Z, const double* Sigma, int spp,
                                      double* mean, double* var, double* cov,
                                      double* dmean_dz, double* dmean_dSigma, double* dcov_dz, double* dcov_dSigma)
 {
-    int rc = predict_guard(h, __func__, GPMPC_METHOD_EM, H);
-    if (rc) return rc;
-    if (!Z || !Sigma) { set_error(h, "gpmpc_predict_em_grad: null Z / Sigma"); return GPMPC_ERR_ARG; }
-    rc = predict_prepare(h, __func__, H, true);
-    if (rc) return rc;
-    NvtxRange nvtx_r("gpmpc.predict_em_grad");
     const EmGradOutputs go = {dmean_dz, dmean_dSigma, dcov_dz, dcov_dSigma};
-    const bool any = dmean_dz || dmean_dSigma || dcov_dz || dcov_dSigma;   // none: the forward call alone, no K^-1 cache
-    return predict_em(h, H, Z, Sigma, spp, mean, var, cov, any ? &go : nullptr);
+    return predict_em_derivs(h, __func__, H, Z, Sigma, spp, mean, var, cov, go, nullptr);
 }
 
-// 'EM' prediction plus its first and second derivatives w.r.t. z and Sigma (see include/gpmpc.h)
 extern "C" int gpmpc_predict_em_hess(gpmpc_handle_t h, int H, const double* Z, const double* Sigma, int spp,
                                      double* mean, double* var, double* cov,
                                      double* dmean_dz, double* dmean_dSigma, double* dcov_dz, double* dcov_dSigma,
                                      double* d2mean_dz2, double* d2mean_dSigma_dz, double* d2mean_dSigma2,
                                      double* d2cov_dz2, double* d2cov_dSigma_dz, double* d2cov_dSigma2)
 {
-    int rc = predict_guard(h, __func__, GPMPC_METHOD_EM, H);
-    if (rc) return rc;
-    if (!Z || !Sigma) { set_error(h, "gpmpc_predict_em_hess: null Z / Sigma"); return GPMPC_ERR_ARG; }
-    if (h->Nx > 16) { set_error(h, "gpmpc_predict_em_hess supports Nx <= 16"); return GPMPC_ERR_ARG; }
-    if (h->Ny > 44) { set_error(h, "EM supports Ny <= 44"); return GPMPC_ERR_ARG; }
-    rc = predict_prepare(h, __func__, H, true);
-    if (rc) return rc;
-    NvtxRange nvtx_r("gpmpc.predict_em_hess");
     const EmGradOutputs go = {dmean_dz, dmean_dSigma, dcov_dz, dcov_dSigma};
     const EmHessOutputs ho = {d2mean_dz2, d2mean_dSigma_dz, d2mean_dSigma2, d2cov_dz2, d2cov_dSigma_dz, d2cov_dSigma2};
-    const bool any_g = dmean_dz || dmean_dSigma || dcov_dz || dcov_dSigma;
-    const bool any_h = d2mean_dz2 || d2mean_dSigma_dz || d2mean_dSigma2 || d2cov_dz2 || d2cov_dSigma_dz || d2cov_dSigma2;
-    return predict_em(h, H, Z, Sigma, spp, mean, var, cov, any_g ? &go : nullptr, any_h ? &ho : nullptr);
+    return predict_em_derivs(h, __func__, H, Z, Sigma, spp, mean, var, cov, go, &ho);
 }
 
 // Row Nk of L and L^-1 of every owned output from l = L^-1 k (rows < Nk of dV): r = Li^T l over the Nk rows l occupies,

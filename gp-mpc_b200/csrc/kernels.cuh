@@ -1027,6 +1027,50 @@ em_prep_kernel(const double* __restrict__ XT, int ldx, int N, int Nx, int Ny, in
     F2[(long long)p * ldn + i] = (i < N) ? f2 : 0.0;
 }
 
+// The 64x64 tiles of the 'EM' pair sums (em_pair_kernel, em_pair_rec_kernel), 4x4 per thread: acc[r][c] = sum_d
+// Ws[d][ty + 16 r] Js[d][tx + 16 c] over the staged W rows of the i block and IJ rows of the j block (stride 64).
+__device__ __forceinline__ void em_tile(const double* Ws, const double* Js, int Nx, int tx, int ty, double (&acc)[4][4])
+{
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) acc[r][c] = 0.0;
+    for (int d = 0; d < Nx; ++d) {
+        double wv[4], jv[4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r) wv[r] = Ws[d * 64 + ty + 16 * r];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) jv[c] = Js[d * 64 + tx + 16 * c];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) acc[r][c] = fma(wv[r], jv[c], acc[r][c]);
+    }
+}
+
+// The cross term of pair p = (a, b) at (i, j) without cancellation: beta_i beta_j (t Q_ij - q_i q_j) =
+// w_ij expm1(x_ij) with w_ij = (beta_i q_i)(beta_j q_j) and x_ij = log t + log Q_ij - log q_i - log q_j -- the
+// reference's  t beta^T Q beta - mean_a mean_b  (:412,416) term by term, before the sums cancel.  The exponent is
+// assembled from its small parts only (never as a difference of O(10) logarithms).
+__device__ __forceinline__ double em_cross_w(const double* __restrict__ alpha, long long sal, const double* __restrict__ LQ,
+                                             int ldn, int a, int b, int i, int j)
+{
+    const double la = LQ[(long long)a * ldn + i], lb = LQ[(long long)b * ldn + j];
+    return (alpha[(long long)a * sal + i] * exp(la)) * (alpha[(long long)b * sal + j] * exp(lb));
+}
+__device__ __forceinline__ double em_cross_x(double cab, const double* __restrict__ E2, const double* __restrict__ F2,
+                                             int ldn, int p, int i, int j, double acc)
+{
+    return cab + E2[(long long)p * ldn + i] + F2[(long long)p * ldn + j] + 2.0 * acc;
+}
+
+// The part of Q_aa (pair p = (a, a)) beyond its rank-one backbone: Q_ij = e^{E_i} e^{F_j} (1 + expm1(2 acc_ij))
+__device__ __forceinline__ double em_rem(const double* __restrict__ E, const double* __restrict__ F, int ldn, int p,
+                                         int i, int j, double acc)
+{
+    return exp(E[(long long)p * ldn + i] + F[(long long)p * ldn + j]) * expm1(2.0 * acc);
+}
+
 // sum_ij beta_a,i beta_b,j (t Q_ij - q_i q_j) for one pair; 64x64 tile per CTA, 4x4 per thread (:394-416).
 // The reference subtracts invK from beta beta^T on the diagonal pairs before the sum (:410-411),
 // which cancels 6-8 digits at cond(K) ~ 1e8-1e10 (negative variances on the car fixture, SURVEY
@@ -1059,21 +1103,7 @@ em_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
     }
     __syncthreads();
     double acc[4][4];
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) acc[r][c] = 0.0;
-    for (int d = 0; d < Nx; ++d) {
-        double wv[4], jv[4];
-#pragma unroll
-        for (int r = 0; r < 4; ++r) wv[r] = Ws[d * 64 + ty + 16 * r];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) jv[c] = Js[d * 64 + tx + 16 * c];
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) acc[r][c] = fma(wv[r], jv[c], acc[r][c]);
-    }
+    em_tile(Ws, Js, Nx, tx, ty, acc);
     double s = 0.0;
 #pragma unroll
     for (int r = 0; r < 4; ++r) {
@@ -1081,18 +1111,11 @@ em_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
             const int j = j0 + tx + 16 * c;
-            // mode 1 stores only the part of Q beyond its rank-one backbone: Q_ij = e^{E_i} e^{F_j} (1 + expm1(2 acc_ij));
-            // the backbone's trace term |L^-1 e^E|^2 is formed like the ME variance (em_qvec_kernel + trmv), which keeps
+            // mode 1 stores only the part of Q beyond its rank-one backbone (em_rem); the backbone's trace term |L^-1 e^E|^2 is formed like the ME variance (em_qvec_kernel + trmv), which keeps
             // EM -> ME exact to ~1e-11 as Sigma -> 0 instead of amplifying the full Q through L^-1 twice
-            if (mode) { if (i < ldq && j < ldq) Qout[(long long)i * ldq + j] = (i < N && j < N) ? exp(E[(long long)p * ldn + i] + F[(long long)p * ldn + j]) * expm1(2.0 * acc[r][c]) : 0.0; }
-            else if (i < N && j < N) {
-                // beta_i beta_j (t Q_ij - q_i q_j) = (beta_i q_i)(beta_j q_j) expm1(log t + log Q_ij - log q_i - log q_j):
-                // the reference's  t beta^T Q beta - mean_a mean_b  (:412,416) term by term, before the sums cancel
-                const double la = LQ[(long long)a * ldn + i], lb = LQ[(long long)b * ldn + j];
-                const double wgt = (alpha[(long long)a * sal + i] * exp(la)) * (alpha[(long long)b * sal + j] * exp(lb));
-                // the exponent is assembled from its small parts only (never as a difference of O(10) logarithms)
-                s = fma(wgt, expm1(cab + E2[(long long)p * ldn + i] + F2[(long long)p * ldn + j] + 2.0 * acc[r][c]), s);
-            }
+            if (mode) { if (i < ldq && j < ldq) Qout[(long long)i * ldq + j] = (i < N && j < N) ? em_rem(E, F, ldn, p, i, j, acc[r][c]) : 0.0; }
+            else if (i < N && j < N)
+                s = fma(em_cross_w(alpha, sal, LQ, ldn, a, b, i, j), expm1(em_cross_x(cab, E2, F2, ldn, p, i, j, acc[r][c])), s);
         }
     }
     if (mode) return;
@@ -1189,187 +1212,6 @@ __global__ void em_finalize_kernel(int Nx, int Ny, int npairs, const double* __r
     }
 }
 
-// ---------------------------------------------------------------------------------------
-// 'EM' first derivatives (gpmpc_predict_em_grad).  Every O(N) / O(N^2) sum ends in a record of
-// RL = 1 + Nx + 2 Nx^2 doubles over a weight m_k (k the "owner" index) and v_k = x_k - z:
-//   [ sum m_k | sum m_k v_k (Nx) | sum m_k v_k v_k^T (Nx^2) | sum_k v_k Y_k^T (Nx^2, pair sums only) ]
-// written as one partial per 64-index block and summed in block order by em_sum_parts_kernel; the host
-// forms the derivatives from the records (gpmpc.cu, em_grad_finish).
-// ---------------------------------------------------------------------------------------
-// Record of weights m_k = x1_k exp(x2_k) (a null operand counts as 1 / 0) over the d-major vectors
-// V[d][k] - z[d] (z may be null), k < n; one 64-index block per CTA (blockIdx.x), one record per blockIdx.y
-// (operands offset by sx, record by srec).  The last Nx^2 slot is written as zero.
-template <int NXP>
-__global__ void __launch_bounds__(256)
-em_moments_kernel(const double* __restrict__ V, int ldv, int n, int Nx, const double* __restrict__ z,
-                  const double* __restrict__ x1, const double* __restrict__ x2, long long sx,
-                  double* __restrict__ part, long long srec, int RL)
-{
-    __shared__ double w[64], vs[NXP * 64];
-    const int tid = threadIdx.x, k0 = blockIdx.x * 64;
-    if (x1) x1 += blockIdx.y * sx;
-    if (x2) x2 += blockIdx.y * sx;
-    if (tid < 64) {
-        const int k = k0 + tid;
-        w[tid] = (k < n) ? (x1 ? x1[k] : 1.0) * (x2 ? exp(x2[k]) : 1.0) : 0.0;
-    }
-    for (int idx = tid; idx < NXP * 64; idx += 256) {
-        const int d = idx >> 6, k = k0 + (idx & 63);
-        vs[idx] = (d < Nx && k < n) ? V[(long long)d * ldv + k] - (z ? z[d] : 0.0) : 0.0;
-    }
-    __syncthreads();
-    double* out = part + blockIdx.y * srec + (long long)blockIdx.x * RL;
-    const int nn = Nx * Nx;
-    for (int q = tid; q < RL; q += 256) {
-        double s = 0.0;
-        if (q == 0) { for (int k = 0; k < 64; ++k) s += w[k]; }
-        else if (q <= Nx) { const int d = q - 1; for (int k = 0; k < 64; ++k) s = fma(w[k], vs[d * 64 + k], s); }
-        else if (q <= Nx + nn) {
-            const int d = (q - 1 - Nx) / Nx, e = (q - 1 - Nx) % Nx;
-            for (int k = 0; k < 64; ++k) s = fma(w[k] * vs[d * 64 + k], vs[e * 64 + k], s);
-        }
-        out[q] = s;
-    }
-}
-
-// Pair sums of one 64-index owner block (blockIdx.x) against every other block, the 64x64 tiles recomputed
-// as em_pair_kernel does (no N x N array is written):
-//   mode 0, pair p = blockIdx.y, orientation o = blockIdx.z:  m_ij = w_ij expm1(delta_ij) (the cross term's
-//     small weights, w_ij = beta_ai q_ai beta_bj q_bj); owner = rows i (o = 0) or columns j (o = 1);
-//     record rec0 + 2p + o.
-//   mode 1, output a = blockIdx.y (pair (a,a)):  m_ij = K^-1_ij Qt_ij with Qt = e^{E_i+F_j} expm1(2 acc_ij) the
-//     O(Sigma) remainder of Q_aa; Kinv = full symmetric K^-1 per output (stride ldn^2); record rec0 + a.
-// The owner's sums over the other index, R_k = sum m and Y_k = sum m v_other, stay in registers across the
-// tiles (fixed order); the record then sums over the owner block in index order.
-template <int NXP>
-__global__ void __launch_bounds__(256)
-em_grad_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
-                    const double* __restrict__ alpha, long long sal,
-                    const double* __restrict__ XT, int ldx, const double* __restrict__ z,
-                    const double* __restrict__ E, const double* __restrict__ F, const double* __restrict__ W,
-                    const double* __restrict__ IJ, int ldn, const double* __restrict__ LQ,
-                    const double* __restrict__ E2, const double* __restrict__ F2,
-                    const double* __restrict__ Kinv, int mode, int rec0, double* __restrict__ part, int nb, int RL)
-{
-    constexpr int KF = NXP / 4 + 1;                  // features per thread: f = g + 4k, f = 0 (ones), 1 + d (v_d)
-    extern __shared__ double sm[];
-    double* Wo = sm;                                  // [NXP][64] W rows of the i block
-    double* Jo = Wo + NXP * 64;                       // [NXP][64] IJ rows of the j block
-    double* Vown = Jo + NXP * 64;                     // [NXP][64] v of the owner block
-    double* Voth = Vown + NXP * 64;                   // [NXP][64] v of the other block
-    double* Ms = Voth + NXP * 64;                     // [64][65] m tile, owner-major
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int nn = Nx * Nx;
-    const int o = mode ? 0 : blockIdx.z;
-    const int p = mode ? blockIdx.y * (blockIdx.y + 1) / 2 + blockIdx.y : blockIdx.y;
-    const double* P = EMP + (long long)Ny * (2 * nn + 2) + (long long)p * (nn + 4);
-    const int a = (int)P[nn + 1], b = (int)P[nn + 2];
-    const double cab = P[nn + 3];
-    const double* Ka = mode ? Kinv + (long long)a * ldn * ldn : nullptr;
-    const int own0 = blockIdx.x * 64, T = (N + 63) / 64;
-    for (int idx = tid; idx < NXP * 64; idx += 256) {
-        const int d = idx >> 6, k = own0 + (idx & 63);
-        const bool ok = d < Nx && k < N;
-        Vown[idx] = ok ? XT[(long long)d * ldx + k] - z[d] : 0.0;
-        if (o == 0) Wo[idx] = ok ? W[((long long)p * Nx + d) * ldn + k] : 0.0;
-        else Jo[idx] = ok ? IJ[((long long)p * Nx + d) * ldn + k] : 0.0;
-    }
-    const int ko = tid & 63, g = tid >> 6;
-    double acc2[KF];
-#pragma unroll
-    for (int q = 0; q < KF; ++q) acc2[q] = 0.0;
-    for (int t = 0; t < T; ++t) {
-        const int oth0 = t * 64;
-        __syncthreads();                              // previous tile's readers are done
-        for (int idx = tid; idx < NXP * 64; idx += 256) {
-            const int d = idx >> 6, k = oth0 + (idx & 63);
-            const bool ok = d < Nx && k < N;
-            Voth[idx] = ok ? XT[(long long)d * ldx + k] - z[d] : 0.0;
-            if (o == 0) Jo[idx] = ok ? IJ[((long long)p * Nx + d) * ldn + k] : 0.0;
-            else Wo[idx] = ok ? W[((long long)p * Nx + d) * ldn + k] : 0.0;
-        }
-        __syncthreads();
-        const int i0 = o ? oth0 : own0, j0 = o ? own0 : oth0;
-        double acc[4][4];
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) acc[r][c] = 0.0;
-        for (int d = 0; d < Nx; ++d) {
-            double wv[4], jv[4];
-#pragma unroll
-            for (int r = 0; r < 4; ++r) wv[r] = Wo[d * 64 + ty + 16 * r];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) jv[c] = Jo[d * 64 + tx + 16 * c];
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) acc[r][c] = fma(wv[r], jv[c], acc[r][c]);
-        }
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const int il = ty + 16 * r, i = i0 + il;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                const int jl = tx + 16 * c, j = j0 + jl;
-                double m = 0.0;
-                if (i < N && j < N) {
-                    if (mode) {
-                        m = Ka[(long long)i * ldn + j] * (exp(E[(long long)p * ldn + i] + F[(long long)p * ldn + j]) * expm1(2.0 * acc[r][c]));
-                    } else {
-                        const double la = LQ[(long long)a * ldn + i], lb = LQ[(long long)b * ldn + j];
-                        const double wgt = (alpha[(long long)a * sal + i] * exp(la)) * (alpha[(long long)b * sal + j] * exp(lb));
-                        m = wgt * expm1(cab + E2[(long long)p * ldn + i] + F2[(long long)p * ldn + j] + 2.0 * acc[r][c]);
-                    }
-                }
-                if (o == 0) Ms[il * 65 + jl] = m; else Ms[jl * 65 + il] = m;
-            }
-        }
-        __syncthreads();
-        for (int x = 0; x < 64; ++x) {
-            const double mv = Ms[ko * 65 + x];
-#pragma unroll
-            for (int q = 0; q < KF; ++q) {
-                const int f = g + 4 * q;
-                if (f <= Nx) acc2[q] = fma(mv, f == 0 ? 1.0 : Voth[(f - 1) * 64 + x], acc2[q]);
-            }
-        }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int q = 0; q < KF; ++q) {
-        const int f = g + 4 * q;
-        if (f <= Nx) Ms[ko * 65 + f] = acc2[q];       // Ms[k][0] = R_k, Ms[k][1+d] = Y_k,d
-    }
-    __syncthreads();
-    const int rec = rec0 + (mode ? (int)blockIdx.y : 2 * p + o);
-    double* out = part + ((long long)rec * nb + blockIdx.x) * RL;
-    for (int q = tid; q < RL; q += 256) {
-        double s = 0.0;
-        if (q == 0) { for (int k = 0; k < 64; ++k) s += Ms[k * 65]; }
-        else if (q <= Nx) { const int d = q - 1; for (int k = 0; k < 64; ++k) s = fma(Ms[k * 65], Vown[d * 64 + k], s); }
-        else if (q <= Nx + nn) {
-            const int d = (q - 1 - Nx) / Nx, e = (q - 1 - Nx) % Nx;
-            for (int k = 0; k < 64; ++k) s = fma(Ms[k * 65] * Vown[d * 64 + k], Vown[e * 64 + k], s);
-        } else {
-            const int d = (q - 1 - Nx - nn) / Nx, e = (q - 1 - Nx - nn) % Nx;
-            for (int k = 0; k < 64; ++k) s = fma(Vown[d * 64 + k], Ms[k * 65 + 1 + e], s);
-        }
-        out[q] = s;
-    }
-}
-
-// rows of the rank-one backbone of Q_aa for L^-1: R[0][i] = e_i = exp(E_i), R[1+d][i] = e_i (x_id - z_d); zero for i >= N
-__global__ void em_bb_rows_kernel(const double* __restrict__ XT, int ldx, int N, int Nx, const double* __restrict__ z,
-                                  const double* __restrict__ E, int n, double* __restrict__ R)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const double e = (i < N) ? exp(E[i]) : 0.0;
-    R[i] = e;
-    for (int d = 0; d < Nx; ++d) R[(long long)(1 + d) * n + i] = (i < N) ? e * (XT[(long long)d * ldx + i] - z[d]) : 0.0;
-}
-
 // out[rec][q] = sum over the nb block partials of rec, in block order
 __global__ void em_sum_parts_kernel(const double* __restrict__ part, int nb, int RL, double* __restrict__ out)
 {
@@ -1382,14 +1224,17 @@ __global__ void em_sum_parts_kernel(const double* __restrict__ part, int nb, int
 }
 
 // ---------------------------------------------------------------------------------------
-// 'EM' second derivatives (gpmpc_predict_em_hess).  The records of em_grad extended to degree 4: per owner index k,
-// features F_k,f over the other index (f runs over the unique monomials of degree <= 2 of the other index's v: 1, v_d,
-// v_d v_e with d <= e), and the record entries
-//   sum_k mono_mo(v_k) F_k,f   for every unique owner monomial mo of degree <= 4 with deg mo + deg f <= 4.
+// 'EM' derivative records (gpmpc_predict_em_grad: D = 2, gpmpc_predict_em_hess: D = 4).  Every O(N) / O(N^2) sum ends in
+// a record over a weight m and v_k = x_k - z: per owner index k, features F_k,f over the other index (f runs over the
+// unique monomials of degree <= D/2 of the other index's v: 1, v_d, and for D = 4 v_d v_e with d <= e), and the entries
+//   sum_k mono_mo(v_k) F_k,f   for every unique owner monomial mo of degree <= D with deg mo + deg f <= D.
 // Monomials are numbered by degree, then lexicographically over sorted index tuples; MONO[4 m + s] holds monomial m's
 // indices (-1 past its degree), ENT[2 q], ENT[2 q + 1] record entry q's (mo, f).  Both tables come from the host
-// (gpmpc.cu, em_hess_tables).  One partial per 64-index owner block, summed by em_sum_parts_kernel.
+// (gpmpc.cu, EmTables).  One partial per 64-index owner block, summed by em_sum_parts_kernel.
 // ---------------------------------------------------------------------------------------
+// monomials of degree <= k (k <= 2) in n variables: the feature count of a record of total degree 2k
+__host__ __device__ constexpr int em_nmono(int n, int k) { return k <= 0 ? 1 : (k == 1 ? 1 + n : 1 + n + n * (n + 1) / 2); }
+
 __device__ __forceinline__ double em_mono(const int* __restrict__ MONO, int m, const double* __restrict__ V, int k)
 {
     double r = 1.0;
@@ -1402,9 +1247,9 @@ __device__ __forceinline__ double em_mono(const int* __restrict__ MONO, int m, c
 }
 
 // record entries of one owner block: Vown [Nx][64], Fown [64][ldf] (features f < nf; entries with f >= nf are zero)
-__device__ __forceinline__ void em_hess_record(const double* __restrict__ Vown, const double* __restrict__ Fown, int ldf, int nf,
-                                               const int* __restrict__ MONO, const int* __restrict__ ENT, int nent,
-                                               double* __restrict__ out)
+__device__ __forceinline__ void em_record(const double* __restrict__ Vown, const double* __restrict__ Fown, int ldf, int nf,
+                                          const int* __restrict__ MONO, const int* __restrict__ ENT, int nent,
+                                          double* __restrict__ out)
 {
     for (int q = threadIdx.x; q < nent; q += blockDim.x) {
         const int mo = ENT[2 * q], f = ENT[2 * q + 1];
@@ -1424,18 +1269,18 @@ __device__ __forceinline__ void em_hess_record(const double* __restrict__ Vown, 
 }
 
 // Owner records with per-owner features: F_k,f = x1_k exp(x2_k) Fc[f][k] (null x1 / Fc count as 1, nf = 1 without Fc),
-// v_k = V[d][k] - z[d], k < n.  One 64-index block per CTA (blockIdx.x), one record per blockIdx.y (x1, x2 offset by sx,
-// Fc by sfc, record by srec).  Serves the mean records (x1 = alpha_a, x2 = log q_a) and the trace backbone (x2 = E,
-// Fc = K^-1 (e o features)).
-template <int NXP>
+// v_k = V[d][k] - z[d] (null z counts as 0), k < n.  One 64-index block per CTA (blockIdx.x), one record per blockIdx.y
+// (x1, x2 offset by sx, Fc by sfc, record by srec).  Serves the mean records (x1 = alpha_a, x2 = log q_a), the trace
+// backbone (x2 = E, Fc = K^-1 e for D = 2, K^-1 (e o features) for D = 4) and the backbone Gram (V = L^-1 rows, z null).
+template <int NXP, int D>
 __global__ void __launch_bounds__(256)
-em_hess_owner_kernel(const double* __restrict__ V, int ldv, int n, int Nx, const double* __restrict__ z,
-                     const double* __restrict__ x1, const double* __restrict__ x2, long long sx,
-                     const double* __restrict__ Fc, long long sfc, int ldfc, int nf,
-                     const int* __restrict__ MONO, const int* __restrict__ ENT, int nent,
-                     double* __restrict__ part, long long srec)
+em_owner_rec_kernel(const double* __restrict__ V, int ldv, int n, int Nx, const double* __restrict__ z,
+                    const double* __restrict__ x1, const double* __restrict__ x2, long long sx,
+                    const double* __restrict__ Fc, long long sfc, int ldfc, int nf,
+                    const int* __restrict__ MONO, const int* __restrict__ ENT, int nent,
+                    double* __restrict__ part, long long srec)
 {
-    constexpr int NFP = 1 + NXP + NXP * (NXP + 1) / 2;
+    constexpr int NFP = em_nmono(NXP, D / 2);
     extern __shared__ double sm[];
     double* Vown = sm;                     // [NXP][64]
     double* Fown = Vown + NXP * 64;        // [64][NFP]
@@ -1445,7 +1290,7 @@ em_hess_owner_kernel(const double* __restrict__ V, int ldv, int n, int Nx, const
     if (Fc) Fc += blockIdx.y * sfc;
     for (int idx = tid; idx < NXP * 64; idx += 256) {
         const int d = idx >> 6, k = k0 + (idx & 63);
-        Vown[idx] = (d < Nx && k < n) ? V[(long long)d * ldv + k] - z[d] : 0.0;
+        Vown[idx] = (d < Nx && k < n) ? V[(long long)d * ldv + k] - (z ? z[d] : 0.0) : 0.0;
     }
     for (int idx = tid; idx < 64 * nf; idx += 256) {
         const int kl = idx / nf, f = idx % nf, k = k0 + kl;
@@ -1454,37 +1299,41 @@ em_hess_owner_kernel(const double* __restrict__ V, int ldv, int n, int Nx, const
         Fown[kl * NFP + f] = w;
     }
     __syncthreads();
-    em_hess_record(Vown, Fown, NFP, nf, MONO, ENT, nent, part + blockIdx.y * srec + (long long)blockIdx.x * nent);
+    em_record(Vown, Fown, NFP, nf, MONO, ENT, nent, part + blockIdx.y * srec + (long long)blockIdx.x * nent);
 }
 
-// Pair records: em_grad_pair_kernel's tiles and weights (mode 0: the cross term's m_ij = w_ij expm1(delta_ij), pair
-// p = blockIdx.y, owner rows (o = 0) or columns (o = 1) by blockIdx.z; mode 1: K^-1_ij times the O(Sigma) remainder of
-// Q_aa, output a = blockIdx.y, owner rows), with the owner's features over every monomial of degree <= 2 of the other
-// index instead of 1 and v (degree <= 1 for o = 1; its other entries are written as zero).  Record rec0 + 2p + o (mode 0) or rec0 + a (mode 1), nent entries each.
-template <int NXP>
+// Pair sums of one 64-index owner block (blockIdx.x) against every other block, the 64x64 tiles recomputed as
+// em_pair_kernel does (no N x N array is written):
+//   mode 0, pair p = blockIdx.y, orientation o = blockIdx.z: the cross term's m_ij = w_ij expm1(x_ij) (em_cross_w,
+//     em_cross_x); owner = rows i (o = 0) or columns j (o = 1); record rec0 + 2p + o.
+//   mode 1, output a = blockIdx.y (pair (a,a)): m_ij = K^-1_ij Qt_ij with Qt the O(Sigma) remainder of Q_aa (em_rem);
+//     Kinv = full symmetric K^-1 per output (stride ldn^2); owner rows; record rec0 + a.
+// The owner's feature sums over the other index, F_k,f = sum m mono_f(v_other), stay in registers across the tiles
+// (fixed order); the record then sums over the owner block in index order.
+template <int NXP, int D>
 __global__ void __launch_bounds__(256)
-em_hess_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
-                    const double* __restrict__ alpha, long long sal,
-                    const double* __restrict__ XT, int ldx, const double* __restrict__ z,
-                    const double* __restrict__ E, const double* __restrict__ F, const double* __restrict__ W,
-                    const double* __restrict__ IJ, int ldn, const double* __restrict__ LQ,
-                    const double* __restrict__ E2, const double* __restrict__ F2,
-                    const double* __restrict__ Kinv, int mode, int rec0,
-                    const int* __restrict__ MONO, const int* __restrict__ ENT, int nent, double* __restrict__ part, int nb)
+em_pair_rec_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
+                   const double* __restrict__ alpha, long long sal,
+                   const double* __restrict__ XT, int ldx, const double* __restrict__ z,
+                   const double* __restrict__ E, const double* __restrict__ F, const double* __restrict__ W,
+                   const double* __restrict__ IJ, int ldn, const double* __restrict__ LQ,
+                   const double* __restrict__ E2, const double* __restrict__ F2,
+                   const double* __restrict__ Kinv, int mode, int rec0,
+                   const int* __restrict__ MONO, const int* __restrict__ ENT, int nent, double* __restrict__ part, int nb)
 {
-    constexpr int NFP = 1 + NXP + NXP * (NXP + 1) / 2;
+    constexpr int NFP = em_nmono(NXP, D / 2);
     constexpr int KF = (NFP + 3) / 4;                 // features per thread: f = g + 4q
     extern __shared__ double sm[];
     double* Wo = sm;                                  // [NXP][64] W rows of the i block
     double* Jo = Wo + NXP * 64;                       // [NXP][64] IJ rows of the j block
     double* Vown = Jo + NXP * 64;                     // [NXP][64] v of the owner block
-    double* Voth = Vown + NXP * 64;                   // [NXP][64] v of the other block
-    double* Ms = Voth + NXP * 64;                     // [64][65] m tile, owner-major
+    double* Ms = Vown + NXP * 64;                     // [64][65] m tile, owner-major
     double* Foth = Ms + 64 * 65;                      // [NFP][64] features of the other block; then [64][NFP] of the owner
+    double* Voth = Foth + 64;                         // v of the other block: feature rows 1..Nx, behind the row of ones
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
     const int o = mode ? 0 : blockIdx.z;
-    // column owners (o = 1) serve only the entries of owner degree >= 3, whose features have degree <= 1
-    const int nn = Nx * Nx, nf = o ? 1 + Nx : 1 + Nx + Nx * (Nx + 1) / 2;
+    // column owners (o = 1) serve only the entries of owner degree > D/2, whose features have degree < D/2
+    const int nn = Nx * Nx, nf = em_nmono(Nx, o ? D / 2 - 1 : D / 2);
     const int p = mode ? blockIdx.y * (blockIdx.y + 1) / 2 + blockIdx.y : blockIdx.y;
     const double* P = EMP + (long long)Ny * (2 * nn + 2) + (long long)p * (nn + 4);
     const int a = (int)P[nn + 1], b = (int)P[nn + 2];
@@ -1498,6 +1347,7 @@ em_hess_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
         if (o == 0) Wo[idx] = ok ? W[((long long)p * Nx + d) * ldn + k] : 0.0;
         else Jo[idx] = ok ? IJ[((long long)p * Nx + d) * ldn + k] : 0.0;
     }
+    if (tid < 64) Foth[tid] = 1.0;
     const int ko = tid & 63, g = tid >> 6;
     double acc2[KF];
 #pragma unroll
@@ -1505,32 +1355,18 @@ em_hess_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
     for (int t = 0; t < T; ++t) {
         const int oth0 = t * 64;
         __syncthreads();                              // previous tile's readers are done
-        for (int idx = tid; idx < NXP * 64; idx += 256) {
+        for (int idx = tid; idx < Nx * 64; idx += 256) {
             const int d = idx >> 6, k = oth0 + (idx & 63);
-            const bool ok = d < Nx && k < N;
+            const bool ok = k < N;
             Voth[idx] = ok ? XT[(long long)d * ldx + k] - z[d] : 0.0;
             if (o == 0) Jo[idx] = ok ? IJ[((long long)p * Nx + d) * ldn + k] : 0.0;
             else Wo[idx] = ok ? W[((long long)p * Nx + d) * ldn + k] : 0.0;
         }
         __syncthreads();
-        for (int idx = tid; idx < nf * 64; idx += 256) Foth[idx] = em_mono(MONO, idx >> 6, Voth, idx & 63);
+        for (int idx = (1 + Nx) * 64 + tid; idx < nf * 64; idx += 256) Foth[idx] = em_mono(MONO, idx >> 6, Voth, idx & 63);
         const int i0 = o ? oth0 : own0, j0 = o ? own0 : oth0;
         double acc[4][4];
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) acc[r][c] = 0.0;
-        for (int d = 0; d < Nx; ++d) {
-            double wv[4], jv[4];
-#pragma unroll
-            for (int r = 0; r < 4; ++r) wv[r] = Wo[d * 64 + ty + 16 * r];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) jv[c] = Jo[d * 64 + tx + 16 * c];
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) acc[r][c] = fma(wv[r], jv[c], acc[r][c]);
-        }
+        em_tile(Wo, Jo, Nx, tx, ty, acc);
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
             const int il = ty + 16 * r, i = i0 + il;
@@ -1538,15 +1374,9 @@ em_hess_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
             for (int c = 0; c < 4; ++c) {
                 const int jl = tx + 16 * c, j = j0 + jl;
                 double m = 0.0;
-                if (i < N && j < N) {
-                    if (mode) {
-                        m = Ka[(long long)i * ldn + j] * (exp(E[(long long)p * ldn + i] + F[(long long)p * ldn + j]) * expm1(2.0 * acc[r][c]));
-                    } else {
-                        const double la = LQ[(long long)a * ldn + i], lb = LQ[(long long)b * ldn + j];
-                        const double wgt = (alpha[(long long)a * sal + i] * exp(la)) * (alpha[(long long)b * sal + j] * exp(lb));
-                        m = wgt * expm1(cab + E2[(long long)p * ldn + i] + F2[(long long)p * ldn + j] + 2.0 * acc[r][c]);
-                    }
-                }
+                if (i < N && j < N)
+                    m = mode ? Ka[(long long)i * ldn + j] * em_rem(E, F, ldn, p, i, j, acc[r][c])
+                             : em_cross_w(alpha, sal, LQ, ldn, a, b, i, j) * expm1(em_cross_x(cab, E2, F2, ldn, p, i, j, acc[r][c]));
                 if (o == 0) Ms[il * 65 + jl] = m; else Ms[jl * 65 + il] = m;
             }
         }
@@ -1568,7 +1398,7 @@ em_hess_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
     }
     __syncthreads();
     const int rec = rec0 + (mode ? (int)blockIdx.y : 2 * p + o);
-    em_hess_record(Vown, Foth, NFP, nf, MONO, ENT, nent, part + ((long long)rec * nb + blockIdx.x) * nent);
+    em_record(Vown, Foth, NFP, nf, MONO, ENT, nent, part + ((long long)rec * nb + blockIdx.x) * nent);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1874,10 +1704,10 @@ em_hess_pair_finish_kernel(int Nx, int Ny, int h0, const double* __restrict__ EM
     }
 }
 
-// backbone feature rows of Q_aa for L^-1: R[f][i] = e_i mono_f(v_i) (f < nf, monomials of degree <= 2); zero for i >= N
-__global__ void em_hess_bb_rows_kernel(const double* __restrict__ XT, int ldx, int N, int Nx, const double* __restrict__ z,
-                                       const double* __restrict__ E, int n, const int* __restrict__ MONO, int nf,
-                                       double* __restrict__ R)
+// backbone feature rows of Q_aa for L^-1: R[f][i] = e_i mono_f(v_i) (f < nf: the record's features); zero for i >= N
+__global__ void em_backbone_rows_kernel(const double* __restrict__ XT, int ldx, int N, int Nx, const double* __restrict__ z,
+                                        const double* __restrict__ E, int n, const int* __restrict__ MONO, int nf,
+                                        double* __restrict__ R)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;

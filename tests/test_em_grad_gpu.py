@@ -119,9 +119,10 @@ def em_grad_errors(case):
 @pytest.mark.parametrize('case', ['tank', 'tank_pp', 'tank_large', 'syn1000', 'syn300', 'syn12'] + NEW_SHAPES)
 def test_em_grad_vs_closed_oracle(case):
     """syn1000: Nx = 8, N ~ 1000 (16 tiles); syn300: Nx = 17, the 32 bucket; syn12: Nx = 12, the 16 bucket of em_prep,
-    em_moments and em_grad_pair; tank_pp: one Sigma per point.  The shapes of test_em_shapes_gpu at Sigma = 0.1 Lambda and
-    Lambda: nx1, nx32 (em_grad_pair_kernel<32>'s opt-in shared memory at its largest), tma (em_moments, em_bb_rows and
-    trmv_lower_T on the 3072 pad), ny9 (nine outputs' records) and reserved (an identity tail of L^-1)."""
+    em_owner_rec and em_pair_rec; tank_pp: one Sigma per point.  The shapes of test_em_shapes_gpu at Sigma = 0.1 Lambda
+    and Lambda: nx1, nx32 (em_pair_rec_kernel<32, 2>'s opt-in shared memory at its largest), tma (em_owner_rec,
+    em_backbone_rows and trmv_lower_T on the 3072 pad), ny9 (nine outputs' records) and reserved (an identity tail of
+    L^-1)."""
     if case.startswith('tma'):
         _require(tma_on_device(), 'the TMA feed')
     errs = em_grad_errors(case)
@@ -133,7 +134,7 @@ def test_em_grad_vs_closed_oracle(case):
 
 
 def test_em_forward_nxp16_vs_exact_moment():
-    """The forward 'EM' moments at Nx = 12 (em_prep / em_moments<16>) on the well-conditioned syn12 model against the
+    """The forward 'EM' moments at Nx = 12 (em_prep / em_owner_rec<16, 2>) on the well-conditioned syn12 model against the
     fp64 restatement gp_exact_moment with postfit's K^-1.  Measured on an H100 SXM at 700 W: mean 1.2e-13, cov
     3.9e-11 (the restatement's own cancellation between beta beta^T and K^-1).  Then the nx12 case of test_em_shapes_gpu
     (N = 600, Ny = 3) against the long-double formula on the engine's alpha and factor at Sigma = 1e-5 Lambda, 0.1 Lambda
