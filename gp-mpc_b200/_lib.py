@@ -309,22 +309,27 @@ class Engine:
                                            _ptr(scale), _ptr(means), _ptr(var), _ptr(cov)))
         return means, var, cov
 
+    def _policy(self, B, Nt, U, scale, K, x_ref, uscale):
+        """The batched roll-outs' policy as their C entries take it: U (B,Nt,Nu), None under K or without inputs; scale
+        (4,Ny); K (Nu,Ny) and, with K only, x_ref (Ny,) and uscale (2,Nu)."""
+        Nu = self.Nx - self.Ny
+        U = _f64(U, (B, Nt, Nu)) if (Nu > 0 and K is None) else None
+        if scale is not None:
+            scale = _f64(scale, (4, self.Ny))
+        if K is None:                                    # x_ref and uscale are read only with K
+            return U, scale, None, None, None
+        return (U, scale, _f64(K, (Nu, self.Ny)), None if x_ref is None else _f64(x_ref, (self.Ny,)),
+                None if uscale is None else _f64(uscale, (2, Nu)))
+
     def rollout_batch(self, z0, U, Sigma0, method=METHOD_TA, scale=None, K=None, x_ref=None, uscale=None):
         """gpmpc_rollout_batch: B trajectories of Nt steps in one pass, open loop or with the feedback u = K (x - x_ref).
         z0:(B,Nx), U:(B,Nt,Nu) (GP input units; with K only its shape is used), Sigma0:(B,Nx,Nx), scale:(4,Ny)|None,
         K:(Nu,Ny)|None, x_ref:(Ny,)|None, uscale:(2,Nu)|None -> means (B,Nt,Ny), vars (B,Nt,Ny), cov_last (B,Ny,Ny)."""
-        Nu = self.Nx - self.Ny
         z0 = _f64(z0).reshape(-1, self.Nx)
         B = z0.shape[0]
         Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
         Nt = int(np.shape(U)[1])
-        U = _f64(U, (B, Nt, Nu)) if (Nu > 0 and K is None) else None
-        if scale is not None:
-            scale = _f64(scale, (4, self.Ny))
-        if K is not None:
-            K = _f64(K, (Nu, self.Ny))
-            x_ref = None if x_ref is None else _f64(x_ref, (self.Ny,))
-            uscale = None if uscale is None else _f64(uscale, (2, Nu))
+        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
         means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
         self._check(self.lib.gpmpc_rollout_batch(self.h, int(method), B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale),
                                                  _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means), _ptr(var), _ptr(cov)))
@@ -339,13 +344,7 @@ class Engine:
         B = z0.shape[0]
         Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
         Nt = int(np.shape(U)[1])
-        U = _f64(U, (B, Nt, Nu)) if (Nu > 0 and K is None) else None
-        if scale is not None:
-            scale = _f64(scale, (4, self.Ny))
-        if K is not None:
-            K = _f64(K, (Nu, self.Ny))
-            x_ref = None if x_ref is None else _f64(x_ref, (self.Ny,))
-            uscale = None if uscale is None else _f64(uscale, (2, Nu))
+        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
         P = self.Nx + (Nu * self.Ny if K is not None else (Nt - 1) * Nu)
         means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
         dmeans = np.empty((B, Nt, self.Ny, P)); dvars = np.empty((B, Nt, self.Ny, P))
@@ -360,20 +359,13 @@ class Engine:
         eps:(B,Nt,Ny) standard normals of the draws, xi:(B,Nt,Ny)|None process-noise normals, scale / K / x_ref / uscale
         as rollout_batch -> samples (B,Nt,Ny) GP output units, z_out (B,Nt,Nx) inputs used, kept (B,Nt,Ny) int32 (1 where
         the point entered the conditioning set)."""
-        Nu = self.Nx - self.Ny
         z0 = _f64(z0).reshape(-1, self.Nx)
         B = z0.shape[0]
         eps = _f64(eps)
         Nt = int(eps.shape[1])
         eps = eps.reshape(B, Nt, self.Ny)
         xi = None if xi is None else _f64(xi, (B, Nt, self.Ny))
-        U = _f64(U, (B, Nt, Nu)) if (Nu > 0 and K is None) else None
-        if scale is not None:
-            scale = _f64(scale, (4, self.Ny))
-        if K is not None:
-            K = _f64(K, (Nu, self.Ny))
-            x_ref = None if x_ref is None else _f64(x_ref, (self.Ny,))
-            uscale = None if uscale is None else _f64(uscale, (2, Nu))
+        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
         samples = np.empty((B, Nt, self.Ny)); z_out = np.empty((B, Nt, self.Nx))
         kept = np.empty((B, Nt, self.Ny), dtype=np.int32)
         self._check(self.lib.gpmpc_rollout_sample(self.h, B, Nt, _ptr(z0), _ptr(U), _ptr(eps), _ptr(xi), _ptr(scale),

@@ -2320,6 +2320,46 @@ static int derivs_prepare(gpmpc_handle_t h, int H, bool second, DerivSlabs* s);
 static int derivs_enqueue(gpmpc_handle_t h, int method, int H, const double* dZ, const double* dSigma, int spp,
                           const DerivSlabs& s);
 
+// Device views of a roll-out's feedback policy, null where absent (x_ref and uscale only with K)
+struct RolloutPolicy { const double *scale, *K, *x_ref, *uscale; };
+
+// A roll-out's policy block [U (B,Nt,Nu), open loop only | scale (4,Ny) | K (Nu,Ny) | x_ref (Ny) | uscale (2,Nu)] at slab
+// offset o: returns the offset past it.  Given the pinned mirror pin, also packs the block there and sets *pol to its
+// views in the device slab d.
+static size_t rollout_policy(int B, int Nt, int Ny, int Nu, const double* U, const double* scale, const double* K,
+                             const double* x_ref, const double* uscale, size_t o, double* pin = nullptr,
+                             const double* d = nullptr, RolloutPolicy* pol = nullptr)
+{
+    const size_t nU = U && !K ? (size_t)B * Nt * Nu : 0, o_sc = o + nU, o_k = o_sc + 4 * (size_t)Ny;
+    const size_t o_xr = o_k + (size_t)Nu * Ny, o_us = o_xr + Ny, end = o_us + 2 * (size_t)Nu;
+    if (!pin) return end;
+    if (nU) memcpy(pin + o, U, nU * 8);
+    if (scale) memcpy(pin + o_sc, scale, 4 * (size_t)Ny * 8);
+    if (K) memcpy(pin + o_k, K, (size_t)Nu * Ny * 8);
+    if (K && x_ref) memcpy(pin + o_xr, x_ref, (size_t)Ny * 8);
+    if (K && uscale) memcpy(pin + o_us, uscale, 2 * (size_t)Nu * 8);
+    *pol = {scale ? d + o_sc : nullptr, K ? d + o_k : nullptr, K && x_ref ? d + o_xr : nullptr, K && uscale ? d + o_us : nullptr};
+    return end;
+}
+
+// The argument checks every roll-out entry shares; nulls is the entry's own null-pointer test
+static int rollout_args(gpmpc_handle_t h, const char* fn, int B, int Nt, bool nulls, const double* U, const double* K)
+{
+    const int Nx = h->Nx, Ny = h->Ny, Nu = Nx - Ny;
+    if (B < 1 || Nt < 1 || nulls || (Nu > 0 && !K && !U)) { set_error(h, "%s: null argument / B < 1 / Nt < 1", fn); return GPMPC_ERR_ARG; }
+    if (Nu < 0) { set_error(h, "%s: needs Nx = Ny + Nu with Nu >= 0 (Nx=%d, Ny=%d)", fn, Nx, Ny); return GPMPC_ERR_ARG; }
+    if (K && Nu == 0) { set_error(h, "%s: a feedback gain needs inputs (Nu = 0)", fn); return GPMPC_ERR_ARG; }
+    return GPMPC_OK;
+}
+
+// (t, b) -> (b, t): row t B + b of the step-major src to row b Nt + t of dst, n doubles per row
+static void rows_by_trajectory(double* dst, const double* src, int B, int Nt, size_t n)
+{
+    for (size_t b = 0; b < (size_t)B; ++b)
+        for (int t = 0; t < Nt; ++t)
+            memcpy(dst + (b * Nt + t) * n, src + ((size_t)t * B + b) * n, n * 8);
+}
+
 // gpmpc_rollout_batch, gpmpc_rollout and with tg gpmpc_rollout_batch_grad; fn names the entry in errors
 static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, int Nt, const double* z0, const double* U,
                          const double* Sigma0, const double* scale, const double* K, const double* x_ref,
@@ -2329,19 +2369,17 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
     if (rc) return rc;
     const int Nx = h->Nx, Ny = h->Ny, Nu = Nx - Ny;
     if (method == GPMPC_METHOD_EM) { set_error(h, "%s: methods ME and TA (EM prepares every point on the host)", fn); return GPMPC_ERR_ARG; }
-    if (B < 1 || Nt < 1 || !z0 || !Sigma0 || !means || !vars || (Nu > 0 && !K && !U)) { set_error(h, "%s: null argument / B < 1 / Nt < 1", fn); return GPMPC_ERR_ARG; }
-    if (Nu < 0) { set_error(h, "%s: needs Nx = Ny + Nu with Nu >= 0 (Nx=%d, Ny=%d)", fn, Nx, Ny); return GPMPC_ERR_ARG; }
-    if (K && Nu == 0) { set_error(h, "%s: a feedback gain needs inputs (Nu = 0)", fn); return GPMPC_ERR_ARG; }
+    rc = rollout_args(h, fn, B, Nt, !z0 || !Sigma0 || !means || !vars, U, K);
+    if (rc) return rc;
     if (tg && (!tg->dmeans || !tg->dvars)) { set_error(h, "%s: null dmeans / dvars", fn); return GPMPC_ERR_ARG; }
     rc = predict_prepare(h, fn, B, true);
     if (rc) return rc;
     NvtxRange nvtx_r(tg ? "gpmpc.rollout_grad" : "gpmpc.rollout");
-    // device slab: [Z (B,Nx) | Sigma (B,Nx,Nx) | U (B,Nt,Nu) | scale (4,Ny) | K (Nu,Ny) | x_ref (Ny) | uscale (2,Nu) |
-    //               means (Nt,B,Ny) | vars (Nt,B,Ny) | cov (Nt,B,Ny,Ny)], host mirror in the pinned buffer.  Step t reads
-    //               and writes B consecutive points, so its outputs are one (B,...) block.
-    const size_t Bs = (size_t)B, nU = U && !K ? Bs * Nt * Nu : 0;
-    const size_t o_sig = Bs * Nx, o_u = o_sig + Bs * Nx * Nx, o_sc = o_u + nU, o_k = o_sc + 4 * (size_t)Ny;
-    const size_t o_xr = o_k + (size_t)Nu * Ny, o_us = o_xr + Ny, o_m = o_us + 2 * (size_t)Nu;
+    // device slab: [Z (B,Nx) | Sigma (B,Nx,Nx) | policy (rollout_policy) | means (Nt,B,Ny) | vars (Nt,B,Ny) |
+    //               cov (Nt,B,Ny,Ny)], host mirror in the pinned buffer.  Step t reads and writes B consecutive points,
+    //               so its outputs are one (B,...) block.
+    const size_t Bs = (size_t)B, o_sig = Bs * Nx, o_u = o_sig + Bs * Nx * Nx;
+    const size_t o_m = rollout_policy(B, Nt, Ny, Nu, U, scale, K, x_ref, uscale, o_u);
     const size_t o_v = o_m + (size_t)Nt * Bs * Ny, o_c = o_v + (size_t)Nt * Bs * Ny, tot = o_c + (size_t)Nt * Bs * Ny * Ny;
     ENSURE(h->dRoll, tot);
     // tangent slab: [dZ (B,P,Nx) | dS (B,P,Nx,Nx), 'TA' only | dmeans (Nt,B,Ny,P) | dvars (Nt,B,Ny,P)], the last two mirrored
@@ -2360,13 +2398,10 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
     double* pin = h->hPinned;
     memcpy(pin, z0, Bs * Nx * 8);
     memcpy(pin + o_sig, Sigma0, Bs * Nx * Nx * 8);
-    if (nU) memcpy(pin + o_u, U, nU * 8);
-    if (scale) memcpy(pin + o_sc, scale, 4 * (size_t)Ny * 8);
-    if (K) memcpy(pin + o_k, K, (size_t)Nu * Ny * 8);
-    if (K && x_ref) memcpy(pin + o_xr, x_ref, (size_t)Ny * 8);
-    if (K && uscale) memcpy(pin + o_us, uscale, 2 * (size_t)Nu * 8);
-    CUDA_TRY(cudaMemcpyAsync(h->dRoll, pin, o_m * 8, cudaMemcpyHostToDevice, h->st));
     double* d = h->dRoll;
+    RolloutPolicy pol;
+    rollout_policy(B, Nt, Ny, Nu, U, scale, K, x_ref, uscale, o_u, pin, d, &pol);
+    CUDA_TRY(cudaMemcpyAsync(d, pin, o_m * 8, cudaMemcpyHostToDevice, h->st));
     const int fb_smem = K ? (Ny + Nu * Ny) * 8 : 0;
     for (int t = 0; t < Nt; ++t) {
         double* cov_t = d + o_c + (size_t)t * Bs * Ny * Ny;
@@ -2382,16 +2417,13 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
             double* g = h->dRollTg;
             rollout_tangent_kernel<<<B, nw * 32, tg_smem, h->st>>>(Ny, Nu, (int)P, t, t == 0, t + 1 == Nt, method == GPMPC_METHOD_TA,
                                                                   h->dJ, ds.dvar, ds.dcov, d + o_m + (size_t)t * Bs * Ny, cov_t,
-                                                                  scale ? d + o_sc : nullptr, K ? d + o_k : nullptr,
-                                                                  K && x_ref ? d + o_xr : nullptr, K && uscale ? d + o_us : nullptr,
-                                                                  g, g + o_ds, g + o_dm + (size_t)t * Bs * Ny * P,
+                                                                  pol.scale, pol.K, pol.x_ref, pol.uscale, g, g + o_ds, g + o_dm + (size_t)t * Bs * Ny * P,
                                                                   g + o_dv + (size_t)t * Bs * Ny * P);
             CUDA_TRY(cudaGetLastError());
         }
         if (t + 1 < Nt) {
             rollout_feedback_kernel<<<B, 256, fb_smem, h->st>>>(d + o_m + (size_t)t * Bs * Ny, cov_t, d + o_u + (size_t)(t + 1) * Nu,
-                                                                (long long)Nt * Nu, scale ? d + o_sc : nullptr, K ? d + o_k : nullptr,
-                                                                K && x_ref ? d + o_xr : nullptr, K && uscale ? d + o_us : nullptr,
+                                                                (long long)Nt * Nu, pol.scale, pol.K, pol.x_ref, pol.uscale,
                                                                 Ny, Nu, d, d + o_sig);
             CUDA_TRY(cudaGetLastError());
         }
@@ -2400,20 +2432,17 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
     if (tg) CUDA_TRY(cudaMemcpyAsync(pin + tot, h->dRollTg + o_dm, (tg_tot - o_dm) * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
     // (t, b) -> (b, t); the reference records diag(covar_x) of every step (gp_class.py:793): the propagated variance, J Sigma J^T included
-    const size_t nyp = (size_t)Ny * P;
+    rows_by_trajectory(means, pin + o_m, B, Nt, Ny);
     for (size_t b = 0; b < Bs; ++b)
         for (int t = 0; t < Nt; ++t) {
             const size_t src = (size_t)t * Bs + b, dst = b * Nt + t;
-            memcpy(means + dst * Ny, pin + o_m + src * Ny, (size_t)Ny * 8);
             for (int a = 0; a < Ny; ++a) vars[dst * Ny + a] = pin[o_c + src * Ny * Ny + (size_t)a * Ny + a];
-            if (tg) {
-                memcpy(tg->dmeans + dst * nyp, pin + tot + src * nyp, nyp * 8);
-                memcpy(tg->dvars + dst * nyp, pin + tot + (o_dv - o_dm) + src * nyp, nyp * 8);
-            }
         }
-    if (cov_last)
-        for (size_t b = 0; b < Bs; ++b)
-            memcpy(cov_last + b * Ny * Ny, pin + o_c + ((size_t)(Nt - 1) * Bs + b) * Ny * Ny, (size_t)Ny * Ny * 8);
+    if (tg) {
+        rows_by_trajectory(tg->dmeans, pin + tot, B, Nt, (size_t)Ny * P);
+        rows_by_trajectory(tg->dvars, pin + tot + (o_dv - o_dm), B, Nt, (size_t)Ny * P);
+    }
+    if (cov_last) rows_by_trajectory(cov_last, pin + o_c + (size_t)(Nt - 1) * Bs * Ny * Ny, B, 1, (size_t)Ny * Ny);
     return GPMPC_OK;
 }
 
@@ -2858,17 +2887,16 @@ extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const doubl
     int rc = predict_guard(h, fn, GPMPC_METHOD_ME, 1);
     if (rc) return rc;
     const int Nx = h->Nx, Ny = h->Ny, Nu = Nx - Ny, np = h->Npad, nl = h->nloc;
-    if (B < 1 || Nt < 1 || !z0 || !eps || !samples || (Nu > 0 && !K && !U)) { set_error(h, "%s: null argument / B < 1 / Nt < 1", fn); return GPMPC_ERR_ARG; }
-    if (Nu < 0) { set_error(h, "%s: needs Nx = Ny + Nu with Nu >= 0 (Nx=%d, Ny=%d)", fn, Nx, Ny); return GPMPC_ERR_ARG; }
-    if (K && Nu == 0) { set_error(h, "%s: a feedback gain needs inputs (Nu = 0)", fn); return GPMPC_ERR_ARG; }
+    rc = rollout_args(h, fn, B, Nt, !z0 || !eps || !samples, U, K);
+    if (rc) return rc;
     const int cond_smem = (Nt + 1) * 8 + Nt * 4;           // sample_cond_kernel: c | conditioning steps
     if (cond_smem > 48 * 1024) { set_error(h, "%s: Nt = %d steps exceed the conditioning kernel's shared memory", fn, Nt); return GPMPC_ERR_ARG; }
     rc = predict_prepare(h, fn, B, true);
     if (rc) return rc;
     NvtxRange nvtx_r("gpmpc.rollout_sample");
-    const size_t Bs = (size_t)B, nE = Bs * Nt * Ny, nX = xi ? nE : 0, nU = U && !K ? Bs * Nt * Nu : 0;
-    const size_t o_xi = nE, o_u = o_xi + nX, o_sc = o_u + nU, o_k = o_sc + 4 * (size_t)Ny, o_xr = o_k + (size_t)Nu * Ny;
-    const size_t o_us = o_xr + Ny, o_z = o_us + 2 * (size_t)Nu, o_s = o_z + (size_t)Nt * Bs * Nx, o_kp = o_s + nE;
+    const size_t Bs = (size_t)B, nE = Bs * Nt * Ny, nX = xi ? nE : 0, o_xi = nE, o_u = o_xi + nX;
+    const size_t o_z = rollout_policy(B, Nt, Ny, Nu, U, scale, K, x_ref, uscale, o_u);
+    const size_t o_s = o_z + (size_t)Nt * Bs * Nx, o_kp = o_s + nE;
     const size_t o_m = o_kp + nE, o_r = o_m + (size_t)nl * Bs, tot = o_r + (size_t)nl * Bs * Nt * Nt;
     const long long sVa = (long long)Nt * B * np;          // V rows of one output: (Nt, B, Npad)
     ENSURE(h->dSmV, nl * sVa);
@@ -2878,13 +2906,10 @@ extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const doubl
     double* pin = h->hPinned;
     memcpy(pin, eps, nE * 8);
     if (nX) memcpy(pin + o_xi, xi, nX * 8);
-    if (nU) memcpy(pin + o_u, U, nU * 8);
-    if (scale) memcpy(pin + o_sc, scale, 4 * (size_t)Ny * 8);
-    if (K) memcpy(pin + o_k, K, (size_t)Nu * Ny * 8);
-    if (K && x_ref) memcpy(pin + o_xr, x_ref, (size_t)Ny * 8);
-    if (K && uscale) memcpy(pin + o_us, uscale, 2 * (size_t)Nu * 8);
-    memcpy(pin + o_z, z0, Bs * Nx * 8);                     // slot 0 of the input history
     double* d = h->dSmp;
+    RolloutPolicy pol;
+    rollout_policy(B, Nt, Ny, Nu, U, scale, K, x_ref, uscale, o_u, pin, d, &pol);
+    memcpy(pin + o_z, z0, Bs * Nx * 8);                     // slot 0 of the input history
     CUDA_TRY(cudaMemcpyAsync(d, pin, (o_z + Bs * Nx) * 8, cudaMemcpyHostToDevice, h->st));
     const int fb_smem = K ? Ny * 8 : 0;
     for (int t = 0; t < Nt; ++t) {
@@ -2897,23 +2922,21 @@ extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const doubl
         CUDA_TRY(cudaGetLastError());
         if (t + 1 < Nt) {
             rollout_feedback_kernel<<<B, 256, fb_smem, h->st>>>(d + o_s + (size_t)t * Bs * Ny, nullptr, d + o_u + (size_t)(t + 1) * Nu,
-                                                                (long long)Nt * Nu, scale ? d + o_sc : nullptr, K ? d + o_k : nullptr,
-                                                                K && x_ref ? d + o_xr : nullptr, K && uscale ? d + o_us : nullptr,
+                                                                (long long)Nt * Nu, pol.scale, pol.K, pol.x_ref, pol.uscale,
                                                                 Ny, Nu, Zt + Bs * Nx, nullptr);
             CUDA_TRY(cudaGetLastError());
         }
     }
     CUDA_TRY(cudaMemcpyAsync(pin + o_z, d + o_z, (o_m - o_z) * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
-    // (t, b) -> (b, t)
-    for (size_t b = 0; b < Bs; ++b)
-        for (int t = 0; t < Nt; ++t) {
-            const size_t src = (size_t)t * Bs + b, dst = b * Nt + t;
-            memcpy(samples + dst * Ny, pin + o_s + src * Ny, (size_t)Ny * 8);
-            if (z_out) memcpy(z_out + dst * Nx, pin + o_z + src * Nx, (size_t)Nx * 8);
-            if (kept)
+    rows_by_trajectory(samples, pin + o_s, B, Nt, Ny);
+    if (z_out) rows_by_trajectory(z_out, pin + o_z, B, Nt, Nx);
+    if (kept)
+        for (size_t b = 0; b < Bs; ++b)
+            for (int t = 0; t < Nt; ++t) {
+                const size_t src = (size_t)t * Bs + b, dst = b * Nt + t;
                 for (int a = 0; a < Ny; ++a) kept[dst * Ny + a] = pin[o_kp + src * Ny + a] != 0.0 ? 1 : 0;
-        }
+            }
     return GPMPC_OK;
 }
 

@@ -559,24 +559,11 @@ class GP:
         its own gain).  'ME' / 'TA' on a single handle run on the device (gpmpc_rollout_batch: one
         predict pass over all trajectories per step, one pass per distinct gain with feedback);
         'EM', sharded models and prior_mean_in_predict keep the host loop."""
-        Nx, Ny, Nu = self.__Nx, self.__Ny, self.__Nu
-        x0 = np.asarray(x0, dtype=np.float64)
-        single = x0.ndim < 2
-        X0 = x0.reshape(1, Ny) if single else x0.reshape(-1, Ny)
+        Ny = self.__Ny
+        X0, U, single, Nt = self.__trajectories(x0, u)
         nb = X0.shape[0]
-        u = np.asarray(u, dtype=np.float64)
-        if single:
-            U = (u.reshape(-1, Nu) if Nu > 0 else np.zeros((u.shape[0] if u.ndim else 0, 0)))[None]   # Nu = 0: Nt = len(u)
-        else:
-            U = u.reshape(nb, -1, Nu) if Nu > 0 else np.zeros((nb, u.shape[1] if u.ndim > 1 else 0, 0))
-        Nt = U.shape[1]
         if feedback:
-            if Nu == 0:
-                raise ValueError('rollout(feedback=True) needs a model with inputs (Nu > 0)')
-            Q = np.eye(Ny) if Q is None else np.asarray(Q, dtype=np.float64)      # gp_class.py:760-766
-            R = np.eye(Nu) if R is None else np.asarray(R, dtype=np.float64)
-            x_ref = np.zeros(Ny) if x_ref is None else np.asarray(x_ref, dtype=np.float64).reshape(Ny)
-        initVar = self.__hyper[:, Nx + 1] ** 2
+            Q, R, x_ref = self.__feedback_defaults('rollout', Q, R, x_ref)
         if methods is None:                             # gp_class.py:747 default; 'EM' only where it can run
             methods = ['TA', 'ME'] if self.__sharded_outputs() else ['EM', 'TA', 'ME']
         methods = list(methods)
@@ -584,14 +571,15 @@ class GP:
         var = np.zeros((len(methods), nb, Nt + 1, Ny))
         # one input covariance per trajectory, shared across methods as in the reference: with feedback, method i+1
         # starts from the Sigma_uu / Sigma_xu blocks that method i left behind (gp_class.py:764, :797-801)
-        covar = np.tile(np.eye(Nx) * 1e-6, (nb, 1, 1))
+        covar = self.__initial_covar(nb)
+        covar_x0 = covar[:, :Ny, :Ny].copy()
         keep = self.__gp_method
         # 'ME' / 'TA' on a single handle: all Nt steps run on the device, same arithmetic as the loop below
         on_device = (device_rollout and self.__comm.world == 1
                      and not (self.__prior_mean_in_predict and self.__has_prior_mean()))
         for i, meth in enumerate(methods):
             self.set_method(meth)
-            covar[:, :Ny, :Ny] = np.diag(initVar)
+            covar[:, :Ny, :Ny] = covar_x0
             mean[i, :, 0, :] = X0
             K = self.__lqr_gains(X0, U[:, 0], Q, R) if feedback else None      # once per method, as the reference
             if on_device and meth in ('ME', 'TA') and Nt > 0 and self.__rollout_device(i, meth, X0, U, covar, K, x_ref,
@@ -624,6 +612,60 @@ class GP:
             Ks.append(lqr(A, Bm, Q, R)[0])
         return np.stack(Ks)
 
+    def __trajectories(self, x0, u):
+        """The roll-outs' shapes: x0:(Ny,) with u:(Nt,Nu), or a batch x0:(B,Ny) with u:(B,Nt,Nu) -> X0 (B,Ny), U (B,Nt,Nu),
+        single, Nt.  With Nu = 0, u only sets Nt."""
+        Ny, Nu = self.__Ny, self.__Nu
+        x0 = np.asarray(x0, dtype=np.float64)
+        single = x0.ndim < 2
+        X0 = x0.reshape(1, Ny) if single else x0.reshape(-1, Ny)
+        nb = X0.shape[0]
+        u = np.asarray(u, dtype=np.float64)
+        if single:
+            U = (u.reshape(-1, Nu) if Nu > 0 else np.zeros((u.shape[0] if u.ndim else 0, 0)))[None]   # Nu = 0: Nt = len(u)
+        else:
+            U = u.reshape(nb, -1, Nu) if Nu > 0 else np.zeros((nb, u.shape[1] if u.ndim > 1 else 0, 0))
+        return X0, U, single, U.shape[1]
+
+    def __feedback_defaults(self, fn, Q, R, x_ref):
+        """Q, R, x_ref of a feedback roll-out with the reference's defaults Q = I, R = I, x_ref = 0 (gp_class.py:760-766);
+        fn names the caller in the error for a model without inputs."""
+        Ny, Nu = self.__Ny, self.__Nu
+        if Nu == 0:
+            raise ValueError('%s(feedback=True) needs a model with inputs (Nu > 0)' % fn)
+        return (np.eye(Ny) if Q is None else np.asarray(Q, dtype=np.float64),
+                np.eye(Nu) if R is None else np.asarray(R, dtype=np.float64),
+                np.zeros(Ny) if x_ref is None else np.asarray(x_ref, dtype=np.float64).reshape(Ny))
+
+    def __initial_covar(self, nb):
+        """The roll-outs' initial input covariance for each of nb trajectories: diag(sn2) on x, 1e-6 on u."""
+        Nx, Ny = self.__Nx, self.__Ny
+        covar = np.tile(np.eye(Nx) * 1e-6, (nb, 1, 1))
+        covar[:, :Ny, :Ny] = np.diag(self.__hyper[:, Nx + 1] ** 2)
+        return covar
+
+    def __engine_start(self, X0, U, K, x_ref):
+        """The engine's view of a roll-out: z0 = [x0, u_0] with u_0 = U[:, 0] open loop or K (x0 - x_ref) with feedback, and
+        U, both in the GP's input units, with scale = [stdY | meanY | meanX | stdX] and uscale = [meanU | stdU], the scalers
+        the engine applies between steps (None without normalize)."""
+        u0 = U[:, 0] if K is None else np.stack([_matmul_seq(K[b], (X0[b] - x_ref)[:, None])[:, 0] for b in range(len(X0))])
+        if not self.__normalize:
+            return np.concatenate([X0, u0], 1), U, None, None
+        zx = self.standardize(X0, self.__meanX, self.__stdX)
+        z0 = np.concatenate([zx, self.standardize(u0, self.__meanU, self.__stdU)], 1)
+        scale = np.stack([self.__stdY, self.__meanY, self.__meanX, self.__stdX])
+        return z0, self.standardize(U, self.__meanU, self.__stdU), scale, np.stack([self.__meanU, self.__stdU])
+
+    @staticmethod
+    def __gain_groups(K, nb):
+        """A roll-out's engine passes as (trajectories, gain): all nb open loop (K None), else one pass per distinct gain."""
+        if K is None:
+            return [(np.arange(nb), None)]
+        groups = {}
+        for b in range(nb):
+            groups.setdefault(K[b].tobytes(), []).append(b)
+        return [(np.array(g), K[g[0]]) for g in groups.values()]
+
     def __feedback_blocks(self, cv, K, covar_x):
         """gp_class.py:797-801: the input blocks of the next step's covariance under u = K x."""
         Ny = self.__Ny
@@ -634,30 +676,17 @@ class GP:
 
     def __rollout_device(self, i, meth, X0, U, covar, K, x_ref, single, mean, var):
         """Method i of every trajectory on the device; False when the engine has no roll-out entry for the case."""
-        eng, nb = self.__engine, X0.shape[0]
+        eng = self.__engine
         use_single = single and K is None and hasattr(eng, 'rollout')       # gpmpc_rollout, the one open-loop trajectory
         if not (use_single or hasattr(eng, 'rollout_batch')):
             return False
-        zx, un, scale, uscale = X0, U, None, None
-        if K is not None:
-            un = np.stack([_matmul_seq(K[b], (X0[b] - x_ref)[:, None])[:, 0] for b in range(nb)])[:, None, :]   # the loop's first u_t
-        if self.__normalize:
-            zx = self.standardize(X0, self.__meanX, self.__stdX)
-            un = self.standardize(un, self.__meanU, self.__stdU)
-            scale = np.stack([self.__stdY, self.__meanY, self.__meanX, self.__stdX])
-            uscale = np.stack([self.__meanU, self.__stdU])
-        z0 = np.concatenate([zx, un[:, 0, :]], 1)
+        z0, Ug, scale, uscale = self.__engine_start(X0, U, K, x_ref)
         method = _GPU_METHODS[meth]
         if use_single:
-            parts = [(np.arange(1),) + tuple(r[None] for r in eng.rollout(z0[0], un[0], covar[0], method, scale))]
-        elif K is None:
-            parts = [(np.arange(nb),) + tuple(eng.rollout_batch(z0, un, covar, method, scale))]
-        else:                                            # one pass per distinct gain
-            groups = {}
-            for b in range(nb):
-                groups.setdefault(K[b].tobytes(), []).append(b)
-            parts = [(g,) + tuple(eng.rollout_batch(z0[g], U[g], covar[g], method, scale, K[g[0]], x_ref, uscale))
-                     for g in map(np.array, groups.values())]
+            parts = [(np.arange(1),) + tuple(r[None] for r in eng.rollout(z0[0], Ug[0], covar[0], method, scale))]
+        else:
+            parts = [(g,) + tuple(eng.rollout_batch(z0[g], Ug[g], covar[g], method, scale, Kg, x_ref, uscale))
+                     for g, Kg in self.__gain_groups(K, len(X0))]
         for g, m_std, v_std, c_last in parts:
             mean[i, g, 1:, :] = self.inverse_mean(m_std, self.__meanY, self.__stdY) if self.__normalize else m_std
             var[i, g, 1:, :] = self.inverse_variance(v_std) if self.__normalize else v_std
@@ -693,55 +722,23 @@ class GP:
             raise NotImplementedError('rollout_grad differentiates the zero-mean posterior the engine holds; '
                                       'prior_mean_in_predict with a prior mean function is not supported')
         Nx, Ny, Nu = self.__Nx, self.__Ny, self.__Nu
-        x0 = np.asarray(x0, dtype=np.float64)
-        single = x0.ndim < 2
-        X0 = x0.reshape(1, Ny) if single else x0.reshape(-1, Ny)
+        X0, U, single, Nt = self.__trajectories(x0, u)
         nb = X0.shape[0]
-        u = np.asarray(u, dtype=np.float64)
-        if single:
-            U = (u.reshape(-1, Nu) if Nu > 0 else np.zeros((u.shape[0] if u.ndim else 0, 0)))[None]
-        else:
-            U = u.reshape(nb, -1, Nu) if Nu > 0 else np.zeros((nb, u.shape[1] if u.ndim > 1 else 0, 0))
-        Nt = U.shape[1]
         if Nt < 1:
             raise ValueError('rollout_grad needs at least one step')
-        K = None
         if feedback:
-            if Nu == 0:
-                raise ValueError('rollout_grad(feedback=True) needs a model with inputs (Nu > 0)')
-            Q = np.eye(Ny) if Q is None else np.asarray(Q, dtype=np.float64)
-            R = np.eye(Nu) if R is None else np.asarray(R, dtype=np.float64)
-            x_ref = np.zeros(Ny) if x_ref is None else np.asarray(x_ref, dtype=np.float64).reshape(Ny)
-            K = self.__lqr_gains(X0, U[:, 0], Q, R)
-        covar = np.tile(np.eye(Nx) * 1e-6, (nb, 1, 1))                 # rollout's initial covariance
-        covar[:, :Ny, :Ny] = np.diag(self.__hyper[:, Nx + 1] ** 2)
-        # z0 and the scalers exactly as __rollout_device forms them, so mean / var are rollout's bits
-        un, scale, uscale = U, None, None
-        if K is not None:
-            un = np.stack([_matmul_seq(K[b], (X0[b] - x_ref)[:, None])[:, 0] for b in range(nb)])[:, None, :]
-        zx = X0
-        sX, sU, sY = np.ones(Ny), np.ones(Nu), np.ones(Ny)
-        if self.__normalize:
-            zx = self.standardize(X0, self.__meanX, self.__stdX)
-            un = self.standardize(un, self.__meanU, self.__stdU)
-            scale = np.stack([self.__stdY, self.__meanY, self.__meanX, self.__stdX])
-            uscale = np.stack([self.__meanU, self.__stdU])
-            sX, sU, sY = self.__stdX, self.__stdU, self.__stdY
-        z0 = np.concatenate([zx, un[:, 0, :]], 1)
+            Q, R, x_ref = self.__feedback_defaults('rollout_grad', Q, R, x_ref)
+        K = self.__lqr_gains(X0, U[:, 0], Q, R) if feedback else None
+        covar = self.__initial_covar(nb)
+        z0, Ug, scale, uscale = self.__engine_start(X0, U, K, x_ref)
+        sX, sU, sY = (self.__stdX, self.__stdU, self.__stdY) if self.__normalize else (np.ones(Ny), np.ones(Nu), np.ones(Ny))
         method_id, eng = _GPU_METHODS[meth], self.__engine
         P = Nx + (Nu * Ny if K is not None else (Nt - 1) * Nu)
         m_std = np.empty((nb, Nt, Ny)); v_std = np.empty((nb, Nt, Ny))
         Dm = np.empty((nb, Nt, Ny, P)); Dv = np.empty((nb, Nt, Ny, P))
-        if K is None:
-            parts = [(np.arange(nb), eng.rollout_batch_grad(z0, un, covar, method_id, scale))]
-        else:                                            # one pass per distinct gain, as rollout
-            groups = {}
-            for b in range(nb):
-                groups.setdefault(K[b].tobytes(), []).append(b)
-            parts = [(g, eng.rollout_batch_grad(z0[g], U[g], covar[g], method_id, scale, K[g[0]], x_ref, uscale))
-                     for g in map(np.array, groups.values())]
-        for g, (mg, vg, _, dmg, dvg) in parts:
-            m_std[g], v_std[g], Dm[g], Dv[g] = mg, vg, dmg, dvg
+        for g, Kg in self.__gain_groups(K, nb):
+            m_std[g], v_std[g], _, Dm[g], Dv[g] = eng.rollout_batch_grad(z0[g], Ug[g], covar[g], method_id, scale, Kg, x_ref,
+                                                                         uscale)
         # caller units: mean = m stdY + meanY, var = v stdY^2; z0 = [(x0 - meanX) / stdX, (u_0 - meanU) / stdU]
         Dm = Dm * sY[None, None, :, None]
         Dv = Dv * (sY ** 2)[None, None, :, None]
@@ -801,47 +798,22 @@ class GP:
         if self.__prior_mean_in_predict and self.__has_prior_mean():
             raise NotImplementedError('sample_rollout draws from the zero-mean posterior the engine holds; '
                                       'prior_mean_in_predict with a prior mean function is not supported')
-        Nx, Ny, Nu = self.__Nx, self.__Ny, self.__Nu
-        x0 = np.asarray(x0, dtype=np.float64)
-        single = x0.ndim < 2
-        X0 = x0.reshape(1, Ny) if single else x0.reshape(-1, Ny)
-        nb = X0.shape[0]
-        u = np.asarray(u, dtype=np.float64)
-        if single:
-            U = (u.reshape(-1, Nu) if Nu > 0 else np.zeros((u.shape[0] if u.ndim else 0, 0)))[None]
-        else:
-            U = u.reshape(nb, -1, Nu) if Nu > 0 else np.zeros((nb, u.shape[1] if u.ndim > 1 else 0, 0))
-        Nt, ns = U.shape[1], int(n_samples)
+        Nx, Ny = self.__Nx, self.__Ny
+        X0, U, single, Nt = self.__trajectories(x0, u)
+        nb, ns = X0.shape[0], int(n_samples)
         if ns < 1 or Nt < 1:
             raise ValueError('sample_rollout needs n_samples >= 1 and at least one step (got %d, %d)' % (ns, Nt))
-        if feedback and Nu == 0:
-            raise ValueError('sample_rollout(feedback=True) needs a model with inputs (Nu > 0)')
+        if feedback:
+            Q, R, x_ref = self.__feedback_defaults('sample_rollout', Q, R, x_ref)
         if Sigma0 is None:
-            S0 = np.eye(Nx) * 1e-6
-            S0[:Ny, :Ny] = np.diag(self.__hyper[:, Nx + 1] ** 2)
-            S0 = np.tile(S0, (nb, 1, 1))
+            S0 = self.__initial_covar(nb)
         else:
             S0 = np.asarray(Sigma0, dtype=np.float64)
             if S0.shape not in ((Nx, Nx), (nb, Nx, Nx)):
                 raise ValueError('Sigma0 must be (%d, %d) or (%d, %d, %d)' % (Nx, Nx, nb, Nx, Nx))
             S0 = np.broadcast_to(S0, (nb, Nx, Nx))
-        K = None
-        if feedback:
-            Q = np.eye(Ny) if Q is None else np.asarray(Q, dtype=np.float64)
-            R = np.eye(Nu) if R is None else np.asarray(R, dtype=np.float64)
-            x_ref = np.zeros(Ny) if x_ref is None else np.asarray(x_ref, dtype=np.float64).reshape(Ny)
-            K = self.__lqr_gains(X0, U[:, 0], Q, R)
-            un = np.stack([_matmul_seq(K[b], (X0[b] - x_ref)[:, None])[:, 0] for b in range(nb)])
-        else:
-            un = U[:, 0]
-        zx, Ug, scale, uscale = X0, U, None, None
-        if self.__normalize:
-            zx = self.standardize(X0, self.__meanX, self.__stdX)
-            un = self.standardize(un, self.__meanU, self.__stdU)
-            Ug = self.standardize(U, self.__meanU, self.__stdU)
-            scale = np.stack([self.__stdY, self.__meanY, self.__meanX, self.__stdX])
-            uscale = np.stack([self.__meanU, self.__stdU])
-        zbar = np.concatenate([zx, un], 1)
+        K = self.__lqr_gains(X0, U[:, 0], Q, R) if feedback else None
+        zbar, Ug, scale, uscale = self.__engine_start(X0, U, K, x_ref)
         rng = np.random.default_rng(seed)
         n0 = rng.standard_normal((nb, ns, Nx))
         eps = rng.standard_normal((nb, ns, Nt, Ny))
@@ -852,17 +824,10 @@ class GP:
         z0f, epsf = z0.reshape(nb * ns, Nx), eps.reshape(nb * ns, Nt, Ny)
         xif = None if xi is None else xi.reshape(nb * ns, Nt, Ny)
         samp = np.empty((nb * ns, Nt, Ny))
-        eng = self.__engine
-        if K is None:
-            samp[:] = eng.rollout_sample(z0f, Ur, epsf, xif, scale)[0]
-        else:                                            # one pass per distinct gain, as rollout
-            groups = {}
-            for b in range(nb):
-                groups.setdefault(K[b].tobytes(), []).append(b)
-            for g in groups.values():
-                r = rows(g)
-                samp[r] = eng.rollout_sample(z0f[r], Ur[r], epsf[r], None if xif is None else xif[r], scale, K[g[0]],
-                                             x_ref, uscale)[0]
+        for g, Kg in self.__gain_groups(K, nb):
+            r = rows(g)
+            samp[r] = self.__engine.rollout_sample(z0f[r], Ur[r], epsf[r], None if xif is None else xif[r], scale, Kg, x_ref,
+                                                   uscale)[0]
         out = np.empty((nb * ns, Nt + 1, Ny))
         out[:, 0] = z0f[:, :Ny]
         out[:, 1:] = samp
