@@ -53,6 +53,7 @@ SYMBOLS = [
     ('gpmpc_rollout', C.c_int, [_H, C.c_int, C.c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp]),
     ('gpmpc_rollout_batch', C.c_int, [_H, C.c_int, C.c_int, C.c_int] + [_dp] * 10),
     ('gpmpc_rollout_batch_grad', C.c_int, [_H, C.c_int, C.c_int, C.c_int] + [_dp] * 12),
+    ('gpmpc_rollout_batch_em', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 10),
     ('gpmpc_rollout_sample', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 10 + [_ip]),
     ('gpmpc_predict_device', C.c_int, [_H, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
@@ -333,6 +334,19 @@ class Engine:
         means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
         self._check(self.lib.gpmpc_rollout_batch(self.h, int(method), B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale),
                                                  _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means), _ptr(var), _ptr(cov)))
+        return means, var, cov
+
+    def rollout_batch_em(self, z0, U, Sigma0, scale=None, K=None, x_ref=None, uscale=None):
+        """gpmpc_rollout_batch_em: rollout_batch with exact moment matching ('EM'), same arguments (no method) and outputs;
+        each trajectory's results are those of the host loop of predict(EM) calls, bit for bit."""
+        z0 = _f64(z0).reshape(-1, self.Nx)
+        B = z0.shape[0]
+        Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
+        Nt = int(np.shape(U)[1])
+        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
+        means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
+        self._check(self.lib.gpmpc_rollout_batch_em(self.h, B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale), _ptr(K),
+                                                    _ptr(x_ref), _ptr(uscale), _ptr(means), _ptr(var), _ptr(cov)))
         return means, var, cov
 
     def rollout_batch_grad(self, z0, U, Sigma0, method=METHOD_TA, scale=None, K=None, x_ref=None, uscale=None):

@@ -206,6 +206,7 @@ struct gpmpc_handle_s {
     std::vector<int> jitter_used;
     int sms = 132;                    // multiprocessors of the device (queried in create)
     int opt_refine = 0, opt_small_tiles = 528;   // 128x64-tile count below which 64x32 tiles are used (4 per SM)
+    int opt_em_points = 0;            // points per batched 'EM' forward (0: the scratch budget EM_CHUNK_BYTES decides)
     // comm
     nccl_comm_t comm = nullptr; int rank = 0, world = 1;
     // peer (CUDA IPC) exchange: [flags: 2*MAXW u64][gather buffer parity 0][parity 1]
@@ -302,7 +303,18 @@ static cudaError_t gemm128(gpmpc_handle_t h, cudaStream_t st, bool bt, const Gem
                   : gemm_launch<64, 32, 2, 2, false, 3, 4>(q, batch, st);
     }
     q.nt = p.nt * 2;
-    if (bt && tiles >= 4LL * h->sms) return gemm_tmap_launch<128, 64, 2, 2, 4, 2>(q, batch, st);
+    if (bt && tiles >= 4LL * h->sms) {
+        if (p.sA != 0 || batch == 1) return gemm_tmap_launch<128, 64, 2, 2, 4, 2>(q, batch, st);
+        // a tensor map cannot step a zero batch stride: one launch per slab (each already fills four waves)
+        for (int z = 0; z < batch; ++z) {
+            GemmParams r = q;
+            r.B += z * p.sB; r.C += z * p.sC;
+            if (r.Cin) r.Cin += z * p.sCin;
+            const cudaError_t e = gemm_tmap_launch<128, 64, 2, 2, 4, 2>(r, 1, st);
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    }
     return bt ? gemm_launch<128, 64, 2, 2, true, 3, 2>(q, batch, st)
               : gemm_launch<128, 64, 2, 2, false, 3, 2>(q, batch, st);
 }
@@ -1191,6 +1203,10 @@ extern "C" int gpmpc_set_option(gpmpc_handle_t h, const char* name, double value
     if (!strcmp(name, "peer_timeout_s")) { h->opt_peer_timeout_s = value > 0.0 ? value : 60.0; return GPMPC_OK; }
     if (!strcmp(name, "small_tiles")) { h->opt_small_tiles = (int)value; return GPMPC_OK; }
     if (!strcmp(name, "peer")) { h->opt_peer = value != 0.0; return GPMPC_OK; }
+    if (!strcmp(name, "em_points")) {          // points per batched 'EM' forward (0 = the scratch budget decides)
+        if (!(value >= 0.0 && value <= 1e9)) { set_error(h, "em_points must be >= 0"); return GPMPC_ERR_ARG; }
+        h->opt_em_points = (int)value; return GPMPC_OK;
+    }
     if (!strcmp(name, "nlml_batch_max")) {     // entries per gpmpc_nlml_batch pass (0 = all): a cap on its scratch
         if (!(value >= 0.0 && value <= 1e9)) { set_error(h, "nlml_batch_max must be >= 0"); return GPMPC_ERR_ARG; }
         h->opt_nlml_batch_max = (int)value; return GPMPC_OK;
@@ -1590,13 +1606,108 @@ static int em_prepare_point(gpmpc_handle_t h, const double* S, double* out)
     return GPMPC_OK;
 }
 
-template <int NXP>
-static cudaError_t launch_em_prep(gpmpc_handle_t h, int npairs, const double* dz, const double* dEMP, int nblk)
+// ------------------------------------------------------------------------------------
+// The batched 'EM' forward (DESIGN 4.8): one launch set per chunk of points, each point in its own slice of the scratch
+// (EmStrides).  The chunk is bounded by a byte budget, dominated by the two Npad^2 slabs per point (Q~ in dKinv, L^-1 Q~ in
+// dU): 20 MB a point in all at Npad 1024, one point from Npad ~ 5800 on.
+// ------------------------------------------------------------------------------------
+#define EM_CHUNK_BYTES (1LL << 30)
+
+static inline int em_npairs(gpmpc_handle_t h) { return h->Ny * (h->Ny + 1) / 2; }
+static inline size_t em_per(gpmpc_handle_t h)     // doubles of one point's em_prepare_point block
 {
-    dim3 g(nblk, h->Ny + npairs);
+    const size_t nn = (size_t)h->Nx * h->Nx;
+    return (size_t)h->Ny * (2 * nn + 2) + (size_t)em_npairs(h) * (nn + 4);
+}
+
+static EmStrides em_strides(gpmpc_handle_t h)
+{
+    const long long np = h->Npad, Ny = h->Ny, npairs = em_npairs(h), T = (h->N + 63) / 64, Tq = np / 64;
+    EmStrides s;
+    s.z = h->Nx; s.emp = (long long)em_per(h);
+    s.mpart = Ny * ((np + 255) / 256); s.pair = npairs * np; s.w = npairs * h->Nx * np;
+    s.lq = Ny * np; s.part = npairs * T * T; s.q = slab(h);
+    s.tr = Ny * (Tq * (Tq + 1) / 2); s.vec = 2 * np + Ny;
+    return s;
+}
+
+// points per forward for H points: the byte budget, the grid's z extent of the pair sums (points x pairs) and em_points
+static int em_chunk(gpmpc_handle_t h, int H)
+{
+    const EmStrides s = em_strides(h);
+    const long long bytes = 8 * (2 * s.q + s.mpart + 4 * s.pair + 2 * s.w + s.lq + s.part + s.tr + s.vec);
+    long long n = std::min<long long>({(long long)H, EM_CHUNK_BYTES / bytes, 65535 / em_npairs(h)});
+    if (h->opt_em_points > 0) n = std::min<long long>(n, h->opt_em_points);
+    return (int)std::max(1LL, n);
+}
+
+// scratch of n points and the em_prepare_point blocks of H points
+static int em_scratch(gpmpc_handle_t h, int n, int H)
+{
+    const EmStrides s = em_strides(h);
+    ENSURE(h->dEmTr, n * s.tr);
+    ENSURE(h->dEmLQ, n * s.lq);
+    ENSURE(h->dEmVec, n * s.vec);
+    ENSURE(h->dEmE, n * s.pair); ENSURE(h->dEmF, n * s.pair);
+    ENSURE(h->dEmE2, n * s.pair); ENSURE(h->dEmF2, n * s.pair);
+    ENSURE(h->dEmW, n * s.w); ENSURE(h->dEmIJ, n * s.w);
+    ENSURE(h->dEmMeanPart, n * s.mpart); ENSURE(h->dEmPart, n * s.part);
+    { int rcs = ensure_nlml_scratch(h); if (rcs) return rcs; }
+    ENSURE(h->dKinv, n * s.q); ENSURE(h->dU, n * s.q);
+    ENSURE(h->dEMP, (long long)H * s.emp);
+    return GPMPC_OK;
+}
+
+template <int NXP>
+static cudaError_t launch_em_prep(gpmpc_handle_t h, int n, int npairs, const double* dz, const double* dEMP, int nblk, const EmStrides& s)
+{
+    dim3 g(nblk, h->Ny + npairs, n);
     em_prep_kernel<NXP><<<g, 256, 0, h->st>>>(h->dXT, h->Npad, h->N, h->Nx, h->Ny, npairs, h->dHyp, h->Nx + 2, h->dAlpha, h->Npad,
-                                              dz, dEMP, h->dEmMeanPart, nblk, h->dEmE, h->dEmF, h->dEmW, h->dEmIJ, h->Npad, h->dEmLQ, h->dEmE2, h->dEmF2);
+                                              dz, dEMP, h->dEmMeanPart, nblk, h->dEmE, h->dEmF, h->dEmW, h->dEmIJ, h->Npad, h->dEmLQ, h->dEmE2, h->dEmF2, s);
     return cudaGetLastError();
+}
+
+// The forward of n <= em_chunk points: z at dz (stride Nx, device), their em_prepare_point blocks at dP (stride em_per, device),
+// mean / var / cov out at strides Ny / Ny / Ny^2 (device).  Point k's scratch stays in slot k for the derivative records.
+static int em_forward(gpmpc_handle_t h, int n, const double* dz, const double* dP, double* mean, double* var, double* cov)
+{
+    const int Nx = h->Nx, Ny = h->Ny, np = h->Npad, npairs = em_npairs(h);
+    const int nblk = (np + 255) / 256, T = (h->N + 63) / 64, Tq = np / 64, ntr = Tq * (Tq + 1) / 2;
+    const EmStrides s = em_strides(h);
+    CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_prep<decltype(nxp)::value>(h, n, npairs, dz, dP, nblk, s); }));
+    em_pair_kernel<<<dim3(T, T, n * npairs), 256, 2 * Nx * 64 * 8, h->st>>>(h->N, Nx, Ny, dP, h->dAlpha, np,
+                                                                          h->dEmE, h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2, h->dEmPart, 0, 0, nullptr, 0, s);
+    CUDA_TRY(cudaGetLastError());
+    // E[var] term of the diagonal pairs, Cholesky-based: t tr(K^-1 Q_aa) = t tr(L^-1 Q_aa L^-T)
+    for (int a = 0; a < Ny; ++a) {
+        const int paa = a * (a + 1) / 2 + a;
+        const double* Li = h->dLi + (long long)a * slab(h);
+        em_pair_kernel<<<dim3(Tq, Tq, n), 256, 2 * Nx * 64 * 8, h->st>>>(h->N, Nx, Ny, dP, h->dAlpha, np,
+                                                                      h->dEmE, h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2, nullptr, 1, paa, h->dKinv, np, s);
+        CUDA_TRY(cudaGetLastError());
+        // rank-one backbone: |L^-1 e^E|^2 (same kernels as alpha's first half)
+        em_qvec_kernel<<<dim3((np + 255) / 256, 1, n), 256, 0, h->st>>>(h->dEmE + (long long)paa * np, h->N, np, h->dEmVec, s);
+        CUDA_TRY(cudaGetLastError());
+        trmv_lower_kernel<<<dim3((np + 7) / 8, 1, n), 256, 0, h->st>>>(Li, np, 0, h->dEmVec, s.vec, h->dEmVec + np, s.vec, np);
+        CUDA_TRY(cudaGetLastError());
+        sumsq_kernel<<<n, 256, 0, h->st>>>(h->dEmVec + np, s.vec, np, h->dEmVec + 2LL * np + a, s.vec);
+        CUDA_TRY(cudaGetLastError());
+        // L^-1 Q~ of every point: the same L^-1 (sA = 0), the feed of one slab so each point keeps its lone bits
+        GemmParams gp;
+        memset(&gp, 0, sizeof(gp));
+        gp.A = Li; gp.lda = np;
+        gp.B = h->dKinv; gp.ldb = np; gp.sB = s.q;    // Q symmetric: row-major (j,k) storage is the NT operand
+        gp.C = h->dU; gp.ldc = np; gp.sC = s.q;
+        gp.mt = np / 128; gp.nt = np / 128; gp.K = np; gp.alpha = 1.0; gp.beta = 0.0;
+        gp.kflags = GEMM_KI_LE; gp.lower = 1;
+        CUDA_TRY(gemm128(h, h->st, true, gp, n, 1));
+        em_trdot_kernel<<<dim3(ntr, n), 256, 0, h->st>>>(h->dU, Li, np, h->dEmTr + (long long)a * ntr, s);
+        CUDA_TRY(cudaGetLastError());
+    }
+    em_finalize_kernel<<<n, 1024, 0, h->st>>>(Nx, Ny, npairs, dP, h->dHyp, Nx + 2, h->dEmMeanPart, nblk, h->dEmPart, T * T,
+                                              h->dEmTr, ntr, h->dEmVec + 2LL * np, mean, var, cov, s);
+    CUDA_TRY(cudaGetLastError());
+    return GPMPC_OK;
 }
 
 // ------------------------------------------------------------------------------------
@@ -1619,8 +1730,12 @@ struct EmHessOutputs {
 // the records of one point (EmTables::nrec order) into rec_out, through R's partials and backbone rows
 template <int NXP, int D>
 static cudaError_t launch_em_records(gpmpc_handle_t h, const EmRecords& R, const double* dz, const double* dP, int npairs,
-                                     int nb, double* rec_out)
+                                     int nb, int slot, double* rec_out)
 {
+    const EmStrides s = em_strides(h);
+    const double *E = h->dEmE + slot * s.pair, *F = h->dEmF + slot * s.pair, *E2 = h->dEmE2 + slot * s.pair;
+    const double *F2 = h->dEmF2 + slot * s.pair, *W = h->dEmW + slot * s.w, *IJ = h->dEmIJ + slot * s.w;
+    const double* LQ = h->dEmLQ + slot * s.lq;
     const EmTables& tb = *R.tb;
     const int N = h->N, Nx = h->Nx, Ny = h->Ny, np = h->Npad, nf = tb.nf, RL = tb.nent;
     constexpr int NFP = em_nmono(NXP, D / 2);
@@ -1633,13 +1748,13 @@ static cudaError_t launch_em_records(gpmpc_handle_t h, const EmRecords& R, const
     cudaError_t e = smem_opt_in<em_pair_rec_kernel<NXP, D>>(smem_pair);
     if (e == cudaSuccess) e = smem_opt_in<em_owner_rec_kernel<NXP, D>>(smem_own);
     if (e != cudaSuccess) return e;
-    em_owner_rec_kernel<NXP, D><<<dim3(nb, Ny), 256, smem_own, h->st>>>(h->dXT, np, N, Nx, dz, h->dAlpha, h->dEmLQ, np, nullptr, 0, 0, 1,
+    em_owner_rec_kernel<NXP, D><<<dim3(nb, Ny), 256, smem_own, h->st>>>(h->dXT, np, N, Nx, dz, h->dAlpha, LQ, np, nullptr, 0, 0, 1,
                                                                          MONO, ENT, RL, part, srec);
-    em_pair_rec_kernel<NXP, D><<<dim3(nb, npairs, 2), 256, smem_pair, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE,
-                                                                               h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2,
+    em_pair_rec_kernel<NXP, D><<<dim3(nb, npairs, 2), 256, smem_pair, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, E,
+                                                                               F, W, IJ, np, LQ, E2, F2,
                                                                                nullptr, 0, r_cross, MONO, ENT, RL, part, nb);
-    em_pair_rec_kernel<NXP, D><<<dim3(nb, Ny, 1), 256, smem_pair, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, h->dEmE,
-                                                                           h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2,
+    em_pair_rec_kernel<NXP, D><<<dim3(nb, Ny, 1), 256, smem_pair, h->st>>>(N, Nx, Ny, dP, h->dAlpha, np, h->dXT, np, dz, E,
+                                                                           F, W, IJ, np, LQ, E2, F2,
                                                                            h->dEmKinv, 1, r_tr, MONO, ENT, RL, part, nb);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     // rank-one backbone e e^T of Q_aa: rows e o mono_f for the nf features through L^-1 in one batched trmv.
@@ -1652,10 +1767,10 @@ static cudaError_t launch_em_records(gpmpc_handle_t h, const EmRecords& R, const
     for (int a = 0; a < Ny; ++a) {
         const int paa = a * (a + 1) / 2 + a;
         const double* Li = h->dLi + (long long)a * slab(h);
-        em_backbone_rows_kernel<<<(np + 255) / 256, 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, h->dEmE + (long long)paa * np, np, MONO, nf, rows);
+        em_backbone_rows_kernel<<<(np + 255) / 256, 256, 0, h->st>>>(h->dXT, np, N, Nx, dz, E + (long long)paa * np, np, MONO, nf, rows);
         trmv_lower_kernel<<<dim3((np + 7) / 8, 1, nf), 256, 0, h->st>>>(Li, np, 0, rows, np, prod, np, np);
         trmv_lower_T_kernel<<<dim3(np / 32, 1, nkz), 256, 0, h->st>>>(Li, np, 0, prod, np, kz, np, np);
-        em_owner_rec_kernel<NXP, D><<<dim3(nb, 1), 256, smem_own, h->st>>>(h->dXT, np, N, Nx, dz, nullptr, h->dEmE + (long long)paa * np, 0,
+        em_owner_rec_kernel<NXP, D><<<dim3(nb, 1), 256, smem_own, h->st>>>(h->dXT, np, N, Nx, dz, nullptr, E + (long long)paa * np, 0,
                                                                             kz, 0, np, nkz, MONO, ENT, RL, part + (long long)(r_bb + a) * srec, 0);
         if (D == 2)
             em_owner_rec_kernel<NXP, D><<<dim3(nb, 1), 256, smem_own, h->st>>>(prod + np, np, N, Nx, nullptr, nullptr, nullptr, 0, nullptr, 0, 0, 1,
@@ -1873,19 +1988,12 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
     const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, np = h->Npad;
     NvtxRange nvtx_r("gpmpc.predict_em");
     if (!Sigma) { set_error(h, "EM needs an input covariance"); return GPMPC_ERR_ARG; }
-    const int npairs = Ny * (Ny + 1) / 2;
+    const int npairs = em_npairs(h);
     if (npairs > 1024) { set_error(h, "EM supports Ny <= 44"); return GPMPC_ERR_ARG; }
-    const size_t per = (size_t)Ny * (2 * nn + 2) + (size_t)npairs * (nn + 4);
-    const int nblk = (np + 255) / 256, T = (h->N + 63) / 64, Tq = np / 64, ntr = Tq * (Tq + 1) / 2;
-    ENSURE(h->dEmTr, (long long)Ny * ntr);
-    ENSURE(h->dEmLQ, (long long)Ny * np);
-    ENSURE(h->dEmVec, 2LL * np + Ny);
-    ENSURE(h->dEmE, (long long)npairs * np); ENSURE(h->dEmF, (long long)npairs * np);
-    ENSURE(h->dEmE2, (long long)npairs * np); ENSURE(h->dEmF2, (long long)npairs * np);
-    ENSURE(h->dEmW, (long long)npairs * Nx * np); ENSURE(h->dEmIJ, (long long)npairs * Nx * np);
-    ENSURE(h->dEmMeanPart, (long long)Ny * nblk); ENSURE(h->dEmPart, (long long)npairs * T * T);
-    { int rcs = ensure_nlml_scratch(h); if (rcs) return rcs; }      // dKinv <- Q_aa, dU <- L^-1 Q_aa (one slab each)
-    ENSURE(h->dEMP, (long long)H * per);
+    const size_t per = em_per(h);
+    const int T = (h->N + 63) / 64;
+    const int nc = em_chunk(h, H);
+    { const int rcs = em_scratch(h, nc, H); if (rcs) return rcs; }
     // the record set of degree D: tables built and uploaded once, scratch for H points
     auto records = [&](int D) -> int {
         EmRecords& R = h->em_rec[D / 2 - 1];
@@ -1935,49 +2043,25 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
     }
     CUDA_TRY(cudaMemcpyAsync(h->dEMP, emp.data(), emp.size() * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, (size_t)H * Nx * 8, cudaMemcpyHostToDevice, h->st));
-    for (int p = 0; p < H; ++p) {
-        const double* dz = h->dZ + (size_t)p * Nx;
-        const double* dP = h->dEMP + (size_t)p * per;
-        CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_prep<decltype(nxp)::value>(h, npairs, dz, dP, nblk); }));
-        em_pair_kernel<<<dim3(T, T, npairs), 256, 2 * Nx * 64 * 8, h->st>>>(h->N, Nx, Ny, dP, h->dAlpha, np,
-                                                                          h->dEmE, h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2, h->dEmPart, 0, 0, nullptr, 0);
-        CUDA_TRY(cudaGetLastError());
-        // E[var] term of the diagonal pairs, Cholesky-based: t tr(K^-1 Q_aa) = t tr(L^-1 Q_aa L^-T)
-        for (int a = 0; a < Ny; ++a) {
-            const int paa = a * (a + 1) / 2 + a;
-            em_pair_kernel<<<dim3(Tq, Tq, 1), 256, 2 * Nx * 64 * 8, h->st>>>(h->N, Nx, Ny, dP, h->dAlpha, np,
-                                                                          h->dEmE, h->dEmF, h->dEmW, h->dEmIJ, np, h->dEmLQ, h->dEmE2, h->dEmF2, nullptr, 1, paa, h->dKinv, np);
-            CUDA_TRY(cudaGetLastError());
-            // rank-one backbone: |L^-1 e^E|^2 (same kernels as alpha's first half)
-            em_qvec_kernel<<<(np + 255) / 256, 256, 0, h->st>>>(h->dEmE + (long long)paa * np, h->N, np, h->dEmVec);
-            CUDA_TRY(cudaGetLastError());
-            trmv_lower_kernel<<<dim3((np + 7) / 8, 1, 1), 256, 0, h->st>>>(h->dLi + (long long)a * slab(h), np, 0, h->dEmVec, 0, h->dEmVec + np, 0, np);
-            CUDA_TRY(cudaGetLastError());
-            sumsq_kernel<<<1, 256, 0, h->st>>>(h->dEmVec + np, np, h->dEmVec + 2LL * np + a);
-            CUDA_TRY(cudaGetLastError());
-            GemmParams gp;
-            memset(&gp, 0, sizeof(gp));
-            gp.A = h->dLi + (long long)a * slab(h); gp.lda = np;
-            gp.B = h->dKinv; gp.ldb = np;                 // Q symmetric: row-major (j,k) storage is the NT operand
-            gp.C = h->dU; gp.ldc = np;
-            gp.mt = np / 128; gp.nt = np / 128; gp.K = np; gp.alpha = 1.0; gp.beta = 0.0;
-            gp.kflags = GEMM_KI_LE; gp.lower = 1;
-            CUDA_TRY(gemm128(h, h->st, true, gp, 1, 1));
-            em_trdot_kernel<<<ntr, 256, 0, h->st>>>(h->dU, h->dLi + (long long)a * slab(h), np, h->dEmTr + (long long)a * ntr);
-            CUDA_TRY(cudaGetLastError());
-        }
-        em_finalize_kernel<<<1, 1024, 0, h->st>>>(Nx, Ny, npairs, dP, h->dHyp, Nx + 2, h->dEmMeanPart, nblk, h->dEmPart, T * T,
-                                                   h->dEmTr, ntr, h->dEmVec + 2LL * np,
-                                                   h->dMean + (size_t)p * Ny, h->dVar + (size_t)p * Ny, h->dCov + (size_t)p * Ny * Ny);
-        CUDA_TRY(cudaGetLastError());
-        if (go) {
-            double* rec = R2.rec + (size_t)p * R2.tb->nrec(Ny) * R2.tb->nent;
-            CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_records<decltype(nxp)::value, 2>(h, R2, dz, dP, npairs, T, rec); }));
-        }
-        if (ho) {
-            double* rec = R4.rec + (size_t)p * R4.tb->nrec(Ny) * R4.tb->nent;
-            CUDA_TRY((Nx <= 8 ? launch_em_records<8, 4>(h, R4, dz, dP, npairs, T, rec)
-                              : launch_em_records<16, 4>(h, R4, dz, dP, npairs, T, rec)));   // Nx <= 16
+    for (int c0 = 0; c0 < H; c0 += nc) {
+        const int n = std::min(nc, H - c0);
+        int rc = em_forward(h, n, h->dZ + (size_t)c0 * Nx, h->dEMP + (size_t)c0 * per, h->dMean + (size_t)c0 * Ny,
+                            h->dVar + (size_t)c0 * Ny, h->dCov + (size_t)c0 * Ny * Ny);
+        if (rc) return rc;
+        // the derivative records of each point of the chunk, from its scratch slot
+        for (int k = 0; k < n && (go || ho); ++k) {
+            const int p = c0 + k;
+            const double* dz = h->dZ + (size_t)p * Nx;
+            const double* dP = h->dEMP + (size_t)p * per;
+            if (go) {
+                double* rec = R2.rec + (size_t)p * R2.tb->nrec(Ny) * R2.tb->nent;
+                CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_records<decltype(nxp)::value, 2>(h, R2, dz, dP, npairs, T, k, rec); }));
+            }
+            if (ho) {
+                double* rec = R4.rec + (size_t)p * R4.tb->nrec(Ny) * R4.tb->nent;
+                CUDA_TRY((Nx <= 8 ? launch_em_records<8, 4>(h, R4, dz, dP, npairs, T, k, rec)
+                                  : launch_em_records<16, 4>(h, R4, dz, dP, npairs, T, k, rec)));   // Nx <= 16
+            }
         }
     }
     if (mean) CUDA_TRY(cudaMemcpyAsync(mean, h->dMean, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
@@ -2360,15 +2444,18 @@ static void rows_by_trajectory(double* dst, const double* src, int B, int Nt, si
             memcpy(dst + (b * Nt + t) * n, src + ((size_t)t * B + b) * n, n * 8);
 }
 
-// gpmpc_rollout_batch, gpmpc_rollout and with tg gpmpc_rollout_batch_grad; fn names the entry in errors
+// gpmpc_rollout_batch, gpmpc_rollout, with tg gpmpc_rollout_batch_grad and with em_entry gpmpc_rollout_batch_em (the one
+// entry that takes 'EM'); fn names the entry in errors
 static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, int Nt, const double* z0, const double* U,
                          const double* Sigma0, const double* scale, const double* K, const double* x_ref,
-                         const double* uscale, double* means, double* vars, double* cov_last, const RolloutTangents* tg = nullptr)
+                         const double* uscale, double* means, double* vars, double* cov_last, const RolloutTangents* tg = nullptr,
+                         bool em_entry = false)
 {
     int rc = predict_guard(h, fn, method, 1);
     if (rc) return rc;
     const int Nx = h->Nx, Ny = h->Ny, Nu = Nx - Ny;
-    if (method == GPMPC_METHOD_EM) { set_error(h, "%s: methods ME and TA (EM prepares every point on the host)", fn); return GPMPC_ERR_ARG; }
+    const bool em = method == GPMPC_METHOD_EM;
+    if (em && !em_entry) { set_error(h, "%s: methods ME and TA (EM: gpmpc_rollout_batch_em)", fn); return GPMPC_ERR_ARG; }
     rc = rollout_args(h, fn, B, Nt, !z0 || !Sigma0 || !means || !vars, U, K);
     if (rc) return rc;
     if (tg && (!tg->dmeans || !tg->dvars)) { set_error(h, "%s: null dmeans / dvars", fn); return GPMPC_ERR_ARG; }
@@ -2402,11 +2489,46 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
     RolloutPolicy pol;
     rollout_policy(B, Nt, Ny, Nu, U, scale, K, x_ref, uscale, o_u, pin, d, &pol);
     CUDA_TRY(cudaMemcpyAsync(d, pin, o_m * 8, cudaMemcpyHostToDevice, h->st));
+    // 'EM': chunks of em_chunk points, the em_prepare_point blocks of the B points staged on the host
+    const int nc = em ? em_chunk(h, B) : 0;
+    const size_t per = em ? em_per(h) : 0;
+    if (em) {
+        rc = em_scratch(h, nc, B);
+        if (rc) return rc;
+    }
+    std::vector<double> emp(Bs * per);
     const int fb_smem = K ? (Ny + Nu * Ny) * 8 : 0;
     for (int t = 0; t < Nt; ++t) {
+        double* mean_t = d + o_m + (size_t)t * Bs * Ny;
+        double* var_t = d + o_v + (size_t)t * Bs * Ny;
         double* cov_t = d + o_c + (size_t)t * Bs * Ny * Ny;
-        rc = predict_core(h, method, B, d, d + o_sig, 1, d + o_m + (size_t)t * Bs * Ny, d + o_v + (size_t)t * Bs * Ny, cov_t, nullptr);
-        if (rc) return rc;
+        if (!em) {
+            rc = predict_core(h, method, B, d, d + o_sig, 1, mean_t, var_t, cov_t, nullptr);
+            if (rc) return rc;
+        } else {
+            // the step's Sigma back to the host (step 0: Sigma0, already in the pinned mirror), its em_prepare_point blocks
+            // there (glibc's log and the host LU, the bits of gpmpc_predict(EM)), then the batched forward over the B points
+            if (t > 0) {
+                CUDA_TRY(cudaMemcpyAsync(pin + o_sig, d + o_sig, Bs * Nx * Nx * 8, cudaMemcpyDeviceToHost, h->st));
+                CUDA_TRY(cudaStreamSynchronize(h->st));
+            }
+            for (int b = 0; b < B; ++b) {
+                rc = em_prepare_point(h, pin + o_sig + (size_t)b * Nx * Nx, emp.data() + (size_t)b * per);
+                if (rc) {
+                    char why[512];
+                    snprintf(why, sizeof(why), "%s", h->err);
+                    set_error(h, "%s: step %d, trajectory %d: %s", fn, t, b, why);
+                    return rc;
+                }
+            }
+            CUDA_TRY(cudaMemcpyAsync(h->dEMP, emp.data(), emp.size() * 8, cudaMemcpyHostToDevice, h->st));
+            for (int b0 = 0; b0 < B; b0 += nc) {
+                const size_t o = (size_t)b0;
+                rc = em_forward(h, std::min(nc, B - b0), d + o * Nx, h->dEMP + o * per, mean_t + o * Ny, var_t + o * Ny,
+                                cov_t + o * Ny * Ny);
+                if (rc) return rc;
+            }
+        }
         if (tg) {                                 // J_t, dvar_t, dcov_t at the same points, then the step's tangents
             rc = derivs_enqueue(h, method, B, d, d + o_sig, 1, ds);
             if (rc) return rc;
@@ -2416,13 +2538,13 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
             CUDA_TRY(smem_opt_in<rollout_tangent_kernel>((NX_MAX * NX_MAX + NX_MAX + NX_MAX * NX_MAX / 2 + nw * (2 * NX_MAX + 2 * NX_MAX * NX_MAX)) * 8));
             double* g = h->dRollTg;
             rollout_tangent_kernel<<<B, nw * 32, tg_smem, h->st>>>(Ny, Nu, (int)P, t, t == 0, t + 1 == Nt, method == GPMPC_METHOD_TA,
-                                                                  h->dJ, ds.dvar, ds.dcov, d + o_m + (size_t)t * Bs * Ny, cov_t,
+                                                                  h->dJ, ds.dvar, ds.dcov, mean_t, cov_t,
                                                                   pol.scale, pol.K, pol.x_ref, pol.uscale, g, g + o_ds, g + o_dm + (size_t)t * Bs * Ny * P,
                                                                   g + o_dv + (size_t)t * Bs * Ny * P);
             CUDA_TRY(cudaGetLastError());
         }
         if (t + 1 < Nt) {
-            rollout_feedback_kernel<<<B, 256, fb_smem, h->st>>>(d + o_m + (size_t)t * Bs * Ny, cov_t, d + o_u + (size_t)(t + 1) * Nu,
+            rollout_feedback_kernel<<<B, 256, fb_smem, h->st>>>(mean_t, cov_t, d + o_u + (size_t)(t + 1) * Nu,
                                                                 (long long)Nt * Nu, pol.scale, pol.K, pol.x_ref, pol.uscale,
                                                                 Ny, Nu, d, d + o_sig);
             CUDA_TRY(cudaGetLastError());
@@ -2451,6 +2573,15 @@ extern "C" int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, 
                                    const double* uscale, double* means, double* vars, double* cov_last)
 {
     return rollout_batch(h, __func__, method, B, Nt, z0, U, Sigma0, scale, K, x_ref, uscale, means, vars, cov_last);
+}
+
+// gpmpc_rollout_batch with 'EM': the same slab, policy and feedback, the step's predict the batched EM forward
+extern "C" int gpmpc_rollout_batch_em(gpmpc_handle_t h, int B, int Nt, const double* z0, const double* U, const double* Sigma0,
+                                      const double* scale, const double* K, const double* x_ref, const double* uscale,
+                                      double* means, double* vars, double* cov_last)
+{
+    return rollout_batch(h, __func__, GPMPC_METHOD_EM, B, Nt, z0, U, Sigma0, scale, K, x_ref, uscale, means, vars, cov_last,
+                         nullptr, true);
 }
 
 // gpmpc_rollout_batch plus the forward-mode derivatives of every step's mean and variance (see include/gpmpc.h)

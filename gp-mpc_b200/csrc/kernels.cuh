@@ -921,7 +921,17 @@ gram_cov_kernel(const double* __restrict__ V, int ldv, long long sV, int n,
 //   per output a :  iR_a = (Sigma + Lambda_a)^-1 ,  c_a = sf2_a prod(ell_a) / sqrt(det(Sigma+Lambda_a))
 //   per pair a>=b:  Qm = (Sigma (iL_a+iL_b) + I)^-1 Sigma/2 ,  t_ab = det(...)^-1/2
 // EMP layout (doubles): [a: iR (Nx*Nx), c, G_a (Nx*Nx), lc_a] * Ny, then [pair: Qm (Nx*Nx), t, a, b, const_ab] * npairs
+// A launch set covers a chunk of points: every buffer below holds one slice per point at the strides of EmStrides, and the
+// point is blockIdx.z (em_pair_kernel's pair sums: blockIdx.z / npairs; em_trdot_kernel: blockIdx.y; em_finalize_kernel:
+// blockIdx.x).  A point's arithmetic does not depend on its slot, so its bits do not depend on the chunk.
 // ---------------------------------------------------------------------------------------
+struct EmStrides {
+    long long z, emp;           // test point (Nx), em_prepare_point block
+    long long mpart, pair, w;   // mean partials (Ny nblk); E, F, E2, F2 (npairs ldn each); W, IJ (npairs Nx ldn each)
+    long long lq, part, q;      // log q (Ny ldn); pair-sum partials (npairs T T); Q~ and L^-1 Q~ slabs (ld^2)
+    long long tr, vec;          // trace partials (Ny ntr); [qv (ldn) | L^-1 qv (ldn) | |L^-1 qv|^2 (Ny)]
+};
+
 template <int NXP>
 __global__ void __launch_bounds__(256)
 em_prep_kernel(const double* __restrict__ XT, int ldx, int N, int Nx, int Ny, int npairs,
@@ -929,11 +939,15 @@ em_prep_kernel(const double* __restrict__ XT, int ldx, int N, int Nx, int Ny, in
                const double* __restrict__ z, const double* __restrict__ EMP,
                double* __restrict__ meanPart, int nblk,
                double* __restrict__ E, double* __restrict__ F, double* __restrict__ W, double* __restrict__ IJ, int ldn,
-               double* __restrict__ LQ, double* __restrict__ E2, double* __restrict__ F2)
+               double* __restrict__ LQ, double* __restrict__ E2, double* __restrict__ F2, EmStrides s)
 {
     __shared__ double M[NXP * NXP], Ga[NXP * NXP], Gb[NXP * NXP];
     __shared__ double red[8];
     const int role = blockIdx.y, tid = threadIdx.x;
+    const long long pt = blockIdx.z;
+    z += pt * s.z; EMP += pt * s.emp; meanPart += pt * s.mpart;
+    E += pt * s.pair; F += pt * s.pair; E2 += pt * s.pair; F2 += pt * s.pair;
+    W += pt * s.w; IJ += pt * s.w; LQ += pt * s.lq;
     const int i = blockIdx.x * 256 + tid;
     const int nn = Nx * Nx;
     double v[NXP];
@@ -1085,12 +1099,18 @@ em_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
                const double* __restrict__ E, const double* __restrict__ F, const double* __restrict__ W,
                const double* __restrict__ IJ, int ldn, const double* __restrict__ LQ,
                const double* __restrict__ E2, const double* __restrict__ F2, double* __restrict__ part,
-               int mode, int pair_q, double* __restrict__ Qout, int ldq)
+               int mode, int pair_q, double* __restrict__ Qout, int ldq, EmStrides st)
 {
     extern __shared__ double sm[];
     double* Ws = sm; double* Js = sm + Nx * 64;
     __shared__ double red[8];
-    const int p = mode ? pair_q : blockIdx.z, nn = Nx * Nx;
+    const int npairs = Ny * (Ny + 1) / 2;
+    const long long pt = mode ? blockIdx.z : blockIdx.z / npairs;
+    const int p = mode ? pair_q : blockIdx.z - (int)pt * npairs, nn = Nx * Nx;
+    EMP += pt * st.emp; LQ += pt * st.lq;
+    E += pt * st.pair; F += pt * st.pair; E2 += pt * st.pair; F2 += pt * st.pair;
+    W += pt * st.w; IJ += pt * st.w;
+    if (mode) Qout += pt * st.q; else part += pt * st.part;
     const double* P = EMP + (long long)Ny * (2 * nn + 2) + (long long)p * (nn + 4);
     const int a = (int)P[nn + 1], b = (int)P[nn + 2];
     const double cab = P[nn + 3];       // log t + (log sf2_a - log c_a) + (log sf2_b - log c_b), from determinants of I + small
@@ -1129,18 +1149,20 @@ em_pair_kernel(int N, int Nx, int Ny, const double* __restrict__ EMP,
     }
 }
 
-// rank-one backbone of Q_aa: qv_i = exp(E_i) (i < N, else 0)
-__global__ void em_qvec_kernel(const double* __restrict__ E, int N, int n, double* __restrict__ qv)
+// rank-one backbone of Q_aa: qv_i = exp(E_i) (i < N, else 0); point blockIdx.z
+__global__ void em_qvec_kernel(const double* __restrict__ E, int N, int n, double* __restrict__ qv, EmStrides s)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    E += blockIdx.z * s.pair; qv += blockIdx.z * s.vec;
     if (i < n) qv[i] = (i < N) ? exp(E[i]) : 0.0;
 }
 
-// out[0] = sum_i v_i^2 (single block, fixed order)
+// out[0] = sum_i v_i^2 (one block per vector, fixed order): vector blockIdx.x at v + blockIdx.x sv, its sum at out + blockIdx.x so
 __global__ void __launch_bounds__(256)
-sumsq_kernel(const double* __restrict__ v, int n, double* __restrict__ out)
+sumsq_kernel(const double* __restrict__ v, long long sv, int n, double* __restrict__ out, long long so)
 {
     __shared__ double red[8];
+    v += blockIdx.x * sv; out += blockIdx.x * so;
     double s = 0.0;
     for (int i = threadIdx.x; i < n; i += 256) s = fma(v[i], v[i], s);
     s = warp_sum(s);
@@ -1154,12 +1176,13 @@ sumsq_kernel(const double* __restrict__ v, int n, double* __restrict__ out)
 }
 
 // tr(L^-1 Q L^-T) = sum_{k >= j} Wm[k][j] Li[k][j] with Wm = L^-1 Q (lower tiles): block partial sums,
-// grid (n/64 * (n/64+1)/2) lower 64x64 tiles
+// grid (n/64 * (n/64+1)/2) lower 64x64 tiles, point blockIdx.y (Wm and part at its slices; Li shared)
 __global__ void __launch_bounds__(256)
-em_trdot_kernel(const double* __restrict__ Wm, const double* __restrict__ Li, int ld, double* __restrict__ part)
+em_trdot_kernel(const double* __restrict__ Wm, const double* __restrict__ Li, int ld, double* __restrict__ part, EmStrides st)
 {
     __shared__ double red[8];
     const int tt = blockIdx.x;
+    Wm += blockIdx.y * st.q; part += blockIdx.y * st.tr;
     int bi = (int)((sqrt(8.0 * (double)tt + 1.0) - 1.0) * 0.5);
     while (bi * (bi + 1) / 2 > tt) --bi;
     while ((bi + 1) * (bi + 2) / 2 <= tt) ++bi;
@@ -1186,9 +1209,14 @@ __global__ void em_finalize_kernel(int Nx, int Ny, int npairs, const double* __r
                                    const double* __restrict__ meanPart, int nblk,
                                    const double* __restrict__ part, int ntile2,
                                    const double* __restrict__ trPart, int ntr, const double* __restrict__ trVec,
-                                   double* __restrict__ mean, double* __restrict__ var, double* __restrict__ cov)
+                                   double* __restrict__ mean, double* __restrict__ var, double* __restrict__ cov, EmStrides st)
 {
     const int tid = threadIdx.x, nn = Nx * Nx;
+    const long long pt = blockIdx.x;     // one CTA per point; mean / var / cov at strides Ny / Ny / Ny^2
+    EMP += pt * st.emp; meanPart += pt * st.mpart; part += pt * st.part; trPart += pt * st.tr; trVec += pt * st.vec;
+    if (mean) mean += pt * Ny;
+    if (var) var += pt * Ny;
+    if (cov) cov += pt * Ny * Ny;
     if (tid < Ny && mean) {
         double s = 0.0;
         for (int b = 0; b < nblk; ++b) s += meanPart[(long long)tid * nblk + b];

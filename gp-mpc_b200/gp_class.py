@@ -556,9 +556,10 @@ class GP:
 
         A batch x0:(B,Ny) with u:(B,Nt,Nu) gives mean, var of shape (len(methods), B, Nt+1, Ny);
         trajectory b is what x0[b], u[b] give alone (its own covariance chain and, with feedback,
-        its own gain).  'ME' / 'TA' on a single handle run on the device (gpmpc_rollout_batch: one
-        predict pass over all trajectories per step, one pass per distinct gain with feedback);
-        'EM', sharded models and prior_mean_in_predict keep the host loop."""
+        its own gain).  On a single handle every method runs on the device (gpmpc_rollout_batch for
+        'ME' / 'TA', gpmpc_rollout_batch_em for 'EM': one predict pass over all trajectories per
+        step, one pass per distinct gain with feedback); sharded models, prior_mean_in_predict and
+        device_rollout=False keep the host loop."""
         Ny = self.__Ny
         X0, U, single, Nt = self.__trajectories(x0, u)
         nb = X0.shape[0]
@@ -574,7 +575,7 @@ class GP:
         covar = self.__initial_covar(nb)
         covar_x0 = covar[:, :Ny, :Ny].copy()
         keep = self.__gp_method
-        # 'ME' / 'TA' on a single handle: all Nt steps run on the device, same arithmetic as the loop below
+        # a single handle: all Nt steps run on the device, same arithmetic as the loop below
         on_device = (device_rollout and self.__comm.world == 1
                      and not (self.__prior_mean_in_predict and self.__has_prior_mean()))
         for i, meth in enumerate(methods):
@@ -582,8 +583,7 @@ class GP:
             covar[:, :Ny, :Ny] = covar_x0
             mean[i, :, 0, :] = X0
             K = self.__lqr_gains(X0, U[:, 0], Q, R) if feedback else None      # once per method, as the reference
-            if on_device and meth in ('ME', 'TA') and Nt > 0 and self.__rollout_device(i, meth, X0, U, covar, K, x_ref,
-                                                                                      single, mean, var):
+            if on_device and Nt > 0 and self.__rollout_device(i, meth, X0, U, covar, K, x_ref, single, mean, var):
                 continue
             for b in range(nb):
                 mean_t = X0[b]
@@ -677,12 +677,16 @@ class GP:
     def __rollout_device(self, i, meth, X0, U, covar, K, x_ref, single, mean, var):
         """Method i of every trajectory on the device; False when the engine has no roll-out entry for the case."""
         eng = self.__engine
-        use_single = single and K is None and hasattr(eng, 'rollout')       # gpmpc_rollout, the one open-loop trajectory
-        if not (use_single or hasattr(eng, 'rollout_batch')):
+        em = meth == 'EM'
+        use_single = not em and single and K is None and hasattr(eng, 'rollout')   # gpmpc_rollout, the one open-loop trajectory
+        if not (use_single or hasattr(eng, 'rollout_batch_em' if em else 'rollout_batch')):
             return False
         z0, Ug, scale, uscale = self.__engine_start(X0, U, K, x_ref)
         method = _GPU_METHODS[meth]
-        if use_single:
+        if em:                                          # gpmpc_rollout_batch_em, a single trajectory as B = 1
+            parts = [(g,) + tuple(eng.rollout_batch_em(z0[g], Ug[g], covar[g], scale, Kg, x_ref, uscale))
+                     for g, Kg in self.__gain_groups(K, len(X0))]
+        elif use_single:
             parts = [(np.arange(1),) + tuple(r[None] for r in eng.rollout(z0[0], Ug[0], covar[0], method, scale))]
         else:
             parts = [(g,) + tuple(eng.rollout_batch(z0[g], Ug[g], covar[g], method, scale, Kg, x_ref, uscale))

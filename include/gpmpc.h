@@ -302,6 +302,22 @@ int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, const doubl
                         const double* Sigma0, const double* scale, const double* K, const double* x_ref,
                         const double* uscale, double* means, double* vars, double* cov_last);
 
+/* gpmpc_rollout_batch with exact moment matching ('EM'): same arguments (no method) and outputs, the same slab layout,
+ * policy and feedback update; only each step's predict differs.  Step t copies the B current Sigma to the host (one copy,
+ * one synchronisation), prepares each point's Nx x Nx quantities there as gpmpc_predict(EM) does, copies them back and
+ * runs the batched 'EM' forward over the B points (chunks of at most gpmpc_set_option("em_points") points, else a scratch
+ * budget).  The preparation stays on the host on purpose: it takes logarithms of determinants, and a device port (CUDA's
+ * log is not glibc's) would break bit-identity with gpmpc_predict(EM); the synchronisation costs microseconds against
+ * about a millisecond of EM device work per point at N = 1000.  Each trajectory's means, vars and cov_last are those of
+ * the host loop of gpmpc_predict(EM, H = 1) calls with the same inputs, bit for bit, whatever B and its row.
+ * GPMPC_ERR_ARG: every argument error of gpmpc_rollout_batch, checked before any work (Nx = Ny + Nu with Nu >= 0 keeps
+ * Ny <= Nx <= 32 inside gpmpc_predict(EM)'s Ny <= 44, so a model with more outputs fails there); Sigma + Lambda not
+ * positive definite at step t (gpmpc_last_error names t and the trajectory; the outputs are then undefined and the handle
+ * stays usable).  GPMPC_ERR_STATE: not factorised, or the handle does not own every output. */
+int gpmpc_rollout_batch_em(gpmpc_handle_t h, int B, int Nt, const double* z0, const double* U, const double* Sigma0,
+                           const double* scale, const double* K, const double* x_ref, const double* uscale,
+                           double* means, double* vars, double* cov_last);
+
 /* gpmpc_rollout_batch plus the exact derivatives of every step's mean and variance w.r.t. what produced the trajectory,
  * by forward-mode tangents carried on the device beside the roll-out (one derivative chain of gpmpc_predict_grad per step
  * on the same points, then one tangent kernel).  Same arguments; means, vars, cov_last are bit-identical to
@@ -365,7 +381,9 @@ int gpmpc_get(gpmpc_handle_t h, int what, int a, double* dst);
  * 0 = two CTAs per SM), "peer" (0/1), "peer_timeout_s" (consumer wait for a peer's flag),
  * "small_tiles" (batched 128x64 tile count of a factorisation GEMM below which it runs on
  * 64x32 tiles; default 4 per SM), "nlml_batch_max" (entries per gpmpc_nlml_batch pass, a cap
- * on its scratch; 0 = all, the default).  Any other name returns GPMPC_ERR_ARG. */
+ * on its scratch; 0 = all, the default), "em_points" (points per batched 'EM' forward, a cap
+ * on its scratch of two Npad^2 slabs per point; 0 = a 1 GiB budget decides, the default; the
+ * results do not depend on it).  Any other name returns GPMPC_ERR_ARG. */
 int gpmpc_set_option(gpmpc_handle_t h, const char* name, double value);
 
 /* Multi-GPU: one process per GPU.  Rank 0 calls gpmpc_comm_unique_id and ships the
