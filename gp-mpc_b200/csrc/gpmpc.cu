@@ -1306,18 +1306,31 @@ static int psk_grid(gpmpc_handle_t h, long long G)
     return (int)std::min<long long>(ctas, h->opt_predict_ctas > 0 ? G : by_work);
 }
 
+// The schedule of the predict product p of the slab B; returns its grid.  A lower-mode product of L^-1 streams it from the
+// panel, on the paired schedule when its tile pairs fill the grid (psk_pair_units: the same choice for every such product
+// at one (nloc, ntb) and grid), on psk_pair_grid's CTAs unless predict_ctas sets the grid.
+static int psk_schedule(gpmpc_handle_t h, PredictParams& p, const double* B)
+{
+    int grid = psk_grid(h, p.G);
+    if (B == h->dLi.p && !p.upper) {
+        p.Lp = h->dLiP;
+        p.upo = psk_pair_units(p.nloc, p.ntb, grid);
+        if (p.upo && h->opt_predict_ctas == 0) grid = psk_pair_grid((long long)p.nloc * p.upo, grid);
+    }
+    return grid;
+}
+
 // the predict product p (psk_base) of A (h-major rows, HB * Npad per output) and the slab B of each output: BM = round8(p.Hc).
-// A lower-mode product of L^-1 streams it from the panel, which panel_refresh must have brought up to date.
+// A product of L^-1 reads its panel, which panel_refresh must have brought up to date.
 static cudaError_t psk_launch(gpmpc_handle_t h, const PredictParams& p0, const double* A, const double* B)
 {
     const long long sA = (long long)HB * h->Npad, sB = slab(h);
-    const int np = h->Npad, grid = psk_grid(h, p0.G);
+    const int np = h->Npad;
     PredictParams p = p0;
-    if (B == h->dLi.p && !p.upper) {
+    const int grid = psk_schedule(h, p, B);
+    if (p.Lp)
         for (int a = 0; a < h->nloc; ++a)
             if (h->panel_row[a] < np) return cudaErrorIllegalState;
-        p.Lp = h->dLiP;
-    }
     switch (round8(p.Hc)) {
     case 8: return psk_launch_bm<8>(p, A, sA, B, sB, np, grid, h->st);
     case 16: return psk_launch_bm<16>(p, A, sA, B, sB, np, grid, h->st);
@@ -3309,7 +3322,7 @@ static int profile_product(gpmpc_handle_t h, const char* fn, int H, const double
     if (rc) return rc;
     PredictParams p;
     psk_base(h, p, H);
-    *grid = psk_grid(h, p.G);
+    *grid = psk_schedule(h, p, h->dLi);
     DevBuf<unsigned long long> dbg;
     ENSURE(dbg, (long long)*grid * 2 + n_tail);
     p.dbg = dbg;

@@ -12,6 +12,9 @@
 // by a range border is completed by its LAST-ARRIVING contributor: everyone else parks its partial
 // accumulators in a per-CTA slot and bumps the tile's counter; the last one adds the parked
 // partials in contributor order (fixed order => bit-reproducible), squares and row-reduces.
+// A lower-mode product of L^-1 from its panel whose tile pairs fill the grid runs the paired schedule instead
+// (psk_pair_units): whole tiles, paired long with short so every unit has the same length, dealt to the CTAs round-robin
+// so the CTAs of one output walk its ks^T in step; no tile is cut.
 // The same "last arriver" idea chains the rest of the step: the CTA that finishes an output's last
 // tile builds that output's [mean,var,J] records (and stores them to the peers), the CTA that
 // finishes the last output publishes the peer flags and assembles the covariances.
@@ -68,6 +71,7 @@ struct PredictParams {
     int upper;                        // 0: B lower triangular (k <= j, v = Linv ks); 1: B upper (k >= j, beta = Linv^T v)
     const double* Lp;                 // lower mode, B = L^-1: its panel copy (panel_pack_kernel), one bulk copy per stage; else null
     long long T, G;                   // k-steps per output (psk_steps_per_output), total = nloc * T
+    int upo;                          // paired schedule: units (tile pairs) per output (psk_pair_units); 0: stream-K
     double* part;                     // [grid][2][BM*PSK_BN] parked partial accumulators (fragment-major)
     unsigned int* tile_cnt;           // [nloc*ntb]
     unsigned int* out_cnt;            // [nloc]
@@ -334,10 +338,63 @@ __host__ __device__ inline int psk_ksteps(int ntb, int nk, int upper, int jt)
 }
 __device__ __forceinline__ int psk_ksteps(const PredictParams& p, int jt) { return psk_ksteps(p.ntb, p.nk, p.upper, jt); }
 
+// The paired schedule (lower mode).  Unit p of an output is tiles ntb-1-p (long, first) and p (short), so every unit has
+// SB (ntb + 1) k-steps -- the middle tile of an odd ntb is a unit alone, and the pair with the half tile of an odd Npad / 128
+// is 8 steps shorter.  Unit u = a upo + p goes to CTA u mod C: the CTAs of one output start its long tiles at k = 0 together
+// and advance at the same rate, so one fetch of a ks^T box serves all of them and only the few outputs in flight keep ks^T
+// in L2.  Each tile is one accumulation chain from k = 0 inside one CTA, so the bits do not depend on C.
+// psk_pair_units: units per output when this schedule applies, else 0.  It applies when every CTA of the grid owns at least
+// one unit and the rounds of units fill at least 7/8 of the grid's unit slots: a CTA's time is its unit count, so 136
+// units on 132 CTAs would take two rounds for the work of one and stay on stream-K (C5 on 132 SMs: 256 units, 0.97).
+__host__ __device__ inline int psk_pair_units(int nloc, int ntb, int grid)
+{
+    const long long upo = (ntb + 1) / 2, units = nloc * upo, rounds = (units + grid - 1) / grid;
+    return (units >= grid && 8 * units >= 7 * rounds * grid) ? (int)upo : 0;
+}
+// the automatic grid of the paired schedule: the fewest CTAs that need no more rounds of units than `grid` CTAs would, so
+// the CTAs' unit counts are equal or one apart and no SM starts a unit it cannot finish with the others (C5 on 132 SMs:
+// 128 CTAs of 2 units each, measured faster than 132 of 2 or 1)
+__host__ __device__ inline int psk_pair_grid(long long units, int grid)
+{
+    const long long rounds = (units + grid - 1) / grid;
+    return (int)((units + rounds - 1) / rounds);
+}
+__host__ __device__ inline int psk_unit_steps(int ntb, int nk, int pu)
+{
+    const int jl = ntb - 1 - pu;
+    return psk_ksteps(ntb, nk, 0, jl) + (pu != jl ? psk_ksteps(ntb, nk, 0, pu) : 0);
+}
+// k-steps of CTA c of C
+__host__ __device__ inline long long psk_pair_cta_steps(int nloc, int ntb, int nk, int upo, long long c, long long C)
+{
+    long long n = 0;
+    for (long long u = c; u < (long long)nloc * upo; u += C) n += psk_unit_steps(ntb, nk, (int)(u % upo));
+    return n;
+}
+// the long tile of unit u, where CTA u starts
+__host__ __device__ inline void psk_pair_first(int ntb, int upo, long long u, int& a, int& jt)
+{
+    a = (int)(u / upo);
+    jt = ntb - 1 - (int)(u - (long long)a * upo);
+}
+// the tile after tile (a, jt) in a CTA's sequence: the short tile of the same unit, or the long tile of unit u + C
+__host__ __device__ inline void psk_pair_next(int ntb, int upo, long long C, int& a, int& jt)
+{
+    if (2 * jt > ntb - 1) jt = ntb - 1 - jt;
+    else psk_pair_first(ntb, upo, (long long)a * upo + jt + C, a, jt);
+}
+
 struct PskIter { int a, jt, s, ks; };
 
-__device__ __forceinline__ void psk_iter_init(PskIter& it, long long g, const PredictParams& p)
+// the first step of CTA c of C: unit c (paired), or position G c / C of the list (stream-K)
+__device__ __forceinline__ void psk_iter_init(PskIter& it, const PredictParams& p, long long c, long long C)
 {
+    if (p.upo) {
+        psk_pair_first(p.ntb, p.upo, c, it.a, it.jt);
+        it.s = 0; it.ks = psk_ksteps(p, it.jt);
+        return;
+    }
+    const long long g = p.G * c / C;
     it.a = (int)(g / p.T);
     const long long r = g - (long long)it.a * p.T;            // (SB/2) jt (jt+1) <= r, about
     int jt = (int)((sqrt(8.0 * (double)r / PSK_SB + 1.0) - 1.0) * 0.5);
@@ -350,7 +407,8 @@ __device__ __forceinline__ void psk_iter_next(PskIter& it, const PredictParams& 
 {
     if (++it.s == it.ks) {
         it.s = 0;
-        if (++it.jt == p.ntb) { it.jt = 0; ++it.a; }
+        if (p.upo) psk_pair_next(p.ntb, p.upo, gridDim.x, it.a, it.jt);
+        else if (++it.jt == p.ntb) { it.jt = 0; ++it.a; }
         it.ks = psk_ksteps(p, it.jt);
     }
 }
@@ -358,8 +416,8 @@ __device__ __forceinline__ void psk_iter_next(PskIter& it, const PredictParams& 
 // The L^-1 panel (dLiP): each output's lower-mode k-step list, block after block in the order the product consumes it.
 // Block g = a T + psk_kstart(jt) + s (PSK_BN x 16 doubles) holds rows jt BN .. jt BN + BN-1 and columns 16 s .. 16 s + 15
 // of output a's L^-1 exactly as the tensor map lands them in a stage: 128-byte rows, the 16-byte chunk c of row r at
-// chunk c ^ (r & 7), rows past Npad (the half tile) zero.  A CTA's range [g0, g0 + nsteps) of the list is then one
-// contiguous stretch of memory.  The far-side 128 x 128 block the upper-half warps skip is copied as L^-1 holds it.
+// chunk c ^ (r & 7), rows past Npad (the half tile) zero.  Each tile, and a stream-K CTA's whole range of the list, is then
+// one contiguous stretch of memory.  The far-side 128 x 128 block the upper-half warps skip is copied as L^-1 holds it.
 // psk_panel_chunk: offset (doubles) in one output's panel of chunk c (columns 16 s + 2c, +1) of row r of tile jt, step s.
 __host__ __device__ inline long long psk_panel_chunk(int ntb, int nk, int jt, int s, int r, int c)
 {
@@ -543,8 +601,8 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
     const long long C = gridDim.x, c = blockIdx.x;
-    const long long g0 = p.G * c / C;
-    const int nsteps = (int)(p.G * (c + 1) / C - g0);           // this CTA's share of the k-step list
+    const int nsteps = p.upo ? (int)psk_pair_cta_steps(p.nloc, p.ntb, p.nk, p.upo, c, C)    // this CTA's share of the
+                             : (int)(p.G * (c + 1) / C - p.G * c / C);                      // k-step list
     if (nsteps <= 0) return;
     if (p.dbg && threadIdx.x == 0) { unsigned long long t0; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0)); p.dbg[2 * blockIdx.x] = t0; }
 
@@ -552,7 +610,6 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
     __shared__ PskIter s_pit;
     __shared__ int s_pg;
     __shared__ uint64_t s_pol[2];
-    __shared__ const double* s_lp;     // this CTA's stretch of the L^-1 panel (null: B through tmB)
     if (tid == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, CW); }
@@ -573,8 +630,9 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
         // ks^T (A) is re-read by every column tile: keep it in L2; L^-1 (B) is streamed exactly once.  Also when ks^T is
         // larger than the L2 (8 outputs at N=16384 on H100: 59 MB vs 50 MB) evict_last measured no slower than evict_normal
         tma_tile_g2s_3d_hint(As + s * A_STAGE, &tmA, k0, 0, it.a, full + s, s_pol[1]);
-        // the panel holds step g0 + pg as the tensor map would land it: one contiguous 32 KB copy instead of 256 rows
-        if (s_lp) bulk_g2s_hint(Bs + s * B_STAGE, s_lp + (long long)pg * B_STAGE, B_STAGE * 8, full + s, s_pol[0]);
+        // the panel holds the step as the tensor map would land it: one contiguous 32 KB copy instead of 256 rows
+        if (p.Lp) bulk_g2s_hint(Bs + s * B_STAGE, p.Lp + ((long long)it.a * p.T + psk_kstart(p, it.jt) + it.s) * B_STAGE,
+                                B_STAGE * 8, full + s, s_pol[0]);
         else tma_tile_g2s_3d_hint(Bs + s * B_STAGE, &tmB, k0, jta * BN, it.a, full + s, s_pol[0]);
         psk_iter_next(it, p);
         s_pit = it;
@@ -587,9 +645,8 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
     asm volatile("griddepcontrol.wait;" ::: "memory");
     if (tid == 0) {
         PskIter it;
-        psk_iter_init(it, g0, p);
+        psk_iter_init(it, p, c, C);
         s_pit = it; s_pg = 0;
-        s_lp = p.Lp ? p.Lp + g0 * B_STAGE : nullptr;
         s_pol[0] = l2_policy_evict_first(); s_pol[1] = l2_policy_evict_last();
 #pragma unroll
         for (int s = 0; s < AHEAD; ++s)
@@ -607,7 +664,7 @@ predict_streamk_kernel(const PredictParams p, const __grid_constant__ CUtensorMa
     }
 
     PskIter cit;
-    psk_iter_init(cit, g0, p);
+    psk_iter_init(cit, p, c, C);
     int cj[4];                                                      // slot j: k = 2j + (t & 1) + 8 (t >> 1)
 #pragma unroll
     for (int j = 0; j < 4; ++j) cj[j] = (((j + 4 * (t >> 1)) ^ g) << 1) + (t & 1);
