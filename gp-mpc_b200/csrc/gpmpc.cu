@@ -183,7 +183,7 @@ struct gpmpc_handle_s {
     DevBuf<double> dIn, dOut;         // [Z | Sigma] and [mean | var | J | cov] slabs: one H2D + one D2H per host call
     int Hcap = 0;                     // test points the slab layout behind dZ .. dCov holds (0: not laid out)
     double* hPinned = nullptr; double* dPinnedAlias = nullptr; size_t hPinnedBytes = 0;
-    // nlml scratch
+    // K^-1 and gradient scratch (ensure_kinv_scratch; dGrad: the gradient of one output)
     DevBuf<double> dU, dKinv, dGradPart, dGrad;
     DevBuf<double> dLoo;              // gpmpc_loo / gpmpc_loo_nlpp: [mean | var | nlpp | c partials | sw | u | b | tmp | 0]
     // gpmpc_nlml_batch: per entry of a pass its own L, Li slabs and recursion workspaces (nlml_batch_scratch)
@@ -469,59 +469,84 @@ static int launch_kbuild(gpmpc_handle_t h, const double* dHyp, const double* dJi
     return GPMPC_OK;
 }
 
-// alpha = Li^T (Li y), log det K and y . alpha for `batch` factor slabs: L, Li at stride slab, targets y at stride sy,
-// tmp and alpha at stride Npad, row-chunk partials P at stride w2slab, res (2 per entry)
-static int launch_alpha_at(gpmpc_handle_t h, const double* L, const double* Li, const double* y, long long sy, double* tmp,
-                           double* P, double* alpha, double* res, int batch)
+// c factor entries, entry s at: the hyper row hyp + s (Nx+2), the jitter jit[s] and the pivot info info[s] of its K build
+// and recursion; its L and L^-1 slabs L, Li + s slab and recursion workspaces W1, W2 + s w2slab (W1 also takes the alpha
+// partials); its target y + s sy; tmp, alpha + s Npad and res + 2 s (log det, y . alpha)
+struct FactorSet {
+    int c;
+    double *hyp, *jit; int* info;
+    double *L, *Li, *W1, *W2;
+    const double* y; long long sy;
+    double *tmp, *alpha, *res;
+};
+
+// the owned outputs al .. al + c - 1 in the model's own slots
+static FactorSet model_entries(gpmpc_handle_t h, int al, int c)
+{
+    const long long np = h->Npad;
+    return {c, h->dHyp + al * (h->Nx + 2LL), h->dJit + al, h->dInfo + al, h->dL + al * slab(h), h->dLi + al * slab(h),
+            h->dW1 + al * w2slab(h), h->dW2 + al * w2slab(h), h->dY + al * np, np, h->dTmp + al * np,
+            h->dAlpha + al * np, h->dRes + 2LL * al};
+}
+
+// alpha = Li^T (Li y), log det K and y . alpha of the entries, from their factor slabs
+static int alpha_pass(gpmpc_handle_t h, const FactorSet& e)
 {
     const int n = h->Npad;
-    dim3 g1((n + 7) / 8, 1, batch);
-    trmv_lower_kernel<<<g1, 256, 0, h->st>>>(Li, n, slab(h), y, sy, tmp, n, n);
+    dim3 g1((n + 7) / 8, 1, e.c);
+    trmv_lower_kernel<<<g1, 256, 0, h->st>>>(e.Li, n, slab(h), e.y, e.sy, e.tmp, n, n);
     CUDA_TRY(cudaGetLastError());
     // alpha = Li^T tmp in row chunks (partials in a W1 workspace, free outside the recursion), then
     // one pass that sums the partials, takes log det and y . alpha
     const int nch = (n + TRT_ROWS - 1) / TRT_ROWS;
-    dim3 g2(n / 32, nch, batch);
-    trmv_lower_T_part_kernel<<<g2, 256, 0, h->st>>>(Li, n, slab(h), tmp, n, P, w2slab(h), n);
+    dim3 g2(n / 32, nch, e.c);
+    trmv_lower_T_part_kernel<<<g2, 256, 0, h->st>>>(e.Li, n, slab(h), e.tmp, n, e.W1, w2slab(h), n);
     CUDA_TRY(cudaGetLastError());
-    alpha_logdet_kernel<<<batch, 1024, 0, h->st>>>(P, w2slab(h), nch, L, n, slab(h), y, sy, alpha, n, n, res);
+    alpha_logdet_kernel<<<e.c, 1024, 0, h->st>>>(e.W1, w2slab(h), nch, e.L, n, slab(h), e.y, e.sy, e.alpha, n, n, e.res);
     CUDA_TRY(cudaGetLastError());
     return GPMPC_OK;
 }
 
-// alpha, log det and y . alpha of `batch` consecutive local outputs starting at local index a, from their factor slabs
-static int launch_alpha(gpmpc_handle_t h, int a, int batch)
+// K(theta) -> L, Li of the entries with the reference's single jitter retry (optimize.py:483-488): one K build at zero
+// jitter and one recursion for all c (GEMM feeds chosen as for sel_batch slabs), then each entry whose pivot failed alone:
+// first at zero jitter when sel_batch > 1 (a lone slab's feeds round differently from the batch's), then with `jitter`.
+// used[s] (host): 0 ok, 1 ok with the jitter, > 1: 1 + the failing pivot.
+static int factor_entries(gpmpc_handle_t h, const FactorSet& e, int sel_batch, double jitter, int* used)
 {
-    const long long n = h->Npad;
-    return launch_alpha_at(h, h->dL + a * slab(h), h->dLi + a * slab(h), h->dY + a * n, n, h->dTmp + a * n,
-                           h->dW1 + a * w2slab(h), h->dAlpha + a * n, h->dRes + 2 * a, batch);
-}
-
-// K(theta) -> L, Li for local output a with the reference's single jitter retry.
-// used: 0 ok, 1 jitter used, >1: 1 + failing pivot.  dHyp = device hyper row of that output.
-static int factor_one(gpmpc_handle_t h, int a, const double* dHyp, double jitter, int* used)
-{
-    double* L = h->dL + (long long)a * slab(h);
-    double* Li = h->dLi + (long long)a * slab(h);
-    *used = 0;
-    panel_stale(h, a, 0);
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        const double jit = attempt ? jitter : 0.0;
-        CUDA_TRY(cudaMemcpyAsync(h->dJit + a, &jit, sizeof(double), cudaMemcpyHostToDevice, h->st));
-        CUDA_TRY(cudaMemsetAsync(h->dInfo + a, 0, sizeof(int), h->st));
-        {   // kbuild indexes hyper/jitter by blockIdx.z (== 0 here): pass row pointers
-            int rck = launch_kbuild(h, dHyp, h->dJit + a, L, 1, 0);
-            if (rck) return rck;
+    const int c = e.c, np = h->Npad;
+    CUDA_TRY(cudaMemsetAsync(e.jit, 0, (size_t)c * sizeof(double), h->st));
+    CUDA_TRY(cudaMemsetAsync(e.info, 0, (size_t)c * sizeof(int), h->st));
+    int rc = launch_kbuild(h, e.hyp, e.jit, e.L, c, 0);
+    if (rc) return rc;
+    rc = potrf_inv_rec(h, e.L, e.Li, slab(h), slab(h), e.info, 0, np, c, sel_batch, e.W1, e.W2);
+    if (rc) return rc;
+    std::vector<int> info(c);
+    CUDA_TRY(cudaMemcpyAsync(info.data(), e.info, (size_t)c * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
+    bool jittered = false;
+    for (int s = 0; s < c; ++s) {
+        used[s] = 0;
+        for (int attempt = sel_batch > 1 ? 0 : 1; info[s] && attempt < 2; ++attempt) {
+            const double jit = attempt ? jitter : 0.0;
+            double* L = e.L + s * slab(h);
+            CUDA_TRY(cudaMemcpyAsync(e.jit + s, &jit, sizeof(double), cudaMemcpyHostToDevice, h->st));
+            CUDA_TRY(cudaMemsetAsync(e.info + s, 0, sizeof(int), h->st));
+            rc = launch_kbuild(h, e.hyp + s * (h->Nx + 2LL), e.jit + s, L, 1, 0);
+            if (rc) return rc;
+            rc = potrf_inv_rec(h, L, e.Li + s * slab(h), slab(h), slab(h), e.info + s, 0, np, 1, 1, e.W1 + s * w2slab(h),
+                               e.W2 + s * w2slab(h));
+            if (rc) return rc;
+            if (attempt) { used[s] = 1; jittered = true; break; }
+            CUDA_TRY(cudaMemcpyAsync(&info[s], e.info + s, sizeof(int), cudaMemcpyDeviceToHost, h->st));
+            CUDA_TRY(cudaStreamSynchronize(h->st));
         }
-        int rc = potrf_inv_rec(h, L, Li, slab(h), slab(h), h->dInfo + a, 0, h->Npad, 1, 1, h->dW1, h->dW2);
-        if (rc) return rc;
-        int info = 0;
-        CUDA_TRY(cudaMemcpyAsync(&info, h->dInfo + a, sizeof(int), cudaMemcpyDeviceToHost, h->st));
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-        if (info == 0) { *used = attempt; return GPMPC_OK; }
-        *used = 1 + info;
     }
-    return GPMPC_ERR_NOTPD;
+    if (jittered) {         // the jittered recursions of every entry, read back together
+        CUDA_TRY(cudaMemcpyAsync(info.data(), e.info, (size_t)c * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+        CUDA_TRY(cudaStreamSynchronize(h->st));
+        for (int s = 0; s < c; ++s) if (used[s]) used[s] += info[s];
+    }
+    return GPMPC_OK;
 }
 
 // ------------------------------------------------------------------------------------
@@ -691,7 +716,7 @@ static int refresh_alpha(gpmpc_handle_t h)
 {
     const int nl = h->nloc;
     factor_caches_stale(h);
-    int rc = launch_alpha(h, 0, nl);
+    int rc = alpha_pass(h, model_entries(h, 0, nl));
     if (rc) return rc;
     std::vector<double> res(2 * nl);
     CUDA_TRY(cudaMemcpyAsync(res.data(), h->dRes, 2 * nl * 8, cudaMemcpyDeviceToHost, h->st));
@@ -758,19 +783,23 @@ static int local_index(gpmpc_handle_t h, int a)
     return a - h->a0;
 }
 
-static int ensure_nlml_scratch(gpmpc_handle_t h)
+// T(T+1)/2 tiles of the gradient's trace pass
+static inline int grad_tiles(gpmpc_handle_t h) { const int T = h->Npad / KB_TILE; return T * (T + 1) / 2; }
+
+// dU, dKinv: the work slabs of compute_kinv, the host extracts, gpmpc_loo_nlpp's gradient, gpmpc_remove and EM;
+// dGradPart: the trace pass's tile partials of the gradients of one output
+static int ensure_kinv_scratch(gpmpc_handle_t h)
 {
-    const int T = h->Npad / KB_TILE;
     ENSURE(h->dU, slab(h));
     ENSURE(h->dKinv, slab(h));
-    ENSURE(h->dGradPart, (long long)T * (T + 1) / 2 * (h->Nx + 2));
+    ENSURE(h->dGradPart, (long long)grad_tiles(h) * (h->Nx + 2));
     return GPMPC_OK;
 }
 
 static int extract_to_host(gpmpc_handle_t h, const double* src, double* dst, int mode)
 {
     const int N = h->N;
-    { int rc = ensure_nlml_scratch(h); if (rc) return rc; }
+    { int rc = ensure_kinv_scratch(h); if (rc) return rc; }
     // stage through dU (N*N fits: Npad >= N)
     dim3 g((N + 127) / 128, N);
     extract_kernel<<<g, 128, 0, h->st>>>(src, h->Npad, h->dU, N, mode);
@@ -786,7 +815,7 @@ extern "C" int gpmpc_build_K(gpmpc_handle_t h, int a, double* K_out)
     if (rc) return rc;
     const int al = local_index(h, a);
     if (al < 0) return GPMPC_ERR_ARG;
-    rc = ensure_nlml_scratch(h);
+    rc = ensure_kinv_scratch(h);
     if (rc) return rc;
     const double zero = 0.0;
     CUDA_TRY(cudaMemcpyAsync(h->dJit + al, &zero, 8, cudaMemcpyHostToDevice, h->st));
@@ -803,27 +832,14 @@ extern "C" int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info)
     if (rc) return rc;
     NvtxRange nvtx_r("gpmpc.factorize");
     const int nl = h->nloc;
-    CUDA_TRY(cudaMemsetAsync(h->dJit, 0, nl * sizeof(double), h->st));
-    CUDA_TRY(cudaMemsetAsync(h->dInfo, 0, nl * sizeof(int), h->st));
-    rc = launch_kbuild(h, h->dHyp, h->dJit, h->dL, nl, 0);
-    if (rc) return rc;
     panel_stale(h, -1, 0);
-    rc = potrf_inv_rec(h, h->dL, h->dLi, slab(h), slab(h), h->dInfo, 0, h->Npad, nl, nl, h->dW1, h->dW2);
+    rc = factor_entries(h, model_entries(h, 0, nl), nl, jitter, h->jitter_used.data());
     if (rc) return rc;
-    std::vector<int> inf(nl, 0);
-    CUDA_TRY(cudaMemcpyAsync(inf.data(), h->dInfo, nl * sizeof(int), cudaMemcpyDeviceToHost, h->st));
-    CUDA_TRY(cudaStreamSynchronize(h->st));
     int worst = GPMPC_OK;
     for (int a = 0; a < nl; ++a) {
-        h->jitter_used[a] = 0;
-        if (inf[a] != 0) {      // optimize.py:483-488: add jitter once, retry, else propagate
-            int used = 0;
-            rc = factor_one(h, a, h->dHyp + (long long)a * (h->Nx + 2), jitter, &used);
-            h->jitter_used[a] = used;
-            if (rc == GPMPC_ERR_NOTPD) { worst = rc; set_error(h, "output %d: K not positive definite even with jitter %g (pivot %d)", h->a0 + a, jitter, used - 1); }
-            else if (rc) return rc;
-        }
-        if (info) info[a] = h->jitter_used[a];
+        const int used = h->jitter_used[a];
+        if (used > 1) { worst = GPMPC_ERR_NOTPD; set_error(h, "output %d: K not positive definite even with jitter %g (pivot %d)", h->a0 + a, jitter, used - 1); }
+        if (info) info[a] = used;
     }
     if (worst) return worst;
     // dJit now holds each output's jitter (0 or the retry's); the appends extend K + that jitter, and dJit itself is
@@ -855,13 +871,10 @@ static int kinv_at(gpmpc_handle_t h, const double* Li, double* U, double* Kinv, 
 // K^-1 (lower) of local output al into dKinv
 static int compute_kinv(gpmpc_handle_t h, int al)
 {
-    int rc = ensure_nlml_scratch(h);
+    int rc = ensure_kinv_scratch(h);
     if (rc) return rc;
     return kinv_at(h, h->dLi + (long long)al * slab(h), h->dU, h->dKinv, 1);
 }
-
-// T(T+1)/2 tiles of the gradient's trace pass
-static inline int grad_tiles(gpmpc_handle_t h) { const int T = h->Npad / KB_TILE; return T * (T + 1) / 2; }
 
 // 1/2 tr((W - alpha alpha^T) dK/dtheta) for every hyper-parameter of `batch` entries: hyper rows at dHyp (stride Nx+2),
 // W = the lower triangle of the Kinv slabs (stride slab), alpha at stride Npad, tile partials in part (grad_tiles rows of
@@ -881,132 +894,102 @@ static int launch_grad_at(gpmpc_handle_t h, const double* dHyp, const double* Ki
     return GPMPC_OK;
 }
 
-// 1/2 tr((W - alpha alpha^T) dK/dtheta) for every hyper-parameter into dGrad, W = the lower triangle in dKinv
-static int launch_grad(gpmpc_handle_t h, const double* dHyp, const double* alpha)
+// Argument check of the objectives gpmpc_nlml, gpmpc_nlml_batch and gpmpc_loo_nlpp (fn) at the S hyper rows theta
+// (stride Nx+2), in this order: the NULL pointers and S (args_ok; a batch's message names them), the model state, the
+// output (its local index into *al), zero length scales (a batch's message names the row)
+static int objective_check(gpmpc_handle_t h, const char* fn, bool batch, bool args_ok, int a, const double* theta, int S,
+                           int* al)
 {
-    return launch_grad_at(h, dHyp, h->dKinv, alpha, h->dGradPart, h->dGrad, 1);
-}
-
-// K(theta) -> L, Li, alpha of local output al for an objective at theta (hyper row in dHypTmp) with the jitter retry of
-// optimize.py:345-350.  The output's factor slabs are the scratch: the model needs gpmpc_factorize afterwards.
-static int factor_at_theta(gpmpc_handle_t h, const char* fn, int al, const double* theta)
-{
-    factor_stale(h);
-    CUDA_TRY(cudaMemcpyAsync(h->dHypTmp, theta, (h->Nx + 2) * 8, cudaMemcpyHostToDevice, h->st));
-    int used = 0;
-    const int rc = factor_one(h, al, h->dHypTmp, 1e-8, &used);
-    if (rc) { if (rc == GPMPC_ERR_NOTPD) set_error(h, "%s: K not positive definite even with jitter", fn); return rc; }
-    return launch_alpha(h, al, 1);
-}
-
-extern "C" int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* nll, double* grad)
-{
-    if (!h || !theta || !nll) return GPMPC_ERR_ARG;
-    int rc = model_guard(h, __func__, NEED_DATA);
+    if (!h) return GPMPC_ERR_ARG;
+    if (!args_ok) { if (batch) set_error(h, "%s: NULL pointer or S < 1", fn); return GPMPC_ERR_ARG; }
+    const int rc = model_guard(h, fn, NEED_DATA);
     if (rc) return rc;
-    const int al = local_index(h, a);
-    if (al < 0) return GPMPC_ERR_ARG;
-    const int m = h->Nx + 2;
-    for (int d = 0; d < h->Nx; ++d) if (theta[d] == 0.0) { set_error(h, "gpmpc_nlml: zero length scale"); return GPMPC_ERR_ARG; }
-    NvtxRange nvtx_r("gpmpc.nlml");
-    rc = factor_at_theta(h, __func__, al, theta);
-    if (rc) return rc;
-    double res[2];
-    CUDA_TRY(cudaMemcpyAsync(res, h->dRes + 2 * al, 16, cudaMemcpyDeviceToHost, h->st));
-    if (grad) {
-        rc = compute_kinv(h, al);
-        if (rc) return rc;
-        rc = launch_grad(h, h->dHypTmp, h->dAlpha + (long long)al * h->Npad);
-        if (rc) return rc;
-        CUDA_TRY(cudaMemcpyAsync(grad, h->dGrad, m * 8, cudaMemcpyDeviceToHost, h->st));
-    }
-    CUDA_TRY(cudaStreamSynchronize(h->st));
-    *nll = 0.5 * res[1] + 0.5 * res[0];                      // optimize.py:355
+    if ((*al = local_index(h, a)) < 0) return GPMPC_ERR_ARG;
+    for (int s = 0; s < S; ++s)
+        for (int d = 0; d < h->Nx; ++d)
+            if (theta[(size_t)s * (h->Nx + 2) + d] == 0.0) {
+                if (batch) set_error(h, "%s: zero length scale in row %d", fn, s);
+                else set_error(h, "%s: zero length scale", fn);
+                return GPMPC_ERR_ARG;
+            }
     return GPMPC_OK;
 }
 
-// gpmpc_nlml_batch scratch for a pass of c entries: the factor slabs dNbL, dNbLi, the recursion workspaces dNbW1, dNbW2
-// (W1 also holds the alpha partials), dNbV = [hyper rows (c, Nx+2) | jitter (c) | tmp (c, Npad) | alpha (c, Npad) |
-// res (c, 2) | gradient partials (c, grad_tiles, Nx+2) | gradients (c, Nx+2)], dNbInfo (c)
-static int nlml_batch_scratch(gpmpc_handle_t h, int c)
+// The objective pass of gpmpc_nlml and gpmpc_nlml_batch at the entries' hyper rows theta (host): the factor step with the
+// 1e-8 jitter retry of optimize.py:345-350, every GEMM on the feed of a single slab, so no entry depends on c; the alpha
+// pass; log det and y . alpha; with grad the gradient in place: U = Li^T into the L slab (log det has been read from it),
+// K^-1 = U U^T into the Li slab (alpha is done), tile partials in part and gradients in g (c rows each); then the NLL.
+// status (host, c): 0, 1 (jitter) or GPMPC_ERR_NOTPD, whose entry runs on with its slabs as they are (every pass is per
+// entry, so it touches no other) and gets NaN.  Without status a failed entry is an error of fn, before the alpha pass.
+static int objective_pass(gpmpc_handle_t h, const char* fn, const FactorSet& e, const double* theta, double* part,
+                          double* g, double* nll, double* grad, int* status)
 {
-    const long long m = h->Nx + 2;
-    ENSURE(h->dNbL, c * slab(h));
-    ENSURE(h->dNbLi, c * slab(h));
-    ENSURE(h->dNbW1, c * w2slab(h));
-    ENSURE(h->dNbW2, c * w2slab(h));
-    ENSURE(h->dNbV, c * (m + 1 + 2LL * h->Npad + 2 + grad_tiles(h) * m + m));
-    ENSURE(h->dNbInfo, c);
-    return GPMPC_OK;
-}
-
-// NLML (and gradient) of local output al at the c hyper rows theta, each on its own slabs with gpmpc_nlml's arithmetic:
-// one K build, one recursion, one alpha pass and one gradient pass for the chunk, and factor_one's jitter retry for an
-// entry whose first factorisation fails.  Every GEMM takes the feed of a single slab, so no entry depends on c.
-static int nlml_batch_pass(gpmpc_handle_t h, int al, int c, const double* theta, double* nll, double* grad, int* status)
-{
-    const int m = h->Nx + 2, np = h->Npad, nt = grad_tiles(h);
-    double* hyp = h->dNbV;
-    double* jit = hyp + (long long)c * m;
-    double* tmp = jit + c;
-    double* alpha = tmp + (long long)c * np;
-    double* res = alpha + (long long)c * np;
-    double* part = res + 2 * c;
-    double* g = part + (long long)c * nt * m;
-    CUDA_TRY(cudaMemcpyAsync(hyp, theta, (size_t)c * m * 8, cudaMemcpyHostToDevice, h->st));
-    CUDA_TRY(cudaMemsetAsync(jit, 0, (size_t)c * 8, h->st));
-    CUDA_TRY(cudaMemsetAsync(h->dNbInfo, 0, (size_t)c * sizeof(int), h->st));
-    int rc = launch_kbuild(h, hyp, jit, h->dNbL, c, 0);
+    const int c = e.c, m = h->Nx + 2;
+    CUDA_TRY(cudaMemcpyAsync(e.hyp, theta, (size_t)c * m * 8, cudaMemcpyHostToDevice, h->st));
+    std::vector<int> used(c);
+    int rc = factor_entries(h, e, 1, 1e-8, used.data());
     if (rc) return rc;
-    rc = potrf_inv_rec(h, h->dNbL, h->dNbLi, slab(h), slab(h), h->dNbInfo, 0, np, c, 1, h->dNbW1, h->dNbW2);
-    if (rc) return rc;
-    std::vector<int> info(c);
-    CUDA_TRY(cudaMemcpyAsync(info.data(), h->dNbInfo, (size_t)c * sizeof(int), cudaMemcpyDeviceToHost, h->st));
-    CUDA_TRY(cudaStreamSynchronize(h->st));
-    bool retried = false;
     for (int s = 0; s < c; ++s) {
-        status[s] = GPMPC_OK;
-        if (!info[s]) continue;
-        // factor_one's second attempt, on this entry's slabs
-        const double jitter = 1e-8;
-        double* L = h->dNbL + s * slab(h);
-        CUDA_TRY(cudaMemcpyAsync(jit + s, &jitter, 8, cudaMemcpyHostToDevice, h->st));
-        CUDA_TRY(cudaMemsetAsync(h->dNbInfo + s, 0, sizeof(int), h->st));
-        rc = launch_kbuild(h, hyp + (long long)s * m, jit + s, L, 1, 0);
-        if (rc) return rc;
-        rc = potrf_inv_rec(h, L, h->dNbLi + s * slab(h), slab(h), slab(h), h->dNbInfo + s, 0, np, 1, 1,
-                           h->dNbW1 + s * w2slab(h), h->dNbW2 + s * w2slab(h));
-        if (rc) return rc;
-        status[s] = 1;
-        retried = true;
+        if (status) status[s] = used[s] > 1 ? GPMPC_ERR_NOTPD : used[s];
+        else if (used[s] > 1) { set_error(h, "%s: K not positive definite even with jitter", fn); return GPMPC_ERR_NOTPD; }
     }
-    if (retried) {
-        CUDA_TRY(cudaMemcpyAsync(info.data(), h->dNbInfo, (size_t)c * sizeof(int), cudaMemcpyDeviceToHost, h->st));
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-        for (int s = 0; s < c; ++s) if (status[s] == 1 && info[s]) status[s] = GPMPC_ERR_NOTPD;
-    }
-    // a failed entry runs on with its slabs as they are: the passes below are per entry, so it touches no other
-    rc = launch_alpha_at(h, h->dNbL, h->dNbLi, h->dY + (long long)al * np, 0, tmp, h->dNbW1, alpha, res, c);
+    rc = alpha_pass(h, e);
     if (rc) return rc;
-    std::vector<double> hres(2 * c);
-    CUDA_TRY(cudaMemcpyAsync(hres.data(), res, (size_t)c * 16, cudaMemcpyDeviceToHost, h->st));
+    std::vector<double> res(2 * c);
+    CUDA_TRY(cudaMemcpyAsync(res.data(), e.res, (size_t)c * 16, cudaMemcpyDeviceToHost, h->st));
     if (grad) {
-        // U = Li^T into the L slab (log det has been read from it), K^-1 = U U^T into the Li slab (alpha is done)
-        rc = kinv_at(h, h->dNbLi, h->dNbL, h->dNbLi, c);
+        rc = kinv_at(h, e.Li, e.L, e.Li, c);
         if (rc) return rc;
-        rc = launch_grad_at(h, hyp, h->dNbLi, alpha, part, g, c);
+        rc = launch_grad_at(h, e.hyp, e.Li, e.alpha, part, g, c);
         if (rc) return rc;
         CUDA_TRY(cudaMemcpyAsync(grad, g, (size_t)c * m * 8, cudaMemcpyDeviceToHost, h->st));
     }
     CUDA_TRY(cudaStreamSynchronize(h->st));
     for (int s = 0; s < c; ++s) {
-        if (status[s] == GPMPC_ERR_NOTPD) {
+        if (used[s] > 1) {
             nll[s] = NAN;
             if (grad) for (int q = 0; q < m; ++q) grad[(size_t)s * m + q] = NAN;
         } else {
-            nll[s] = 0.5 * hres[2 * s + 1] + 0.5 * hres[2 * s];   // gpmpc_nlml's sum
+            nll[s] = 0.5 * res[2 * s + 1] + 0.5 * res[2 * s];      // optimize.py:355
         }
     }
+    return GPMPC_OK;
+}
+
+extern "C" int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* nll, double* grad)
+{
+    int al = 0;
+    int rc = objective_check(h, __func__, false, theta && nll, a, theta, 1, &al);
+    if (rc) return rc;
+    NvtxRange nvtx_r("gpmpc.nlml");
+    if (grad) ENSURE(h->dGradPart, (long long)grad_tiles(h) * (h->Nx + 2));
+    // a one-entry pass in output al's own slots, the hyper row in dHypTmp: the model needs gpmpc_factorize afterwards
+    factor_stale(h);
+    FactorSet e = model_entries(h, al, 1);
+    e.hyp = h->dHypTmp;
+    return objective_pass(h, __func__, e, theta, h->dGradPart, h->dGrad, nll, grad, nullptr);
+}
+
+// gpmpc_nlml_batch scratch for a pass of c entries of local output al: the factor slabs dNbL, dNbLi, the recursion
+// workspaces dNbW1, dNbW2, the pivot infos dNbInfo and dNbV = [hyper rows (c, Nx+2) | jitter (c) | tmp (c, Npad) |
+// alpha (c, Npad) | res (c, 2) | gradient partials (c, grad_tiles, Nx+2) | gradients (c, Nx+2)]; every entry's target is
+// al's y.  The entries go to *e, the gradient partials and gradients to *part and *g.
+static int nlml_batch_scratch(gpmpc_handle_t h, int al, int c, FactorSet* e, double** part, double** g)
+{
+    const long long m = h->Nx + 2, np = h->Npad;
+    ENSURE(h->dNbL, c * slab(h));
+    ENSURE(h->dNbLi, c * slab(h));
+    ENSURE(h->dNbW1, c * w2slab(h));
+    ENSURE(h->dNbW2, c * w2slab(h));
+    ENSURE(h->dNbV, c * (m + 1 + 2 * np + 2 + grad_tiles(h) * m + m));
+    ENSURE(h->dNbInfo, c);
+    double* jit = h->dNbV + c * m;
+    double* tmp = jit + c;
+    double* alpha = tmp + c * np;
+    double* res = alpha + c * np;
+    *e = {c, h->dNbV, jit, h->dNbInfo, h->dNbL, h->dNbLi, h->dNbW1, h->dNbW2, h->dY + al * np, 0, tmp, alpha, res};
+    *part = res + 2 * c;
+    *g = *part + c * grad_tiles(h) * m;
     return GPMPC_OK;
 }
 
@@ -1019,25 +1002,18 @@ static void nlml_batch_release(gpmpc_handle_t h)
 extern "C" int gpmpc_nlml_batch(gpmpc_handle_t h, int a, int S, const double* theta, double* nll, double* grad,
                                 int* status)
 {
-    if (!h) return GPMPC_ERR_ARG;
-    if (!theta || !nll || !status || S < 1) { set_error(h, "gpmpc_nlml_batch: NULL pointer or S < 1"); return GPMPC_ERR_ARG; }
-    int rc = model_guard(h, __func__, NEED_DATA);
+    int al = 0;
+    int rc = objective_check(h, __func__, true, theta && nll && status && S >= 1, a, theta, S, &al);
     if (rc) return rc;
-    const int al = local_index(h, a);
-    if (al < 0) return GPMPC_ERR_ARG;
     const int m = h->Nx + 2;
-    for (int s = 0; s < S; ++s)
-        for (int d = 0; d < h->Nx; ++d)
-            if (theta[(size_t)s * m + d] == 0.0) {
-                set_error(h, "gpmpc_nlml_batch: zero length scale in row %d", s);
-                return GPMPC_ERR_ARG;
-            }
     NvtxRange nvtx_r("gpmpc.nlml_batch");
     // results do not depend on the pass size, so a pass that does not fit is halved
     int pass = h->opt_nlml_batch_max > 0 ? std::min(S, h->opt_nlml_batch_max) : S;
     for (int s0 = 0; s0 < S;) {
         const int c = std::min(pass, S - s0);
-        rc = nlml_batch_scratch(h, c);
+        FactorSet e;
+        double *part, *g;
+        rc = nlml_batch_scratch(h, al, c, &e, &part, &g);
         if (rc) {
             const bool oom = cudaGetLastError() == cudaErrorMemoryAllocation;
             nlml_batch_release(h);
@@ -1045,7 +1021,8 @@ extern "C" int gpmpc_nlml_batch(gpmpc_handle_t h, int a, int S, const double* th
             pass = c / 2;
             continue;
         }
-        rc = nlml_batch_pass(h, al, c, theta + (size_t)s0 * m, nll + s0, grad ? grad + (size_t)s0 * m : nullptr, status + s0);
+        rc = objective_pass(h, __func__, e, theta + (size_t)s0 * m, part, g, nll + s0,
+                            grad ? grad + (size_t)s0 * m : nullptr, status + s0);
         if (rc) return rc;
         s0 += c;
     }
@@ -1110,16 +1087,22 @@ extern "C" int gpmpc_loo(gpmpc_handle_t h, double* mean, double* var, double* nl
 
 extern "C" int gpmpc_loo_nlpp(gpmpc_handle_t h, int a, const double* theta, double* nlpp, double* grad)
 {
-    if (!h || !theta || !nlpp) return GPMPC_ERR_ARG;
-    int rc = model_guard(h, __func__, NEED_DATA);
+    int al = 0;
+    int rc = objective_check(h, __func__, false, theta && nlpp, a, theta, 1, &al);
     if (rc) return rc;
-    const int al = local_index(h, a);
-    if (al < 0) return GPMPC_ERR_ARG;
     const int m = h->Nx + 2, N = h->N, np = h->Npad;
-    for (int d = 0; d < h->Nx; ++d) if (theta[d] == 0.0) { set_error(h, "gpmpc_loo_nlpp: zero length scale"); return GPMPC_ERR_ARG; }
     if (N < 2) { set_error(h, "gpmpc_loo_nlpp: needs N >= 2 training points (N = %d)", N); return GPMPC_ERR_ARG; }
     NvtxRange nvtx_r("gpmpc.loo_nlpp");
-    rc = factor_at_theta(h, __func__, al, theta);
+    // gpmpc_nlml's factor step and alpha pass in output al's own slots: the model needs gpmpc_factorize afterwards
+    factor_stale(h);
+    FactorSet e = model_entries(h, al, 1);
+    e.hyp = h->dHypTmp;
+    CUDA_TRY(cudaMemcpyAsync(e.hyp, theta, m * 8, cudaMemcpyHostToDevice, h->st));
+    int used = 0;
+    rc = factor_entries(h, e, 1, 1e-8, &used);
+    if (rc) return rc;
+    if (used > 1) { set_error(h, "gpmpc_loo_nlpp: K not positive definite even with jitter"); return GPMPC_ERR_NOTPD; }
+    rc = alpha_pass(h, e);
     if (rc) return rc;
     LooLayout o;
     rc = loo_layout(h, 1, &o);
@@ -1129,14 +1112,12 @@ extern "C" int gpmpc_loo_nlpp(gpmpc_handle_t h, int a, const double* theta, doub
     double val = 0.0;
     CUDA_TRY(cudaMemcpyAsync(&val, o.nlpp, 8, cudaMemcpyDeviceToHost, h->st));
     if (grad) {
-        const double* Li = h->dLi + (long long)al * slab(h);
-        const double* alpha = h->dAlpha + (long long)al * np;
         rc = compute_kinv(h, al);                          // C (lower) in dKinv
         if (rc) return rc;
         // b = C u = Li^T (Li u)
-        trmv_lower_kernel<<<(N + 7) / 8, 256, 0, h->st>>>(Li, np, 0, o.u, 0, o.tmp, 0, N);
+        trmv_lower_kernel<<<(N + 7) / 8, 256, 0, h->st>>>(e.Li, np, 0, o.u, 0, o.tmp, 0, N);
         CUDA_TRY(cudaGetLastError());
-        trmv_lower_T_kernel<<<(N + 31) / 32, 256, 0, h->st>>>(Li, np, 0, o.tmp, 0, o.b, 0, N);
+        trmv_lower_T_kernel<<<(N + 31) / 32, 256, 0, h->st>>>(e.Li, np, 0, o.tmp, 0, o.b, 0, N);
         CUDA_TRY(cudaGetLastError());
         // G = (C diag(sqrt w)) (C diag(sqrt w))^T = C diag(w) C: lower tiles into dKinv, over C diag(sqrt w) in dU
         loo_mirror_scale_kernel<<<dim3(np / 32, np / 32), dim3(32, 8), 0, h->st>>>(h->dKinv, np, o.sw, h->dU, N);
@@ -1146,11 +1127,11 @@ extern "C" int gpmpc_loo_nlpp(gpmpc_handle_t h, int a, const double* theta, doub
         p.A = h->dU; p.lda = np; p.B = h->dU; p.ldb = np; p.C = h->dKinv; p.ldc = np;
         p.mt = np / 128; p.nt = np / 128; p.K = np; p.alpha = 1.0; p.beta = 0.0; p.lower = 1;
         CUDA_TRY(gemm128(h, h->st, true, p, 1, 1));
-        loo_w_kernel<<<dim3((N + 255) / 256, N), 256, 0, h->st>>>(h->dKinv, np, o.b, alpha, N);
+        loo_w_kernel<<<dim3((N + 255) / 256, N), 256, 0, h->st>>>(h->dKinv, np, o.b, e.alpha, N);
         CUDA_TRY(cudaGetLastError());
         // the trace pass with W in place of K^-1 and alpha = 0: 1/2 tr(W dK/dtheta), doubled on the host (exact)
         CUDA_TRY(cudaMemsetAsync(o.zero, 0, (size_t)np * 8, h->st));
-        rc = launch_grad(h, h->dHypTmp, o.zero);
+        rc = launch_grad_at(h, e.hyp, h->dKinv, o.zero, h->dGradPart, h->dGrad, 1);
         if (rc) return rc;
         CUDA_TRY(cudaMemcpyAsync(grad, h->dGrad, m * 8, cudaMemcpyDeviceToHost, h->st));
     }
@@ -1665,7 +1646,7 @@ static int em_scratch(gpmpc_handle_t h, int n, int H)
     ENSURE(h->dEmE2, n * s.pair); ENSURE(h->dEmF2, n * s.pair);
     ENSURE(h->dEmW, n * s.w); ENSURE(h->dEmIJ, n * s.w);
     ENSURE(h->dEmMeanPart, n * s.mpart); ENSURE(h->dEmPart, n * s.part);
-    { int rcs = ensure_nlml_scratch(h); if (rcs) return rcs; }
+    { int rcs = ensure_kinv_scratch(h); if (rcs) return rcs; }
     ENSURE(h->dKinv, n * s.q); ENSURE(h->dU, n * s.q);
     ENSURE(h->dEMP, (long long)H * s.emp);
     return GPMPC_OK;
@@ -3173,7 +3154,7 @@ extern "C" int gpmpc_remove(gpmpc_handle_t h, int n, const int* idx)
     if (order[0] >= N || order[n - 1] < 0) { set_error(h, "gpmpc_remove: index out of range [0, %d)", N); return GPMPC_ERR_ARG; }
     for (int k = 1; k < n; ++k)
         if (order[k] == order[k - 1]) { set_error(h, "gpmpc_remove: index %d given twice", order[k]); return GPMPC_ERR_ARG; }
-    rc = ensure_nlml_scratch(h);          // dU / dKinv: the work slabs of the new rows
+    rc = ensure_kinv_scratch(h);          // dU / dKinv: the work slabs of the new rows
     if (rc) return rc;
     ENSURE(h->dRm, (long long)nl * 3 * np);
     NvtxRange nvtx_r("gpmpc.remove");

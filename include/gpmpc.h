@@ -109,7 +109,8 @@ int gpmpc_factorize(gpmpc_handle_t h, double jitter, int* info);
  * (grad != NULL) its analytic gradient:  NLL = 1/2 y^T alpha + 1/2 logdet K (no
  * N/2 log 2pi term), with the same jitter retry.  Replaces calc_NLL_numpy,
  * optimize.py:322-356; the gradient replaces SLSQP's finite differences
- * (optimize.py:466-467).  Invalidates the factorisation of output a. */
+ * (optimize.py:466-467).  Invalidates the factorisation of output a: the evaluation,
+ * gradient included, works in that output's factor slabs and needs no other Npad^2 scratch. */
 int gpmpc_nlml(gpmpc_handle_t h, int a, const double* theta, double* nll, double* grad);
 
 /* gpmpc_nlml at S hyper-parameter points of global output a in one pass.
@@ -142,7 +143,8 @@ int gpmpc_loo(gpmpc_handle_t h, double* mean, double* var, double* nlpp);
  * with the same single 1e-8 jitter retry, returns the NLPP of gpmpc_loo and (grad != NULL) its analytic gradient
  * (R&W eq. 5.13 as a trace: dNLPP/dtheta_j = tr(W dK/dtheta_j), W = C diag(w) C - sym(b alpha^T),
  * w_i = (1 + alpha_i^2/c_i) / (2 c_i), b = C (alpha / c)).  The NLPP has the same bits with and without grad.
- * Same argument checks as gpmpc_nlml, and GPMPC_ERR_ARG for N < 2.  Scratch: gpmpc_nlml's two Npad^2 slabs.
+ * Same argument checks as gpmpc_nlml, and GPMPC_ERR_ARG for N < 2.  Scratch: the two Npad^2 slabs of
+ * gpmpc_get(GPMPC_GET_INVK).
  * Invalidates the factorisation of output a. */
 int gpmpc_loo_nlpp(gpmpc_handle_t h, int a, const double* theta, double* nlpp, double* grad);
 
@@ -192,7 +194,7 @@ int gpmpc_append_greedy(gpmpc_handle_t h, int n, const double* Xc, const double*
  * its broken update_data (gp_class.py:384-471).
  *   n = 0: no-op.  GPMPC_ERR_STATE: not factorised.  GPMPC_ERR_ARG: n < 0, idx NULL with n > 0, an index outside
  *   [0, N), a duplicate, or n >= N (one point must remain).  Every check runs before any work: an error leaves the
- *   model bit-identical.  Scratch: the two Npad^2 slabs of gpmpc_nlml's gradient (allocated once, if not yet). */
+ *   model bit-identical.  Scratch: the two Npad^2 slabs of gpmpc_get(GPMPC_GET_INVK) (allocated once, if not yet). */
 int gpmpc_remove(gpmpc_handle_t h, int n, const int* idx);
 
 /* Full posterior covariance between H test points for every OWNED output:

@@ -1,7 +1,8 @@
 """gpmpc_loo / gpmpc_loo_nlpp / GP.loo_predict / GP.validate_loo / optimizer_opts={'objective': 'loo'} on the GPU: the
 leave-one-out predictions and their NLPP against the numpy oracle (oracle/loo_oracle.py), the analytic gradient against
 the oracle's and against central differences of the engine's own value, handles after appends and removals, sharded
-handles, determinism, the scratch the gradient shares with gpmpc_nlml, the argument and state checks, and an LOO fit."""
+handles, determinism, the scratch the gradient shares with gpmpc_nlml, the jitter retry, the argument and state checks,
+and an LOO fit."""
 import ctypes as C
 
 import numpy as np
@@ -137,6 +138,29 @@ def test_nlml_bits_do_not_change_around_loo_nlpp():
     eng.factorize()
     post = orc.postfit(X, Y[:, 1:2], hyper[1:2], lapack_general_solve=False)
     assert relinf(eng.get(_L().GET_INVK, 1), post['invK'][0]) < 1e-7
+
+
+def test_loo_nlpp_takes_the_jitter_retry_of_factorize():
+    """Duplicated points and sn = 1e-10 make K singular in fp64: loo_nlpp factorises K + 1e-8 I, so its value is the
+    bits of gpmpc_loo on the model gpmpc_factorize(1e-8) builds at the same theta (info 1).  A NaN signal std fails
+    with and without the jitter: LinAlgError, as gpmpc_nlml raises."""
+    N, Nx = 1100, 6
+    p = orc.synthetic_problem(N, Nx, 3, config_id=301)
+    X = p['X'].copy(); X[N // 2:] = X[:N - N // 2]
+    Y = p['Y'][:, 1:2]
+    th = p['hyper'][1].copy(); th[Nx + 1] = 1e-10
+    eng = _L().Engine(N, Nx, 1, device=0)
+    eng.set_data(X, Y)
+    f = eng.loo_nlpp(0, th, grad=False)
+    eng.set_hyper(th[None, :])
+    assert list(eng.factorize(1e-8)) == [1]
+    assert np.float64(f).tobytes() == eng.loo()[2][0].tobytes()
+    nan = th.copy(); nan[Nx] = np.nan
+    with pytest.raises(np.linalg.LinAlgError):
+        eng.loo_nlpp(0, nan)
+    with pytest.raises(np.linalg.LinAlgError):
+        eng.nlml(0, nan)
+    eng.close()
 
 
 def test_null_buffers():
