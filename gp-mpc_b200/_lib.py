@@ -54,6 +54,7 @@ SYMBOLS = [
     ('gpmpc_rollout_batch', C.c_int, [_H, C.c_int, C.c_int, C.c_int] + [_dp] * 10),
     ('gpmpc_rollout_batch_grad', C.c_int, [_H, C.c_int, C.c_int, C.c_int] + [_dp] * 12),
     ('gpmpc_rollout_batch_em', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 10),
+    ('gpmpc_rollout_batch_em_grad', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 12),
     ('gpmpc_rollout_sample', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 10 + [_ip]),
     ('gpmpc_predict_device', C.c_int, [_H, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
@@ -365,6 +366,23 @@ class Engine:
         self._check(self.lib.gpmpc_rollout_batch_grad(self.h, int(method), B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0),
                                                       _ptr(scale), _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means),
                                                       _ptr(var), _ptr(cov), _ptr(dmeans), _ptr(dvars)))
+        return means, var, cov, dmeans, dvars
+
+    def rollout_batch_em_grad(self, z0, U, Sigma0, scale=None, K=None, x_ref=None, uscale=None):
+        """gpmpc_rollout_batch_em_grad: rollout_batch_em's arguments and outputs (bit for bit) plus dmeans, dvars
+        (B,Nt,Ny,P) with rollout_batch_grad's parameter columns, for exact moment matching ('EM')."""
+        Nu = self.Nx - self.Ny
+        z0 = _f64(z0).reshape(-1, self.Nx)
+        B = z0.shape[0]
+        Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
+        Nt = int(np.shape(U)[1])
+        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
+        P = self.Nx + (Nu * self.Ny if K is not None else (Nt - 1) * Nu)
+        means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
+        dmeans = np.empty((B, Nt, self.Ny, P)); dvars = np.empty((B, Nt, self.Ny, P))
+        self._check(self.lib.gpmpc_rollout_batch_em_grad(self.h, B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale),
+                                                         _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means), _ptr(var),
+                                                         _ptr(cov), _ptr(dmeans), _ptr(dvars)))
         return means, var, cov, dmeans, dvars
 
     def rollout_sample(self, z0, U, eps, xi=None, scale=None, K=None, x_ref=None, uscale=None):

@@ -177,7 +177,7 @@ struct gpmpc_handle_s {
     DevBuf<double> dG;
     double *dZ = nullptr, *dSigma = nullptr, *dMean = nullptr, *dVar = nullptr, *dJ = nullptr, *dCov = nullptr;   // in dIn / dOut
     DevBuf<double> dRoll;             // gpmpc_rollout_batch: [Z | Sigma | U | scale | K | x_ref | uscale | means | vars | cov]
-    DevBuf<double> dRollTg;           // gpmpc_rollout_batch_grad: [dZ | dSigma ('TA') | dmeans | dvars]
+    DevBuf<double> dRollTg;           // gpmpc_rollout_batch_grad, _em_grad: [dZ | dSigma ('TA', 'EM') | dmeans | dvars | 'EM' blocks]
     DevBuf<double> dSmV;              // gpmpc_rollout_sample: V rows of every step (nloc, Nt, B, Npad)
     DevBuf<double> dSmp;              //   [eps | xi | U | scale | K | x_ref | uscale | Z (Nt,B,Nx) | samples | kept | m | R]
     DevBuf<double> dIn, dOut;         // [Z | Sigma] and [mean | var | J | cov] slabs: one H2D + one D2H per host call
@@ -1975,42 +1975,112 @@ static int em_hess_pair_params(gpmpc_handle_t h, const double* S, const double* 
     return GPMPC_OK;
 }
 
+// The record set of degree D for H points: its tables built and uploaded once, the block partials, the records of H points
+// and the backbone rows
+static int em_records_prepare(gpmpc_handle_t h, int D, int H)
+{
+    const int Ny = h->Ny, T = (h->N + 63) / 64;
+    EmRecords& R = h->em_rec[D / 2 - 1];
+    if (!R.tb) R.tb.reset(new EmTables(h->Nx, D));
+    EmTables& tb = *R.tb;
+    ENSURE(R.part, (long long)tb.nrec(Ny) * T * tb.nent);
+    ENSURE(R.rec, (long long)H * tb.nrec(Ny) * tb.nent);
+    ENSURE(R.bb, 3LL * tb.nf * h->Npad);
+    ENSURE(R.idx, (long long)tb.dev.size());
+    if (tb.uploaded_to != R.idx.p) {
+        CUDA_TRY(cudaMemcpyAsync(R.idx, tb.dev.data(), tb.dev.size() * 4, cudaMemcpyHostToDevice, h->st));
+        tb.uploaded_to = R.idx.p;
+    }
+    return GPMPC_OK;
+}
+
+// The full symmetric K^-1 of every output that the records' trace terms read (dEmKinv, 8 B Ny Npad^2, kept until the next
+// factor change)
+static int em_kinv_prepare(gpmpc_handle_t h)
+{
+    const int np = h->Npad;
+    ENSURE(h->dEmKinv, (long long)h->Ny * slab(h));
+    if (!h->em_kinv_valid) {        // K^-1 = U U^T per output (compute_kinv, lower), stored full and symmetric
+        for (int a = 0; a < h->Ny; ++a) {
+            int rck = compute_kinv(h, a);
+            if (rck) return rck;
+            sym_from_lower_kernel<<<dim3(np / 32, np / 32), dim3(32, 8), 0, h->st>>>(h->dKinv, h->dEmKinv + (long long)a * slab(h), np);
+            CUDA_TRY(cudaGetLastError());
+        }
+        h->em_kinv_valid = true;
+    }
+    return GPMPC_OK;
+}
+
+// The derivative records of the n points of one em_forward chunk, point k from its scratch slot k: z at dz and the
+// em_prepare_point blocks at dP (strides Nx and em_per, device); D = 2 records to rec2 and D = 4 records to rec4, one
+// point's records apart (null: not wanted).  The slots are overwritten by the next chunk's forward.
+static int em_chunk_records(gpmpc_handle_t h, int n, const double* dz, const double* dP, double* rec2, double* rec4)
+{
+    const int Nx = h->Nx, Ny = h->Ny, npairs = em_npairs(h), T = (h->N + 63) / 64;
+    const size_t per = em_per(h);
+    const EmRecords& R2 = h->em_rec[0];
+    const EmRecords& R4 = h->em_rec[1];
+    for (int k = 0; k < n && (rec2 || rec4); ++k) {
+        const double* z = dz + (size_t)k * Nx;
+        const double* P = dP + (size_t)k * per;
+        if (rec2) {
+            double* rec = rec2 + (size_t)k * R2.tb->nrec(Ny) * R2.tb->nent;
+            CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_records<decltype(nxp)::value, 2>(h, R2, z, P, npairs, T, k, rec); }));
+        }
+        if (rec4) {
+            double* rec = rec4 + (size_t)k * R4.tb->nrec(Ny) * R4.tb->nent;
+            CUDA_TRY((Nx <= 8 ? launch_em_records<8, 4>(h, R4, z, P, npairs, T, k, rec)
+                              : launch_em_records<16, 4>(h, R4, z, P, npairs, T, k, rec)));   // Nx <= 16
+        }
+    }
+    return GPMPC_OK;
+}
+
+// em_grad_finish of H points on the host: Sigma (one per point with spp, else shared), their em_prepare_point blocks emp,
+// D = 2 records recs and means mh, each at its per-point stride; point p's outputs at p times their block in go (null
+// members skipped).  On failure *bad (if given) is the failing point.
+static int em_grad_finish_points(gpmpc_handle_t h, int H, const double* Sigma, int spp, const double* emp, const double* recs,
+                                 const double* mh, const EmGradOutputs& go, int* bad = nullptr)
+{
+    const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx;
+    const EmTables& tb = *h->em_rec[0].tb;
+    const size_t per = em_per(h), rl = (size_t)tb.nrec(Ny) * tb.nent;
+    for (int p = 0; p < H; ++p) {
+        const int rc = em_grad_finish(h, tb, Sigma + (spp ? (size_t)p * nn : 0), emp + (size_t)p * per, recs + (size_t)p * rl,
+                                      mh + (size_t)p * Ny,
+                                      go.dmean_dz ? go.dmean_dz + (size_t)p * Ny * Nx : nullptr,
+                                      go.dmean_dSigma ? go.dmean_dSigma + (size_t)p * Ny * nn : nullptr,
+                                      go.dcov_dz ? go.dcov_dz + (size_t)p * Ny * Ny * Nx : nullptr,
+                                      go.dcov_dSigma ? go.dcov_dSigma + (size_t)p * Ny * Ny * nn : nullptr);
+        if (rc) {
+            if (bad) *bad = p;
+            return rc;
+        }
+    }
+    return GPMPC_OK;
+}
+
 static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Sigma, int spp,
                       double* mean, double* var, double* cov, const EmGradOutputs* go = nullptr,
                       const EmHessOutputs* ho = nullptr)
 {
-    const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, np = h->Npad;
+    const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx;
     NvtxRange nvtx_r("gpmpc.predict_em");
     if (!Sigma) { set_error(h, "EM needs an input covariance"); return GPMPC_ERR_ARG; }
     const int npairs = em_npairs(h);
     if (npairs > 1024) { set_error(h, "EM supports Ny <= 44"); return GPMPC_ERR_ARG; }
     const size_t per = em_per(h);
-    const int T = (h->N + 63) / 64;
     const int nc = em_chunk(h, H);
     { const int rcs = em_scratch(h, nc, H); if (rcs) return rcs; }
-    // the record set of degree D: tables built and uploaded once, scratch for H points
-    auto records = [&](int D) -> int {
-        EmRecords& R = h->em_rec[D / 2 - 1];
-        if (!R.tb) R.tb.reset(new EmTables(Nx, D));
-        EmTables& tb = *R.tb;
-        ENSURE(R.part, (long long)tb.nrec(Ny) * T * tb.nent);
-        ENSURE(R.rec, (long long)H * tb.nrec(Ny) * tb.nent);
-        ENSURE(R.bb, 3LL * tb.nf * np);
-        ENSURE(R.idx, (long long)tb.dev.size());
-        if (tb.uploaded_to != R.idx.p) {
-            CUDA_TRY(cudaMemcpyAsync(R.idx, tb.dev.data(), tb.dev.size() * 4, cudaMemcpyHostToDevice, h->st));
-            tb.uploaded_to = R.idx.p;
-        }
-        return GPMPC_OK;
-    };
     EmRecords& R2 = h->em_rec[0];
     EmRecords& R4 = h->em_rec[1];
-    if (go) { const int rc = records(2); if (rc) return rc; }
+    if (go) { const int rc = em_records_prepare(h, 2, H); if (rc) return rc; }
     const long long TS = 1 + Nx + nn + (long long)nn * Nx + (long long)nn * nn, Q = (long long)nn * nn;
     const long long per_pair = 6 * TS + 8 * Q, nout = (long long)nn + nn * Nx + nn * nn;    // finish scratch per CTA; one output slab
     const int Hc = (int)std::max(1LL, std::min((long long)H, (64LL << 20) / ((long long)npairs * per_pair)));   // points per finish launch
     if (ho) {
-        const int rc = records(4);
+        const int rc = em_records_prepare(h, 4, H);
         if (rc) return rc;
         ENSURE(h->dEmHEHP, (long long)H * npairs * (9 * nn + 1));
         ENSURE(h->dEmHMU, (long long)H * Ny * TS);
@@ -2018,18 +2088,7 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
         ENSURE(h->dEmHScr, std::max((long long)H * Ny * Q, (long long)Hc * npairs * per_pair));
         ENSURE(h->dEmHOut, (long long)H * (Ny + Ny * Ny) * nout);
     }
-    if (go || ho) {
-        ENSURE(h->dEmKinv, (long long)Ny * slab(h));
-        if (!h->em_kinv_valid) {        // K^-1 = U U^T per output (compute_kinv, lower), stored full and symmetric
-            for (int a = 0; a < Ny; ++a) {
-                int rck = compute_kinv(h, a);
-                if (rck) return rck;
-                sym_from_lower_kernel<<<dim3(np / 32, np / 32), dim3(32, 8), 0, h->st>>>(h->dKinv, h->dEmKinv + (long long)a * slab(h), np);
-                CUDA_TRY(cudaGetLastError());
-            }
-            h->em_kinv_valid = true;
-        }
-    }
+    if (go || ho) { const int rc = em_kinv_prepare(h); if (rc) return rc; }
     std::vector<double> emp((size_t)H * per);
     for (int p = 0; p < H; ++p) {
         int rc = em_prepare_point(h, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per);
@@ -2042,21 +2101,10 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
         int rc = em_forward(h, n, h->dZ + (size_t)c0 * Nx, h->dEMP + (size_t)c0 * per, h->dMean + (size_t)c0 * Ny,
                             h->dVar + (size_t)c0 * Ny, h->dCov + (size_t)c0 * Ny * Ny);
         if (rc) return rc;
-        // the derivative records of each point of the chunk, from its scratch slot
-        for (int k = 0; k < n && (go || ho); ++k) {
-            const int p = c0 + k;
-            const double* dz = h->dZ + (size_t)p * Nx;
-            const double* dP = h->dEMP + (size_t)p * per;
-            if (go) {
-                double* rec = R2.rec + (size_t)p * R2.tb->nrec(Ny) * R2.tb->nent;
-                CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_records<decltype(nxp)::value, 2>(h, R2, dz, dP, npairs, T, k, rec); }));
-            }
-            if (ho) {
-                double* rec = R4.rec + (size_t)p * R4.tb->nrec(Ny) * R4.tb->nent;
-                CUDA_TRY((Nx <= 8 ? launch_em_records<8, 4>(h, R4, dz, dP, npairs, T, k, rec)
-                                  : launch_em_records<16, 4>(h, R4, dz, dP, npairs, T, k, rec)));   // Nx <= 16
-            }
-        }
+        rc = em_chunk_records(h, n, h->dZ + (size_t)c0 * Nx, h->dEMP + (size_t)c0 * per,
+                              go ? R2.rec + (size_t)c0 * R2.tb->nrec(Ny) * R2.tb->nent : nullptr,
+                              ho ? R4.rec + (size_t)c0 * R4.tb->nrec(Ny) * R4.tb->nent : nullptr);
+        if (rc) return rc;
     }
     if (mean) CUDA_TRY(cudaMemcpyAsync(mean, h->dMean, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
     if (var) CUDA_TRY(cudaMemcpyAsync(var, h->dVar, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
@@ -2102,15 +2150,7 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
         CUDA_TRY(cudaMemcpyAsync(recs.data(), R2.rec, recs.size() * 8, cudaMemcpyDeviceToHost, h->st));
         CUDA_TRY(cudaMemcpyAsync(mh.data(), h->dMean, mh.size() * 8, cudaMemcpyDeviceToHost, h->st));
         CUDA_TRY(cudaStreamSynchronize(h->st));
-        for (int p = 0; p < H; ++p) {
-            const int rc = em_grad_finish(h, tb, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per, recs.data() + (size_t)p * rl,
-                                          mh.data() + (size_t)p * Ny,
-                                          go->dmean_dz ? go->dmean_dz + (size_t)p * Ny * Nx : nullptr,
-                                          go->dmean_dSigma ? go->dmean_dSigma + (size_t)p * Ny * nn : nullptr,
-                                          go->dcov_dz ? go->dcov_dz + (size_t)p * Ny * Ny * Nx : nullptr,
-                                          go->dcov_dSigma ? go->dcov_dSigma + (size_t)p * Ny * Ny * nn : nullptr);
-            if (rc) return rc;
-        }
+        return em_grad_finish_points(h, H, Sigma, spp, emp.data(), recs.data(), mh.data(), *go);
     }
     return GPMPC_OK;
 }
@@ -2248,6 +2288,102 @@ rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restr
 // At t = 0 the tangents are the unit columns of z0 and zero covariance (nothing is read).  Each warp owns one column at a
 // time and rewrites it in place; every sum runs in index order in one thread, so a trajectory's bits do not depend on B.
 // Dynamic shared memory: J (Ny Nx) | x~ (Ny) | C K^T (Ny Nu) | K C (Nu Ny) | per warp [dz (Nx) | dm (Ny) | dC (Ny Ny) | T (Ny Nx)].
+//
+// The two stages every tangent kernel shares.  tangent_policy: per trajectory, before its columns, x~ = x - x_ref (feedback,
+// unless last) and, with Sigma tangents (sig), C K^T and K C; cov_t is the trajectory's.
+__device__ __forceinline__ void tangent_policy(int Ny, int Nu, int b, bool fb_next, bool sig, const double* __restrict__ mean_t,
+                                               const double* __restrict__ cov_t, const double* __restrict__ scale,
+                                               const double* __restrict__ K, const double* __restrict__ x_ref,
+                                               double* xt, double* CKt, double* KC)
+{
+    const int tid = threadIdx.x;
+    if (fb_next) {
+        for (int k = tid; k < Ny; k += blockDim.x) {
+            const double m = mean_t[(size_t)b * Ny + k];
+            const double x = scale ? m * scale[k] + scale[Ny + k] : m;
+            xt[k] = x_ref ? x - x_ref[k] : x;
+        }
+        if (sig)
+            for (int idx = tid; idx < Ny * Nu; idx += blockDim.x) {
+                const int r = idx / Nu, i = idx - r * Nu;
+                double s1 = 0.0, s2 = 0.0;
+                for (int k = 0; k < Ny; ++k) {
+                    s1 = fma(cov_t[r * Ny + k], K[i * Ny + k], s1);      // (C K^T)[r][i]
+                    s2 = fma(K[i * Ny + k], cov_t[k * Ny + r], s2);      // (K C)[i][r]
+                }
+                CKt[idx] = s1; KC[i * Ny + r] = s2;
+            }
+    }
+}
+
+// tangent_column: one warp's column p after dm (wm) and dC (wC) are formed: dmeans_t, dvars_t and, unless last, the next
+// tangents dz into z and, with Sigma tangents (sig), dSigma into S, with wT (at least Nu Ny) as scratch for K dC.
+__device__ __forceinline__ void tangent_column(int Ny, int Nu, int P, int t, int p, int b, int first, int last, bool sig,
+                                               const double* wm, const double* wC, double* wT, const double* xt,
+                                               const double* CKt, const double* KC, const double* __restrict__ cov_t,
+                                               const double* __restrict__ scale, const double* __restrict__ K,
+                                               const double* __restrict__ uscale, double* __restrict__ z,
+                                               double* __restrict__ S, double* __restrict__ dmeans_t,
+                                               double* __restrict__ dvars_t)
+{
+    const int Nx = Ny + Nu, lane = threadIdx.x & 31;
+    const bool fb = K != nullptr;
+    for (int a = lane; a < Ny; a += 32) {
+        dmeans_t[((size_t)b * Ny + a) * P + p] = wm[a];
+        dvars_t[((size_t)b * Ny + a) * P + p] = wC[a * Ny + a];
+    }
+    if (!last) {
+        // the entry of K this column stands for (ki, kk), or -1
+        const int q = p - Nx, ki = (fb && q >= 0) ? q / Ny : -1, kk = (fb && q >= 0) ? q - ki * Ny : -1;
+        for (int j = lane; j < Nx; j += 32) {
+            double d;
+            if (j < Ny) {
+                d = wm[j];
+                if (scale) d = d * scale[j] / scale[3 * Ny + j];
+            } else if (!fb) {
+                d = (p == Nx + t * Nu + (j - Ny)) ? 1.0 : 0.0;
+            } else {
+                const int i = j - Ny;
+                d = 0.0;
+                for (int k = 0; k < Ny; ++k) d = fma(K[i * Ny + k], scale ? wm[k] * scale[k] : wm[k], d);
+                if (i == ki) d += xt[kk];
+                if (uscale) d = d / uscale[Nu + i];
+            }
+            z[j] = d;
+        }
+        if (sig) {
+            if (fb)
+                for (int idx = lane; idx < Nu * Ny; idx += 32) {     // K dC, into T (read only above this point)
+                    const int i = idx / Ny, c = idx - i * Ny;
+                    double s = 0.0;
+                    for (int k = 0; k < Ny; ++k) s = fma(K[i * Ny + k], wC[k * Ny + c], s);
+                    wT[idx] = s;
+                }
+            __syncwarp();
+            for (int idx = lane; idx < Nx * Nx; idx += 32) {
+                const int r = idx / Nx, c = idx - r * Nx;
+                if (r < Ny && c < Ny) { S[idx] = wC[r * Ny + c]; continue; }
+                if (!fb) {                                           // u blocks kept (zero at the start)
+                    if (first) S[idx] = 0.0;
+                    continue;
+                }
+                double s = 0.0;
+                if (r < Ny || c < Ny) {                              // dS_xu[x][i] = (dC K^T + C dK^T)[x][i], dS_ux its transpose
+                    const int x = r < Ny ? r : c, i = (r < Ny ? c : r) - Ny;
+                    for (int k = 0; k < Ny; ++k) s = fma(wC[x * Ny + k], K[i * Ny + k], s);
+                    if (i == ki) s += cov_t[x * Ny + kk];
+                } else {                                             // dS_uu[i][j]
+                    const int i = r - Ny, j = c - Ny;
+                    for (int k = 0; k < Ny; ++k) s = fma(wT[i * Ny + k], K[j * Ny + k], s);
+                    if (i == ki) s += CKt[kk * Nu + j];
+                    if (j == ki) s += KC[i * Ny + kk];
+                }
+                S[idx] = s;
+            }
+        }
+    }
+}
+
 __global__ void __launch_bounds__(256, 2)
 rollout_tangent_kernel(int Ny, int Nu, int P, int t, int first, int last, int method_ta,
                        const double* __restrict__ J, const double* __restrict__ dvar, const double* __restrict__ dcov,
@@ -2270,23 +2406,7 @@ rollout_tangent_kernel(int Ny, int Nu, int P, int t, int first, int last, int me
     J += (size_t)b * Ny * Nx;
     cov_t += (size_t)b * Ny * Ny;
     for (int i = tid; i < Ny * Nx; i += blockDim.x) sJ[i] = J[i];
-    if (fb && !last) {
-        for (int k = tid; k < Ny; k += blockDim.x) {
-            const double m = mean_t[(size_t)b * Ny + k];
-            const double x = scale ? m * scale[k] + scale[Ny + k] : m;
-            xt[k] = x_ref ? x - x_ref[k] : x;
-        }
-        if (method_ta)
-            for (int idx = tid; idx < Ny * Nu; idx += blockDim.x) {
-                const int r = idx / Nu, i = idx - r * Nu;
-                double s1 = 0.0, s2 = 0.0;
-                for (int k = 0; k < Ny; ++k) {
-                    s1 = fma(cov_t[r * Ny + k], K[i * Ny + k], s1);      // (C K^T)[r][i]
-                    s2 = fma(K[i * Ny + k], cov_t[k * Ny + r], s2);      // (K C)[i][r]
-                }
-                CKt[idx] = s1; KC[i * Ny + r] = s2;
-            }
-    }
+    tangent_policy(Ny, Nu, b, fb && !last, method_ta, mean_t, cov_t, scale, K, x_ref, xt, CKt, KC);
     __syncthreads();
     const double* dcv = dcov + (size_t)b * Ny * Ny * Nx;
     const double* dvr = dvar + (size_t)b * Ny * Nx;
@@ -2324,60 +2444,80 @@ rollout_tangent_kernel(int Ny, int Nu, int P, int t, int first, int last, int me
             wC[idx] = s;
         }
         __syncwarp();
+        tangent_column(Ny, Nu, P, t, p, b, first, last, method_ta, wm, wC, wT, xt, CKt, KC, cov_t, scale, K, uscale, z, S,
+                       dmeans_t, dvars_t);
+        __syncwarp();
+    }
+}
+
+// Forward-mode tangents of one 'EM' roll-out step (gpmpc_rollout_batch_em_grad), one CTA per trajectory b: the parameters,
+// tangent slabs (dS always: the 'EM' mean depends on Sigma), outputs and next tangents of rollout_tangent_kernel.  Step t
+// reads gpmpc_predict_em_grad's blocks at (z_t, Sigma_t), per trajectory dmz (Ny,Nx), dmS (Ny,Nx,Nx), dcz (Ny,Ny,Nx) and
+// dcS (Ny,Ny,Nx,Nx), and forms per parameter
+//   dm = dmz dz + sum_{d,e} dmS[., d, e] dS[d, e],   dC = dcz dz + sum_{d,e} dcS[., ., d, e] dS[d, e]
+// over all Nx^2 entries of the symmetric dS: the blocks hold every other entry fixed, so this is the directional derivative.
+// At t = 0 dS is zero and is not read.  dmz and the column's dS are staged in shared memory; dmS and dcS are read from global
+// memory (Ny^2 Nx^2 doubles a trajectory do not fit at Nx = 32).  Every sum runs in index order in one thread.
+// Dynamic shared memory: dmz (Ny Nx) | x~ (Ny) | C K^T (Ny Nu) | K C (Nu Ny) | per warp [dz (Nx) | dm (Ny) | dC (Ny Ny) |
+// K dC (Nu Ny) | dS (Nx Nx)].
+__global__ void __launch_bounds__(256, 2)
+rollout_tangent_em_kernel(int Ny, int Nu, int P, int t, int first, int last,
+                          const double* __restrict__ dmz, const double* __restrict__ dmS, const double* __restrict__ dcz,
+                          const double* __restrict__ dcS, const double* __restrict__ mean_t, const double* __restrict__ cov_t,
+                          const double* __restrict__ scale, const double* __restrict__ K, const double* __restrict__ x_ref,
+                          const double* __restrict__ uscale, double* __restrict__ dZ, double* __restrict__ dS,
+                          double* __restrict__ dmeans_t, double* __restrict__ dvars_t)
+{
+    extern __shared__ double tg_sh[];
+    const int Nx = Ny + Nu, nn = Nx * Nx, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+    const int b = blockIdx.x;
+    double* sG = tg_sh;
+    double* xt = sG + Ny * Nx;
+    double* CKt = xt + Ny;
+    double* KC = CKt + Ny * Nu;
+    const int per_warp = Nx + Ny + Ny * Ny + Nu * Ny + nn;
+    double* wz = KC + Nu * Ny + warp * per_warp;
+    double* wm = wz + Nx;
+    double* wC = wm + Ny;
+    double* wT = wC + Ny * Ny;
+    double* wS = wT + Nu * Ny;
+    dmz += (size_t)b * Ny * Nx;
+    dmS += (size_t)b * Ny * nn;
+    dcz += (size_t)b * Ny * Ny * Nx;
+    dcS += (size_t)b * Ny * Ny * nn;
+    cov_t += (size_t)b * Ny * Ny;
+    for (int i = tid; i < Ny * Nx; i += blockDim.x) sG[i] = dmz[i];
+    tangent_policy(Ny, Nu, b, K != nullptr && !last, true, mean_t, cov_t, scale, K, x_ref, xt, CKt, KC);
+    __syncthreads();
+    for (int p = warp; p < P; p += nwarps) {
+        double* z = dZ + ((size_t)b * P + p) * Nx;
+        double* S = dS + ((size_t)b * P + p) * nn;
+        for (int e = lane; e < Nx; e += 32) wz[e] = first ? (e == p ? 1.0 : 0.0) : z[e];
+        if (!first)
+            for (int q = lane; q < nn; q += 32) wS[q] = S[q];
+        __syncwarp();
         for (int a = lane; a < Ny; a += 32) {
-            dmeans_t[((size_t)b * Ny + a) * P + p] = wm[a];
-            dvars_t[((size_t)b * Ny + a) * P + p] = wC[a * Ny + a];
-        }
-        if (!last) {
-            // the entry of K this column stands for (ki, kk), or -1
-            const int q = p - Nx, ki = (fb && q >= 0) ? q / Ny : -1, kk = (fb && q >= 0) ? q - ki * Ny : -1;
-            for (int j = lane; j < Nx; j += 32) {
-                double d;
-                if (j < Ny) {
-                    d = wm[j];
-                    if (scale) d = d * scale[j] / scale[3 * Ny + j];
-                } else if (!fb) {
-                    d = (p == Nx + t * Nu + (j - Ny)) ? 1.0 : 0.0;
-                } else {
-                    const int i = j - Ny;
-                    d = 0.0;
-                    for (int k = 0; k < Ny; ++k) d = fma(K[i * Ny + k], scale ? wm[k] * scale[k] : wm[k], d);
-                    if (i == ki) d += xt[kk];
-                    if (uscale) d = d / uscale[Nu + i];
-                }
-                z[j] = d;
+            double s = 0.0;
+            for (int e = 0; e < Nx; ++e) s = fma(sG[a * Nx + e], wz[e], s);
+            if (!first) {
+                const double* g = dmS + (size_t)a * nn;
+                for (int q = 0; q < nn; ++q) s = fma(g[q], wS[q], s);
             }
-            if (method_ta) {
-                if (fb)
-                    for (int idx = lane; idx < Nu * Ny; idx += 32) {     // K dC, into T (read only above this point)
-                        const int i = idx / Ny, c = idx - i * Ny;
-                        double s = 0.0;
-                        for (int k = 0; k < Ny; ++k) s = fma(K[i * Ny + k], wC[k * Ny + c], s);
-                        wT[idx] = s;
-                    }
-                __syncwarp();
-                for (int idx = lane; idx < Nx * Nx; idx += 32) {
-                    const int r = idx / Nx, c = idx - r * Nx;
-                    if (r < Ny && c < Ny) { S[idx] = wC[r * Ny + c]; continue; }
-                    if (!fb) {                                           // u blocks kept (zero at the start)
-                        if (first) S[idx] = 0.0;
-                        continue;
-                    }
-                    double s = 0.0;
-                    if (r < Ny || c < Ny) {                              // dS_xu[x][i] = (dC K^T + C dK^T)[x][i], dS_ux its transpose
-                        const int x = r < Ny ? r : c, i = (r < Ny ? c : r) - Ny;
-                        for (int k = 0; k < Ny; ++k) s = fma(wC[x * Ny + k], K[i * Ny + k], s);
-                        if (i == ki) s += cov_t[x * Ny + kk];
-                    } else {                                             // dS_uu[i][j]
-                        const int i = r - Ny, j = c - Ny;
-                        for (int k = 0; k < Ny; ++k) s = fma(wT[i * Ny + k], K[j * Ny + k], s);
-                        if (i == ki) s += CKt[kk * Nu + j];
-                        if (j == ki) s += KC[i * Ny + kk];
-                    }
-                    S[idx] = s;
-                }
-            }
+            wm[a] = s;
         }
+        for (int idx = lane; idx < Ny * Ny; idx += 32) {
+            const double* gz = dcz + (size_t)idx * Nx;
+            double s = 0.0;
+            for (int e = 0; e < Nx; ++e) s = fma(gz[e], wz[e], s);
+            if (!first) {
+                const double* g = dcS + (size_t)idx * nn;
+                for (int q = 0; q < nn; ++q) s = fma(g[q], wS[q], s);
+            }
+            wC[idx] = s;
+        }
+        __syncwarp();
+        tangent_column(Ny, Nu, P, t, p, b, first, last, true, wm, wC, wT, xt, CKt, KC, cov_t, scale, K, uscale, z, S,
+                       dmeans_t, dvars_t);
         __syncwarp();
     }
 }
@@ -2438,8 +2578,8 @@ static void rows_by_trajectory(double* dst, const double* src, int B, int Nt, si
             memcpy(dst + (b * Nt + t) * n, src + ((size_t)t * B + b) * n, n * 8);
 }
 
-// gpmpc_rollout_batch, gpmpc_rollout, with tg gpmpc_rollout_batch_grad and with em_entry gpmpc_rollout_batch_em (the one
-// entry that takes 'EM'); fn names the entry in errors
+// gpmpc_rollout_batch, gpmpc_rollout, with tg gpmpc_rollout_batch_grad and with em_entry gpmpc_rollout_batch_em (the
+// entries that take 'EM'; with tg gpmpc_rollout_batch_em_grad); fn names the entry in errors
 static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, int Nt, const double* z0, const double* U,
                          const double* Sigma0, const double* scale, const double* K, const double* x_ref,
                          const double* uscale, double* means, double* vars, double* cov_last, const RolloutTangents* tg = nullptr,
@@ -2463,18 +2603,23 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
     const size_t o_m = rollout_policy(B, Nt, Ny, Nu, U, scale, K, x_ref, uscale, o_u);
     const size_t o_v = o_m + (size_t)Nt * Bs * Ny, o_c = o_v + (size_t)Nt * Bs * Ny, tot = o_c + (size_t)Nt * Bs * Ny * Ny;
     ENSURE(h->dRoll, tot);
-    // tangent slab: [dZ (B,P,Nx) | dS (B,P,Nx,Nx), 'TA' only | dmeans (Nt,B,Ny,P) | dvars (Nt,B,Ny,P)], the last two mirrored
-    // in the pinned buffer after the roll-out's outputs
+    // tangent slab: [dZ (B,P,Nx) | dS (B,P,Nx,Nx), 'TA' and 'EM' | dmeans (Nt,B,Ny,P) | dvars (Nt,B,Ny,P) | 'EM': the step's
+    // gpmpc_predict_em_grad blocks dmz (B,Ny,Nx) | dmS (B,Ny,Nx,Nx) | dcz (B,Ny,Ny,Nx) | dcS (B,Ny,Ny,Nx,Nx)], dmeans and
+    // dvars mirrored in the pinned buffer after the roll-out's outputs
+    const size_t nn = (size_t)Nx * Nx;
     const size_t P = !tg ? 0 : Nx + (K ? (size_t)Nu * Ny : (size_t)(Nt - 1) * Nu);
-    const size_t o_ds = Bs * P * Nx, o_dm = o_ds + (method == GPMPC_METHOD_TA ? Bs * P * Nx * Nx : 0);
-    const size_t o_dv = o_dm + (size_t)Nt * Bs * Ny * P, tg_tot = o_dv + (size_t)Nt * Bs * Ny * P;
+    const size_t o_ds = Bs * P * Nx, o_dm = o_ds + (method != GPMPC_METHOD_ME ? Bs * P * nn : 0);
+    const size_t o_dv = o_dm + (size_t)Nt * Bs * Ny * P, o_g = o_dv + (size_t)Nt * Bs * Ny * P;
+    const size_t n_mz = Bs * Ny * Nx, n_mS = Bs * Ny * nn, n_cz = Bs * Ny * Ny * Nx, n_g = em ? n_mz + n_mS + n_cz + n_cz * Nx : 0;
     DerivSlabs ds;
     if (tg) {
-        rc = derivs_prepare(h, B, false, &ds);
-        if (rc) return rc;
-        ENSURE(h->dRollTg, tg_tot);
+        if (!em) {
+            rc = derivs_prepare(h, B, false, &ds);
+            if (rc) return rc;
+        }
+        ENSURE(h->dRollTg, o_g + n_g);
     }
-    rc = ensure_pinned(h, (tot + (tg ? tg_tot - o_dm : 0)) * 8);
+    rc = ensure_pinned(h, (tot + (tg ? o_g - o_dm : 0)) * 8);
     if (rc) return rc;
     double* pin = h->hPinned;
     memcpy(pin, z0, Bs * Nx * 8);
@@ -2490,7 +2635,16 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
         rc = em_scratch(h, nc, B);
         if (rc) return rc;
     }
-    std::vector<double> emp(Bs * per);
+    // 'EM' tangents: the D = 2 records of the B points of a step, K^-1, and the host side of gpmpc_predict_em_grad's finish
+    if (em && tg) {
+        rc = em_records_prepare(h, 2, B);
+        if (rc) return rc;
+        rc = em_kinv_prepare(h);
+        if (rc) return rc;
+    }
+    const size_t rl = em && tg ? (size_t)h->em_rec[0].tb->nrec(Ny) * h->em_rec[0].tb->nent : 0;
+    std::vector<double> emp(Bs * per), recs(Bs * rl), mh(em && tg ? Bs * Ny : 0), hg(n_g);
+    const EmGradOutputs hgo = {hg.data(), hg.data() + n_mz, hg.data() + n_mz + n_mS, hg.data() + n_mz + n_mS + n_cz};
     const int fb_smem = K ? (Ny + Nu * Ny) * 8 : 0;
     for (int t = 0; t < Nt; ++t) {
         double* mean_t = d + o_m + (size_t)t * Bs * Ny;
@@ -2518,23 +2672,58 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
             CUDA_TRY(cudaMemcpyAsync(h->dEMP, emp.data(), emp.size() * 8, cudaMemcpyHostToDevice, h->st));
             for (int b0 = 0; b0 < B; b0 += nc) {
                 const size_t o = (size_t)b0;
-                rc = em_forward(h, std::min(nc, B - b0), d + o * Nx, h->dEMP + o * per, mean_t + o * Ny, var_t + o * Ny,
-                                cov_t + o * Ny * Ny);
+                const int n = std::min(nc, B - b0);
+                rc = em_forward(h, n, d + o * Nx, h->dEMP + o * per, mean_t + o * Ny, var_t + o * Ny, cov_t + o * Ny * Ny);
                 if (rc) return rc;
+                if (tg) {                         // the chunk's records, from the scratch slots its forward left
+                    rc = em_chunk_records(h, n, d + o * Nx, h->dEMP + o * per, h->em_rec[0].rec + o * rl, nullptr);
+                    if (rc) return rc;
+                }
+            }
+            if (tg) {
+                // gpmpc_predict_em_grad's finish at (z_t, Sigma_t): records and means to the host (the step's second
+                // synchronisation), em_grad_finish per point with the Sigma_t and em_prepare_point blocks held here, the four
+                // blocks back to the device
+                CUDA_TRY(cudaMemcpyAsync(recs.data(), h->em_rec[0].rec, recs.size() * 8, cudaMemcpyDeviceToHost, h->st));
+                CUDA_TRY(cudaMemcpyAsync(mh.data(), mean_t, mh.size() * 8, cudaMemcpyDeviceToHost, h->st));
+                CUDA_TRY(cudaStreamSynchronize(h->st));
+                int bad = 0;
+                rc = em_grad_finish_points(h, B, pin + o_sig, 1, emp.data(), recs.data(), mh.data(), hgo, &bad);
+                if (rc) {
+                    char why[512];
+                    snprintf(why, sizeof(why), "%s", h->err);
+                    set_error(h, "%s: step %d, trajectory %d: %s", fn, t, bad, why);
+                    return rc;
+                }
+                CUDA_TRY(cudaMemcpyAsync(h->dRollTg + o_g, hg.data(), hg.size() * 8, cudaMemcpyHostToDevice, h->st));
             }
         }
-        if (tg) {                                 // J_t, dvar_t, dcov_t at the same points, then the step's tangents
-            rc = derivs_enqueue(h, method, B, d, d + o_sig, 1, ds);
-            if (rc) return rc;
-            const int nw = 8, per_warp = Nx + Ny + Ny * Ny + Ny * Nx;
-            const int tg_smem = (Ny * Nx + Ny + 2 * Ny * Nu + nw * per_warp) * 8;
-            // largest layout: Ny = Nx = NX_MAX for J and the warps, Ny = Nu = NX_MAX / 2 for C K^T and K C
-            CUDA_TRY(smem_opt_in<rollout_tangent_kernel>((NX_MAX * NX_MAX + NX_MAX + NX_MAX * NX_MAX / 2 + nw * (2 * NX_MAX + 2 * NX_MAX * NX_MAX)) * 8));
+        if (tg) {                                 // the step's derivatives at the same points, then its tangents
+            const int nw = 8;
+            // largest layout: Ny = Nx = NX_MAX for J and the warps, Ny = Nu = NX_MAX / 2 for C K^T and K C (either kernel)
+            const int smem_max = (NX_MAX * NX_MAX + NX_MAX + NX_MAX * NX_MAX / 2 + nw * (2 * NX_MAX + 2 * NX_MAX * NX_MAX)) * 8;
             double* g = h->dRollTg;
-            rollout_tangent_kernel<<<B, nw * 32, tg_smem, h->st>>>(Ny, Nu, (int)P, t, t == 0, t + 1 == Nt, method == GPMPC_METHOD_TA,
-                                                                  h->dJ, ds.dvar, ds.dcov, mean_t, cov_t,
-                                                                  pol.scale, pol.K, pol.x_ref, pol.uscale, g, g + o_ds, g + o_dm + (size_t)t * Bs * Ny * P,
-                                                                  g + o_dv + (size_t)t * Bs * Ny * P);
+            if (!em) {                            // J_t, dvar_t, dcov_t
+                rc = derivs_enqueue(h, method, B, d, d + o_sig, 1, ds);
+                if (rc) return rc;
+                const int per_warp = Nx + Ny + Ny * Ny + Ny * Nx;
+                const int tg_smem = (Ny * Nx + Ny + 2 * Ny * Nu + nw * per_warp) * 8;
+                CUDA_TRY(smem_opt_in<rollout_tangent_kernel>(smem_max));
+                rollout_tangent_kernel<<<B, nw * 32, tg_smem, h->st>>>(Ny, Nu, (int)P, t, t == 0, t + 1 == Nt, method == GPMPC_METHOD_TA,
+                                                                      h->dJ, ds.dvar, ds.dcov, mean_t, cov_t,
+                                                                      pol.scale, pol.K, pol.x_ref, pol.uscale, g, g + o_ds, g + o_dm + (size_t)t * Bs * Ny * P,
+                                                                      g + o_dv + (size_t)t * Bs * Ny * P);
+            } else {
+                const int per_warp = Nx + Ny + Ny * Ny + Nu * Ny + Nx * Nx;
+                const int tg_smem = (Ny * Nx + Ny + 2 * Ny * Nu + nw * per_warp) * 8;
+                CUDA_TRY(smem_opt_in<rollout_tangent_em_kernel>(smem_max));
+                const double* G = g + o_g;
+                rollout_tangent_em_kernel<<<B, nw * 32, tg_smem, h->st>>>(Ny, Nu, (int)P, t, t == 0, t + 1 == Nt, G, G + n_mz,
+                                                                         G + n_mz + n_mS, G + n_mz + n_mS + n_cz, mean_t, cov_t,
+                                                                         pol.scale, pol.K, pol.x_ref, pol.uscale, g, g + o_ds,
+                                                                         g + o_dm + (size_t)t * Bs * Ny * P,
+                                                                         g + o_dv + (size_t)t * Bs * Ny * P);
+            }
             CUDA_TRY(cudaGetLastError());
         }
         if (t + 1 < Nt) {
@@ -2545,7 +2734,7 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
         }
     }
     CUDA_TRY(cudaMemcpyAsync(pin + o_m, d + o_m, (tot - o_m) * 8, cudaMemcpyDeviceToHost, h->st));
-    if (tg) CUDA_TRY(cudaMemcpyAsync(pin + tot, h->dRollTg + o_dm, (tg_tot - o_dm) * 8, cudaMemcpyDeviceToHost, h->st));
+    if (tg) CUDA_TRY(cudaMemcpyAsync(pin + tot, h->dRollTg + o_dm, (o_g - o_dm) * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
     // (t, b) -> (b, t); the reference records diag(covar_x) of every step (gp_class.py:793): the propagated variance, J Sigma J^T included
     rows_by_trajectory(means, pin + o_m, B, Nt, Ny);
@@ -2586,6 +2775,17 @@ extern "C" int gpmpc_rollout_batch_grad(gpmpc_handle_t h, int method, int B, int
 {
     const RolloutTangents tg = {dmeans, dvars};
     return rollout_batch(h, __func__, method, B, Nt, z0, U, Sigma0, scale, K, x_ref, uscale, means, vars, cov_last, &tg);
+}
+
+// gpmpc_rollout_batch_em plus the forward-mode derivatives of gpmpc_rollout_batch_grad (see include/gpmpc.h)
+extern "C" int gpmpc_rollout_batch_em_grad(gpmpc_handle_t h, int B, int Nt, const double* z0, const double* U,
+                                           const double* Sigma0, const double* scale, const double* K, const double* x_ref,
+                                           const double* uscale, double* means, double* vars, double* cov_last,
+                                           double* dmeans, double* dvars)
+{
+    const RolloutTangents tg = {dmeans, dvars};
+    return rollout_batch(h, __func__, GPMPC_METHOD_EM, B, Nt, z0, U, Sigma0, scale, K, x_ref, uscale, means, vars, cov_last,
+                         &tg, true);
 }
 
 // the single open-loop trajectory: B = 1 of the batched loop

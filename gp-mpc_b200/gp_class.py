@@ -703,8 +703,10 @@ class GP:
     def rollout_grad(self, x0, u, method=None, feedback=False, x_ref=None, Q=None, R=None):
         """ ``rollout`` for one method with the exact derivatives of every step's mean and variance w.r.t. what produced
         the trajectory: the start x0 and, open loop, the inputs u, or with feedback=True the gain K.  Forward-mode
-        tangents run on the device beside the roll-out (gpmpc_rollout_batch_grad), so one call replaces the P + 1
-        roll-outs of a difference quotient and carries no truncation error.
+        tangents run on the device beside the roll-out (gpmpc_rollout_batch_grad for 'ME' and 'TA',
+        gpmpc_rollout_batch_em_grad for 'EM'), so one call replaces the P + 1 roll-outs of a difference quotient and carries
+        no truncation error.  'EM' needs an engine with that entry; its tangents carry the input covariance as well, since
+        the exact moment-matched mean depends on it.
 
         Shapes follow ``rollout``: x0:(Ny,) with u:(Nt,Nu), or a batch x0:(B,Ny) with u:(B,Nt,Nu), which adds a leading B
         axis to every array below.  Returns a dict in caller units:
@@ -718,7 +720,8 @@ class GP:
         differentiated, so dmean_dx0 is the derivative of the closed loop under that fixed K, including u_0 = K (x0 - x_ref).
         method defaults to the GP's gp_method. """
         meth = self.__gp_method if method is None else method
-        if meth not in ('ME', 'TA'):
+        eng = self.__engine
+        if not (meth in ('ME', 'TA') or (meth == 'EM' and hasattr(eng, 'rollout_batch_em_grad'))):
             raise NotImplementedError("rollout_grad differentiates gp_method 'ME' and 'TA' (got %r)" % (meth,))
         if self.__comm.world > 1:
             raise NotImplementedError('rollout_grad needs all outputs on one GPU (build the GP with a single-process Comm)')
@@ -736,13 +739,15 @@ class GP:
         covar = self.__initial_covar(nb)
         z0, Ug, scale, uscale = self.__engine_start(X0, U, K, x_ref)
         sX, sU, sY = (self.__stdX, self.__stdU, self.__stdY) if self.__normalize else (np.ones(Ny), np.ones(Nu), np.ones(Ny))
-        method_id, eng = _GPU_METHODS[meth], self.__engine
         P = Nx + (Nu * Ny if K is not None else (Nt - 1) * Nu)
         m_std = np.empty((nb, Nt, Ny)); v_std = np.empty((nb, Nt, Ny))
         Dm = np.empty((nb, Nt, Ny, P)); Dv = np.empty((nb, Nt, Ny, P))
         for g, Kg in self.__gain_groups(K, nb):
-            m_std[g], v_std[g], _, Dm[g], Dv[g] = eng.rollout_batch_grad(z0[g], Ug[g], covar[g], method_id, scale, Kg, x_ref,
-                                                                         uscale)
+            if meth == 'EM':
+                r = eng.rollout_batch_em_grad(z0[g], Ug[g], covar[g], scale, Kg, x_ref, uscale)
+            else:
+                r = eng.rollout_batch_grad(z0[g], Ug[g], covar[g], _GPU_METHODS[meth], scale, Kg, x_ref, uscale)
+            m_std[g], v_std[g], _, Dm[g], Dv[g] = r
         # caller units: mean = m stdY + meanY, var = v stdY^2; z0 = [(x0 - meanX) / stdX, (u_0 - meanU) / stdU]
         Dm = Dm * sY[None, None, :, None]
         Dv = Dv * (sY ** 2)[None, None, :, None]

@@ -342,6 +342,29 @@ int gpmpc_rollout_batch_grad(gpmpc_handle_t h, int method, int B, int Nt, const 
                              const double* uscale, double* means, double* vars, double* cov_last,
                              double* dmeans, double* dvars);
 
+/* gpmpc_rollout_batch_em plus the exact derivatives of every step's mean and variance: the 'EM' counterpart of
+ * gpmpc_rollout_batch_grad.  Arguments as gpmpc_rollout_batch_em; means, vars, cov_last are bit-identical to its.  dmeans,
+ * dvars (B, Nt, Ny, P), both required, have gpmpc_rollout_batch_grad's shapes, parameter columns (z0[b], then U rows
+ * 1..Nt-1 open loop or K row-major with feedback), units and next-tangent rules.  Sigma0, scale, x_ref and uscale are held
+ * fixed.  Per parameter, step t takes the four blocks of gpmpc_predict_em_grad at (z_t, Sigma_t), bit-identical to that
+ * entry's at the same inputs, and forms
+ *   dm = dmean_dz dz + sum_{d,e} dmean_dSigma[., d, e] dSigma[d, e],  dC = dcov_dz dz + sum_{d,e} dcov_dSigma[., ., d, e] dSigma[d, e]
+ * summed over all Nx^2 entries of the symmetric dSigma (the blocks hold every other entry fixed, so this is the directional
+ * derivative); dvars = diag(dC).  Unlike 'TA' the mean depends on Sigma, so Sigma tangents are carried in open loop too.
+ * Each step synchronises twice: once to bring Sigma_t to the host (as gpmpc_rollout_batch_em) and once to bring the
+ * step's derivative records and means there, where the derivatives are finished as gpmpc_predict_em_grad finishes them.
+ * Every sum runs in a fixed order: trajectory b's results do not depend on B, its row or gpmpc_set_option("em_points").
+ * GPMPC_ERR_ARG: every argument error of gpmpc_rollout_batch_em, or dmeans / dvars NULL, checked before any work; Sigma +
+ * Lambda not positive definite at step t (gpmpc_last_error names t and the trajectory; the outputs are then undefined and
+ * the handle stays usable).  GPMPC_ERR_STATE: not factorised, or the handle does not own every output.  Device memory
+ * beyond gpmpc_rollout_batch_em's: the full symmetric K^-1 per output of gpmpc_predict_em_grad (8 B Ny Npad^2, kept until
+ * the next factor change; 17 GB at N = 16384, Ny = 8), that entry's D = 2 records of B points, 8 B P (Nx + Nx^2) bytes of
+ * tangents, 8 B (Ny Nx + Ny Nx^2 + Ny^2 Nx + Ny^2 Nx^2) bytes of derivative blocks and 16 Nt B Ny P bytes of outputs. */
+int gpmpc_rollout_batch_em_grad(gpmpc_handle_t h, int B, int Nt, const double* z0, const double* U,
+                                const double* Sigma0, const double* scale, const double* K, const double* x_ref,
+                                const double* uscale, double* means, double* vars, double* cov_last,
+                                double* dmeans, double* dvars);
+
 /* Sample trajectories of the learned dynamics: each of the B trajectories is one draw f of the GP posterior, evaluated along
  * the inputs that draw visits.  Per output a and step t, f_t(z_t) is drawn conditioned on the values the same draw took
  * at the earlier points z_0 .. z_{t-1} of the trajectory, so the whole trajectory satisfies f - m = R eps with R the
