@@ -56,6 +56,7 @@ SYMBOLS = [
     ('gpmpc_rollout_batch_em', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 10),
     ('gpmpc_rollout_batch_em_grad', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 12),
     ('gpmpc_rollout_sample', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 10 + [_ip]),
+    ('gpmpc_rollout_sample_grad', C.c_int, [_H, C.c_int, C.c_int] + [_dp] * 10 + [_ip, _dp]),
     ('gpmpc_predict_device', C.c_int, [_H, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     ('gpmpc_get', C.c_int, [_H, C.c_int, C.c_int, _dp]),
@@ -404,6 +405,27 @@ class Engine:
                                                   _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(samples), _ptr(z_out),
                                                   kept.ctypes.data_as(_ip)))
         return samples, z_out, kept
+
+    def rollout_sample_grad(self, z0, U, eps, xi=None, scale=None, K=None, x_ref=None, uscale=None):
+        """gpmpc_rollout_sample_grad: rollout_sample's arguments and outputs (bit for bit) plus dsamples (B,Nt,Ny,P), the
+        derivatives of every draw (GP output units) with eps and xi held fixed, w.r.t. rollout_batch_grad's P parameters
+        [z0[b] | U[b,1:] row-major] open loop or [z0[b] | K row-major] with K."""
+        Nu = self.Nx - self.Ny
+        z0 = _f64(z0).reshape(-1, self.Nx)
+        B = z0.shape[0]
+        eps = _f64(eps)
+        Nt = int(eps.shape[1])
+        eps = eps.reshape(B, Nt, self.Ny)
+        xi = None if xi is None else _f64(xi, (B, Nt, self.Ny))
+        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
+        P = self.Nx + (Nu * self.Ny if K is not None else (Nt - 1) * Nu)
+        samples = np.empty((B, Nt, self.Ny)); z_out = np.empty((B, Nt, self.Nx))
+        kept = np.empty((B, Nt, self.Ny), dtype=np.int32)
+        dsamples = np.empty((B, Nt, self.Ny, P))
+        self._check(self.lib.gpmpc_rollout_sample_grad(self.h, B, Nt, _ptr(z0), _ptr(U), _ptr(eps), _ptr(xi), _ptr(scale),
+                                                       _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(samples), _ptr(z_out),
+                                                       kept.ctypes.data_as(_ip), _ptr(dsamples)))
+        return samples, z_out, kept, dsamples
 
     def predict_grad(self, Z, Sigma=None, method=METHOD_TA, want_hess=False):
         """Predict + first derivatives w.r.t. the test inputs (gpmpc_predict_grad).

@@ -180,6 +180,8 @@ struct gpmpc_handle_s {
     DevBuf<double> dRollTg;           // gpmpc_rollout_batch_grad, _em_grad: [dZ | dSigma ('TA', 'EM') | dmeans | dvars | 'EM' blocks]
     DevBuf<double> dSmV;              // gpmpc_rollout_sample: V rows of every step (nloc, Nt, B, Npad)
     DevBuf<double> dSmp;              //   [eps | xi | U | scale | K | x_ref | uscale | Z (Nt,B,Nx) | samples | kept | m | R]
+    DevBuf<double> dSmB;              // gpmpc_rollout_sample_grad: beta rows of every step (nloc, Nt, B, Npad)
+    DevBuf<double> dSmTg;             //   [G (nloc,B,Nt,2,Nx) | dR (nloc,B,P,Nt,Nt) | dz (Nt,B,P,Nx) | dsamples (Nt,B,Ny,P)]
     DevBuf<double> dIn, dOut;         // [Z | Sigma] and [mean | var | J | cov] slabs: one H2D + one D2H per host call
     int Hcap = 0;                     // test points the slab layout behind dZ .. dCov holds (0: not laid out)
     double* hPinned = nullptr; double* dPinnedAlias = nullptr; size_t hPinnedBytes = 0;
@@ -2316,6 +2318,35 @@ __device__ __forceinline__ void tangent_policy(int Ny, int Nu, int b, bool fb_ne
     }
 }
 
+// tangent_next_z: one warp's next input tangent z of column p from step t's output tangent wm (dm, or df of a draw) and,
+// with K, x~ of tangent_policy: dz[:Ny] = wm stdY / stdX; open loop the unit tangent of U[t+1]; with K
+// du = (K dx + dK x~) / stdU.
+__device__ __forceinline__ void tangent_next_z(int Ny, int Nu, int t, int p, const double* wm, const double* xt,
+                                               const double* __restrict__ scale, const double* __restrict__ K,
+                                               const double* __restrict__ uscale, double* __restrict__ z)
+{
+    const int Nx = Ny + Nu, lane = threadIdx.x & 31;
+    const bool fb = K != nullptr;
+    // the entry of K this column stands for (ki, kk), or -1
+    const int q = p - Nx, ki = (fb && q >= 0) ? q / Ny : -1, kk = (fb && q >= 0) ? q - ki * Ny : -1;
+    for (int j = lane; j < Nx; j += 32) {
+        double d;
+        if (j < Ny) {
+            d = wm[j];
+            if (scale) d = d * scale[j] / scale[3 * Ny + j];
+        } else if (!fb) {
+            d = (p == Nx + t * Nu + (j - Ny)) ? 1.0 : 0.0;
+        } else {
+            const int i = j - Ny;
+            d = 0.0;
+            for (int k = 0; k < Ny; ++k) d = fma(K[i * Ny + k], scale ? wm[k] * scale[k] : wm[k], d);
+            if (i == ki) d += xt[kk];
+            if (uscale) d = d / uscale[Nu + i];
+        }
+        z[j] = d;
+    }
+}
+
 // tangent_column: one warp's column p after dm (wm) and dC (wC) are formed: dmeans_t, dvars_t and, unless last, the next
 // tangents dz into z and, with Sigma tangents (sig), dSigma into S, with wT (at least Nu Ny) as scratch for K dC.
 __device__ __forceinline__ void tangent_column(int Ny, int Nu, int P, int t, int p, int b, int first, int last, bool sig,
@@ -2335,22 +2366,7 @@ __device__ __forceinline__ void tangent_column(int Ny, int Nu, int P, int t, int
     if (!last) {
         // the entry of K this column stands for (ki, kk), or -1
         const int q = p - Nx, ki = (fb && q >= 0) ? q / Ny : -1, kk = (fb && q >= 0) ? q - ki * Ny : -1;
-        for (int j = lane; j < Nx; j += 32) {
-            double d;
-            if (j < Ny) {
-                d = wm[j];
-                if (scale) d = d * scale[j] / scale[3 * Ny + j];
-            } else if (!fb) {
-                d = (p == Nx + t * Nu + (j - Ny)) ? 1.0 : 0.0;
-            } else {
-                const int i = j - Ny;
-                d = 0.0;
-                for (int k = 0; k < Ny; ++k) d = fma(K[i * Ny + k], scale ? wm[k] * scale[k] : wm[k], d);
-                if (i == ki) d += xt[kk];
-                if (uscale) d = d / uscale[Nu + i];
-            }
-            z[j] = d;
-        }
+        tangent_next_z(Ny, Nu, t, p, wm, xt, scale, K, uscale, z);
         if (sig) {
             if (fb)
                 for (int idx = lane; idx < Nu * Ny; idx += 32) {     // K dC, into T (read only above this point)
@@ -2522,6 +2538,34 @@ rollout_tangent_em_kernel(int Ny, int Nu, int P, int t, int first, int last,
     }
 }
 
+// The input tangents of step t of a sampled roll-out (gpmpc_rollout_sample_grad), one CTA per trajectory b, warps over
+// the P columns: at t = 0 the unit columns of z0, else tangent_next_z of step t-1's draw tangents dsamp_prev (B, Ny, P)
+// with x the draw samp_prev (B, Ny) in place of the mean, as rollout_feedback_kernel forms the next input from it.
+// Writes dZt (B, P, Nx).  Dynamic shared memory: x~ (Ny) | per warp df (Ny).
+__global__ void __launch_bounds__(256, 2)
+sample_next_kernel(int Ny, int Nu, int P, int t, const double* __restrict__ samp_prev, const double* __restrict__ dsamp_prev,
+                   const double* __restrict__ scale, const double* __restrict__ K, const double* __restrict__ x_ref,
+                   const double* __restrict__ uscale, double* __restrict__ dZt)
+{
+    extern __shared__ double sn_sh[];
+    const int Nx = Ny + Nu, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5, b = blockIdx.x;
+    double* xt = sn_sh;
+    double* wm = xt + Ny + warp * Ny;
+    if (t > 0) tangent_policy(Ny, Nu, b, K != nullptr, false, samp_prev, nullptr, scale, K, x_ref, xt, nullptr, nullptr);
+    __syncthreads();
+    for (int p = warp; p < P; p += nwarps) {
+        double* z = dZt + ((size_t)b * P + p) * Nx;
+        if (t == 0) {
+            for (int e = lane; e < Nx; e += 32) z[e] = e == p ? 1.0 : 0.0;
+            continue;
+        }
+        for (int a = lane; a < Ny; a += 32) wm[a] = dsamp_prev[((size_t)b * Ny + a) * P + p];
+        __syncwarp();
+        tangent_next_z(Ny, Nu, t - 1, p, wm, xt, scale, K, uscale, z);
+        __syncwarp();
+    }
+}
+
 // Host outputs of the tangent stage of rollout_batch (gpmpc_rollout_batch_grad): (B, Nt, Ny, P) each
 struct RolloutTangents {
     double *dmeans, *dvars;
@@ -2536,7 +2580,7 @@ struct DerivSlabs {
 
 static int derivs_prepare(gpmpc_handle_t h, int H, bool second, DerivSlabs* s);
 static int derivs_enqueue(gpmpc_handle_t h, int method, int H, const double* dZ, const double* dSigma, int spp,
-                          const DerivSlabs& s);
+                          const DerivSlabs& s, double* beta = nullptr, long long sbeta = 0);
 
 // Device views of a roll-out's feedback policy, null where absent (x_ref and uscale only with K)
 struct RolloutPolicy { const double *scale, *K, *x_ref, *uscale; };
@@ -2951,8 +2995,10 @@ static int derivs_prepare(gpmpc_handle_t h, int H, bool second, DerivSlabs* s)
 // per 64-point chunk ks, v = Linv ks with the gather records, beta = Linv^T v, the block partials of dvar / mean Hessian
 // and their finalisation (with s.d2var, the second-derivative passes); then the assembly of mean, var, J, cov into dOut
 // and d cov / dz.  gpmpc_predict_grad / _hess run it on their uploaded points, gpmpc_rollout_batch_grad on every step's.
+// beta (may be null): every chunk's beta rows are copied there, row h of output a at beta + a * sbeta + h * Npad
+// (gpmpc_rollout_sample_grad's store).
 static int derivs_enqueue(gpmpc_handle_t h, int method, int H, const double* dZ, const double* dSigma, int spp,
-                          const DerivSlabs& s)
+                          const DerivSlabs& s, double* beta, long long sbeta)
 {
     const int np = h->Npad, Nx = h->Nx, Ny = h->Ny;
     const int nblk_g = (np + GR_CHUNK - 1) / GR_CHUNK;
@@ -2969,6 +3015,11 @@ static int derivs_enqueue(gpmpc_handle_t h, int method, int H, const double* dZ,
         psk_base(h, p, Hc, 1);                                // beta = Linv^T v = K^-1 ks  (rows of V times U^T)
         p.Vout = h->dBeta; p.sV = (long long)HB * np; p.ldv = np;
         CUDA_TRY(psk_launch(h, p, h->dV, h->dUall));
+        if (beta) {
+            copy2d_kernel<<<dim3(16, std::min(Hc, 64), h->nloc), 128, 0, h->st>>>(h->dBeta, np, (long long)HB * np,
+                                                                           beta + (long long)h0 * np, np, sbeta, Hc, np);
+            CUDA_TRY(cudaGetLastError());
+        }
         CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_grad_reduce<decltype(nxp)::value>(h, dZc, Hc, nblk_g); }));
         grad_finalize_kernel<<<dim3(Hc, h->nloc), 128, 0, h->st>>>(h->dPDV, h->dPH, nblk_g, Hc, h->dHyp, Nx + 2, Nx, Ny,
                                                                    h->dG, H, h0, s.dvar, s.hess);
@@ -3203,12 +3254,14 @@ extern "C" int gpmpc_posterior_cov(gpmpc_handle_t h, int H, const double* Z, dou
 // Sampled roll-outs (kernels.cuh, sample_cond_kernel): per step the V rows of the B current inputs go to slot t of the
 // store (solve_rows, with their means), one CTA per (trajectory, output) draws f_t conditioned on the trajectory's
 // earlier kept points, and rollout_feedback_kernel forms the next input from f_t.  All steps are enqueued back to back;
-// one D2H copy and one synchronisation at the end.
-extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const double* z0, const double* U, const double* eps,
-                                    const double* xi, const double* scale, const double* K, const double* x_ref,
-                                    const double* uscale, double* samples, double* z_out, int* kept)
+// one D2H copy and one synchronisation at the end.  With dsamples (gpmpc_rollout_sample_grad, DESIGN 4.16) each step
+// also runs the derivative chain on the same points (J, dvar_dz, and beta rows into slot t of the beta store), then after
+// the draw sample_cross_kernel, sample_next_kernel (step t's input tangents) and sample_tangent_kernel; without it the
+// launches are exactly those of the draw alone.
+static int rollout_sample(gpmpc_handle_t h, const char* fn, int B, int Nt, const double* z0, const double* U,
+                          const double* eps, const double* xi, const double* scale, const double* K, const double* x_ref,
+                          const double* uscale, double* samples, double* z_out, int* kept, bool tg, double* dsamples)
 {
-    const char* fn = __func__;
     int rc = predict_guard(h, fn, GPMPC_METHOD_ME, 1);
     if (rc) return rc;
     const int Nx = h->Nx, Ny = h->Ny, Nu = Nx - Ny, np = h->Npad, nl = h->nloc;
@@ -3216,9 +3269,14 @@ extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const doubl
     if (rc) return rc;
     const int cond_smem = (Nt + 1) * 8 + Nt * 4;           // sample_cond_kernel: c | conditioning steps
     if (cond_smem > 48 * 1024) { set_error(h, "%s: Nt = %d steps exceed the conditioning kernel's shared memory", fn, Nt); return GPMPC_ERR_ARG; }
+    if (tg && !dsamples) { set_error(h, "%s: null dsamples", fn); return GPMPC_ERR_ARG; }
+    if (tg && Nt > SAMPLE_GRAD_NT_MAX) {
+        set_error(h, "%s: Nt = %d steps exceed the tangent kernel's shared memory (Nt <= %d)", fn, Nt, SAMPLE_GRAD_NT_MAX);
+        return GPMPC_ERR_ARG;
+    }
     rc = predict_prepare(h, fn, B, true);
     if (rc) return rc;
-    NvtxRange nvtx_r("gpmpc.rollout_sample");
+    NvtxRange nvtx_r(tg ? "gpmpc.rollout_sample_grad" : "gpmpc.rollout_sample");
     const size_t Bs = (size_t)B, nE = Bs * Nt * Ny, nX = xi ? nE : 0, o_xi = nE, o_u = o_xi + nX;
     const size_t o_z = rollout_policy(B, Nt, Ny, Nu, U, scale, K, x_ref, uscale, o_u);
     const size_t o_s = o_z + (size_t)Nt * Bs * Nx, o_kp = o_s + nE;
@@ -3226,7 +3284,20 @@ extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const doubl
     const long long sVa = (long long)Nt * B * np;          // V rows of one output: (Nt, B, Npad)
     ENSURE(h->dSmV, nl * sVa);
     ENSURE(h->dSmp, tot);
-    rc = ensure_pinned(h, o_m * 8);
+    // tangent slab [G (nloc,B,Nt,2,Nx) | dR (nloc,B,P,Nt,Nt) | dz (Nt,B,P,Nx) | dsamples (Nt,B,Ny,P)]; the beta store is
+    // laid out like the V store.  dsamples is mirrored in the pinned buffer after the draw's outputs.
+    const size_t P = !tg ? 0 : Nx + (K ? (size_t)Nu * Ny : (size_t)(Nt - 1) * Nu);
+    const size_t o_dr = (size_t)nl * Bs * Nt * 2 * Nx, o_dz = o_dr + (size_t)nl * Bs * P * Nt * Nt;
+    const size_t o_ds = o_dz + (size_t)Nt * Bs * P * Nx, nDs = tg ? (size_t)Nt * Bs * Ny * P : 0;
+    const int nw = 8, tg_smem = (Nt + 1 + Nt * Nt + nw * Nt) * 8 + Nt * 4, nx_smem = (Ny + nw * Ny) * 8;
+    DerivSlabs ds;
+    if (tg) {
+        rc = derivs_prepare(h, B, false, &ds);
+        if (rc) return rc;
+        ENSURE(h->dSmB, nl * sVa);
+        ENSURE(h->dSmTg, o_ds + nDs);
+    }
+    rc = ensure_pinned(h, (o_m + nDs) * 8);
     if (rc) return rc;
     double* pin = h->hPinned;
     memcpy(pin, eps, nE * 8);
@@ -3237,14 +3308,35 @@ extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const doubl
     memcpy(pin + o_z, z0, Bs * Nx * 8);                     // slot 0 of the input history
     CUDA_TRY(cudaMemcpyAsync(d, pin, (o_z + Bs * Nx) * 8, cudaMemcpyHostToDevice, h->st));
     const int fb_smem = K ? Ny * 8 : 0;
+    double* g = tg ? h->dSmTg.p : nullptr;
     for (int t = 0; t < Nt; ++t) {
         double* Zt = d + o_z + (size_t)t * Bs * Nx;
         rc = solve_rows(h, Zt, B, h->dSmV + (long long)t * B * np, sVa, d + o_m);
         if (rc) return rc;
+        if (tg) {                                           // J_t, dvar_dz_t and the beta rows of the step's points
+            rc = derivs_enqueue(h, GPMPC_METHOD_ME, B, Zt, nullptr, 1, ds, h->dSmB + (long long)t * B * np, sVa);
+            if (rc) return rc;
+        }
         sample_cond_kernel<<<dim3(B, nl), 256, cond_smem, h->st>>>(h->dSmV, sVa, np, h->N, d + o_m, d + o_z, h->dHyp, Nx + 2,
                                                                  Nx, Ny, d, xi ? d + o_xi : nullptr, d + o_r, d + o_kp,
                                                                  d + o_s, Nt, t, SAMPLE_DELTA);
         CUDA_TRY(cudaGetLastError());
+        if (tg) {
+            if (t > 0) {
+                sample_cross_kernel<<<dim3(B, nl, t), 256, 0, h->st>>>(h->dSmB, sVa, np, h->dXT, np, h->N, d + o_z, h->dHyp,
+                                                                       Nx + 2, Nx, Ny, d + o_kp, g, Nt, t);
+                CUDA_TRY(cudaGetLastError());
+            }
+            double* ds_t = g + o_ds + (size_t)t * Bs * Ny * P;
+            sample_next_kernel<<<B, nw * 32, nx_smem, h->st>>>(Ny, Nu, (int)P, t, d + o_s + (size_t)(t > 0 ? t - 1 : 0) * Bs * Ny,
+                                                               ds_t - (t > 0 ? Bs * Ny * P : 0), pol.scale, pol.K, pol.x_ref,
+                                                               pol.uscale, g + o_dz + (size_t)t * Bs * P * Nx);
+            CUDA_TRY(cudaGetLastError());
+            sample_tangent_kernel<<<dim3(B, nl), nw * 32, tg_smem, h->st>>>(h->dSmV, sVa, np, h->N, d + o_z, h->dHyp, Nx + 2,
+                                                                           Nx, Ny, d, d + o_r, d + o_kp, h->dJ, ds.dvar, g,
+                                                                           g + o_dz, g + o_dr, ds_t, (int)P, Nt, t);
+            CUDA_TRY(cudaGetLastError());
+        }
         if (t + 1 < Nt) {
             rollout_feedback_kernel<<<B, 256, fb_smem, h->st>>>(d + o_s + (size_t)t * Bs * Ny, nullptr, d + o_u + (size_t)(t + 1) * Nu,
                                                                 (long long)Nt * Nu, pol.scale, pol.K, pol.x_ref, pol.uscale,
@@ -3253,6 +3345,7 @@ extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const doubl
         }
     }
     CUDA_TRY(cudaMemcpyAsync(pin + o_z, d + o_z, (o_m - o_z) * 8, cudaMemcpyDeviceToHost, h->st));
+    if (tg) CUDA_TRY(cudaMemcpyAsync(pin + o_m, g + o_ds, nDs * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));
     rows_by_trajectory(samples, pin + o_s, B, Nt, Ny);
     if (z_out) rows_by_trajectory(z_out, pin + o_z, B, Nt, Nx);
@@ -3262,7 +3355,23 @@ extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const doubl
                 const size_t src = (size_t)t * Bs + b, dst = b * Nt + t;
                 for (int a = 0; a < Ny; ++a) kept[dst * Ny + a] = pin[o_kp + src * Ny + a] != 0.0 ? 1 : 0;
             }
+    if (tg) rows_by_trajectory(dsamples, pin + o_m, B, Nt, (size_t)Ny * P);
     return GPMPC_OK;
+}
+
+extern "C" int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const double* z0, const double* U, const double* eps,
+                                    const double* xi, const double* scale, const double* K, const double* x_ref,
+                                    const double* uscale, double* samples, double* z_out, int* kept)
+{
+    return rollout_sample(h, __func__, B, Nt, z0, U, eps, xi, scale, K, x_ref, uscale, samples, z_out, kept, false, nullptr);
+}
+
+// gpmpc_rollout_sample plus the pathwise derivatives of every draw (see include/gpmpc.h)
+extern "C" int gpmpc_rollout_sample_grad(gpmpc_handle_t h, int B, int Nt, const double* z0, const double* U, const double* eps,
+                                         const double* xi, const double* scale, const double* K, const double* x_ref,
+                                         const double* uscale, double* samples, double* z_out, int* kept, double* dsamples)
+{
+    return rollout_sample(h, __func__, B, Nt, z0, U, eps, xi, scale, K, x_ref, uscale, samples, z_out, kept, true, dsamples);
 }
 
 // Greedy max-variance selection (kernels.cuh, greedy_*): the pool's V and variances are formed once, then each step

@@ -1975,6 +1975,43 @@ ks_mean_kernel(const double* __restrict__ PMJ, int nblk, int Nx, int H, int nloc
     m[(long long)a * sm + r] = s0 + s1;
 }
 
+// Steps of a differentiated sampled roll-out (gpmpc_rollout_sample_grad): the tangent kernel keeps R (Nt^2 doubles) and
+// per-warp rows in shared memory under 48 KB
+#define SAMPLE_GRAD_NT_MAX 64
+
+// The conditioning steps of (b, a) before step t into idx (thread 0; the caller synchronises), and their count
+__device__ __forceinline__ int sample_cond_steps(const double* __restrict__ kept, int B, int b, int Ny, int a, int t, int* idx)
+{
+    int k = 0;
+    for (int s = 0; s < t; ++s)
+        if (kept[((long long)s * B + b) * Ny + a] != 0.0) idx[k++] = s;
+    return k;
+}
+
+// c[j] = k(z_t, z_s) - v_t . v_s for the k conditioning steps s = idx[j] and c[k] = sf2 - |v_t|^2, one warp per j (every
+// thread of a 256-thread CTA calls it; the caller synchronises).  Va: the V rows of output a; hp: its hyper row.  The
+// arithmetic of sample_cond_kernel's own loop, bit for bit (that kernel keeps its inline copy: calling these helpers
+// from it costs it a spill).
+__device__ __forceinline__ void sample_cond_c(const double* __restrict__ Va, int ldv, int N, const double* __restrict__ Zh,
+                                              const double* __restrict__ hp, int Nx, int B, int b, int t, int k,
+                                              const int* idx, double sf2, double* c)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const double* vt = Va + ((long long)t * B + b) * ldv;
+    const double* zt = Zh + ((long long)t * B + b) * Nx;
+    for (int j = warp; j <= k; j += 8) {                  // j = k: the point itself
+        const int s = (j < k) ? idx[j] : t;
+        const double dot = warp_dot(vt, Va + ((long long)s * B + b) * ldv, N);
+        double q = 0.0;
+        if (j < k && lane < Nx) {                         // Nx <= 32; direct differences
+            const double df = (zt[lane] - Zh[((long long)s * B + b) * Nx + lane]) / hp[lane];
+            q = df * df;
+        }
+        q = warp_sum(q);
+        if (lane == 0) c[j] = ((j < k) ? sf2 * exp(-0.5 * q) : sf2) - dot;
+    }
+}
+
 // One CTA per (trajectory b, output a) at step t, grid (B, nloc).  V rows of (a, s, b) at V + a sVa + (s B + b) ldv;
 // Zh (Nt, B, Nx); m (nloc, B) of this step; eps, xi (B, Nt, Ny) (xi may be null); Rf (nloc, B, Nt, Nt);
 // kept, samp (Nt, B, Ny).  Dynamic shared memory: c (Nt + 1 doubles) | conditioning steps (Nt ints).
@@ -2039,6 +2076,185 @@ sample_cond_kernel(const double* __restrict__ V, long long sVa, int ldv, int N, 
     const long long o = ((long long)t * B + b) * Ny + a;
     kept[o] = keep ? 1.0 : 0.0;
     samp[o] = xi ? f + hp[Nx + 1] * xi[((long long)b * Nt + t) * Ny + a] : f;
+}
+
+// Pathwise derivatives of the draws (gpmpc_rollout_sample_grad, DESIGN 4.16).  With beta_s = K_a^-1 ks_s and
+// d_e ks_t[i] = -(z_t,e - x_i,e) / ell_e^2 ks_t[i], the derivative of c_ts = k(z_t, z_s) - ks_t^T K^-1 ks_s is
+// g(t,s) . dz_t + g(s,t) . dz_s with
+//   g(t,s)_e = -(z_t,e - z_s,e) / ell_e^2 k(z_t, z_s) + sum_i (z_t,e - x_i,e) ks_t[i] beta_s[i] / ell_e^2.
+// One CTA per (trajectory b, output a, j-th conditioning step s of step t), grid (B, nloc, t); a CTA with j past the
+// conditioning set exits.  ks_t and ks_s are recomputed from X^T (direct differences, as the ks kernel forms them) in
+// tiles of 256 points: each thread forms ks_t[i] beta_s[i] and ks_s[i] beta_t[i] of one point, then warp w sums the
+// products with (z - x_i) for e = w, w + 8, ...  Beta rows of (a, s, b) at Beta + a sBa + (s B + b) ldb; XT (Nx, ldx);
+// Zh (Nt, B, Nx); G (nloc, B, Nt, 2, Nx): [g(t,s) | g(s,t)] at row j.  Every sum runs in a fixed order.
+__global__ void __launch_bounds__(256)
+sample_cross_kernel(const double* __restrict__ Beta, long long sBa, int ldb, const double* __restrict__ XT, int ldx, int N,
+                    const double* __restrict__ Zh, const double* __restrict__ hyp, int hyp_ld, int Nx, int Ny,
+                    const double* __restrict__ kept, double* __restrict__ G, int Nt, int t)
+{
+    __shared__ double wk[2][256], zts[32], zss[32], il2[32];
+    __shared__ int idx[SAMPLE_GRAD_NT_MAX];
+    __shared__ int s_s;
+    const int b = blockIdx.x, a = blockIdx.y, j = blockIdx.z, B = gridDim.x;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) {
+        const int k = sample_cond_steps(kept, B, b, Ny, a, t, idx);
+        s_s = j < k ? idx[j] : -1;
+    }
+    __syncthreads();
+    const int s = s_s;
+    if (s < 0) return;                                    // uniform over the CTA
+    const double* hp = hyp + (long long)a * hyp_ld;
+    if (tid < Nx) {
+        zts[tid] = Zh[((long long)t * B + b) * Nx + tid];
+        zss[tid] = Zh[((long long)s * B + b) * Nx + tid];
+        il2[tid] = 1.0 / (hp[tid] * hp[tid]);
+    }
+    __syncthreads();
+    const double sf2 = hp[Nx] * hp[Nx];
+    const double* bt = Beta + (long long)a * sBa + ((long long)t * B + b) * ldb;
+    const double* bs = Beta + (long long)a * sBa + ((long long)s * B + b) * ldb;
+    double acc1[4] = {0.0, 0.0, 0.0, 0.0}, acc2[4] = {0.0, 0.0, 0.0, 0.0};   // e = warp + 8 r, Nx <= 32
+    for (int i0 = 0; i0 < N; i0 += 256) {
+        const int i = i0 + tid;
+        double w1 = 0.0, w2 = 0.0;
+        if (i < N) {
+            double qt = 0.0, qs = 0.0;
+            for (int e = 0; e < Nx; ++e) {
+                const double x = XT[(long long)e * ldx + i];
+                const double dt = (zts[e] - x) / hp[e], ds = (zss[e] - x) / hp[e];
+                qt = fma(dt, dt, qt);
+                qs = fma(ds, ds, qs);
+            }
+            w1 = sf2 * exp(-0.5 * qt) * bs[i];
+            w2 = sf2 * exp(-0.5 * qs) * bt[i];
+        }
+        __syncthreads();                                  // the previous tile's products are consumed
+        wk[0][tid] = w1;
+        wk[1][tid] = w2;
+        __syncthreads();
+        const int n = min(256, N - i0);
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int e = warp + 8 * r;
+            if (e < Nx)
+                for (int ii = lane; ii < n; ii += 32) {
+                    const double x = XT[(long long)e * ldx + i0 + ii];
+                    acc1[r] = fma(zts[e] - x, wk[0][ii], acc1[r]);
+                    acc2[r] = fma(zss[e] - x, wk[1][ii], acc2[r]);
+                }
+        }
+    }
+    double q = 0.0;
+    if (lane < Nx) {
+        const double df = (zts[lane] - zss[lane]) / hp[lane];
+        q = df * df;
+    }
+    const double kts = sf2 * exp(-0.5 * warp_sum(q));
+    double* g = G + (((long long)a * B + b) * Nt + j) * 2 * Nx;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int e = warp + 8 * r;
+        const double s1 = warp_sum(acc1[r]), s2 = warp_sum(acc2[r]);
+        if (lane == 0 && e < Nx) {
+            const double dz = zts[e] - zss[e];
+            g[e] = (s1 - dz * kts) * il2[e];
+            g[Nx + e] = (s2 + dz * kts) * il2[e];
+        }
+    }
+}
+
+// The tangent stage of one sampled step, one CTA per (trajectory b, output a), grid (B, nloc), 8 warps over the P
+// parameter columns.  With w = R^-1 c and d = c_tt - |w|^2 re-formed as sample_cond_kernel forms them and the kept flag of
+// step t (the branch the draw took), per column p:
+//   dm = J_t dz_t,  dc_tt = dvar_dz_t . dz_t,  dc_j = g(t,s_j) . dz_t + g(s_j,t) . dz_{s_j},
+//   dw = R^-1 (dc - dR w),  dd = dc_tt - 2 w . dw,  df = dm + dw . eps_S (+ dd / (2 sqrt d) eps_t when kept),
+// and when kept the new row [dw, dd / (2 sqrt d)] of dR.  J, dvar (B, Ny, Nx) of the derivative chain at the step's points;
+// G of sample_cross_kernel; dZh (Nt, B, P, Nx) the tangent history; dRf (nloc, B, P, Nt, Nt); dsamp (B, Ny, P) of step t.
+// Every sum runs in index order in one thread.  Dynamic shared memory: c (Nt + 1) | R (Nt Nt) | per warp dw (Nt) |
+// conditioning steps (Nt ints).
+__global__ void __launch_bounds__(256)
+sample_tangent_kernel(const double* __restrict__ V, long long sVa, int ldv, int N, const double* __restrict__ Zh,
+                      const double* __restrict__ hyp, int hyp_ld, int Nx, int Ny, const double* __restrict__ eps,
+                      const double* __restrict__ Rf, const double* __restrict__ kept, const double* __restrict__ J,
+                      const double* __restrict__ dvar, const double* __restrict__ G, const double* __restrict__ dZh,
+                      double* __restrict__ dRf, double* __restrict__ dsamp, int P, int Nt, int t)
+{
+    extern __shared__ double st_sh[];
+    __shared__ int nk_s;
+    const int b = blockIdx.x, a = blockIdx.y, B = gridDim.x;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    double* c = st_sh;
+    double* sR = c + Nt + 1;
+    double* tw = sR + Nt * Nt + warp * Nt;
+    int* idx = reinterpret_cast<int*>(sR + Nt * Nt + 8 * Nt);
+    const double* hp = hyp + (long long)a * hyp_ld;
+    const double* R = Rf + ((long long)a * B + b) * Nt * Nt;
+    if (tid == 0) nk_s = sample_cond_steps(kept, B, b, Ny, a, t, idx);
+    __syncthreads();
+    const int k = nk_s;
+    const double sf2 = hp[Nx] * hp[Nx];
+    sample_cond_c(V + (long long)a * sVa, ldv, N, Zh, hp, Nx, B, b, t, k, idx, sf2, c);
+    for (int i = tid; i < k * Nt; i += 256) sR[i] = R[i];
+    __syncthreads();
+    if (tid == 0) {                                       // w and d with sample_cond_kernel's arithmetic
+        double ww = 0.0;
+        for (int j = 0; j < k; ++j) {
+            double w = c[j];
+            for (int i = 0; i < j; ++i) w -= sR[j * Nt + i] * c[i];
+            w /= sR[j * Nt + j];
+            c[j] = w;
+            ww += w * w;
+        }
+        c[k] -= ww;
+    }
+    __syncthreads();
+    const bool keep = kept[((long long)t * B + b) * Ny + a] != 0.0;
+    const double sd2 = keep ? 2.0 * sqrt(c[k]) : 1.0;
+    const double* e = eps + (long long)b * Nt * Ny + a;   // eps of (b, s, a) at e[s Ny]
+    const double* Ja = J + ((long long)b * Ny + a) * Nx;
+    const double* dva = dvar + ((long long)b * Ny + a) * Nx;
+    const double* Gab = G + ((long long)a * B + b) * Nt * 2 * Nx;
+    for (int p = warp; p < P; p += 8) {
+        const double* dzt = dZh + (((long long)t * B + b) * P + p) * Nx;
+        double* dR = dRf + (((long long)a * B + b) * P + p) * Nt * Nt;
+        for (int j = lane; j < k; j += 32) {              // dc_j - (dR w)_j
+            const double* g = Gab + (long long)j * 2 * Nx;
+            const double* dzs = dZh + (((long long)idx[j] * B + b) * P + p) * Nx;
+            double s = 0.0;
+            for (int q = 0; q < Nx; ++q) s = fma(g[q], dzt[q], s);
+            for (int q = 0; q < Nx; ++q) s = fma(g[Nx + q], dzs[q], s);
+            for (int i = 0; i <= j; ++i) s = fma(-dR[j * Nt + i], c[i], s);
+            tw[j] = s;
+        }
+        __syncwarp();
+        if (lane == 0) {
+            double dm = 0.0, dct = 0.0;
+            for (int q = 0; q < Nx; ++q) {
+                dm = fma(Ja[q], dzt[q], dm);
+                dct = fma(dva[q], dzt[q], dct);
+            }
+            double wdw = 0.0, df = dm;
+            for (int j = 0; j < k; ++j) {                 // dw = R^-1 (dc - dR w), in place
+                double s = tw[j];
+                for (int i = 0; i < j; ++i) s = fma(-sR[j * Nt + i], tw[i], s);
+                s /= sR[j * Nt + j];
+                tw[j] = s;
+                wdw = fma(c[j], s, wdw);
+                df = fma(s, e[(long long)idx[j] * Ny], df);
+            }
+            if (keep) {
+                const double dq = (dct - 2.0 * wdw) / sd2;
+                df = fma(dq, e[(long long)t * Ny], df);
+                dR[k * Nt + k] = dq;
+            }
+            dsamp[((long long)b * Ny + a) * P + p] = df;
+        }
+        __syncwarp();
+        if (keep)
+            for (int j = lane; j < k; j += 32) dR[k * Nt + j] = tw[j];
+        __syncwarp();
+    }
 }
 
 // ---------------------------------------------------------------------------------------

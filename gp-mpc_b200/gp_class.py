@@ -738,7 +738,7 @@ class GP:
         K = self.__lqr_gains(X0, U[:, 0], Q, R) if feedback else None
         covar = self.__initial_covar(nb)
         z0, Ug, scale, uscale = self.__engine_start(X0, U, K, x_ref)
-        sX, sU, sY = (self.__stdX, self.__stdU, self.__stdY) if self.__normalize else (np.ones(Ny), np.ones(Nu), np.ones(Ny))
+        sY = self.__stdY if self.__normalize else np.ones(Ny)
         P = Nx + (Nu * Ny if K is not None else (Nt - 1) * Nu)
         m_std = np.empty((nb, Nt, Ny)); v_std = np.empty((nb, Nt, Ny))
         Dm = np.empty((nb, Nt, Ny, P)); Dv = np.empty((nb, Nt, Ny, P))
@@ -756,26 +756,37 @@ class GP:
         out['mean'][:, 1:] = self.inverse_mean(m_std, self.__meanY, self.__stdY) if self.__normalize else m_std
         out['var'][:, 1:] = self.inverse_variance(v_std) if self.__normalize else v_std
         for key, D in (('mean', Dm), ('var', Dv)):
-            d_x0 = np.zeros((nb, Nt + 1, Ny, Ny))
-            if key == 'mean':
-                d_x0[:, 0] = np.eye(Ny)
-            d_x0[:, 1:] = D[..., :Ny] / sX
-            d_u0 = D[..., Ny:Nx] / sU                    # w.r.t. u_0 in caller units (nb, Nt, Ny, Nu)
-            if K is None:
-                d_u = np.zeros((nb, Nt + 1, Ny, Nt, Nu))
-                d_u[:, 1:, :, 0, :] = d_u0
-                d_u[:, 1:, :, 1:, :] = (D[..., Nx:] / np.tile(sU, Nt - 1)).reshape(nb, Nt, Ny, Nt - 1, Nu)
-                out['d%s_du' % key] = d_u
-            else:                                        # u_0 = K (x0 - x_ref): both x0 and K enter z0's tail
-                d_x0[:, 1:] += np.einsum('btai,bik->btak', d_u0, K)
-                d_K = np.zeros((nb, Nt + 1, Ny, Nu, Ny))
-                d_K[:, 1:] = D[..., Nx:].reshape(nb, Nt, Ny, Nu, Ny)
-                d_K[:, 1:] += d_u0[..., :, None] * (X0 - x_ref)[:, None, None, None, :]
-                out['d%s_dK' % key] = d_K
+            d_x0, d_p = self.__caller_derivs(D, X0, K, x_ref, key == 'mean')
+            out['d%s_%s' % (key, 'du' if K is None else 'dK')] = d_p
             out['d%s_dx0' % key] = d_x0
         if single:
             return {k: v[0] for k, v in out.items()}
         return out
+
+    def __caller_derivs(self, D, X0, K, x_ref, identity):
+        """The engine's derivative columns D (n, Nt, Ny, P) of a quantity already in caller units, for trajectories that
+        start at X0 (n, Ny) with gains K (n, Nu, Ny) or None, w.r.t. the caller's parameters: d_x0 (n, Nt+1, Ny, Ny), row 0
+        the identity if ``identity`` else zero, and d_u (n, Nt+1, Ny, Nt, Nu) open loop or d_K (n, Nt+1, Ny, Nu, Ny).  The
+        engine's columns are z0 = [(x0 - meanX) / stdX, (u_0 - meanU) / stdU], then U rows 1.. or K row-major."""
+        Nx, Ny, Nu = self.__Nx, self.__Ny, self.__Nu
+        sX, sU = (self.__stdX, self.__stdU) if self.__normalize else (np.ones(Ny), np.ones(Nu))
+        nb, Nt = D.shape[0], D.shape[1]
+        d_x0 = np.zeros((nb, Nt + 1, Ny, Ny))
+        if identity:
+            d_x0[:, 0] = np.eye(Ny)
+        d_x0[:, 1:] = D[..., :Ny] / sX
+        d_u0 = D[..., Ny:Nx] / sU                        # w.r.t. u_0 in caller units (nb, Nt, Ny, Nu)
+        if K is None:
+            d_u = np.zeros((nb, Nt + 1, Ny, Nt, Nu))
+            d_u[:, 1:, :, 0, :] = d_u0
+            d_u[:, 1:, :, 1:, :] = (D[..., Nx:] / np.tile(sU, Nt - 1)).reshape(nb, Nt, Ny, Nt - 1, Nu)
+            return d_x0, d_u
+        # u_0 = K (x0 - x_ref): both x0 and K enter z0's tail
+        d_x0[:, 1:] += np.einsum('btai,bik->btak', d_u0, K)
+        d_K = np.zeros((nb, Nt + 1, Ny, Nu, Ny))
+        d_K[:, 1:] = D[..., Nx:].reshape(nb, Nt, Ny, Nu, Ny)
+        d_K[:, 1:] += d_u0[..., :, None] * (X0 - x_ref)[:, None, None, None, :]
+        return d_x0, d_K
 
     def sample_rollout(self, x0, u, n_samples, seed=None, Sigma0=None, feedback=False, x_ref=None, Q=None, R=None,
                        process_noise=False):
@@ -802,18 +813,74 @@ class GP:
         ``rollout`` does with the mean.  ``rollout`` feeds the Y-standardised covariance as the input covariance of the
         next step (q4), so differences between the spread of the samples and its propagated variances at t >= 2 can
         come from that quirk as well as from the approximations. """
+        d = self.__sample_setup('sample_rollout', x0, u, n_samples, seed, Sigma0, feedback, x_ref, Q, R, process_noise)
+        nb, ns, Nt, Ny = d['nb'], d['ns'], d['Nt'], self.__Ny
+        samp = np.empty((nb * ns, Nt, Ny))
+        for r, Kg in d['passes']:
+            samp[r] = self.__engine.rollout_sample(d['z0'][r], d['U'][r], d['eps'][r], None if d['xi'] is None else d['xi'][r],
+                                                   d['scale'], Kg, d['x_ref'], d['uscale'])[0]
+        out = self.__sample_states(d, samp)
+        return out[0] if d['single'] else out
+
+    def sample_rollout_grad(self, x0, u, n_samples, seed=None, Sigma0=None, feedback=False, x_ref=None, Q=None, R=None,
+                            process_noise=False):
+        """ ``sample_rollout`` with the pathwise derivatives of every sampled state, the draws held fixed (the
+        reparameterisation gradient of a Monte Carlo objective over them, as scenario MPC and PILCO-style policy search
+        use), w.r.t. the start x0 and, open loop, the inputs u, or with feedback=True the gain K (gpmpc_rollout_sample_grad:
+        forward-mode tangents beside the draws on the device, one call instead of the P + 1 calls of a difference
+        quotient, exact on either side of the rule that drops a point from the conditioning set).
+
+        Arguments, draws (same seed: the same samples, bit for bit) and shapes follow ``sample_rollout``; a batch x0:(B,Ny)
+        adds a leading B axis to every array below.  Returns a dict in caller units:
+          samples (n_samples, Nt+1, Ny)                    ``sample_rollout``'s array
+          kept (n_samples, Nt, Ny)                         1 where the step's point entered its draw's conditioning set
+          dsamples_dx0 (n_samples, Nt+1, Ny, Ny)           row 0 is the identity
+          open loop:  dsamples_du (n_samples, Nt+1, Ny, Nt, Nu)   d samples[t] / d u[s, i]
+          feedback:   dsamples_dK (n_samples, Nt+1, Ny, Nu, Ny)   d samples[t] / d K[i, k]
+        The drawn start is z_0 = zbar + F n with Sigma0 (and so F) held fixed, so it moves with zbar = [x0, u_0].  As in
+        ``rollout_grad`` the gain is held fixed at the LQR gain (not differentiated through the Riccati equation), and
+        u_0 = K (x0 - x_ref) is differentiated w.r.t. both x0 and K.  Where a draw drops a point (kept = 0) the derivative is
+        that of the branch taken. """
+        if not hasattr(self.__engine, 'rollout_sample_grad'):
+            raise NotImplementedError('sample_rollout_grad needs an engine with gpmpc_rollout_sample_grad')
+        d = self.__sample_setup('sample_rollout_grad', x0, u, n_samples, seed, Sigma0, feedback, x_ref, Q, R, process_noise)
+        nb, ns, Nt, Ny, Nx, Nu = d['nb'], d['ns'], d['Nt'], self.__Ny, self.__Nx, self.__Nu
+        K = d['K']
+        P = Nx + (Nu * Ny if K is not None else (Nt - 1) * Nu)
+        samp = np.empty((nb * ns, Nt, Ny)); kept = np.empty((nb * ns, Nt, Ny), dtype=np.int32)
+        D = np.empty((nb * ns, Nt, Ny, P))
+        for r, Kg in d['passes']:
+            samp[r], _, kept[r], D[r] = self.__engine.rollout_sample_grad(
+                d['z0'][r], d['U'][r], d['eps'][r], None if d['xi'] is None else d['xi'][r], d['scale'], Kg, d['x_ref'],
+                d['uscale'])
+        if self.__normalize:
+            D = D * self.__stdY[None, None, :, None]
+        # the chain through zbar: every draw of trajectory b starts at X0[b] with gain K[b]
+        d_x0, d_p = self.__caller_derivs(D, np.repeat(d['X0'], ns, 0), None if K is None else np.repeat(K, ns, 0),
+                                         d['x_ref'], True)
+        out = dict(samples=self.__sample_states(d, samp), kept=kept.reshape(nb, ns, Nt, Ny),
+                   dsamples_dx0=d_x0.reshape((nb, ns) + d_x0.shape[1:]))
+        out['dsamples_du' if K is None else 'dsamples_dK'] = d_p.reshape((nb, ns) + d_p.shape[1:])
+        if d['single']:
+            return {k: v[0] for k, v in out.items()}
+        return out
+
+    def __sample_setup(self, fn, x0, u, n_samples, seed, Sigma0, feedback, x_ref, Q, R, process_noise):
+        """The checks, gains and draws of a sampled roll-out (``sample_rollout``'s documented order) and the engine's view
+        of them, flattened to rows b n_samples + j: a dict with X0, single, nb, ns, Nt, K, x_ref, z0, U, eps, xi, scale,
+        uscale and passes, the engine passes as (rows, gain).  fn names the caller in errors."""
         if self.__sharded_outputs():
-            raise NotImplementedError('sample_rollout needs all outputs on one GPU (build the GP with a single-process Comm)')
+            raise NotImplementedError('%s needs all outputs on one GPU (build the GP with a single-process Comm)' % fn)
         if self.__prior_mean_in_predict and self.__has_prior_mean():
-            raise NotImplementedError('sample_rollout draws from the zero-mean posterior the engine holds; '
-                                      'prior_mean_in_predict with a prior mean function is not supported')
+            raise NotImplementedError('%s draws from the zero-mean posterior the engine holds; '
+                                      'prior_mean_in_predict with a prior mean function is not supported' % fn)
         Nx, Ny = self.__Nx, self.__Ny
         X0, U, single, Nt = self.__trajectories(x0, u)
         nb, ns = X0.shape[0], int(n_samples)
         if ns < 1 or Nt < 1:
-            raise ValueError('sample_rollout needs n_samples >= 1 and at least one step (got %d, %d)' % (ns, Nt))
+            raise ValueError('%s needs n_samples >= 1 and at least one step (got %d, %d)' % (fn, ns, Nt))
         if feedback:
-            Q, R, x_ref = self.__feedback_defaults('sample_rollout', Q, R, x_ref)
+            Q, R, x_ref = self.__feedback_defaults(fn, Q, R, x_ref)
         if Sigma0 is None:
             S0 = self.__initial_covar(nb)
         else:
@@ -828,23 +895,22 @@ class GP:
         eps = rng.standard_normal((nb, ns, Nt, Ny))
         xi = rng.standard_normal((nb, ns, Nt, Ny)) if process_noise else None
         z0 = np.stack([zbar[b] + n0[b] @ _sqrt_psd(S0[b]).T for b in range(nb)])        # (nb, ns, Nx)
-        Ur = np.repeat(Ug, ns, 0)
         rows = lambda g: (np.asarray(g)[:, None] * ns + np.arange(ns)[None, :]).reshape(-1)
-        z0f, epsf = z0.reshape(nb * ns, Nx), eps.reshape(nb * ns, Nt, Ny)
-        xif = None if xi is None else xi.reshape(nb * ns, Nt, Ny)
-        samp = np.empty((nb * ns, Nt, Ny))
-        for g, Kg in self.__gain_groups(K, nb):
-            r = rows(g)
-            samp[r] = self.__engine.rollout_sample(z0f[r], Ur[r], epsf[r], None if xif is None else xif[r], scale, Kg, x_ref,
-                                                   uscale)[0]
+        return dict(X0=X0, single=single, nb=nb, ns=ns, Nt=Nt, K=K, x_ref=x_ref, z0=z0.reshape(nb * ns, Nx),
+                    U=np.repeat(Ug, ns, 0), eps=eps.reshape(nb * ns, Nt, Ny),
+                    xi=None if xi is None else xi.reshape(nb * ns, Nt, Ny), scale=scale, uscale=uscale,
+                    passes=[(rows(g), Kg) for g, Kg in self.__gain_groups(K, nb)])
+
+    def __sample_states(self, d, samp):
+        """The sampled states (nb, ns, Nt+1, Ny) in caller units: row 0 the drawn starts, then the engine's draws samp."""
+        nb, ns, Nt, Ny = d['nb'], d['ns'], d['Nt'], self.__Ny
         out = np.empty((nb * ns, Nt + 1, Ny))
-        out[:, 0] = z0f[:, :Ny]
+        out[:, 0] = d['z0'][:, :Ny]
         out[:, 1:] = samp
         if self.__normalize:
             out[:, 0] = self.inverse_mean(out[:, 0], self.__meanX, self.__stdX)
             out[:, 1:] = self.inverse_mean(out[:, 1:], self.__meanY, self.__stdY)
-        out = out.reshape(nb, ns, Nt + 1, Ny)
-        return out[0] if single else out
+        return out.reshape(nb, ns, Nt + 1, Ny)
 
     def get_size(self):
         """ (N, Ny, Nu)  (reference gp_class.py:266-274) """

@@ -389,6 +389,30 @@ int gpmpc_rollout_sample(gpmpc_handle_t h, int B, int Nt, const double* z0, cons
                          const double* xi, const double* scale, const double* K, const double* x_ref,
                          const double* uscale, double* samples, double* z_out, int* kept);
 
+/* gpmpc_rollout_sample plus the pathwise derivatives of every draw with its normals eps (and xi) held fixed: what a
+ * sample-average objective over fixed draws (scenario MPC, reparameterised policy search) needs.  Arguments as
+ * gpmpc_rollout_sample; samples, z_out and kept are bit-identical to its.  dsamples (B, Nt, Ny, P), required, GP output
+ * units, with gpmpc_rollout_batch_grad's parameter columns: z0[b] (Nx), then U rows 1..Nt-1 open loop or K row-major with
+ * feedback (P = Nx + (Nt-1) Nu, Nx + Nu Ny, or Nx when Nu = 0); scale, x_ref and uscale are held fixed.  Per output a and
+ * step t, with beta_s = K_a^-1 k_a(X, z_s), w = R^-1 c and d = c_tt - |w|^2 of the draw:
+ *   dm = J dz_t,  dc_tt = dvar_dz . dz_t,  dc_s = g(t,s) . dz_t + g(s,t) . dz_s  (s kept before t),
+ *   g(t,s)_e = -(z_t,e - z_s,e) / ell_e^2 k(z_t, z_s) + sum_i (z_t,e - x_i,e) / ell_e^2 k(x_i, z_t) beta_s[i],
+ *   dw = R^-1 (dc - dR w),  dd = dc_tt - 2 w . dw,  df = dm + dw . eps_S (+ dd / (2 sqrt d) eps_t when kept),
+ * where J, dvar_dz are gpmpc_predict_grad's at z_t and dR carries the tangent of R's rows.  The kept decision is the
+ * draw's and is not differentiated: the result is the derivative of the branch taken.  The next tangent is
+ * gpmpc_rollout_batch_grad's with dm replaced by df and the mean by the sample.  Every sum runs in a fixed order:
+ * trajectory b's results do not depend on B or its row.  GPMPC_ERR_ARG: every argument error of gpmpc_rollout_sample,
+ * dsamples NULL, or Nt > 64 (the tangent kernel keeps each trajectory's R in shared memory); GPMPC_ERR_STATE: not
+ * factorised, or the handle does not own every output.  Every check runs before any work.  Device memory beyond
+ * gpmpc_rollout_sample's: the beta store 8 Ny Nt B Npad bytes (as large as its V store), U = L^-1^T of the derivative
+ * chain 8 Ny Npad^2 bytes (17 GB at Ny = 8, Npad = 16384), the tangents of R 8 Ny B P Nt^2 bytes, the tangent history
+ * 8 Nt B P Nx bytes, 16 Ny B Nt Nx bytes of cross terms and 8 Nt B Ny P bytes of outputs.  At Ny = 8, Npad = 16384 with
+ * B = 256, Nt = 30 the two stores alone are 16 GB beside the 55 GB of the factor and its copies: that does not fit on
+ * an 80 GB card; B = 64 does. */
+int gpmpc_rollout_sample_grad(gpmpc_handle_t h, int B, int Nt, const double* z0, const double* U, const double* eps,
+                              const double* xi, const double* scale, const double* K, const double* x_ref,
+                              const double* uscale, double* samples, double* z_out, int* kept, double* dsamples);
+
 /* Problem sizes of a handle (GP.get_size, gp_class.py:266-274: N, and Nx, Ny). */
 int gpmpc_get_size(gpmpc_handle_t h, int* N, int* Nx, int* Ny);
 

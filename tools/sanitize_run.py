@@ -48,6 +48,8 @@ print('em_grad finite', all(bool(np.isfinite(eg[k]).all()) for k in eg), np.arra
 pc = eng.posterior_cov(p['Z'][:5])
 sm, _, kept = eng.rollout_sample(p['Z'][:3], np.repeat(p['Z'][:3, None, Ny:], 4, 1), np.ones((3, 4, Ny)))
 print('rollout_sample finite', bool(np.isfinite(sm).all()), int(kept.sum()), flush=True)
+smg, _, _, dsm = eng.rollout_sample_grad(p['Z'][:3], np.repeat(p['Z'][:3, None, Ny:], 4, 1), np.ones((3, 4, Ny)))
+print('rollout_sample_grad finite', bool(np.isfinite(dsm).all()), np.array_equal(smg, sm), flush=True)
 _, _, ln = eng.loo()
 fl, gl = eng.loo_nlpp(0, p['hyper'][0] * 0.9, grad=True)
 print('loo', ln, fl, bool(np.isfinite(gl).all()), flush=True)
