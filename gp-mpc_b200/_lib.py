@@ -324,67 +324,66 @@ class Engine:
         return (U, scale, _f64(K, (Nu, self.Ny)), None if x_ref is None else _f64(x_ref, (self.Ny,)),
                 None if uscale is None else _f64(uscale, (2, Nu)))
 
+    def _params(self, Nt, K):
+        """P, the parameter columns of a differentiated roll-out: [z0 | U rows 1 .. Nt-1] open loop, [z0 | K] with K."""
+        Nu = self.Nx - self.Ny
+        return self.Nx + (Nu * self.Ny if K is not None else (Nt - 1) * Nu)
+
+    def _rollout_batch(self, entry, method, tangents, z0, U, Sigma0, scale, K, x_ref, uscale):
+        """The body of the batched roll-out wrappers: entry is the C function, method None for the 'EM' entries (which
+        take none), tangents whether dmeans and dvars are returned."""
+        z0 = _f64(z0).reshape(-1, self.Nx)
+        B = z0.shape[0]
+        Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
+        Nt = int(np.shape(U)[1])
+        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
+        out = [np.empty((B, Nt, self.Ny)), np.empty((B, Nt, self.Ny)), np.empty((B, self.Ny, self.Ny))]
+        if tangents:
+            P = self._params(Nt, K)
+            out += [np.empty((B, Nt, self.Ny, P)), np.empty((B, Nt, self.Ny, P))]
+        head = (self.h,) if method is None else (self.h, int(method))
+        self._check(entry(*head, B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale), _ptr(K), _ptr(x_ref), _ptr(uscale),
+                          *[_ptr(a) for a in out]))
+        return tuple(out)
+
     def rollout_batch(self, z0, U, Sigma0, method=METHOD_TA, scale=None, K=None, x_ref=None, uscale=None):
         """gpmpc_rollout_batch: B trajectories of Nt steps in one pass, open loop or with the feedback u = K (x - x_ref).
         z0:(B,Nx), U:(B,Nt,Nu) (GP input units; with K only its shape is used), Sigma0:(B,Nx,Nx), scale:(4,Ny)|None,
         K:(Nu,Ny)|None, x_ref:(Ny,)|None, uscale:(2,Nu)|None -> means (B,Nt,Ny), vars (B,Nt,Ny), cov_last (B,Ny,Ny)."""
-        z0 = _f64(z0).reshape(-1, self.Nx)
-        B = z0.shape[0]
-        Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
-        Nt = int(np.shape(U)[1])
-        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
-        means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
-        self._check(self.lib.gpmpc_rollout_batch(self.h, int(method), B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale),
-                                                 _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means), _ptr(var), _ptr(cov)))
-        return means, var, cov
+        return self._rollout_batch(self.lib.gpmpc_rollout_batch, method, False, z0, U, Sigma0, scale, K, x_ref, uscale)
 
     def rollout_batch_em(self, z0, U, Sigma0, scale=None, K=None, x_ref=None, uscale=None):
         """gpmpc_rollout_batch_em: rollout_batch with exact moment matching ('EM'), same arguments (no method) and outputs;
         each trajectory's results are those of the host loop of predict(EM) calls, bit for bit."""
-        z0 = _f64(z0).reshape(-1, self.Nx)
-        B = z0.shape[0]
-        Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
-        Nt = int(np.shape(U)[1])
-        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
-        means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
-        self._check(self.lib.gpmpc_rollout_batch_em(self.h, B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale), _ptr(K),
-                                                    _ptr(x_ref), _ptr(uscale), _ptr(means), _ptr(var), _ptr(cov)))
-        return means, var, cov
+        return self._rollout_batch(self.lib.gpmpc_rollout_batch_em, None, False, z0, U, Sigma0, scale, K, x_ref, uscale)
 
     def rollout_batch_grad(self, z0, U, Sigma0, method=METHOD_TA, scale=None, K=None, x_ref=None, uscale=None):
         """gpmpc_rollout_batch_grad: rollout_batch's arguments and outputs (bit for bit) plus dmeans, dvars (B,Nt,Ny,P), the
         derivatives of every step's mean and variance (GP output units) w.r.t. P = Nx + (Nt-1) Nu parameters [z0[b] |
         U[b,1:] row-major] open loop, or P = Nx + Nu Ny parameters [z0[b] | K row-major] with K."""
-        Nu = self.Nx - self.Ny
-        z0 = _f64(z0).reshape(-1, self.Nx)
-        B = z0.shape[0]
-        Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
-        Nt = int(np.shape(U)[1])
-        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
-        P = self.Nx + (Nu * self.Ny if K is not None else (Nt - 1) * Nu)
-        means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
-        dmeans = np.empty((B, Nt, self.Ny, P)); dvars = np.empty((B, Nt, self.Ny, P))
-        self._check(self.lib.gpmpc_rollout_batch_grad(self.h, int(method), B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0),
-                                                      _ptr(scale), _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means),
-                                                      _ptr(var), _ptr(cov), _ptr(dmeans), _ptr(dvars)))
-        return means, var, cov, dmeans, dvars
+        return self._rollout_batch(self.lib.gpmpc_rollout_batch_grad, method, True, z0, U, Sigma0, scale, K, x_ref, uscale)
 
     def rollout_batch_em_grad(self, z0, U, Sigma0, scale=None, K=None, x_ref=None, uscale=None):
         """gpmpc_rollout_batch_em_grad: rollout_batch_em's arguments and outputs (bit for bit) plus dmeans, dvars
         (B,Nt,Ny,P) with rollout_batch_grad's parameter columns, for exact moment matching ('EM')."""
-        Nu = self.Nx - self.Ny
+        return self._rollout_batch(self.lib.gpmpc_rollout_batch_em_grad, None, True, z0, U, Sigma0, scale, K, x_ref,
+                                   uscale)
+
+    def _rollout_sample(self, entry, tangents, z0, U, eps, xi, scale, K, x_ref, uscale):
+        """The body of the sampled roll-out wrappers: entry is the C function, tangents whether dsamples is returned."""
         z0 = _f64(z0).reshape(-1, self.Nx)
         B = z0.shape[0]
-        Sigma0 = _f64(Sigma0, (B, self.Nx, self.Nx))
-        Nt = int(np.shape(U)[1])
+        eps = _f64(eps)
+        Nt = int(eps.shape[1])
+        eps = eps.reshape(B, Nt, self.Ny)
+        xi = None if xi is None else _f64(xi, (B, Nt, self.Ny))
         U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
-        P = self.Nx + (Nu * self.Ny if K is not None else (Nt - 1) * Nu)
-        means = np.empty((B, Nt, self.Ny)); var = np.empty((B, Nt, self.Ny)); cov = np.empty((B, self.Ny, self.Ny))
-        dmeans = np.empty((B, Nt, self.Ny, P)); dvars = np.empty((B, Nt, self.Ny, P))
-        self._check(self.lib.gpmpc_rollout_batch_em_grad(self.h, B, Nt, _ptr(z0), _ptr(U), _ptr(Sigma0), _ptr(scale),
-                                                         _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(means), _ptr(var),
-                                                         _ptr(cov), _ptr(dmeans), _ptr(dvars)))
-        return means, var, cov, dmeans, dvars
+        samples = np.empty((B, Nt, self.Ny)); z_out = np.empty((B, Nt, self.Nx))
+        kept = np.empty((B, Nt, self.Ny), dtype=np.int32)
+        out = [samples, z_out, kept] + ([np.empty((B, Nt, self.Ny, self._params(Nt, K)))] if tangents else [])
+        self._check(entry(self.h, B, Nt, _ptr(z0), _ptr(U), _ptr(eps), _ptr(xi), _ptr(scale), _ptr(K), _ptr(x_ref),
+                          _ptr(uscale), _ptr(samples), _ptr(z_out), kept.ctypes.data_as(_ip), *[_ptr(a) for a in out[3:]]))
+        return tuple(out)
 
     def rollout_sample(self, z0, U, eps, xi=None, scale=None, K=None, x_ref=None, uscale=None):
         """gpmpc_rollout_sample: B trajectories of Nt steps, each one consistent draw of the GP posterior along the inputs
@@ -392,40 +391,13 @@ class Engine:
         eps:(B,Nt,Ny) standard normals of the draws, xi:(B,Nt,Ny)|None process-noise normals, scale / K / x_ref / uscale
         as rollout_batch -> samples (B,Nt,Ny) GP output units, z_out (B,Nt,Nx) inputs used, kept (B,Nt,Ny) int32 (1 where
         the point entered the conditioning set)."""
-        z0 = _f64(z0).reshape(-1, self.Nx)
-        B = z0.shape[0]
-        eps = _f64(eps)
-        Nt = int(eps.shape[1])
-        eps = eps.reshape(B, Nt, self.Ny)
-        xi = None if xi is None else _f64(xi, (B, Nt, self.Ny))
-        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
-        samples = np.empty((B, Nt, self.Ny)); z_out = np.empty((B, Nt, self.Nx))
-        kept = np.empty((B, Nt, self.Ny), dtype=np.int32)
-        self._check(self.lib.gpmpc_rollout_sample(self.h, B, Nt, _ptr(z0), _ptr(U), _ptr(eps), _ptr(xi), _ptr(scale),
-                                                  _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(samples), _ptr(z_out),
-                                                  kept.ctypes.data_as(_ip)))
-        return samples, z_out, kept
+        return self._rollout_sample(self.lib.gpmpc_rollout_sample, False, z0, U, eps, xi, scale, K, x_ref, uscale)
 
     def rollout_sample_grad(self, z0, U, eps, xi=None, scale=None, K=None, x_ref=None, uscale=None):
         """gpmpc_rollout_sample_grad: rollout_sample's arguments and outputs (bit for bit) plus dsamples (B,Nt,Ny,P), the
         derivatives of every draw (GP output units) with eps and xi held fixed, w.r.t. rollout_batch_grad's P parameters
         [z0[b] | U[b,1:] row-major] open loop or [z0[b] | K row-major] with K."""
-        Nu = self.Nx - self.Ny
-        z0 = _f64(z0).reshape(-1, self.Nx)
-        B = z0.shape[0]
-        eps = _f64(eps)
-        Nt = int(eps.shape[1])
-        eps = eps.reshape(B, Nt, self.Ny)
-        xi = None if xi is None else _f64(xi, (B, Nt, self.Ny))
-        U, scale, K, x_ref, uscale = self._policy(B, Nt, U, scale, K, x_ref, uscale)
-        P = self.Nx + (Nu * self.Ny if K is not None else (Nt - 1) * Nu)
-        samples = np.empty((B, Nt, self.Ny)); z_out = np.empty((B, Nt, self.Nx))
-        kept = np.empty((B, Nt, self.Ny), dtype=np.int32)
-        dsamples = np.empty((B, Nt, self.Ny, P))
-        self._check(self.lib.gpmpc_rollout_sample_grad(self.h, B, Nt, _ptr(z0), _ptr(U), _ptr(eps), _ptr(xi), _ptr(scale),
-                                                       _ptr(K), _ptr(x_ref), _ptr(uscale), _ptr(samples), _ptr(z_out),
-                                                       kept.ctypes.data_as(_ip), _ptr(dsamples)))
-        return samples, z_out, kept, dsamples
+        return self._rollout_sample(self.lib.gpmpc_rollout_sample_grad, True, z0, U, eps, xi, scale, K, x_ref, uscale)
 
     def predict_grad(self, Z, Sigma=None, method=METHOD_TA, want_hess=False):
         """Predict + first derivatives w.r.t. the test inputs (gpmpc_predict_grad).

@@ -1637,10 +1637,11 @@ static int em_chunk(gpmpc_handle_t h, int H)
     return (int)std::max(1LL, n);
 }
 
-// scratch of n points and the em_prepare_point blocks of H points
-static int em_scratch(gpmpc_handle_t h, int n, int H)
+// scratch of one em_chunk of H points and the em_prepare_point blocks of all H
+static int em_scratch(gpmpc_handle_t h, int H)
 {
     const EmStrides s = em_strides(h);
+    const int n = em_chunk(h, H);
     ENSURE(h->dEmTr, n * s.tr);
     ENSURE(h->dEmLQ, n * s.lq);
     ENSURE(h->dEmVec, n * s.vec);
@@ -2014,43 +2015,69 @@ static int em_kinv_prepare(gpmpc_handle_t h)
     return GPMPC_OK;
 }
 
-// The derivative records of the n points of one em_forward chunk, point k from its scratch slot k: z at dz and the
-// em_prepare_point blocks at dP (strides Nx and em_per, device); D = 2 records to rec2 and D = 4 records to rec4, one
-// point's records apart (null: not wanted).  The slots are overwritten by the next chunk's forward.
-static int em_chunk_records(gpmpc_handle_t h, int n, const double* dz, const double* dP, double* rec2, double* rec4)
+// The 'EM' pass over H points, shared by predict_em and the 'EM' roll-out step: z at dz (device, stride Nx), Sigma on the
+// host (one per point with spp, else shared).  Every point's em_prepare_point block goes to emp (host, em_per doubles a
+// point; the caller keeps it for the derivative finishes) and then up to dEMP.  Per em_chunk of points em_forward writes
+// mean / var / cov (device, strides Ny / Ny / Ny^2); then, from the scratch slots that forward left (the next chunk
+// overwrites them), each point's records of degree 2 go to em_rec[0].rec when rec2 and of degree 4 to em_rec[1].rec when
+// rec4.  When em_prepare_point rejects a point, its error code returns and *bad (if given) is that point.
+static int em_pass(gpmpc_handle_t h, int H, const double* dz, const double* Sigma, int spp, double* emp, double* mean,
+                   double* var, double* cov, bool rec2, bool rec4, int* bad = nullptr)
 {
-    const int Nx = h->Nx, Ny = h->Ny, npairs = em_npairs(h), T = (h->N + 63) / 64;
+    const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx, npairs = em_npairs(h), T = (h->N + 63) / 64, nc = em_chunk(h, H);
     const size_t per = em_per(h);
     const EmRecords& R2 = h->em_rec[0];
     const EmRecords& R4 = h->em_rec[1];
-    for (int k = 0; k < n && (rec2 || rec4); ++k) {
-        const double* z = dz + (size_t)k * Nx;
-        const double* P = dP + (size_t)k * per;
-        if (rec2) {
-            double* rec = rec2 + (size_t)k * R2.tb->nrec(Ny) * R2.tb->nent;
-            CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_records<decltype(nxp)::value, 2>(h, R2, z, P, npairs, T, k, rec); }));
+    for (int p = 0; p < H; ++p) {
+        const int rc = em_prepare_point(h, Sigma + (spp ? (size_t)p * nn : 0), emp + (size_t)p * per);
+        if (rc) {
+            if (bad) *bad = p;
+            return rc;
         }
-        if (rec4) {
-            double* rec = rec4 + (size_t)k * R4.tb->nrec(Ny) * R4.tb->nent;
-            CUDA_TRY((Nx <= 8 ? launch_em_records<8, 4>(h, R4, z, P, npairs, T, k, rec)
-                              : launch_em_records<16, 4>(h, R4, z, P, npairs, T, k, rec)));   // Nx <= 16
+    }
+    CUDA_TRY(cudaMemcpyAsync(h->dEMP, emp, (size_t)H * per * 8, cudaMemcpyHostToDevice, h->st));
+    for (int c0 = 0; c0 < H; c0 += nc) {
+        const int n = std::min(nc, H - c0);
+        const double* zc = dz + (size_t)c0 * Nx;
+        const double* Pc = h->dEMP + (size_t)c0 * per;
+        const int rc = em_forward(h, n, zc, Pc, mean + (size_t)c0 * Ny, var + (size_t)c0 * Ny, cov + (size_t)c0 * Ny * Ny);
+        if (rc) return rc;
+        for (int k = 0; k < n && (rec2 || rec4); ++k) {
+            const size_t p = (size_t)c0 + k;
+            const double* z = zc + (size_t)k * Nx;
+            const double* P = Pc + (size_t)k * per;
+            if (rec2) {
+                double* rec = R2.rec + p * R2.tb->nrec(Ny) * R2.tb->nent;
+                CUDA_TRY(nxp_dispatch(Nx, [&](auto nxp) { return launch_em_records<decltype(nxp)::value, 2>(h, R2, z, P, npairs, T, k, rec); }));
+            }
+            if (rec4) {
+                double* rec = R4.rec + p * R4.tb->nrec(Ny) * R4.tb->nent;
+                CUDA_TRY((Nx <= 8 ? launch_em_records<8, 4>(h, R4, z, P, npairs, T, k, rec)
+                                  : launch_em_records<16, 4>(h, R4, z, P, npairs, T, k, rec)));   // Nx <= 16
+            }
         }
     }
     return GPMPC_OK;
 }
 
-// em_grad_finish of H points on the host: Sigma (one per point with spp, else shared), their em_prepare_point blocks emp,
-// D = 2 records recs and means mh, each at its per-point stride; point p's outputs at p times their block in go (null
-// members skipped).  On failure *bad (if given) is the failing point.
-static int em_grad_finish_points(gpmpc_handle_t h, int H, const double* Sigma, int spp, const double* emp, const double* recs,
-                                 const double* mh, const EmGradOutputs& go, int* bad = nullptr)
+// The first-derivative finish of H points after em_pass with rec2: the D = 2 records and the means (dmean, device) to the
+// host, one synchronisation, then em_grad_finish per point with Sigma (one per point with spp, else shared) and em_pass's
+// blocks emp; point p's outputs at p times their block in go (null members skipped).  On failure *bad (if given) is the
+// failing point.
+static int em_grad_finish_points(gpmpc_handle_t h, int H, const double* Sigma, int spp, const double* emp,
+                                 const double* dmean, const EmGradOutputs& go, int* bad = nullptr)
 {
     const int Nx = h->Nx, Ny = h->Ny, nn = Nx * Nx;
-    const EmTables& tb = *h->em_rec[0].tb;
+    const EmRecords& R2 = h->em_rec[0];
+    const EmTables& tb = *R2.tb;
     const size_t per = em_per(h), rl = (size_t)tb.nrec(Ny) * tb.nent;
+    std::vector<double> recs((size_t)H * rl), mh((size_t)H * Ny);
+    CUDA_TRY(cudaMemcpyAsync(recs.data(), R2.rec, recs.size() * 8, cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaMemcpyAsync(mh.data(), dmean, mh.size() * 8, cudaMemcpyDeviceToHost, h->st));
+    CUDA_TRY(cudaStreamSynchronize(h->st));
     for (int p = 0; p < H; ++p) {
-        const int rc = em_grad_finish(h, tb, Sigma + (spp ? (size_t)p * nn : 0), emp + (size_t)p * per, recs + (size_t)p * rl,
-                                      mh + (size_t)p * Ny,
+        const int rc = em_grad_finish(h, tb, Sigma + (spp ? (size_t)p * nn : 0), emp + (size_t)p * per, recs.data() + (size_t)p * rl,
+                                      mh.data() + (size_t)p * Ny,
                                       go.dmean_dz ? go.dmean_dz + (size_t)p * Ny * Nx : nullptr,
                                       go.dmean_dSigma ? go.dmean_dSigma + (size_t)p * Ny * nn : nullptr,
                                       go.dcov_dz ? go.dcov_dz + (size_t)p * Ny * Ny * Nx : nullptr,
@@ -2073,10 +2100,7 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
     const int npairs = em_npairs(h);
     if (npairs > 1024) { set_error(h, "EM supports Ny <= 44"); return GPMPC_ERR_ARG; }
     const size_t per = em_per(h);
-    const int nc = em_chunk(h, H);
-    { const int rcs = em_scratch(h, nc, H); if (rcs) return rcs; }
-    EmRecords& R2 = h->em_rec[0];
-    EmRecords& R4 = h->em_rec[1];
+    { const int rcs = em_scratch(h, H); if (rcs) return rcs; }
     if (go) { const int rc = em_records_prepare(h, 2, H); if (rc) return rc; }
     const long long TS = 1 + Nx + nn + (long long)nn * Nx + (long long)nn * nn, Q = (long long)nn * nn;
     const long long per_pair = 6 * TS + 8 * Q, nout = (long long)nn + nn * Nx + nn * nn;    // finish scratch per CTA; one output slab
@@ -2091,23 +2115,10 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
         ENSURE(h->dEmHOut, (long long)H * (Ny + Ny * Ny) * nout);
     }
     if (go || ho) { const int rc = em_kinv_prepare(h); if (rc) return rc; }
-    std::vector<double> emp((size_t)H * per);
-    for (int p = 0; p < H; ++p) {
-        int rc = em_prepare_point(h, Sigma + (spp ? (size_t)p * nn : 0), emp.data() + (size_t)p * per);
-        if (rc) return rc;
-    }
-    CUDA_TRY(cudaMemcpyAsync(h->dEMP, emp.data(), emp.size() * 8, cudaMemcpyHostToDevice, h->st));
     CUDA_TRY(cudaMemcpyAsync(h->dZ, Z, (size_t)H * Nx * 8, cudaMemcpyHostToDevice, h->st));
-    for (int c0 = 0; c0 < H; c0 += nc) {
-        const int n = std::min(nc, H - c0);
-        int rc = em_forward(h, n, h->dZ + (size_t)c0 * Nx, h->dEMP + (size_t)c0 * per, h->dMean + (size_t)c0 * Ny,
-                            h->dVar + (size_t)c0 * Ny, h->dCov + (size_t)c0 * Ny * Ny);
-        if (rc) return rc;
-        rc = em_chunk_records(h, n, h->dZ + (size_t)c0 * Nx, h->dEMP + (size_t)c0 * per,
-                              go ? R2.rec + (size_t)c0 * R2.tb->nrec(Ny) * R2.tb->nent : nullptr,
-                              ho ? R4.rec + (size_t)c0 * R4.tb->nrec(Ny) * R4.tb->nent : nullptr);
-        if (rc) return rc;
-    }
+    std::vector<double> emp((size_t)H * per);
+    const int rc = em_pass(h, H, h->dZ, Sigma, spp, emp.data(), h->dMean, h->dVar, h->dCov, go != nullptr, ho != nullptr);
+    if (rc) return rc;
     if (mean) CUDA_TRY(cudaMemcpyAsync(mean, h->dMean, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
     if (var) CUDA_TRY(cudaMemcpyAsync(var, h->dVar, (size_t)H * Ny * 8, cudaMemcpyDeviceToHost, h->st));
     if (cov) CUDA_TRY(cudaMemcpyAsync(cov, h->dCov, (size_t)H * Ny * Ny * 8, cudaMemcpyDeviceToHost, h->st));
@@ -2119,6 +2130,7 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
             if (rc) return rc;
         }
         CUDA_TRY(cudaMemcpyAsync(h->dEmHEHP, ehp.data(), ehp.size() * 8, cudaMemcpyHostToDevice, h->st));
+        const EmRecords& R4 = h->em_rec[1];
         const EmTables& tb = *R4.tb;
         const int nrech = tb.nrec(Ny);
         const int* MID = tb.d_mid(R4.idx);
@@ -2143,17 +2155,8 @@ static int predict_em(gpmpc_handle_t h, int H, const double* Z, const double* Si
         for (int q = 0; q < 6; ++q)
             if (dst[q]) CUDA_TRY(cudaMemcpyAsync(dst[q], src[q], cnt[q] * 8, cudaMemcpyDeviceToHost, h->st));
     }
-    if (!go) {
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-    } else {
-        const EmTables& tb = *R2.tb;
-        const size_t rl = (size_t)tb.nrec(Ny) * tb.nent;
-        std::vector<double> recs((size_t)H * rl), mh((size_t)H * Ny);
-        CUDA_TRY(cudaMemcpyAsync(recs.data(), R2.rec, recs.size() * 8, cudaMemcpyDeviceToHost, h->st));
-        CUDA_TRY(cudaMemcpyAsync(mh.data(), h->dMean, mh.size() * 8, cudaMemcpyDeviceToHost, h->st));
-        CUDA_TRY(cudaStreamSynchronize(h->st));
-        return em_grad_finish_points(h, H, Sigma, spp, emp.data(), recs.data(), mh.data(), *go);
-    }
+    if (go) return em_grad_finish_points(h, H, Sigma, spp, emp.data(), h->dMean, *go);
+    CUDA_TRY(cudaStreamSynchronize(h->st));
     return GPMPC_OK;
 }
 
@@ -2213,8 +2216,15 @@ extern "C" int gpmpc_predict_device(gpmpc_handle_t h, int method, int H, const d
 //               (gp_class.py:770-804 with the LQR gain of mpc_class.py:956-976; cov stays in the GP's units, q4)
 // with the reference's operation order (gp_class.py:629-638), so the trajectory is the host loop's bit for bit in open loop.
 // ------------------------------------------------------------------------------------
-// One CTA per trajectory b.  Dynamic shared memory with K: x (Ny) | K cov (Nu x Ny).  Null cov_t and Sigma: only the next
-// input is formed (gpmpc_rollout_sample).
+// One CTA per trajectory b.  Null cov_t and Sigma: only the next input is formed (gpmpc_rollout_sample).  The roll-out
+// kernels' dynamic shared memory is laid out once for kernel and launch, as kernels.cuh's SampleCondSmem; per-warp
+// offsets count from the warp's slice.  rollout_feedback_kernel, with K: x (Ny) | K cov (Nu Ny), with cov only.
+struct FeedbackSmem { long long KC; int bytes; };
+__host__ __device__ __forceinline__ FeedbackSmem rollout_feedback_smem(int Ny, int Nu, bool with_K, bool with_cov)
+{
+    return {Ny, with_K ? (Ny + (with_cov ? Nu * Ny : 0)) * 8 : 0};
+}
+
 __global__ void __launch_bounds__(256)
 rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restrict__ cov_t, const double* __restrict__ u_t,
                         long long u_stride, const double* __restrict__ scale, const double* __restrict__ K,
@@ -2245,7 +2255,7 @@ rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restr
             Sigma[r * Nx + c] = cov_t[idx];
         }
     if (!K) return;                                          // uniform over the CTA
-    double* KC = fb_sh + Ny;
+    double* KC = fb_sh + rollout_feedback_smem(Ny, Nu, true, with_cov).KC;
     __syncthreads();
     // u = K (x - x_ref), standardised as GP.predict standardises its input
     for (int i = tid; i < Nu; i += 256) {
@@ -2287,10 +2297,25 @@ rollout_feedback_kernel(const double* __restrict__ mean_t, const double* __restr
 //   dz[:Ny] = dm * stdY / stdX (dm without scale);  open loop: dz[Ny+i] = [p is U[t+1][i]], dS x block = dC, u blocks kept;
 //   feedback, x~ = x - x_ref, dx = dm * stdY:  du = (K dx + dK x~) / stdU,  dS_xu = dC K^T + C dK^T,
 //   dS_uu = dK C K^T + K dC K^T + K C dK^T  (dK = the unit matrix of p when p is an entry of K, else 0).
-// At t = 0 the tangents are the unit columns of z0 and zero covariance (nothing is read).  Each warp owns one column at a
-// time and rewrites it in place; every sum runs in index order in one thread, so a trajectory's bits do not depend on B.
-// Dynamic shared memory: J (Ny Nx) | x~ (Ny) | C K^T (Ny Nu) | K C (Nu Ny) | per warp [dz (Nx) | dm (Ny) | dC (Ny Ny) | T (Ny Nx)].
+// At t = 0 the tangents are the unit columns of z0 and zero covariance (nothing is read).  Each of the ROLL_TG_WARPS warps
+// owns one column at a time and rewrites it in place; every sum runs in index order in one thread, so a trajectory's bits
+// do not depend on B.  Dynamic shared memory: rollout_tangent_smem(em = false).
 //
+// The dynamic shared memory of rollout_tangent_kernel (em = false) and rollout_tangent_em_kernel (em = true): J or dmz
+// (Ny Nx) | x~ (Ny) | C K^T (Ny Nu) | K C (Nu Ny) | per warp [dz (Nx) | dm (Ny) | dC (Ny Ny) | T (Ny Nx)], or with em per
+// warp [dz (Nx) | dm (Ny) | dC (Ny Ny) | K dC (Nu Ny) | dS (Nx Nx)].
+struct TangentSmem { long long xt, CKt, KC, warps, wm, wC, wT, wS; int per_warp, bytes; };
+__host__ __device__ __forceinline__ TangentSmem rollout_tangent_smem(int Ny, int Nu, bool em)
+{
+    const int Nx = Ny + Nu;
+    TangentSmem L;
+    L.xt = Ny * Nx; L.CKt = L.xt + Ny; L.KC = L.CKt + Ny * Nu; L.warps = L.KC + Nu * Ny;
+    L.wm = Nx; L.wC = L.wm + Ny; L.wT = L.wC + Ny * Ny; L.wS = L.wT + (em ? Nu * Ny : Ny * Nx);
+    L.per_warp = (int)(em ? L.wS + Nx * Nx : L.wS);
+    L.bytes = (int)(L.warps + ROLL_TG_WARPS * L.per_warp) * 8;
+    return L;
+}
+
 // The two stages every tangent kernel shares.  tangent_policy: per trajectory, before its columns, x~ = x - x_ref (feedback,
 // unless last) and, with Sigma tangents (sig), C K^T and K C; cov_t is the trajectory's.
 __device__ __forceinline__ void tangent_policy(int Ny, int Nu, int b, bool fb_next, bool sig, const double* __restrict__ mean_t,
@@ -2400,7 +2425,7 @@ __device__ __forceinline__ void tangent_column(int Ny, int Nu, int P, int t, int
     }
 }
 
-__global__ void __launch_bounds__(256, 2)
+__global__ void __launch_bounds__(ROLL_TG_WARPS * 32, 2)
 rollout_tangent_kernel(int Ny, int Nu, int P, int t, int first, int last, int method_ta,
                        const double* __restrict__ J, const double* __restrict__ dvar, const double* __restrict__ dcov,
                        const double* __restrict__ mean_t, const double* __restrict__ cov_t, const double* __restrict__ scale,
@@ -2410,15 +2435,15 @@ rollout_tangent_kernel(int Ny, int Nu, int P, int t, int first, int last, int me
     extern __shared__ double tg_sh[];
     const int Nx = Ny + Nu, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5, b = blockIdx.x;
     const bool fb = K != nullptr;
+    const TangentSmem L = rollout_tangent_smem(Ny, Nu, false);
     double* sJ = tg_sh;
-    double* xt = sJ + Ny * Nx;
-    double* CKt = xt + Ny;
-    double* KC = CKt + Ny * Nu;
-    const int per_warp = Nx + Ny + Ny * Ny + Ny * Nx;
-    double* wz = KC + Nu * Ny + warp * per_warp;
-    double* wm = wz + Nx;
-    double* wC = wm + Ny;
-    double* wT = wC + Ny * Ny;
+    double* xt = tg_sh + L.xt;
+    double* CKt = tg_sh + L.CKt;
+    double* KC = tg_sh + L.KC;
+    double* wz = tg_sh + L.warps + warp * L.per_warp;
+    double* wm = wz + L.wm;
+    double* wC = wz + L.wC;
+    double* wT = wz + L.wT;
     J += (size_t)b * Ny * Nx;
     cov_t += (size_t)b * Ny * Ny;
     for (int i = tid; i < Ny * Nx; i += blockDim.x) sJ[i] = J[i];
@@ -2474,9 +2499,8 @@ rollout_tangent_kernel(int Ny, int Nu, int P, int t, int first, int last, int me
 // over all Nx^2 entries of the symmetric dS: the blocks hold every other entry fixed, so this is the directional derivative.
 // At t = 0 dS is zero and is not read.  dmz and the column's dS are staged in shared memory; dmS and dcS are read from global
 // memory (Ny^2 Nx^2 doubles a trajectory do not fit at Nx = 32).  Every sum runs in index order in one thread.
-// Dynamic shared memory: dmz (Ny Nx) | x~ (Ny) | C K^T (Ny Nu) | K C (Nu Ny) | per warp [dz (Nx) | dm (Ny) | dC (Ny Ny) |
-// K dC (Nu Ny) | dS (Nx Nx)].
-__global__ void __launch_bounds__(256, 2)
+// Dynamic shared memory: rollout_tangent_smem(em = true).
+__global__ void __launch_bounds__(ROLL_TG_WARPS * 32, 2)
 rollout_tangent_em_kernel(int Ny, int Nu, int P, int t, int first, int last,
                           const double* __restrict__ dmz, const double* __restrict__ dmS, const double* __restrict__ dcz,
                           const double* __restrict__ dcS, const double* __restrict__ mean_t, const double* __restrict__ cov_t,
@@ -2487,16 +2511,16 @@ rollout_tangent_em_kernel(int Ny, int Nu, int P, int t, int first, int last,
     extern __shared__ double tg_sh[];
     const int Nx = Ny + Nu, nn = Nx * Nx, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const int b = blockIdx.x;
+    const TangentSmem L = rollout_tangent_smem(Ny, Nu, true);
     double* sG = tg_sh;
-    double* xt = sG + Ny * Nx;
-    double* CKt = xt + Ny;
-    double* KC = CKt + Ny * Nu;
-    const int per_warp = Nx + Ny + Ny * Ny + Nu * Ny + nn;
-    double* wz = KC + Nu * Ny + warp * per_warp;
-    double* wm = wz + Nx;
-    double* wC = wm + Ny;
-    double* wT = wC + Ny * Ny;
-    double* wS = wT + Nu * Ny;
+    double* xt = tg_sh + L.xt;
+    double* CKt = tg_sh + L.CKt;
+    double* KC = tg_sh + L.KC;
+    double* wz = tg_sh + L.warps + warp * L.per_warp;
+    double* wm = wz + L.wm;
+    double* wC = wz + L.wC;
+    double* wT = wz + L.wT;
+    double* wS = wz + L.wS;
     dmz += (size_t)b * Ny * Nx;
     dmS += (size_t)b * Ny * nn;
     dcz += (size_t)b * Ny * Ny * Nx;
@@ -2542,7 +2566,13 @@ rollout_tangent_em_kernel(int Ny, int Nu, int P, int t, int first, int last,
 // the P columns: at t = 0 the unit columns of z0, else tangent_next_z of step t-1's draw tangents dsamp_prev (B, Ny, P)
 // with x the draw samp_prev (B, Ny) in place of the mean, as rollout_feedback_kernel forms the next input from it.
 // Writes dZt (B, P, Nx).  Dynamic shared memory: x~ (Ny) | per warp df (Ny).
-__global__ void __launch_bounds__(256, 2)
+struct SampleNextSmem { long long warps; int bytes; };
+__host__ __device__ __forceinline__ SampleNextSmem sample_next_smem(int Ny)
+{
+    return {Ny, (Ny + ROLL_TG_WARPS * Ny) * 8};
+}
+
+__global__ void __launch_bounds__(ROLL_TG_WARPS * 32, 2)
 sample_next_kernel(int Ny, int Nu, int P, int t, const double* __restrict__ samp_prev, const double* __restrict__ dsamp_prev,
                    const double* __restrict__ scale, const double* __restrict__ K, const double* __restrict__ x_ref,
                    const double* __restrict__ uscale, double* __restrict__ dZt)
@@ -2550,7 +2580,7 @@ sample_next_kernel(int Ny, int Nu, int P, int t, const double* __restrict__ samp
     extern __shared__ double sn_sh[];
     const int Nx = Ny + Nu, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5, b = blockIdx.x;
     double* xt = sn_sh;
-    double* wm = xt + Ny + warp * Ny;
+    double* wm = sn_sh + sample_next_smem(Ny).warps + warp * Ny;
     if (t > 0) tangent_policy(Ny, Nu, b, K != nullptr, false, samp_prev, nullptr, scale, K, x_ref, xt, nullptr, nullptr);
     __syncthreads();
     for (int p = warp; p < P; p += nwarps) {
@@ -2614,6 +2644,9 @@ static int rollout_args(gpmpc_handle_t h, const char* fn, int B, int Nt, bool nu
     return GPMPC_OK;
 }
 
+// P, the parameters of a differentiated roll-out: [z0 (Nx) | K row-major (Nu Ny)] with K, else [z0 | U rows 1 .. Nt-1]
+static size_t rollout_params(int Nx, int Ny, int Nt, bool with_K) { return Nx + (size_t)(Nx - Ny) * (with_K ? Ny : Nt - 1); }
+
 // (t, b) -> (b, t): row t B + b of the step-major src to row b Nt + t of dst, n doubles per row
 static void rows_by_trajectory(double* dst, const double* src, int B, int Nt, size_t n)
 {
@@ -2651,7 +2684,7 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
     // gpmpc_predict_em_grad blocks dmz (B,Ny,Nx) | dmS (B,Ny,Nx,Nx) | dcz (B,Ny,Ny,Nx) | dcS (B,Ny,Ny,Nx,Nx)], dmeans and
     // dvars mirrored in the pinned buffer after the roll-out's outputs
     const size_t nn = (size_t)Nx * Nx;
-    const size_t P = !tg ? 0 : Nx + (K ? (size_t)Nu * Ny : (size_t)(Nt - 1) * Nu);
+    const size_t P = tg ? rollout_params(Nx, Ny, Nt, K != nullptr) : 0;
     const size_t o_ds = Bs * P * Nx, o_dm = o_ds + (method != GPMPC_METHOD_ME ? Bs * P * nn : 0);
     const size_t o_dv = o_dm + (size_t)Nt * Bs * Ny * P, o_g = o_dv + (size_t)Nt * Bs * Ny * P;
     const size_t n_mz = Bs * Ny * Nx, n_mS = Bs * Ny * nn, n_cz = Bs * Ny * Ny * Nx, n_g = em ? n_mz + n_mS + n_cz + n_cz * Nx : 0;
@@ -2672,24 +2705,17 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
     RolloutPolicy pol;
     rollout_policy(B, Nt, Ny, Nu, U, scale, K, x_ref, uscale, o_u, pin, d, &pol);
     CUDA_TRY(cudaMemcpyAsync(d, pin, o_m * 8, cudaMemcpyHostToDevice, h->st));
-    // 'EM': chunks of em_chunk points, the em_prepare_point blocks of the B points staged on the host
-    const int nc = em ? em_chunk(h, B) : 0;
-    const size_t per = em ? em_per(h) : 0;
+    // 'EM': the scratch of em_pass over the B points and, with tangents, the D = 2 records of a step's points and K^-1;
+    // the em_prepare_point blocks and gpmpc_predict_em_grad's blocks staged on the host
     if (em) {
-        rc = em_scratch(h, nc, B);
+        rc = em_scratch(h, B);
+        if (!rc && tg) rc = em_records_prepare(h, 2, B);
+        if (!rc && tg) rc = em_kinv_prepare(h);
         if (rc) return rc;
     }
-    // 'EM' tangents: the D = 2 records of the B points of a step, K^-1, and the host side of gpmpc_predict_em_grad's finish
-    if (em && tg) {
-        rc = em_records_prepare(h, 2, B);
-        if (rc) return rc;
-        rc = em_kinv_prepare(h);
-        if (rc) return rc;
-    }
-    const size_t rl = em && tg ? (size_t)h->em_rec[0].tb->nrec(Ny) * h->em_rec[0].tb->nent : 0;
-    std::vector<double> emp(Bs * per), recs(Bs * rl), mh(em && tg ? Bs * Ny : 0), hg(n_g);
+    std::vector<double> emp(em ? Bs * em_per(h) : 0), hg(n_g);
     const EmGradOutputs hgo = {hg.data(), hg.data() + n_mz, hg.data() + n_mz + n_mS, hg.data() + n_mz + n_mS + n_cz};
-    const int fb_smem = K ? (Ny + Nu * Ny) * 8 : 0;
+    const int fb_smem = rollout_feedback_smem(Ny, Nu, K != nullptr, true).bytes;
     for (int t = 0; t < Nt; ++t) {
         double* mean_t = d + o_m + (size_t)t * Bs * Ny;
         double* var_t = d + o_v + (size_t)t * Bs * Ny;
@@ -2698,71 +2724,43 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
             rc = predict_core(h, method, B, d, d + o_sig, 1, mean_t, var_t, cov_t, nullptr);
             if (rc) return rc;
         } else {
-            // the step's Sigma back to the host (step 0: Sigma0, already in the pinned mirror), its em_prepare_point blocks
-            // there (glibc's log and the host LU, the bits of gpmpc_predict(EM)), then the batched forward over the B points
+            // the step's Sigma back to the host (step 0: Sigma0, already in the pinned mirror), then predict_em's pass over
+            // the B points (the em_prepare_point blocks from glibc's log and the host LU: the bits of gpmpc_predict(EM))
             if (t > 0) {
                 CUDA_TRY(cudaMemcpyAsync(pin + o_sig, d + o_sig, Bs * Nx * Nx * 8, cudaMemcpyDeviceToHost, h->st));
                 CUDA_TRY(cudaStreamSynchronize(h->st));
             }
-            for (int b = 0; b < B; ++b) {
-                rc = em_prepare_point(h, pin + o_sig + (size_t)b * Nx * Nx, emp.data() + (size_t)b * per);
-                if (rc) {
-                    char why[512];
-                    snprintf(why, sizeof(why), "%s", h->err);
-                    set_error(h, "%s: step %d, trajectory %d: %s", fn, t, b, why);
-                    return rc;
-                }
-            }
-            CUDA_TRY(cudaMemcpyAsync(h->dEMP, emp.data(), emp.size() * 8, cudaMemcpyHostToDevice, h->st));
-            for (int b0 = 0; b0 < B; b0 += nc) {
-                const size_t o = (size_t)b0;
-                const int n = std::min(nc, B - b0);
-                rc = em_forward(h, n, d + o * Nx, h->dEMP + o * per, mean_t + o * Ny, var_t + o * Ny, cov_t + o * Ny * Ny);
-                if (rc) return rc;
-                if (tg) {                         // the chunk's records, from the scratch slots its forward left
-                    rc = em_chunk_records(h, n, d + o * Nx, h->dEMP + o * per, h->em_rec[0].rec + o * rl, nullptr);
-                    if (rc) return rc;
-                }
-            }
-            if (tg) {
-                // gpmpc_predict_em_grad's finish at (z_t, Sigma_t): records and means to the host (the step's second
-                // synchronisation), em_grad_finish per point with the Sigma_t and em_prepare_point blocks held here, the four
-                // blocks back to the device
-                CUDA_TRY(cudaMemcpyAsync(recs.data(), h->em_rec[0].rec, recs.size() * 8, cudaMemcpyDeviceToHost, h->st));
-                CUDA_TRY(cudaMemcpyAsync(mh.data(), mean_t, mh.size() * 8, cudaMemcpyDeviceToHost, h->st));
-                CUDA_TRY(cudaStreamSynchronize(h->st));
-                int bad = 0;
-                rc = em_grad_finish_points(h, B, pin + o_sig, 1, emp.data(), recs.data(), mh.data(), hgo, &bad);
-                if (rc) {
+            int bad = -1;
+            rc = em_pass(h, B, d, pin + o_sig, 1, emp.data(), mean_t, var_t, cov_t, tg != nullptr, false, &bad);
+            // gpmpc_predict_em_grad's finish at (z_t, Sigma_t), the step's second synchronisation; its blocks go back up below
+            if (!rc && tg) rc = em_grad_finish_points(h, B, pin + o_sig, 1, emp.data(), mean_t, hgo, &bad);
+            if (rc) {
+                if (bad >= 0) {                   // a rejected point: name the step and the trajectory
                     char why[512];
                     snprintf(why, sizeof(why), "%s", h->err);
                     set_error(h, "%s: step %d, trajectory %d: %s", fn, t, bad, why);
-                    return rc;
                 }
-                CUDA_TRY(cudaMemcpyAsync(h->dRollTg + o_g, hg.data(), hg.size() * 8, cudaMemcpyHostToDevice, h->st));
+                return rc;
             }
+            if (tg) CUDA_TRY(cudaMemcpyAsync(h->dRollTg + o_g, hg.data(), hg.size() * 8, cudaMemcpyHostToDevice, h->st));
         }
         if (tg) {                                 // the step's derivatives at the same points, then its tangents
-            const int nw = 8;
-            // largest layout: Ny = Nx = NX_MAX for J and the warps, Ny = Nu = NX_MAX / 2 for C K^T and K C (either kernel)
-            const int smem_max = (NX_MAX * NX_MAX + NX_MAX + NX_MAX * NX_MAX / 2 + nw * (2 * NX_MAX + 2 * NX_MAX * NX_MAX)) * 8;
+            // the opt-in covers every shape: either layout grows with Nu at a fixed Ny and with Ny at Nx = NX_MAX
+            const int smem_max = rollout_tangent_smem(NX_MAX, 0, em).bytes;
+            const int tg_smem = rollout_tangent_smem(Ny, Nu, em).bytes;
             double* g = h->dRollTg;
             if (!em) {                            // J_t, dvar_t, dcov_t
                 rc = derivs_enqueue(h, method, B, d, d + o_sig, 1, ds);
                 if (rc) return rc;
-                const int per_warp = Nx + Ny + Ny * Ny + Ny * Nx;
-                const int tg_smem = (Ny * Nx + Ny + 2 * Ny * Nu + nw * per_warp) * 8;
                 CUDA_TRY(smem_opt_in<rollout_tangent_kernel>(smem_max));
-                rollout_tangent_kernel<<<B, nw * 32, tg_smem, h->st>>>(Ny, Nu, (int)P, t, t == 0, t + 1 == Nt, method == GPMPC_METHOD_TA,
+                rollout_tangent_kernel<<<B, ROLL_TG_WARPS * 32, tg_smem, h->st>>>(Ny, Nu, (int)P, t, t == 0, t + 1 == Nt, method == GPMPC_METHOD_TA,
                                                                       h->dJ, ds.dvar, ds.dcov, mean_t, cov_t,
                                                                       pol.scale, pol.K, pol.x_ref, pol.uscale, g, g + o_ds, g + o_dm + (size_t)t * Bs * Ny * P,
                                                                       g + o_dv + (size_t)t * Bs * Ny * P);
             } else {
-                const int per_warp = Nx + Ny + Ny * Ny + Nu * Ny + Nx * Nx;
-                const int tg_smem = (Ny * Nx + Ny + 2 * Ny * Nu + nw * per_warp) * 8;
                 CUDA_TRY(smem_opt_in<rollout_tangent_em_kernel>(smem_max));
                 const double* G = g + o_g;
-                rollout_tangent_em_kernel<<<B, nw * 32, tg_smem, h->st>>>(Ny, Nu, (int)P, t, t == 0, t + 1 == Nt, G, G + n_mz,
+                rollout_tangent_em_kernel<<<B, ROLL_TG_WARPS * 32, tg_smem, h->st>>>(Ny, Nu, (int)P, t, t == 0, t + 1 == Nt, G, G + n_mz,
                                                                          G + n_mz + n_mS, G + n_mz + n_mS + n_cz, mean_t, cov_t,
                                                                          pol.scale, pol.K, pol.x_ref, pol.uscale, g, g + o_ds,
                                                                          g + o_dm + (size_t)t * Bs * Ny * P,
@@ -3267,7 +3265,7 @@ static int rollout_sample(gpmpc_handle_t h, const char* fn, int B, int Nt, const
     const int Nx = h->Nx, Ny = h->Ny, Nu = Nx - Ny, np = h->Npad, nl = h->nloc;
     rc = rollout_args(h, fn, B, Nt, !z0 || !eps || !samples, U, K);
     if (rc) return rc;
-    const int cond_smem = (Nt + 1) * 8 + Nt * 4;           // sample_cond_kernel: c | conditioning steps
+    const int cond_smem = sample_cond_smem(Nt).bytes;
     if (cond_smem > 48 * 1024) { set_error(h, "%s: Nt = %d steps exceed the conditioning kernel's shared memory", fn, Nt); return GPMPC_ERR_ARG; }
     if (tg && !dsamples) { set_error(h, "%s: null dsamples", fn); return GPMPC_ERR_ARG; }
     if (tg && Nt > SAMPLE_GRAD_NT_MAX) {
@@ -3286,10 +3284,10 @@ static int rollout_sample(gpmpc_handle_t h, const char* fn, int B, int Nt, const
     ENSURE(h->dSmp, tot);
     // tangent slab [G (nloc,B,Nt,2,Nx) | dR (nloc,B,P,Nt,Nt) | dz (Nt,B,P,Nx) | dsamples (Nt,B,Ny,P)]; the beta store is
     // laid out like the V store.  dsamples is mirrored in the pinned buffer after the draw's outputs.
-    const size_t P = !tg ? 0 : Nx + (K ? (size_t)Nu * Ny : (size_t)(Nt - 1) * Nu);
+    const size_t P = tg ? rollout_params(Nx, Ny, Nt, K != nullptr) : 0;
     const size_t o_dr = (size_t)nl * Bs * Nt * 2 * Nx, o_dz = o_dr + (size_t)nl * Bs * P * Nt * Nt;
     const size_t o_ds = o_dz + (size_t)Nt * Bs * P * Nx, nDs = tg ? (size_t)Nt * Bs * Ny * P : 0;
-    const int nw = 8, tg_smem = (Nt + 1 + Nt * Nt + nw * Nt) * 8 + Nt * 4, nx_smem = (Ny + nw * Ny) * 8;
+    const int tg_smem = sample_tangent_smem(Nt).bytes, nx_smem = sample_next_smem(Ny).bytes;
     DerivSlabs ds;
     if (tg) {
         rc = derivs_prepare(h, B, false, &ds);
@@ -3307,7 +3305,7 @@ static int rollout_sample(gpmpc_handle_t h, const char* fn, int B, int Nt, const
     rollout_policy(B, Nt, Ny, Nu, U, scale, K, x_ref, uscale, o_u, pin, d, &pol);
     memcpy(pin + o_z, z0, Bs * Nx * 8);                     // slot 0 of the input history
     CUDA_TRY(cudaMemcpyAsync(d, pin, (o_z + Bs * Nx) * 8, cudaMemcpyHostToDevice, h->st));
-    const int fb_smem = K ? Ny * 8 : 0;
+    const int fb_smem = rollout_feedback_smem(Ny, Nu, K != nullptr, false).bytes;
     double* g = tg ? h->dSmTg.p : nullptr;
     for (int t = 0; t < Nt; ++t) {
         double* Zt = d + o_z + (size_t)t * Bs * Nx;
@@ -3328,11 +3326,11 @@ static int rollout_sample(gpmpc_handle_t h, const char* fn, int B, int Nt, const
                 CUDA_TRY(cudaGetLastError());
             }
             double* ds_t = g + o_ds + (size_t)t * Bs * Ny * P;
-            sample_next_kernel<<<B, nw * 32, nx_smem, h->st>>>(Ny, Nu, (int)P, t, d + o_s + (size_t)(t > 0 ? t - 1 : 0) * Bs * Ny,
+            sample_next_kernel<<<B, ROLL_TG_WARPS * 32, nx_smem, h->st>>>(Ny, Nu, (int)P, t, d + o_s + (size_t)(t > 0 ? t - 1 : 0) * Bs * Ny,
                                                                ds_t - (t > 0 ? Bs * Ny * P : 0), pol.scale, pol.K, pol.x_ref,
                                                                pol.uscale, g + o_dz + (size_t)t * Bs * P * Nx);
             CUDA_TRY(cudaGetLastError());
-            sample_tangent_kernel<<<dim3(B, nl), nw * 32, tg_smem, h->st>>>(h->dSmV, sVa, np, h->N, d + o_z, h->dHyp, Nx + 2,
+            sample_tangent_kernel<<<dim3(B, nl), ROLL_TG_WARPS * 32, tg_smem, h->st>>>(h->dSmV, sVa, np, h->N, d + o_z, h->dHyp, Nx + 2,
                                                                            Nx, Ny, d, d + o_r, d + o_kp, h->dJ, ds.dvar, g,
                                                                            g + o_dz, g + o_dr, ds_t, (int)P, Nt, t);
             CUDA_TRY(cudaGetLastError());

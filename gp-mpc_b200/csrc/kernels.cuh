@@ -1979,6 +1979,28 @@ ks_mean_kernel(const double* __restrict__ PMJ, int nblk, int Nx, int H, int nloc
 // per-warp rows in shared memory under 48 KB
 #define SAMPLE_GRAD_NT_MAX 64
 
+// Warps of a CTA of the roll-outs' tangent stage (rollout_tangent_kernel, rollout_tangent_em_kernel, sample_next_kernel,
+// sample_tangent_kernel): each warp owns one parameter column at a time and a slice of the dynamic shared memory
+#define ROLL_TG_WARPS 8
+
+// The dynamic shared memory of the sampled roll-outs' kernels, written once for the kernel that carves it and for the
+// launch that sizes it: offsets in doubles from the start of the buffer, and the launch's bytes.  The offsets are 64-bit
+// sums of int terms, the address arithmetic of stepping a pointer term by term, which keeps the kernels' registers.
+// sample_cond_kernel: c (Nt + 1) | conditioning steps (Nt ints)
+struct SampleCondSmem { long long idx; int bytes; };
+__host__ __device__ __forceinline__ SampleCondSmem sample_cond_smem(int Nt)
+{
+    return {(long long)Nt + 1, (Nt + 1) * 8 + Nt * 4};
+}
+
+// sample_tangent_kernel: c (Nt + 1) | R (Nt Nt) | per warp dw (Nt) | conditioning steps (Nt ints)
+struct SampleTangentSmem { long long R, tw, idx; int bytes; };
+__host__ __device__ __forceinline__ SampleTangentSmem sample_tangent_smem(int Nt)
+{
+    const long long R = (long long)Nt + 1, tw = R + Nt * Nt, idx = tw + ROLL_TG_WARPS * Nt;
+    return {R, tw, idx, (int)idx * 8 + Nt * 4};
+}
+
 // The conditioning steps of (b, a) before step t into idx (thread 0; the caller synchronises), and their count
 __device__ __forceinline__ int sample_cond_steps(const double* __restrict__ kept, int B, int b, int Ny, int a, int t, int* idx)
 {
@@ -1989,7 +2011,7 @@ __device__ __forceinline__ int sample_cond_steps(const double* __restrict__ kept
 }
 
 // c[j] = k(z_t, z_s) - v_t . v_s for the k conditioning steps s = idx[j] and c[k] = sf2 - |v_t|^2, one warp per j (every
-// thread of a 256-thread CTA calls it; the caller synchronises).  Va: the V rows of output a; hp: its hyper row.  The
+// thread of a CTA of ROLL_TG_WARPS warps calls it; the caller synchronises).  Va: the V rows of output a; hp: its hyper row.  The
 // arithmetic of sample_cond_kernel's own loop, bit for bit (that kernel keeps its inline copy: calling these helpers
 // from it costs it a spill).
 __device__ __forceinline__ void sample_cond_c(const double* __restrict__ Va, int ldv, int N, const double* __restrict__ Zh,
@@ -1999,7 +2021,7 @@ __device__ __forceinline__ void sample_cond_c(const double* __restrict__ Va, int
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const double* vt = Va + ((long long)t * B + b) * ldv;
     const double* zt = Zh + ((long long)t * B + b) * Nx;
-    for (int j = warp; j <= k; j += 8) {                  // j = k: the point itself
+    for (int j = warp; j <= k; j += ROLL_TG_WARPS) {      // j = k: the point itself
         const int s = (j < k) ? idx[j] : t;
         const double dot = warp_dot(vt, Va + ((long long)s * B + b) * ldv, N);
         double q = 0.0;
@@ -2014,7 +2036,7 @@ __device__ __forceinline__ void sample_cond_c(const double* __restrict__ Va, int
 
 // One CTA per (trajectory b, output a) at step t, grid (B, nloc).  V rows of (a, s, b) at V + a sVa + (s B + b) ldv;
 // Zh (Nt, B, Nx); m (nloc, B) of this step; eps, xi (B, Nt, Ny) (xi may be null); Rf (nloc, B, Nt, Nt);
-// kept, samp (Nt, B, Ny).  Dynamic shared memory: c (Nt + 1 doubles) | conditioning steps (Nt ints).
+// kept, samp (Nt, B, Ny).  Dynamic shared memory: sample_cond_smem.
 __global__ void __launch_bounds__(256)
 sample_cond_kernel(const double* __restrict__ V, long long sVa, int ldv, int N, const double* __restrict__ m,
                    const double* __restrict__ Zh, const double* __restrict__ hyp, int hyp_ld, int Nx, int Ny,
@@ -2026,7 +2048,7 @@ sample_cond_kernel(const double* __restrict__ V, long long sVa, int ldv, int N, 
     const int b = blockIdx.x, a = blockIdx.y, B = gridDim.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     double* c = sc_sh;
-    int* idx = reinterpret_cast<int*>(sc_sh + Nt + 1);
+    int* idx = reinterpret_cast<int*>(sc_sh + sample_cond_smem(Nt).idx);
     const double* hp = hyp + (long long)a * hyp_ld;
     const double* Va = V + (long long)a * sVa;
     const double* vt = Va + ((long long)t * B + b) * ldv;
@@ -2164,16 +2186,15 @@ sample_cross_kernel(const double* __restrict__ Beta, long long sBa, int ldb, con
     }
 }
 
-// The tangent stage of one sampled step, one CTA per (trajectory b, output a), grid (B, nloc), 8 warps over the P
-// parameter columns.  With w = R^-1 c and d = c_tt - |w|^2 re-formed as sample_cond_kernel forms them and the kept flag of
+// The tangent stage of one sampled step, one CTA per (trajectory b, output a), grid (B, nloc), ROLL_TG_WARPS warps over
+// the P parameter columns.  With w = R^-1 c and d = c_tt - |w|^2 re-formed as sample_cond_kernel forms them and the kept flag of
 // step t (the branch the draw took), per column p:
 //   dm = J_t dz_t,  dc_tt = dvar_dz_t . dz_t,  dc_j = g(t,s_j) . dz_t + g(s_j,t) . dz_{s_j},
 //   dw = R^-1 (dc - dR w),  dd = dc_tt - 2 w . dw,  df = dm + dw . eps_S (+ dd / (2 sqrt d) eps_t when kept),
 // and when kept the new row [dw, dd / (2 sqrt d)] of dR.  J, dvar (B, Ny, Nx) of the derivative chain at the step's points;
 // G of sample_cross_kernel; dZh (Nt, B, P, Nx) the tangent history; dRf (nloc, B, P, Nt, Nt); dsamp (B, Ny, P) of step t.
-// Every sum runs in index order in one thread.  Dynamic shared memory: c (Nt + 1) | R (Nt Nt) | per warp dw (Nt) |
-// conditioning steps (Nt ints).
-__global__ void __launch_bounds__(256)
+// Every sum runs in index order in one thread.  Dynamic shared memory: sample_tangent_smem.
+__global__ void __launch_bounds__(ROLL_TG_WARPS * 32)
 sample_tangent_kernel(const double* __restrict__ V, long long sVa, int ldv, int N, const double* __restrict__ Zh,
                       const double* __restrict__ hyp, int hyp_ld, int Nx, int Ny, const double* __restrict__ eps,
                       const double* __restrict__ Rf, const double* __restrict__ kept, const double* __restrict__ J,
@@ -2184,10 +2205,11 @@ sample_tangent_kernel(const double* __restrict__ V, long long sVa, int ldv, int 
     __shared__ int nk_s;
     const int b = blockIdx.x, a = blockIdx.y, B = gridDim.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const SampleTangentSmem L = sample_tangent_smem(Nt);
     double* c = st_sh;
-    double* sR = c + Nt + 1;
-    double* tw = sR + Nt * Nt + warp * Nt;
-    int* idx = reinterpret_cast<int*>(sR + Nt * Nt + 8 * Nt);
+    double* sR = st_sh + L.R;
+    double* tw = st_sh + L.tw + warp * Nt;
+    int* idx = reinterpret_cast<int*>(st_sh + L.idx);
     const double* hp = hyp + (long long)a * hyp_ld;
     const double* R = Rf + ((long long)a * B + b) * Nt * Nt;
     if (tid == 0) nk_s = sample_cond_steps(kept, B, b, Ny, a, t, idx);
@@ -2195,7 +2217,7 @@ sample_tangent_kernel(const double* __restrict__ V, long long sVa, int ldv, int 
     const int k = nk_s;
     const double sf2 = hp[Nx] * hp[Nx];
     sample_cond_c(V + (long long)a * sVa, ldv, N, Zh, hp, Nx, B, b, t, k, idx, sf2, c);
-    for (int i = tid; i < k * Nt; i += 256) sR[i] = R[i];
+    for (int i = tid; i < k * Nt; i += ROLL_TG_WARPS * 32) sR[i] = R[i];
     __syncthreads();
     if (tid == 0) {                                       // w and d with sample_cond_kernel's arithmetic
         double ww = 0.0;
@@ -2215,7 +2237,7 @@ sample_tangent_kernel(const double* __restrict__ V, long long sVa, int ldv, int 
     const double* Ja = J + ((long long)b * Ny + a) * Nx;
     const double* dva = dvar + ((long long)b * Ny + a) * Nx;
     const double* Gab = G + ((long long)a * B + b) * Nt * 2 * Nx;
-    for (int p = warp; p < P; p += 8) {
+    for (int p = warp; p < P; p += ROLL_TG_WARPS) {
         const double* dzt = dZh + (((long long)t * B + b) * P + p) * Nx;
         double* dR = dRf + (((long long)a * B + b) * P + p) * Nt * Nt;
         for (int j = lane; j < k; j += 32) {              // dc_j - (dR w)_j

@@ -728,7 +728,7 @@ class GP:
         if self.__prior_mean_in_predict and self.__has_prior_mean():
             raise NotImplementedError('rollout_grad differentiates the zero-mean posterior the engine holds; '
                                       'prior_mean_in_predict with a prior mean function is not supported')
-        Nx, Ny, Nu = self.__Nx, self.__Ny, self.__Nu
+        Ny = self.__Ny
         X0, U, single, Nt = self.__trajectories(x0, u)
         nb = X0.shape[0]
         if Nt < 1:
@@ -739,7 +739,7 @@ class GP:
         covar = self.__initial_covar(nb)
         z0, Ug, scale, uscale = self.__engine_start(X0, U, K, x_ref)
         sY = self.__stdY if self.__normalize else np.ones(Ny)
-        P = Nx + (Nu * Ny if K is not None else (Nt - 1) * Nu)
+        P = self.__params(Nt, K)
         m_std = np.empty((nb, Nt, Ny)); v_std = np.empty((nb, Nt, Ny))
         Dm = np.empty((nb, Nt, Ny, P)); Dv = np.empty((nb, Nt, Ny, P))
         for g, Kg in self.__gain_groups(K, nb):
@@ -762,6 +762,11 @@ class GP:
         if single:
             return {k: v[0] for k, v in out.items()}
         return out
+
+    def __params(self, Nt, K):
+        """P, the engine's derivative columns of a roll-out: [z0 | U rows 1 .. Nt-1] open loop, [z0 | K row-major] with K."""
+        Nu = self.__Nu
+        return self.__Nx + (Nu * self.__Ny if K is not None else (Nt - 1) * Nu)
 
     def __caller_derivs(self, D, X0, K, x_ref, identity):
         """The engine's derivative columns D (n, Nt, Ny, P) of a quantity already in caller units, for trajectories that
@@ -844,9 +849,9 @@ class GP:
         if not hasattr(self.__engine, 'rollout_sample_grad'):
             raise NotImplementedError('sample_rollout_grad needs an engine with gpmpc_rollout_sample_grad')
         d = self.__sample_setup('sample_rollout_grad', x0, u, n_samples, seed, Sigma0, feedback, x_ref, Q, R, process_noise)
-        nb, ns, Nt, Ny, Nx, Nu = d['nb'], d['ns'], d['Nt'], self.__Ny, self.__Nx, self.__Nu
+        nb, ns, Nt, Ny = d['nb'], d['ns'], d['Nt'], self.__Ny
         K = d['K']
-        P = Nx + (Nu * Ny if K is not None else (Nt - 1) * Nu)
+        P = self.__params(Nt, K)
         samp = np.empty((nb * ns, Nt, Ny)); kept = np.empty((nb * ns, Nt, Ny), dtype=np.int32)
         D = np.empty((nb * ns, Nt, Ny, P))
         for r, Kg in d['passes']:

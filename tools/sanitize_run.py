@@ -1,7 +1,8 @@
 """Small end-to-end pass over every kernel of the engine for compute-sanitizer
 (memcheck / racecheck / synccheck / initcheck):  K build, leaf + DMMA GEMMs (cp.async feeds; the TMA
 tensor-map feed on a second, 24-output handle), alpha, NLML + gradient, the persistent stream-K predict kernel with tile
-fix-ups (several grid sizes, lower and upper mode), gpmpc_predict_device, gpmpc_predict's copy transports, predict_grad, EM and its derivatives, rank-1 append, greedy append, removal, GP.covar, sampled roll-outs, leave-one-out cross-validation and its gradient.
+fix-ups (several grid sizes, lower and upper mode), gpmpc_predict_device, gpmpc_predict's copy transports, predict_grad, EM and its derivatives, rank-1 append, greedy append, removal, GP.covar, sampled and batched roll-outs
+(ME, TA, EM) with their tangents, leave-one-out cross-validation and its gradient.
     compute-sanitizer --tool racecheck python tools/sanitize_run.py"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -50,6 +51,19 @@ sm, _, kept = eng.rollout_sample(p['Z'][:3], np.repeat(p['Z'][:3, None, Ny:], 4,
 print('rollout_sample finite', bool(np.isfinite(sm).all()), int(kept.sum()), flush=True)
 smg, _, _, dsm = eng.rollout_sample_grad(p['Z'][:3], np.repeat(p['Z'][:3, None, Ny:], 4, 1), np.ones((3, 4, Ny)))
 print('rollout_sample_grad finite', bool(np.isfinite(dsm).all()), np.array_equal(smg, sm), flush=True)
+# batched roll-outs and their tangents: 'TA' with a feedback gain, 'ME' open loop, and 'EM' one point per chunk
+zb, Ub, Sb = p['Z'][:3], np.repeat(p['Z'][:3, None, Ny:], 3, 1), np.tile(1e-4 * np.eye(Nx), (3, 1, 1))
+for name, meth, Kb in (('TA K', L.METHOD_TA, 0.1 * np.ones((Nx - Ny, Ny))), ('ME', L.METHOD_ME, None)):
+    rb = eng.rollout_batch(zb, Ub, Sb, meth, K=Kb)
+    rg = eng.rollout_batch_grad(zb, Ub, Sb, meth, K=Kb)
+    print('rollout_batch(_grad) %s' % name, all(np.array_equal(a, b) for a, b in zip(rb, rg)),
+          bool(np.isfinite(rg[3]).all() and np.isfinite(rg[4]).all()), flush=True)
+eng.set_option('em_points', 1)
+re_ = eng.rollout_batch_em(zb[:2], Ub[:2, :2], Sb[:2])
+reg = eng.rollout_batch_em_grad(zb[:2], Ub[:2, :2], Sb[:2])
+print('rollout_batch_em(_grad)', all(np.array_equal(a, b) for a, b in zip(re_, reg)),
+      bool(np.isfinite(reg[3]).all() and np.isfinite(reg[4]).all()), flush=True)
+eng.set_option('em_points', 0)
 _, _, ln = eng.loo()
 fl, gl = eng.loo_nlpp(0, p['hyper'][0] * 0.9, grad=True)
 print('loo', ln, fl, bool(np.isfinite(gl).all()), flush=True)
