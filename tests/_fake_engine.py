@@ -1,10 +1,14 @@
-"""CPU stand-in for gp_mpc_b200.Engine used ONLY by the world_size-2 gloo tests of the
-host-side multi-GPU logic (partitioning, id broadcast, hyper gather, result assembly).
-The numerics come from the oracle; the product never imports this."""
+"""CPU stand-ins for gp_mpc_b200.Engine, for the tests of the host-side logic without a GPU: the world_size-2 gloo tests
+of the multi-GPU logic (partitioning, id broadcast, hyper gather, result assembly), the GP class and the roll-outs; and
+the fixture GPs and problems those tests build on them.  The numerics come from the oracle; the product never imports
+this."""
 import numpy as np
 import torch.distributed as dist
 
+import gp_mpc_b200
+from gp_mpc_b200.gp_class import _matmul_seq
 from oracle import gp_oracle as orc
+from tests._util import load_fixture
 
 
 class OracleEngine:
@@ -108,3 +112,92 @@ class OracleEngineWithRollout(OracleEngine):
                 Sg[:Ny, :Ny] = cov[0]
         return means, var, cov[0]
 
+
+
+class OracleEngineWithRolloutBatch(OracleEngineWithRollout):
+    """Adds a numpy restatement of gpmpc_rollout_batch (include/gpmpc.h): one predict step for all trajectories, then
+    rollout_feedback_kernel's update per trajectory."""
+
+    def rollout_batch(self, z0, U, Sigma0, method=1, scale=None, K=None, x_ref=None, uscale=None):
+        Ny, Nx = self.Ny, self.Nx
+        Nu = Nx - Ny
+        Z = np.array(z0, dtype=np.float64).reshape(-1, Nx)
+        B, Nt = Z.shape[0], np.shape(U)[1]
+        S = np.array(Sigma0, dtype=np.float64).reshape(B, Nx, Nx)
+        means = np.empty((B, Nt, Ny)); var = np.empty((B, Nt, Ny)); cov = None
+        for t in range(Nt):
+            # every trajectory's point on its own, as the device computes each point independently of the others
+            parts = [self.predict(Z[b:b + 1], S[b], method, True, False) for b in range(B)]
+            m = np.concatenate([p[0] for p in parts]); cov = np.concatenate([p[2] for p in parts])
+            means[:, t] = m
+            var[:, t] = np.diagonal(cov, axis1=1, axis2=2)
+            if t + 1 == Nt:
+                break
+            x = m if scale is None else m * scale[0] + scale[1]
+            Z[:, :Ny] = x if scale is None else (x - scale[2]) / scale[3]
+            for b in range(B):
+                if K is None:
+                    Z[b, Ny:] = U[b, t + 1]
+                else:
+                    ub = _matmul_seq(K, (x[b] - (0.0 if x_ref is None else x_ref))[:, None])[:, 0]
+                    Z[b, Ny:] = ub if uscale is None else (ub - uscale[0]) / uscale[1]
+                    cov_xu = _matmul_seq(cov[b], K.T)
+                    S[b, Ny:, Ny:] = _matmul_seq(_matmul_seq(K, cov[b]), K.T)
+                    S[b, Ny:, :Ny] = cov_xu.T
+                    S[b, :Ny, Ny:] = cov_xu
+                S[b, :Ny, :Ny] = cov[b]
+        return means, var, cov
+
+
+class TwoRanks:
+    """A two-rank communicator stand-in: enough for a GP sharded by output to be built on one process."""
+    rank, world = 0, 2
+
+    def broadcast_object(self, obj, src=0):
+        return obj
+
+    def allgather_object(self, obj):
+        return [obj, obj]
+
+    def barrier(self):
+        pass
+
+
+def sharded(base):
+    """base with a comm_init that only records its rank and world: with TwoRanks, a GP sharded by output is built on one
+    process."""
+    class ShardEngine(base):
+        def comm_init(self, uid, rank, world):
+            self.rank, self.world = rank, world
+    return ShardEngine
+
+
+def fixture_gp(name, factory=None, **kw):
+    """A GP of a stored fixture with its hyper-parameters (the engine factorises), and the fixture; factory replaces the
+    device engine, kw override GP's arguments."""
+    m = load_fixture(name)
+    args = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'], hyper=dict(hyper=m['hyper']))
+    if factory is not None:
+        args['engine_factory'] = factory
+    if m['normalize']:
+        args.update(meta=m['meta'], xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
+    args.update(kw)
+    return gp_mpc_b200.GP(m['X'], m['Y'], **args), m
+
+
+def sample_model(name):
+    """The model dict of a fixture, or of the synthetic problem of the sampled roll-out tests."""
+    if name == 'synthetic':
+        p = orc.synthetic_problem(150, 5, 3, config_id=2)
+        p['hyper'][:, :5] = 1.5
+        return dict(X=p['X'], Y=p['Y'], hyper=p['hyper'], normalize=False)
+    return load_fixture(name)
+
+
+def problem(case):
+    """X, Y, hyper of a stored fixture ('tank', 'car') or of a small synthetic problem."""
+    if case in ('tank', 'car'):
+        m = load_fixture(case)
+        return m['X'], m['Y'], m['hyper']
+    p = orc.synthetic_problem(300, 5, 2, config_id=17)
+    return p['X'], p['Y'], p['hyper']

@@ -117,3 +117,12 @@ def rollout_sample_grad(model, Linv, z0, U, eps, xi=None, scale=None, K=None, x_
             z, dz = np.concatenate([zx, un]), np.concatenate([dzx, du])
         z_out[b] = Z
     return dict(samples=samples, z_out=z_out, kept=kept, dsamples=D, d=dvals)
+
+
+MARGIN = 1e3                # every d is at least MARGIN delta sf2 away from the delta rule's threshold
+
+
+def assert_margin(d, hyper):
+    Nx = hyper.shape[1] - 2
+    thr = so.DELTA * hyper[:, Nx] ** 2
+    assert (np.abs(d - thr) >= MARGIN * thr).all(), 'a step sits within the margin of the delta rule'

@@ -2,7 +2,6 @@
 downdate the CUDA path runs, the host selection path of the GP class through an oracle-backed engine without a device
 selection, standardisation, argument checks, and two gloo ranks with sharded outputs."""
 import os
-import socket
 
 import numpy as np
 import pytest
@@ -13,7 +12,7 @@ import gp_mpc_b200
 from oracle import gp_oracle as orc
 from oracle import greedy_oracle as gro
 from tests._fake_engine import OracleEngine
-from tests._util import load_fixture
+from tests._util import free_port, load_fixture
 
 
 class HostSelectEngine(OracleEngine):
@@ -119,10 +118,6 @@ def test_no_op_and_argument_errors():
         gp.update_data(X_new, Y_new)
 
 
-def _free_port():
-    s = socket.socket(); s.bind(('127.0.0.1', 0)); p = s.getsockname()[1]; s.close(); return p
-
-
 def _worker(rank, world, port, q):
     os.environ['MASTER_ADDR'] = '127.0.0.1'; os.environ['MASTER_PORT'] = str(port)
     dist.init_process_group('gloo', rank=rank, world_size=world)
@@ -145,7 +140,7 @@ def test_two_ranks_with_sharded_outputs_pick_the_same_points():
     world = 2
     ctx = mp.get_context('spawn')
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
     for pr in procs:
         pr.start()
@@ -212,7 +207,7 @@ def test_replicated_ranks_make_the_refit_decision_together():
     world = 2
     ctx = mp.get_context('spawn')
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_replicated_worker, args=(r, world, port, q)) for r in range(world)]
     for pr in procs:
         pr.start()

@@ -7,24 +7,13 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle import greedy_oracle as gro
+from tests._engines import fit
 from tests._util import load_fixture, relinf
 
 pytestmark = pytest.mark.gpu
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _fit(X, Y, hyper, **kw):
-    eng = _L().Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, **kw)
-    eng.set_data(X, Y)
-    eng.set_hyper(hyper)
-    eng.factorize()
-    return eng
 
 
 def _pool(X, n, scale, seed):
@@ -55,7 +44,6 @@ def _preds_vs(eng, X, Y, hyper, Z, Sigma):
     post = orc.postfit(X, Y, hyper, lapack_general_solve=False)
     mo, vo = orc.gp_mean_var(X, hyper, post['alpha'], post['chol'], Z)
     Jo = orc.gp_mean_jac(X, hyper, post['alpha'], Z)
-    L = _L()
     m, v, c, J = eng.predict(Z, Sigma, L.METHOD_TA)
     assert relinf(m, mo) < 1e-6 and relinf(v, vo) < 1e-6 and relinf(J, Jo) < 1e-6
     assert relinf(c, orc.ta_cov(vo, Jo, Sigma)) < 1e-6
@@ -67,11 +55,10 @@ def _preds_vs(eng, X, Y, hyper, Z, Sigma):
 @pytest.mark.parametrize('case', CASES, ids=[str(c) for c in CASES])
 def test_picks_and_model_match_the_oracle(case):
     X, Y, hyper, Xc, Yc, n_new = case_data(case)
-    L = _L()
     N = X.shape[0]
     ref = gro.greedy_select(X, hyper, Xc, n_new)
     assert np.all(ref['gap'] > 1e-8)                       # no near-tie: the picks are well defined
-    eng = _fit(X, Y, hyper, capacity=N + n_new)
+    eng = fit(X, Y, hyper, capacity=N + n_new)
     picked, score, ok = eng.append_greedy(Xc, Yc, n_new)
     assert ok and eng.N == N + n_new
     np.testing.assert_array_equal(picked, ref['picked'])
@@ -90,7 +77,7 @@ def test_picks_and_model_match_the_oracle(case):
         assert relinf(eng.get(L.GET_CHOL, a), post['chol'][a]) < tol_chol
         assert relinf(eng.get(L.GET_ALPHA, a), post['alpha'][a]) < tol_alpha
     # the derivative caches (Li^T, EM K^-1) follow the appends: same results as a handle fitted on the augmented data
-    ref_eng = _fit(Xa, Ya, hyper)
+    ref_eng = fit(Xa, Ya, hyper)
     g1, g2 = eng.predict_grad(Z, Sigma, L.METHOD_TA), ref_eng.predict_grad(Z, Sigma, L.METHOD_TA)
     for k in ('mean', 'var', 'jac', 'dvar_dz', 'dcov_dz'):
         assert relinf(g1[k], g2[k]) < 1e-6, k
@@ -104,10 +91,9 @@ def test_picks_and_model_match_the_oracle(case):
 
 def test_two_calls_give_identical_bits():
     X, Y, hyper, Xc, Yc, _ = case_data((700, 5, 3, 300, 17))
-    L = _L()
     out = []
     for _ in range(2):
-        eng = _fit(X, Y, hyper, capacity=X.shape[0] + 40)
+        eng = fit(X, Y, hyper, capacity=X.shape[0] + 40)
         picked, score, ok = eng.append_greedy(Xc, Yc, 40)
         assert ok
         out.append((picked, score, [eng.get(L.GET_CHOL, a) for a in range(3)], [eng.get(L.GET_LINV, a) for a in range(3)]))
@@ -123,8 +109,7 @@ def test_two_calls_give_identical_bits():
 def test_reserved_capacity_matches_an_unreserved_handle(N):
     p = orc.synthetic_problem(N, 4, 2, config_id=N + 3, H=6)
     X, Y, hyper, Z, Sigma = p['X'], p['Y'], p['hyper'], p['Z'], p['Sigma']
-    L = _L()
-    plain, res = _fit(X, Y, hyper), _fit(X, Y, hyper, capacity=N + 300)
+    plain, res = fit(X, Y, hyper), fit(X, Y, hyper, capacity=N + 300)
     assert plain.capacity == -(-N // 128) * 128 and res.capacity == -(-(N + 300) // 128) * 128
     # a larger padded size splits the recursion and the predict product's stream-K work differently: rounding only
     for a in range(2):
@@ -174,7 +159,6 @@ def test_gp_selects_at_a_full_padded_size_in_one_device_call(monkeypatch):
 
 def test_state_and_argument_errors_leave_the_model_untouched():
     X, Y, hyper, Xc, Yc, _ = case_data((130, 2, 3, 65, 65))
-    L = _L()
     lib = L.load()
     Z = X[:4] + 0.1
     ip = C.POINTER(C.c_int)
@@ -187,7 +171,7 @@ def test_state_and_argument_errors_leave_the_model_untouched():
             P=picked.ctypes.data_as(ip), A=C.byref(added)).items()}
         return lib.gpmpc_append_greedy(eng.h, n, ptr['X'], ptr['Y'], n_new, ptr['P'], None, ptr['A'])
 
-    eng = _fit(X, Y, hyper)                                # capacity 256
+    eng = fit(X, Y, hyper)                                # capacity 256
     before = eng.predict(Z, 1e-4 * np.eye(2), L.METHOD_TA)
     assert call(eng, 65, 66) == L.ERR_ARG                  # n_new > n
     assert call(eng, 65, -1) == L.ERR_ARG
@@ -201,7 +185,7 @@ def test_state_and_argument_errors_leave_the_model_untouched():
     for u, v in zip(before, after):
         assert u.tobytes() == v.tobytes()
     assert eng.N == 130
-    sharded = _fit(X, Y, hyper, out_begin=1, out_count=2)
+    sharded = fit(X, Y, hyper, out_begin=1, out_count=2)
     assert call(sharded, 65, 3) == L.ERR_STATE
     fresh = L.Engine(X.shape[0], 2, 3, device=0, capacity=200)
     fresh.set_data(X, Y)
@@ -252,7 +236,7 @@ def _singular_problem():
 
 
 def _greedy_raw(eng, Xc, Yc, n_new):
-    lib = _L().load()
+    lib = L.load()
     Xc = np.ascontiguousarray(Xc, dtype=np.float64); Yc = np.ascontiguousarray(Yc, dtype=np.float64)
     picked = np.full(n_new, -1, dtype=np.int32); score = np.zeros(n_new); added = C.c_int(-7)
     rc = lib.gpmpc_append_greedy(eng.h, Xc.shape[0], Xc.ctypes.data_as(C.POINTER(C.c_double)),
@@ -264,13 +248,12 @@ def _greedy_raw(eng, Xc, Yc, n_new):
 @pytest.mark.parametrize('where', ['last', 'earlier', 'only'])
 def test_a_failed_pivot_is_reported_at_any_pick(where):
     X, Y, hyper, far = _singular_problem()
-    L = _L()
     N = X.shape[0]
     Xc = {'last': [far[0], far[1], X[5]], 'earlier': [X[5], far[0], X[7], far[1]], 'only': [X[5]]}[where]
     Xc = np.array(Xc)
     n_new = Xc.shape[0]
     Yc = np.zeros((n_new, 2))
-    eng = _fit(X, Y, hyper, capacity=N + n_new)
+    eng = fit(X, Y, hyper, capacity=N + n_new)
     rc, added, picked, score = _greedy_raw(eng, Xc, Yc, n_new)
     assert rc == L.ERR_NOTPD
     assert 'positive definiteness' in L.load().gpmpc_last_error(eng.h).decode()
@@ -287,7 +270,6 @@ def test_a_failed_pivot_is_reported_at_any_pick(where):
 def test_gp_recovers_from_failed_pivots_by_refactorising():
     import gp_mpc_b200
     X, Y, hyper, far = _singular_problem()
-    L = _L()
     gp = gp_mpc_b200.GP(X, Y, hyper=dict(hyper=hyper), normalize=False)
     Xc = np.array([X[5], far[0], X[7], far[1]])
     Yc = np.random.default_rng(1).standard_normal((4, 2))

@@ -7,19 +7,13 @@ import re
 
 import numpy as np
 import pytest
+from tests._engines import built_lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _lib():
-    import __graft_entry__ as g
-    g.build()
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
 def test_library_exports_every_declared_symbol():
-    L = _lib()
+    L = built_lib()
     lib = L.load()
     hdr = open(os.path.join(ROOT, 'include', 'gpmpc.h')).read()
     declared = set(re.findall(r'\b(gpmpc_[A-Za-z_0-9]+)\s*\(', hdr))
@@ -38,7 +32,7 @@ def test_no_cpu_fallback():
     import torch
     if torch.cuda.is_available():
         pytest.skip('GPU present')
-    L = _lib()
+    L = built_lib()
     with pytest.raises(L.GpmpcError) as e:
         L.Engine(10, 2, 1)
     assert 'no CPU path' in str(e.value)
@@ -97,7 +91,7 @@ def test_bench_workload_generator_matches_the_oracle_generator():
 
 def test_casadi_external_metadata_without_a_gpu():
     """The `casadi.external` helper functions answer without a device; patterns exist only once bound."""
-    lib = _lib().load()
+    lib = built_lib().load()
     assert lib.gp_b200_n_in() == 2 and lib.gp_b200_n_out() == 2
     assert lib.jac_gp_b200_n_in() == 4 and lib.jac_gp_b200_n_out() == 4
     assert [lib.gp_b200_name_in(i) for i in range(2)] == [b'z', b'sigma']

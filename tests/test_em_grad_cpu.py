@@ -8,8 +8,8 @@ from scipy.linalg import cho_solve
 from oracle import em_grad_oracle as emo
 from oracle import gp_oracle as orc
 from oracle import hess_oracle as hor
+from tests._em_cases import sigmas
 from tests._util import load_fixture, relinf
-from tests.test_em_shapes_gpu import sigmas
 
 
 def _problem(case):

@@ -8,61 +8,16 @@ import numpy as np
 import pytest
 from scipy.linalg import cho_solve
 
+from gp_mpc_b200 import _lib as L
 from oracle import em_grad_oracle as emo
 from oracle import gp_oracle as orc
+from tests._em_cases import check_case, em_errors, em_terms, engine_alpha_chol, grad_case, tma_on_device
+from tests._engines import ccs, fit, gp_from_fixture, require
 from tests._util import load_fixture, load_golden, relinf
-from tests.test_dispatch_gpu import _require
-from tests.test_em_shapes_gpu import CASES, check_case, em_errors, em_problem, em_terms, sigmas, tma_on_device
 
 pytestmark = pytest.mark.gpu
 
 DERIV = ('dmean_dz', 'dmean_dSigma', 'dcov_dz', 'dcov_dSigma')
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _fit(X, Y, hyper, **kw):
-    import gp_mpc_b200
-    eng = gp_mpc_b200.Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, **kw)
-    eng.set_data(X, Y)
-    eng.set_hyper(hyper)
-    eng.factorize()
-    return eng
-
-
-def _case(case):
-    """X, Y, hyper, Z, Sigma and the handle's capacity of a case; '<shape>_s<scale>' is a case of test_em_shapes_gpu at
-    the input covariance of that scale (0.1 Lambda correlated, or Lambda)."""
-    if '_s' in case:
-        name, scale = case.split('_s')
-        X, Y, hyper, Z = em_problem(name)
-        return X, Y, hyper, Z[:1] if name == 'tma' else Z[:2], sigmas(hyper, X.shape[1])[scale], CASES[name][3]
-    if case.startswith('tank'):
-        m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
-        rng = np.random.default_rng(5)
-        Nx = X.shape[1]
-        Z = X[rng.choice(X.shape[0], 4, replace=False)] + 0.05 * rng.standard_normal((4, Nx))
-        A = rng.standard_normal((Nx, Nx)); Sigma = 1e-3 * np.eye(Nx) + 1e-4 * A @ A.T
-        if case == 'tank_large':          # about a tenth of the smallest length scale squared
-            Sigma = 0.1 * np.min(hyper[:, :Nx] ** 2) * (np.eye(Nx) + 0.1 * (A @ A.T) / np.abs(A @ A.T).max())
-        if case == 'tank_pp':
-            Sigma = np.stack([Sigma * (1 + 0.1 * h) for h in range(Z.shape[0])])
-        return X, Y, hyper, Z, Sigma, None
-    N, Nx, Ny, H = {'syn1000': (1000, 8, 4, 3), 'syn300': (300, 17, 2, 2), 'syn12': (600, 12, 3, 3)}[case]
-    p = orc.synthetic_problem(N, Nx, Ny, config_id=N + Nx, H=H)
-    hyper = p['hyper']
-    if case == 'syn12':                   # well-conditioned (sn = 0.3): alpha and K^-1 carry no conditioning error
-        hyper = hyper.copy(); hyper[:, Nx + 1] = 0.3
-    return p['X'], p['Y'], hyper, p['Z'], p['Sigma'], None
-
-
-def _engine_factor(eng, Ny):
-    L = _L()
-    return (np.stack([eng.get(L.GET_ALPHA, a) for a in range(Ny)]),
-            np.stack([eng.get(L.GET_CHOL, a) for a in range(Ny)]))
 
 
 def forward_errors(o, ref, X, hyper, alpha, chol, Z, Sigma):
@@ -92,10 +47,9 @@ FWD_TOL = (1e-15, 1e-15)
 def em_grad_errors(case):
     """The engine's predict_em_grad on a case against em_grad_closed on the engine's own alpha and factor: relative errors
     of the four derivatives and normalised errors of mean and cov, after the bit-level checks."""
-    X, Y, hyper, Z, Sigma, cap = _case(case)
+    X, Y, hyper, Z, Sigma, cap = grad_case(case)
     Ny = Y.shape[1]
-    eng = _fit(X, Y, hyper, capacity=cap)
-    L = _L()
+    eng = fit(X, Y, hyper, capacity=cap)
     o = eng.predict_em_grad(Z, Sigma)
     mean, var, cov, _ = eng.predict(Z, Sigma, L.METHOD_EM, want_jac=False)
     assert np.array_equal(o['mean'], mean) and np.array_equal(o['var'], var) and np.array_equal(o['cov'], cov)
@@ -108,7 +62,7 @@ def em_grad_errors(case):
     o2 = eng.predict_em_grad(Z, Sigma)
     for k in o:
         assert np.array_equal(o[k], o2[k]), k
-    alpha, chol = _engine_factor(eng, Ny)
+    alpha, chol = engine_alpha_chol(eng, Ny)
     eng.close()
     ref = emo.em_grad_closed(X, hyper, alpha, chol, Z, Sigma)
     errs = {k: relinf(o[k], ref[k]) for k in DERIV}
@@ -124,7 +78,7 @@ def test_em_grad_vs_closed_oracle(case):
     em_backbone_rows and trmv_lower_T on the 3072 pad), ny9 (nine outputs' records) and reserved (an identity tail of
     L^-1)."""
     if case.startswith('tma'):
-        _require(tma_on_device(), 'the TMA feed')
+        require(tma_on_device(), 'the TMA feed')
     errs = em_grad_errors(case)
     tm, tc = GRAD_TOL.get(case, (1e-6, 1e-5))
     assert errs['dmean_dz'] < tm and errs['dmean_dSigma'] < tm, errs
@@ -139,9 +93,9 @@ def test_em_forward_nxp16_vs_exact_moment():
     3.9e-11 (the restatement's own cancellation between beta beta^T and K^-1).  Then the nx12 case of test_em_shapes_gpu
     (N = 600, Ny = 3) against the long-double formula on the engine's alpha and factor at Sigma = 1e-5 Lambda, 0.1 Lambda
     and Lambda, under that file's bars (measured: mean 2.7e-17, cov 1.2e-18 of the sums of |terms|)."""
-    X, Y, hyper, Z, Sigma, _ = _case('syn12')
-    eng = _fit(X, Y, hyper)
-    mean, _, cov, _ = eng.predict(Z, Sigma, _L().METHOD_EM, want_jac=False)
+    X, Y, hyper, Z, Sigma, _ = grad_case('syn12')
+    eng = fit(X, Y, hyper)
+    mean, _, cov, _ = eng.predict(Z, Sigma, L.METHOD_EM, want_jac=False)
     eng.close()
     post = orc.postfit(X, Y, hyper, lapack_general_solve=False)
     for h in range(Z.shape[0]):
@@ -159,8 +113,7 @@ def test_em_grad_vs_differences_of_the_engine(case, tol):
     rng = np.random.default_rng(11)
     Z = X[:2] + 0.05 * rng.standard_normal((2, Nx))
     A = rng.standard_normal((Nx, Nx)); S = 1e-3 * np.eye(Nx) + 1e-4 * A @ A.T
-    eng = _fit(X, Y, hyper)
-    L = _L()
+    eng = fit(X, Y, hyper)
     o = eng.predict_em_grad(Z, S)
     for k in DERIV:
         assert np.all(np.isfinite(o[k])), k
@@ -191,10 +144,10 @@ def test_em_grad_vs_differences_of_the_engine(case, tol):
 
 
 def test_em_grad_argument_checks():
-    L = _L(); lib = L.load()
+    lib = L.load()
     m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
     Ny, Nx = Y.shape[1], X.shape[1]
-    eng = _fit(X, Y, hyper)
+    eng = fit(X, Y, hyper)
     Z = np.ascontiguousarray(X[:3] + 0.01)
     S = 1e-3 * np.eye(Nx)
     dp = C.POINTER(C.c_double)
@@ -212,7 +165,7 @@ def test_em_grad_argument_checks():
         assert lib.gpmpc_predict_em_grad(eng.h, 3, Z.ctypes.data_as(dp), S.ctypes.data_as(dp), 0, *ptrs) == L.OK
         assert np.array_equal(out, full[name]), name
     eng.close()
-    part = _fit(X, Y, hyper, out_begin=0, out_count=Ny - 1)
+    part = fit(X, Y, hyper, out_begin=0, out_count=Ny - 1)
     with pytest.raises(L.GpmpcError) as e:
         part.predict_em_grad(Z, S)
     assert e.value.code == L.ERR_STATE
@@ -226,12 +179,12 @@ def test_em_grad_after_append_matches_a_refit():
     rng = np.random.default_rng(3)
     Z = X[:3] + 0.05 * rng.standard_normal((3, Nx))
     S = 1e-3 * np.eye(Nx)
-    eng = _fit(X[:-2], Y[:-2], hyper)
+    eng = fit(X[:-2], Y[:-2], hyper)
     eng.predict_em_grad(Z, S)                   # builds the cache for the smaller model
     assert eng.append(X[-2], Y[-2]) and eng.append(X[-1], Y[-1])
     got = eng.predict_em_grad(Z, S)
     eng.close()
-    ref_eng = _fit(X, Y, hyper)
+    ref_eng = fit(X, Y, hyper)
     ref = ref_eng.predict_em_grad(Z, S)
     ref_eng.close()
     for k in DERIV:
@@ -239,8 +192,7 @@ def test_em_grad_after_append_matches_a_refit():
 
 
 def test_gp_predict_batch_grad_em_vs_central_differences():
-    from tests.test_gpu_parity import _gp_from_fixture
-    gp, m = _gp_from_fixture('tank')
+    gp, m = gp_from_fixture('tank')
     assert m['normalize']
     d = load_golden('derived', 'tank')
     xs = np.tile(d['x0'], (3, 1)) * (1 + 0.02 * np.arange(3)[:, None]); us = np.tile(d['u0'], (3, 1))
@@ -268,25 +220,18 @@ def test_gp_predict_batch_grad_em_vs_central_differences():
     gp.close()
 
 
-def _ccs(ptr):
-    nrow, ncol = ptr[0], ptr[1]
-    colind = [ptr[2 + k] for k in range(ncol + 1)]
-    rows = [ptr[2 + ncol + 1 + k] for k in range(colind[-1])]
-    return nrow, ncol, colind, rows
-
-
 def test_casadi_external_entry_points_with_em():
     """gp_b200_bind(EM) driven through ctypes the way CasADi drives it: gp_b200 equals gpmpc_predict(EM), the CCS
     nonzeros of jac_gp_b200 equal gpmpc_predict_em_grad (jac_mean_sigma and jac_cov_sigma block-diagonal, column
     d + Nx*e <-> Sigma[d][e]), and jac_jac_gp_b200 reports failure."""
     m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
     Ny, Nx, Nt = Y.shape[1], X.shape[1], 4
-    eng = _fit(X, Y, hyper)
-    Lb = _L(); lib = Lb.load()
+    eng = fit(X, Y, hyper)
+    lib = L.load()
     rng = np.random.default_rng(8)
     Z = X[:Nt] + 0.1 * rng.standard_normal((Nt, Nx))
     Sg = np.stack([1e-3 * np.eye(Nx) + 1e-4 * (lambda A: A @ A.T)(rng.standard_normal((Nx, Nx))) for _ in range(Nt)])
-    assert lib.gp_b200_bind(eng.h, Lb.METHOD_EM, Nt) == 0
+    assert lib.gp_b200_bind(eng.h, L.METHOD_EM, Nt) == 0
     dp = C.POINTER(C.c_double)
 
     def call(fn, ins, outs):
@@ -301,7 +246,7 @@ def test_casadi_external_entry_points_with_em():
     o = eng.predict_em_grad(Z, Sg)
     assert np.array_equal(mean_cm, o['mean'])
     assert np.array_equal(cov_cm, np.transpose(o['cov'], (0, 2, 1)))
-    pats = [_ccs(lib.jac_gp_b200_sparsity_out(k)) for k in range(4)]
+    pats = [ccs(lib.jac_gp_b200_sparsity_out(k)) for k in range(4)]
     assert [(p[0], p[1], p[2][-1]) for p in pats] == [
         (Ny * Nt, Nx * Nt, Ny * Nx * Nt), (Ny * Nt, Nx * Nx * Nt, Ny * Nx * Nx * Nt),
         (Ny * Ny * Nt, Nx * Nt, Ny * Ny * Nx * Nt), (Ny * Ny * Nt, Nx * Nx * Nt, Ny * Ny * Nx * Nx * Nt)]
@@ -314,7 +259,7 @@ def test_casadi_external_entry_points_with_em():
     exp_cs = np.transpose(o['dcov_dSigma'], (0, 4, 3, 2, 1)).reshape(-1)               # t, e, d, b, a
     for got, exp in zip(outs, (exp_mz, exp_ms, exp_cz, exp_cs)):
         assert np.array_equal(got, exp)
-    jj = [_ccs(lib.jac_jac_gp_b200_sparsity_out(k)) for k in range(16)]
+    jj = [ccs(lib.jac_jac_gp_b200_sparsity_out(k)) for k in range(16)]
     jins = [z_cm, s_cm, mean_cm, cov_cm] + [np.zeros(max(1, p[2][-1])) for p in pats]
     assert call(lib.jac_jac_gp_b200, jins, [np.zeros(max(1, p[2][-1])) for p in jj]) != 0
     lib.gp_b200_unbind()

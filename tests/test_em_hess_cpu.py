@@ -15,7 +15,7 @@ from oracle import em_hess_oracle as emh
 from oracle import gp_oracle as orc
 from oracle import hess_oracle as hor
 from tests._fake_engine import OracleEngine
-from tests._util import load_fixture, relinf
+from tests._util import d4, load_fixture, relinf
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -36,11 +36,6 @@ def _problem(case):
     return X, Y, hyper, Z, Sigma, alpha, chol
 
 
-def _d4(fun, h):
-    r = {k: fun(k * h) for k in (-2, -1, 1, 2)}
-    return {key: (r[-2][key] - 8 * r[-1][key] + 8 * r[1][key] - r[2][key]) / (12 * h) for key in r[1]}
-
-
 @pytest.mark.parametrize('case', ['tank', 'car', 'syn'])
 def test_em_hess_oracle_vs_differences_of_the_gradient_oracle(case):
     X, Y, hyper, Z, Sigma, alpha, chol = _problem(case)
@@ -53,7 +48,7 @@ def test_em_hess_oracle_vs_differences_of_the_gradient_oracle(case):
                                                  ('dcov_dz', 'd2cov_dz2'), ('dcov_dSigma', 'd2cov_dSigma_dz'))}
     for f in range(Nx):
         e = np.zeros(Nx); e[f] = 1.0
-        d = _d4(lambda s: g(Z + s * e, Sigma), 1e-2)
+        d = d4(lambda s: g(Z + s * e, Sigma), 1e-2)
         for k in fz:
             fz[k][..., f] = d[k]
     assert relinf(cl['d2mean_dz2'], fz['dmean_dz']) < tol
@@ -63,7 +58,7 @@ def test_em_hess_oracle_vs_differences_of_the_gradient_oracle(case):
     for f in range(Nx):
         for gg in range(f + 1):
             E = np.zeros((Nx, Nx)); E[f, gg] = E[gg, f] = 1.0
-            d = _d4(lambda s: g(Z, Sigma + s * E), 1e-4)
+            d = d4(lambda s: g(Z, Sigma + s * E), 1e-4)
             scale = 1.0 if f == gg else 2.0
             assert relinf(scale * cl['d2mean_dSigma2'][..., f, gg], d['dmean_dSigma']) < tol, (f, gg)
             if case != 'car':       # car's cond(K) ~ 1e10 noise in the gradient oracle's cov, amplified by 1 / 1e-4
@@ -150,12 +145,12 @@ def test_gp_predict_batch_em_hess_chain_rule():
     for f in range(Nx):
         st = 1e-3 * max(1.0, abs(z[0, f]))
         e = np.zeros(Nx); e[f] = st
-        d = _d4(lambda s: gp.predict_batch_grad((z + s * e / st)[:, :Ny], (z + s * e / st)[:, Ny:], S, method='EM'), st)
+        d = d4(lambda s: gp.predict_batch_grad((z + s * e / st)[:, :Ny], (z + s * e / st)[:, Ny:], S, method='EM'), st)
         assert relinf(h['d2mean_dz2'][..., f], d['dmean_dz']) < 1e-4
         assert relinf(h['d2mean_dSigma_dz'][..., f], d['dmean_dSigma']) < 1e-4
         assert relinf(h['d2cov_dz2'][..., f], d['dcov_dz']) < 1e-3
         assert relinf(h['d2cov_dSigma_dz'][..., f], d['dcov_dSigma']) < 1e-3
     E = np.zeros((Nx, Nx)); E[0, 1] = E[1, 0] = 1.0
-    d = _d4(lambda s: gp.predict_batch_grad(x, u, S + s * E, method='EM'), 1e-4)
+    d = d4(lambda s: gp.predict_batch_grad(x, u, S + s * E, method='EM'), 1e-4)
     assert relinf(2 * h['d2mean_dSigma2'][..., 0, 1], d['dmean_dSigma']) < 1e-4
     assert relinf(2 * h['d2cov_dSigma2'][..., 0, 1], d['dcov_dSigma']) < 1e-3

@@ -8,12 +8,13 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import em_grad_oracle as emg
 from oracle import em_hess_oracle as emh
 from oracle import gp_oracle as orc
-from tests._util import load_fixture, load_golden, relinf
-from tests.test_em_grad_gpu import _case, _ccs, _engine_factor, _fit, _L
-from tests.test_em_shapes_gpu import CASES, em_problem, sigmas
+from tests._em_cases import em_problem, engine_alpha_chol, grad_case, sigmas
+from tests._engines import ccs, fit, gp_from_fixture
+from tests._util import d4, load_fixture, load_golden, relinf
 
 pytestmark = pytest.mark.gpu
 
@@ -37,7 +38,7 @@ def _hess_case(case):
         p = orc.synthetic_problem(300, 16, 2, config_id=316, H=1)
         hyper = p['hyper'].copy(); hyper[:, 17] = 0.3
         return p['X'], p['Y'], hyper, p['Z'][:1], sigmas(hyper, 16)['0.1'], None
-    X, Y, hyper, Z, Sigma, cap = _case(case)
+    X, Y, hyper, Z, Sigma, cap = grad_case(case)
     if '_s' in case or case.startswith('syn'):
         Z = Z[:1]
     return X, Y, hyper, Z, Sigma, cap
@@ -64,7 +65,7 @@ def em_hess_errors(case):
     bit-level checks: errors of every output / pair block normalised by its sum of |terms| (em_hess_terms)."""
     X, Y, hyper, Z, Sigma, cap = _hess_case(case)
     Ny = Y.shape[1]
-    eng = _fit(X, Y, hyper, capacity=cap)
+    eng = fit(X, Y, hyper, capacity=cap)
     o = eng.predict_em_hess(Z, Sigma)
     g = eng.predict_em_grad(Z, Sigma)
     for k in FIRST:
@@ -75,7 +76,7 @@ def em_hess_errors(case):
     o2 = eng.predict_em_hess(Z, Sigma)
     for k in o:
         assert np.array_equal(o[k], o2[k]), k
-    alpha, chol = _engine_factor(eng, Ny)
+    alpha, chol = engine_alpha_chol(eng, Ny)
     eng.close()
     ref = emh.em_hess_closed(X, hyper, alpha, chol, Z, Sigma)
     return emh.normalised_errors(o, ref, emh.em_hess_terms(X, hyper, alpha, chol, Z, Sigma))
@@ -99,19 +100,14 @@ def test_em_hess_vs_closed_oracle(case):
 
 
 def test_em_hess_points_are_independent_of_their_batch():
-    X, Y, hyper, Z, Sigma, _ = _case('tank_pp')
-    eng = _fit(X, Y, hyper)
+    X, Y, hyper, Z, Sigma, _ = grad_case('tank_pp')
+    eng = fit(X, Y, hyper)
     full = eng.predict_em_hess(Z, Sigma)
     for p in (0, Z.shape[0] - 1):
         one = eng.predict_em_hess(Z[p:p + 1], Sigma[p:p + 1])
         for k in one:
             assert np.array_equal(one[k][0], full[k][p]), (p, k)
     eng.close()
-
-
-def _d4(fun, h):
-    r = {k: fun(k * h) for k in (-2, -1, 1, 2)}
-    return {key: (r[-2][key] - 8 * r[-1][key] + 8 * r[1][key] - r[2][key]) / (12 * h) for key in r[1]}
 
 
 @pytest.mark.parametrize('case,tol', [('tank', 1e-5), ('car', 1e-3)])
@@ -123,14 +119,14 @@ def test_em_hess_vs_differences_of_the_engine(case, tol):
     rng = np.random.default_rng(11)
     Z = X[:2] + 0.05 * rng.standard_normal((2, Nx))
     A = rng.standard_normal((Nx, Nx)); S = 1e-3 * np.eye(Nx) + 1e-4 * A @ A.T
-    eng = _fit(X, Y, hyper)
+    eng = fit(X, Y, hyper)
     o = eng.predict_em_hess(Z, S)
     pairs = (('dmean_dz', 'd2mean_dz2'), ('dmean_dSigma', 'd2mean_dSigma_dz'), ('dcov_dz', 'd2cov_dz2'),
              ('dcov_dSigma', 'd2cov_dSigma_dz'))
     fz = {k: np.zeros_like(o[k2]) for k, k2 in pairs}
     for f in range(Nx):
         e = np.zeros(Nx); e[f] = 1.0
-        d = _d4(lambda s: eng.predict_em_grad(Z + s * e, S), 3e-2)
+        d = d4(lambda s: eng.predict_em_grad(Z + s * e, S), 3e-2)
         for k in fz:
             fz[k][..., f] = d[k]
     for k, k2 in pairs:
@@ -138,7 +134,7 @@ def test_em_hess_vs_differences_of_the_engine(case, tol):
     for f in range(Nx):
         for g in range(f + 1):
             E = np.zeros((Nx, Nx)); E[f, g] = E[g, f] = 1.0
-            d = _d4(lambda s: eng.predict_em_grad(Z, S + s * E), 3e-4)
+            d = d4(lambda s: eng.predict_em_grad(Z, S + s * E), 3e-4)
             sc = 1.0 if f == g else 2.0
             assert relinf(sc * o['d2mean_dSigma2'][..., f, g], d['dmean_dSigma']) < tol, (f, g)
             assert relinf(sc * o['d2cov_dSigma2'][..., f, g], d['dcov_dSigma']) < tol, (f, g)
@@ -148,8 +144,8 @@ def test_em_hess_vs_differences_of_the_engine(case, tol):
 def test_em_hess_heat_equation_identities():
     """At an arbitrary Sigma: dmean_dSigma = 1/2 d2mean_dz2, dcov_dSigma = 1/2 d2cov_dz2 + sym(J_a J_b^T), and
     d2mean_dSigma2 is fully symmetric in its four Sigma / z indices (it is 1/4 d^4 mean / dz^4)."""
-    X, Y, hyper, Z, Sigma, _ = _case('syn12')
-    eng = _fit(X, Y, hyper)
+    X, Y, hyper, Z, Sigma, _ = grad_case('syn12')
+    eng = fit(X, Y, hyper)
     o = eng.predict_em_hess(Z, Sigma)
     eng.close()
     assert relinf(o['dmean_dSigma'], 0.5 * o['d2mean_dz2']) < 1e-12
@@ -165,10 +161,9 @@ def test_em_hess_at_zero_sigma_against_me_ta():
     of d2cov_dz2 = d2var_dz2 and its off-diagonal ~ 0, and d2cov_dSigma_dz for a != b = the symmetrised TA mixed term."""
     m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
     Nx, Ny = X.shape[1], Y.shape[1]
-    L = _L()
     rng = np.random.default_rng(4)
     Z = X[:3] + 0.05 * rng.standard_normal((3, Nx))
-    eng = _fit(X, Y, hyper)
+    eng = fit(X, Y, hyper)
     o = eng.predict_em_hess(Z, np.zeros((Nx, Nx)))
     me = eng.predict_hess(Z, None, L.METHOD_ME)
     eng.close()
@@ -190,13 +185,13 @@ def test_em_hess_argument_checks():
     """Nx = 17, a null Sigma, a handle that owns only some outputs and an unfactorised handle return their codes; the
     model still predicts the same afterwards."""
     import gp_mpc_b200
-    L = _L(); lib = L.load()
+    lib = L.load()
     dp = C.POINTER(C.c_double)
     m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
     Ny, Nx = Y.shape[1], X.shape[1]
     Z = np.ascontiguousarray(X[:2] + 0.01)
     S = 1e-3 * np.eye(Nx)
-    eng = _fit(X, Y, hyper)
+    eng = fit(X, Y, hyper)
     before = eng.predict_em_hess(Z, S)
     assert lib.gpmpc_predict_em_hess(eng.h, 2, Z.ctypes.data_as(dp), None, 0, *([None] * 13)) == L.ERR_ARG
     assert lib.gpmpc_predict_em_hess(eng.h, 0, Z.ctypes.data_as(dp), S.ctypes.data_as(dp), 0, *([None] * 13)) == L.ERR_ARG
@@ -204,7 +199,7 @@ def test_em_hess_argument_checks():
     for k in before:
         assert np.array_equal(before[k], after[k]), k
     eng.close()
-    part = _fit(X, Y, hyper, out_begin=0, out_count=Ny - 1)
+    part = fit(X, Y, hyper, out_begin=0, out_count=Ny - 1)
     with pytest.raises(L.GpmpcError) as e:
         part.predict_em_hess(Z, S)
     assert e.value.code == L.ERR_STATE
@@ -216,7 +211,7 @@ def test_em_hess_argument_checks():
     assert e.value.code == L.ERR_STATE
     raw.close()
     X17, Y17, h17, Z17 = em_problem('nx17')
-    e17 = _fit(X17, Y17, h17)
+    e17 = fit(X17, Y17, h17)
     with pytest.raises(L.GpmpcError) as e:
         e17.predict_em_hess(Z17[:1], sigmas(h17, 17)['0.1'])
     assert e.value.code == L.ERR_ARG
@@ -230,8 +225,8 @@ def test_casadi_external_with_em_hess():
     pattern order while the other eight are empty."""
     m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
     Ny, Nx, Nt = Y.shape[1], X.shape[1], 3
-    eng = _fit(X, Y, hyper)
-    Lb = _L(); lib = Lb.load()
+    eng = fit(X, Y, hyper)
+    lib = L.load()
     rng = np.random.default_rng(8)
     Z = X[:Nt] + 0.1 * rng.standard_normal((Nt, Nx))
     Sg = np.stack([1e-3 * np.eye(Nx) + 1e-4 * (lambda A: A @ A.T)(rng.standard_normal((Nx, Nx))) for _ in range(Nt)])
@@ -248,12 +243,12 @@ def test_casadi_external_with_em_hess():
     def run():
         mean_cm = np.empty((Nt, Ny)); cov_cm = np.empty((Nt, Ny, Ny))
         assert call(lib.gp_b200, [z_cm, s_cm], [mean_cm, cov_cm]) == 0
-        pats = [_ccs(lib.jac_gp_b200_sparsity_out(k)) for k in range(4)]
+        pats = [ccs(lib.jac_gp_b200_sparsity_out(k)) for k in range(4)]
         outs = [np.zeros(p[2][-1]) for p in pats]
         assert call(lib.jac_gp_b200, [z_cm, s_cm, mean_cm, cov_cm], outs) == 0
         return mean_cm, cov_cm, pats, outs
 
-    assert lib.gp_b200_bind(eng.h, Lb.METHOD_EM, Nt) == 0
+    assert lib.gp_b200_bind(eng.h, L.METHOD_EM, Nt) == 0
     ref = run()
     assert lib.gp_b200_bind_em_hess(eng.h, Nt) == 0
     got = run()
@@ -262,7 +257,7 @@ def test_casadi_external_with_em_hess():
     for a, b in zip(ref[3], got[3]):
         assert np.array_equal(a, b)
     mean_cm, cov_cm, pats, outs = got
-    jj = [_ccs(lib.jac_jac_gp_b200_sparsity_out(k)) for k in range(16)]
+    jj = [ccs(lib.jac_jac_gp_b200_sparsity_out(k)) for k in range(16)]
     res = [np.zeros(max(1, p[2][-1])) for p in jj]
     assert call(lib.jac_jac_gp_b200, [z_cm, s_cm, mean_cm, cov_cm] + outs, res) == 0
     o = eng.predict_em_hess(Z, Sg)
@@ -288,8 +283,7 @@ def test_casadi_external_with_em_hess():
 def test_gp_predict_batch_em_hess_vs_differences():
     """GP.predict_batch_em_hess (normalize=True) against fourth-order differences of GP.predict_batch_grad('EM') in the
     caller's units, and its first-order entries bit-identical to predict_batch_grad's."""
-    from tests.test_gpu_parity import _gp_from_fixture
-    gp, m = _gp_from_fixture('tank')
+    gp, m = gp_from_fixture('tank')
     assert m['normalize']
     d = load_golden('derived', 'tank')
     xs = np.tile(d['x0'], (2, 1)) * (1 + 0.02 * np.arange(2)[:, None]); us = np.tile(d['u0'], (2, 1))
@@ -303,13 +297,13 @@ def test_gp_predict_batch_em_hess_vs_differences():
     for f in range(Nx):
         st = 1e-2 * max(1.0, abs(zs[0, f]))
         e = np.zeros(Nx); e[f] = 1.0
-        dd = _d4(lambda s: gp.predict_batch_grad((zs + s * e)[:, :Ny], (zs + s * e)[:, Ny:], Sigma, method='EM'), st)
+        dd = d4(lambda s: gp.predict_batch_grad((zs + s * e)[:, :Ny], (zs + s * e)[:, Ny:], Sigma, method='EM'), st)
         assert relinf(h['d2mean_dz2'][..., f], dd['dmean_dz']) < 1e-4
         assert relinf(h['d2mean_dSigma_dz'][..., f], dd['dmean_dSigma']) < 1e-4
         assert relinf(h['d2cov_dz2'][..., f], dd['dcov_dz']) < 1e-3
         assert relinf(h['d2cov_dSigma_dz'][..., f], dd['dcov_dSigma']) < 1e-3
     E = np.zeros((Nx, Nx)); E[0, 1] = E[1, 0] = 1.0
-    dd = _d4(lambda s: gp.predict_batch_grad(xs, us, Sigma + s * E, method='EM'), 3e-4)
+    dd = d4(lambda s: gp.predict_batch_grad(xs, us, Sigma + s * E, method='EM'), 3e-4)
     assert relinf(2 * h['d2mean_dSigma2'][..., 0, 1], dd['dmean_dSigma']) < 1e-4
     assert relinf(2 * h['d2cov_dSigma2'][..., 0, 1], dd['dcov_dSigma']) < 1e-3
     gp.close()

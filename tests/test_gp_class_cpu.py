@@ -8,18 +8,12 @@ import pytest
 
 import gp_mpc_b200
 from oracle import gp_oracle as orc
-from tests._fake_engine import OracleEngine, OracleEngineWithRollout
-from tests._util import load_fixture, load_golden, relinf
+from tests._fake_engine import OracleEngine, OracleEngineWithRollout, fixture_gp
+from tests._util import load_golden, relinf
 
 
 def _gp(name, **kw):
-    m = load_fixture(name)
-    args = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'], hyper=dict(hyper=m['hyper']),
-                engine_factory=OracleEngine)
-    if m['normalize']:
-        args.update(meta=m['meta'], xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
-    args.update(kw)
-    return gp_mpc_b200.GP(m['X'], m['Y'], **args), m
+    return fixture_gp(name, OracleEngine, **kw)
 
 
 @pytest.mark.parametrize('name', ['tank', 'car'])

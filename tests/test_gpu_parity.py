@@ -7,7 +7,9 @@ import os
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
+from tests._engines import fit, gp_from_fixture
 from tests._util import load_fixture, load_golden, relinf
 
 pytestmark = pytest.mark.gpu
@@ -18,19 +20,6 @@ TOL = 1e-6
 def _engine(N, Nx, Ny, **kw):
     import gp_mpc_b200
     return gp_mpc_b200.Engine(N, Nx, Ny, device=0, **kw)
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _fit_engine(X, Y, hyper):
-    eng = _engine(X.shape[0], X.shape[1], Y.shape[1])
-    eng.set_data(X, Y)
-    eng.set_hyper(hyper)
-    info = eng.factorize()
-    return eng, info
 
 
 # ------------------------------------------------------------------ a1/a2 K build
@@ -55,9 +44,8 @@ def test_kbuild_matches_oracle(case):
 @pytest.mark.parametrize('name', ['tank', 'car'])
 def test_factorize_reproduces_stored_model(name):
     m = load_fixture(name)
-    eng, info = _fit_engine(m['X'], m['Y'], m['hyper'])
+    eng, info = fit(m['X'], m['Y'], m['hyper'], with_info=True)
     assert not info.any()
-    L = _L()
     N = m['X'].shape[0]
     for a in range(m['hyper'].shape[0]):
         chol = eng.get(L.GET_CHOL, a)
@@ -82,8 +70,7 @@ def test_factorize_reproduces_stored_model(name):
 def test_factorize_synthetic_vs_oracle(N):
     p = orc.synthetic_problem(N, 8, 3, config_id=N)
     post = orc.postfit(p['X'], p['Y'], p['hyper'], lapack_general_solve=False)
-    eng, info = _fit_engine(p['X'], p['Y'], p['hyper'])
-    L = _L()
+    eng, info = fit(p['X'], p['Y'], p['hyper'], with_info=True)
     for a in range(3):
         assert relinf(eng.get(L.GET_CHOL, a), post['chol'][a]) < 1e-10
         assert relinf(eng.get(L.GET_ALPHA, a), post['alpha'][a]) < 1e-7
@@ -100,7 +87,7 @@ def test_jitter_retry_and_not_pd():
     info = eng.factorize(1e-8)
     assert info[0] == 1                                     # succeeded after jitter
     Ko = orc.covSEard(X, X, hyper[0, :3], 1.0) + (1e-20 + 1e-8) * np.eye(40)
-    assert relinf(eng.get(_L().GET_CHOL, 0), np.linalg.cholesky(Ko)) < 1e-6
+    assert relinf(eng.get(L.GET_CHOL, 0), np.linalg.cholesky(Ko)) < 1e-6
     with pytest.raises(np.linalg.LinAlgError):
         eng.factorize(0.0)                                  # retry with zero jitter must fail again
     eng.close()
@@ -110,8 +97,7 @@ def test_jitter_retry_and_not_pd():
 @pytest.mark.parametrize('name', ['tank', 'car'])
 def test_predict_fixture_batch(name):
     m = load_fixture(name); d = load_golden('derived', name)
-    eng, _ = _fit_engine(m['X'], m['Y'], m['hyper'])
-    L = _L()
+    eng, _ = fit(m['X'], m['Y'], m['hyper'], with_info=True)
     mean, var, cov, jac = eng.predict(d['Zs'], d['Sigma'], L.METHOD_TA)
     assert relinf(mean, d['mean_b']) < TOL
     assert relinf(var, d['var_b']) < TOL
@@ -134,21 +120,21 @@ def test_predict_synthetic_vs_oracle(N, Nx, Ny, H):
     mo, vo = orc.gp_mean_var(p['X'], p['hyper'], post['alpha'], post['chol'], p['Z'])
     Jo = orc.gp_mean_jac(p['X'], p['hyper'], post['alpha'], p['Z'])
     co = orc.ta_cov(vo, Jo, p['Sigma'])
-    eng, _ = _fit_engine(p['X'], p['Y'], p['hyper'])
-    mean, var, cov, jac = eng.predict(p['Z'], p['Sigma'], _L().METHOD_TA)
+    eng, _ = fit(p['X'], p['Y'], p['hyper'], with_info=True)
+    mean, var, cov, jac = eng.predict(p['Z'], p['Sigma'], L.METHOD_TA)
     assert relinf(mean, mo) < TOL and relinf(var, vo) < TOL and relinf(jac, Jo) < TOL and relinf(cov, co) < TOL
     assert (var > 0).all()
     # per-point input covariances (one Sigma per shooting node, mpc_class.py:265-275)
     Sg = np.stack([p['Sigma'] * (1 + 0.1 * h) for h in range(H)])
-    _, _, cov_pp, _ = eng.predict(p['Z'], Sg, _L().METHOD_TA)
+    _, _, cov_pp, _ = eng.predict(p['Z'], Sg, L.METHOD_TA)
     assert relinf(cov_pp, orc.ta_cov(vo, Jo, Sg)) < TOL
     # the stream-K partition (persistent grid size) must not change the result beyond rounding,
     # and a fixed partition is bit-reproducible (parked partials are added in contributor order)
-    mean_b, var_b, cov_b, jac_b = eng.predict(p['Z'], p['Sigma'], _L().METHOD_TA)
+    mean_b, var_b, cov_b, jac_b = eng.predict(p['Z'], p['Sigma'], L.METHOD_TA)
     assert np.array_equal(var_b, var) and np.array_equal(mean_b, mean) and np.array_equal(cov_b, cov)
     for ctas in (1, 7, 1000):
         eng.set_option('predict_ctas', ctas)
-        mean_s, var_s, cov_s, jac_s = eng.predict(p['Z'], p['Sigma'], _L().METHOD_TA)
+        mean_s, var_s, cov_s, jac_s = eng.predict(p['Z'], p['Sigma'], L.METHOD_TA)
         assert relinf(var_s, var) < 1e-9 and np.array_equal(mean_s, mean) and np.array_equal(jac_s, jac)
         assert relinf(cov_s, cov) < 1e-9
     eng.close()
@@ -157,9 +143,8 @@ def test_predict_synthetic_vs_oracle(N, Nx, Ny, H):
 def test_profiling_entry_points_leave_the_engine_intact():
     """gpmpc_profile (ks / product / product + tail selectors), gpmpc_profile_balance and gpmpc_profile_tail run the
     production kernels on the engine's own buffers: times are positive and the next predict call is bit-identical."""
-    L = _L()
     p = orc.synthetic_problem(700, 6, 3, config_id=77, H=40)
-    eng, _ = _fit_engine(p['X'], p['Y'], p['hyper'])
+    eng, _ = fit(p['X'], p['Y'], p['hyper'], with_info=True)
     ref = eng.predict(p['Z'], p['Sigma'], L.METHOD_TA)
     for what in (L.PROF_KS, L.PROF_TRIGEMM, L.PROF_PREDICT_TAIL):
         ms = eng.profile(what, n=40, reps=3)
@@ -180,8 +165,7 @@ def test_full_size_properties_n4096():
     columns, the interpolation identity Kf alpha = y - sn2 alpha at training points, var > 0."""
     N, Nx, Ny = 4096, 8, 2
     p = orc.synthetic_problem(N, Nx, Ny, config_id=3, H=30)
-    eng, _ = _fit_engine(p['X'], p['Y'], p['hyper'])
-    L = _L()
+    eng, _ = fit(p['X'], p['Y'], p['hyper'], with_info=True)
     idx = np.arange(0, N, 137)[:30]
     mean, var, _, _ = eng.predict(p['X'][idx], None, L.METHOD_ME, want_jac=False)
     for a in range(Ny):
@@ -205,9 +189,8 @@ def test_full_size_properties_n16384():
     reduces to ME when Sigma = 0; (6) refinement and split-K variants agree."""
     N, Nx, H = 16384, 10, 50
     p = orc.synthetic_problem(N, Nx, 1, config_id=5, H=H)
-    eng, info = _fit_engine(p['X'], p['Y'], p['hyper'])
+    eng, info = fit(p['X'], p['Y'], p['hyper'], with_info=True)
     assert not info.any()
-    L = _L()
     idx = np.arange(0, N, 331)[:H]
     mean, var, _, _ = eng.predict(p['X'][idx], None, L.METHOD_ME, want_jac=False)
     alpha = eng.get(L.GET_ALPHA, 0)
@@ -242,9 +225,8 @@ def test_c3_full_size_vs_oracle():
     predict_large): chol <= 1e-9, mean / var / J / cov <= 1e-6 (batch-inf-norm relative)."""
     N, Nx, Ny, H = 4096, 8, 6, 30
     p = orc.synthetic_problem(N, Nx, Ny, config_id=3, H=H)
-    eng, info = _fit_engine(p['X'], p['Y'], p['hyper'])
+    eng, info = fit(p['X'], p['Y'], p['hyper'], with_info=True)
     assert not info.any()
-    L = _L()
     mean, var, cov, jac = eng.predict(p['Z'], p['Sigma'], L.METHOD_TA)
     mo = np.zeros((H, Ny)); vo = np.zeros((H, Ny)); Jo = np.zeros((H, Ny, Nx))
     for a in range(Ny):
@@ -295,9 +277,8 @@ def test_c5_full_size_vs_independent_cholesky():
     solves): chol <= 1e-9, mean / var / J / cov <= 1e-6."""
     N, Nx, H = 16384, 10, 50
     p = orc.synthetic_problem(N, Nx, 1, config_id=5, H=H)
-    eng, info = _fit_engine(p['X'], p['Y'], p['hyper'])
+    eng, info = fit(p['X'], p['Y'], p['hyper'], with_info=True)
     assert not info.any()
-    L = _L()
     mean, var, cov, jac = eng.predict(p['Z'], p['Sigma'], L.METHOD_TA)
     f = orc.factor_large(p['X'], p['Y'][:, 0], p['hyper'][0])
     assert not f['jitter']
@@ -329,8 +310,7 @@ def test_predict_grad_vs_central_differences(case):
         n = int(case[3:]); p = orc.synthetic_problem(n, 7 if n == 700 else 17, 3, config_id=n, H=9 if n == 700 else 66)
         X, Y, hyper, Z, Sigma = p['X'], p['Y'], p['hyper'], p['Z'], p['Sigma']
     Ny, Nx = Y.shape[1], X.shape[1]
-    eng, _ = _fit_engine(X, Y, hyper)
-    L = _L()
+    eng, _ = fit(X, Y, hyper, with_info=True)
     post = orc.postfit(X, Y, hyper, lapack_general_solve=False)
     Sg = np.stack([Sigma * (1 + 0.05 * h) for h in range(Z.shape[0])])
     for method, name, S in ((L.METHOD_TA, 'TA', Sg), (L.METHOD_ME, 'ME', None)):
@@ -355,12 +335,12 @@ def test_casadi_external_entry_points():
     import ctypes as C
     m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
     Ny, Nx, Nt = 4, 6, 5
-    eng, _ = _fit_engine(X, Y, hyper)
-    Lb = _L(); lib = Lb.load()
+    eng, _ = fit(X, Y, hyper, with_info=True)
+    lib = L.load()
     rng = np.random.default_rng(8)
     Z = X[:Nt] + 0.1 * rng.standard_normal((Nt, Nx))
     Sg = np.stack([1e-3 * np.eye(Nx) + 1e-4 * (lambda A: A @ A.T)(rng.standard_normal((Nx, Nx))) for _ in range(Nt)])
-    assert lib.gp_b200_bind(eng.h, Lb.METHOD_TA, Nt) == 0
+    assert lib.gp_b200_bind(eng.h, L.METHOD_TA, Nt) == 0
     assert lib.gp_b200_n_in() == 2 and lib.gp_b200_n_out() == 2
     assert lib.jac_gp_b200_n_in() == 4 and lib.jac_gp_b200_n_out() == 4
     assert lib.gp_b200_name_in(0) == b'z' and lib.gp_b200_name_out(1) == b'cov'
@@ -380,9 +360,9 @@ def test_casadi_external_entry_points():
     s_cm = np.ascontiguousarray(np.transpose(Sg, (0, 2, 1)))
     mean_cm = np.empty((Nt, Ny)); cov_cm = np.empty((Nt, Ny, Ny))
     call(lib.gp_b200, [z_cm, s_cm], [mean_cm, cov_cm])
-    mean, var, cov, jac = eng.predict(Z, Sg, Lb.METHOD_TA)
+    mean, var, cov, jac = eng.predict(Z, Sg, L.METHOD_TA)
     assert np.array_equal(mean_cm, mean) and np.array_equal(cov_cm, np.transpose(cov, (0, 2, 1)))   # column-major blocks
-    g = eng.predict_grad(Z, Sg, Lb.METHOD_TA)
+    g = eng.predict_grad(Z, Sg, L.METHOD_TA)
 
     def ccs(ptr):
         nrow, ncol = ptr[0], ptr[1]
@@ -428,7 +408,7 @@ def test_casadi_external_entry_points():
     eng.close()
     # the GP-class view: derivatives in the caller's units (chain rule through the scalers) vs central
     # differences of GP.predict_batch itself
-    gp, m = _gp_from_fixture('tank')
+    gp, m = gp_from_fixture('tank')
     d = load_golden('derived', 'tank')
     xs = np.tile(d['x0'], (3, 1)) * (1 + 0.02 * np.arange(3)[:, None]); us = np.tile(d['u0'], (3, 1))
     gg = gp.predict_batch_grad(xs, us, d['Sigma'])
@@ -454,12 +434,11 @@ def test_exact_moment_matching_vs_extended_precision():
     identical, better conditioned form (Cholesky-based trace for the invK term, expm1 for
     t Q - q q^T), so unlike the reference's fp64 expression it stays meaningful on the car fixture
     (cond(K) ~ 1e10, where the reference formula in fp64 returns negative variances, SURVEY q18)."""
-    L = _L()
     # accuracy floor: alpha = K^-1 y itself carries eps*cond(K) relative error (5e-9 tank, 7e-6 car), amplified by the
     # beta^T (t Q - q q^T) beta contraction -- a property of the formula in fp64, shared by every evaluation order
     for name, tol_cov in (('tank', 1e-4), ('car', 0.25)):
         m = load_fixture(name); g = load_golden('em_mp', name)
-        eng, _ = _fit_engine(m['X'], m['Y'], m['hyper'])
+        eng, _ = fit(m['X'], m['Y'], m['hyper'], with_info=True)
         mean, var, cov, _ = eng.predict(g['Z'], g['Sigma'], L.METHOD_EM, want_jac=False)
         assert relinf(mean, g['mean']) < (TOL if name == 'tank' else 1e-3), relinf(mean, g['mean'])
         assert relinf(cov, g['cov']) < tol_cov, relinf(cov, g['cov'])
@@ -483,7 +462,7 @@ def test_exact_moment_matching_vs_extended_precision():
         eng.close()
     # through the GP class at the example's operating point, against the stored-model answer
     d = load_golden('derived', 'tank')
-    gp, m = _gp_from_fixture('tank')
+    gp, m = gp_from_fixture('tank')
     gp.set_method('EM')
     mean, cov = gp.predict(d['x0'], d['u0'], d['Sigma'])
     assert relinf(mean, d['mean_em']) < TOL
@@ -544,7 +523,7 @@ def test_prior_mean_functions_on_the_gpu():
     th = hyper[0].copy()
     eng.set_y(0, Y[:, 0] - Phi @ th[5:])
     nll, g = eng.nlml(0, th[:5], grad=True)
-    gm = -Phi.T @ eng.get(_L().GET_ALPHA_NLML, 0)
+    gm = -Phi.T @ eng.get(L.GET_ALPHA_NLML, 0)
     ref = lambda t: orc.calc_NLL(t[:5], X, Y[:, 0] - Phi @ t[5:], False)
     assert nll == pytest.approx(ref(th), rel=1e-10)
     for j in range(4):
@@ -576,21 +555,11 @@ def test_prior_mean_functions_on_the_gpu():
 
 
 # ------------------------------------------------------------------ the GP class (drop-in boundary)
-def _gp_from_fixture(name):
-    import gp_mpc_b200
-    m = load_fixture(name)
-    kw = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'],
-              hyper=dict(hyper=m['hyper'], invK=m['invK'], alpha=m['alpha'], chol=m['chol'],
-                         length_scale=m['length_scale'], signal_var=m['signal_var'],
-                         noise_var=m['noise_var'], mean=m['mean']))
-    if m['normalize']:
-        kw.update(meta=m['meta'], xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
-    return gp_mpc_b200.GP(m['X'], m['Y'], **kw), m
 
 
 @pytest.mark.parametrize('name', ['tank', 'car'])
 def test_gp_class_known_answers(name):
-    gp, m = _gp_from_fixture(name)
+    gp, m = gp_from_fixture(name)
     d = load_golden('derived', name)
     N, Ny, Nu = gp.get_size()
     assert (N, Ny, Nu) == (m['X'].shape[0], m['Y'].shape[1], m['X'].shape[1] - m['Y'].shape[1])
@@ -609,7 +578,7 @@ def test_gp_class_known_answers(name):
 
 
 def test_gp_class_validate_and_io(tmp_path):
-    gp, m = _gp_from_fixture('tank')
+    gp, m = gp_from_fixture('tank')
     rng = np.random.default_rng(1)
     Xt = m['meta']['meanZ'] + m['meta']['stdZ'] * rng.standard_normal((25, 6)) * 0.5
     Yt = m['meta']['meanY'] + m['meta']['stdY'] * rng.standard_normal((25, 4)) * 0.5
@@ -723,10 +692,10 @@ def test_edge_sizes(N, Nx, Ny, H):
     post = orc.postfit(X, Y, hyper, lapack_general_solve=False)
     mo, vo = orc.gp_mean_var(X, hyper, post['alpha'], post['chol'], Z)
     Jo = orc.gp_mean_jac(X, hyper, post['alpha'], Z); co = orc.ta_cov(vo, Jo, Sig)
-    eng, info = _fit_engine(X, Y, hyper)
-    mean, var, cov, jac = eng.predict(Z, Sig, _L().METHOD_TA)
+    eng, info = fit(X, Y, hyper, with_info=True)
+    mean, var, cov, jac = eng.predict(Z, Sig, L.METHOD_TA)
     assert relinf(mean, mo) < TOL and relinf(var, vo) < TOL and relinf(cov, co) < TOL and relinf(jac, Jo) < TOL
-    assert relinf(eng.get(_L().GET_CHOL, Ny - 1), post['chol'][Ny - 1]) < 1e-10
+    assert relinf(eng.get(L.GET_CHOL, Ny - 1), post['chol'][Ny - 1]) < 1e-10
     pc = eng.posterior_cov(Z[:min(H, 7)])
     ks = orc.covSEard(X, Z[:min(H, 7)], hyper[0, :Nx], hyper[0, Nx] ** 2)
     v = np.linalg.solve(post['chol'][0], ks)
@@ -736,7 +705,6 @@ def test_edge_sizes(N, Nx, Ny, H):
 
 def test_argument_errors_fail_loudly():
     import gp_mpc_b200
-    L = _L()
     with pytest.raises(L.GpmpcError):
         gp_mpc_b200.Engine(10, 33, 1, device=0)                  # Nx above NX_MAX
     with pytest.raises(L.GpmpcError):
@@ -802,7 +770,7 @@ def test_autonomous_system_nu_zero_rollout():
 def test_device_rollout_equals_the_host_loop(name):
     """gpmpc_rollout (all steps enqueued on the device, state fed back by a kernel) against GP.rollout's host loop
     (one predict call per step, gp_class.py:777-804): same operation order, so the trajectories agree to rounding."""
-    gp, m = _gp_from_fixture(name)
+    gp, m = gp_from_fixture(name)
     d = load_golden('derived', name)
     useq = np.tile(d['u0'], (12, 1)) * (1 + 0.02 * np.arange(12)[:, None])
     rm, rv = gp.rollout(d['x0'], useq, methods=['TA', 'ME'])
@@ -843,7 +811,7 @@ def test_rank1_append_matches_a_full_refit():
     assert relinf(gp.get_chol(), post['chol']) < 1e-10
     assert relinf(gp.get_alpha(), post['alpha']) < 1e-7
     mo, vo = orc.gp_mean_var(X[:128], hyper, post['alpha'], post['chol'], p['Z'])
-    mean, var, _, _ = gp.engine.predict(p['Z'], None, _L().METHOD_ME, want_jac=False)
+    mean, var, _, _ = gp.engine.predict(p['Z'], None, L.METHOD_ME, want_jac=False)
     assert relinf(mean, mo) < TOL and relinf(var, vo) < TOL
     gp.append_data(X[128:], Y[128:])                        # capacity exceeded -> refit path
     assert gp.get_size()[0] == 134

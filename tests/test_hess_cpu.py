@@ -9,6 +9,7 @@ import pytest
 
 from oracle import gp_oracle as orc
 from oracle import hess_oracle as hor
+from tests._engines import built_lib
 from tests._util import load_fixture, relinf
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -54,19 +55,12 @@ def test_predict_grad_closed_vs_fd_oracle():
     assert relinf(cl['dvar'], fd['dvar']) < 1e-5 and relinf(cl['dcov'], fd['dcov']) < 1e-5
 
 
-def _lib():
-    import __graft_entry__ as g
-    g.build()
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
 JJ_OUT = ['jac_%s_%s' % (o, i) for o in ('jac_mean_z', 'jac_mean_sigma', 'jac_cov_z', 'jac_cov_sigma')
           for i in ('z', 'sigma', 'out_mean', 'out_cov')]
 
 
 def test_jac_jac_metadata_without_a_gpu():
-    L = _lib(); lib = L.load()
+    L = built_lib(); lib = L.load()
     assert lib.jac_jac_gp_b200_n_in() == 8 and lib.jac_jac_gp_b200_n_out() == 16
     assert [lib.jac_jac_gp_b200_name_in(i) for i in range(8)] == [
         b'z', b'sigma', b'out_mean', b'out_cov', b'out_jac_mean_z', b'out_jac_mean_sigma', b'out_jac_cov_z', b'out_jac_cov_sigma']
@@ -78,7 +72,7 @@ def test_jac_jac_metadata_without_a_gpu():
 
 
 def test_library_exports_every_jac_jac_symbol():
-    L = _lib(); lib = L.load()
+    L = built_lib(); lib = L.load()
     hdr = open(os.path.join(ROOT, 'include', 'gpmpc_casadi.h')).read().split('#ifndef GPMPC_CASADI_H')[1]
     declared = set(re.findall(r'\b(jac_jac_gp_b200[A-Za-z_0-9]*)\s*\(', hdr))
     assert {'jac_jac_gp_b200', 'jac_jac_gp_b200_sparsity_out', 'jac_jac_gp_b200_incref'} <= declared

@@ -8,27 +8,15 @@ import itertools
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle import hess_oracle as hor
+from tests._engines import ccs, fit, gp_from_fixture
 from tests._util import load_fixture, load_golden, relinf
 
 pytestmark = pytest.mark.gpu
 
 FIRST = ('mean', 'var', 'cov', 'jac', 'dvar_dz', 'dcov_dz', 'hess')
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _fit(X, Y, hyper, **kw):
-    import gp_mpc_b200
-    eng = gp_mpc_b200.Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, **kw)
-    eng.set_data(X, Y)
-    eng.set_hyper(hyper)
-    eng.factorize()
-    return eng
 
 
 def _case(case):
@@ -56,8 +44,7 @@ def _all_perms_equal(T):
 def test_predict_hess_vs_oracle(case):
     """syn4200 (Nx = 12): 5 points per derivative pass, 14 passes per 64-point chunk, two chunks, N > 4096."""
     X, Y, hyper, Z, Sigma, alpha, chol = _case(case)
-    eng = _fit(X, Y, hyper)
-    L = _L()
+    eng = fit(X, Y, hyper)
     Sg = np.stack([Sigma * (1 + 0.05 * h) for h in range(Z.shape[0])])
     tol = 3e-5 if case == 'car' else 1e-6
     for method, name, S in ((L.METHOD_TA, 'TA', Sg), (L.METHOD_ME, 'ME', None)):
@@ -79,10 +66,10 @@ def test_predict_hess_vs_oracle(case):
 
 
 def test_predict_hess_argument_checks():
-    L = _L(); lib = L.load()
+    lib = L.load()
     m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
     Ny, Nx = Y.shape[1], X.shape[1]
-    eng = _fit(X, Y, hyper)
+    eng = fit(X, Y, hyper)
     Z = X[:3] + 0.01
     S = 1e-3 * np.eye(Nx)
     with pytest.raises(L.GpmpcError) as e:
@@ -98,18 +85,11 @@ def test_predict_hess_argument_checks():
     assert rc == L.OK and np.array_equal(d2cov, full['d2cov_dz2'])
     eng.close()
     # a handle that owns only some of the outputs
-    part = _fit(X, Y, hyper, out_begin=0, out_count=Ny - 1)
+    part = fit(X, Y, hyper, out_begin=0, out_count=Ny - 1)
     with pytest.raises(L.GpmpcError) as e:
         part.predict_hess(Z, S, L.METHOD_TA)
     assert e.value.code == L.ERR_STATE
     part.close()
-
-
-def _ccs(ptr):
-    nrow, ncol = ptr[0], ptr[1]
-    colind = [ptr[2 + k] for k in range(ncol + 1)]
-    rows = [ptr[2 + ncol + 1 + k] for k in range(colind[-1])]
-    return nrow, ncol, colind, rows
 
 
 def _dense(pat, vals):
@@ -127,9 +107,9 @@ def test_jac_jac_external_entry_points(method):
     gpmpc_predict_hess and against central differences of jac_gp_b200's own outputs."""
     m = load_fixture('tank'); X, Y, hyper = m['X'], m['Y'], m['hyper']
     Ny, Nx, Nt = 4, 6, 5
-    eng = _fit(X, Y, hyper)
-    Lb = _L(); lib = Lb.load()
-    meth = Lb.METHOD_TA if method == 'TA' else Lb.METHOD_ME
+    eng = fit(X, Y, hyper)
+    lib = L.load()
+    meth = L.METHOD_TA if method == 'TA' else L.METHOD_ME
     rng = np.random.default_rng(8)
     Z = X[:Nt] + 0.1 * rng.standard_normal((Nt, Nx))
     Sg = np.stack([1e-3 * np.eye(Nx) + 1e-4 * (lambda A: A @ A.T)(rng.standard_normal((Nx, Nx))) for _ in range(Nt)])
@@ -145,7 +125,7 @@ def test_jac_jac_external_entry_points(method):
     s_cm = np.ascontiguousarray(np.transpose(Sg, (0, 2, 1)))               # Nx x Nx*Nt column-major
     mean_cm = np.empty((Nt, Ny)); cov_cm = np.empty((Nt, Ny, Ny))
     call(lib.gp_b200, [z_cm, s_cm], [mean_cm, cov_cm])
-    jpats = [_ccs(lib.jac_gp_b200_sparsity_out(k)) for k in range(4)]
+    jpats = [ccs(lib.jac_gp_b200_sparsity_out(k)) for k in range(4)]
 
     def jac_dense(z, s):
         outs = [np.zeros(max(1, p[2][-1])) for p in jpats]
@@ -153,10 +133,10 @@ def test_jac_jac_external_entry_points(method):
         return [_dense(p, v) for p, v in zip(jpats, outs)]
 
     for k in range(4):                                                    # inputs 4..7 carry jac_gp_b200's patterns
-        assert _ccs(lib.jac_jac_gp_b200_sparsity_in(4 + k)) == jpats[k]
+        assert ccs(lib.jac_jac_gp_b200_sparsity_in(4 + k)) == jpats[k]
     n_in = [Nx * Nt, Nx * Nx * Nt, Ny * Nt, Ny * Ny * Nt]
     n_o = [p[0] * p[1] for p in jpats]
-    pats = [_ccs(lib.jac_jac_gp_b200_sparsity_out(k)) for k in range(16)]
+    pats = [ccs(lib.jac_jac_gp_b200_sparsity_out(k)) for k in range(16)]
     ta = method == 'TA'
     nnz = {0: Nt * Ny * Nx * Nx, 8: Nt * Ny * Ny * Nx * Nx, 9: Nt * Ny * Ny * Nx ** 3 if ta else 0,
            12: Nt * Ny * Ny * Nx ** 3 if ta else 0}
@@ -197,8 +177,7 @@ def test_jac_jac_external_entry_points(method):
 
 
 def test_gp_predict_batch_hess_vs_central_differences():
-    from tests.test_gpu_parity import _gp_from_fixture
-    gp, m = _gp_from_fixture('tank')
+    gp, m = gp_from_fixture('tank')
     assert m['normalize']
     d = load_golden('derived', 'tank')
     xs = np.tile(d['x0'], (3, 1)) * (1 + 0.02 * np.arange(3)[:, None]); us = np.tile(d['u0'], (3, 1))

@@ -25,18 +25,14 @@ import math
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from tests import _kernel_range as kr
-from tests.test_dispatch_gpu import ks_chunk
+from tests._engines import ks_chunk
 
 pytestmark = pytest.mark.gpu
 
 SFS = (2.0 ** -20, 1.0, 2.0 ** 6 * 3)
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
 
 
 def _engine(X, Y, hyper, capacity=None, factorize=True):
@@ -104,7 +100,6 @@ def _designs_k():
 def test_K_entries_across_the_exponent_range(design, sf):
     """Every off-diagonal entry within entry_ref's allowance, the clamped ones bit for bit; each design has entries below
     the clamp."""
-    L = _L()
     name, X, ell = _designs_k()[design]
     sn = 1e-3 * sf
     Y = np.zeros((X.shape[0], 1)); Y[0] = 1.0
@@ -143,7 +138,6 @@ def test_lower_build_through_L(sf):
     off-diagonal K_ij <= 2^-30 sf2 on an ordered grid, the terms L_ik L_jk (k < j < i) are below K_ij by 2^-120 or
     more, so (L L^T)_ij = L_ij L_jj = K_ij to rounding, and L_jj^2 = sf2 + sn2.  Subnormal L_ij (K_ij near 2^-1020 over
     L_jj > 1) carry an absolute rounding of 2^-1075."""
-    L = _L()
     rng = np.random.default_rng(31)
     X = _sparse_grid(384, rng)
     ell = np.array([1.0])
@@ -205,7 +199,6 @@ def test_ks_values_one_by_one(ch, Nx, Ny, N):
     where the scaled difference adds an absolute u_r (|xs| + |zs|) per dimension and, at sf = 3 2^6 (alpha ~ 3e-5),
     the terms alpha_i 2^-1020 are subnormal and carry an absolute rounding of 2^-1075 per fma; var = sf2 - |L^-1 ks|^2 within its
     cancellation-aware bound."""
-    L = _L()
     assert ks_chunk(-(-N // 128) * 128, Ny, Nx) == ch
     rng = np.random.default_rng(1000 + 10 * Nx + Ny + ch)
     ell = np.exp(rng.uniform(np.log(0.05), np.log(20.0), Nx))          # a different length scale per dimension
@@ -265,7 +258,6 @@ def test_power_of_two_rescaling_is_exact(s):
     dvar_dz and dcov_dz by 1/s, the mean Hessian and the second derivatives of var and cov by 1/s^2, d3mean_dz3 by
     1/s^3), the EM derivatives w.r.t. Sigma by 1/s^2, and the NLML's ell-gradient by 1/s.  An absolute constant in any
     of these kernels would break the equality."""
-    L = _L()
     p = orc.synthetic_problem(700, 6, 2, config_id=61, H=40)
     X, Y, hyper, Z, Sigma = p['X'], p['Y'], p['hyper'].copy(), p['Z'], p['Sigma']
     hs = hyper.copy(); hs[:, :6] *= s
@@ -314,7 +306,6 @@ def test_centre_follows_appends_and_removals(greedy):
     K, L, alpha, log det, nlml and loo_nlpp; and every entry of its K must meet the direct-difference reference at the
     bound for a centre at the current mean.  With the centre left at the old mean, |u|^2 reaches ~6e5 and the bound on
     t grows ten-thousandfold."""
-    L = _L()
     rng = np.random.default_rng(77)
     Nx, N0, n_new = 4, 256, 512
     X0 = rng.standard_normal((N0, Nx))
@@ -422,7 +413,6 @@ def test_regimes_end_to_end(regime):
     from oracle import em_grad_oracle as emo
     from oracle import hess_oracle as hso
     from oracle import loo_oracle as loo
-    L = _L()
     name, X, hyper, extra = _regimes()[regime]
     N, Nx = X.shape
     rng = np.random.default_rng(405 + regime)

@@ -9,16 +9,8 @@ from gp_mpc_b200.mean_functions import mean_function
 from gp_mpc_b200.optimize import bounds_and_init, train_gp_b200
 from oracle import gp_oracle as orc
 from oracle import loo_oracle as lo
-from tests._fake_engine import OracleEngine
-from tests._util import load_fixture, relinf
-
-
-def _problem(case):
-    if case in ('tank', 'car'):
-        m = load_fixture(case)
-        return m['X'], m['Y'], m['hyper']
-    p = orc.synthetic_problem(300, 5, 2, config_id=17)
-    return p['X'], p['Y'], p['hyper']
+from tests._fake_engine import OracleEngine, problem
+from tests._util import load_fixture, projected, relinf
 
 
 # (mean, var, nlpp) of the closed form against the refits: both carry cond(K) eps (~6e7 tank, ~7e10 car, ~2e6 synthetic)
@@ -27,7 +19,7 @@ TOL = {'tank': (1e-10, 1e-9, 1e-10), 'car': (1e-8, 1e-7, 1e-7), 'synthetic': (1e
 
 @pytest.mark.parametrize('case', ['tank', 'car', 'synthetic'])
 def test_closed_form_matches_drop_one_refits(case):
-    X, Y, hyper = _problem(case)
+    X, Y, hyper = problem(case)
     tm, tv, tn = TOL[case]
     for a in range(Y.shape[1]):
         cf = lo.closed_form(X, Y[:, a], hyper[a])
@@ -43,7 +35,7 @@ GRAD = {'tank': (1e-9, 1e-8, 1e-5, 1e-2), 'car': (1e-9, 1e-5, 1e-4, 1e-2), 'synt
 
 @pytest.mark.parametrize('case', ['tank', 'car', 'synthetic'])
 def test_gradient_forms_agree(case):
-    X, Y, hyper = _problem(case)
+    X, Y, hyper = problem(case)
     t_tr, t_comp, t_fd, rel = GRAD[case]
     for a in range(min(2, Y.shape[1])):
         theta = hyper[a] * np.linspace(0.9, 1.1, X.shape[1] + 2)
@@ -55,7 +47,7 @@ def test_gradient_forms_agree(case):
 
 
 def test_w_matrix_is_symmetric_and_its_trace_gives_the_noise_derivative():
-    X, Y, hyper = _problem('synthetic')
+    X, Y, hyper = problem('synthetic')
     W = lo.w_matrix(X, Y[:, 0], hyper[0])
     assert np.array_equal(W, W.T) or relinf(W, W.T) < 1e-14
     sn = hyper[0][-1]
@@ -162,12 +154,6 @@ def test_objective_option_errors_come_before_any_engine_call(opts):
     assert eng.calls == []
 
 
-def _projected(g, th, bounds):
-    """The gradient with the components that point out of an active bound zeroed (active: within 1e-8 of its range)."""
-    tol = 1e-8 * (bounds[:, 1] - bounds[:, 0])
-    return np.where((th <= bounds[:, 0] + tol) & (g > 0), 0.0, np.where((th >= bounds[:, 1] - tol) & (g < 0), 0.0, g))
-
-
 def test_loo_objective_fit():
     """SLSQP runs on loo_nlpp alone and reaches a stationary point of it (|projected dNLPP/dtheta_j * theta_j| <= 1e-5
     |NLPP|) below the initial point and below the NLML fit on the same objective.  The LOO objective is not convex: on
@@ -186,5 +172,5 @@ def test_loo_objective_fit():
         th, th_ml = gp._GP__hyper[a, :5], ml._GP__hyper[a, :5]
         bounds, init = bounds_and_init(X, Y[:, a])
         f, g = eng.loo_nlpp(a, th)
-        assert np.abs(_projected(g, th, bounds) * th).max() < 1e-5 * abs(f)
+        assert np.abs(projected(g, th, bounds) * th).max() < 1e-5 * abs(f)
         assert f < eng.loo_nlpp(a, init, grad=False) and f < eng.loo_nlpp(a, th_ml, grad=False)

@@ -8,33 +8,13 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle import loo_oracle as lo
-from tests._util import load_fixture, relinf
+from tests._engines import fit, problem
+from tests._util import load_fixture, projected, relinf
 
 pytestmark = pytest.mark.gpu
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _fit(X, Y, hyper, **kw):
-    eng = _L().Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, **kw)
-    eng.set_data(X, Y)
-    eng.set_hyper(hyper)
-    eng.factorize()
-    return eng
-
-
-def _problem(case):
-    if case in ('tank', 'car'):
-        m = load_fixture(case)
-        return m['X'], m['Y'], m['hyper']
-    N, Nx, Ny = case
-    p = orc.synthetic_problem(N, Nx, Ny, config_id=N + Nx)
-    return p['X'], p['Y'], p['hyper']
 
 
 def _check_loo(eng, X, Y, hyper, tol):
@@ -58,14 +38,14 @@ GRAD_COMPONENT_TOL = {'tank': 1e-4, 'car': 1e-3, 'syn1000x8': 1e-6, 'syn4096x10'
 
 @pytest.mark.parametrize('case', list(CASES))
 def test_loo_matches_the_oracle(case):
-    X, Y, hyper = _problem(CASES[case])
-    _check_loo(_fit(X, Y, hyper), X, Y, hyper, TOL[case])
+    X, Y, hyper = problem(CASES[case])
+    _check_loo(fit(X, Y, hyper), X, Y, hyper, TOL[case])
 
 
 @pytest.mark.parametrize('case', list(CASES))
 def test_loo_nlpp_and_its_gradient(case):
-    X, Y, hyper = _problem(CASES[case])
-    eng = _L().Engine(X.shape[0], X.shape[1], Y.shape[1], device=0)
+    X, Y, hyper = problem(CASES[case])
+    eng = L.Engine(X.shape[0], X.shape[1], Y.shape[1], device=0)
     eng.set_data(X, Y)
     a = Y.shape[1] - 1
     theta = hyper[a] * np.linspace(0.9, 1.1, X.shape[1] + 2)       # away from the stored fit
@@ -85,8 +65,8 @@ def test_loo_nlpp_and_its_gradient(case):
 
 
 def test_after_appends_on_a_reserved_handle_and_after_removals():
-    X, Y, hyper = _problem((900, 6, 2))
-    eng = _fit(X[:700], Y[:700], hyper, capacity=1000)
+    X, Y, hyper = problem((900, 6, 2))
+    eng = fit(X[:700], Y[:700], hyper, capacity=1000)
     for k in range(700, 760):
         assert eng.append(X[k], Y[k])
     _check_loo(eng, X[:760], Y[:760], hyper, 1e-9)
@@ -101,16 +81,16 @@ def test_after_appends_on_a_reserved_handle_and_after_removals():
 
 
 def test_a_sharded_handle_returns_the_full_handles_rows():
-    X, Y, hyper = _problem((700, 5, 4))
-    full = _fit(X, Y, hyper).loo()
-    part = _fit(X, Y, hyper, out_begin=1, out_count=2).loo()
+    X, Y, hyper = problem((700, 5, 4))
+    full = fit(X, Y, hyper).loo()
+    part = fit(X, Y, hyper, out_begin=1, out_count=2).loo()
     for u, v in zip(part, full):
         assert u.tobytes() == v[1:3].tobytes()
 
 
 def test_repeated_calls_are_bit_identical_and_nlpp_does_not_depend_on_grad():
-    X, Y, hyper = _problem((1000, 8, 3))
-    eng = _fit(X, Y, hyper)
+    X, Y, hyper = problem((1000, 8, 3))
+    eng = fit(X, Y, hyper)
     r1, r2 = eng.loo(), eng.loo()
     for u, v in zip(r1, r2):
         assert u.tobytes() == v.tobytes()
@@ -123,8 +103,8 @@ def test_repeated_calls_are_bit_identical_and_nlpp_does_not_depend_on_grad():
 
 
 def test_nlml_bits_do_not_change_around_loo_nlpp():
-    X, Y, hyper = _problem((1000, 8, 3))
-    eng = _L().Engine(1000, 8, 3, device=0)
+    X, Y, hyper = problem((1000, 8, 3))
+    eng = L.Engine(1000, 8, 3, device=0)
     eng.set_data(X, Y)
     f1, g1 = eng.nlml(1, hyper[1])
     eng.loo_nlpp(1, hyper[1] * 1.05)
@@ -137,7 +117,7 @@ def test_nlml_bits_do_not_change_around_loo_nlpp():
     eng.loo_nlpp(1, hyper[1] * 0.95)
     eng.factorize()
     post = orc.postfit(X, Y[:, 1:2], hyper[1:2], lapack_general_solve=False)
-    assert relinf(eng.get(_L().GET_INVK, 1), post['invK'][0]) < 1e-7
+    assert relinf(eng.get(L.GET_INVK, 1), post['invK'][0]) < 1e-7
 
 
 def test_loo_nlpp_takes_the_jitter_retry_of_factorize():
@@ -149,7 +129,7 @@ def test_loo_nlpp_takes_the_jitter_retry_of_factorize():
     X = p['X'].copy(); X[N // 2:] = X[:N - N // 2]
     Y = p['Y'][:, 1:2]
     th = p['hyper'][1].copy(); th[Nx + 1] = 1e-10
-    eng = _L().Engine(N, Nx, 1, device=0)
+    eng = L.Engine(N, Nx, 1, device=0)
     eng.set_data(X, Y)
     f = eng.loo_nlpp(0, th, grad=False)
     eng.set_hyper(th[None, :])
@@ -164,9 +144,8 @@ def test_loo_nlpp_takes_the_jitter_retry_of_factorize():
 
 
 def test_null_buffers():
-    X, Y, hyper = _problem((300, 4, 2))
-    L = _L()
-    eng = _fit(X, Y, hyper)
+    X, Y, hyper = problem((300, 4, 2))
+    eng = fit(X, Y, hyper)
     mean, var, nlpp = eng.loo()
     lib, dp = L.load(), C.POINTER(C.c_double)
     for mask in range(8):
@@ -178,11 +157,10 @@ def test_null_buffers():
 
 
 def test_state_and_argument_errors_leave_the_model_untouched():
-    X, Y, hyper = _problem((300, 3, 2))
-    L = _L()
+    X, Y, hyper = problem((300, 3, 2))
     lib, dp = L.load(), C.POINTER(C.c_double)
     Z = X[:4] + 0.1
-    eng = _fit(X, Y, hyper)
+    eng = fit(X, Y, hyper)
     before = eng.predict(Z, 1e-4 * np.eye(3), L.METHOD_TA)
     loo_before = eng.loo()
     th = np.ascontiguousarray(hyper[0])
@@ -212,7 +190,7 @@ def test_state_and_argument_errors_leave_the_model_untouched():
         fresh.loo()
     assert e.value.code == L.ERR_STATE
     # N = 1: nothing is left to predict a point from
-    small = _fit(X[:3], Y[:3], hyper)
+    small = fit(X[:3], Y[:3], hyper)
     small.remove([0, 2])
     Zs = X[:2]
     before = small.predict(Zs, None, L.METHOD_ME)
@@ -241,12 +219,6 @@ def test_gp_loo_predict_and_validate_loo():
     assert smse.shape == (4,) and np.all(smse > 0)
 
 
-def _projected(g, th, bounds):
-    """The gradient with the components that point out of an active bound zeroed (active: within 1e-8 of its range)."""
-    tol = 1e-8 * (bounds[:, 1] - bounds[:, 0])
-    return np.where((th <= bounds[:, 0] + tol) & (g > 0), 0.0, np.where((th >= bounds[:, 1] - tol) & (g < 0), 0.0, g))
-
-
 def test_gp_optimize_with_the_loo_objective():
     """SLSQP on gpmpc_loo_nlpp (concurrent per-output fits): a stationary point of the LOO objective within the bounds
     (|projected dNLPP/dtheta_j * theta_j| <= 1e-5 |NLPP|), below the initial point and below the NLML fit on the same
@@ -257,13 +229,13 @@ def test_gp_optimize_with_the_loo_objective():
     X, Y = p['X'], p['Y']
     gp_loo = gp_mpc_b200.GP(X, Y, normalize=False, optimizer_opts={'objective': 'loo'})
     gp_ml = gp_mpc_b200.GP(X, Y, normalize=False)
-    eng = _L().Engine(500, 4, 2, device=0)
+    eng = L.Engine(500, 4, 2, device=0)
     eng.set_data(X, Y)
     for a in range(2):
         th, th_ml = gp_loo._GP__hyper[a, :6], gp_ml._GP__hyper[a, :6]
         bounds, init = bounds_and_init(X, Y[:, a])
         f, g = eng.loo_nlpp(a, th)
-        pg = _projected(g, th, bounds)
+        pg = projected(g, th, bounds)
         f_init, f_ml = eng.loo_nlpp(a, init, grad=False), eng.loo_nlpp(a, th_ml, grad=False)
         stat = np.abs(pg * th).max() / abs(f)
         print('output %d: nlpp %.6f (init %.6f, nlml fit %.6f), |projected grad * theta| / |nlpp| %.2e'

@@ -6,23 +6,12 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
+from tests._engines import fit
 from tests._util import relinf
 
 pytestmark = pytest.mark.gpu
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _fit(X, Y, hyper, **kw):
-    eng = _L().Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, **kw)
-    eng.set_data(X, Y)
-    eng.set_hyper(hyper)
-    eng.factorize()
-    return eng
 
 
 def _singular_problem():
@@ -37,10 +26,9 @@ def _singular_problem():
 
 
 def test_a_failed_append_keeps_its_point_and_refactorises_on_it():
-    L = _L()
     X, Y, hyper = _singular_problem()
     N0 = X.shape[0]
-    eng = _fit(X, Y, hyper, capacity=N0 + 2)
+    eng = fit(X, Y, hyper, capacity=N0 + 2)
     x_new, y_new = X[5], np.array([0.25, -0.5])
     assert eng.append(x_new, y_new) is False
     # the handle's count, read before anything sizes a host buffer by Engine.N
@@ -54,7 +42,7 @@ def test_a_failed_append_keeps_its_point_and_refactorises_on_it():
     info = eng.factorize()                                # the duplicate needs the jitter retry
     assert np.all(info == 1)
     Xa, Ya = np.vstack([X, x_new]), np.vstack([Y, y_new])
-    fresh = _fit(Xa, Ya, hyper)
+    fresh = fit(Xa, Ya, hyper)
     assert np.array_equal(fresh.factorize(), info)
     for a in range(2):
         chol, ref = eng.get(L.GET_CHOL, a), fresh.get(L.GET_CHOL, a)

@@ -3,7 +3,6 @@ broadcast, per-rank training + hyper all-gather, gathered prediction, and the 'p
 fallback when there are fewer outputs than ranks.  The engine is the oracle-backed stand-in
 (tests/_fake_engine.py); on the GPU box the same GP code drives libgpmpc + NCCL."""
 import os
-import socket
 
 import numpy as np
 import pytest
@@ -12,10 +11,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from oracle import gp_oracle as orc
-
-
-def _free_port():
-    s = socket.socket(); s.bind(('127.0.0.1', 0)); p = s.getsockname()[1]; s.close(); return p
+from tests._util import free_port
 
 
 def _worker(rank, world, port, case, q):
@@ -74,7 +70,7 @@ def test_two_ranks(case):
     world = 2
     ctx = mp.get_context('spawn')
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_worker, args=(r, world, port, case, q)) for r in range(world)]
     for pr in procs:
         pr.start()

@@ -7,19 +7,15 @@ import re
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from tests._util import GOLDEN, load_fixture, relinf
 
 pytestmark = pytest.mark.gpu
 
 
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
 def _engine(X, Y, **kw):
-    eng = _L().Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, **kw)
+    eng = L.Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, **kw)
     eng.set_data(X, Y)
     return eng
 
@@ -95,14 +91,14 @@ def test_a_notpd_entry_leaves_the_others_and_reports_what_nlml_reports():
     nan[4] = np.nan                           # a NaN signal std fails every pivot, with and without the jitter
     th = np.vstack([good[0], nan, good[1], dup, good[2]])
     nll, g, st = eng.nlml_batch(0, th)
-    assert st[1] == _L().ERR_NOTPD and np.isnan(nll[1]) and np.isnan(g[1]).all()
+    assert st[1] == L.ERR_NOTPD and np.isnan(nll[1]) and np.isnan(g[1]).all()
     alone_nll, alone_g, _ = eng.nlml_batch(0, good)
     for i, s in ((0, 0), (2, 1), (4, 2)):
         assert st[i] == 0 and nll[i] == alone_nll[s] and np.array_equal(g[i], alone_g[s])
     for i in range(len(th)):
         # status against nlml's outcome and against factorize's jitter report at the same row
         hyp = th[i:i + 1]
-        if st[i] == _L().ERR_NOTPD:
+        if st[i] == L.ERR_NOTPD:
             with pytest.raises(np.linalg.LinAlgError):
                 eng.nlml(0, th[i])
             eng.set_hyper(hyp)
@@ -117,7 +113,6 @@ def test_a_notpd_entry_leaves_the_others_and_reports_what_nlml_reports():
 
 
 def test_the_factorisation_is_left_as_it_was():
-    L = _L()
     p = orc.synthetic_problem(700, 5, 3, config_id=21)
     eng = _engine(p['X'], p['Y'])
     eng.set_hyper(p['hyper'])
@@ -139,7 +134,6 @@ def test_the_factorisation_is_left_as_it_was():
 
 
 def test_argument_and_state_errors_come_before_any_work():
-    L = _L()
     p = orc.synthetic_problem(200, 3, 2, config_id=3)
     th = _thetas(p['hyper'][0], 3, 0)
     eng = L.Engine(200, 3, 2, out_begin=1, out_count=1, device=0)

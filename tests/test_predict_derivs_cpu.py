@@ -7,6 +7,7 @@ from scipy.linalg import solve_triangular
 
 from oracle import gp_oracle as orc
 from oracle import hess_oracle as hor
+from tests._util import normalised
 
 OUTS = ('mean', 'var', 'J', 'dvar_dz', 'hess', 'd2var_dz2', 'd3mean_dz3', 'cov', 'dcov_dz', 'd2cov_dz2')
 EXTENDED = np.finfo(np.longdouble).eps < 1e-18
@@ -88,13 +89,6 @@ def mp_reference(X, hyper, alpha, linv, Z, S, dps=40):
                             + Hm[a][d][k] * Sg[d][e] * Hm[b][e][g] + Jm[a][d] * Sg[d][e] * T3[b][e][g][k]
                             for d in R for e in R))
     return out
-
-
-def normalised(x, ref, scale):
-    """Largest |x - ref| / scale; entries with a zero scale must agree exactly."""
-    d = np.abs(np.asarray(x, dtype=np.longdouble) - np.asarray(ref, dtype=np.longdouble))
-    assert not np.any(d[scale == 0]), 'a difference where the sum of |terms| is 0'
-    return float(np.max(np.divide(d, scale, out=np.zeros_like(d), where=scale > 0), initial=0.0))
 
 
 @needs_ld

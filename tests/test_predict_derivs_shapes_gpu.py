@@ -26,15 +26,17 @@ TA ways (case in brackets):
 
 and at sn = 1e-2 (nx8, cond(K) ~ 1e7) no larger: mean 2.0e-17, jac 3.3e-17, hess 1.2e-16, d3mean_dz3 1.5e-16, the rest
 <= 1.4e-20.  The outputs built from alpha ks alone (mean, jac, hess, d3mean_dz3) carry the few-ulp error of each ks; the
-ones through L^-1 are normalised by sums that include |L^-1| ks, so their errors are orders of magnitude smaller.  TOL
-is 10x each maximum rounded up to a power of ten.  The smallest guard ratios, all at sn = 1e-2, are 3.0e-10 (a block of
-d2var_dz2) and 5.7e-10 (dvar_dz), 4.1e-8 (the Sigma terms of dcov_dz) and 1.1e-8 (Sigma^T in dcov_dz), against the
+ones through L^-1 are normalised by sums that include |L^-1| ks, so their errors are orders of magnitude smaller.
+PREDICT_TOL (tests/_util.py) is 10x each maximum rounded up to a power of ten.  The smallest guard ratios, all at
+sn = 1e-2, are 3.0e-10 (a block of d2var_dz2) and 5.7e-10 (dvar_dz), 4.1e-8 (the Sigma terms of dcov_dz) and 1.1e-8 (Sigma^T in dcov_dz), against the
 guard's 1e4 x 1e-16; a block of hess or d3mean_dz3 moves them by >= 3.9e-3 against 1e4 x 1e-14."""
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import hess_oracle as hor
 from oracle import gp_oracle as orc
+from tests._util import PREDICT_TOL, normalised
 
 pytestmark = pytest.mark.gpu
 
@@ -54,17 +56,9 @@ CASES = {
 }
 FAMILIES = ('mean', 'var', 'cov', 'jac', 'dvar_dz', 'dcov_dz', 'hess', 'd2var_dz2', 'd3mean_dz3', 'd2cov_dz2')
 REF_KEY = dict(jac='J')
-# bars on the largest error normalised by the sum of |terms|, per output family (measured maxima in the module docstring)
-TOL = dict(mean=1e-15, var=1e-16, cov=1e-16, jac=1e-15, dvar_dz=1e-16, dcov_dz=1e-16, hess=1e-14, d2var_dz2=1e-16,
-           d3mean_dz3=1e-14, d2cov_dz2=1e-16)
 GUARD = 1e4
 # the three TA ways: one shared Sigma (spp 0), a per-point stack (spp 1), a non-symmetric shared Sigma
 SIGMA_WAYS = ('shared', 'stack', 'skew')
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
 
 
 def problem(name, H=None, seed=0):
@@ -111,16 +105,8 @@ def fit(name):
 
 def engine_factor(eng, Ny):
     """The engine's alpha (Ny, N) and L^-1 (Ny, N, N)."""
-    L = _L()
     return (np.stack([eng.get(L.GET_ALPHA, a) for a in range(Ny)]),
             np.stack([eng.get(L.GET_LINV, a) for a in range(Ny)]))
-
-
-def normalised(x, ref, scale):
-    """Largest |x - ref| / scale over the entries; entries whose sum of |terms| is 0 must be exactly 0 on both sides."""
-    d = np.abs(np.asarray(x, dtype=np.longdouble) - ref)
-    assert not np.any(d[scale == 0]), 'a nonzero entry where the sum of |terms| is 0'
-    return float(np.max(np.divide(d, scale, out=np.zeros_like(d), where=scale > 0), initial=0.0))
 
 
 def block_terms(X, hyper, alpha, linv, Z, lo, hi):
@@ -160,7 +146,7 @@ def check_guards(X, hyper, alpha, linv, Z, core, core_abs, S):
         for k, v in part.items():
             for a in range(Ny):
                 r = guard_ratio(v[:, a], core_abs[k][:, a])
-                assert r >= GUARD * TOL[k], ('block', lo, a, k, r)
+                assert r >= GUARD * PREDICT_TOL[k], ('block', lo, a, k, r)
                 seen['block ' + k] = min(seen.get('block ' + k, np.inf), r)
     if S is not None:
         me = hor.cov_derivs(core, None, 'ME')
@@ -169,7 +155,7 @@ def check_guards(X, hyper, alpha, linv, Z, core, core_abs, S):
             ab = hor.cov_derivs(core_abs, np.abs(S[way]), 'TA')
             for k in ('dcov_dz', 'd2cov_dz2'):
                 r = guard_ratio(ta[k] - me[k], ab[k])
-                assert r >= GUARD * TOL[k], ('Sigma terms', way, k, r)
+                assert r >= GUARD * PREDICT_TOL[k], ('Sigma terms', way, k, r)
                 seen['Sigma ' + k] = min(seen.get('Sigma ' + k, np.inf), r)
     # Sigma -> Sigma^T leaves the a = b blocks unchanged (Hm_a and T_a are symmetric in their derivative indices), so
     # only a pair of outputs, and only Nx > 1, can tell a transposed Sigma apart
@@ -179,7 +165,7 @@ def check_guards(X, hyper, alpha, linv, Z, core, core_abs, S):
         ab = hor.cov_derivs(core_abs, np.abs(S['skew']), 'TA')
         for k in ('dcov_dz', 'd2cov_dz2'):
             r = guard_ratio(tr[k] - sk[k], ab[k])
-            assert r >= GUARD * TOL[k], ('Sigma^T', k, r)
+            assert r >= GUARD * PREDICT_TOL[k], ('Sigma^T', k, r)
             seen['Sigma^T ' + k] = r
     return seen
 
@@ -188,7 +174,6 @@ def case_errors(name):
     """Per call ('ME', 'TA shared', 'TA stack', 'TA skew'): the largest normalised error of each output family, after
     the guards (their smallest ratios under 'guards').  On the reserved handle every call is repeated and must give the
     same bits."""
-    L = _L()
     _, Nx, Ny, H, _, _ = CASES[name]
     eng, X, Y, hyper, Z = fit(name)
     alpha, linv = engine_factor(eng, Ny)
@@ -214,13 +199,13 @@ def case_errors(name):
 
 @pytest.mark.parametrize('name', list(CASES))
 def test_predict_derivs_vs_long_double(name):
-    """Every output of ME and of the three TA ways against the reference, within TOL of the sums of |terms|, after the
-    guards."""
+    """Every output of ME and of the three TA ways against the reference, within PREDICT_TOL of the sums of |terms|,
+    after the guards."""
     res = case_errors(name)
     for c, errs in res.items():
         if c == 'guards':
             continue
-        bad = {k: e for k, e in errs.items() if not e <= TOL[k]}
+        bad = {k: e for k, e in errs.items() if not e <= PREDICT_TOL[k]}
         assert not bad, (name, c, bad)
 
 
@@ -229,7 +214,6 @@ def test_derivs_do_not_depend_on_batch_or_row(name):
     """A point's outputs have the same bits in batches of 1, R, R + 1, 64 and 65 points at permuted rows, for ME and for
     TA with a per-point Sigma: every sum of the derivative chain runs in a fixed order whatever the batch, and the
     derivative product gives a row the same bits at BM 64 and BM 16."""
-    L = _L()
     _, Nx, Ny, _, _, _ = CASES[name]
     R = 64 // Nx
     eng, X, Y, hyper, _ = fit(name)

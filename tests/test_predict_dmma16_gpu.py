@@ -4,7 +4,9 @@ repeat calls at a fixed stream-K partition are bit-identical."""
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
+from tests._engines import synthetic_engine
 
 
 pytestmark = pytest.mark.gpu
@@ -13,27 +15,11 @@ POOL = 130
 HS = [1, 7, 8, 9, 50, 56, 64, 65, 130]
 
 
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _engine(N, Nx, Ny, seed):
-    import gp_mpc_b200
-    p = orc.synthetic_problem(N, Nx, Ny, config_id=seed, H=POOL)
-    eng = gp_mpc_b200.Engine(N, Nx, Ny, device=0)
-    eng.set_data(p['X'], p['Y'])
-    eng.set_hyper(p['hyper'])
-    assert not eng.factorize().any()
-    return eng, p
-
-
 @pytest.mark.parametrize('Ny', [1, 8])
 def test_point_results_do_not_depend_on_chunk_size_or_row(Ny):
     """N = 1000 (not a multiple of 128): the same points at shuffled rows of batches of every size give bitwise the
     same var and cov as in the full batch of 130 (two 64-point chunks and one of 2)."""
-    L = _L()
-    eng, p = _engine(1000, 6, Ny, seed=4242 + Ny)
+    eng, p = synthetic_engine(1000, 6, Ny, seed=4242 + Ny, H=POOL)
     Z, Sigma = p['Z'], p['Sigma']
     _, var_ref, cov_ref, _ = eng.predict(Z, Sigma, L.METHOD_TA)
     assert (var_ref > 0).all()
@@ -50,8 +36,7 @@ def test_point_results_do_not_depend_on_chunk_size_or_row(Ny):
 @pytest.mark.parametrize('Ny', [1, 8])
 def test_var_matches_linv_ks_from_the_engine(Ny):
     """var = sf2 - |L^-1 ks|^2 with L^-1 read back from the engine (GET_LINV) and ks formed in numpy."""
-    L = _L()
-    eng, p = _engine(1000, 6, Ny, seed=777 + Ny)
+    eng, p = synthetic_engine(1000, 6, Ny, seed=777 + Ny, H=POOL)
     X, Z, hyper = p['X'], p['Z'], p['hyper']
     Nx = X.shape[1]
     for H in (1, 50, 130):
@@ -68,8 +53,7 @@ def test_var_matches_linv_ks_from_the_engine(Ny):
 
 @pytest.mark.parametrize('ctas', [1, 7, 1000])
 def test_repeat_calls_are_bit_identical(ctas):
-    L = _L()
-    eng, p = _engine(1000, 6, 8, seed=99)
+    eng, p = synthetic_engine(1000, 6, 8, seed=99, H=POOL)
     eng.set_option('predict_ctas', ctas)
     for H in (9, 56, 130):
         first = eng.predict(p['Z'][:H], p['Sigma'], L.METHOD_TA)

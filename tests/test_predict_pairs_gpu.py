@@ -8,8 +8,9 @@ for a point in any row of an H = 1, 8 or 50 batch, and from predict_grad, whose 
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
-from tests.test_predict_panel_gpu import VAR_TOL
+from tests._util import PREDICT_VAR_TOL
 
 pytestmark = pytest.mark.gpu
 
@@ -19,16 +20,11 @@ SIZES = (8320, 8448, 16384)
 GRIDS = {16384: (0, 64, 132), 8320: (68, 34, 136), 8448: (68, 34, 136)}      # first: the grid of the other tests
 
 
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
 @pytest.fixture(scope='module', params=SIZES)
 def model(request):
     N = request.param
     p = orc.synthetic_problem(N, NX, NY, config_id=900 + N % 97, H=H)
-    eng = _L().Engine(N, NX, NY, device=0)
+    eng = L.Engine(N, NX, NY, device=0)
     eng.set_data(p['X'], p['Y'])
     eng.set_hyper(p['hyper'])
     assert not eng.factorize().any()
@@ -38,7 +34,7 @@ def model(request):
 
 
 def predict_var(eng, Z, Sigma):
-    return eng.predict(Z, Sigma, _L().METHOD_TA, want_cov=False, want_jac=False)[1]
+    return eng.predict(Z, Sigma, L.METHOD_TA, want_cov=False, want_jac=False)[1]
 
 
 def test_var_matches_long_double_linv_ks(model):
@@ -52,7 +48,7 @@ def test_var_matches_long_double_linv_ks(model):
         ell, sf2 = LD(1) * hyper[a, :NX], LD(hyper[a, NX]) ** 2
         d = (X.astype(LD)[:, None, :] - Z[None, :, :]) / ell
         ks = sf2 * np.exp(-0.5 * np.sum(d * d, axis=2))                  # (N, 2)
-        Li = eng.get(_L().GET_LINV, a)
+        Li = eng.get(L.GET_LINV, a)
         v, w = np.zeros((N, len(rows)), LD), np.zeros((N, len(rows)), LD)
         for r0 in range(0, N, 2048):                                   # L^-1 is lower triangular
             r1 = min(N, r0 + 2048)
@@ -62,7 +58,7 @@ def test_var_matches_long_double_linv_ks(model):
         ref, scale = sf2 - np.sum(v * v, axis=0), sf2 + np.sum(w * w, axis=0)
         err = float(np.max(np.abs(var[rows, a].astype(LD) - ref) / scale))
         worst = max(worst, err)
-        assert err <= VAR_TOL, (N, a, err)
+        assert err <= PREDICT_VAR_TOL, (N, a, err)
     print('MEASURED N=%d var vs long double %.2e' % (N, worst))
 
 
@@ -94,5 +90,5 @@ def test_predict_grad_product_repeats_the_fused_var(model):
     if N == 16384:
         pytest.skip('U = L^-T of 8 outputs at N = 16384 does not fit next to the predict buffers')
     Z = p['Z'][:8]
-    g = eng.predict_grad(Z, p['Sigma'], _L().METHOD_TA)
+    g = eng.predict_grad(Z, p['Sigma'], L.METHOD_TA)
     assert np.array_equal(g['var'], predict_var(eng, Z, p['Sigma']))

@@ -13,20 +13,15 @@ test_predict_derivs_shapes_gpu."""
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle import hess_oracle as hor
-from tests.test_predict_derivs_shapes_gpu import TOL as PTOL, normalised
+from tests._util import PREDICT_TOL, PREDICT_VAR_TOL, normalised
 
 pytestmark = pytest.mark.gpu
 
 LD = np.longdouble
-VAR_TOL = 1e-16          # a stale band is an O(1) error; the fp64 product measured at most 2.7e-19 of the scale
 HS = (1, 50, 65)
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
 
 
 def problem(N, Nx, Ny, seed=0, sn=0.1):
@@ -37,7 +32,7 @@ def problem(N, Nx, Ny, seed=0, sn=0.1):
 
 
 def engine(X, Y, hyper, cap=None, out_begin=0, out_count=None):
-    eng = _L().Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, capacity=cap, out_begin=out_begin,
+    eng = L.Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, capacity=cap, out_begin=out_begin,
                       out_count=out_count)
     eng.set_data(X, Y)
     eng.set_hyper(hyper)
@@ -52,7 +47,6 @@ def points(X, H, seed):
 
 def var_ref(eng, X, hyper, Z):
     """(ref, scale), each (H, out_count): sf2 - |L^-1 ks|^2 and sf2 + (|L^-1| |ks|)^2 in long double."""
-    L = _L()
     Nx = X.shape[1]
     ref, scale = [], []
     for a in eng.local_outputs:
@@ -68,7 +62,6 @@ def var_ref(eng, X, hyper, Z):
 
 def check(eng, X, hyper, label, hs=HS):
     """var of gpmpc_predict (all outputs on the handle) and the diagonal of gpmpc_posterior_cov against var_ref."""
-    L = _L()
     full = eng.out_begin == 0 and eng.out_count == eng.Ny
     Zs = [points(X, H, seed=H + X.shape[0]) for H in hs]
     ref_all, scale_all = var_ref(eng, X, hyper, np.vstack(Zs))
@@ -84,7 +77,7 @@ def check(eng, X, hyper, label, hs=HS):
         for k, v in got.items():
             err = float(np.max(np.abs(v.astype(LD) - ref) / scale))
             print('MEASURED', label, k, 'H=%d' % H, '%.2e' % err)
-            assert err <= VAR_TOL, (label, k, H, err)
+            assert err <= PREDICT_VAR_TOL, (label, k, H, err)
 
 
 # name -> (N, Nx, Ny): Npad / 128 = 2 (N < 256), 3 (half tile), 5, 6
@@ -183,7 +176,6 @@ def test_sharded_handle():
 def test_other_products_of_linv():
     """predict_grad / predict_hess repeat their bits and match the long-double reference; roll-outs repeat their bits;
     the refinement (two L^-1 products and one of L) matches var_ref."""
-    L = _L()
     Nx, Ny = 5, 3
     X, Y, hyper = problem(300, Nx, Ny)
     eng = engine(X[:290], Y[:290], hyper, cap=400)
@@ -203,7 +195,7 @@ def test_other_products_of_linv():
         for k in keys:
             err = normalised(out[k], ref[k], ab[k])
             print('MEASURED', k, '%.2e' % err)
-            assert err <= PTOL[k], (k, err)
+            assert err <= PREDICT_TOL[k], (k, err)
     Nu = Nx - Ny
     z0 = np.tile(X[:1], (4, 1))
     U = 0.1 * np.ones((4, 5, Nu))

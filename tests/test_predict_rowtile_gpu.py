@@ -6,7 +6,9 @@ any persistent-grid size."""
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
+from tests._engines import synthetic_engine
 from tests._util import relinf
 
 
@@ -16,25 +18,9 @@ POOL = 130
 SIZES = [(1100, 1), (1100, 8), (100, 1), (100, 8)]
 
 
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _engine(N, Nx, Ny, seed):
-    import gp_mpc_b200
-    p = orc.synthetic_problem(N, Nx, Ny, config_id=seed, H=POOL)
-    eng = gp_mpc_b200.Engine(N, Nx, Ny, device=0)
-    eng.set_data(p['X'], p['Y'])
-    eng.set_hyper(p['hyper'])
-    assert not eng.factorize().any()
-    return eng, p
-
-
 @pytest.mark.parametrize('N,Ny', SIZES)
 def test_half_tile_var_matches_linv_ks(N, Ny):
-    L = _L()
-    eng, p = _engine(N, 6, Ny, seed=31 + N + Ny)
+    eng, p = synthetic_engine(N, 6, Ny, seed=31 + N + Ny, H=POOL)
     X, Z, hyper = p['X'], p['Z'], p['hyper']
     for H in (1, 56, 130):
         _, var, _, _ = eng.predict(Z[:H], None, L.METHOD_ME, want_cov=False, want_jac=False)
@@ -47,8 +33,7 @@ def test_half_tile_var_matches_linv_ks(N, Ny):
 
 @pytest.mark.parametrize('N,Ny', SIZES)
 def test_half_tile_results_do_not_depend_on_batch_or_row(N, Ny):
-    L = _L()
-    eng, p = _engine(N, 6, Ny, seed=57 + N + Ny)
+    eng, p = synthetic_engine(N, 6, Ny, seed=57 + N + Ny, H=POOL)
     Z, Sigma = p['Z'], p['Sigma']
     _, var_ref, cov_ref, _ = eng.predict(Z, Sigma, L.METHOD_TA)
     rng = np.random.default_rng(N + Ny)
@@ -62,8 +47,7 @@ def test_half_tile_results_do_not_depend_on_batch_or_row(N, Ny):
 
 @pytest.mark.parametrize('N,Ny', SIZES)
 def test_half_tile_refine_and_grad_vs_oracle(N, Ny):
-    L = _L()
-    eng, p = _engine(N, 6, Ny, seed=83 + N + Ny)
+    eng, p = synthetic_engine(N, 6, Ny, seed=83 + N + Ny, H=POOL)
     X, Y, hyper, Z, Sigma = p['X'], p['Y'], p['hyper'], p['Z'][:9], p['Sigma']
     post = orc.postfit(X, Y, hyper, lapack_general_solve=False)
     mo, vo = orc.gp_mean_var(X, hyper, post['alpha'], post['chol'], Z)
@@ -89,7 +73,6 @@ def test_refine_after_a_full_k_build_vs_oracle(N):
     """A full K build (PROF_KBUILD_FULL) leaves K's upper triangle in output 0's L slab and the factorisation rewrites only
     the lower one: the refinement's product with L must not read the 128 x 128 blocks above the diagonal."""
     import gp_mpc_b200
-    L = _L()
     p = orc.synthetic_problem(N, 6, 2, config_id=11, H=POOL)
     X, Y, hyper, Z, Sigma = p['X'], p['Y'], p['hyper'], p['Z'][:20], p['Sigma']
     eng = gp_mpc_b200.Engine(N, 6, 2, device=0)
@@ -107,8 +90,7 @@ def test_refine_after_a_full_k_build_vs_oracle(N):
 
 @pytest.mark.parametrize('ctas', [1, 7, 133, 1000])
 def test_half_tile_repeat_calls_are_bit_identical(ctas):
-    L = _L()
-    eng, p = _engine(1100, 6, 8, seed=5)
+    eng, p = synthetic_engine(1100, 6, 8, seed=5, H=POOL)
     eng.set_option('predict_ctas', ctas)
     for H in (9, 56, 130):
         first = eng.predict(p['Z'][:H], p['Sigma'], L.METHOD_TA)

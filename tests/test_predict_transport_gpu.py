@@ -15,7 +15,9 @@ import threading
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
+from tests._engines import npad
 from tests._util import relinf
 
 TOL = 1e-6
@@ -58,10 +60,6 @@ def transport(npad, nloc, Nx, Ny, H, hcap, has_sigma, spp, outputs=OUTPUTS):
     return zc_in, zc_out
 
 
-def _npad(n):
-    return -(-n // 128) * 128
-
-
 # C. one shape per (zc_in, zc_out): name -> (N, Nx, Ny, H)
 SHAPES = {(1, 1): (300, 5, 3, 20),          # small problem
           (0, 1): (300, 6, 4, 65),          # one point past a chunk: dIn, outputs still small
@@ -79,18 +77,18 @@ def test_transport_model_reaches_every_branch():
     copies out for some output subsets with mean NULL, so the D2H source offset lo is not 0."""
     for want, (N, Nx, Ny, H) in SHAPES.items():
         for has_sigma, spp in ((True, 0), (True, 1), (False, 0)):
-            assert transport(_npad(N), Ny, Nx, Ny, H, 0, has_sigma, spp) == want, (want, has_sigma, spp)
-            assert transport(_npad(N), Ny, Nx, Ny, H, grow(0, H), has_sigma, spp) == want
+            assert transport(npad(N), Ny, Nx, Ny, H, 0, has_sigma, spp) == want, (want, has_sigma, spp)
+            assert transport(npad(N), Ny, Nx, Ny, H, grow(0, H), has_sigma, spp) == want
     N, Nx, Ny, H = HIST
-    assert transport(_npad(N), Ny, Nx, Ny, H, 0, True, 0) == (1, 1)
+    assert transport(npad(N), Ny, Nx, Ny, H, 0, True, 0) == (1, 1)
     assert grow(grow(0, H), H_BIG) == H_BIG
-    assert transport(_npad(N), Ny, Nx, Ny, H, H_BIG, True, 0) == (0, 0)
-    assert transport(_npad(N), Ny, Nx, Ny, H_BIG, 0, True, 0) == (0, 0)
+    assert transport(npad(N), Ny, Nx, Ny, H, H_BIG, True, 0) == (0, 0)
+    assert transport(npad(N), Ny, Nx, Ny, H_BIG, 0, True, 0) == (0, 0)
     N, Nx, Ny, H = SHAPES[(0, 0)]
-    outs = [s for s in _subsets() if not transport(_npad(N), Ny, Nx, Ny, H, H, True, 0, s)[1]]
+    outs = [s for s in _subsets() if not transport(npad(N), Ny, Nx, Ny, H, H, True, 0, s)[1]]
     assert ('jac',) in outs and ('var', 'cov') in outs and ('cov',) in outs and ('mean',) not in outs
     N, Nx, Ny, H = SHAPES[(1, 1)]
-    assert all(transport(_npad(N), Ny, Nx, Ny, H, 64, True, 0, s) == (1, 1) for s in _subsets())
+    assert all(transport(npad(N), Ny, Nx, Ny, H, 64, True, 0, s) == (1, 1) for s in _subsets())
     # the C5 headline shape: copy in (the ks grid re-reads Z too often for zero-copy), zero-copy out
     assert transport(16384, 8, 10, 8, 50, 0, True, 0) == (0, 1)
 
@@ -100,11 +98,6 @@ def _subsets():
 
 
 # ------------------------------------------------------------------ GPU helpers
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
 def _ptr(t):
     return None if t is None else t.data_ptr()
 
@@ -132,7 +125,7 @@ class Model:
         self.eng.close()
 
     def transport(self, H, has_sigma, spp, outputs=OUTPUTS):
-        return transport(_npad(self.N), self.Ny, self.Nx, self.Ny, H, self.hcap, has_sigma, spp, outputs)
+        return transport(npad(self.N), self.Ny, self.Nx, self.Ny, H, self.hcap, has_sigma, spp, outputs)
 
     def inputs(self, H, spp):
         """Distinct test points and input covariances: (Z (H,Nx), Sigma (Nx,Nx) or (H,Nx,Nx))."""
@@ -180,7 +173,7 @@ class Model:
         alpha, chol = self.factors()
         mo, vo = orc.gp_mean_var(self.X, self.hyper, alpha, chol, Z)
         Jo = orc.gp_mean_jac(self.X, self.hyper, alpha, Z)
-        co = orc.ta_cov(vo, Jo, Sigma) if method == _L().METHOD_TA else orc.me_cov(vo)
+        co = orc.ta_cov(vo, Jo, Sigma) if method == L.METHOD_TA else orc.me_cov(vo)
         return dict(mean=mo, var=vo, cov=co, jac=Jo)
 
 
@@ -214,7 +207,6 @@ def _bench_model(name):
 def _bench_step(m, w):
     """bench.py's timed step: TA, one Sigma (spp = 0), device outputs, sync = False, then one synchronize."""
     import torch
-    L = _L()
     outs = m.device(torch.from_numpy(w['Z']).cuda(), torch.from_numpy(w['Sigma']).cuda(), L.METHOD_TA, sync=False)
     m.eng.synchronize()
     return _np(outs)
@@ -226,7 +218,6 @@ def test_bench_step_vs_oracle(name):
     """The outputs of bench.py's timed call at C2 (N=1000) and C3 (N=4096), every output against independent CPU factors
     (factor_large / predict_large / ta_cov), and bit for bit against gpmpc_predict on the same handle."""
     m, w = _bench_model(name)
-    L = _L()
     Ny, Nx, H = m.Ny, m.Nx, w['Z'].shape[0]
     got = _bench_step(m, w)
     mo = np.zeros((H, Ny)); vo = np.zeros((H, Ny)); Jo = np.zeros((H, Ny, Nx))
@@ -246,7 +237,6 @@ def test_bench_step_c5():
     bits for all 8 outputs, and output Ny-1 matches an independent CPU factor at 1e-6 (bench.py's own parity check
     compares the separate e2e call)."""
     m, w = _bench_model('c5')
-    L = _L()
     Ny = m.Ny
     got = _bench_step(m, w)
     again = _bench_step(m, w)
@@ -269,7 +259,6 @@ def test_device_entry_sigma_per_point_me_and_no_sigma():
     """gpmpc_predict_device with one Sigma per point, with ME and dSigma = NULL, and with TA, d_cov = NULL and
     dSigma = NULL (allowed: only a covariance output needs Sigma, gpmpc.cu:1496): the oracle at 1e-6 and
     gpmpc_predict's bits."""
-    L = _L()
     m = Model(300, 6, 3, config_id=11)
     Z, Sg = m.inputs(30, spp=1)
     got = _np(m.device(Z, Sg, L.METHOD_TA))
@@ -301,7 +290,6 @@ def test_device_outputs_stay_in_their_regions():
     """gpmpc_predict_device writing into slices at odd element offsets of NaN-filled buffers, at H = 20 (the fused
     assembly) and H = 2100 (assemble_kernel): the plain call's bits inside, the sentinels untouched outside."""
     import torch
-    L = _L()
     m = Model(*SHAPES[(0, 0)][:3], config_id=12)
     for H in (20, H_BIG):
         Z, S = m.inputs(H, spp=0)
@@ -324,7 +312,6 @@ def test_device_outputs_stay_in_their_regions():
 def _host_call(m, method, Z, Sigma, names):
     """gpmpc_predict through ctypes into caller-side buffers at odd offsets of NaN-filled arrays; NULL for the outputs
     not in names.  Returns (rc, outputs, buffers)."""
-    L = _L()
     lib = L.load()
     H = Z.shape[0]
     Z = np.ascontiguousarray(Z)
@@ -353,7 +340,6 @@ def test_host_output_subsets(want):
     odd offsets inside NaN sentinels, on a zero-copy shape and on the copy-out shape: each output is the full call's,
     bit for bit, and nothing outside it is written.  The subsets move lo, the first output of the D2H span; on the
     copy-out shape jac, cov and (var, cov) copy out with mean NULL.  The call with every output NULL returns OK."""
-    L = _L()
     N, Nx, Ny, H = SHAPES[want]
     m = Model(N, Nx, Ny, config_id=13)
     Z, S = m.inputs(H, spp=0)
@@ -383,7 +369,6 @@ def test_transports_agree_bit_for_bit(want):
     """On the shape of each (zc_in, zc_out): gpmpc_predict and gpmpc_predict_device give the same bits for TA with one
     Sigma, TA with a Sigma per point and ME, and both match the oracle (gp_mean_var / gp_mean_jac / ta_cov) at 1e-6.
     The device entry reads and writes device memory directly, so it is the common reference of all four transports."""
-    L = _L()
     N, Nx, Ny, H = SHAPES[want]
     m = Model(N, Nx, Ny, config_id=14 + N)
     for method, spp in ((L.METHOD_TA, 0), (L.METHOD_TA, 1), (L.METHOD_ME, 0)):
@@ -403,7 +388,6 @@ def test_small_call_after_a_large_one():
     """A small TA call on a fresh handle goes zero-copy both ways; after one call of 2100 points the same call copies
     both ways (the capacity-based layout, DESIGN 7).  The two small calls give the same bits, and the large call matches
     the oracle."""
-    L = _L()
     N, Nx, Ny, H = HIST
     m = Model(N, Nx, Ny, config_id=15)
     Z, S = m.inputs(H, spp=0)
@@ -431,7 +415,6 @@ def _sequence(m, host_at=None):
     fourth call and H = 2100 grows the gather buffer dG while earlier calls may still run.  host_at: index of a host
     gpmpc_predict call placed before that device call.  Returns [(H, method, Z, S, ctas, outputs)]."""
     import torch
-    L = _L()
     calls = []
     big_ctas = 4 * torch.cuda.get_device_properties(0).multi_processor_count + 8    # above the default grid
     m.eng.set_option('predict_ctas', 0)
@@ -476,7 +459,6 @@ def test_back_to_back_without_sync():
 
 # ------------------------------------------------------------------ F. two handles, two host threads
 def _mixed_calls(m, n=20):
-    L = _L()
     out = []
     for i in range(n):
         H = (5, 64, 70, 33)[i % 4]
@@ -487,7 +469,7 @@ def _mixed_calls(m, n=20):
 
 def _run_calls(m, calls, results, barrier=None):
     import torch
-    ta = _L().METHOD_TA
+    ta = L.METHOD_TA
     try:
         dev = []
         for Z, S, method, kind in calls:          # device copies of the inputs, made before the threads meet

@@ -8,7 +8,7 @@ from scipy.linalg import solve_triangular
 import gp_mpc_b200
 from oracle import gp_oracle as orc
 from oracle import remove_oracle as rmo
-from tests._fake_engine import OracleEngine
+from tests._fake_engine import OracleEngine, problem
 from tests._util import load_fixture, relinf
 
 
@@ -21,14 +21,6 @@ def _inv(L):
     return solve_triangular(L, np.eye(L.shape[0]), lower=True)
 
 
-def _problem(case):
-    if case in ('tank', 'car'):
-        m = load_fixture(case)
-        return m['X'], m['Y'], m['hyper']
-    p = orc.synthetic_problem(300, 5, 2, config_id=17)
-    return p['X'], p['Y'], p['hyper']
-
-
 # (chol, L^-1, alpha).  L^-1 and alpha of two factorisations of the same K differ by about cond(K) eps, even where the
 # removal is exact (the last point): cond(K) ~ 6e7 for tank, ~ 7e10 for car, ~ 2e6 for the synthetic problem
 TOL = {'tank': (1e-11, 5e-9, 1e-8), 'car': (1e-9, 5e-6, 1e-5), 'synthetic': (1e-11, 1e-9, 1e-9)}
@@ -37,7 +29,7 @@ TOL = {'tank': (1e-11, 5e-9, 1e-8), 'car': (1e-9, 5e-6, 1e-5), 'synthetic': (1e-
 @pytest.mark.parametrize('case', ['tank', 'car', 'synthetic'])
 @pytest.mark.parametrize('where', ['first', 'middle', 'last', 'several'])
 def test_oracle_form_matches_a_refit(case, where):
-    X, Y, hyper = _problem(case)
+    X, Y, hyper = problem(case)
     N = X.shape[0]
     idx = {'first': [0], 'middle': [N // 2], 'last': [N - 1], 'several': [N // 3, 0, N - 1, 7, N // 2]}[where]
     keep = np.setdiff1d(np.arange(N), idx)

@@ -6,33 +6,13 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle import greedy_oracle as gro
-from tests._util import load_fixture, relinf
+from tests._engines import fit, problem
+from tests._util import relinf
 
 pytestmark = pytest.mark.gpu
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _fit(X, Y, hyper, **kw):
-    eng = _L().Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, **kw)
-    eng.set_data(X, Y)
-    eng.set_hyper(hyper)
-    eng.factorize()
-    return eng
-
-
-def _problem(case):
-    if case in ('tank', 'car'):
-        m = load_fixture(case)
-        return m['X'], m['Y'], m['hyper']
-    N, Nx, Ny = case
-    p = orc.synthetic_problem(N, Nx, Ny, config_id=N + Nx)
-    return p['X'], p['Y'], p['hyper']
 
 
 def _indices(where, N):
@@ -50,7 +30,6 @@ def _preds_vs(eng, X, Y, hyper, Z, Sigma, post=None):
     post = post or orc.postfit(X, Y, hyper, lapack_general_solve=False)
     mo, vo = orc.gp_mean_var(X, hyper, post['alpha'], post['chol'], Z)
     Jo = orc.gp_mean_jac(X, hyper, post['alpha'], Z)
-    L = _L()
     m, v, c, J = eng.predict(Z, Sigma, L.METHOD_TA)
     assert relinf(m, mo) < 1e-6 and relinf(v, vo) < 1e-6 and relinf(J, Jo) < 1e-6
     assert relinf(c, orc.ta_cov(vo, Jo, Sigma)) < 1e-6
@@ -67,11 +46,10 @@ CASES = [('tank', w) for w in ('first', 'middle', 'last', 'several')] + \
 
 @pytest.mark.parametrize('case,where', CASES, ids=['%s-%s' % c for c in CASES])
 def test_removal_matches_a_refit(case, where):
-    X, Y, hyper = _problem(case)
-    L = _L()
+    X, Y, hyper = problem(case)
     N = X.shape[0]
     idx = _indices(where, N)
-    eng = _fit(X, Y, hyper)
+    eng = fit(X, Y, hyper)
     cap = eng.capacity
     eng.remove(idx)
     assert eng.N == N - len(idx) and eng.capacity == cap
@@ -92,20 +70,19 @@ def test_removal_matches_a_refit(case, where):
 @pytest.mark.parametrize('N', [129, 257])
 def test_removal_across_a_padding_boundary(N):
     """129 -> 128 and 257 -> 256 points: the last 128-block becomes all identity tail (the padded size stays)."""
-    X, Y, hyper = _problem((N, 3, 2))
-    eng = _fit(X, Y, hyper)
+    X, Y, hyper = problem((N, 3, 2))
+    eng = fit(X, Y, hyper)
     eng.remove([N // 2])
     assert eng.N == N - 1 and eng.capacity == -(-N // 128) * 128
     keep = np.setdiff1d(np.arange(N), [N // 2])
     post = _preds_vs(eng, X[keep], Y[keep], hyper, _points(X, 6, 2), 1e-4 * np.eye(3))
     for a in range(2):
-        assert relinf(eng.get(_L().GET_CHOL, a), post['chol'][a]) < 1e-10
+        assert relinf(eng.get(L.GET_CHOL, a), post['chol'][a]) < 1e-10
 
 
 def test_a_sharded_handle_updates_the_outputs_it_owns():
-    X, Y, hyper = _problem((700, 5, 4))
-    L = _L()
-    eng = _fit(X, Y, hyper, out_begin=1, out_count=2)
+    X, Y, hyper = problem((700, 5, 4))
+    eng = fit(X, Y, hyper, out_begin=1, out_count=2)
     eng.remove([600, 3, 128])
     keep = np.setdiff1d(np.arange(700), [600, 3, 128])
     post = orc.postfit(X[keep], Y[keep], hyper, lapack_general_solve=False)
@@ -119,15 +96,14 @@ def test_every_entry_point_matches_a_fresh_handle():
     diagonal blocks and the identity tail feed the stream-K product like a fresh factorisation's."""
     p = orc.synthetic_problem(700, 4, 2, config_id=31, H=6)
     X, Y, hyper, Z, Sigma = p['X'], p['Y'], p['hyper'], p['Z'], p['Sigma']
-    L = _L()
     idx = [699, 128, 0, 127, 350, 256]
     keep = np.setdiff1d(np.arange(700), idx)
-    eng = _fit(X, Y, hyper)
+    eng = fit(X, Y, hyper)
     # the derivative caches (Li^T, EM K^-1) are built before the removal and must not survive it
     eng.predict_grad(Z, Sigma, L.METHOD_TA)
     eng.predict_em_grad(Z[:2], Sigma)
     eng.remove(idx)
-    fresh = _fit(X[keep], Y[keep], hyper)
+    fresh = fit(X[keep], Y[keep], hyper)
     assert eng.capacity == fresh.capacity
     for a in range(2):
         assert relinf(eng.get(L.GET_CHOL, a), fresh.get(L.GET_CHOL, a)) < 1e-11
@@ -160,8 +136,7 @@ def test_a_sliding_window_at_a_full_padded_size():
     Nw, cycles = 4096, 256
     p = orc.synthetic_problem(Nw + cycles, 4, 2, config_id=41)
     X, Y, hyper = p['X'], p['Y'], p['hyper']
-    L = _L()
-    eng = _fit(X[:Nw], Y[:Nw], hyper)
+    eng = fit(X[:Nw], Y[:Nw], hyper)
     assert eng.capacity == Nw
     for c in range(cycles):
         eng.remove([0])
@@ -175,9 +150,8 @@ def test_a_sliding_window_at_a_full_padded_size():
 
 
 def test_freed_capacity_takes_appends_and_greedy_appends():
-    X, Y, hyper = _problem((256, 3, 2))
-    L = _L()
-    eng = _fit(X, Y, hyper)
+    X, Y, hyper = problem((256, 3, 2))
+    eng = fit(X, Y, hyper)
     assert eng.capacity == 256
     eng.remove([10, 200, 0, 130, 64, 255])
     Xn = _points(X, 3, 5); Yn = np.random.default_rng(6).standard_normal((3, 2))
@@ -199,13 +173,12 @@ def test_freed_capacity_takes_appends_and_greedy_appends():
 
 
 def test_two_handles_give_identical_bits():
-    X, Y, hyper = _problem((1000, 8, 6))
-    L = _L()
+    X, Y, hyper = problem((1000, 8, 6))
     Z = _points(X, 7, 2)
     Xn = _points(X, 4, 3); Yn = np.random.default_rng(4).standard_normal((4, 6))
     out = []
     for _ in range(2):
-        eng = _fit(X, Y, hyper)
+        eng = fit(X, Y, hyper)
         eng.remove([999, 0, 513, 128])
         for k in range(4):
             assert eng.append(Xn[k], Yn[k])
@@ -219,11 +192,10 @@ def test_two_handles_give_identical_bits():
 
 
 def test_state_and_argument_errors_leave_the_model_untouched():
-    X, Y, hyper = _problem((300, 3, 2))
-    L = _L()
+    X, Y, hyper = problem((300, 3, 2))
     lib = L.load()
     Z = _points(X, 4, 1)
-    eng = _fit(X, Y, hyper)
+    eng = fit(X, Y, hyper)
     before = eng.predict(Z, 1e-4 * np.eye(3), L.METHOD_TA)
 
     def call(idx, n=None, null=False):

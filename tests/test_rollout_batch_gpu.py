@@ -5,33 +5,12 @@ import ctypes
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle.rollout_oracle import predict_compare_loop
-from tests._util import load_fixture, load_golden, relinf
+from tests._fake_engine import fixture_gp
+from tests._util import relinf, trajectories
 
 pytestmark = pytest.mark.gpu
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _gp(name):
-    import gp_mpc_b200
-    m = load_fixture(name)
-    kw = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'], hyper=dict(hyper=m['hyper']))
-    if m['normalize']:
-        kw.update(meta=m['meta'], xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
-    return gp_mpc_b200.GP(m['X'], m['Y'], **kw), m
-
-
-def _case(name, nb, Nt):
-    d = load_golden('derived', name)
-    x0 = np.asarray(d['x0'], dtype=np.float64)
-    u0 = np.asarray(d['u0'], dtype=np.float64)
-    X0 = np.stack([x0 * (1 + 0.01 * (b % 23) - 0.004 * (b % 7)) for b in range(nb)])
-    U = np.stack([np.tile(u0, (Nt, 1)) * (1 + 0.03 * np.arange(Nt)[:, None] + 0.005 * (b % 11)) for b in range(nb)])
-    return X0, U, 0.9 * x0 + 0.1
 
 
 def _scalers(m, X0, U):
@@ -47,8 +26,8 @@ def _scalers(m, X0, U):
 @pytest.mark.parametrize('name', ['tank', 'car'])
 def test_batched_open_loop_equals_the_host_loop(name, B):
     """B trajectories in one predict pass per step (two 64-point chunks above 64) equal the per-step host loop."""
-    gp, m = _gp(name)
-    X0, U, _ = _case(name, B, 4)
+    gp, m = fixture_gp(name)
+    X0, U, _ = trajectories(name, B, 4, cyclic=True)
     rm, rv = gp.rollout(X0, U, methods=['TA', 'ME'])
     hm, hv = gp.rollout(X0, U, methods=['TA', 'ME'], device_rollout=False)
     assert rm.shape == (2, B, 5, m['Y'].shape[1])
@@ -60,10 +39,9 @@ def test_batched_open_loop_equals_the_host_loop(name, B):
 
 @pytest.mark.parametrize('name', ['tank', 'car'])
 def test_single_entry_is_the_batch_of_one_bit_for_bit(name):
-    L = _L()
-    gp, m = _gp(name)
+    gp, m = fixture_gp(name)
     eng = gp.engine
-    X0, U, _ = _case(name, 3, 6)
+    X0, U, _ = trajectories(name, 3, 6, cyclic=True)
     Ny = X0.shape[1]
     zx, un, scale, _ = _scalers(m, X0, U)
     z0 = np.concatenate([zx, un[:, 0]], 1)
@@ -87,8 +65,8 @@ def test_device_feedback_equals_host_loop_and_predict_compare(name, B):
     """GP.rollout(feedback=True) on the device (the gain of each trajectory's (x0, u[0]); u_t = K (mean_t - x_ref), input
     blocks K cov K^T, cov K^T) against the host loop (1e-12) and predict_compare's restatement with the CPU factor (1e-6,
     as every GPU-against-oracle comparison here)."""
-    gp, m = _gp(name)
-    X0, U, x_ref = _case(name, B, 8)
+    gp, m = fixture_gp(name)
+    X0, U, x_ref = trajectories(name, B, 8, cyclic=True)
     rm, rv = gp.rollout(X0, U, methods=['TA', 'ME'], feedback=True, x_ref=x_ref)
     hm, hv = gp.rollout(X0, U, methods=['TA', 'ME'], feedback=True, x_ref=x_ref, device_rollout=False)
     assert relinf(rm, hm) < 1e-12 and relinf(rv, hv) < 1e-12
@@ -101,10 +79,9 @@ def test_device_feedback_equals_host_loop_and_predict_compare(name, B):
 @pytest.mark.parametrize('name', ['tank', 'car'])
 def test_shared_gain_batch_equals_one_trajectory_at_a_time(name):
     """One gain for B = 5 different starts in a single pass (five CTAs of the feedback kernel) equals five B = 1 passes."""
-    L = _L()
-    gp, m = _gp(name)
+    gp, m = fixture_gp(name)
     eng = gp.engine
-    X0, U, x_ref = _case(name, 5, 7)
+    X0, U, x_ref = trajectories(name, 5, 7, cyclic=True)
     Ny, Nu = X0.shape[1], U.shape[2]
     A, Bm = gp.discrete_linearize(X0[0], U[0, 0], None)
     import gp_mpc_b200
@@ -143,9 +120,8 @@ def test_batched_autonomous_system():
 
 def test_argument_checks():
     import gp_mpc_b200
-    L = _L()
     lib = L.load()
-    gp, m = _gp('tank')
+    gp, m = fixture_gp('tank')
     eng = gp.engine
     Nx, Ny = 6, 4
     z0 = np.zeros((2, Nx)); U = np.zeros((2, 3, 2)); S = np.tile(np.eye(Nx) * 1e-3, (2, 1, 1))
@@ -183,9 +159,8 @@ def test_argument_checks():
 def test_default_methods_run_em_on_the_host_and_ta_me_on_the_device():
     """GP.rollout(feedback=True) with the reference's default methods ['EM', 'TA', 'ME']: 'EM' takes the host loop, 'TA' and
     'ME' the batched entry, and the result equals the all-host loop ('EM' bit for bit)."""
-    L = _L()
-    gp, m = _gp('tank')
-    X0, U, x_ref = _case('tank', 2, 5)
+    gp, m = fixture_gp('tank')
+    X0, U, x_ref = trajectories('tank', 2, 5, cyclic=True)
     eng = gp.engine
     calls = []
     real = eng.rollout_batch

@@ -8,10 +8,8 @@ import numpy as np
 import pytest
 
 import gp_mpc_b200
-from tests._fake_engine import OracleEngineWithRollout
-from tests._util import load_fixture, load_golden, relinf
-from tests.test_rollout_feedback_cpu import OracleEngineWithRolloutBatch
-from tests.test_sample_rollout_cpu import _TwoRanks
+from tests._fake_engine import OracleEngineWithRollout, OracleEngineWithRolloutBatch, TwoRanks, fixture_gp, sharded
+from tests._util import relinf, trajectories
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -27,9 +25,7 @@ class RecordingEmEngine(OracleEngineWithRolloutBatch):
         return self.rollout_batch(z0, U, Sigma0, 2, scale, K, x_ref, uscale)
 
 
-class _ShardEngine(RecordingEmEngine):
-    def comm_init(self, uid, rank, world):
-        self.rank, self.world = rank, world
+_ShardEngine = sharded(RecordingEmEngine)
 
 
 @pytest.fixture(autouse=True)
@@ -39,22 +35,11 @@ def _calls():
 
 
 def _gp(name, factory=RecordingEmEngine, **extra):
-    m = load_fixture(name)
-    args = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'], hyper=dict(hyper=m['hyper']),
-                engine_factory=factory)
-    if m['normalize']:
-        args.update(meta=m['meta'], xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
-    args.update(extra)
-    return gp_mpc_b200.GP(m['X'], m['Y'], **args), m
+    return fixture_gp(name, factory, **extra)
 
 
 def _case(name, nb, Nt=5):
-    d = load_golden('derived', name)
-    x0 = np.asarray(d['x0'], dtype=np.float64)
-    u0 = np.asarray(d['u0'], dtype=np.float64)
-    X0 = np.stack([x0 * (1 + 0.05 * b) for b in range(nb)])
-    U = np.stack([np.tile(u0, (Nt, 1)) * (1 + 0.03 * np.arange(Nt)[:, None] + 0.02 * b) for b in range(nb)])
-    return X0, U, 0.9 * x0 + 0.1
+    return trajectories(name, nb, Nt, cyclic=False)
 
 
 def test_single_open_loop_trajectory_is_one_call_of_b_1(_calls):
@@ -109,7 +94,7 @@ def test_host_loop_models(_calls):
     pm.rollout(X0, U, methods=['EM'])
     old, _ = _gp('tank', OracleEngineWithRollout)
     old.rollout(X0, U, methods=['EM'])
-    sh, _ = _gp('tank', _ShardEngine, comm=_TwoRanks(), normalize=False, meta=None)
+    sh, _ = _gp('tank', _ShardEngine, comm=TwoRanks(), normalize=False, meta=None)
     with pytest.raises(NotImplementedError, match='needs all outputs on one GPU'):
         sh.rollout(X0, U, methods=['EM'])
     assert _calls == []

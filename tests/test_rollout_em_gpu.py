@@ -7,52 +7,26 @@ import ctypes
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle.rollout_oracle_ld import feedback_inputs64
-from tests._util import load_fixture, load_golden
-from tests.test_dispatch_gpu import _require
-from tests.test_em_shapes_gpu import EM_TOL, em_errors, em_terms, engine_factor, tma_on_device
+from tests._em_cases import EM_TOL, em_errors, em_terms, engine_factor, feedback_sigma, tma_on_device
+from tests._engines import require
+from tests._fake_engine import fixture_gp
+from tests._util import assert_same, trajectories
 
 pytestmark = pytest.mark.gpu
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _gp(name):
-    import gp_mpc_b200
-    m = load_fixture(name)
-    kw = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'], hyper=dict(hyper=m['hyper']))
-    if m['normalize']:
-        kw.update(meta=m['meta'], xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
-    return gp_mpc_b200.GP(m['X'], m['Y'], **kw), m
-
-
-def _case(name, nb, Nt):
-    d = load_golden('derived', name)
-    x0 = np.asarray(d['x0'], dtype=np.float64)
-    u0 = np.asarray(d['u0'], dtype=np.float64)
-    X0 = np.stack([x0 * (1 + 0.01 * (b % 23) - 0.004 * (b % 7)) for b in range(nb)])
-    U = np.stack([np.tile(u0, (Nt, 1)) * (1 + 0.03 * np.arange(Nt)[:, None] + 0.005 * (b % 11)) for b in range(nb)])
-    return X0, U, 0.9 * x0 + 0.1
-
-
-def _same(a, b):
-    for x, y in zip(a, b):
-        assert np.array_equal(x, y)
 
 
 @pytest.mark.parametrize('B', [1, 3, 65])
 @pytest.mark.parametrize('name', ['tank', 'car'])
 def test_open_loop_equals_the_host_loop_bit_for_bit(name, B):
     """B = 65 runs as one chunk; B = 1 also as the single trajectory x0:(Ny,), which GP.rollout sends as B = 1."""
-    gp, m = _gp(name)
-    X0, U, _ = _case(name, B, 4)
-    _same(gp.rollout(X0, U, methods=['EM']), gp.rollout(X0, U, methods=['EM'], device_rollout=False))
+    gp, m = fixture_gp(name)
+    X0, U, _ = trajectories(name, B, 4, cyclic=True)
+    assert_same(gp.rollout(X0, U, methods=['EM']), gp.rollout(X0, U, methods=['EM'], device_rollout=False))
     if B == 1:
-        _same(gp.rollout(X0[0], U[0], methods=['EM']), gp.rollout(X0[0], U[0], methods=['EM'], device_rollout=False))
+        assert_same(gp.rollout(X0[0], U[0], methods=['EM']), gp.rollout(X0[0], U[0], methods=['EM'], device_rollout=False))
     gp.close()
 
 
@@ -60,12 +34,12 @@ def test_open_loop_equals_the_host_loop_bit_for_bit(name, B):
 @pytest.mark.parametrize('name', ['tank', 'car'])
 def test_feedback_equals_the_host_loop_bit_for_bit(name, B):
     """A gain per trajectory (one engine pass each), and one gain shared by all (a single pass of B trajectories)."""
-    gp, m = _gp(name)
-    X0, U, x_ref = _case(name, B, 6)
+    gp, m = fixture_gp(name)
+    X0, U, x_ref = trajectories(name, B, 6, cyclic=True)
     kw = dict(methods=['EM'], feedback=True, x_ref=x_ref)
-    _same(gp.rollout(X0, U, **kw), gp.rollout(X0, U, device_rollout=False, **kw))
+    assert_same(gp.rollout(X0, U, **kw), gp.rollout(X0, U, device_rollout=False, **kw))
     X0[:] = X0[0]; U[:, 0] = U[0, 0]                       # one linearisation point: one gain
-    _same(gp.rollout(X0, U, **kw), gp.rollout(X0, U, device_rollout=False, **kw))
+    assert_same(gp.rollout(X0, U, **kw), gp.rollout(X0, U, device_rollout=False, **kw))
     gp.close()
 
 
@@ -79,7 +53,7 @@ def test_autonomous_system_equals_the_host_loop():
     gp = gp_mpc_b200.GP(X, Y, normalize=False, gp_method='EM', hyper=dict(hyper=hyper))
     X0 = np.array([[1.0, 0.5], [-0.5, 1.5], [0.2, -1.0]])
     rm, rv = gp.rollout(X0, np.zeros((3, 12, 0)), methods=['EM'])
-    _same((rm, rv), gp.rollout(X0, np.zeros((3, 12, 0)), methods=['EM'], device_rollout=False))
+    assert_same((rm, rv), gp.rollout(X0, np.zeros((3, 12, 0)), methods=['EM'], device_rollout=False))
     assert rm.shape == (1, 3, 13, 2) and (rv[0, :, 1:] > 0).all()
     gp.close()
 
@@ -87,8 +61,7 @@ def test_autonomous_system_equals_the_host_loop():
 def test_predict_em_points_do_not_depend_on_the_chunk():
     """gpmpc_predict(EM) at H = 7 equals seven H = 1 calls with the em_points cap at 1, 3 and unlimited; the same for
     gpmpc_predict_em_grad at H = 5."""
-    L = _L()
-    gp, m = _gp('car')
+    gp, m = fixture_gp('car')
     eng = gp.engine
     rng = np.random.default_rng(3)
     Nx = m['X'].shape[1]
@@ -112,8 +85,8 @@ def test_predict_em_points_do_not_depend_on_the_chunk():
 
 def _engine_case(name, B, Nt, feedback):
     """The fixture's engine and the engine-unit inputs of a roll-out: z0, U, Sigma0, scale and the policy."""
-    gp, m = _gp(name)
-    X0, U, x_ref = _case(name, B, Nt)
+    gp, m = fixture_gp(name)
+    X0, U, x_ref = trajectories(name, B, Nt, cyclic=True)
     Ny, Nu = X0.shape[1], U.shape[2]
     st = m.get('meta')
     scale = np.stack([st['stdY'], st['meanY'], st['meanX'], st['stdX']]) if m['normalize'] else None
@@ -136,34 +109,16 @@ def test_rollout_does_not_depend_on_b_chunk_or_row_and_a_prefix_is_a_prefix(name
     full = eng.rollout_batch_em(z0, U, S, **pol)
     for cap in (1, 3):
         eng.set_option('em_points', cap)
-        _same(full, eng.rollout_batch_em(z0, U, S, **pol))
+        assert_same(full, eng.rollout_batch_em(z0, U, S, **pol))
     eng.set_option('em_points', 0)
     for b in (0, 3):
         one = eng.rollout_batch_em(z0[b:b + 1], U[b:b + 1], S[b:b + 1], **pol)
-        _same([x[b] for x in full], [x[0] for x in one])
+        assert_same([x[b] for x in full], [x[0] for x in one])
     rev = eng.rollout_batch_em(z0[::-1].copy(), U[::-1].copy(), S[::-1].copy(), **pol)
-    _same([x[::-1] for x in rev], full)
+    assert_same([x[::-1] for x in rev], full)
     prefix = eng.rollout_batch_em(z0, U[:, :3], S, **pol)
-    _same((prefix[0], prefix[1]), (full[0][:, :3], full[1][:, :3]))
+    assert_same((prefix[0], prefix[1]), (full[0][:, :3], full[1][:, :3]))
     gp.close()
-
-
-def _feedback_sigma(S0, cov, K):
-    """rollout_feedback_kernel's next Sigma from cov (Ny, Ny): sums in index order, no fused multiply-add."""
-    Ny = cov.shape[0]
-    S = S0.copy()
-    S[:Ny, :Ny] = cov
-    if K is None:
-        return S
-    Nu = K.shape[0]
-    KC = np.zeros((Nu, Ny)); CK = np.zeros((Ny, Nu)); KCK = np.zeros((Nu, Nu))
-    for k in range(Ny):
-        KC = KC + K[:, k][:, None] * cov[k][None, :]
-        CK = CK + cov[:, k][:, None] * K[:, k][None, :]
-    for k in range(Ny):
-        KCK = KCK + KC[:, k][:, None] * K[:, k][None, :]
-    S[:Ny, Ny:] = CK; S[Ny:, :Ny] = CK.T; S[Ny:, Ny:] = KCK
-    return S
 
 
 # name -> (N, Nx, Ny): 17 pair tiles against 18 trace tiles; Npad 3072 puts the trace product on the TMA feed
@@ -178,7 +133,7 @@ def test_every_step_against_long_double(name, feedback):
     single-step and keeps test_em_shapes_gpu's bar (errors over the sums of |terms|)."""
     import gp_mpc_b200
     if name == 'tma':
-        _require(tma_on_device(), 'the TMA feed')
+        require(tma_on_device(), 'the TMA feed')
     N, Nx, Ny = LD_CASES[name]
     Nu, B, Nt = Nx - Ny, 2, 3
     p = orc.synthetic_problem(N, Nx, Ny, config_id=700 + Nx, H=B)
@@ -200,8 +155,8 @@ def test_every_step_against_long_double(name, feedback):
     for t in range(Nt):
         z = z0 if t == 0 else feedback_inputs64(means[:, t - 1], None, K, pol['x_ref'], None, U[:, t])
         for b in range(B):
-            S = S0[b] if t == 0 else _feedback_sigma(S0[b], covs[t - 1][b], K)
-            one = eng.predict(z[b:b + 1], S, _L().METHOD_EM, want_jac=False)
+            S = S0[b] if t == 0 else feedback_sigma(S0[b], covs[t - 1][b], K)
+            one = eng.predict(z[b:b + 1], S, L.METHOD_EM, want_jac=False)
             assert np.array_equal(one[0][0], means[b, t])          # the engine's step is its predict at these inputs
             ref = orc.gp_exact_moment(kinv, p['X'], p['Y'], hyper, z[b], S, extended=True, beta=alpha)
             e = em_errors(one[0][0], one[2][0], ref, em_terms(p['X'], hyper, alpha, kinv, z[b], S))
@@ -212,7 +167,6 @@ def test_every_step_against_long_double(name, feedback):
 
 def test_error_codes():
     import gp_mpc_b200
-    L = _L()
     lib = L.load()
     p = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
     # Ny = 45 (every model with Nu >= 0 has Ny <= Nx <= 32)
@@ -223,7 +177,7 @@ def test_error_codes():
         e1.rollout_batch_em(np.zeros((1, 3)), np.zeros((1, 2, 0)), np.eye(3)[None] * 1e-3)
     assert e.value.code == L.ERR_ARG
     e1.close()
-    gp, m = _gp('tank')
+    gp, m = fixture_gp('tank')
     eng = gp.engine
     Nx, Ny = 6, 4
     z0 = np.zeros((2, Nx)); U = np.zeros((2, 3, 2)); S = np.tile(np.eye(Nx) * 1e-3, (2, 1, 1))
@@ -244,7 +198,7 @@ def test_error_codes():
     with pytest.raises(L.GpmpcError) as e:
         eng.rollout_batch_em(z0, U, bad)
     assert e.value.code == L.ERR_ARG and 'step 0' in str(e.value)
-    _same(before, eng.predict(Z, S[0], L.METHOD_EM, want_jac=False))
+    assert_same(before, eng.predict(Z, S[0], L.METHOD_EM, want_jac=False))
     gp.close()
     # a handle that owns only some outputs
     e3 = gp_mpc_b200.Engine(m['X'].shape[0], Nx, Ny, out_begin=0, out_count=2, device=0)

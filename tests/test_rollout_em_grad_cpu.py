@@ -13,9 +13,9 @@ from gp_mpc_b200.gp_class import _matmul_seq
 from oracle import em_grad_oracle, rollout_oracle
 from oracle import gp_oracle as orc
 from oracle.rollout_oracle import predict_compare_loop
+from tests._fake_engine import OracleEngineWithRolloutBatch, fixture_gp
 from tests._rollout_em_grad_oracle import rollout_em_grad
-from tests._util import load_fixture, load_golden, relinf
-from tests.test_rollout_feedback_cpu import OracleEngineWithRolloutBatch
+from tests._util import central, load_fixture, relinf, trajectories
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -77,12 +77,7 @@ class OracleEngineWithRolloutBatchEmGrad(OracleEngineWithRolloutBatch):
 
 
 def _gp(name):
-    m = load_fixture(name)
-    args = dict(mean_func='zero', gp_method='EM', normalize=m['normalize'], hyper=dict(hyper=m['hyper']),
-                engine_factory=OracleEngineWithRolloutBatchEmGrad)
-    if m['normalize']:
-        args.update(meta=m['meta'], xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
-    gp = gp_mpc_b200.GP(m['X'], m['Y'], **args)
+    gp, m = fixture_gp(name, OracleEngineWithRolloutBatchEmGrad, gp_method='EM')
     eng = gp.engine
     model = dict(X=eng.X, Y=eng.Y, hyper=m['hyper'], alpha=eng.post['alpha'], chol=eng.post['chol'],
                  invK=eng.post['invK'], normalize=m['normalize'], meta=m.get('meta'))     # the stand-in's own factor
@@ -90,32 +85,12 @@ def _gp(name):
 
 
 def _case(name, nb=1, Nt=5):
-    d = load_golden('derived', name)
-    x0 = np.asarray(d['x0'], dtype=np.float64)
-    u0 = np.asarray(d['u0'], dtype=np.float64)
-    X0 = np.stack([x0 * (1 + 0.05 * b) for b in range(nb)])
-    U = np.stack([np.tile(u0, (Nt, 1)) * (1 + 0.03 * np.arange(Nt)[:, None] + 0.02 * b) for b in range(nb)])
-    return X0, U, 0.9 * x0 + 0.1
+    return trajectories(name, nb, Nt, cyclic=False)
 
 
 def _gain(model, x0, u0):
     A, Bm = orc.discrete_linearize(model, x0, u0)
     return rollout_oracle.lqr_gain(A, Bm, np.eye(A.shape[0]), np.eye(Bm.shape[1]))[0]
-
-
-def _central(f, p, rel):
-    """Central differences of f (returning mean, var) at the parameter array p, one entry at a time."""
-    p = np.asarray(p, dtype=np.float64)
-    dm, dv = [], []
-    for j in np.ndindex(p.shape):
-        h = rel * max(1.0, abs(p[j]))
-        pp = p.copy(); pp[j] += h
-        pm = p.copy(); pm[j] -= h
-        (mp, vp), (mm, vm) = f(pp), f(pm)
-        dm.append((mp - mm) / (2 * h)); dv.append((vp - vm) / (2 * h))
-    sh = p.shape
-    return (np.moveaxis(np.array(dm), 0, -1).reshape(dm[0].shape + sh),
-            np.moveaxis(np.array(dv), 0, -1).reshape(dv[0].shape + sh))
 
 
 def _resolvable(name):
@@ -159,16 +134,16 @@ def test_oracle_equals_central_differences_of_predict_compare(name, feedback, mo
     assert np.array_equal(o['mean'], pm) and np.array_equal(o['var'], pv)        # the same arithmetic
     rel, tm, tv = _FD[name]
     worst = []
-    fm, fv = _central(lambda p: loop(p, u), x0, rel)
+    fm, fv = central(lambda p: loop(p, u), x0, rel)
     worst += [relinf(o['dmean_dx0'], fm), relinf(o['dvar_dx0'], fv)]
     if feedback:
         def with_gain(Kp):
             gain[0] = Kp
             return loop(x0, u)
-        fm, fv = _central(with_gain, K0, rel)
+        fm, fv = central(with_gain, K0, rel)
         worst += [relinf(o['dmean_dK'], fm), relinf(o['dvar_dK'], fv)]
     else:
-        fm, fv = _central(lambda p: loop(x0, p), u, rel)
+        fm, fv = central(lambda p: loop(x0, p), u, rel)
         worst += [relinf(o['dmean_du'], fm), relinf(o['dvar_du'], fv)]
     print('[fd] %s fb=%s %s' % (name, feedback, ['%.1e' % w for w in worst]))
     assert max(worst[0::2]) < tm and max(worst[1::2]) < tv, worst

@@ -7,18 +7,15 @@ import ctypes
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle.rollout_oracle_ld import feedback_inputs64
+from tests._em_cases import feedback_sigma
+from tests._engines import lqr_gain
 from tests._rollout_em_grad_oracle import rollout_em_grad
-from tests._util import load_fixture, load_golden, relinf
-from tests.test_rollout_em_gpu import _feedback_sigma
+from tests._util import assert_same, load_fixture, relinf, trajectories
 
 pytestmark = pytest.mark.gpu
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
 
 
 def _gp(name, sn_floor=None):
@@ -55,12 +52,7 @@ def _case(name, m, nb, Nt):
         X0 = rows[:, :Ny]
         U = np.repeat(rows[:, None, Ny:], Nt, 1) * (1 + 0.01 * np.arange(Nt)[None, :, None])
         return X0, U, 0.5 * X0[0]
-    d = load_golden('derived', name)
-    x0 = np.asarray(d['x0'], dtype=np.float64)
-    u0 = np.asarray(d['u0'], dtype=np.float64)
-    X0 = np.stack([x0 * (1 + 0.01 * (b % 23) - 0.004 * (b % 7)) for b in range(nb)])
-    U = np.stack([np.tile(u0, (Nt, 1)) * (1 + 0.03 * np.arange(Nt)[:, None] + 0.005 * (b % 11)) for b in range(nb)])
-    return X0, U, 0.9 * x0 + 0.1
+    return trajectories(name, nb, Nt, cyclic=True)
 
 
 def _inputs(m, X0, U, K=None, x_ref=None):
@@ -84,16 +76,6 @@ def _inputs(m, X0, U, K=None, x_ref=None):
     return np.concatenate([zx, un[:, 0, :Nu]], 1), (un if K is None else U), S, pol
 
 
-def _gain(gp, X0, U):
-    Ny, Nu = X0.shape[1], U.shape[2]
-    return gp._GP__lqr_gains(X0[:1], U[:1, 0], np.eye(Ny), np.eye(Nu))[0]
-
-
-def _same(a, b):
-    for x, y in zip(a, b):
-        assert np.array_equal(x, y)
-
-
 @pytest.mark.parametrize('B', [1, 3, 5])
 @pytest.mark.parametrize('name', ['tank', 'car', 'synthetic'])
 def test_rollout_is_rollout_batch_em_bit_for_bit(name, B):
@@ -105,12 +87,12 @@ def test_rollout_is_rollout_batch_em_bit_for_bit(name, B):
     X0, U, x_ref = _case(name, m, B, 4)
     Ny, Nx = X0.shape[1], m['X'].shape[1]
     Nu = Nx - Ny
-    K = _gain(gp, X0, U)
+    K = lqr_gain(gp, X0, U)
     for fb in (False, True):
         z0, Ug, S, pol = _inputs(m, X0, U, K if fb else None, x_ref)
         ref = eng.rollout_batch_em(z0, Ug, S, **pol)
         got = eng.rollout_batch_em_grad(z0, Ug, S, **pol)
-        _same(ref, got[:3])
+        assert_same(ref, got[:3])
         P = Nx + (Nu * Ny if fb else 3 * Nu)
         assert got[3].shape == got[4].shape == (B, 4, Ny, P)
         assert np.isfinite(got[3]).all() and np.isfinite(got[4]).all()
@@ -124,19 +106,19 @@ def test_one_trajectory_equals_its_row_and_calls_repeat(name):
     gp, m = _gp(name)
     eng = gp.engine
     X0, U, x_ref = _case(name, m, 5, 5)
-    K = _gain(gp, X0, U)
+    K = lqr_gain(gp, X0, U)
     for fb in (False, True):
         z0, Ug, S, pol = _inputs(m, X0, U, K if fb else None, x_ref)
         eng.set_option('em_points', 0)
         full = eng.rollout_batch_em_grad(z0, Ug, S, **pol)
-        _same(full, eng.rollout_batch_em_grad(z0, Ug, S, **pol))
+        assert_same(full, eng.rollout_batch_em_grad(z0, Ug, S, **pol))
         for cap in (1, 2):
             eng.set_option('em_points', cap)
-            _same(full, eng.rollout_batch_em_grad(z0, Ug, S, **pol))
+            assert_same(full, eng.rollout_batch_em_grad(z0, Ug, S, **pol))
         eng.set_option('em_points', 0)
         for b in (0, 3):
             one = eng.rollout_batch_em_grad(z0[b:b + 1], Ug[b:b + 1], S[b:b + 1], **pol)
-            _same([x[b] for x in full], [x[0] for x in one])
+            assert_same([x[b] for x in full], [x[0] for x in one])
     gp.close()
 
 
@@ -161,7 +143,7 @@ def _chain(eng, z0, U, S0, means, covs, scale=None, K=None, x_ref=None, uscale=N
             z, S = z0, S0
         else:
             z = feedback_inputs64(means[:, t - 1], scale, K, x_ref, uscale, U[:, t] if K is None else None)
-            S = np.stack([_feedback_sigma(S0[b], covs[t - 1][b], K) for b in range(B)])
+            S = np.stack([feedback_sigma(S0[b], covs[t - 1][b], K) for b in range(B)])
         g = eng.predict_em_grad(z, S)
         for b in range(B):
             dm = g['dmean_dz'][b] @ dz[b] + np.einsum('ade,dep->ap', g['dmean_dSigma'][b], dS[b])
@@ -199,7 +181,7 @@ def test_chain_on_the_engines_own_derivatives(name, fb):
     gp, m = _gp(name)
     eng = gp.engine
     X0, U, x_ref = _case(name, m, 3, 4)
-    K = _gain(gp, X0, U) if fb else None
+    K = lqr_gain(gp, X0, U) if fb else None
     z0, Ug, S, pol = _inputs(m, X0, U, K, x_ref)
     means, _, _, dm, dv = eng.rollout_batch_em_grad(z0, Ug, S, **pol)
     covs = [eng.rollout_batch_em(z0, Ug[:, :t], S, **pol)[2] for t in range(1, 4)]
@@ -226,7 +208,7 @@ def test_derivatives_equal_central_differences_on_the_device(name, fb):
     eng = gp.engine
     Nt = 6
     X0, U, x_ref = _case(name, m, 2, Nt)
-    K = _gain(gp, X0, U) if fb else None
+    K = lqr_gain(gp, X0, U) if fb else None
     z0, Ug, S, pol = _inputs(m, X0, U, K, x_ref)
     Ny, Nx = X0.shape[1], z0.shape[1]
     Nu = Nx - Ny
@@ -306,7 +288,7 @@ def test_autonomous_model_has_the_start_as_only_parameter():
     X0 = np.array([[1.0, 0.5], [-0.5, 1.5]])
     out = gp.engine.rollout_batch_em_grad(X0, np.zeros((2, 8, 0)), np.tile(np.eye(2) * 1e-3, (2, 1, 1)))
     assert out[3].shape == (2, 8, 2, 2)
-    _same(gp.engine.rollout_batch_em(X0, np.zeros((2, 8, 0)), np.tile(np.eye(2) * 1e-3, (2, 1, 1))), out[:3])
+    assert_same(gp.engine.rollout_batch_em(X0, np.zeros((2, 8, 0)), np.tile(np.eye(2) * 1e-3, (2, 1, 1))), out[:3])
     model = _model(dict(X=X, Y=Y, hyper=hyper, normalize=False))
     r = gp.rollout_grad(X0, np.zeros((2, 8, 0)), method='EM')
     assert r['dmean_du'].shape == (2, 9, 2, 8, 0)
@@ -321,7 +303,6 @@ def test_autonomous_model_has_the_start_as_only_parameter():
 
 def test_error_codes():
     import gp_mpc_b200
-    L = _L()
     lib = L.load()
     p = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
     gp, m = _gp('tank')
@@ -348,7 +329,7 @@ def test_error_codes():
     with pytest.raises(L.GpmpcError) as e:
         eng.rollout_batch_em_grad(z0, U, bad)
     assert e.value.code == L.ERR_ARG and 'step 0' in str(e.value) and 'trajectory 1' in str(e.value)
-    _same(good, eng.rollout_batch_em_grad(z0, U, S))
+    assert_same(good, eng.rollout_batch_em_grad(z0, U, S))
     # gpmpc_rollout_batch_grad keeps rejecting 'EM'
     assert lib.gpmpc_rollout_batch_grad(eng.h, L.METHOD_EM, 2, 3, p(z0), p(U), p(S), None, None, None, None, o, o, None,
                                         o, o) == L.ERR_ARG

@@ -8,69 +8,22 @@ import numpy as np
 import pytest
 
 import gp_mpc_b200
-from gp_mpc_b200.gp_class import _matmul_seq
 from oracle.rollout_oracle import predict_compare_loop
-from tests._fake_engine import OracleEngine, OracleEngineWithRollout
-from tests._util import load_fixture, load_golden, relinf
+from tests._fake_engine import OracleEngine, OracleEngineWithRolloutBatch, fixture_gp
+from tests._util import relinf, trajectories
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-class OracleEngineWithRolloutBatch(OracleEngineWithRollout):
-    """Adds a numpy restatement of gpmpc_rollout_batch (include/gpmpc.h): one predict step for all trajectories, then
-    rollout_feedback_kernel's update per trajectory."""
-
-    def rollout_batch(self, z0, U, Sigma0, method=1, scale=None, K=None, x_ref=None, uscale=None):
-        Ny, Nx = self.Ny, self.Nx
-        Nu = Nx - Ny
-        Z = np.array(z0, dtype=np.float64).reshape(-1, Nx)
-        B, Nt = Z.shape[0], np.shape(U)[1]
-        S = np.array(Sigma0, dtype=np.float64).reshape(B, Nx, Nx)
-        means = np.empty((B, Nt, Ny)); var = np.empty((B, Nt, Ny)); cov = None
-        for t in range(Nt):
-            # every trajectory's point on its own, as the device computes each point independently of the others
-            parts = [self.predict(Z[b:b + 1], S[b], method, True, False) for b in range(B)]
-            m = np.concatenate([p[0] for p in parts]); cov = np.concatenate([p[2] for p in parts])
-            means[:, t] = m
-            var[:, t] = np.diagonal(cov, axis1=1, axis2=2)
-            if t + 1 == Nt:
-                break
-            x = m if scale is None else m * scale[0] + scale[1]
-            Z[:, :Ny] = x if scale is None else (x - scale[2]) / scale[3]
-            for b in range(B):
-                if K is None:
-                    Z[b, Ny:] = U[b, t + 1]
-                else:
-                    ub = _matmul_seq(K, (x[b] - (0.0 if x_ref is None else x_ref))[:, None])[:, 0]
-                    Z[b, Ny:] = ub if uscale is None else (ub - uscale[0]) / uscale[1]
-                    cov_xu = _matmul_seq(cov[b], K.T)
-                    S[b, Ny:, Ny:] = _matmul_seq(_matmul_seq(K, cov[b]), K.T)
-                    S[b, Ny:, :Ny] = cov_xu.T
-                    S[b, :Ny, Ny:] = cov_xu
-                S[b, :Ny, :Ny] = cov[b]
-        return means, var, cov
-
-
 def _gp(name, factory=OracleEngine):
-    m = load_fixture(name)
-    args = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'], hyper=dict(hyper=m['hyper']),
-                engine_factory=factory)
-    if m['normalize']:
-        args.update(meta=m['meta'], xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
-    gp = gp_mpc_b200.GP(m['X'], m['Y'], **args)
+    gp, m = fixture_gp(name, factory)
     model = dict(X=m['X'], Y=m['Y'], hyper=m['hyper'], alpha=gp.get_alpha(), chol=gp.get_chol(),
                  normalize=m['normalize'], meta=m.get('meta'))          # the stand-in engine's own factor
     return gp, model
 
 
 def _case(name, nb=1, Nt=8):
-    d = load_golden('derived', name)
-    x0 = np.asarray(d['x0'], dtype=np.float64)
-    u0 = np.asarray(d['u0'], dtype=np.float64)
-    X0 = np.stack([x0 * (1 + 0.05 * b) for b in range(nb)])
-    U = np.stack([np.tile(u0, (Nt, 1)) * (1 + 0.03 * np.arange(Nt)[:, None] + 0.02 * b) for b in range(nb)])
-    x_ref = 0.9 * x0 + 0.1
-    return X0, U, x_ref
+    return trajectories(name, nb, Nt, cyclic=False)
 
 
 @pytest.mark.parametrize('name', ['tank', 'car'])

@@ -12,10 +12,8 @@ from gp_mpc_b200.gp_class import _matmul_seq
 from oracle import hess_oracle, rollout_oracle
 from oracle.rollout_grad_oracle import rollout_grad
 from oracle.rollout_oracle import predict_compare_loop
-from tests._fake_engine import OracleEngine
-from tests._util import load_fixture, load_golden, relinf
-from tests.test_rollout_feedback_cpu import OracleEngineWithRolloutBatch
-from tests.test_sample_rollout_cpu import _TwoRanks
+from tests._fake_engine import OracleEngine, OracleEngineWithRolloutBatch, TwoRanks, fixture_gp, sharded
+from tests._util import central, load_fixture, relinf, trajectories
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -80,44 +78,19 @@ class OracleEngineWithRolloutBatchGrad(OracleEngineWithRolloutBatch):
 
 
 def _gp(name, factory=OracleEngineWithRolloutBatchGrad):
-    m = load_fixture(name)
-    args = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'], hyper=dict(hyper=m['hyper']),
-                engine_factory=factory)
-    if m['normalize']:
-        args.update(meta=m['meta'], xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
-    gp = gp_mpc_b200.GP(m['X'], m['Y'], **args)
+    gp, m = fixture_gp(name, factory)
     model = dict(X=m['X'], Y=m['Y'], hyper=m['hyper'], alpha=gp.get_alpha(), chol=gp.get_chol(),
                  normalize=m['normalize'], meta=m.get('meta'))          # the stand-in engine's own factor
     return gp, model
 
 
 def _case(name, nb=1, Nt=6):
-    d = load_golden('derived', name)
-    x0 = np.asarray(d['x0'], dtype=np.float64)
-    u0 = np.asarray(d['u0'], dtype=np.float64)
-    X0 = np.stack([x0 * (1 + 0.05 * b) for b in range(nb)])
-    U = np.stack([np.tile(u0, (Nt, 1)) * (1 + 0.03 * np.arange(Nt)[:, None] + 0.02 * b) for b in range(nb)])
-    return X0, U, 0.9 * x0 + 0.1
+    return trajectories(name, nb, Nt, cyclic=False)
 
 
 def _gain(model, x0, u0):
     A, Bm = rollout_oracle.orc.discrete_linearize(model, x0, u0)
     return rollout_oracle.lqr_gain(A, Bm, np.eye(A.shape[0]), np.eye(Bm.shape[1]))[0]
-
-
-def _central(f, p, rel):
-    """Central differences of f (returning mean, var) at the parameter array p, one entry at a time."""
-    p = np.asarray(p, dtype=np.float64)
-    dm, dv = [], []
-    for j in np.ndindex(p.shape):
-        h = rel * max(1.0, abs(p[j]))
-        pp = p.copy(); pp[j] += h
-        pm = p.copy(); pm[j] -= h
-        (mp, vp), (mm, vm) = f(pp), f(pm)
-        dm.append((mp - mm) / (2 * h)); dv.append((vp - vm) / (2 * h))
-    sh = p.shape
-    return (np.moveaxis(np.array(dm), 0, -1).reshape(dm[0].shape + sh),
-            np.moveaxis(np.array(dv), 0, -1).reshape(dv[0].shape + sh))
 
 
 # (relative step, tolerance on the mean blocks, on the variance blocks), from the agreement measured with the oracle
@@ -148,16 +121,16 @@ def test_oracle_equals_central_differences_of_predict_compare(name, method, feed
     pm, pv = loop(x0, u)
     assert relinf(o['mean'], pm) < 1e-12 and relinf(o['var'], pv) < 1e-10       # J: another summation order than gp_mean_jac
     rel, tm, tv = _FD[name]
-    fm, fv = _central(lambda p: loop(p, u), x0, rel)
+    fm, fv = central(lambda p: loop(p, u), x0, rel)
     assert relinf(o['dmean_dx0'], fm) < tm and relinf(o['dvar_dx0'], fv) < tv
     if feedback:
         def with_gain(Kp):
             gain[0] = Kp
             return loop(x0, u)
-        fm, fv = _central(with_gain, K0, rel)
+        fm, fv = central(with_gain, K0, rel)
         assert relinf(o['dmean_dK'], fm) < tm and relinf(o['dvar_dK'], fv) < tv
     else:
-        fm, fv = _central(lambda p: loop(x0, p), u, rel)
+        fm, fv = central(lambda p: loop(x0, p), u, rel)
         assert relinf(o['dmean_du'], fm) < tm and relinf(o['dvar_du'], fv) < tv
     assert np.abs(o['dvar_dx0']).max() > 0                     # the variance really depends on the start
 
@@ -209,9 +182,7 @@ def test_default_method_and_autonomous_model():
     assert relinf(a['dmean_dx0'], o['dmean_dx0']) < 1e-10 and relinf(a['dvar_dx0'], o['dvar_dx0']) < 1e-10
 
 
-class _ShardEngine(OracleEngineWithRolloutBatchGrad):
-    def comm_init(self, uid, rank, world):
-        self.rank, self.world = rank, world
+_ShardEngine = sharded(OracleEngineWithRolloutBatchGrad)
 
 
 def test_not_implemented_cases():
@@ -222,7 +193,7 @@ def test_not_implemented_cases():
     with pytest.raises(ValueError):
         gp.rollout_grad(X0[0], np.zeros((0, 2)))
     fm = load_fixture('tank')
-    sh = gp_mpc_b200.GP(fm['X'], fm['Y'], normalize=False, hyper=dict(hyper=fm['hyper']), comm=_TwoRanks(),
+    sh = gp_mpc_b200.GP(fm['X'], fm['Y'], normalize=False, hyper=dict(hyper=fm['hyper']), comm=TwoRanks(),
                         engine_factory=_ShardEngine)
     with pytest.raises(NotImplementedError, match='needs all outputs on one GPU'):
         sh.rollout_grad(X0[0], U[0])

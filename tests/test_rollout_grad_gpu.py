@@ -6,16 +6,14 @@ import ctypes
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle.rollout_grad_oracle import rollout_grad
-from tests._util import load_fixture, load_golden, relinf
+from tests._engines import lqr_gain
+from tests._fake_engine import fixture_gp
+from tests._util import relinf, trajectories
 
 pytestmark = pytest.mark.gpu
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
 
 
 def _gp(name):
@@ -28,11 +26,7 @@ def _gp(name):
         m = dict(X=w['X'], Y=w['Y'], hyper=w['hyper'], normalize=False, Z=w['Z'])
         gp = gp_mpc_b200.GP(w['X'], w['Y'], normalize=False, hyper=dict(hyper=w['hyper']))
     else:
-        m = load_fixture(name)
-        kw = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'], hyper=dict(hyper=m['hyper']))
-        if m['normalize']:
-            kw.update(meta=m['meta'], xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
-        gp = gp_mpc_b200.GP(m['X'], m['Y'], **kw)
+        gp, m = fixture_gp(name)
     return gp, m
 
 
@@ -49,12 +43,7 @@ def _case(name, m, nb, Nt):
         X0 = rows[:, :Ny] * (1 + 0.002 * (np.arange(nb) // m['Z'].shape[0]))[:, None]
         U = np.repeat(rows[:, None, Ny:], Nt, 1) * (1 + 0.01 * np.arange(Nt)[None, :, None])
         return X0, U, 0.5 * X0[0]
-    d = load_golden('derived', name)
-    x0 = np.asarray(d['x0'], dtype=np.float64)
-    u0 = np.asarray(d['u0'], dtype=np.float64)
-    X0 = np.stack([x0 * (1 + 0.01 * (b % 23) - 0.004 * (b % 7)) for b in range(nb)])
-    U = np.stack([np.tile(u0, (Nt, 1)) * (1 + 0.03 * np.arange(Nt)[:, None] + 0.005 * (b % 11)) for b in range(nb)])
-    return X0, U, 0.9 * x0 + 0.1
+    return trajectories(name, nb, Nt, cyclic=True)
 
 
 def _inputs(gp, m, X0, U, K=None, x_ref=None):
@@ -75,23 +64,17 @@ def _inputs(gp, m, X0, U, K=None, x_ref=None):
     return np.concatenate([zx, un[:, 0, :Nu]], 1), (un if K is None else U), S, scale, uscale
 
 
-def _gain(gp, X0, U):
-    Ny, Nu = X0.shape[1], U.shape[2]
-    return gp._GP__lqr_gains(X0[:1], U[:1, 0], np.eye(Ny), np.eye(Nu))[0]
-
-
 @pytest.mark.parametrize('B', [1, 3, 64, 65, 130])
 @pytest.mark.parametrize('name', ['tank', 'car', 'synthetic'])
 def test_rollout_is_rollout_batch_bit_for_bit(name, B):
     """means, vars, cov_last equal gpmpc_rollout_batch's for 'TA' and 'ME', open loop and with feedback, across the 64-point
     chunks of the predict pass; the derivatives are finite and have the documented shape."""
-    L = _L()
     gp, m = _gp(name)
     eng = gp.engine
     X0, U, x_ref = _case(name, m, B, 4)
     Ny, Nx = X0.shape[1], m['X'].shape[1]
     Nu = Nx - Ny
-    K = _gain(gp, X0, U)
+    K = lqr_gain(gp, X0, U)
     for meth in (L.METHOD_TA, L.METHOD_ME):
         for fb in (False, True):
             z0, Ug, S, scale, uscale = _inputs(gp, m, X0, U, K if fb else None, x_ref)
@@ -110,11 +93,10 @@ def test_rollout_is_rollout_batch_bit_for_bit(name, B):
 def test_one_trajectory_equals_its_row_and_calls_repeat(name):
     """Trajectory b alone equals row b of a batch bit for bit (every sum in a fixed order, one CTA per trajectory), and two
     identical calls give identical bits."""
-    L = _L()
     gp, m = _gp(name)
     eng = gp.engine
     X0, U, x_ref = _case(name, m, 5, 6)
-    K = _gain(gp, X0, U)
+    K = lqr_gain(gp, X0, U)
     for meth in (L.METHOD_TA, L.METHOD_ME):
         for fb in (False, True):
             z0, Ug, S, scale, uscale = _inputs(gp, m, X0, U, K if fb else None, x_ref)
@@ -141,7 +123,6 @@ _FD_TOL = dict(mean=2e-6, var=4e-4)
 def test_derivatives_equal_central_differences_on_the_device(name, meth):
     """Open loop, Nt = 8: dmeans / dvars against central differences of gpmpc_rollout_batch on the same device in every
     parameter (z0, then U rows 1..Nt-1); no CPU factor is involved."""
-    L = _L()
     gp, m = _gp(name)
     eng = gp.engine
     method = L.METHOD_TA if meth == 'TA' else L.METHOD_ME
@@ -227,7 +208,6 @@ def test_autonomous_model_has_the_start_as_only_parameter():
 
 def test_error_codes_leave_the_model_unchanged():
     import gp_mpc_b200
-    L = _L()
     lib = L.load()
     gp, m = _gp('tank')
     eng = gp.engine

@@ -25,8 +25,10 @@ variances sit at rounding level near DELTA sf2 (a closed loop of 12 steps left 4
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle.rollout_oracle_ld import DS_BLOCKS, LD, MARGIN, SIGMA_BLOCKS, rollout_ld, sample_ld
+from tests._util import normalised
 
 pytestmark = pytest.mark.gpu
 
@@ -66,15 +68,9 @@ TOL = dict(mean=8e-16, var=6e-17, cov_last=6e-17, dmean=2e-15, dvar=2e-16, sampl
 GUARD = 1e4
 
 
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
 def _problem(N, Nx, Ny, Nu, B, Nt, opts, seed):
     """Engine (factorised), X, hyper, alpha, L^-1 (long double) and the roll-out arguments of one case."""
     import gp_mpc_b200
-    L = _L()
     p = orc.synthetic_problem(N, Nx, Ny, config_id=900 + Nx + Ny, H=1)
     p['hyper'][:, Nx + 1] = 0.1                      # variances well above sn^2 = 1e-4, so their derivatives pass the guards
     eng = gp_mpc_b200.Engine(N, Nx, Ny, device=0)
@@ -100,13 +96,6 @@ def _problem(N, Nx, Ny, Nu, B, Nt, opts, seed):
         if 'xref' in opts:
             arg['x_ref'] = 0.2 * rng.standard_normal(Ny)
     return eng, p['X'], p['hyper'], alpha, linv, z0, U, S0, arg
-
-
-def normalised(x, ref, scale):
-    """Largest |x - ref| / scale over the entries; entries whose sum of |terms| is 0 must be exactly 0 on both sides."""
-    d = np.abs(np.asarray(x, dtype=LD) - ref)
-    assert not np.any(d[scale == 0]), 'a nonzero entry where the sum of |terms| is 0'
-    return float(np.max(np.divide(d, scale, out=np.zeros_like(d), where=scale > 0), initial=0.0))
 
 
 def _ratio(part, scale):
@@ -148,7 +137,6 @@ def case_errors(name):
     guards (their smallest ratios under 'guards').  Asserts that gpmpc_rollout_batch gives the same means, vars and
     cov_last bits and that trajectories run alone give their rows' bits."""
     N, Nx, Ny, Nu, B, Nt, opts = CASES[name]
-    L = _L()
     eng, X, hyper, alpha, linv, z0, U, S0, arg = _problem(N, Nx, Ny, Nu, B, Nt, opts, 0)
     res = dict(guards={})
     for fb in ((False, True) if Nu else (False,)):

@@ -10,7 +10,7 @@ import pytest
 import gp_mpc_b200
 from oracle import gp_oracle as orc
 from oracle import sample_oracle as so
-from tests._fake_engine import OracleEngine
+from tests._fake_engine import OracleEngine, TwoRanks, sample_model, sharded
 from tests._util import load_fixture, load_golden, relinf
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -28,16 +28,8 @@ class OracleEngineWithSample(OracleEngine):
         return so.rollout_sample(model, Linv, z0, U, np.asarray(eps), xi, scale, K, x_ref, uscale)
 
 
-def _model(name):
-    if name == 'synthetic':
-        p = orc.synthetic_problem(150, 5, 3, config_id=2)
-        p['hyper'][:, :5] = 1.5
-        return dict(X=p['X'], Y=p['Y'], hyper=p['hyper'], normalize=False)
-    return load_fixture(name)
-
-
 def _gp(name, factory=OracleEngineWithSample, **kw):
-    m = _model(name)
+    m = sample_model(name)
     args = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'], hyper=dict(hyper=m['hyper']),
                 engine_factory=factory)
     if m['normalize']:
@@ -57,7 +49,7 @@ def _path(m, T, rng):
 
 @pytest.mark.parametrize('name', ['tank', 'car', 'synthetic'])
 def test_sequential_conditioning_is_the_joint_cholesky_draw(name):
-    m = _model(name)
+    m = sample_model(name)
     post = orc.postfit(m['X'], m['Y'], m['hyper'], lapack_general_solve=False)
     rng = np.random.default_rng(3)
     Z = _path(m, 12, rng)
@@ -194,23 +186,7 @@ def test_feedback_runs_one_pass_per_distinct_gain():
     assert relinf(z_out[:, 1:, 4:], (u_app - st['meanU']) / st['stdU']) < 1e-12
 
 
-class _TwoRanks:
-    """A two-rank communicator stand-in: enough for a GP sharded by output to be built on one process."""
-    rank, world = 0, 2
-
-    def broadcast_object(self, obj, src=0):
-        return obj
-
-    def allgather_object(self, obj):
-        return [obj, obj]
-
-    def barrier(self):
-        pass
-
-
-class _ShardEngine(OracleEngineWithSample):
-    def comm_init(self, uid, rank, world):
-        self.rank, self.world = rank, world
+_ShardEngine = sharded(OracleEngineWithSample)
 
 
 def test_argument_errors():
@@ -230,7 +206,7 @@ def test_argument_errors():
         auto.sample_rollout(np.zeros(2), np.zeros((3, 0)), 2, feedback=True)
     assert auto.sample_rollout(np.zeros(2), np.zeros((3, 0)), 2, seed=0).shape == (2, 4, 2)
     # sharded by output over two ranks
-    sh = gp_mpc_b200.GP(m['X'], m['Y'], normalize=False, hyper=dict(hyper=m['hyper']), comm=_TwoRanks(),
+    sh = gp_mpc_b200.GP(m['X'], m['Y'], normalize=False, hyper=dict(hyper=m['hyper']), comm=TwoRanks(),
                         engine_factory=_ShardEngine)
     with pytest.raises(NotImplementedError, match='needs all outputs on one GPU'):
         sh.sample_rollout(x0, U, 2)

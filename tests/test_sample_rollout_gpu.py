@@ -6,8 +6,10 @@ import numpy as np
 import pytest
 import scipy.linalg
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle import sample_oracle as so
+from tests._engines import sample_engine
 from tests._util import load_fixture, load_golden, relinf
 
 pytestmark = pytest.mark.gpu
@@ -15,25 +17,6 @@ pytestmark = pytest.mark.gpu
 # |f - m - R eps| / sqrt(sf2) over the kept points (DESIGN 4.12): tank's slow dynamics visit strongly correlated points,
 # so R has small pivots and its inverse amplifies the last-bit differences between the host's and the device's covariances
 TOL = {'synthetic': 1e-8, 'tank': 1e-6}
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _engine(name):
-    """(engine, model dict) for a fixture or the synthetic problems."""
-    import gp_mpc_b200
-    if name == 'synthetic':                              # N = 1000, Nx = 8, Ny = 6 (Nu = 2)
-        p = orc.synthetic_problem(1000, 8, 6, config_id=4)
-        m = dict(X=p['X'], Y=p['Y'], hyper=p['hyper'], normalize=False)
-    else:
-        m = load_fixture(name)
-    N, Nx = m['X'].shape
-    eng = gp_mpc_b200.Engine(N, Nx, m['Y'].shape[1], device=0)
-    eng.set_data(m['X'], m['Y']); eng.set_hyper(m['hyper']); eng.factorize()
-    return eng, m
 
 
 def _inputs(m, B, Nt, seed):
@@ -50,7 +33,6 @@ def _joint_error(eng, m, samples, z_out, kept, eps, Linv=None, alpha=None):
     """max over (b, a) of |f - m - R eps| / sqrt(sf2) over the kept points, V and m from the given factor (default: the
     engine's own L^-1 and alpha)."""
     Nx, Ny = m['X'].shape[1], m['Y'].shape[1]
-    L = _L()
     Linv = [eng.get(L.GET_LINV, a) for a in range(Ny)] if Linv is None else Linv
     alpha = [eng.get(L.GET_ALPHA, a) for a in range(Ny)] if alpha is None else alpha
     err = 0.0
@@ -65,8 +47,7 @@ def _joint_error(eng, m, samples, z_out, kept, eps, Linv=None, alpha=None):
 
 @pytest.mark.parametrize('name', ['tank', 'car', 'synthetic'])
 def test_step_one_is_the_predicted_mean_plus_sqrt_var_eps(name):
-    L = _L()
-    eng, m = _engine(name)
+    eng, m = sample_engine(name)
     B = 70
     z0, U, _ = _inputs(m, B, 1, 1)
     Ny = m['Y'].shape[1]
@@ -83,7 +64,7 @@ def test_step_one_is_the_predicted_mean_plus_sqrt_var_eps(name):
 def test_teacher_forced_joint_identity(name, B):
     """f - m = R eps over every trajectory's kept points, R = chol of the joint posterior covariance of its visited
     inputs formed on the host from the engine's own L^-1."""
-    eng, m = _engine(name)
+    eng, m = sample_engine(name)
     z0, U, eps = _inputs(m, B, 12, B)
     samples, z_out, kept = eng.rollout_sample(z0, U, eps)
     assert np.isfinite(samples).all() and kept[:, 0].all()
@@ -94,7 +75,7 @@ def test_teacher_forced_joint_identity(name, B):
 @pytest.mark.parametrize('name', ['tank', 'car'])
 def test_joint_identity_against_a_lapack_factor(name):
     """The same identity with V and m from an independent LAPACK factor.  car: cond(K) ~ 1e10 (DESIGN 4.12)."""
-    eng, m = _engine(name)
+    eng, m = sample_engine(name)
     Ny = m['Y'].shape[1]
     z0, U, eps = _inputs(m, 16, 12, 7)
     samples, z_out, kept = eng.rollout_sample(z0, U, eps)
@@ -127,7 +108,7 @@ def test_degenerate_path_of_a_contractive_model():
 
 
 def test_bit_identical_alone_in_a_batch_and_on_repeat():
-    eng, m = _engine('synthetic')
+    eng, m = sample_engine('synthetic')
     z0, U, eps = _inputs(m, 130, 6, 3)
     full = eng.rollout_sample(z0, U, eps)
     again = eng.rollout_sample(z0, U, eps)
@@ -143,7 +124,6 @@ def test_bit_identical_alone_in_a_batch_and_on_repeat():
 def test_feedback_applies_the_gain_to_each_sampled_state():
     """u_t = K (x_t - x_ref), standardised, where x_t is the sampled state: recomputed on the host."""
     import gp_mpc_b200
-    L = _L()
     m = load_fixture('tank')
     kw = dict(mean_func='zero', gp_method='TA', normalize=True, hyper=dict(hyper=m['hyper']), meta=m['meta'],
               xlb=m['xlb'], xub=m['xub'], ulb=m['ulb'], uub=m['uub'])
@@ -170,14 +150,12 @@ def test_feedback_applies_the_gain_to_each_sampled_state():
     s2 = gp.engine.rollout_sample(z0, np.zeros((B, Nt, 2)), np.zeros((B, Nt, 4)), None, scale, 2 * K, x_ref, uscale)[0]
     s1 = gp.engine.rollout_sample(z0, np.zeros((B, Nt, 2)), np.zeros((B, Nt, 4)), None, scale, K, x_ref, uscale)[0]
     assert relinf(s1, s2) > 1e-6
-    del L
     gp.close()
 
 
 def test_step_one_statistics_match_exact_moment_matching():
     """8192 draws from N(z0, Sigma0): the sample mean and covariance of step 1 lie within 5 standard errors of 'EM'."""
-    L = _L()
-    eng, m = _engine('tank')
+    eng, m = sample_engine('tank')
     d = load_golden('derived', 'tank')
     st = m['meta']
     Nx, Ny = 6, 4
@@ -199,9 +177,8 @@ def test_step_one_statistics_match_exact_moment_matching():
 
 def test_argument_and_state_errors_leave_the_model_usable():
     import gp_mpc_b200
-    L = _L()
     lib = L.load()
-    eng, m = _engine('tank')
+    eng, m = sample_engine('tank')
     Nx, Ny = 6, 4
     z0, U, eps = _inputs(m, 2, 3, 0)
     K = np.zeros((2, Ny))

@@ -12,11 +12,10 @@ import gp_mpc_b200
 from oracle import gp_oracle as orc
 from oracle import sample_oracle as so
 from tests import _sample_grad_oracle as sgo
-from tests._fake_engine import OracleEngine
-from tests._util import load_fixture, load_golden
+from tests._fake_engine import OracleEngine, TwoRanks, sample_model, sharded
+from tests._util import load_golden
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-MARGIN = 1e3                # every d is at least MARGIN delta sf2 away from the delta rule's threshold
 # Central-difference step and bar (relative to 1 + max |derivative|).  The error of a quotient is the draw's rounding over
 # the step: R^-1 enters the draw twice and tank's and car's pivots are small (cond K ~ 1e10 on car), so their draws carry
 # ~1e-10 of rounding and need a step of 1e-4 (errors measured up to 8e-7 there, 7e-5 at a step of 1e-6); the
@@ -46,17 +45,9 @@ class OracleEngineWithSampleGrad(OracleEngine):
         return r['samples'], r['z_out'], r['kept'], r['dsamples']
 
 
-def _model(name):
-    if name == 'synthetic':
-        p = orc.synthetic_problem(150, 5, 3, config_id=2)
-        p['hyper'][:, :5] = 1.5
-        return dict(X=p['X'], Y=p['Y'], hyper=p['hyper'], normalize=False)
-    return load_fixture(name)
-
-
 def _engine_problem(name, feedback, Nt=4, B=2, seed=0):
     """A factor and a roll-out of B trajectories in the engine's units: model, Linv, args of rollout_sample_grad."""
-    m = _model(name)
+    m = sample_model(name)
     post = orc.postfit(m['X'], m['Y'], m['hyper'], lapack_general_solve=False)
     model = dict(X=m['X'], hyper=m['hyper'], alpha=post['alpha'], chol=post['chol'])
     Linv = np.stack([np.linalg.inv(L) for L in post['chol']])
@@ -103,18 +94,12 @@ def _perturbed(args, p, h):
     return a
 
 
-def _assert_margin(d, hyper):
-    Nx = hyper.shape[1] - 2
-    thr = so.DELTA * hyper[:, Nx] ** 2
-    assert (np.abs(d - thr) >= MARGIN * thr).all(), 'a step sits within the margin of the delta rule'
-
-
 @pytest.mark.parametrize('feedback', [False, True])
 @pytest.mark.parametrize('name', ['tank', 'car', 'synthetic'])
 def test_oracle_matches_central_differences_of_the_draws(name, feedback):
     model, Linv, args = _engine_problem(name, feedback)
     r = sgo.rollout_sample_grad(model, Linv, **args)
-    _assert_margin(r['d'], model['hyper'])
+    sgo.assert_margin(r['d'], model['hyper'])
     s0, _, k0 = so.rollout_sample(model, Linv, **args)
     assert np.array_equal(r['kept'], k0) and np.abs(r['samples'] - s0).max() <= 1e-12 * (1 + np.abs(s0).max())
     D = r['dsamples']
@@ -132,7 +117,7 @@ def test_oracle_matches_central_differences_of_the_draws(name, feedback):
 def test_oracle_matches_the_joint_cholesky_form(name):
     """Teacher-forced along a fixed path Z moved in a direction dZ: the sequential recursion's df against differences of
     f_S = m_S + chol(C[S, S]) eps_S, an independent route to the same draw."""
-    m = _model(name)
+    m = sample_model(name)
     post = orc.postfit(m['X'], m['Y'], m['hyper'], lapack_general_solve=False)
     rng = np.random.default_rng(4)
     Nx, T = m['X'].shape[1], 8
@@ -147,7 +132,7 @@ def test_oracle_matches_the_joint_cholesky_form(name):
             _, g, d[t], kept = c.step(Z[:t + 1], dZ[:t + 1], eps[:t + 1])
             assert kept
             df[t] = g[0]
-        _assert_margin(d[None], m['hyper'][a:a + 1])
+        sgo.assert_margin(d[None], m['hyper'][a:a + 1])
 
         def joint(Zp):
             mu, C = so.path_moments(m['X'], m['hyper'][a], post['alpha'][a], Linv, Zp)
@@ -161,7 +146,7 @@ def test_oracle_matches_the_joint_cholesky_form(name):
 def test_a_skipped_point_takes_the_branch_taken():
     """A return to an earlier point is dropped by the delta rule: its draw is the conditional mean, whose derivative is
     the derivative of the value the draw already has there."""
-    m = _model('synthetic')
+    m = sample_model('synthetic')
     post = orc.postfit(m['X'], m['Y'], m['hyper'], lapack_general_solve=False)
     rng = np.random.default_rng(2)
     Nx, T = m['X'].shape[1], 4
@@ -179,7 +164,7 @@ def test_a_skipped_point_takes_the_branch_taken():
 
 
 def _gp(name, factory=OracleEngineWithSampleGrad, **kw):
-    m = _model(name)
+    m = sample_model(name)
     args = dict(mean_func='zero', gp_method='TA', normalize=m['normalize'], hyper=dict(hyper=m['hyper']),
                 engine_factory=factory)
     if m['normalize']:
@@ -274,22 +259,7 @@ def test_feedback_runs_one_pass_per_distinct_gain():
     assert np.array_equal(r['samples'], gp.sample_rollout(X0, U, 2, seed=1, feedback=True, x_ref=0.9 * x0 + 0.1))
 
 
-class _TwoRanks:
-    rank, world = 0, 2
-
-    def broadcast_object(self, obj, src=0):
-        return obj
-
-    def allgather_object(self, obj):
-        return [obj, obj]
-
-    def barrier(self):
-        pass
-
-
-class _ShardEngine(OracleEngineWithSampleGrad):
-    def comm_init(self, uid, rank, world):
-        self.rank, self.world = rank, world
+_ShardEngine = sharded(OracleEngineWithSampleGrad)
 
 
 def test_argument_errors():
@@ -309,7 +279,7 @@ def test_argument_errors():
         auto.sample_rollout_grad(np.zeros(2), np.zeros((3, 0)), 2, feedback=True)
     r = auto.sample_rollout_grad(np.zeros(2), np.zeros((3, 0)), 2, seed=0)
     assert r['dsamples_dx0'].shape == (2, 4, 2, 2) and r['dsamples_du'].shape == (2, 4, 2, 3, 0)
-    sh = gp_mpc_b200.GP(m['X'], m['Y'], normalize=False, hyper=dict(hyper=m['hyper']), comm=_TwoRanks(),
+    sh = gp_mpc_b200.GP(m['X'], m['Y'], normalize=False, hyper=dict(hyper=m['hyper']), comm=TwoRanks(),
                         engine_factory=_ShardEngine)
     with pytest.raises(NotImplementedError, match='needs all outputs on one GPU'):
         sh.sample_rollout_grad(x0, U, 2)

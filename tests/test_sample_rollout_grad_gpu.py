@@ -5,14 +5,15 @@ error codes, and the gradient of a Monte Carlo objective through GP.sample_rollo
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle import sample_oracle as so
 from tests import _sample_grad_oracle as sgo
+from tests._engines import sample_engine
 from tests._util import load_fixture, load_golden
 
 pytestmark = pytest.mark.gpu
 
-MARGIN = 1e3                # every d is at least MARGIN delta sf2 away from the delta rule's threshold
 # Central-difference step and bar relative to 1 + max |derivative| (DESIGN 4.16): the quotient's error is the draw's
 # rounding over the step; R^-1 enters twice and tank's pivots are small, so tank needs a wider step than the synthetic case
 STEP = dict(synthetic=1e-6, tank=1e-4)
@@ -20,24 +21,6 @@ BAR = dict(synthetic=2e-5, tank=5e-6)
 # the device against the checker, relative to 1 + max |derivative|: two different roundings of the same recursion,
 # amplified by R^-1 twice on tank's small pivots
 ORACLE_BAR = dict(synthetic=1e-7, tank=1e-5)
-
-
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
-def _engine(name):
-    import gp_mpc_b200
-    if name == 'synthetic':                              # N = 1000, Nx = 8, Ny = 6 (Nu = 2)
-        p = orc.synthetic_problem(1000, 8, 6, config_id=4)
-        m = dict(X=p['X'], Y=p['Y'], hyper=p['hyper'], normalize=False)
-    else:
-        m = load_fixture(name)
-    N, Nx = m['X'].shape
-    eng = gp_mpc_b200.Engine(N, Nx, m['Y'].shape[1], device=0)
-    eng.set_data(m['X'], m['Y']); eng.set_hyper(m['hyper']); eng.factorize()
-    return eng, m
 
 
 def _inputs(m, B, Nt, seed, spread=0.3):
@@ -51,18 +34,11 @@ def _inputs(m, B, Nt, seed, spread=0.3):
 
 
 def _factor(eng, m):
-    L = _L()
     Ny = m['Y'].shape[1]
     Linv = np.stack([eng.get(L.GET_LINV, a) for a in range(Ny)])
     model = dict(X=m['X'], hyper=m['hyper'], alpha=np.stack([eng.get(L.GET_ALPHA, a) for a in range(Ny)]),
                  chol=np.stack([np.linalg.inv(Li) for Li in Linv]))
     return model, Linv
-
-
-def _assert_margin(d, hyper):
-    Nx = hyper.shape[1] - 2
-    thr = so.DELTA * hyper[:, Nx] ** 2
-    assert (np.abs(d - thr) >= MARGIN * thr).all(), 'a step sits within the margin of the delta rule'
 
 
 def _perturbed(z0, U, K, p, h):
@@ -81,7 +57,7 @@ def _perturbed(z0, U, K, p, h):
 
 @pytest.mark.parametrize('B', [1, 64, 65, 130])
 def test_draws_are_rollout_sample_bit_for_bit(B):
-    eng, m = _engine('synthetic')
+    eng, m = sample_engine('synthetic')
     z0, U, eps, xi = _inputs(m, B, 6, B)
     Ny, Nx = m['Y'].shape[1], m['X'].shape[1]
     K = 0.1 * np.random.default_rng(B).standard_normal((Nx - Ny, Ny))
@@ -97,8 +73,7 @@ def test_draws_are_rollout_sample_bit_for_bit(B):
 @pytest.mark.parametrize('name', ['synthetic', 'tank'])
 def test_step_one_against_predict_grad(name):
     """df_0 = J dz + (dvar_dz . dz) / (2 sqrt(var)) eps_0 on the unit columns of z0."""
-    L = _L()
-    eng, m = _engine(name)
+    eng, m = sample_engine(name)
     B = 70
     z0, U, eps, _ = _inputs(m, B, 1, 2)
     _, _, kept, D = eng.rollout_sample_grad(z0, U, eps)
@@ -116,7 +91,7 @@ SPREAD = dict(synthetic=0.3, tank=1.0)
 
 @pytest.mark.parametrize('name, feedback', [('synthetic', False), ('synthetic', True), ('tank', False)])
 def test_central_differences_on_the_device(name, feedback):
-    eng, m = _engine(name)
+    eng, m = sample_engine(name)
     Nt = 12 if name == 'synthetic' else 5
     Ny, Nx = m['Y'].shape[1], m['X'].shape[1]
     z0, U, eps, xi = _inputs(m, 2, Nt, 5, SPREAD[name])
@@ -124,7 +99,7 @@ def test_central_differences_on_the_device(name, feedback):
     x_ref = np.full(Ny, 0.1) if feedback else None
     s, z_out, kept, D = eng.rollout_sample_grad(z0, U, eps, xi, None, K, x_ref)
     model, Linv = _factor(eng, m)
-    _assert_margin(sgo.rollout_sample_grad(model, Linv, z0, U, eps, xi, None, K, x_ref)['d'], m['hyper'])
+    sgo.assert_margin(sgo.rollout_sample_grad(model, Linv, z0, U, eps, xi, None, K, x_ref)['d'], m['hyper'])
     h = STEP[name]
     for p in range(D.shape[-1]):
         sp = eng.rollout_sample(*_perturbed(z0, U, K, p, h)[:2], eps, xi, None, _perturbed(z0, U, K, p, h)[2], x_ref)
@@ -139,7 +114,7 @@ def test_central_differences_on_the_device(name, feedback):
 @pytest.mark.parametrize('name', ['synthetic', 'tank'])
 def test_against_the_checker(name, lapack):
     """The device against the numpy recursion on the engine's own L^-1 and alpha, or on a LAPACK factor."""
-    eng, m = _engine(name)
+    eng, m = sample_engine(name)
     z0, U, eps, xi = _inputs(m, 3, 8 if name == 'synthetic' else 5, 7, SPREAD[name])
     s, z_out, kept, D = eng.rollout_sample_grad(z0, U, eps, xi)
     if lapack:
@@ -178,7 +153,7 @@ def test_a_model_whose_draws_drop_points():
 
 
 def test_bit_identical_alone_in_a_batch_and_on_repeat():
-    eng, m = _engine('synthetic')
+    eng, m = sample_engine('synthetic')
     z0, U, eps, xi = _inputs(m, 130, 6, 3)
     full = eng.rollout_sample_grad(z0, U, eps, xi)
     again = eng.rollout_sample_grad(z0, U, eps, xi)
@@ -193,8 +168,7 @@ def test_bit_identical_alone_in_a_batch_and_on_repeat():
 
 def test_error_codes_leave_the_model_usable():
     import gp_mpc_b200
-    L = _L()
-    eng, m = _engine('synthetic')
+    eng, m = sample_engine('synthetic')
     z0, U, eps, _ = _inputs(m, 2, 4, 1)
     Ny, Nx = m['Y'].shape[1], m['X'].shape[1]
     h = eng.h

@@ -33,10 +33,11 @@ the first window; DRIFT_TOL is about 10x the larger of each."""
 import numpy as np
 import pytest
 
+from gp_mpc_b200 import _lib as L
 from oracle import gp_oracle as orc
 from oracle import hess_oracle as hor
 from oracle import update_oracle_ld as upd
-from tests.test_predict_derivs_shapes_gpu import TOL as PTOL, normalised
+from tests._util import PREDICT_TOL, normalised
 
 pytestmark = pytest.mark.gpu
 
@@ -49,11 +50,6 @@ REF_KEY = dict(jac='J')
 DRIFT_TOL = dict(backward=1e-12, inverse=4e-13)
 
 
-def _L():
-    import gp_mpc_b200
-    return gp_mpc_b200._lib
-
-
 def problem(N, Nx, Ny, sn=0.3, seed=0):
     p = orc.synthetic_problem(N, Nx, Ny, config_id=900 + 7 * Nx + Ny + seed)
     hyper = p['hyper'].copy()
@@ -62,7 +58,7 @@ def problem(N, Nx, Ny, sn=0.3, seed=0):
 
 
 def fit(X, Y, hyper, cap=None, out_begin=0, out_count=None):
-    eng = _L().Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, capacity=cap, out_begin=out_begin,
+    eng = L.Engine(X.shape[0], X.shape[1], Y.shape[1], device=0, capacity=cap, out_begin=out_begin,
                       out_count=out_count)
     eng.set_data(X, Y)
     eng.set_hyper(hyper)
@@ -71,7 +67,6 @@ def fit(X, Y, hyper, cap=None, out_begin=0, out_count=None):
 
 
 def factors(eng):
-    L = _L()
     return [upd.factor(eng.get(L.GET_CHOL, a), eng.get(L.GET_LINV, a)) for a in eng.local_outputs]
 
 
@@ -85,7 +80,6 @@ def check(eng, pre, post, rows, X, Y, hyper, near):
     bits of `pre`, rows >= rows within the scales; alpha and log det; then TA at H = 8 points 0.05 from the training
     inputs `near` (skipped on a sharded handle).  X, Y: the data after the update; hyper: the owned rows.
     Returns the largest normalised error of each quantity."""
-    L = _L()
     got = factors(eng)
     N = X.shape[0]
     err = dict(L=0.0, Li=0.0, alpha=0.0, logdet=0.0)
@@ -120,7 +114,7 @@ def check(eng, pre, post, rows, X, Y, hyper, near):
 
 def assert_within(name, err):
     print('MEASURED', name, {k: '%.2e' % v for k, v in err.items()})
-    bad = {k: e for k, e in err.items() if not e <= TOL.get(k, PTOL.get(k))}
+    bad = {k: e for k, e in err.items() if not e <= TOL.get(k, PREDICT_TOL.get(k))}
     assert not bad, (name, bad)
 
 
@@ -215,7 +209,6 @@ def test_append_onto_a_jittered_factor():
     and holds the factor of K + 1e-8 I.  A far point and then a near one are appended, with a K build in between
     (GET_K, which reuses the K build's jitter scratch).  Each new row must be the factor of K_aug + 1e-8 I: the
     reference puts the jitter on the new diagonal entry of output 1 and on none of the others."""
-    L = _L()
     N, Nx = 300, 6
     X, Y, hyper = problem(N + 2, Nx, 3, sn=1e-2, seed=1)
     X[N // 2:N] = X[:N - N // 2]
@@ -240,7 +233,7 @@ def test_append_onto_a_jittered_factor():
     assert abs(float(Lg[-1] @ Lg[-1] - kd)) < 1e-14
     eng.close()
     print('MEASURED jitter', {k: '%.2e' % v for k, v in errs.items()})
-    bad = {k: e for k, e in errs.items() if not e <= TOL.get(k.split()[0], PTOL.get(k.split()[0]))}
+    bad = {k: e for k, e in errs.items() if not e <= TOL.get(k.split()[0], PREDICT_TOL.get(k.split()[0]))}
     assert not bad, bad
 
 
@@ -299,7 +292,6 @@ def test_sliding_window_drift():
     """A window of N = Npad = 1024 points (no spare row) slides through 2048 cycles of remove([0]) + append; after 256
     and 2048 cycles the factor's backward error against the window's K and the error of L^-1 as L's inverse stay
     within DRIFT_TOL (compare the fresh factorisation's, printed alongside)."""
-    L = _L()
     N, Nx, C = 1024, 4, 2048
     X, Y, hyper = problem(N + C, Nx, 1, sn=0.1)
     eng, info = fit(X[:N], Y[:N], hyper)
