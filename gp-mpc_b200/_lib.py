@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('GPMPC_LIB', os.path.join(_HERE, 'lib', 'libgpmpc.so'))
 
 OK, ERR_ARG, ERR_CUDA, ERR_STATE, ERR_NCCL, ERR_NOTPD = 0, -1, -2, -3, -4, -5
-METHOD_ME, METHOD_TA, METHOD_EM = 0, 1, 2
+METHOD_ME, METHOD_TA, METHOD_EM, METHOD_UT = 0, 1, 2, 3
 GET_CHOL, GET_ALPHA, GET_INVK, GET_K, GET_LOGDET, GET_LINV, GET_ALPHA_NLML = range(7)
 PROF_KBUILD_FULL, PROF_KBUILD_LOWER, PROF_SYRK, PROF_FACTORIZE, PROF_TRIGEMM, PROF_KS, PROF_PREDICT_TAIL, PROF_PANEL = range(8)
 
@@ -260,6 +260,12 @@ class Engine:
     def set_option(self, name, value):
         self._check(self.lib.gpmpc_set_option(self.h, name.encode(), float(value)))
 
+    def set_ut_params(self, alpha=1.0, beta=0.0, kappa=0.0):
+        """The unscented transform's (alpha, beta, kappa) for METHOD_UT (options "ut_alpha", "ut_beta", "ut_kappa"; the
+        defaults are the engine's).  Raises GpmpcError for alpha <= 0 or kappa <= -Nx."""
+        for name, v in (('ut_alpha', alpha), ('ut_beta', beta), ('ut_kappa', kappa)):
+            self.set_option(name, v)
+
     # -- predict ----------------------------------------------------------------------
     def _points(self, Z, Sigma):
         """Z -> (H,Nx); Sigma: None, one (Nx,Nx) for every point or one per point (H,Nx,Nx) -> (Z, Sigma, H, spp)."""
@@ -273,7 +279,8 @@ class Engine:
         return Z, Sigma, H, spp
 
     def predict(self, Z, Sigma=None, method=METHOD_TA, want_cov=True, want_jac=True):
-        """Z:(H,Nx) -> mean:(H,Ny), var:(H,Ny), cov:(H,Ny,Ny)|None, jac:(H,Ny,Nx)|None (host arrays).
+        """Z:(H,Nx) -> mean:(H,Ny), var:(H,Ny), cov:(H,Ny,Ny)|None, jac:(H,Ny,Nx)|None (host arrays).  METHOD_UT needs
+        Sigma; its jac is the 'ME' Jacobian at Z.
         Building the six ctypes pointer objects was a visible share of a small call, so the call
         goes through per-shape staging arrays whose pointers are built once; the results are returned as fresh copies."""
         Z, Sigma, H, spp = self._points(Z, Sigma)

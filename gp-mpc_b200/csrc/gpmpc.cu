@@ -3,6 +3,7 @@
 #include "../../include/gpmpc.h"
 
 #include <dlfcn.h>
+#include <limits.h>
 #include <math.h>
 #include <stdarg.h>
 #include <stdlib.h>
@@ -10,6 +11,7 @@
 
 #include <algorithm>
 #include <array>
+#include <cmath>
 #include <functional>
 #include <map>
 #include <memory>
@@ -209,6 +211,8 @@ struct gpmpc_handle_s {
     int sms = 132;                    // multiprocessors of the device (queried in create)
     int opt_refine = 0, opt_small_tiles = 528;   // 128x64-tile count below which 64x32 tiles are used (4 per SM)
     int opt_em_points = 0;            // points per batched 'EM' forward (0: the scratch budget EM_CHUNK_BYTES decides)
+    double ut_alpha = 1.0, ut_beta = 0.0, ut_kappa = 0.0;   // 'UT' parameters (options "ut_alpha", "ut_beta", "ut_kappa")
+    DevBuf<double> dUt;               // 'UT' pass: [sigma points (Hs,Nx) | 'ME' means (Hs,Ny) | variances (Hs,Ny) | J (Hs,Ny,Nx)]
     // comm
     nccl_comm_t comm = nullptr; int rank = 0, world = 1;
     // peer (CUDA IPC) exchange: [flags: 2*MAXW u64][gather buffer parity 0][parity 1]
@@ -1194,6 +1198,17 @@ extern "C" int gpmpc_set_option(gpmpc_handle_t h, const char* name, double value
         if (!(value >= 0.0 && value <= 1e9)) { set_error(h, "nlml_batch_max must be >= 0"); return GPMPC_ERR_ARG; }
         h->opt_nlml_batch_max = (int)value; return GPMPC_OK;
     }
+    if (!strcmp(name, "ut_alpha") || !strcmp(name, "ut_beta") || !strcmp(name, "ut_kappa")) {
+        double a = h->ut_alpha, b = h->ut_beta, k = h->ut_kappa;
+        (name[3] == 'a' ? a : name[3] == 'b' ? b : k) = value;
+        const double n = h->Nx, lam = a * a * (n + k) - n;
+        if (!std::isfinite(value) || !(a > 0.0) || !(n + lam > 0.0)) {
+            set_error(h, "%s = %g: 'UT' needs a finite value, alpha > 0 and n + lambda > 0 (kappa > -Nx)", name, value);
+            return GPMPC_ERR_ARG;
+        }
+        h->ut_alpha = a; h->ut_beta = b; h->ut_kappa = k;
+        return GPMPC_OK;
+    }
     set_error(h, "unknown option %s", name);
     return GPMPC_ERR_ARG;
 }
@@ -1513,6 +1528,135 @@ static int predict_core(gpmpc_handle_t h, int method, int H, const double* dZ, c
         assemble_kernel<<<std::min(H, 2048), 128, smem, h->st>>>(as);
         CUDA_TRY(cudaGetLastError());
     }
+    return GPMPC_OK;
+}
+
+// ------------------------------------------------------------------------------------
+// 'UT': the unscented transform around the unchanged 'ME' pass.  With n = Nx, lambda = alpha^2 (n + kappa) - n and
+// c = sqrt(n + lambda), the 2n+1 sigma points of (z, Sigma) are z, then z + c S_j, z - c S_j for j = 1..n (S_j column j
+// of the semidefinite lower Cholesky factor S of Sigma); the weights are W0m = lambda / (n + lambda),
+// W0c = W0m + 1 - alpha^2 + beta, Wi = 1 / (2 (n + lambda)).  ut_sigma_kernel writes the points, predict_core evaluates
+// 'ME' at all of them in one pass, ut_combine_kernel recombines: every sum runs in point order with separate multiplies
+// and adds, so a point's results depend on its own inputs only.
+// ------------------------------------------------------------------------------------
+struct UtWeights { double c, wm0, wc0, wi; };
+
+static UtWeights ut_weights(gpmpc_handle_t h)
+{
+    const double n = h->Nx, a2 = h->ut_alpha * h->ut_alpha, lam = a2 * (n + h->ut_kappa) - n;
+    return {std::sqrt(n + lam), lam / (n + lam), lam / (n + lam) + 1.0 - a2 + h->ut_beta, 1.0 / (2.0 * (n + lam))};
+}
+
+// points of the pass behind H 'UT' points
+static inline long long ut_points(gpmpc_handle_t h, long long H) { return H * (2LL * h->Nx + 1); }
+
+// One warp per point p: S = the lower Cholesky factor of Sigma_p (Sigma or Sigma + p Nx^2) in shared memory, left-looking
+// column by column.  A pivot <= 1e-14 max(diag Sigma), or <= 0, makes its column exactly zero (a semidefinite Sigma: a zero
+// u-block, a rank-Ny feedback covariance).  Lane i owns row i.  Then the 2 Nx + 1 rows of point p into Zs.
+__global__ void __launch_bounds__(32)
+ut_sigma_kernel(const double* __restrict__ Z, const double* __restrict__ Sigma, int spp, int Nx, double c,
+                double* __restrict__ Zs)
+{
+    __shared__ double L[NX_MAX * (NX_MAX + 1)];
+    constexpr int LD = NX_MAX + 1;
+    const int p = blockIdx.x, i = threadIdx.x;
+    const double* S = Sigma + (spp ? (size_t)p * Nx * Nx : 0);
+    for (int idx = i; idx < Nx * Nx; idx += 32) {
+        const int r = idx / Nx, k = idx - r * Nx;
+        L[r * LD + k] = k <= r ? S[idx] : 0.0;
+    }
+    __syncwarp();
+    double dmax = 0.0;
+    for (int k = 0; k < Nx; ++k) dmax = fmax(dmax, L[k * LD + k]);
+    const double tol = 1e-14 * dmax;
+    for (int j = 0; j < Nx; ++j) {
+        double d = L[j * LD + j];                            // every lane forms the same pivot in the same order
+        for (int k = 0; k < j; ++k) d = __dsub_rn(d, __dmul_rn(L[j * LD + k], L[j * LD + k]));
+        const bool keep = d > tol;
+        const double piv = keep ? sqrt(d) : 0.0;
+        double s = 0.0;
+        if (i > j && i < Nx) {
+            s = L[i * LD + j];
+            for (int k = 0; k < j; ++k) s = __dsub_rn(s, __dmul_rn(L[i * LD + k], L[j * LD + k]));
+        }
+        __syncwarp();
+        if (i == j) L[j * LD + j] = piv;
+        if (i > j && i < Nx) L[i * LD + j] = keep ? __ddiv_rn(s, piv) : 0.0;
+        __syncwarp();
+    }
+    const double* z = Z + (size_t)p * Nx;
+    double* out = Zs + (size_t)p * (2 * Nx + 1) * Nx;
+    if (i < Nx) {
+        const double ze = z[i];
+        out[i] = ze;
+        for (int j = 0; j < Nx; ++j) {
+            const double s = __dmul_rn(c, L[i * LD + j]);
+            out[(2 * j + 1) * Nx + i] = __dadd_rn(ze, s);
+            out[(2 * j + 2) * Nx + i] = __dsub_rn(ze, s);
+        }
+    }
+}
+
+// One CTA per point p: the 2 Nx + 1 'ME' means m and variances v of its sigma points (rows p (2 Nx + 1) .. of the pass) ->
+//   mean = sum_i Wim m_i,  cov = sum_i Wic (m_i - mean)(m_i - mean)^T + diag(sum_i Wim v_i),  var = diag(cov),
+// each sum from i = 0 in point order; jac = the 'ME' Jacobian at z (row 0).  Every output may be null.
+__global__ void __launch_bounds__(128)
+ut_combine_kernel(const double* __restrict__ m, const double* __restrict__ v, const double* __restrict__ J, int Nx, int Ny,
+                  double wm0, double wc0, double wi, double* __restrict__ mean, double* __restrict__ var,
+                  double* __restrict__ cov, double* __restrict__ jac)
+{
+    extern __shared__ double ut_sh[];                        // mean (Ny) | sum_i Wim v_i (Ny)
+    const int p = blockIdx.x, tid = threadIdx.x, np = 2 * Nx + 1;
+    m += (size_t)p * np * Ny; v += (size_t)p * np * Ny;
+    for (int a = tid; a < Ny; a += blockDim.x) {
+        double s = 0.0, sv = 0.0;
+        for (int k = 0; k < np; ++k) {
+            const double w = k ? wi : wm0;
+            s = __dadd_rn(s, __dmul_rn(w, m[k * Ny + a]));
+            sv = __dadd_rn(sv, __dmul_rn(w, v[k * Ny + a]));
+        }
+        ut_sh[a] = s; ut_sh[Ny + a] = sv;
+        if (mean) mean[(size_t)p * Ny + a] = s;
+    }
+    __syncthreads();
+    const int n_out = cov ? Ny * Ny : (var ? Ny : 0);        // without cov only the diagonal is formed
+    for (int idx = tid; idx < n_out; idx += blockDim.x) {
+        const int a = cov ? idx / Ny : idx, b = cov ? idx - a * Ny : idx;
+        const double ma = ut_sh[a], mb = ut_sh[b];
+        double s = 0.0;
+        for (int k = 0; k < np; ++k)
+            s = __dadd_rn(s, __dmul_rn(k ? wi : wc0, __dmul_rn(__dsub_rn(m[k * Ny + a], ma), __dsub_rn(m[k * Ny + b], mb))));
+        if (a == b) {
+            s = __dadd_rn(s, ut_sh[Ny + a]);
+            if (var) var[(size_t)p * Ny + a] = s;
+        }
+        if (cov) cov[(size_t)p * Ny * Ny + idx] = s;
+    }
+    if (jac)
+        for (int idx = tid; idx < Ny * Nx; idx += blockDim.x)
+            jac[(size_t)p * Ny * Nx + idx] = J[(size_t)p * np * Ny * Nx + idx];
+}
+
+// 'UT' at the H points dZ (H,Nx) with covariances dSigma (one, or one per point), device pointers: the sigma points into
+// dUt, one 'ME' pass of predict_core over the H (2 Nx + 1) points (the caller's predict_prepare has laid out the
+// buffers for that many), the recombination into the outputs (any may be null).
+static int ut_pass(gpmpc_handle_t h, int H, const double* dZ, const double* dSigma, int spp, double* mean, double* var,
+                   double* cov, double* jac)
+{
+    const int Nx = h->Nx, Ny = h->Ny;
+    const long long Hs = ut_points(h, H);
+    ENSURE(h->dUt, Hs * (Nx + 2 * Ny + (jac ? (long long)Ny * Nx : 0)));
+    double* Zs = h->dUt;
+    double* m = Zs + Hs * Nx;
+    double* v = m + Hs * Ny;
+    double* J = jac ? v + Hs * Ny : nullptr;
+    const UtWeights w = ut_weights(h);
+    ut_sigma_kernel<<<H, 32, 0, h->st>>>(dZ, dSigma, spp, Nx, w.c, Zs);
+    CUDA_TRY(cudaGetLastError());
+    const int rc = predict_core(h, GPMPC_METHOD_ME, (int)Hs, Zs, nullptr, 0, m, v, nullptr, J);
+    if (rc) return rc;
+    ut_combine_kernel<<<H, 128, 2 * Ny * 8, h->st>>>(m, v, J, Nx, Ny, w.wm0, w.wc0, w.wi, mean, var, cov, jac);
+    CUDA_TRY(cudaGetLastError());
     return GPMPC_OK;
 }
 
@@ -2173,12 +2317,24 @@ static int peer_status_check(gpmpc_handle_t h)
     return GPMPC_OK;
 }
 
-// First check of every predict-family entry `fn` (the name its errors carry): a factorised model, H >= 1 and a known method.
-static int predict_guard(gpmpc_handle_t h, const char* fn, int method, int H)
+// The 'UT' pass of H points must be indexable by int
+static int ut_size_check(gpmpc_handle_t h, const char* fn, int H)
+{
+    if (ut_points(h, H) > INT_MAX) { set_error(h, "%s: H (2 Nx + 1) = %lld 'UT' points exceed INT_MAX", fn, ut_points(h, H)); return GPMPC_ERR_ARG; }
+    return GPMPC_OK;
+}
+
+// First check of every predict-family entry `fn` (the name its errors carry): a factorised model, H >= 1 and a known method;
+// 'UT' only where the entry takes it (ut).
+static int predict_guard(gpmpc_handle_t h, const char* fn, int method, int H, bool ut = false)
 {
     const int rc = model_guard(h, fn, NEED_FACTOR);
     if (rc) return rc;
     if (H < 1) { set_error(h, "%s: H < 1", fn); return GPMPC_ERR_ARG; }
+    if (method == GPMPC_METHOD_UT) {
+        if (!ut) { set_error(h, "%s: method UT is taken by gpmpc_predict, gpmpc_predict_device, gpmpc_rollout and gpmpc_rollout_batch only", fn); return GPMPC_ERR_ARG; }
+        return ut_size_check(h, fn, H);
+    }
     if (method != GPMPC_METHOD_ME && method != GPMPC_METHOD_TA && method != GPMPC_METHOD_EM) { set_error(h, "%s: unknown method %d", fn, method); return GPMPC_ERR_ARG; }
     return GPMPC_OK;
 }
@@ -2194,13 +2350,15 @@ static int predict_prepare(gpmpc_handle_t h, const char* fn, int H, bool all_out
 extern "C" int gpmpc_predict_device(gpmpc_handle_t h, int method, int H, const double* dZ, const double* dSigma,
                                     int spp, double* d_mean, double* d_var, double* d_cov, double* d_jac, int sync)
 {
-    int rc = predict_guard(h, __func__, method, H);
+    int rc = predict_guard(h, __func__, method, H, true);
     if (rc) return rc;
+    const bool ut = method == GPMPC_METHOD_UT;
     if (method == GPMPC_METHOD_EM) { set_error(h, "gpmpc_predict_device: EM needs host inputs (use gpmpc_predict)"); return GPMPC_ERR_ARG; }
-    if (!dZ || (method == GPMPC_METHOD_TA && d_cov && !dSigma)) { set_error(h, "gpmpc_predict_device: null Z / Sigma"); return GPMPC_ERR_ARG; }
-    rc = predict_prepare(h, __func__, H, false);
+    if (!dZ || (method == GPMPC_METHOD_TA && d_cov && !dSigma) || (ut && !dSigma)) { set_error(h, "gpmpc_predict_device: null Z / Sigma"); return GPMPC_ERR_ARG; }
+    rc = predict_prepare(h, __func__, ut ? (int)ut_points(h, H) : H, ut);
     if (rc) return rc;
-    rc = predict_core(h, method, H, dZ, dSigma, spp, d_mean, d_var, d_cov, d_jac);
+    rc = ut ? ut_pass(h, H, dZ, dSigma, spp, d_mean, d_var, d_cov, d_jac)
+            : predict_core(h, method, H, dZ, dSigma, spp, d_mean, d_var, d_cov, d_jac);
     if (rc) return rc;
     if (sync) CUDA_TRY(cudaStreamSynchronize(h->st));
     return GPMPC_OK;
@@ -2662,15 +2820,16 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
                          const double* uscale, double* means, double* vars, double* cov_last, const RolloutTangents* tg = nullptr,
                          bool em_entry = false)
 {
-    int rc = predict_guard(h, fn, method, 1);
+    int rc = predict_guard(h, fn, method, 1, !tg && !em_entry);
     if (rc) return rc;
     const int Nx = h->Nx, Ny = h->Ny, Nu = Nx - Ny;
-    const bool em = method == GPMPC_METHOD_EM;
-    if (em && !em_entry) { set_error(h, "%s: methods ME and TA (EM: gpmpc_rollout_batch_em)", fn); return GPMPC_ERR_ARG; }
+    const bool em = method == GPMPC_METHOD_EM, ut = method == GPMPC_METHOD_UT;
+    if (em && !em_entry) { set_error(h, "%s: methods ME, TA and UT (EM: gpmpc_rollout_batch_em)", fn); return GPMPC_ERR_ARG; }
     rc = rollout_args(h, fn, B, Nt, !z0 || !Sigma0 || !means || !vars, U, K);
+    if (!rc && ut) rc = ut_size_check(h, fn, B);
     if (rc) return rc;
     if (tg && (!tg->dmeans || !tg->dvars)) { set_error(h, "%s: null dmeans / dvars", fn); return GPMPC_ERR_ARG; }
-    rc = predict_prepare(h, fn, B, true);
+    rc = predict_prepare(h, fn, ut ? (int)ut_points(h, B) : B, true);
     if (rc) return rc;
     NvtxRange nvtx_r(tg ? "gpmpc.rollout_grad" : "gpmpc.rollout");
     // device slab: [Z (B,Nx) | Sigma (B,Nx,Nx) | policy (rollout_policy) | means (Nt,B,Ny) | vars (Nt,B,Ny) |
@@ -2721,7 +2880,8 @@ static int rollout_batch(gpmpc_handle_t h, const char* fn, int method, int B, in
         double* var_t = d + o_v + (size_t)t * Bs * Ny;
         double* cov_t = d + o_c + (size_t)t * Bs * Ny * Ny;
         if (!em) {
-            rc = predict_core(h, method, B, d, d + o_sig, 1, mean_t, var_t, cov_t, nullptr);
+            rc = ut ? ut_pass(h, B, d, d + o_sig, 1, mean_t, var_t, cov_t, nullptr)
+                    : predict_core(h, method, B, d, d + o_sig, 1, mean_t, var_t, cov_t, nullptr);
             if (rc) return rc;
         } else {
             // the step's Sigma back to the host (step 0: Sigma0, already in the pinned mirror), then predict_em's pass over
@@ -2840,15 +3000,16 @@ extern "C" int gpmpc_rollout(gpmpc_handle_t h, int method, int Nt, const double*
 extern "C" int gpmpc_predict(gpmpc_handle_t h, int method, int H, const double* Z, const double* Sigma,
                              int spp, double* mean, double* var, double* cov, double* jac)
 {
-    int rc = predict_guard(h, __func__, method, H);
+    int rc = predict_guard(h, __func__, method, H, true);
     if (rc) return rc;
-    if (!Z || (method == GPMPC_METHOD_TA && cov && !Sigma)) { set_error(h, "gpmpc_predict: null Z / Sigma"); return GPMPC_ERR_ARG; }
+    const bool ut = method == GPMPC_METHOD_UT;
+    if (!Z || (method == GPMPC_METHOD_TA && cov && !Sigma) || (ut && !Sigma)) { set_error(h, "gpmpc_predict: null Z / Sigma"); return GPMPC_ERR_ARG; }
     if (method == GPMPC_METHOD_EM && jac) { set_error(h, "gpmpc_predict: EM does not return a Jacobian"); return GPMPC_ERR_ARG; }
-    rc = predict_prepare(h, __func__, H, method == GPMPC_METHOD_EM);
+    rc = predict_prepare(h, __func__, ut ? (int)ut_points(h, H) : H, method == GPMPC_METHOD_EM || ut);
     if (rc) return rc;
     if (method == GPMPC_METHOD_EM) return predict_em(h, H, Z, Sigma, spp, mean, var, cov);
     const int Nx = h->Nx, Ny = h->Ny;
-    const size_t nz = (size_t)H * Nx, ns = (method == GPMPC_METHOD_TA && Sigma) ? (size_t)(spp ? H : 1) * Nx * Nx : 0;
+    const size_t nz = (size_t)H * Nx, ns = ((method == GPMPC_METHOD_TA && Sigma) || ut) ? (size_t)(spp ? H : 1) * Nx * Nx : 0;
     const size_t nm = (size_t)H * Ny, nj = (size_t)H * Ny * Nx, nc = (size_t)H * Ny * Ny;
     // device slabs: [Z | Sigma] and [mean | var | J | cov] at capacity-based offsets -> one copy each way
     const size_t cap = (size_t)h->Hcap;
@@ -2876,8 +3037,12 @@ extern "C" int gpmpc_predict(gpmpc_handle_t h, int method, int H, const double* 
     if (zc_in) { dZ_ = h->dPinnedAlias; dS_ = h->dPinnedAlias + cap * Nx; }
     else CUDA_TRY(cudaMemcpyAsync(h->dIn, pin, in_span * 8, cudaMemcpyHostToDevice, h->st));
     auto fld = [&](size_t off) { return zc_out ? h->dPinnedAlias + in_span + (off - lo) : h->dOut + off; };
-    rc = predict_core(h, method, H, dZ_, dS_, spp, mean ? fld(0) : nullptr, var ? fld(off_var) : nullptr,
-                      cov ? fld(off_c) : nullptr, jac ? fld(off_j) : nullptr);
+    double* o_mean = mean ? fld(0) : nullptr;
+    double* o_var = var ? fld(off_var) : nullptr;
+    double* o_cov = cov ? fld(off_c) : nullptr;
+    double* o_jac = jac ? fld(off_j) : nullptr;
+    rc = ut ? ut_pass(h, H, dZ_, dS_, spp, o_mean, o_var, o_cov, o_jac)
+            : predict_core(h, method, H, dZ_, dS_, spp, o_mean, o_var, o_cov, o_jac);
     if (rc) return rc;
     if (out_span && !zc_out) CUDA_TRY(cudaMemcpyAsync(po, h->dOut + lo, out_span * 8, cudaMemcpyDeviceToHost, h->st));
     CUDA_TRY(cudaStreamSynchronize(h->st));

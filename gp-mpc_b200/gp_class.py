@@ -29,8 +29,9 @@ from .mean_functions import mean_function, mean_jacobian
 from .optimize import fit_objective, train_gp_b200
 from .partition import choose_mode, output_block, point_block
 
-_GPU_METHODS = {'ME': _lib.METHOD_ME, 'TA': _lib.METHOD_TA, 'EM': _lib.METHOD_EM}
-_KNOWN_METHODS = ('ME', 'TA', 'EM', 'old_ME', 'old_TA')      # gp_class.py:197-205
+_GPU_METHODS = {'ME': _lib.METHOD_ME, 'TA': _lib.METHOD_TA, 'EM': _lib.METHOD_EM, 'UT': _lib.METHOD_UT}
+_KNOWN_METHODS = ('ME', 'TA', 'EM', 'UT', 'old_ME', 'old_TA')      # gp_class.py:197-205, and the unscented transform
+_SIGMA_METHODS = ('TA', 'EM', 'UT')                                # the methods that read the input covariance
 
 
 def _matmul_seq(A, B):
@@ -104,6 +105,7 @@ class GP:
         self.__engine = None
         self.__invK = None
         self.__prior_mean_in_predict = bool(prior_mean_in_predict)
+        self.__ut_params = None                      # (alpha, beta, kappa) of 'UT'; None: the engine's defaults
         self.__xlb = self.__xub = self.__ulb = self.__uub = None
 
         if meta is not None:                         # gp_class.py:42-50
@@ -157,6 +159,8 @@ class GP:
         kw = {} if capacity is None else dict(capacity=int(capacity))
         self.__engine = self.__engine_factory(self.__N, self.__Nx, self.__Ny, b, n, self.__device, **kw)
         self.__engine.set_data(self.__X, self.__Y)
+        if self.__ut_params is not None:
+            self.__engine.set_ut_params(*self.__ut_params)
         if c.world > 1 and self.__mode == 'outputs':
             uid = self.__engine_factory.comm_unique_id() if c.rank == 0 else None
             uid = c.broadcast_object(uid, src=0)
@@ -324,18 +328,30 @@ class GP:
         return np.array(SMSE).flatten(), np.array(MNLP).flatten()
 
     # ------------------------------------------------------------------ prediction
-    def set_method(self, gp_method='TA'):
+    def set_method(self, gp_method='TA', ut_params=None):
         """ Select wich GP function to use  (reference gp_class.py:193-242)
 
             'ME': Mean Equivalence (normal GP), 'TA': 1st order Taylor Approximation and
             'EM': exact moment matching run on the GPU.  The deprecated 'old_ME'/'old_TA' are
             valid names in the reference but out of scope here (SURVEY section 2).
+            'UT' (not in the reference): the unscented transform, 'ME' evaluated at the 2 Nx + 1 sigma points of the
+            input distribution and recombined (include/gpmpc.h, GPMPC_METHOD_UT); its mean moves with the input
+            covariance and is exact for mean functions up to cubic.  ut_params = (alpha, beta, kappa) sets its
+            parameters and is kept for later 'UT' calls; until given, the engine's defaults (1, 0, 0) apply.
         """
         if gp_method not in _KNOWN_METHODS:
             raise NameError('No GP method called: ' + gp_method)        # gp_class.py:237
         if gp_method not in _GPU_METHODS:
             raise NotImplementedError("gp_method %r is not implemented by the GPU engine "
-                                      "(available: 'ME', 'TA', 'EM')" % gp_method)
+                                      "(available: 'ME', 'TA', 'EM', 'UT')" % gp_method)
+        if gp_method == 'UT':
+            self.__check_ut()
+            if ut_params is not None:
+                alpha, beta, kappa = (float(v) for v in ut_params)
+                self.__engine.set_ut_params(alpha, beta, kappa)
+                self.__ut_params = (alpha, beta, kappa)
+        elif ut_params is not None:
+            raise ValueError("ut_params applies to gp_method 'UT' only (got %r)" % gp_method)
         if gp_method == 'EM' and self.__sharded_outputs():
             # exact moment matching couples every pair of outputs (gp_functions.py:394-412): it
             # needs all Ny factors on one GPU, which the by-output sharding does not provide
@@ -347,10 +363,23 @@ class GP:
     def __sharded_outputs(self):
         return self.__comm.world > 1 and getattr(self, '_GP__mode', 'outputs') == 'outputs'
 
+    def __check_ut(self):
+        """The cases 'UT' does not cover: outputs sharded over ranks, and a prior mean added in predict."""
+        if self.__sharded_outputs():
+            # the recombination couples every pair of outputs at the same sigma points
+            raise NotImplementedError("gp_method 'UT' needs all outputs on one GPU; this GP is sharded by output over "
+                                      "%d ranks (use 'TA'/'ME', or build the GP with a single-process Comm)"
+                                      % self.__comm.world)
+        if self.__prior_mean_in_predict and self.__has_prior_mean():
+            raise NotImplementedError("gp_method 'UT' transforms the zero-mean posterior the engine holds; "
+                                      "prior_mean_in_predict with a prior mean function is not supported")
+
     def __predict_std(self, Z, Sigma, method, want_cov=True, want_jac=True):
         """Batched predict in the GP's standardised space.  Z:(H,Nx)."""
         Z = np.ascontiguousarray(Z, dtype=np.float64).reshape(-1, self.__Nx)
         c = self.__comm
+        if method == 'UT':
+            self.__check_ut()
         add_pm = self.__prior_mean_in_predict and self.__has_prior_mean() and method != 'EM'
         need_jac = want_jac or add_pm
         if c.world > 1 and self.__mode == 'points':
@@ -394,9 +423,9 @@ class GP:
             x = self.standardize(x, self.__meanX, self.__stdX)
             u = self.standardize(u, self.__meanU, self.__stdU)
         Z = np.hstack([x, u])
-        if cov is None and method in ('TA', 'EM'):
+        if cov is None and method in _SIGMA_METHODS:
             cov = np.zeros((self.__Nx, self.__Nx))      # no input uncertainty: TA reduces to diag(var)
-        mean, var, c, _ = self.__predict_std(Z, cov if method in ('TA', 'EM') else None, method, True, False)
+        mean, var, c, _ = self.__predict_std(Z, cov if method in _SIGMA_METHODS else None, method, True, False)
         if self.__normalize:
             mean = self.inverse_mean(mean, self.__meanY, self.__stdY)
         return mean, c
@@ -557,7 +586,7 @@ class GP:
         A batch x0:(B,Ny) with u:(B,Nt,Nu) gives mean, var of shape (len(methods), B, Nt+1, Ny);
         trajectory b is what x0[b], u[b] give alone (its own covariance chain and, with feedback,
         its own gain).  On a single handle every method runs on the device (gpmpc_rollout_batch for
-        'ME' / 'TA', gpmpc_rollout_batch_em for 'EM': one predict pass over all trajectories per
+        'ME' / 'TA' / 'UT', gpmpc_rollout_batch_em for 'EM': one predict pass over all trajectories per
         step, one pass per distinct gain with feedback); sharded models, prior_mean_in_predict and
         device_rollout=False keep the host loop."""
         Ny = self.__Ny

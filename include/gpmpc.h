@@ -40,7 +40,27 @@ enum {
 };
 
 /* propagation method of GP.set_method / GP.predict (gp_class.py:193-237) */
-enum { GPMPC_METHOD_ME = 0, GPMPC_METHOD_TA = 1, GPMPC_METHOD_EM = 2 /* gp_exact_moment, gp_functions.py:344-418; host API only */ };
+enum { GPMPC_METHOD_ME = 0, GPMPC_METHOD_TA = 1, GPMPC_METHOD_EM = 2 /* gp_exact_moment, gp_functions.py:344-418; host API only */,
+       GPMPC_METHOD_UT = 3 /* unscented transform, below */ };
+
+/* 'UT', the unscented transform of the input distribution N(z, Sigma) through the 'ME' prediction.  With n = Nx and the
+ * options "ut_alpha", "ut_beta", "ut_kappa" (alpha, beta, kappa; defaults 1, 0, 0), lambda = alpha^2 (n + kappa) - n and
+ * c = sqrt(n + lambda):
+ *   sigma points, in this order:  z_0 = z,  z_{2j-1} = z + c S_j,  z_{2j} = z - c S_j  (j = 1..n)
+ *   S = the lower Cholesky factor of Sigma (S S^T = Sigma, S_j its column j), semidefinite input accepted: a pivot
+ *       <= 1e-14 max(diag Sigma), or <= 0, makes its column exactly zero without error (a zero u-block, a rank-Ny
+ *       feedback covariance).  That column's two points fall on z_0; the rule stays of degree 3 (the second moment
+ *       along every column of S is matched).
+ *   weights:  W0m = lambda / (n + lambda),  W0c = W0m + 1 - alpha^2 + beta,  Wi = 1 / (2 (n + lambda)) for i >= 1
+ *   with m_i, v_i the 'ME' mean and variance of every output at z_i:
+ *     mean = sum_i Wim m_i,  cov = sum_i Wic (m_i - mean)(m_i - mean)^T + diag(sum_i Wim v_i),  var = diag(cov)
+ *     jac  = the 'ME' Jacobian at z_0: the linearisation at the mean, not a UT quantity
+ * The defaults give lambda = 0, W0 = 0 and spread sqrt(n): the symmetric cubature rule, all weights non-negative.  The
+ * mean is exact for mean functions up to cubic.  W0c < 0 (for example kappa < 0 or a small alpha) can make cov indefinite.
+ * Every sum runs in point order: a point's results do not depend on H or its row.  One 'UT' point costs the predict work
+ * of 2 Nx + 1 'ME' points, evaluated in one pass over H (2 Nx + 1) points; the handle's capacity grows to that count.
+ * Taken by gpmpc_predict, gpmpc_predict_device (Sigma required), gpmpc_rollout and gpmpc_rollout_batch, on a handle
+ * that owns every output (GPMPC_ERR_STATE otherwise); every other entry returns GPMPC_ERR_ARG for it. */
 
 /* selector of gpmpc_get */
 enum {
@@ -150,7 +170,7 @@ int gpmpc_loo_nlpp(gpmpc_handle_t h, int a, const double* theta, double* nlpp, d
 
 /* Batched prediction at H test points (host buffers; copies are part of the call).
  * Z:(H,Nx) in the GP's input space; Sigma:(Nx,Nx) or (H,Nx,Nx) when sigma_per_point
- * (ignored for ME, may be NULL); outputs (any may be NULL): mean:(H,Ny) var:(H,Ny)
+ * (ignored for ME, may be NULL; required for UT); outputs (any may be NULL): mean:(H,Ny) var:(H,Ny)
  * cov:(H,Ny,Ny) jac:(H,Ny,Nx).  With a communicator attached every rank passes the
  * same Z/Sigma and receives all Ny outputs (one all-gather of H*(2+Nx) doubles per
  * output).  Replaces build_gp / build_TA_cov evaluation gp_functions.py:111-147,
@@ -279,7 +299,7 @@ int gpmpc_predict_em_hess(gpmpc_handle_t h, int H, const double* Z, const double
  *                       inverse_mean / standardize pair of gp_class.py:629-638 in the same operation order
  *   means, vars (Nt, Ny) predicted means / diag(cov_t) (the propagated variance the reference records, gp_class.py:793)
  *                       in the GP's output units, cov_last (Ny, Ny) or NULL
- * method GPMPC_METHOD_ME or _TA; the handle must own all outputs.  Same as gpmpc_rollout_batch with B = 1, K = NULL. */
+ * method GPMPC_METHOD_ME, _TA or _UT; the handle must own all outputs.  Same as gpmpc_rollout_batch with B = 1, K = NULL. */
 int gpmpc_rollout(gpmpc_handle_t h, int method, int Nt, const double* z0, const double* U, const double* Sigma0,
                   const double* scale, double* means, double* vars, double* cov_last);
 
@@ -299,7 +319,9 @@ int gpmpc_rollout(gpmpc_handle_t h, int method, int Nt, const double* z0, const 
  *   x_ref   (Ny)          caller units, NULL = 0 (read only with K)
  *   uscale  (2, Nu)       [meanU | stdU] or NULL (read only with K)
  *   means, vars (B, Nt, Ny) as gpmpc_rollout per trajectory;  cov_last (B, Ny, Ny) or NULL
- * Methods ME and TA (EM: GPMPC_ERR_ARG); B, Nt >= 1; the handle must own all outputs (GPMPC_ERR_STATE). */
+ * Methods ME, TA and UT (EM: GPMPC_ERR_ARG); B, Nt >= 1; the handle must own all outputs (GPMPC_ERR_STATE).  With UT each
+ * step is one 'ME' pass over the B (2 Nx + 1) sigma points of the B current (z_t, Sigma_t), formed on the device, and the
+ * recombination; the next input and covariance follow the same rules as ME and TA. */
 int gpmpc_rollout_batch(gpmpc_handle_t h, int method, int B, int Nt, const double* z0, const double* U,
                         const double* Sigma0, const double* scale, const double* K, const double* x_ref,
                         const double* uscale, double* means, double* vars, double* cov_last);
@@ -432,7 +454,9 @@ int gpmpc_get(gpmpc_handle_t h, int what, int a, double* dst);
  * 64x32 tiles; default 4 per SM), "nlml_batch_max" (entries per gpmpc_nlml_batch pass, a cap
  * on its scratch; 0 = all, the default), "em_points" (points per batched 'EM' forward, a cap
  * on its scratch of two Npad^2 slabs per point; 0 = a 1 GiB budget decides, the default; the
- * results do not depend on it).  Any other name returns GPMPC_ERR_ARG. */
+ * results do not depend on it), "ut_alpha", "ut_beta", "ut_kappa" (the 'UT' parameters, see GPMPC_METHOD_UT;
+ * GPMPC_ERR_ARG and no change for a non-finite value, alpha <= 0 or n + lambda <= 0, i.e. kappa <= -Nx).  Any other
+ * name returns GPMPC_ERR_ARG. */
 int gpmpc_set_option(gpmpc_handle_t h, const char* name, double value);
 
 /* Multi-GPU: one process per GPU.  Rank 0 calls gpmpc_comm_unique_id and ships the
